@@ -472,6 +472,21 @@ extern "C" int tsm_device_counts(tsm_ctx* c, void** dptr, int64_t* n_int64) {
 
 extern "C" int tsm_last_launch_count(tsm_ctx* c) { return c ? c->launches : 0; }
 
+#if TSM_PHASE_CLOCKS
+// Build variant only (tools/phase_clocks.py): SM cycles per k_scan phase (ScanPhase order) summed over every warp and
+// launch since the last reset.
+extern "C" int tsm_phase_clocks(unsigned long long* out, int n, int reset) {
+  if (!out || n < (int)PH_N) return TSM_E_ARG;
+  CU(cudaDeviceSynchronize());
+  CU(cudaMemcpyFromSymbol(out, g_scan_phase_clk, sizeof(unsigned long long) * PH_N));
+  if (reset) {
+    const unsigned long long zero[PH_N] = {};
+    CU(cudaMemcpyToSymbol(g_scan_phase_clk, zero, sizeof(zero)));
+  }
+  return TSM_OK;
+}
+#endif
+
 extern "C" int tsm_last_kernel_ms(tsm_ctx* c, float* ms4) {
   if (!c || !ms4) return TSM_E_ARG;
   if (!c->scanned || c->n_files == 0 || c->ev_last < 0) return TSM_E_STATE;

@@ -220,8 +220,10 @@ __device__ __forceinline__ const uint32_t* scan_lut() {
 
 // Slow path: a line that starts in this chunk but ends behind the staged bytes.  Walked by lane 0
 // straight from HBM (correct for any length; lines longer than 240 B past a chunk edge are rare).
-__device__ __noinline__ uint32_t long_line(const ScanParams& p, const uint32_t* lut, uint32_t first, uint32_t f,
-                                           uint32_t fo, uint32_t size, int ext, uint32_t s, Accum& ac, uint32_t* fl_out = nullptr) {
+// Everything goes in and out by value: no argument of this call lives in local memory.
+struct LongLine { uint32_t e, fl; Accum ac; };           // file-relative end of the line, its LF_* flags, the accumulators
+__device__ __noinline__ LongLine long_line(const ScanParams& p, const uint32_t* lut, uint32_t first, uint32_t f,
+                                           uint32_t fo, uint32_t size, int ext, uint32_t s, Accum ac) {
   const uint8_t* g = p.arena + fo;
   const GmemByte lb{g};
   uint32_t e = s;
@@ -243,8 +245,7 @@ __device__ __noinline__ uint32_t long_line(const ScanParams& p, const uint32_t* 
     if (slot < p.hev_cap) p.hev[slot] = tsm_header_event{f, s, e - s, (fl >> 2) & 1u};
     else p.ctrl->overflow = 1;
   }
-  if (fl_out) *fl_out = fl;
-  return e;                                              // file-relative end of the line
+  return LongLine{e, fl, ac};
 }
 
 // Stage the bytes [max(cb-16,0), min(cb+CH+EXT, size)) of a file so that file byte cb sits at buf+PRE.

@@ -15,8 +15,9 @@
 //            the line is the neighbour lane's), pattern flags from the word's stored OR, per-file counters, the candidate
 //            (assertion line) list for k_classify; with TSM_SCAN_LINE_HASHES the line's record (hash, end, flag) as well.
 //
-// Table addresses are formed by IMAD (FMA pipe) instead of LEA (ALU pipe), and the walk is one rolled loop: the kernel is
-// latency / issue bound and sensitive to its instruction-cache footprint (profiles/h100_variants.txt).
+// Table addresses are formed by IMAD (FMA pipe) instead of LEA (ALU pipe), and the walk is a rolled loop: the kernel is
+// latency / issue bound and sensitive to its instruction-cache footprint (profiles/h100_variants.txt).  Where its cycles go:
+// profiles/h100_phases.txt (the TSM_PHASE_CLOCKS build variant).
 // There is no reference kernel: the reference ships data only (SURVEY.md section 0).  Rules cite docs/SPEC.md.
 #pragma once
 #include "tsm_scan_kernels.cuh"
@@ -29,9 +30,6 @@ namespace tsm {
 #ifndef TSM_SCAN2_CTAS
 #define TSM_SCAN2_CTAS 2
 #endif
-#ifndef TSM_RW2_SHIFT
-#define TSM_RW2_SHIFT 2
-#endif
 #ifndef TSM_WALK_UNROLL
 #define TSM_WALK_UNROLL 1         // H100: 1.5 % (C2) / 1.9 % (C4) less k_scan time than 2 (profiles/h100_variants.txt)
 #endif
@@ -41,7 +39,7 @@ constexpr int SCAN2_WARPS = TSM_SCAN2_WARPS, SCAN2_CTAS_PER_SM = TSM_SCAN2_CTAS,
 constexpr uint32_t NWORD = BUF / 8;                      // 544 words of 8 bytes, 17 per stripe
 constexpr uint32_t O2_ARUN = BUF;                        // u32[NWORD + 1]  OR of the states since the last newline word, in front of every word
 constexpr uint32_t SLOT_TAIL = NWORD;                    //                 (+ one slot: the line that ends with the data)
-constexpr uint32_t RW2_SHIFT = TSM_RW2_SHIFT, RW2_PER_STRIPE = 16u >> RW2_SHIFT;   // hash-prefix checkpoint behind every 2^RW2_SHIFT-th word
+constexpr uint32_t RW2_PER_STRIPE = 4;                   // hash-prefix checkpoint behind words 3, 7, 11 and 15 of every stripe
 constexpr uint32_t O2_RW = O2_ARUN + ((NWORD + 1) * 4 + 7) / 8 * 8;   // u64[32 * RW2_PER_STRIPE]
 constexpr uint32_t O2_WENT = O2_RW + 32 * RW2_PER_STRIPE * 8;         // u16[WENT_CAP]   newline words in order (bit 15: mixed)
 constexpr uint32_t WENT_CAP = NWORD + 8;
@@ -50,11 +48,36 @@ constexpr uint32_t O2_LTAB = O2_WENT + WENT_CAP * 2;     // u16[LCAP]       line
 constexpr uint32_t O2_BASE = O2_LTAB + (LCAP + 8) * 2;   // u64[33]         hash prefix at every stripe start (+ total)
 constexpr uint32_t Q2_CAP = 64;
 constexpr uint32_t O2_Q = O2_BASE + 34 * 8;              // u16[Q2_CAP]     mixed words
-constexpr uint32_t O2_CTL = O2_Q + Q2_CAP * 2;           // u32 queue length, pad, u64 mbarrier
+constexpr uint32_t O2_CTL = O2_Q + Q2_CAP * 2;           // u32 queue length, u32 mbarrier phase, u64 mbarrier
 constexpr uint32_t WARP_SMEM2 = ((O2_CTL + 16 + 127) / 128) * 128;
-// per CTA in front of the warps: automaton table (1 KB), per-language masks + the opaque 4 (128 B), rotations of '\n' (61 x 8 B)
+// Phase clocks: a build variant (-DTSM_PHASE_CLOCKS=1, read by tools/phase_clocks.py) in which lane 0 of every warp
+// adds the SM-clock cycles of each phase of the chunk loop into a per-CTA table, flushed to g_scan_phase_clk at exit.
+#ifndef TSM_PHASE_CLOCKS
+#define TSM_PHASE_CLOCKS 0
+#endif
+enum ScanPhase { PH_WAIT, PH_ZERO, PH_WALK, PH_SCANS, PH_MIXED, PH_RECORDS, PH_FINISH, PH_LONG, PH_FLUSH, PH_N };
+#if TSM_PHASE_CLOCKS
+__device__ unsigned long long g_scan_phase_clk[PH_N];
+#endif
+struct PhaseClock {
+#if TSM_PHASE_CLOCKS
+  uint32_t* tab;                                         // per CTA, shared memory
+  long long t;
+  __device__ __forceinline__ void mark(int ph, int lane) {
+    const long long now = clock64();
+    if (lane == 0) atomicAdd(tab + ph, (uint32_t)(now - t));
+    t = now;
+  }
+#else
+  __device__ __forceinline__ void mark(int, int) {}
+#endif
+};
+
+// per CTA in front of the warps: automaton table (1 KB), per-language masks + LutRef (128 B), rotations of '\n' (61 x 8 B)
+// (+ the phase-clock table in that build variant)
 constexpr uint32_t O2_T0A = LUT_BYTES;
-constexpr uint32_t CTA_BYTES2 = LUT_BYTES + 512;
+constexpr uint32_t O2_PHASE = LUT_BYTES + 512;
+constexpr uint32_t CTA_BYTES2 = LUT_BYTES + 512 + (TSM_PHASE_CLOCKS ? 128 : 0);
 constexpr uint32_t SCAN2_SMEM = CTA_BYTES2 + SCAN2_WARPS * WARP_SMEM2;
 constexpr uint32_t O2_LUTB = SCAN2_SMEM;                 // Rev-B trigger table (only the TSM_SCAN_REV_B instantiation): 256 x u32 behind the warps
 constexpr uint32_t SCAN2_SMEM_B = SCAN2_SMEM + 1024;
@@ -74,28 +97,31 @@ constexpr uint32_t REVB_BIT = 1u;                        // in the stored ORs: b
 #ifndef TSM_PIPE_BALANCE
 #define TSM_PIPE_BALANCE 1
 #endif
+// Both operands come from shared memory (LutRef, written by the kernel prologue), so the compiler keeps them in
+// registers for the whole pass instead of forming the table address again for every word.
+struct LutRef { uint32_t four, base; };                  // 4 (from a launch parameter) and the table's shared-window address
+__device__ __forceinline__ LutRef lut_ref() { return LutRef{scan_lut()[256 + 12], scan_lut()[256 + 13]}; }
 template <bool REVB>
-__device__ __forceinline__ void lut_at(uint32_t idx, uint32_t four, uint32_t& v, uint32_t& v2) {
+__device__ __forceinline__ void lut_at(uint32_t idx, LutRef t, uint32_t& v, uint32_t& v2) {
 #if TSM_PIPE_BALANCE
   uint32_t addr;
-  asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(addr) : "r"(idx), "r"(four), "r"(smem_u32(scan_lut())));
+  asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(addr) : "r"(idx), "r"(t.four), "r"(t.base));
   asm("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
   if (REVB) asm("ld.shared.u32 %0, [%1+%2];" : "=r"(v2) : "r"(addr), "n"(O2_LUTB));
 #else
-  (void)four;
+  (void)t;
   v = scan_lut()[idx];
   if (REVB) v2 = scan_lut()[O2_LUTB / 4 + idx];
 #endif
 }
-__device__ __forceinline__ uint32_t opaque_four() { return scan_lut()[256 + 12]; }   // written by the kernel prologue from a launch parameter
 
 struct Auto { uint32_t D, D2; };                         // automaton state (D2: the Rev-B word, unused otherwise)
 
 // One automaton step; returns the states that count for the OR of a line (Rev-B: bit 0 = a Rev-B trigger ended).
 template <bool REVB>
-__device__ __forceinline__ uint32_t step1(Auto& a, uint32_t byte, uint32_t four) {
+__device__ __forceinline__ uint32_t step1(Auto& a, uint32_t byte, LutRef t) {
   uint32_t m, m2 = 0;
-  lut_at<REVB>(byte, four, m, m2);
+  lut_at<REVB>(byte, t, m, m2);
   a.D = ((a.D + a.D) | B_FIRST) & m;
   if (!REVB) return a.D;
   a.D2 = ((a.D2 + a.D2) | B2_FIRST) & m2;
@@ -104,13 +130,13 @@ __device__ __forceinline__ uint32_t step1(Auto& a, uint32_t byte, uint32_t four)
 
 // Eight automaton steps over one 8-byte word; A collects every state of the word.
 template <bool REVB>
-__device__ __forceinline__ void step8b(unsigned long long w, Auto& a, uint32_t& A, uint32_t four) {
+__device__ __forceinline__ void step8b(unsigned long long w, Auto& a, uint32_t& A, LutRef t) {
   const uint32_t lo = (uint32_t)w, hi = (uint32_t)(w >> 32);
   uint32_t A2 = 0;
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     uint32_t m, m2 = 0;
-    lut_at<REVB>(__byte_perm(k < 4 ? lo : hi, 0, 0x4440 + (k & 3)), four, m, m2);
+    lut_at<REVB>(__byte_perm(k < 4 ? lo : hi, 0, 0x4440 + (k & 3)), t, m, m2);
     a.D = ((a.D + a.D) | B_FIRST) & m;
     A |= a.D;
     if (REVB) { a.D2 = ((a.D2 + a.D2) | B2_FIRST) & m2; A2 |= a.D2; }
@@ -138,34 +164,35 @@ __device__ __noinline__ WalkOut walk2(uint8_t* wb, uint32_t fin, int lane) {
   const uint8_t* sp = wb + pos0;
   uint32_t* ar = reinterpret_cast<uint32_t*>(wb + O2_ARUN) + (uint32_t)lane * 17u;
   unsigned long long* rw = reinterpret_cast<unsigned long long*>(wb + O2_RW) + (uint32_t)lane * RW2_PER_STRIPE;
-  const uint32_t four = opaque_four();
+  const LutRef t = lut_ref();
   Auto au{0u, 0u};
   if (lane) {                                            // state in front of the stripe: no state looks back more than 8 bytes
     uint32_t A = 0;                                      // (the longest pattern, Rev B's TESTEQUAL, has 9)
-    step8b<REVB>(*reinterpret_cast<const unsigned long long*>(sp - 8), au, A, four);
+    step8b<REVB>(*reinterpret_cast<const unsigned long long*>(sp - 8), au, A, t);
   }
   unsigned long long R = 0;
   uint32_t run = 0, nlr = 0;                             // nlr: newline-word bits, the newest word in bit 0
-#pragma unroll 1
-  for (uint32_t g = 0; g < 5; ++g) {
-#pragma unroll WALK_UNROLL
-    for (uint32_t k = 0; k < 4; ++k) {
-      if (g == 4 && k) break;
-      const unsigned long long w = *reinterpret_cast<const unsigned long long*>(sp + 32u * g + 8u * k);
-      uint32_t A = 0;
-      step8b<REVB>(w, au, A, four);
-      R = ror3_61(R) + fold61(w);                        // lazily reduced: stays below 2^63
-      if (((k + 1u) & ((1u << RW2_SHIFT) - 1u)) == 0u && g < 4u) rw[(4u * g + k) >> RW2_SHIFT] = R;   // (not behind the 17th word)
-      ar[4u * g + k] = run;
-      nlr = __funnelshift_l(A, nlr, 1);                  // bit 31 of A: the word holds a newline
-      const bool nl = (int32_t)A < 0;
-      if (nl && (A & fin)) {                             // rare: a pattern ends in a newline word
-        const uint32_t slot = atomicAdd(reinterpret_cast<uint32_t*>(wb + O2_CTL), 1u);
-        if (slot < Q2_CAP) reinterpret_cast<uint16_t*>(wb + O2_Q)[slot] = (uint16_t)((uint32_t)lane * 17u + 4u * g + k);
-      }
-      run = nl ? 0u : (run | A);
+  auto word = [&](uint32_t k) {                          // word k of the stripe
+    const unsigned long long w = *reinterpret_cast<const unsigned long long*>(sp + 8u * k);
+    uint32_t A = 0;
+    step8b<REVB>(w, au, A, t);
+    R = ror3_61(R) + fold61(w);                          // lazily reduced: stays below 2^63
+    ar[k] = run;
+    nlr = __funnelshift_l(A, nlr, 1);                    // bit 31 of A: the word holds a newline
+    const bool nl = (int32_t)A < 0;
+    if (nl && (A & fin)) {                               // rare: a pattern ends in a newline word
+      const uint32_t slot = atomicAdd(reinterpret_cast<uint32_t*>(wb + O2_CTL), 1u);
+      if (slot < Q2_CAP) reinterpret_cast<uint16_t*>(wb + O2_Q)[slot] = (uint16_t)((uint32_t)lane * 17u + k);
     }
+    run = nl ? 0u : (run | A);
+  };
+#pragma unroll 1
+  for (uint32_t g = 0; g < 4; ++g) {
+#pragma unroll WALK_UNROLL
+    for (uint32_t k = 0; k < 4; ++k) word(4u * g + k);
+    rw[g] = R;
   }
+  word(16);                                              // (no checkpoint behind the 17th word)
   // stripe totals (frame of the stripe's last word) -> absolute frame -> exclusive scan
   unsigned long long incl = rotl61(canon61(R), (3u * (17u * (uint32_t)lane + 16u)) % 61u);
 #pragma unroll
@@ -186,15 +213,15 @@ __device__ __noinline__ WalkOut walk2(uint8_t* wb, uint32_t fin, int lane) {
 // entry.  Lines inside the word are walked by the finish pass itself (LR_MIXED asks for it).
 template <bool REVB>
 __device__ __noinline__ void resolve_mixed(uint8_t* wb, uint32_t g, uint32_t i, uint32_t n_went) {
-  const uint32_t four = opaque_four();
+  const LutRef t = lut_ref();
   Auto au{0u, 0u};
   uint32_t A = 0;
-  step8b<REVB>(*reinterpret_cast<const unsigned long long*>(wb + 8u * g - 8u), au, A, four);   // g >= 2: the first 16 bytes are zeros
+  step8b<REVB>(*reinterpret_cast<const unsigned long long*>(wb + 8u * g - 8u), au, A, t);   // g >= 2: the first 16 bytes are zeros
   unsigned long long w = *reinterpret_cast<const unsigned long long*>(wb + 8u * g);
   uint32_t pre = 0, post = 0, seen = 0;
 #pragma unroll
   for (int b = 0; b < 8; ++b) {
-    const uint32_t d = step1<REVB>(au, (uint32_t)w & 0xFFu, four);
+    const uint32_t d = step1<REVB>(au, (uint32_t)w & 0xFFu, t);
     const uint32_t m = (uint32_t)((int32_t)au.D >> 31);  // all ones at a newline
     pre |= d & ~seen;
     seen |= m;
@@ -265,7 +292,8 @@ __device__ __noinline__ bool revb_trigger_gmem(const uint8_t* g, uint32_t s, uin
   return false;
 }
 
-struct FinishState {                                     // carried from one window of line records to the next
+struct FinishState {                                     // carried from one window of line records to the next (by value: no local memory)
+  Accum ac;                                              // the chunk's per-file counters
   uint32_t prev_last;                                    // newline in front of the next line
   unsigned long long prevP;                              // hash prefix of the bytes [0, prev_last]
   uint32_t lh_base, lh_done;                             // TSM_SCAN_LINE_HASHES: the chunk's region of the staging arrays, records written
@@ -277,15 +305,15 @@ struct FinishState {                                     // carried from one win
 // (start < lim).  The starts of the assertion lines are compacted (u16 each) over the records already consumed
 // and go to the global candidate list at the end of the window.
 template <bool REVB>
-__device__ __noinline__ void finish_lines2(const ScanParams& p, uint8_t* wb, const uint32_t* lc, uint32_t n, uint32_t lim,
-                                           bool skip_first, uint32_t f, uint32_t cb, int ext, int lane, Accum& ac, FinishState& fs) {
+__device__ __noinline__ FinishState finish_lines2(const ScanParams& p, uint8_t* wb, const uint32_t* lc, uint32_t n, uint32_t lim,
+                                                  bool skip_first, uint32_t f, uint32_t cb, int ext, int lane, FinishState fs) {
   uint16_t* ltab = reinterpret_cast<uint16_t*>(wb + O2_LTAB);
   const uint32_t* arun = reinterpret_cast<const uint32_t*>(wb + O2_ARUN);
   const unsigned long long* t0a = reinterpret_cast<const unsigned long long*>(scan_lut()) + O2_T0A / 8;
   const uint32_t g1 = lc[1], g2 = lc[2];
   const SmemByte lb{wb};
   const bool want_hev = (p.flags & TSM_SCAN_HEADER_EVENTS) != 0, want_lh = (p.flags & TSM_SCAN_LINE_HASHES) != 0;
-  Accum a = ac;
+  Accum a = fs.ac;
   uint32_t nc = 0, lh_done = fs.lh_done;
   uint32_t prev_last = fs.prev_last;
   unsigned long long prevP = fs.prevP;
@@ -297,12 +325,12 @@ __device__ __noinline__ void finish_lines2(const ScanParams& p, uint8_t* wb, con
     const bool isv = (rec & LR_VIRT) != 0;
     const uint32_t g = min(e >> 3, NWORD - 1u), b1 = e - 8u * g + (isv ? 0u : 1u);   // bytes of word g up to and including the newline
     // ---- Pn: hash prefix of the bytes [0, e] (SPEC section 3; lazily reduced, < 2^62 + 8)
-    const uint32_t l = g / 17u, i = g - 17u * l, c0 = i >> RW2_SHIFT, ns = i & ((1u << RW2_SHIFT) - 1u);
+    const uint32_t l = g / 17u, i = g - 17u * l, c0 = i >> 2, ns = i & 3u;
     unsigned long long R = 0;
     if (c0) R = *reinterpret_cast<const unsigned long long*>(wb + O2_RW + 8u * (l * RW2_PER_STRIPE + c0 - 1u));
     const unsigned long long* wp = reinterpret_cast<const unsigned long long*>(wb) + (g - ns);   // words since the checkpoint
 #pragma unroll
-    for (uint32_t t = 0; t + 1u < (1u << RW2_SHIFT); ++t)
+    for (uint32_t t = 0; t < 3u; ++t)
       if (ns > t) R = ror3_61(R) + fold61(wp[t]);
     const unsigned long long w = *reinterpret_cast<const unsigned long long*>(wb + 8u * g);
     const uint32_t r3g = (3u * g) % 61u;
@@ -338,8 +366,8 @@ __device__ __noinline__ void finish_lines2(const ScanParams& p, uint8_t* wb, con
       if (rec & LR_FIRST) A = arun[isv ? SLOT_TAIL : g];
       else if (rec & LR_MIXED) {                         // a line inside a mixed word: its own states
         Auto au{0u, 0u};
-        const uint32_t four = opaque_four();
-        for (uint32_t q = s; q < e; ++q) A |= step1<REVB>(au, lb(q), four);
+        const LutRef t = lut_ref();
+        for (uint32_t q = s; q < e; ++q) A |= step1<REVB>(au, lb(q), t);
       }
       fl = line_flags2<REVB>(s, e, A, g1, g2, ext, lb, a);
       if (want_hev && (fl & LF_HDR)) emit_header(p, f, cb + s - PRE, e - s, fl);
@@ -369,21 +397,21 @@ __device__ __noinline__ void finish_lines2(const ScanParams& p, uint8_t* wb, con
     }
   }
   __syncwarp();
-  ac = a;
+  fs.ac = a;
   fs.prev_last = prev_last;
   fs.prevP = prevP;
   fs.lh_done = lh_done;
+  return fs;
 }
 
 template <bool REVB>
 __device__ __forceinline__ void process_chunk2(const ScanParams& p, const uint32_t* lc, uint8_t* wb, uint32_t uslot, uint32_t f,
-                                               uint32_t cb, uint32_t fo, uint32_t size, int ext, int lane) {
+                                               uint32_t cb, uint32_t size, int ext, int lane, PhaseClock& pc) {
   const uint32_t ce = min(cb + CH, size);
   const uint32_t le = min(ce + EXT, size);
   const uint32_t lim = PRE + (ce - cb);                  // buffer position just past the owned bytes
   const uint32_t lim2 = PRE + (le - cb);                 // ... past the staged bytes
   const bool skip_first = (cb != 0) && (wb[PRE - 1] != '\n');   // chunk starts inside a foreign line
-  Accum ac{0, 0, 0, 0, 0};
   __syncwarp();
   // ---- everything outside the staged range [PRE, lim2) becomes zeros: no pass has to mask its loads
   //      (a zero byte is no newline, matches no pattern and adds nothing to the hash prefix)
@@ -395,7 +423,9 @@ __device__ __forceinline__ void process_chunk2(const ScanParams& p, const uint32
   }
   if (lane == 0) *reinterpret_cast<uint32_t*>(wb + O2_CTL) = 0u;
   __syncwarp();
+  pc.mark(PH_ZERO, lane);
   const WalkOut wo = walk2<REVB>(wb, lc[0], lane);
+  pc.mark(PH_WALK, lane);
   // ---- newline words behind the owned bytes: only the first one matters (it ends the last owned line)
   const uint32_t w0 = 17u * (uint32_t)lane, lim_w = (lim + 7u) >> 3;
   const uint32_t ownbits = lim_w <= w0 ? 0u : (lim_w - w0 >= 17u ? 0x1FFFFu : (1u << (lim_w - w0)) - 1u);
@@ -427,6 +457,7 @@ __device__ __forceinline__ void process_chunk2(const ScanParams& p, const uint32
     if (lane == 0) arun[SLOT_TAIL] = tail_all;
   }
   __syncwarp();
+  pc.mark(PH_SCANS, lane);
   // ---- mixed words
   {
     const uint32_t nq_all = *reinterpret_cast<const uint32_t*>(wb + O2_CTL);
@@ -454,10 +485,11 @@ __device__ __forceinline__ void process_chunk2(const ScanParams& p, const uint32
       }
     }
   }
+  pc.mark(PH_MIXED, lane);
   // ---- newline words -> one record per line (dense: one lane per newline word, SWAR for the newline bytes),
   //      finished window by window (one window unless the chunk has more than ~LCAP lines)
   uint16_t* ltab = reinterpret_cast<uint16_t*>(wb + O2_LTAB);
-  FinishState fs{PRE - 1u, 0ull, 0u, 0u};                // (the 16 bytes in front of the chunk are zeros)
+  FinishState fs{{0, 0, 0, 0, 0}, PRE - 1u, 0ull, 0u, 0u};   // (the 16 bytes in front of the chunk are zeros)
   const bool want_lh = (p.flags & TSM_SCAN_LINE_HASHES) != 0;
   if (want_lh) {                                         // one region for the chunk's line records: newlines of the kept words + 1
     uint32_t tot = 0;
@@ -499,7 +531,9 @@ __device__ __forceinline__ void process_chunk2(const ScanParams& p, const uint32
     n_rec += __shfl_sync(0xffffffffu, in2, 31);
     __syncwarp();
     if (n_rec + 256u > LCAP && base + 32u < n_went) {    // the next round may not fit: finish what is there
-      finish_lines2<REVB>(p, wb, lc, n_rec, lim, skip_first, f, cb, ext, lane, ac, fs);
+      pc.mark(PH_RECORDS, lane);
+      fs = finish_lines2<REVB>(p, wb, lc, n_rec, lim, skip_first, f, cb, ext, lane, fs);
+      pc.mark(PH_FINISH, lane);
       n_rec = 0;
     }
   }
@@ -512,12 +546,18 @@ __device__ __forceinline__ void process_chunk2(const ScanParams& p, const uint32
     } else tail_long = true;
   }
   __syncwarp();
-  if (n_rec) finish_lines2<REVB>(p, wb, lc, n_rec, lim, skip_first, f, cb, ext, lane, ac, fs);
+  pc.mark(PH_RECORDS, lane);
+  if (n_rec) fs = finish_lines2<REVB>(p, wb, lc, n_rec, lim, skip_first, f, cb, ext, lane, fs);
+  pc.mark(PH_FINISH, lane);
+  Accum ac = fs.ac;
   if (tail_long && lane == 0) {
     const unsigned long long d0 = ac.digest;
-    uint32_t fl = 0;
     const uint32_t ls = cb + tail_start - PRE;
-    const uint32_t e = long_line(p, scan_lut(), B_FIRST, f, fo, size, ext, ls, ac, &fl);
+    const uint32_t fo = (uint32_t)p.off[f];              // (read again here: kept in a register it spilled in the Rev-B kernel)
+    const LongLine ll = long_line(p, scan_lut(), B_FIRST, f, fo, size, ext, ls, ac);
+    const uint32_t e = ll.e;
+    uint32_t fl = ll.fl;
+    ac = ll.ac;
     if (REVB && ext != 0 && !(fl & LF_CAND) && revb_trigger_gmem(p.arena + fo, ls, e)) {   // Rev-B triggers of a long line: plain search in HBM
       fl |= LF_CAND;
       ac.asserts++;
@@ -532,6 +572,7 @@ __device__ __forceinline__ void process_chunk2(const ScanParams& p, const uint32
       if (slot < p.lh_cap) { p.lh_hash[slot] = ac.digest - d0; p.lh_end[slot] = e; p.lh_flag[slot] = (uint8_t)(fl & LF_CAND); }
     }
   }
+  pc.mark(PH_LONG, lane);
   // ---- per-file counters: warp reduce (the digest as three partial sums: low halves keep their carries),
   //      then one store (single-chunk file) or one atomic per counter
   ac.lines = __reduce_add_sync(0xffffffffu, ac.lines);
@@ -558,10 +599,11 @@ __device__ __forceinline__ void process_chunk2(const ScanParams& p, const uint32
       if (ac.digest) atomicAdd(reinterpret_cast<unsigned long long*>(&st->digest), ac.digest);
     }
   }
+  pc.mark(PH_FLUSH, lane);
 }
 
 template <bool REVB>
-__global__ void __launch_bounds__(SCAN2_WARPS * 32, SCAN2_CTAS_PER_SM) k_scan_t(ScanParams p) {
+__global__ void __launch_bounds__(SCAN2_WARPS * 32, SCAN2_CTAS_PER_SM) k_scan_t(const __grid_constant__ ScanParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint32_t* lut_all = reinterpret_cast<uint32_t*>(smem);  // [0,256) the automaton table, then 3 x 4 per-language masks, the opaque 4
   for (int i = threadIdx.x; i < 256; i += blockDim.x) lut_all[i] = c_lut[i];
@@ -572,18 +614,27 @@ __global__ void __launch_bounds__(SCAN2_WARPS * 32, SCAN2_CTAS_PER_SM) k_scan_t(
     lut_all[256 + t] = lang == 2 ? 0u : v;
   }
   if (threadIdx.x == 12) lut_all[256 + 12] = p.four;
+  if (threadIdx.x == 13) lut_all[256 + 13] = smem_u32(lut_all);
   if (REVB) for (int i = threadIdx.x; i < 256; i += blockDim.x) lut_all[O2_LUTB / 4 + i] = c_lut_b[i];
+  PhaseClock pc;
+#if TSM_PHASE_CLOCKS
+  pc.tab = reinterpret_cast<uint32_t*>(smem + O2_PHASE);
+  if (threadIdx.x < PH_N) pc.tab[threadIdx.x] = 0u;
+#endif
   if (threadIdx.x >= 32 && threadIdx.x < 32 + 61)        // rotations of the newline byte: 0x0A * 2^r mod 2^61-1
     reinterpret_cast<unsigned long long*>(smem + O2_T0A)[threadIdx.x - 32] = rotl61(0x0Aull, threadIdx.x - 32);
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint8_t* wb = smem + CTA_BYTES2 + warp * WARP_SMEM2;
   uint64_t* bar = reinterpret_cast<uint64_t*>(wb + O2_CTL + 8);
-  if (lane == 0) { mbar_init(bar, 1); fence_mbar_init(); }
+  uint32_t* phase = reinterpret_cast<uint32_t*>(wb + O2_CTL + 4);   // (in shared memory: as a register it spilled in the Rev-B kernel)
+  if (lane == 0) { mbar_init(bar, 1); fence_mbar_init(); *phase = 0u; }
   __syncwarp();
   const uint32_t n_units = p.slab->n_units;
-  uint32_t phase = 0;
   Unit cur = claim_unit(p, n_units, lane);
+#if TSM_PHASE_CLOCKS
+  pc.t = clock64();
+#endif
 #ifndef TSM_LOCKSTEP2
 #define TSM_LOCKSTEP2 0
 #endif
@@ -597,17 +648,24 @@ __global__ void __launch_bounds__(SCAN2_WARPS * 32, SCAN2_CTAS_PER_SM) k_scan_t(
     __syncwarp();
     if (lane == 0) issue_load(p, wb, bar, cur.fo, cur.size, cur.cb);
     const Unit nxt = claim_unit(p, n_units, lane);       // metadata of the next unit arrives during this chunk
-    while (!mbar_try_wait(bar, phase)) {}
-    phase ^= 1;
+    const uint32_t ph = *phase;
+    while (!mbar_try_wait(bar, ph)) {}
+    __syncwarp();
+    if (lane == 0) *phase = ph ^ 1u;
+    pc.mark(PH_WAIT, lane);
     const uint32_t lang = cur.ext == 0 ? 2u : (cur.ext == TSM_EXT_PY ? 0u : 1u);
-    process_chunk2<REVB>(p, lut_all + 256u + 4u * lang, wb, p.unit_base + cur.u, cur.f, cur.cb, cur.fo, cur.size, cur.ext, lane);
+    process_chunk2<REVB>(p, lut_all + 256u + 4u * lang, wb, p.unit_base + cur.u, cur.f, cur.cb, cur.size, cur.ext, lane, pc);
     __syncwarp();
     cur = nxt;
   }
+#if TSM_PHASE_CLOCKS
+  __syncthreads();
+  if (threadIdx.x < PH_N) atomicAdd(&g_scan_phase_clk[threadIdx.x], (unsigned long long)pc.tab[threadIdx.x]);
+#endif
 }
 
 // The two instantiations: canonical Rev A (the hot path, what bench.py times) and Rev B (TSM_SCAN_REV_B).
-template __global__ void k_scan_t<false>(ScanParams);
-template __global__ void k_scan_t<true>(ScanParams);
+template __global__ void k_scan_t<false>(const __grid_constant__ ScanParams);
+template __global__ void k_scan_t<true>(const __grid_constant__ ScanParams);
 
 }  // namespace tsm
