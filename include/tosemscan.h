@@ -28,7 +28,8 @@ typedef enum {
   TSM_OK = 0,
   TSM_E_ARG = -1,        /* null / negative / inconsistent argument */
   TSM_E_LAYOUT = -2,     /* corpus violates SPEC section 1 (alignment, bounds, grp >= n_groups) */
-  TSM_E_CAPACITY = -3,   /* corpus or event count exceeds what the ctx was created for */
+  TSM_E_CAPACITY = -3,   /* corpus exceeds what the ctx was created for (arena bytes, files, groups), a list would
+                            need more than 2^32 - 16 entries, or caller-supplied output arrays are too small */
   TSM_E_CUDA = -4,       /* CUDA runtime error (no device, launch failure, ...) */
   TSM_E_NOMEM = -5,
   TSM_E_STATE = -6       /* call order (e.g. scan_resident before upload) */
@@ -91,8 +92,10 @@ int tsm_abi_version(void);
 const char* tsm_strerror(int status);
 const char* tsm_category_name(int id);   /* "" for 0/reserved, "<other>" for 127 */
 
-/* Context sized for corpora up to (max_arena_bytes, max_files, max_groups) and max_events events
- * of each kind (0 = derive from max_arena_bytes). */
+/* Context sized for corpora up to (max_arena_bytes, max_files, max_groups).  max_events is the initial size of the
+ * device candidate and event lists (0 = max_arena_bytes / 32 + max_files).  It is not a limit: when a scan finds more
+ * assertion lines or headers than the lists hold, tsm_download (and so tsm_scan) grows them to the counts the scan
+ * reached and scans the resident arena once more, and later scans keep the larger lists. */
 int tsm_create(tsm_ctx** out, int device, int64_t max_arena_bytes, int32_t max_files,
                int32_t max_groups, int64_t max_events);
 void tsm_destroy(tsm_ctx* ctx);
@@ -105,9 +108,13 @@ int tsm_scan(tsm_ctx* ctx, const tsm_corpus* corpus, tsm_result* result, uint32_
 /* Resident path (what bench.py's `value` times): upload once, scan many times, fetch once. */
 int tsm_upload(tsm_ctx* ctx, const tsm_corpus* corpus, void* stream);
 int tsm_scan_resident(tsm_ctx* ctx, uint32_t flags, void* stream);       /* kernels only, async */
-int tsm_download(tsm_ctx* ctx, tsm_result* result, void* stream);        /* synchronises */
+/* Synchronises.  If aev_cap or hev_cap is smaller than the number of events of that kind, the call returns
+ * TSM_E_CAPACITY with n_aev and n_hev set to both counts (everything else is filled): size the arrays and call
+ * tsm_download again, the scan is not repeated. */
+int tsm_download(tsm_ctx* ctx, tsm_result* result, void* stream);
 /* Device address of the [n_groups+1][K] int64 count table of the last scan (row n_groups = global),
- * for the single multi-GPU allreduce (SURVEY.md section 8e); valid until the next scan. */
+ * for the single multi-GPU allreduce (SURVEY.md section 8e); valid until the next scan.  The table is complete
+ * once tsm_download has returned: a scan whose candidate list overflowed is redone there. */
 int tsm_device_counts(tsm_ctx* ctx, void** dptr, int64_t* n_int64);
 /* Kernel launches issued by the last tsm_scan / tsm_scan_resident call. */
 int tsm_last_launch_count(tsm_ctx* ctx);

@@ -134,7 +134,9 @@ TOKENS = [b"assert", b"ASSERT_", b"Assert", b"assert ", b"EXPECT_", b"EXPECT_EQ"
           b"!", b"(!", b"assert (", b"F", b"TEST_"]
 
 
-def fuzz_file(rng: random.Random, size: int, nl_rate=0.08, long_lines=False) -> bytes:
+def fuzz_file(rng: random.Random, size: int, nl_rate=0.08, long_lines=False, binary=False) -> bytes:
+    """binary=True: every byte value, CRs in one draw of eight, and runs of 0xFF / 0x00 (the Mersenne-61 hash edges of
+    SPEC section 3) between the tokens."""
     out = bytearray()
     while len(out) < size:
         r = rng.random()
@@ -142,6 +144,12 @@ def fuzz_file(rng: random.Random, size: int, nl_rate=0.08, long_lines=False) -> 
             out += b"\n"
         elif r < nl_rate + 0.02 and long_lines:
             out += bytes(rng.choice(b"abcdefgxyz ._(") for _ in range(rng.randrange(200, 6000)))
+        elif binary and r < nl_rate + 0.15:
+            out += b"\r"
+        elif binary and r < nl_rate + 0.45:
+            out += bytes([rng.randrange(256)])
+        elif binary and r < nl_rate + 0.5:
+            out += bytes([rng.choice((0x00, 0xFF))]) * rng.randrange(1, 20)
         else:
             out += rng.choice(TOKENS)
     out = bytes(out[:size])
@@ -150,7 +158,7 @@ def fuzz_file(rng: random.Random, size: int, nl_rate=0.08, long_lines=False) -> 
     return out
 
 
-def fuzz_corpus(seed: int, n_files: int, max_size: int, long_lines=False):
+def fuzz_corpus(seed: int, n_files: int, max_size: int, long_lines=False, binary=False):
     rng = random.Random(seed)
     files, exts = [], []
     for i in range(n_files):
@@ -162,10 +170,56 @@ def fuzz_corpus(seed: int, n_files: int, max_size: int, long_lines=False):
             size = min(size, max_size)
         else:
             size = rng.randrange(1, max_size)
-        files.append(fuzz_file(rng, size, nl_rate=rng.choice([0.01, 0.05, 0.1, 0.3]), long_lines=long_lines))
+        files.append(fuzz_file(rng, size, nl_rate=rng.choice([0.01, 0.05, 0.1, 0.3]), long_lines=long_lines, binary=binary))
         exts.append(rng.choice([0, 1, 1, 2, 2, 3, 4, 5, 6]))
     grps = [rng.randrange(0, 5) for _ in range(n_files)]
     return files, np.array(exts, np.uint8), np.array(grps, np.uint16)
+
+
+M61 = (1 << 61) - 1
+
+
+def cr_wrap_content(rng: random.Random, n: int) -> bytes:
+    """n >= 8 bytes without LF whose value N (SPEC section 3) makes the line `content + CR` hash to
+    (N + 13 * 256^n) mod (2^61 - 1) below 13 * 256^n mod (2^61 - 1): dropping the CR has to wrap around the modulus.
+    (Below 8 bytes N + 13 * 256^n < 2^61 - 1 and it cannot.)  The top bytes are random; the low 8 pick the residue."""
+    cr = 13 * pow(256, n, M61) % M61
+    while True:
+        high = bytes(rng.choice(range(11, 256)) for _ in range(n - 8))
+        r = M61 - 1 - rng.randrange(cr)                  # N mod p in [p - cr, p)
+        low = (r - 8 * int.from_bytes(high, "little")) % M61   # 256^8 = 2^64 = 8 mod 2^61 - 1
+        c = low.to_bytes(8, "little") + high
+        if b"\n" not in c:
+            return c
+
+
+def hash_edge_contents(seed=5):
+    """Line contents at the edges of the Mersenne-61 line hash: 0xFF runs (every byte 2^8 - 1, values >= 2^61), multiples
+    of 2^61 - 1 (value 0 mod p, also with zero bytes behind), CR steps that wrap, zero bytes and bare CRs."""
+    rng = random.Random(seed)
+    out = [b"\xff" * n for n in range(1, 301)]
+    for k in range(1, 40):
+        v = (k * M61).to_bytes((k * M61).bit_length() // 8 + 1, "little")
+        out += [c for c in (v, v + b"\x00", v + b"\x00" * 5) if b"\n" not in c]
+    out += [cr_wrap_content(rng, n) + b"\r" for n in range(8, 301, 2)]
+    out += [b"\x00" * n for n in (1, 2, 7, 8, 9, 15, 16, 17, 61, 62, 300)]
+    out += [b"\r", b"\r\r", b"x\r\r", b"\xff" * 8 + b"\r", b"\x00\r"]
+    return out
+
+
+def table_name_variants(names):
+    """Each category table name and its near misses: one byte flipped, dropped or appended at every position, a
+    prefix, and cuts / extensions to the lengths around the 8- and 16-byte load boundaries of the device lookup."""
+    out = []
+    for nm in names:
+        out.append(nm)
+        for i in range(len(nm)):
+            out.append(nm[:i] + bytes([nm[i] ^ 0x20 if nm[i] != 0x5F else 0x41]) + nm[i + 1:])
+            out.append(nm[:i] + nm[i + 1:])
+        out += [nm + b"x", nm + b"_", nm + b"0", b"x" + nm, b"my_" + nm, b"_" + nm]
+        out += [nm[:k] for k in (6, 7, 8, 9, 15, 16, 17) if k < len(nm)]
+        out += [nm + b"q" * (k - len(nm)) for k in (8, 9, 16, 17, 24) if k > len(nm)]
+    return list(dict.fromkeys(out))
 
 
 def edge_corpus():

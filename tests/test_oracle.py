@@ -9,32 +9,10 @@ import pytest
 
 import corpus_util as cu
 import orc
+from spec_ref import py_bytes_hash, py_lines
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-M61 = (1 << 61) - 1
 MASK = (1 << 64) - 1
-
-
-def py_bytes_hash(b: bytes) -> int:
-    """SPEC section 3 with Python big integers."""
-    h = int.from_bytes(b, "little") % M61
-    x = h ^ ((len(b) * 0x9E3779B97F4A7C15) & MASK)
-    x ^= x >> 30
-    x = (x * 0xBF58476D1CE4E5B9) & MASK
-    x ^= x >> 27
-    x = (x * 0x94D049BB133111EB) & MASK
-    x ^= x >> 31
-    return x
-
-
-def py_lines(data: bytes):
-    """SPEC section 2."""
-    if not data:
-        return []
-    parts = data.split(b"\n")
-    if parts[-1] == b"":
-        parts.pop()
-    return parts
 
 
 def test_hash_matches_bigint_definition():

@@ -507,11 +507,31 @@ extern "C" int tsm_kernel_ms_stats(tsm_ctx* c, double* sum_ms4, int64_t* n_scans
   return TSM_OK;
 }
 
-extern "C" int tsm_download(tsm_ctx* c, tsm_result* r, void* stream) {
-  if (!c || !r) return TSM_E_ARG;
-  if (!c->scanned) return TSM_E_STATE;
-  CU(cudaSetDevice(c->device));
-  cudaStream_t st = (cudaStream_t)stream;
+// Candidate and event lists of the size the counters of an overflowed scan reached (k_scan and k_classify count every
+// entry, also those past the end of a list).  The new buffers are allocated before the old ones are freed, so that a
+// failed allocation leaves the ctx as it was.
+static int grow_event_buffers(tsm_ctx* c, int64_t need) {
+  if (need <= c->max_events) return TSM_OK;
+  if (need > 0xFFFFFFF0ll) return TSM_E_CAPACITY;
+  unsigned long long* cand = nullptr;
+  tsm_assert_event* aev = nullptr;
+  tsm_header_event* hev = nullptr;
+  const bool ok = cudaMalloc((void**)&cand, sizeof(unsigned long long) * (size_t)need) == cudaSuccess &&
+                  (!c->d_aev || cudaMalloc((void**)&aev, sizeof(tsm_assert_event) * (size_t)need) == cudaSuccess) &&
+                  (!c->d_hev || cudaMalloc((void**)&hev, sizeof(tsm_header_event) * (size_t)need) == cudaSuccess);
+  if (!ok) {
+    cudaGetLastError();                                  // (not sticky: later launches must not report it)
+    cudaFree(cand); cudaFree(aev); cudaFree(hev);
+    return TSM_E_CUDA;
+  }
+  cudaFree(c->d_cand); cudaFree(c->d_aev); cudaFree(c->d_hev);
+  c->d_cand = cand; c->d_aev = aev; c->d_hev = hev;
+  c->max_events = need;
+  return TSM_OK;
+}
+
+// The per-file records, the count tables and the control block of the last scan to the host (synchronises).
+static int download_tables(tsm_ctx* c, tsm_result* r, cudaStream_t st) {
   const int n = c->n_files, G = c->n_groups;
   unsigned long long* h_tot = reinterpret_cast<unsigned long long*>(c->h_ctrl + 1);   // pinned tail
   CU(cudaMemcpyAsync(c->h_ctrl, c->d_ctrl, sizeof(Ctrl), cudaMemcpyDeviceToHost, st));
@@ -521,20 +541,40 @@ extern "C" int tsm_download(tsm_ctx* c, tsm_result* r, void* stream) {
   if (r->global_counts) CU(cudaMemcpyAsync(r->global_counts, c->d_counts + (size_t)G * TSM_K, sizeof(int64_t) * TSM_K, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   for (int i = 0; i < 4; ++i) r->totals[i] = (int64_t)h_tot[i];
+  return TSM_OK;
+}
+
+extern "C" int tsm_download(tsm_ctx* c, tsm_result* r, void* stream) {
+  if (!c || !r) return TSM_E_ARG;
+  if (!c->scanned) return TSM_E_STATE;
+  CU(cudaSetDevice(c->device));
+  cudaStream_t st = (cudaStream_t)stream;
   r->n_aev = 0; r->n_hev = 0;
-  if (c->h_ctrl->overflow) return TSM_E_CAPACITY;
-  if ((c->last_flags & TSM_SCAN_ASSERT_EVENTS) && r->aev) {
+  int rc = download_tables(c, r, st);
+  if (rc != TSM_OK) return rc;
+  if (c->h_ctrl->overflow) {                             // more candidates or events than the lists hold: grow them to the
+    const Ctrl& k = *c->h_ctrl;                          // counts and scan the resident arena once more
+    rc = grow_event_buffers(c, std::max<int64_t>(k.n_cand, std::max(k.n_hev, k.n_aev)));
+    if (rc == TSM_OK) rc = launch_scan(c, c->last_flags, st, nullptr);
+    if (rc == TSM_OK) rc = download_tables(c, r, st);
+    if (rc != TSM_OK) return rc;
+    if (c->h_ctrl->overflow) return TSM_E_CAPACITY;
+  }
+  const bool want_aev = (c->last_flags & TSM_SCAN_ASSERT_EVENTS) && r->aev, want_hev = (c->last_flags & TSM_SCAN_HEADER_EVENTS) && r->hev;
+  if ((want_aev && (int64_t)c->h_ctrl->n_aev > r->aev_cap) || (want_hev && (int64_t)c->h_ctrl->n_hev > r->hev_cap)) {
+    r->n_aev = c->h_ctrl->n_aev; r->n_hev = c->h_ctrl->n_hev;   // the caller's arrays are too small: both sizes, to call again
+    return TSM_E_CAPACITY;
+  }
+  if (want_aev) {
     const int64_t m = c->h_ctrl->n_aev;
-    if (m > r->aev_cap) { r->n_aev = m; return TSM_E_CAPACITY; }
     CU(cudaMemcpyAsync(r->aev, c->d_aev, sizeof(tsm_assert_event) * (size_t)m, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     std::sort(r->aev, r->aev + m, [](const tsm_assert_event& a, const tsm_assert_event& b) {
       return a.file != b.file ? a.file < b.file : a.line_off < b.line_off; });
     r->n_aev = m;
   } else if (c->last_flags & TSM_SCAN_ASSERT_EVENTS) r->n_aev = c->h_ctrl->n_aev;
-  if ((c->last_flags & TSM_SCAN_HEADER_EVENTS) && r->hev) {
+  if (want_hev) {
     const int64_t m = c->h_ctrl->n_hev;
-    if (m > r->hev_cap) { r->n_hev = m; return TSM_E_CAPACITY; }
     CU(cudaMemcpyAsync(r->hev, c->d_hev, sizeof(tsm_header_event) * (size_t)m, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     std::sort(r->hev, r->hev + m, [](const tsm_header_event& a, const tsm_header_event& b) {

@@ -385,7 +385,13 @@ static int cmd_scan(const std::vector<std::string>& roots, const std::string& ro
       tsm_result r{};
       r.stats = stats.data(); r.group_counts = group_counts.data();
       r.aev = aev.data(); r.aev_cap = cap; r.hev = hev.data(); r.hev_cap = cap;
-      ck(tsm_scan(ctx, &c, &r, TSM_SCAN_ASSERT_EVENTS | TSM_SCAN_HEADER_EVENTS | (rev_b ? TSM_SCAN_REV_B : 0u), st), "tsm_scan");
+      int rc = tsm_scan(ctx, &c, &r, TSM_SCAN_ASSERT_EVENTS | TSM_SCAN_HEADER_EVENTS | (rev_b ? TSM_SCAN_REV_B : 0u), st);
+      if (rc == TSM_E_CAPACITY && (r.n_aev > cap || r.n_hev > cap)) {   // denser than bytes / 8 events: fetch again at the size
+        aev.resize((size_t)std::max<int64_t>(r.n_aev, 1)); hev.resize((size_t)std::max<int64_t>(r.n_hev, 1));   // tsm_download reports
+        r.aev = aev.data(); r.aev_cap = (int64_t)aev.size(); r.hev = hev.data(); r.hev_cap = (int64_t)hev.size();
+        rc = tsm_download(ctx, &r, st);
+      }
+      ck(rc, "tsm_scan");
       aev.resize((size_t)r.n_aev); hev.resize((size_t)r.n_hev);
       void* dptr = nullptr; int64_t n64 = 0;
       ck(tsm_device_counts(ctx, &dptr, &n64), "tsm_device_counts");

@@ -19,6 +19,7 @@ EXT = {"py": 1, "cc": 2, "cpp": 3, "java": 4, "c": 5, "h": 6}
 SCAN_ASSERT_EVENTS = 1
 SCAN_HEADER_EVENTS = 2
 SCAN_REV_B = 8            # docs/SPEC.md section 4b (golden G1)
+TSM_E_CAPACITY = -3
 
 FILE_STAT = np.dtype([("n_lines", "<u4"), ("n_assert", "<u4"), ("n_headers", "<u4"),
                       ("n_fixture", "<u4"), ("digest", "<u8")])
@@ -381,6 +382,11 @@ class Scanner:
         return res, r
 
     @staticmethod
+    def _events_too_small(r, flags):
+        """tsm_download's TSM_E_CAPACITY for host event arrays shorter than the scan's events (it reports both counts)."""
+        return bool((flags & SCAN_ASSERT_EVENTS and r.n_aev > r.aev_cap) or (flags & SCAN_HEADER_EVENTS and r.n_hev > r.hev_cap))
+
+    @staticmethod
     def _finish(res, r, flags):
         res["totals"] = np.array(list(r.totals), np.int64)
         if flags & SCAN_ASSERT_EVENTS:
@@ -397,6 +403,9 @@ class Scanner:
         res, r = self._result(corpus.n_files, corpus.n_groups, flags, cap, reuse)
         cs = corpus.c_struct()
         rc = lib().tsm_scan(self._ctx, C.byref(cs), C.byref(r), flags, stream)
+        if rc == TSM_E_CAPACITY and self._events_too_small(r, flags):   # more events than `cap`: fetch them again, sized
+            res, r = self._result(corpus.n_files, corpus.n_groups, flags, max(r.n_aev, r.n_hev), reuse)
+            rc = lib().tsm_download(self._ctx, C.byref(r), stream)
         if rc:
             raise TsmError(rc, "tsm_scan")
         self._corpus = corpus                               # tsm_scan leaves this corpus resident: download() reads its results
@@ -419,6 +428,9 @@ class Scanner:
         cap = int(event_cap if event_cap is not None else max(c.source_bytes // 8 + 16, 1024))
         res, r = self._result(c.n_files, c.n_groups, flags, cap)
         rc = lib().tsm_download(self._ctx, C.byref(r), stream)
+        if rc == TSM_E_CAPACITY and self._events_too_small(r, flags):
+            res, r = self._result(c.n_files, c.n_groups, flags, max(r.n_aev, r.n_hev))
+            rc = lib().tsm_download(self._ctx, C.byref(r), stream)
         if rc:
             raise TsmError(rc, "tsm_download")
         return self._finish(res, r, flags)
