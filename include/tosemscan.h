@@ -153,6 +153,26 @@ int tsm_diff_upload(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news
 int tsm_diff_resident(tsm_ctx* ctx, int64_t* added, int64_t* removed, tsm_diff_detail* detail, void* stream);
 int tsm_diff_last_ms(tsm_ctx* ctx, float* ms3);
 
+/* Changed assertion lines (docs/SPEC.md section 8): the lines the canonical edit script deletes from old or inserts into new
+ * that are assertion lines (Rev A), each classified as a scan classifies it.  Deleted lines count under olds->grp, inserted
+ * lines under news->grp; both corpora must have the same n_groups (else TSM_E_ARG).  An event is the scan's event of that
+ * line (tsm_assert_event) with file = pair index and offsets relative to that side's file.  A pair the detail does not
+ * trace (added_assert = removed_assert = -1) contributes nothing.  added / removed / detail are those of
+ * tsm_diff_pairs_detail (detail may be NULL).  Any pointer of tsm_diff_asserts may be NULL (that output is skipped); n_aev and
+ * n_rev are always set.  If aev_cap or rev_cap is smaller than its count, the call returns TSM_E_CAPACITY with both counts
+ * set and everything else filled: size the arrays and call again. */
+typedef struct tsm_diff_asserts {
+  int64_t* added_counts;     /* [n_groups][TSM_NUM_CATEGORIES], inserted lines by news->grp */
+  int64_t* removed_counts;   /* [n_groups][TSM_NUM_CATEGORIES], deleted lines by olds->grp */
+  tsm_assert_event* aev; int64_t aev_cap; int64_t n_aev;   /* inserted lines, new side, canonical (file, line_off) order */
+  tsm_assert_event* rev; int64_t rev_cap; int64_t n_rev;   /* deleted lines, old side, same order */
+} tsm_diff_asserts;
+int tsm_diff_pairs_asserts(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                           tsm_diff_detail* detail, tsm_diff_asserts* out, void* stream);
+/* The same over the sides of the last tsm_diff_upload (whose grp it keeps); TSM_E_LAYOUT if a grp there was >= n_groups. */
+int tsm_diff_resident_asserts(tsm_ctx* ctx, int64_t* added, int64_t* removed, tsm_diff_detail* detail, tsm_diff_asserts* out,
+                              void* stream);
+
 /* S9 line / n-gram hashes (docs/SPEC.md section 3; SURVEY.md section 8a S9 - a design choice of the north star, attested by no
  * artefact of the package): the records of every line of every file, files in order, from ONE pass of the scan
  * kernel over the source.  line_base[n_files+1] and *n_lines are always filled; line_hash (SPEC section 3), line_end

@@ -183,6 +183,18 @@ static void build_elut(uint32_t* lut) {                  // operator patterns of
 
 static void free_res_pair(tsm_ctx* c);
 
+template <bool EMIT> static cudaError_t diff_small_smem() {   // the dynamic shared memory of the four k_diff_small sizes
+  cudaError_t e = cudaFuncSetAttribute(k_diff_small<DS1_HCAP, DS1_DCAP, DS1_WARPS, EMIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)(DS1_WARPS * ds_warp_bytes(DS1_HCAP, DS1_DCAP)));
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_diff_small<DS2_HCAP, DS2_DCAP, DS2_WARPS, EMIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                 (int)(DS2_WARPS * ds_warp_bytes(DS2_HCAP, DS2_DCAP)));
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_diff_small<DS3_HCAP, DS3_DCAP, DS3_WARPS, EMIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                 (int)(DS3_WARPS * ds_warp_bytes(DS3_HCAP, DS3_DCAP)));
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_diff_small<DS4_HCAP, DS4_DCAP, DS4_WARPS, EMIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                 (int)(DS4_WARPS * ds_warp_bytes(DS4_HCAP, DS4_DCAP)));
+  return e;
+}
+
 extern "C" void tsm_destroy(tsm_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
@@ -269,14 +281,7 @@ extern "C" int tsm_create(tsm_ctx** out, int device, int64_t max_arena_bytes, in
         cudaMemcpyToSymbol(c_lut_b, lutb, sizeof lutb) != cudaSuccess ||
         cudaFuncSetAttribute(k_scan_t<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN2_SMEM) != cudaSuccess ||
         cudaFuncSetAttribute(k_scan_t<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN2_SMEM_B) != cudaSuccess ||
-        cudaFuncSetAttribute(k_diff_small<DS1_HCAP, DS1_DCAP, DS1_WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)(DS1_WARPS * ds_warp_bytes(DS1_HCAP, DS1_DCAP))) != cudaSuccess ||
-        cudaFuncSetAttribute(k_diff_small<DS2_HCAP, DS2_DCAP, DS2_WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)(DS2_WARPS * ds_warp_bytes(DS2_HCAP, DS2_DCAP))) != cudaSuccess ||
-        cudaFuncSetAttribute(k_diff_small<DS3_HCAP, DS3_DCAP, DS3_WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)(DS3_WARPS * ds_warp_bytes(DS3_HCAP, DS3_DCAP))) != cudaSuccess ||
-        cudaFuncSetAttribute(k_diff_small<DS4_HCAP, DS4_DCAP, DS4_WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)(DS4_WARPS * ds_warp_bytes(DS4_HCAP, DS4_DCAP))) != cudaSuccess)
+        diff_small_smem<false>() != cudaSuccess || diff_small_smem<true>() != cudaSuccess)
       rc = TSM_E_CUDA;
   }
   if (rc != TSM_OK) {
@@ -668,7 +673,7 @@ extern "C" void tsm_host_free(void* p) { if (p) cudaFreeHost(p); }
 namespace {
 struct HostSide {                                         // device image of one side of the pairs + its line records
   int32_t n = 0; size_t ab = 0; uint32_t unit_cap = 0;
-  DevBuf arena, off, len, ext, line_base, line_end, line_hash, line_flag;
+  DevBuf arena, off, len, ext, grp, line_base, line_end, line_hash, line_flag;   // (grp: only for the changed assertion lines)
   DevBuf unit_file, unit_begin, cnt, unit_first, bsum, zero, stats, unit_lines, unit_out, unit_line_base, s_hash, s_end, s_flag;
   std::vector<unsigned long long> base;                   // host copy of line_base (only when asked for)
   uint32_t n_units = 0;                                   // (file, chunk) work units: sum of ceil(len / 4 KiB)
@@ -713,6 +718,14 @@ int side_upload(const tsm_corpus* k, HostSide& h, cudaStream_t st) {
   CU(cudaMemcpyAsync(h.len.p, k->len, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
   if (k->ext) CU(cudaMemcpyAsync(h.ext.p, k->ext, (size_t)n, cudaMemcpyHostToDevice, st));
   else CU(cudaMemsetAsync(h.ext.p, 0, (size_t)n, st));
+  return TSM_OK;
+}
+
+// The group tags of an uploaded side (NULL = all 0), which the [group][category] tables of the changed assertion lines use.
+int side_upload_grp(const tsm_corpus* k, HostSide& h, cudaStream_t st) {
+  if (!h.grp.alloc(sizeof(uint16_t) * (size_t)h.n)) return TSM_E_CUDA;
+  if (k->grp) CU(cudaMemcpyAsync(h.grp.p, k->grp, sizeof(uint16_t) * (size_t)h.n, cudaMemcpyHostToDevice, st));
+  else CU(cudaMemsetAsync(h.grp.p, 0, sizeof(uint16_t) * (size_t)h.n, st));
   return TSM_OK;
 }
 
@@ -830,13 +843,24 @@ int side_records(tsm_ctx* c, HostSide& h, cudaStream_t st, float* scan_ms) {
 }
 }  // namespace
 
-struct HostSidePair { HostSide A, B; int32_t n = 0; bool have_records = false; };
+struct HostSidePair {
+  HostSide A, B; int32_t n = 0; bool have_records = false;
+  int32_t groups_a = 1, groups_b = 1; bool grp_ok = true;  // n_groups of both sides, every grp < n_groups (for the assertion tables)
+};
 
 static void free_res_pair(tsm_ctx* c) {
   if (!c->res_pair) return;
   PoolScope pool_scope(&c->pool);                          // the buffers go back to the ctx's pool
   delete c->res_pair;
   c->res_pair = nullptr;
+}
+
+static int check_groups(const tsm_corpus* k) {           // SPEC section 1: every grp below n_groups
+  if (k->n_groups < 1) return TSM_E_ARG;
+  if (k->grp)
+    for (int32_t i = 0; i < k->n_files; ++i)
+      if (k->grp[i] >= k->n_groups) return TSM_E_LAYOUT;
+  return TSM_OK;
 }
 
 static int check_pair_layout(const tsm_corpus* olds, const tsm_corpus* news, bool with_ext) {
@@ -858,20 +882,36 @@ static int check_pair_layout(const tsm_corpus* olds, const tsm_corpus* news, boo
 // k_myers_trace (rows of V in global memory sized from those distances, then the canonical script: hunks, changed
 // assertion lines).  A pair whose distance D needs more than TSM_DIFF_TRACE_MAX_INTS trace entries ((D+1)(D+2)/2) is
 // not traced: it is reported as ONE hunk (add / del / mod by its counts) with added_assert = removed_assert = -1
-// (tosemscan.h).  diff_ms[1] = k_diff_small, diff_ms[2] = the two kernels of the left-over pairs.
+// (tosemscan.h).  diff_ms[1] = k_diff_small, diff_ms[2] = the two kernels of the left-over pairs.  With `sink` (needs
+// `detail`) the EMIT variants of k_diff_small and k_myers_trace also list the changed assertion lines.
+template <bool EMIT>
+static void launch_diff_small(tsm_ctx* c, const HostSide& A, const HostSide& B, int32_t n, const uint8_t* fa, const uint8_t* fb,
+                              uint32_t* cnt, int32_t* const todo[4], long long* da, long long* dr, tsm_diff_detail* d_det,
+                              const AssertSink& sink, cudaStream_t st) {
+  constexpr uint32_t kSmem1 = DS1_WARPS * ds_warp_bytes(DS1_HCAP, DS1_DCAP), kSmem2 = DS2_WARPS * ds_warp_bytes(DS2_HCAP, DS2_DCAP),
+                     kSmem3 = DS3_WARPS * ds_warp_bytes(DS3_HCAP, DS3_DCAP), kSmem4 = DS4_WARPS * ds_warp_bytes(DS4_HCAP, DS4_DCAP);
+  static_assert(kSmem1 * 4 + 4 * 1024 <= 233472 && kSmem2 * 6 + 6 * 1024 <= 233472 && kSmem3 * 5 + 5 * 1024 <= 233472 &&
+                kSmem4 * 3 + 3 * 1024 <= 233472, "pairs per SM");
+  // (the kernels' dynamic shared memory limits are raised per device in tsm_create)
+  k_diff_small<DS1_HCAP, DS1_DCAP, DS1_WARPS, EMIT><<<std::min((n + DS1_WARPS - 1) / DS1_WARPS, c->sms * 4), DS1_WARPS * 32, kSmem1, st>>>(
+      A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, nullptr, nullptr, n, cnt + 4, da, dr, d_det, todo[0], cnt + 0, sink);
+  k_diff_small<DS2_HCAP, DS2_DCAP, DS2_WARPS, EMIT><<<std::min((n + DS2_WARPS - 1) / DS2_WARPS, c->sms * 6), DS2_WARPS * 32, kSmem2, st>>>(
+      A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, todo[0], cnt + 0, n, cnt + 5, da, dr, d_det, todo[1], cnt + 1, sink);
+  k_diff_small<DS3_HCAP, DS3_DCAP, DS3_WARPS, EMIT><<<std::min(n, c->sms * 5), DS3_WARPS * 32, kSmem3, st>>>(
+      A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, todo[1], cnt + 1, n, cnt + 6, da, dr, d_det, todo[2], cnt + 2, sink);
+  k_diff_small<DS4_HCAP, DS4_DCAP, DS4_WARPS, EMIT><<<std::min(n, c->sms * 3), DS4_WARPS * 32, kSmem4, st>>>(
+      A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, todo[2], cnt + 2, n, cnt + 7, da, dr, d_det, todo[3], cnt + 3, sink);
+}
+
 static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* added, int64_t* removed,
-                     tsm_diff_detail* detail, cudaStream_t st) {
+                     tsm_diff_detail* detail, cudaStream_t st, const AssertSink* sink = nullptr) {
   static_assert(sizeof(long long) == sizeof(int64_t), "int64");
   DevBuf d_add, d_rem, d_detail, d_todo1, d_todo2, d_todo3, d_todo, d_ntodo;
   if (!d_add.alloc(sizeof(long long) * (size_t)n) || !d_rem.alloc(sizeof(long long) * (size_t)n) ||
       !d_todo1.alloc(sizeof(int32_t) * (size_t)n) || !d_todo2.alloc(sizeof(int32_t) * (size_t)n) || !d_todo3.alloc(sizeof(int32_t) * (size_t)n) || !d_todo.alloc(sizeof(int32_t) * (size_t)n) ||
       !d_ntodo.alloc(64) || (detail && !d_detail.alloc(sizeof(tsm_diff_detail) * (size_t)n)))
     return TSM_E_CUDA;
-  constexpr uint32_t kSmem1 = DS1_WARPS * ds_warp_bytes(DS1_HCAP, DS1_DCAP), kSmem2 = DS2_WARPS * ds_warp_bytes(DS2_HCAP, DS2_DCAP),
-                     kSmem3 = DS3_WARPS * ds_warp_bytes(DS3_HCAP, DS3_DCAP), kSmem4 = DS4_WARPS * ds_warp_bytes(DS4_HCAP, DS4_DCAP);
-  static_assert(kSmem1 * 4 + 4 * 1024 <= 233472 && kSmem2 * 6 + 6 * 1024 <= 233472 && kSmem3 * 5 + 5 * 1024 <= 233472 &&
-                kSmem4 * 3 + 3 * 1024 <= 233472, "pairs per SM");
-  // (the kernels' dynamic shared memory limits are raised per device in tsm_create)
+  if (sink && !detail) return TSM_E_ARG;
   CU(cudaMemsetAsync(d_ntodo.p, 0, 64, st));
   CU(cudaMemsetAsync(d_add.p, 0, sizeof(long long) * (size_t)n, st));     // (the first copy back covers every pair, also the ones
   CU(cudaMemsetAsync(d_rem.p, 0, sizeof(long long) * (size_t)n, st));     //  the four sizes leave to k_myers / k_myers_trace)
@@ -882,15 +922,10 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
   tsm_diff_detail* d_det = detail ? d_detail.as<tsm_diff_detail>() : nullptr;
   long long* da = d_add.as<long long>();
   long long* dr = d_rem.as<long long>();
+  int32_t* const todo_lists[4] = {d_todo1.as<int32_t>(), d_todo2.as<int32_t>(), d_todo3.as<int32_t>(), d_todo.as<int32_t>()};
   CU(cudaEventRecord(c->diff_ev[2], st));
-  k_diff_small<DS1_HCAP, DS1_DCAP, DS1_WARPS><<<std::min((n + DS1_WARPS - 1) / DS1_WARPS, c->sms * 4), DS1_WARPS * 32, kSmem1, st>>>(
-      A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, nullptr, nullptr, n, cnt + 4, da, dr, d_det, d_todo1.as<int32_t>(), cnt + 0);
-  k_diff_small<DS2_HCAP, DS2_DCAP, DS2_WARPS><<<std::min((n + DS2_WARPS - 1) / DS2_WARPS, c->sms * 6), DS2_WARPS * 32, kSmem2, st>>>(
-      A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, d_todo1.as<int32_t>(), cnt + 0, n, cnt + 5, da, dr, d_det, d_todo2.as<int32_t>(), cnt + 1);
-  k_diff_small<DS3_HCAP, DS3_DCAP, DS3_WARPS><<<std::min(n, c->sms * 5), DS3_WARPS * 32, kSmem3, st>>>(
-      A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, d_todo2.as<int32_t>(), cnt + 1, n, cnt + 6, da, dr, d_det, d_todo3.as<int32_t>(), cnt + 2);
-  k_diff_small<DS4_HCAP, DS4_DCAP, DS4_WARPS><<<std::min(n, c->sms * 3), DS4_WARPS * 32, kSmem4, st>>>(
-      A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, d_todo3.as<int32_t>(), cnt + 2, n, cnt + 7, da, dr, d_det, d_todo.as<int32_t>(), cnt + 3);
+  if (sink) launch_diff_small<true>(c, A, B, n, fa, fb, cnt, todo_lists, da, dr, d_det, *sink, st);
+  else launch_diff_small<false>(c, A, B, n, fa, fb, cnt, todo_lists, da, dr, d_det, AssertSink{}, st);
   CU(cudaEventRecord(c->diff_ev[3], st));
   CU(cudaGetLastError());
   uint32_t* pin_nt = reinterpret_cast<uint32_t*>(c->h_diff + 80);
@@ -961,10 +996,17 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
     CU(cudaMemcpyAsync(d_tbase.as<unsigned long long>() + p0, tbase.data() + p0, sizeof(unsigned long long) * (size_t)(p1 - p0),
                        cudaMemcpyHostToDevice, st));
     CU(cudaEventRecord(c->diff_ev[4], st));
-    k_myers_trace<<<((p1 - p0) * 32 + 127) / 128, 128, 0, st>>>(
-        A.d.line_hash, A.d.line_base, A.d.line_flag, B.d.line_hash, B.d.line_base, B.d.line_flag, (int32_t)p0, (int32_t)(p1 - p0),
-        d_trace.as<int32_t>(), d_tbase.as<unsigned long long>(), d_add.as<long long>(), d_rem.as<long long>(),
-        (long long)TSM_DIFF_TRACE_MAX_D, d_detail.as<tsm_diff_detail>(), d_todo.as<int32_t>());
+    const unsigned grid = ((p1 - p0) * 32 + 127) / 128;
+    if (sink)
+      k_myers_trace<true><<<grid, 128, 0, st>>>(
+          A.d.line_hash, A.d.line_base, A.d.line_flag, B.d.line_hash, B.d.line_base, B.d.line_flag, (int32_t)p0, (int32_t)(p1 - p0),
+          d_trace.as<int32_t>(), d_tbase.as<unsigned long long>(), d_add.as<long long>(), d_rem.as<long long>(),
+          (long long)TSM_DIFF_TRACE_MAX_D, d_detail.as<tsm_diff_detail>(), d_todo.as<int32_t>(), *sink);
+    else
+      k_myers_trace<false><<<grid, 128, 0, st>>>(
+          A.d.line_hash, A.d.line_base, A.d.line_flag, B.d.line_hash, B.d.line_base, B.d.line_flag, (int32_t)p0, (int32_t)(p1 - p0),
+          d_trace.as<int32_t>(), d_tbase.as<unsigned long long>(), d_add.as<long long>(), d_rem.as<long long>(),
+          (long long)TSM_DIFF_TRACE_MAX_D, d_detail.as<tsm_diff_detail>(), d_todo.as<int32_t>(), AssertSink{});
     CU(cudaEventRecord(c->diff_ev[5], st));
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(st));
@@ -1015,9 +1057,14 @@ extern "C" int tsm_diff_upload(tsm_ctx* c, const tsm_corpus* olds, const tsm_cor
   SyncGuard guard(st);
   c->res_pair = new (std::nothrow) HostSidePair;
   if (!c->res_pair) return TSM_E_NOMEM;
-  c->res_pair->n = olds->n_files;
-  rc = side_upload(olds, c->res_pair->A, st);
-  if (rc == TSM_OK) rc = side_upload(news, c->res_pair->B, st);
+  HostSidePair& P = *c->res_pair;
+  P.n = olds->n_files;
+  P.groups_a = olds->n_groups; P.groups_b = news->n_groups;
+  P.grp_ok = check_groups(olds) == TSM_OK && check_groups(news) == TSM_OK;
+  rc = side_upload(olds, P.A, st);
+  if (rc == TSM_OK) rc = side_upload(news, P.B, st);
+  if (rc == TSM_OK) rc = side_upload_grp(olds, P.A, st);
+  if (rc == TSM_OK) rc = side_upload_grp(news, P.B, st);
   if (rc == TSM_OK) rc = cudaStreamSynchronize(st) == cudaSuccess ? TSM_OK : TSM_E_CUDA;
   if (rc != TSM_OK) { delete c->res_pair; c->res_pair = nullptr; }
   return rc;
@@ -1049,6 +1096,142 @@ extern "C" int tsm_diff_last_ms(tsm_ctx* c, float* ms3) {
 extern "C" int tsm_diff_pairs(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news,
                               int64_t* added, int64_t* removed, void* stream) {
   return tsm_diff_pairs_detail(c, olds, news, added, removed, nullptr, stream);
+}
+
+// Events (any order, file < n_files) into the canonical (file, line_off) order: a counting sort by file, then the few events
+// of each file by line_off.  A comparison sort of the whole array costs milliseconds for a C5 batch; this is linear.
+static void sort_events_by_file(tsm_assert_event* ev, uint32_t m, int32_t n_files) {
+  if (m < 2) return;
+  std::vector<uint32_t> pos((size_t)n_files + 1, 0);
+  for (uint32_t i = 0; i < m; ++i) pos[(size_t)ev[i].file + 1]++;
+  for (int32_t f = 0; f < n_files; ++f) pos[(size_t)f + 1] += pos[(size_t)f];
+  std::vector<tsm_assert_event> tmp(m);
+  std::vector<uint32_t> at(pos.begin(), pos.end() - 1);
+  for (uint32_t i = 0; i < m; ++i) tmp[at[ev[i].file]++] = ev[i];
+  for (int32_t f = 0; f < n_files; ++f)
+    if (pos[(size_t)f + 1] - pos[(size_t)f] > 1)
+      std::sort(tmp.begin() + pos[(size_t)f], tmp.begin() + pos[(size_t)f + 1],
+                [](const tsm_assert_event& a, const tsm_assert_event& b) { return a.line_off < b.line_off; });
+  std::copy(tmp.begin(), tmp.end(), ev);
+}
+
+// Changed assertion lines (docs/SPEC.md section 8): diff_core with the EMIT kernels, then per side ONE k_classify launch
+// over the list they filled, with a ScanParams over that side's arena, tags and groups and a Ctrl of its own whose n_cand
+// is the list's counter - a changed line is classified by the code, and so with the result, of a scan.  Each list holds
+// one entry per line of its side, a bound known before the launch that no side can exceed.
+static int diff_asserts(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int32_t n_groups, int64_t* added, int64_t* removed,
+                        tsm_diff_detail* detail, tsm_diff_asserts* out, cudaStream_t st) {
+  std::vector<tsm_diff_detail> own;                        // the lists need the assertion flags, which come with the detail
+  if (!detail) { own.resize((size_t)n); detail = own.data(); }
+  HostSide* side[2] = {&A, &B};                            // side 0: deleted lines of `old`, side 1: inserted lines of `new`
+  DevBuf d_list[2], d_ctrl, d_counts[2], d_aev[2];
+  AssertSink sink{};
+  if (!d_ctrl.alloc(2 * 64)) return TSM_E_CUDA;
+  Ctrl* ctrl[2] = {d_ctrl.as<Ctrl>(), reinterpret_cast<Ctrl*>(d_ctrl.as<uint8_t>() + 64)};
+  for (int s = 0; s < 2; ++s) {
+    const unsigned long long lines = side[s]->total;
+    if (lines > 0xFFFFFFF0ull) return TSM_E_CAPACITY;
+    if (!d_list[s].alloc(sizeof(unsigned long long) * (size_t)(lines ? lines : 1))) return TSM_E_CUDA;
+    sink.list[s] = d_list[s].as<unsigned long long>(); sink.n[s] = &ctrl[s]->n_cand; sink.cap[s] = (uint32_t)lines;
+    sink.line_end[s] = side[s]->d.line_end;
+  }
+  CU(cudaMemsetAsync(d_ctrl.p, 0, 2 * 64, st));            // n_cand = cls_done = 0
+  int rc = diff_core(c, A, B, n, added, removed, detail, st, &sink);
+  if (rc != TSM_OK) return rc;
+  Ctrl hc[2];
+  for (int s = 0; s < 2; ++s) CU(cudaMemcpyAsync(&hc[s], ctrl[s], sizeof(Ctrl), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const uint32_t nc[2] = {hc[0].n_cand, hc[1].n_cand};
+  if (nc[0] > sink.cap[0] || nc[1] > sink.cap[1]) return TSM_E_CAPACITY;   // (more changed lines than lines: never)
+  tsm_assert_event* const h_ev[2] = {out->rev, out->aev};
+  const int64_t h_cap[2] = {out->rev_cap, out->aev_cap};
+  int64_t* const h_counts[2] = {out->removed_counts, out->added_counts};
+  const size_t table = (size_t)(n_groups + 1) * TSM_K;     // [n_groups + 1][K]: k_classify also fills the global row
+  const size_t hist = CLS_SMEM_BASE + sizeof(uint32_t) * (n_groups <= 16 ? (size_t)n_groups * TSM_K : 0);
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_classify_t<false>, 256, hist) != cudaSuccess || per_sm < 1) per_sm = 4;
+  for (int s = 0; s < 2; ++s) {
+    if (!d_counts[s].alloc(sizeof(unsigned long long) * table) ||
+        (h_ev[s] && !d_aev[s].alloc(sizeof(tsm_assert_event) * (size_t)std::max(nc[s], 1u))))
+      return TSM_E_CUDA;
+    CU(cudaMemsetAsync(d_counts[s].p, 0, sizeof(unsigned long long) * table, st));
+    if (nc[s] == 0) continue;
+    const HostSide& h = *side[s];
+    ScanParams p{};
+    p.arena = h.arena.as<uint8_t>(); p.off = h.off.as<int32_t>(); p.len = h.len.as<int32_t>(); p.ext = h.ext.as<uint8_t>();
+    p.grp = h.grp.as<uint16_t>(); p.n_files = n; p.n_groups = n_groups;
+    p.ctrl = ctrl[s];
+    p.cand = sink.list[s]; p.cand_cap = sink.cap[s];
+    p.aev = d_aev[s].as<tsm_assert_event>(); p.aev_cap = h_ev[s] ? nc[s] : 0;
+    p.counts = d_counts[s].as<unsigned long long>();
+    p.flags = h_ev[s] ? TSM_SCAN_ASSERT_EVENTS : 0u; p.four = 4; p.cls_last = 0;
+    k_classify_t<false><<<std::min<uint32_t>((uint32_t)(c->sms * per_sm), (nc[s] + 255) / 256), 256, hist, st>>>(p);
+    CU(cudaGetLastError());
+    c->launches++;
+  }
+  for (int s = 0; s < 2; ++s)
+    if (h_counts[s]) CU(cudaMemcpyAsync(h_counts[s], d_counts[s].p, sizeof(int64_t) * (size_t)n_groups * TSM_K, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  out->n_rev = nc[0]; out->n_aev = nc[1];
+  if ((h_ev[0] && nc[0] > h_cap[0]) || (h_ev[1] && nc[1] > h_cap[1])) return TSM_E_CAPACITY;   // both counts set: size and call again
+  for (int s = 0; s < 2; ++s)
+    if (h_ev[s] && nc[s]) CU(cudaMemcpyAsync(h_ev[s], d_aev[s].p, sizeof(tsm_assert_event) * nc[s], cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  for (int s = 0; s < 2; ++s)
+    if (h_ev[s]) sort_events_by_file(h_ev[s], nc[s], n);
+  return TSM_OK;
+}
+
+extern "C" int tsm_diff_pairs_asserts(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                                      tsm_diff_detail* detail, tsm_diff_asserts* out, void* stream) {
+  if (!c || !olds || !news || !added || !removed || !out || olds->n_files != news->n_files || olds->n_groups != news->n_groups)
+    return TSM_E_ARG;
+  int rc = check_groups(olds);
+  if (rc == TSM_OK) rc = check_groups(news);
+  if (rc != TSM_OK) return rc;
+  const int32_t n = olds->n_files;
+  out->n_aev = out->n_rev = 0;
+  if (n == 0) {
+    for (int64_t* t : {out->added_counts, out->removed_counts})
+      if (t) memset(t, 0, sizeof(int64_t) * (size_t)olds->n_groups * TSM_K);
+    return TSM_OK;
+  }
+  rc = check_pair_layout(olds, news, true);
+  if (rc != TSM_OK) return rc;
+  CU(cudaSetDevice(c->device));
+  PoolScope pool_scope(&c->pool);
+  cudaStream_t st = (cudaStream_t)stream;
+  HostSide A, B;
+  SyncGuard guard(st);
+  c->diff_ms[0] = 0;
+  rc = side_upload(olds, A, st);
+  if (rc == TSM_OK) rc = side_upload(news, B, st);
+  if (rc == TSM_OK) rc = side_upload_grp(olds, A, st);
+  if (rc == TSM_OK) rc = side_upload_grp(news, B, st);
+  HostSide* both[2] = {&A, &B};
+  if (rc == TSM_OK) rc = sides_records(c, both, 2, st, &c->diff_ms[0], false);
+  if (rc != TSM_OK) return rc;
+  return diff_asserts(c, A, B, n, olds->n_groups, added, removed, detail, out, st);
+}
+
+extern "C" int tsm_diff_resident_asserts(tsm_ctx* c, int64_t* added, int64_t* removed, tsm_diff_detail* detail,
+                                         tsm_diff_asserts* out, void* stream) {
+  if (!c || !added || !removed || !out) return TSM_E_ARG;
+  if (!c->res_pair) return TSM_E_STATE;
+  HostSidePair& P = *c->res_pair;
+  if (P.groups_a != P.groups_b) return TSM_E_ARG;
+  if (!P.grp_ok) return TSM_E_LAYOUT;
+  out->n_aev = out->n_rev = 0;
+  CU(cudaSetDevice(c->device));
+  PoolScope pool_scope(&c->pool);
+  cudaStream_t st = (cudaStream_t)stream;
+  SyncGuard guard(st);
+  c->diff_ms[0] = 0;
+  P.A.launches = P.B.launches = 0;
+  HostSide* both[2] = {&P.A, &P.B};
+  int rc = sides_records(c, both, 2, st, &c->diff_ms[0], false);
+  if (rc != TSM_OK) return rc;
+  return diff_asserts(c, P.A, P.B, P.n, P.groups_a, added, removed, detail, out, st);
 }
 
 // ------------------------------------------------------------------------------------- S9 line / n-gram hashes

@@ -12,6 +12,9 @@
 //                   them holds (middle above 4 096 lines, distance above 127) is left to the two kernels below
 //   k_myers         warp per pair: the same search with V in global scratch (any size)
 //   k_myers_trace   the same with one row of V kept per D in global memory, then the backtrack
+//
+// k_diff_small and k_myers_trace have a second variant (EMIT) that also lists the changed assertion lines (SPEC section 8)
+// for k_classify; the variant without it is the same code as before the lists existed.
 #pragma once
 #include "tsm_scan_kernels.cuh"
 
@@ -26,6 +29,39 @@ struct DiffSide {                   // one corpus (old or new) on the device
   const uint8_t* ext;               // [n] S1 tags (NULL = all 0), only read when line_flag != NULL
   uint8_t* line_flag;               // [total lines] 1 = assertion line (SPEC section 4); NULL = not wanted
 };
+
+// Where the EMIT variants put the changed assertion lines: side 0 = deleted lines of `old`, side 1 = inserted lines of `new`,
+// each as (pair << 32 | file-relative line start), the candidate format of k_classify.  n[s] is the n_cand of the Ctrl that
+// k_classify reads for side s; it counts every line, also those past cap[s], so that the host sees an overflow.
+struct AssertSink {
+  unsigned long long* list[2];
+  uint32_t* n[2];
+  uint32_t cap[2];
+  const uint32_t* line_end[2];      // DiffSide::line_end of each side
+};
+
+// Candidate of line g (global line index) of pair pr, whose file starts at line `first` of its side.
+__device__ __forceinline__ unsigned long long sink_key(const AssertSink& s, int side, int pr, unsigned long long first,
+                                                       unsigned long long g) {
+  return ((unsigned long long)(uint32_t)pr << 32) | (g == first ? 0u : s.line_end[side][g - 1] + 1u);
+}
+__device__ __forceinline__ void sink_put(const AssertSink& s, int side, unsigned long long key) {   // one lane
+  const uint32_t slot = atomicAdd(s.n[side], 1u);
+  if (slot < s.cap[side]) s.list[side][slot] = key;
+}
+// Every flagged line of the run [g0, g0 + cnt) (flags q[0 .. cnt)): the whole warp, one atomic per 32 lines.
+__device__ __forceinline__ void sink_run(const AssertSink& s, int side, int pr, unsigned long long first, unsigned long long g0,
+                                         const uint8_t* q, int cnt, int lane) {
+  for (int i0 = 0; i0 < cnt; i0 += 32) {
+    const int i = i0 + lane;
+    const bool f = i < cnt && q[i] != 0;
+    const uint32_t bal = __ballot_sync(0xffffffffu, f);
+    if (!bal) continue;
+    const uint32_t base = warp_reserve(s.n[side], (uint32_t)__popc(bal), lane);
+    const uint32_t slot = base + (uint32_t)__popc(bal & ((1u << lane) - 1u));
+    if (f && slot < s.cap[side]) s.list[side][slot] = sink_key(s, side, pr, first, g0 + (unsigned long long)i);
+  }
+}
 
 // Follow a diagonal while the lines are equal.  Four positions are compared per round trip to HBM / L2 (the loads
 // of one round do not depend on each other); the clamped indices keep speculative reads inside the sequences.
@@ -61,11 +97,11 @@ __host__ __device__ constexpr uint32_t ds_warp_bytes(int hcap, int dcap) { retur
 //     is finished by the whole warp, 32 lines per step: a long unchanged stretch costs a few ballots, not hundreds of
 //     dependent loads;
 //   * the assertion-line flags of the middle are staged next to the hashes: the backtrack reads shared memory only.
-template <int HCAP, int DCAP>
+template <int HCAP, int DCAP, bool EMIT>
 __device__ __forceinline__ bool diff_one(uint8_t* mine, int pr, int lane,
     const unsigned long long* ha, const unsigned long long* la, const uint8_t* fa,
     const unsigned long long* hb, const unsigned long long* lb, const uint8_t* fb,
-    long long* added, long long* removed, tsm_diff_detail* detail) {
+    long long* added, long long* removed, tsm_diff_detail* detail, const AssertSink& sink) {
   constexpr int NQ = (DCAP + 32) / 32;                    // row entries per lane
   unsigned long long* sa = reinterpret_cast<unsigned long long*>(mine);
   int32_t* rows = reinterpret_cast<int32_t*>(mine + HCAP * 8);
@@ -105,6 +141,10 @@ __device__ __forceinline__ bool diff_one(uint8_t* mine, int pr, int lane,
       for (int k = 16; k; k >>= 1) { ca += __shfl_xor_sync(0xffffffffu, ca, k); cb += __shfl_xor_sync(0xffffffffu, cb, k); }
       if (n) { h_del = 1; r_as = ca; }
       if (m) { h_add = 1; a_as = cb; }
+      if constexpr (EMIT) {
+        sink_run(sink, 0, pr, la[pr], la[pr] + pre, qa, n, lane);
+        sink_run(sink, 1, pr, lb[pr], lb[pr] + pre, qb, m, lane);
+      }
     }
   } else {
     if (n + m > HCAP) return false;
@@ -189,6 +229,10 @@ __device__ __forceinline__ bool diff_one(uint8_t* mine, int pr, int lane,
         in_hunk = true;
         if (down) { has_add = true; a_as += sfb[py] != 0; }
         else { has_del = true; r_as += sfa[px] != 0; }
+        if constexpr (EMIT) {
+          if (down && sfb[py]) sink_put(sink, 1, sink_key(sink, 1, pr, lb[pr], lb[pr] + pre + py));
+          if (!down && sfa[px]) sink_put(sink, 0, sink_key(sink, 0, pr, la[pr], la[pr] + pre + px));
+        }
         x = px; y = py;
       }
       if (in_hunk) { if (has_add && has_del) ++h_mod; else if (has_add) ++h_add; else ++h_del; }
@@ -205,12 +249,12 @@ __device__ __forceinline__ bool diff_one(uint8_t* mine, int pr, int lane,
 
 // Persistent warps, pairs handed out by an atomic counter (their cost varies by two orders of magnitude).  The pairs
 // are todo_in[0 .. *n_in) when todo_in is given, else 0 .. n_all; what this size cannot finish goes to todo_out.
-template <int HCAP, int DCAP, int WARPS>
+template <int HCAP, int DCAP, int WARPS, bool EMIT>
 __global__ void __launch_bounds__(WARPS * 32) k_diff_small(
     const unsigned long long* ha, const unsigned long long* la, const uint8_t* fa,
     const unsigned long long* hb, const unsigned long long* lb, const uint8_t* fb,
     const int32_t* todo_in, const uint32_t* n_in, int32_t n_all, uint32_t* work,
-    long long* added, long long* removed, tsm_diff_detail* detail, int32_t* todo_out, uint32_t* n_out) {
+    long long* added, long long* removed, tsm_diff_detail* detail, int32_t* todo_out, uint32_t* n_out, AssertSink sink) {
   extern __shared__ __align__(16) uint8_t ds_smem[];
   const int lane = threadIdx.x & 31;
   uint8_t* mine = ds_smem + (threadIdx.x >> 5) * ds_warp_bytes(HCAP, DCAP);
@@ -221,7 +265,7 @@ __global__ void __launch_bounds__(WARPS * 32) k_diff_small(
     slot = __shfl_sync(0xffffffffu, slot, 0);
     if (slot >= limit) return;
     const int pr = todo_in ? todo_in[slot] : (int)slot;
-    if (!diff_one<HCAP, DCAP>(mine, pr, lane, ha, la, fa, hb, lb, fb, added, removed, detail) && lane == 0)
+    if (!diff_one<HCAP, DCAP, EMIT>(mine, pr, lane, ha, la, fa, hb, lb, fb, added, removed, detail, sink) && lane == 0)
       todo_out[atomicAdd(n_out, 1u)] = pr;
   }
 }
@@ -289,11 +333,12 @@ __global__ void k_myers(const unsigned long long* ha, const unsigned long long* 
 // Hunks and their classification (docs/SPEC.md section 8): the same search with one row of V kept per D
 // (row d holds the diagonals -d, -d+2, ..., d), then the canonical backtrack by lane 0.
 // trace_base[pr] = first int of pair pr's rows, sized (D+1)(D+2)/2 from the distances of k_myers.
+template <bool EMIT>
 __global__ void k_myers_trace(const unsigned long long* ha, const unsigned long long* la, const uint8_t* fa,
                               const unsigned long long* hb, const unsigned long long* lb, const uint8_t* fb,
                               int32_t pair0, int32_t n_pairs, int32_t* trace, const unsigned long long* trace_base,
                               const long long* added, const long long* removed, long long max_d, tsm_diff_detail* detail,
-                              const int32_t* todo) {
+                              const int32_t* todo, AssertSink sink) {
   const int slot = pair0 + ((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (slot >= pair0 + n_pairs) return;
   const int pr = todo ? todo[slot] : slot;                // trace_base is indexed by slot
@@ -328,6 +373,10 @@ __global__ void k_myers_trace(const unsigned long long* ha, const unsigned long 
     for (int k = 16; k; k >>= 1) { ca += __shfl_xor_sync(0xffffffffu, ca, k); cb += __shfl_xor_sync(0xffffffffu, cb, k); }
     if (n) { h_del = 1; r_as = ca; }
     if (m) { h_add = 1; a_as = cb; }
+    if constexpr (EMIT) {
+      sink_run(sink, 0, pr, la[pr], la[pr] + pre, qa, n, lane);
+      sink_run(sink, 1, pr, lb[pr], lb[pr] + pre, qb, m, lane);
+    }
   } else {
     int32_t* R = trace + trace_base[slot];
     int D = 0;
@@ -369,6 +418,10 @@ __global__ void k_myers_trace(const unsigned long long* ha, const unsigned long 
         in_hunk = true;
         if (down) { has_add = true; a_as += qb[py] != 0; }
         else { has_del = true; r_as += qa[px] != 0; }
+        if constexpr (EMIT) {
+          if (down && qb[py]) sink_put(sink, 1, sink_key(sink, 1, pr, lb[pr], lb[pr] + pre + py));
+          if (!down && qa[px]) sink_put(sink, 0, sink_key(sink, 0, pr, la[pr], la[pr] + pre + px));
+        }
         x = px; y = py;
       }
       if (in_hunk) { if (has_add && has_del) ++h_mod; else if (has_add) ++h_add; else ++h_del; }

@@ -17,10 +17,10 @@
 //
 //   tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N]
 //   tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]
-//   tosem-scan diff   <old-root> <new-root> [--out F]
+//   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F]
 //   tosem-scan body   <project-root>... [--out F]
 //   tosem-scan releases <snapshot-root>=<tag>... [--out F]   |   releases --git <repository> [<revision>...] [--out F]
-//   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F]
+//   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]
 #include <algorithm>
 #include <atomic>
 #include <cctype>
@@ -239,6 +239,17 @@ static void load_batch(const std::vector<FileEntry>& files, Batch& b) {
 static void cu_ck(cudaError_t e, const char* what) { if (e != cudaSuccess) die(std::string(what) + ": " + cudaGetErrorString(e)); }
 static void nccl_ck(ncclResult_t r, const char* what) { if (r != ncclSuccess) die(std::string(what) + ": " + ncclGetErrorString(r)); }
 
+// The statement of an assertion event (the statement may be longer than the 16-bit event field: its end is re-derived on the
+// host if saturated) and its category cell (the verbatim identifier for 127, docs/SPEC.md section 6).
+static std::string event_statement(const uint8_t* base, int32_t size, const tsm_assert_event& ev) {
+  uint32_t sl = ev.stmt_len;
+  if (sl == 65535) { const uint8_t* p = base + ev.stmt_off; uint32_t e = 0, last = 0; while (ev.stmt_off + e < (uint32_t)size && p[e] != '\n' && p[e] != '(') { if (!is_w(p[e])) last = e + 1; ++e; } sl = last; }
+  return std::string((const char*)base + ev.stmt_off, sl);
+}
+static std::string event_category(const uint8_t* base, const tsm_assert_event& ev) {
+  return ev.cat == 127 ? std::string((const char*)base + ev.ident_off, ev.ident_len) : std::string(tsm_category_name(ev.cat));
+}
+
 // The raw rows (fileName, extension, test_name, method, statement, counts, category: ML-Testing-v1.xlsx!apollo_tests:R1) and
 // the summary row (Id, FileName, total assert, assertion: Release-Meta-tpot.csv:1-2) of one file, from its events.
 static void render_file(const FileEntry& f, int64_t id, const uint8_t* base, int32_t size, uint32_t slot, const tsm_file_stat& st,
@@ -256,11 +267,7 @@ static void render_file(const FileEntry& f, int64_t id, const uint8_t* base, int
       cur_hdr = h.line_off; cur_fix = (h.kind & 1u) != 0;
       cur_method = method_string(f.ext, base + h.line_off, h.line_len);
     }
-    // the statement may be longer than the 16-bit event field: re-derive its end on the host if saturated
-    uint32_t sl = ev.stmt_len;
-    if (sl == 65535) { const uint8_t* p = base + ev.stmt_off; uint32_t e = 0, last = 0; while (ev.stmt_off + e < (uint32_t)size && p[e] != '\n' && p[e] != '(') { if (!is_w(p[e])) last = e + 1; ++e; } sl = last; }
-    std::string stmt((const char*)base + ev.stmt_off, sl);
-    std::string cat = ev.cat == 127 ? std::string((const char*)base + ev.ident_off, ev.ident_len) : std::string(tsm_category_name(ev.cat));
+    const std::string stmt = event_statement(base, size, ev), cat = event_category(base, ev);
     auto key = std::make_pair(cur_hdr, stmt);
     auto it = index.find(key);
     if (it == index.end()) { index[key] = rows.size(); rows.push_back({cur_hdr, stmt, ev.cat, cat, 1, cur_fix, cur_method}); }
@@ -1018,7 +1025,50 @@ static int cmd_releases(const std::vector<std::string>& specs_in, const std::str
 }
 
 // ---------------------------------------------------------------------------------- diff (S8)
-static int cmd_diff(const std::string& old_root, const std::string& new_root, const std::string& out_path) {
+// Changed assertion lines (docs/SPEC.md section 8) of one diff call: [n_groups][K] tables by group and the events of both
+// sides (tsm_diff_pairs_asserts), event arrays grown to the counts the library reports when they are too small.
+struct ChangedAsserts { std::vector<int64_t> added_counts, removed_counts; std::vector<tsm_assert_event> aev, rev; };
+static void diff_asserts(tsm_ctx* ctx, const tsm_corpus& ca, const tsm_corpus& cn, int64_t* added, int64_t* removed,
+                         tsm_diff_detail* det, ChangedAsserts& r) {
+  const size_t table = (size_t)ca.n_groups * TSM_NUM_CATEGORIES;
+  r.added_counts.assign(table, 0); r.removed_counts.assign(table, 0);
+  int64_t cap = ((int64_t)ca.off[ca.n_files] + cn.off[cn.n_files]) / 64 + 1024;
+  for (;;) {
+    r.aev.resize((size_t)cap); r.rev.resize((size_t)cap);
+    tsm_diff_asserts o{r.added_counts.data(), r.removed_counts.data(), r.aev.data(), cap, 0, r.rev.data(), cap, 0};
+    const int rc = tsm_diff_pairs_asserts(ctx, &ca, &cn, added, removed, det, &o, nullptr);
+    if (rc == TSM_E_CAPACITY && std::max(o.n_aev, o.n_rev) > cap) { cap = std::max(o.n_aev, o.n_rev); continue; }
+    ck(rc, "tsm_diff_pairs_asserts");
+    r.aev.resize((size_t)o.n_aev); r.rev.resize((size_t)o.n_rev);
+    return;
+  }
+}
+// The --asserts rows of pair `pair` on one side: `lead` cells, fileName, change ('+' new side, '-' old side), 1-based line
+// number in that side's file, statement, category.  `k` walks the side's events (canonical order) across calls.
+static void assert_rows(std::ostream& os, const std::vector<std::string>& lead, const std::string& path, const uint8_t* base,
+                        int32_t size, const std::vector<tsm_assert_event>& ev, size_t& k, uint32_t pair, const char* change) {
+  uint32_t pos = 0;
+  int64_t line = 1;
+  for (; k < ev.size() && ev[k].file == pair; ++k) {
+    const tsm_assert_event& e = ev[k];
+    for (; pos < e.line_off; ++pos) line += base[pos] == '\n';
+    std::vector<std::string> row = lead;
+    row.insert(row.end(), {path, change, std::to_string(line), event_statement(base, size, e), event_category(base, e)});
+    csv_row(os, row);
+  }
+}
+// The --assert-churn rows of one [K] pair of rows: every category with a changed line.
+static void churn_rows(std::ostream& os, const std::vector<std::string>& lead, const int64_t* added, const int64_t* removed) {
+  for (int k = 0; k < TSM_NUM_CATEGORIES; ++k)
+    if (added[k] || removed[k]) {
+      std::vector<std::string> row = lead;
+      row.insert(row.end(), {tsm_category_name(k), std::to_string(added[k]), std::to_string(removed[k])});
+      csv_row(os, row);
+    }
+}
+
+static int cmd_diff(const std::string& old_root, const std::string& new_root, const std::string& out_path,
+                    const std::string& asserts_path, const std::string& churn_path) {
   std::vector<FileEntry> a, b;
   walk(old_root, 0, true, a);
   walk(new_root, 0, true, b);
@@ -1082,8 +1132,25 @@ static int cmd_diff(const std::string& old_root, const std::string& new_root, co
   for (size_t i = 0; i < pairs.size(); ++i) { A.ext[i] = (uint8_t)ext_tag(pairs[i].rel); N.ext[i] = A.ext[i]; }
   std::vector<int64_t> added(pairs.size()), removed(pairs.size());
   std::vector<tsm_diff_detail> det(pairs.size());
-  ck(tsm_diff_pairs_detail(ctx, &ca, &cn, added.data(), removed.data(), det.data(), nullptr), "tsm_diff_pairs_detail");
+  ChangedAsserts ch;
+  if (asserts_path.empty() && churn_path.empty())
+    ck(tsm_diff_pairs_detail(ctx, &ca, &cn, added.data(), removed.data(), det.data(), nullptr), "tsm_diff_pairs_detail");
+  else diff_asserts(ctx, ca, cn, added.data(), removed.data(), det.data(), ch);
   tsm_destroy(ctx);
+  if (!asserts_path.empty()) {
+    std::ofstream as(asserts_path, std::ios::binary);
+    csv_row(as, {"fileName", "change", "line", "statement", "category"});
+    size_t ka = 0, kr = 0;
+    for (size_t i = 0; i < pairs.size(); ++i) {
+      assert_rows(as, {}, pairs[i].rel, A.arena + A.off[i], A.len[i], ch.rev, kr, (uint32_t)i, "-");
+      assert_rows(as, {}, pairs[i].rel, N.arena + N.off[i], N.len[i], ch.aev, ka, (uint32_t)i, "+");
+    }
+  }
+  if (!churn_path.empty()) {
+    std::ofstream cs(churn_path, std::ios::binary);
+    csv_row(cs, {"category", "added", "removed"});
+    churn_rows(cs, {}, ch.added_counts.data(), ch.removed_counts.data());
+  }
   std::ofstream os;
   if (!out_path.empty()) {
     os.open(out_path, std::ios::binary);
@@ -1142,7 +1209,7 @@ static void tree_diff(gitstore::Store& gs, const gitstore::Oid* a, const gitstor
 // --dry-run: no GPU - the rows carry the object names, sizes and an FNV-1a checksum of both blobs instead of the counts
 // (what the CPU tests compare with `git diff-tree` / `git cat-file`).
 static int cmd_history(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files, const std::string& out_path,
-                       bool dry_run) {
+                       bool dry_run, const std::string& asserts_path, const std::string& churn_path) {
   gitstore::Store gs;
   std::string err;
   if (!gs.open(repo, err)) die(err);
@@ -1175,6 +1242,14 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
     if (dry_run) csv_row(os, {"commit", "parent", "time", "fileName", "old_blob", "new_blob", "old_size", "new_size", "old_fnv", "new_fnv"});
     else csv_row(os, {"commit", "parent", "time", "fileName", "cloc", "added", "removed", "hunks_add", "hunks_del", "hunks_mod", "added_assert", "removed_assert"});
   }
+  const bool want_asserts = !dry_run && (!asserts_path.empty() || !churn_path.empty());
+  std::ofstream as;
+  if (!dry_run && !asserts_path.empty()) {
+    as.open(asserts_path, std::ios::binary);
+    csv_row(as, {"commit", "parent", "time", "fileName", "change", "line", "statement", "category"});
+  }
+  // per commit with changed assertion lines: its [K] added and removed rows (a commit's files may span two batches)
+  std::map<size_t, std::vector<int64_t>> churn;
   tsm_ctx* ctx = nullptr;
   if (!dry_run) ck(tsm_create(&ctx, 0, 1 << 20, 16, 1, 0), "tsm_create");
   std::vector<int64_t> per_add(chain.size(), 0), per_rem(chain.size(), 0), per_files(chain.size(), 0);
@@ -1186,8 +1261,9 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
     std::vector<std::vector<uint8_t>> bo, bn;
     std::vector<size_t> idx;
     int64_t so = 0, sn = 0;
-    size_t r1 = r0;
+    size_t r1 = r0, commits = 0;                           // with the assertion tables, a commit is a group: at most 65 535 per batch
     for (; r1 < rows.size() && so < kBatch && sn < kBatch; ++r1) {
+      if (want_asserts && (r1 == r0 || rows[r1].step != rows[r1 - 1].step) && ++commits > 65535) break;
       const BlobChange& c = rows[r1].ch;
       gitstore::Object x, y;
       if (c.has_o && (!gs.read(c.o, x) || x.type != gitstore::OBJ_BLOB)) die("unreadable blob " + c.o.hex());
@@ -1222,11 +1298,41 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
       };
       pack(A, bo); pack(N, bn);
       for (size_t i = 0; i < n; ++i) { A.ext[i] = (uint8_t)ext_tag(rows[idx[i]].ch.path); N.ext[i] = A.ext[i]; }
-      tsm_corpus ca{A.arena, A.off.data(), A.len.data(), A.ext.data(), A.grp.data(), (int32_t)n, 1};
-      tsm_corpus cn{N.arena, N.off.data(), N.len.data(), N.ext.data(), N.grp.data(), (int32_t)n, 1};
+      std::vector<size_t> group_step;                        // group g of the batch = commit group_step[g]
+      for (size_t i = 0; want_asserts && i < n; ++i) {
+        if (group_step.empty() || group_step.back() != rows[idx[i]].step) group_step.push_back(rows[idx[i]].step);
+        A.grp[i] = N.grp[i] = (uint16_t)(group_step.size() - 1);
+      }
+      const int32_t n_groups = want_asserts ? (int32_t)group_step.size() : 1;
+      tsm_corpus ca{A.arena, A.off.data(), A.len.data(), A.ext.data(), A.grp.data(), (int32_t)n, n_groups};
+      tsm_corpus cn{N.arena, N.off.data(), N.len.data(), N.ext.data(), N.grp.data(), (int32_t)n, n_groups};
       std::vector<int64_t> added(n), removed(n);
       std::vector<tsm_diff_detail> det(n);
-      ck(tsm_diff_pairs_detail(ctx, &ca, &cn, added.data(), removed.data(), det.data(), nullptr), "tsm_diff_pairs_detail");
+      ChangedAsserts chg;
+      if (!want_asserts) {
+        ck(tsm_diff_pairs_detail(ctx, &ca, &cn, added.data(), removed.data(), det.data(), nullptr), "tsm_diff_pairs_detail");
+      } else {
+        diff_asserts(ctx, ca, cn, added.data(), removed.data(), det.data(), chg);
+        for (size_t g = 0; g < group_step.size(); ++g) {
+          const int64_t* ad = chg.added_counts.data() + g * TSM_NUM_CATEGORIES;
+          const int64_t* rm = chg.removed_counts.data() + g * TSM_NUM_CATEGORIES;
+          if (std::all_of(ad, ad + TSM_NUM_CATEGORIES, [](int64_t v) { return v == 0; }) &&
+              std::all_of(rm, rm + TSM_NUM_CATEGORIES, [](int64_t v) { return v == 0; })) continue;
+          std::vector<int64_t>& t = churn[group_step[g]];
+          t.resize(2 * TSM_NUM_CATEGORIES, 0);
+          for (int k = 0; k < TSM_NUM_CATEGORIES; ++k) { t[(size_t)k] += ad[k]; t[(size_t)(TSM_NUM_CATEGORIES + k)] += rm[k]; }
+        }
+        if (as.is_open()) {
+          size_t ka = 0, kr = 0;
+          for (size_t i = 0; i < n; ++i) {
+            const Row& r = rows[idx[i]];
+            const Step& st = chain[r.step];
+            const std::vector<std::string> lead{st.id.hex(), st.c.parents.empty() ? "" : st.c.parents[0].hex(), std::to_string(st.c.time)};
+            assert_rows(as, lead, r.ch.path, A.arena + A.off[i], A.len[i], chg.rev, kr, (uint32_t)i, "-");
+            assert_rows(as, lead, r.ch.path, N.arena + N.off[i], N.len[i], chg.aev, ka, (uint32_t)i, "+");
+          }
+        }
+      }
       for (size_t i = 0; i < n; ++i) {
         const Row& r = rows[idx[i]];
         per_add[r.step] += added[i]; per_rem[r.step] += removed[i]; per_files[r.step]++;
@@ -1244,6 +1350,11 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
     r0 = r1;
   }
   if (ctx) tsm_destroy(ctx);
+  if (want_asserts && !churn_path.empty()) {
+    std::ofstream cs(churn_path, std::ios::binary);
+    csv_row(cs, {"commit", "category", "added", "removed"});
+    for (const auto& kv : churn) churn_rows(cs, {chain[kv.first].id.hex()}, kv.second.data(), kv.second.data() + TSM_NUM_CATEGORIES);
+  }
   printf("commit,files,cloc,added,removed\r\n");
   int64_t ta = 0, tr = 0;
   for (size_t i = 0; i < chain.size(); ++i) {
@@ -1260,10 +1371,10 @@ static void usage() {
   fprintf(stderr,
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
           "       tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]\n"
-          "       tosem-scan diff   <old-root> <new-root> [--out F]\n"
+          "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F]\n"
           "       tosem-scan body   <project-root>... [--out F]\n"
           "       tosem-scan releases <snapshot-root>=<tag>... [--out F]   |   releases --git <repository> [<revision>...] [--out F]\n"
-          "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F]\n"
+          "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
           "Scans run on the GPU through libtosemscan.so (sm_90a); there is no CPU fallback.\n");
 }
 
@@ -1287,8 +1398,9 @@ int main(int argc, char** argv) {
   if (cmd == "releases") { if (pos.empty() && !opt.count("--git")) die("releases needs <root>=<tag>... or --git <repository>"); return cmd_releases(pos, opt["--out"], opt["--git"]); }
   if (cmd == "body") { if (pos.empty()) die("body needs at least one project root"); return cmd_body(pos, opt["--out"]); }
   if (cmd == "history") { if (pos.size() != 1) die("history needs the repository"); return cmd_history(pos[0], opt.count("--rev") ? opt["--rev"] : "HEAD",
-                                                  opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0, all_files, opt["--out"], dry_run); }
-  if (cmd == "diff") { if (pos.size() != 2) die("diff needs <old-root> <new-root>"); return cmd_diff(pos[0], pos[1], opt["--out"]); }
+                                                  opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0, all_files, opt["--out"], dry_run,
+                                                  opt["--asserts"], opt["--assert-churn"]); }
+  if (cmd == "diff") { if (pos.size() != 2) die("diff needs <old-root> <new-root>"); return cmd_diff(pos[0], pos[1], opt["--out"], opt["--asserts"], opt["--assert-churn"]); }
   usage();
   return 2;
 }

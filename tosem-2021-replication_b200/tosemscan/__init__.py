@@ -33,7 +33,8 @@ DIFF_DETAIL = np.dtype([("hunks_add", "<i8"), ("hunks_del", "<i8"), ("hunks_mod"
 # every symbol include/tosemscan.h declares (tests check the library exports exactly these)
 SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create", "tsm_destroy", "tsm_scan",
            "tsm_upload", "tsm_scan_resident", "tsm_download", "tsm_device_counts", "tsm_last_launch_count", "tsm_last_kernel_ms", "tsm_kernel_ms_stats",
-           "tsm_diff_pairs", "tsm_diff_pairs_detail", "tsm_statements", "tsm_line_hashes", "tsm_diff_upload", "tsm_diff_resident", "tsm_diff_last_ms", "tsm_reduce", "tsm_host_alloc", "tsm_host_free", "tsm_layout", "tsm_gen_sizes",
+           "tsm_diff_pairs", "tsm_diff_pairs_detail", "tsm_statements", "tsm_line_hashes", "tsm_diff_upload", "tsm_diff_resident", "tsm_diff_last_ms",
+           "tsm_diff_pairs_asserts", "tsm_diff_resident_asserts", "tsm_reduce", "tsm_host_alloc", "tsm_host_free", "tsm_layout", "tsm_gen_sizes",
            "tsm_gen_fill", "tsm_gen_edit", "tsm_gen_pair_sizes", "tsm_gen_pair_fill"]
 
 
@@ -53,6 +54,12 @@ class _Result(C.Structure):
                 ("aev", C.c_void_p), ("aev_cap", C.c_int64), ("n_aev", C.c_int64),
                 ("hev", C.c_void_p), ("hev_cap", C.c_int64), ("n_hev", C.c_int64),
                 ("totals", C.c_int64 * 4)]
+
+
+class _DiffAsserts(C.Structure):
+    _fields_ = [("added_counts", C.c_void_p), ("removed_counts", C.c_void_p),
+                ("aev", C.c_void_p), ("aev_cap", C.c_int64), ("n_aev", C.c_int64),
+                ("rev", C.c_void_p), ("rev_cap", C.c_int64), ("n_rev", C.c_int64)]
 
 
 _lib = None
@@ -127,6 +134,11 @@ def lib():
         L.tsm_diff_upload.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus), C.c_void_p]
         L.tsm_diff_resident.restype = C.c_int
         L.tsm_diff_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.tsm_diff_pairs_asserts.restype = C.c_int
+        L.tsm_diff_pairs_asserts.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 3 + \
+            [C.POINTER(_DiffAsserts), C.c_void_p]
+        L.tsm_diff_resident_asserts.restype = C.c_int
+        L.tsm_diff_resident_asserts.argtypes = [C.c_void_p] * 4 + [C.POINTER(_DiffAsserts), C.c_void_p]
         L.tsm_diff_last_ms.restype = C.c_int
         L.tsm_diff_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 3)]
         _lib = L
@@ -509,12 +521,20 @@ class Scanner:
             raise TsmError(rc, "tsm_statements")
         return base, end[:n.value], kind[:n.value]
 
-    def diff_pairs(self, olds, news, stream=None, detail=False):
-        """S8 churn per pair; with detail=True also the hunks of the canonical edit script (SPEC section 8)."""
+    def diff_pairs(self, olds, news, stream=None, detail=False, asserts=False):
+        """S8 churn per pair; with detail=True also the hunks of the canonical edit script (SPEC section 8).  asserts=True:
+        (added, removed, detail, added_counts, removed_counts, added_events, removed_events) - the changed assertion lines,
+        as [n_groups][K] tables by the side's group and as events (inserted lines of `news`, deleted lines of `olds`)."""
         n = olds.n_files
         added = np.zeros(n, np.int64)
         removed = np.zeros(n, np.int64)
         a, b = olds.c_struct(), news.c_struct()
+        if asserts:
+            det = np.zeros(max(n, 1), DIFF_DETAIL)
+            cap = (olds.source_bytes + news.source_bytes) // 1024 + 4096   # a guess: more events cost one more call
+            return (added, removed, det[:n]) + self._diff_asserts(
+                lambda r: lib().tsm_diff_pairs_asserts(self._ctx, C.byref(a), C.byref(b), _p(added), _p(removed), _p(det), C.byref(r),
+                                                       stream), olds.n_groups, cap, "tsm_diff_pairs_asserts")
         if not detail:
             rc = lib().tsm_diff_pairs(self._ctx, C.byref(a), C.byref(b), _p(added), _p(removed), stream)
             if rc:
@@ -526,6 +546,25 @@ class Scanner:
             raise TsmError(rc, "tsm_diff_pairs_detail")
         return added, removed, det[:n]
 
+    @staticmethod
+    def _diff_asserts(call, n_groups, cap, what, events=None):
+        """(added_counts, removed_counts, added_events, removed_events) of one tsm_diff_*_asserts call; arrays too small for
+        the events (TSM_E_CAPACITY with both counts) are sized from the counts and the call is made again.  events(cap):
+        the two event arrays of at least cap entries (default: new arrays)."""
+        events = events or (lambda c: (np.zeros(max(c, 1), ASSERT_EVENT), np.zeros(max(c, 1), ASSERT_EVENT)))
+        for _ in range(2):
+            ac, rc_ = np.zeros((n_groups, K), np.int64), np.zeros((n_groups, K), np.int64)
+            aev, rev = events(cap)
+            r = _DiffAsserts(_p(ac), _p(rc_), _p(aev), cap, 0, _p(rev), cap, 0)
+            rc = call(r)
+            if rc == TSM_E_CAPACITY and max(r.n_aev, r.n_rev) > cap:
+                cap = int(max(r.n_aev, r.n_rev))
+                continue
+            if rc:
+                raise TsmError(rc, what)
+            return ac, rc_, aev[:r.n_aev], rev[:r.n_rev]
+        raise TsmError(TSM_E_CAPACITY, what)
+
     def diff_upload(self, olds, news, stream=None):
         """Both sides of the pairs to HBM, kept by the ctx (tsm_diff_upload)."""
         a, b = olds.c_struct(), news.c_struct()
@@ -533,19 +572,38 @@ class Scanner:
         if rc:
             raise TsmError(rc, "tsm_diff_upload")
         self._pairs = olds.n_files
+        self._pair_groups = olds.n_groups
+        self._pair_bytes = olds.source_bytes + news.source_bytes
         n = max(self._pairs, 1)                              # results land in pinned memory: D2H at the PCIe rate, no staging copy
         bufs = [host_buffer(n * 8), host_buffer(n * 8), host_buffer(n * DIFF_DETAIL.itemsize)]
         self._diff_pins = [b[1] for b in bufs]
         self._diff_out = (bufs[0][0][:self._pairs * 8].view(np.int64), bufs[1][0][:self._pairs * 8].view(np.int64),
                           bufs[2][0][:n * DIFF_DETAIL.itemsize].view(DIFF_DETAIL))
 
-    def diff_resident(self, detail=True, stream=None):
-        """The diff kernels over the resident sides; returns (added, removed[, detail]) - buffers reused across calls."""
+    def diff_resident(self, detail=True, stream=None, asserts=False, event_cap=None):
+        """The diff kernels over the resident sides; returns (added, removed[, detail]) - buffers reused across calls.
+        asserts=True: (added, removed, detail, added_counts, removed_counts, added_events, removed_events) as diff_pairs; the
+        event arrays are pinned buffers kept by the Scanner too (valid until the next such call)."""
         added, removed, det = self._diff_out
+        if asserts:
+            cap = int(event_cap if event_cap is not None else self._pair_bytes // 1024 + 4096)
+            return (added, removed, det[:self._pairs]) + self._diff_asserts(
+                lambda r: lib().tsm_diff_resident_asserts(self._ctx, _p(added), _p(removed), _p(det), C.byref(r), stream),
+                self._pair_groups, cap, "tsm_diff_resident_asserts", self._event_buffers)
         rc = lib().tsm_diff_resident(self._ctx, _p(added), _p(removed), _p(det) if detail else None, stream)
         if rc:
             raise TsmError(rc, "tsm_diff_resident")
         return (added, removed, det[:self._pairs]) if detail else (added, removed)
+
+    def _event_buffers(self, cap):
+        """Two pinned event arrays of at least cap entries, grown when a call needs more (a fresh pageable array per call
+        costs more host time than the classification of a C5 batch)."""
+        if getattr(self, "_ev_cap", 0) < cap:
+            bufs = [host_buffer(cap * ASSERT_EVENT.itemsize) for _ in range(2)]
+            self._ev_pins = [b[1] for b in bufs]
+            self._ev_bufs = tuple(b[0][:cap * ASSERT_EVENT.itemsize].view(ASSERT_EVENT) for b in bufs)
+            self._ev_cap = cap
+        return self._ev_bufs
 
     def diff_last_ms(self):
         """Device time of the last diff call: [k_scan over both sides, k_diff_small, k_myers + k_myers_trace of the pairs it left over] in ms."""
