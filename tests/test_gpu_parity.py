@@ -1,5 +1,7 @@
 """GPU parity tests: the sm_90a product path, through the C ABI, against the CPU oracle on the
 same seeded inputs.  Integer / byte work: the bar is bit-exact equality of every output."""
+import ctypes as C
+
 import numpy as np
 import pytest
 
@@ -230,6 +232,116 @@ def test_errors_are_reported_not_swallowed(scanner):
         small.scan(ts.pack([b"x" * 9000], [1]))
     assert e.value.status == -3
     small.close()
+
+
+OK, ARG, LAYOUT = 0, -1, -2
+FAULTS = ("none", "misaligned_off", "negative_off", "negative_len", "runs_into_next", "off_far_past_arena", "misaligned_end",
+          "ext_7", "ext_null", "grp_out_of_range", "no_groups", "groups_mismatch", "groups_mismatch_and_misaligned_off")
+# status per fault (in FAULTS order) of every corpus-taking entry point; diff_resident(_asserts) follow a diff_upload of a
+# clean pair and then one of the faulty pair, so that a rejected upload shows that the ctx keeps the clean one
+STATUS = {
+    "scan":                  (OK, LAYOUT, LAYOUT, LAYOUT, LAYOUT, LAYOUT, LAYOUT, LAYOUT, ARG, LAYOUT, ARG, OK, LAYOUT),
+    "upload":                (OK, LAYOUT, LAYOUT, LAYOUT, LAYOUT, LAYOUT, LAYOUT, LAYOUT, ARG, LAYOUT, ARG, OK, LAYOUT),
+    "diff_pairs":            (OK, LAYOUT, LAYOUT, LAYOUT, LAYOUT, LAYOUT, OK, OK, OK, OK, OK, OK, LAYOUT),
+    "diff_pairs_detail":     (OK, LAYOUT, LAYOUT, LAYOUT, LAYOUT, LAYOUT, OK, LAYOUT, OK, OK, OK, OK, LAYOUT),
+    "diff_pairs_asserts":    (OK, LAYOUT, LAYOUT, LAYOUT, LAYOUT, LAYOUT, OK, LAYOUT, OK, LAYOUT, ARG, ARG, ARG),
+    "diff_upload":           (OK, LAYOUT, LAYOUT, LAYOUT, LAYOUT, LAYOUT, OK, LAYOUT, OK, OK, OK, OK, LAYOUT),
+    "diff_resident":         (OK, OK, OK, OK, OK, OK, OK, OK, OK, OK, OK, OK, OK),
+    "diff_resident_asserts": (OK, OK, OK, OK, OK, OK, OK, OK, OK, LAYOUT, LAYOUT, ARG, OK),
+    "line_hashes":           (OK, LAYOUT, LAYOUT, LAYOUT, LAYOUT, LAYOUT, OK, LAYOUT, OK, OK, OK, OK, LAYOUT),
+    "statements":            (OK, LAYOUT, LAYOUT, LAYOUT, LAYOUT, LAYOUT, OK, OK, OK, OK, OK, OK, LAYOUT),
+}
+
+
+def _fault_corpus(files, fault):
+    """Three files in an arena with room past off[n], n_groups 2, and one fault of the layout or tag rules (SPEC section 1).
+    Returns the tsm_corpus and the arrays it points into."""
+    off = np.array([0, 128, 256, 384], np.int32)
+    arena = np.zeros(1024, np.uint8)
+    for o, f in zip(off, files):
+        arena[o:o + len(f)] = np.frombuffer(f, np.uint8)
+    a = {"arena": arena, "off": off, "len": np.array([len(f) for f in files], np.int32), "ext": np.ones(3, np.uint8),
+         "grp": np.array([0, 1, 0], np.uint16)}
+    n_groups = 2
+    if fault in ("misaligned_off", "groups_mismatch_and_misaligned_off"):
+        off[1] = 130
+    elif fault == "negative_off":
+        off[0] = -128
+    elif fault == "negative_len":
+        a["len"][1] = -1
+    elif fault == "runs_into_next":
+        a["len"][1] = 200
+    elif fault == "off_far_past_arena":
+        off[1] = 2 ** 31 - 128
+    elif fault == "misaligned_end":
+        off[3] = 385
+    elif fault == "ext_7":
+        a["ext"][1] = 7
+    elif fault == "ext_null":
+        a["ext"] = None
+    elif fault == "grp_out_of_range":
+        a["grp"][1] = 2
+    elif fault == "no_groups":
+        n_groups = 0
+    if fault.startswith("groups_mismatch"):
+        n_groups = 3
+    k = ts._Corpus(*(ts._p(a[f]) for f in ("arena", "off", "len", "ext", "grp")), 3, n_groups)
+    return k, a
+
+
+def _call(entry, ctx, old, new, clean):
+    """One call of `entry` on the corpus `new` (pair calls: on the pair (old, new)); returns its status."""
+    L = ts.lib()
+    add, rem, det = np.zeros(3, np.int64), np.zeros(3, np.int64), np.zeros(3, ts.DIFF_DETAIL)
+    tables = np.zeros((2, 3 * ts.K), np.int64)
+    out, res = ts._DiffAsserts(ts._p(tables[0]), ts._p(tables[1]), None, 0, 0, None, 0, 0), ts._Result()
+    base, n_lines = np.zeros(4, np.int64), C.c_int64()
+    line_end, line_kind = np.zeros(256, np.uint32), np.zeros(256, np.uint8)
+    o, k = C.byref(old), C.byref(new)
+    if entry == "scan":
+        return L.tsm_scan(ctx, k, C.byref(res), 0, None)
+    if entry == "upload":
+        return L.tsm_upload(ctx, k, None)
+    if entry == "diff_pairs":
+        return L.tsm_diff_pairs(ctx, o, k, ts._p(add), ts._p(rem), None)
+    if entry == "diff_pairs_detail":
+        return L.tsm_diff_pairs_detail(ctx, o, k, ts._p(add), ts._p(rem), ts._p(det), None)
+    if entry == "diff_pairs_asserts":
+        return L.tsm_diff_pairs_asserts(ctx, o, k, ts._p(add), ts._p(rem), None, C.byref(out), None)
+    if entry == "diff_upload":
+        return L.tsm_diff_upload(ctx, o, k, None)
+    if entry.startswith("diff_resident"):
+        assert L.tsm_diff_upload(ctx, C.byref(clean), C.byref(clean), None) == OK
+        L.tsm_diff_upload(ctx, o, k, None)
+        if entry == "diff_resident":
+            return L.tsm_diff_resident(ctx, ts._p(add), ts._p(rem), ts._p(det), None)
+        return L.tsm_diff_resident_asserts(ctx, ts._p(add), ts._p(rem), ts._p(det), C.byref(out), None)
+    if entry == "line_hashes":
+        return L.tsm_line_hashes(ctx, k, ts._p(base), None, None, None, 256, C.byref(n_lines), 0, None, None)
+    assert entry == "statements"
+    return L.tsm_statements(ctx, k, ts._p(base), ts._p(line_end), ts._p(line_kind), 256, C.byref(n_lines), None)
+
+
+@pytest.mark.parametrize("entry", sorted(STATUS))
+def test_layout_and_tag_faults_give_the_same_status_everywhere(entry):
+    """The exact status of every corpus-taking entry point for one fault at a time: which of the rules (ext, grp, n_groups,
+    off[n]) each call checks, and in which order.  A pair call gets the fault on either side, the other side none (for
+    no_groups: n_groups 0 as well)."""
+    old_files = [b"assert x == 1\n", b"def test_a():\n    self.assertTrue(y)\n", b"x = 1\n"]
+    new_files = [b"assert x == 2\n", b"def test_a():\n    assert y\n    z = 1\n", b"x = 1\ny = 2\n"]
+    sc = ts.Scanner(device=0, max_arena_bytes=1 << 20, max_files=16, max_groups=4)
+    clean, clean_arrays = _fault_corpus(new_files, "none")
+    bad = {}
+    for fault, want in zip(FAULTS, STATUS[entry]):
+        partner = "no_groups" if fault == "no_groups" else "none"
+        for faulty in ("new", "old") if entry.startswith("diff") else ("new",):
+            old, old_arrays = _fault_corpus(old_files, fault if faulty == "old" else partner)
+            new, new_arrays = _fault_corpus(new_files, fault if faulty == "new" else partner)
+            got = _call(entry, sc._ctx, old, new, clean)
+            if got != want:
+                bad[fault, faulty] = (got, want)
+    sc.close()
+    assert not bad, bad
 
 
 def _pairs(seed, n, size_cap, lam=6.0):

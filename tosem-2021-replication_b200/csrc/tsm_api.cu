@@ -67,7 +67,7 @@ struct SyncGuard {                                        // error paths: wait f
 struct tsm_ctx {
   int device = 0;
   ScratchPool pool;
-  int cls_grid = 0; size_t cls_smem = (size_t)-1;        // launch shape of k_classify for the current histogram size
+  int cls_per_sm = 0; size_t cls_smem = (size_t)-1;      // resident k_classify blocks per SM at cls_smem bytes of histogram
   int sms = 0;
   int64_t max_arena = 0;
   int32_t max_files = 0, max_groups = 0;
@@ -293,8 +293,11 @@ extern "C" int tsm_create(tsm_ctx** out, int device, int64_t max_arena_bytes, in
   return TSM_OK;
 }
 
-// Layout rules of docs/SPEC.md section 1.  The O(1) part, and the per-file part over [f0, f1) (prev_end carries the end of
-// the file in front): tsm_scan checks a slab's files while the slab in front of it is on the wire.
+// Layout rules of docs/SPEC.md section 1.  check_corpus_head: the O(1) part, for the scan's corpus.  check_files: the
+// per-file part over files [f0, f1) - aligned starts, every file inside [off[i], off[i+1]) (so the offsets ascend and no
+// file runs into the next), and the range inside the arena (off[f1] <= off[n_files]: tsm_scan copies a slab's bytes
+// [off[f0], off[f1]) before it has checked the files behind the slab) - plus, as the caller asks, every ext <= TSM_EXT_H
+// (if ext is given) and check_groups.  tsm_scan checks a slab's files while the slab in front of it is on the wire.
 static int check_corpus_head(const tsm_ctx* c, const tsm_corpus* k) {
   if (!k || k->n_files < 0 || k->n_groups < 1 || (k->n_files > 0 && (!k->arena || !k->off || !k->len || !k->ext)))
     return TSM_E_ARG;
@@ -305,44 +308,49 @@ static int check_corpus_head(const tsm_ctx* c, const tsm_corpus* k) {
   if (total > c->max_arena) return TSM_E_CAPACITY;
   return TSM_OK;
 }
-static int check_files(const tsm_corpus* k, int32_t f0, int32_t f1, int64_t& prev_end) {
-  const int64_t total = k->off[k->n_files];
-  for (int32_t i = f0; i < f1; ++i) {
-    const int64_t o = k->off[i], l = k->len[i];
-    if (o < prev_end || (o & (TSM_ALIGN - 1)) || l < 0 || o + l > (int64_t)k->off[i + 1] || (int64_t)k->off[i + 1] > total) return TSM_E_LAYOUT;
-    if (k->grp && k->grp[i] >= k->n_groups) return TSM_E_LAYOUT;
-    if (k->ext[i] > TSM_EXT_H) return TSM_E_LAYOUT;
-    prev_end = o + l;
-  }
+static int check_groups(const tsm_corpus* k, int32_t f0, int32_t f1) {   // every grp of files [f0, f1) below n_groups
+  if (k->n_groups < 1) return TSM_E_ARG;
+  if (k->grp)
+    for (int32_t i = f0; i < f1; ++i)
+      if (k->grp[i] >= k->n_groups) return TSM_E_LAYOUT;
   return TSM_OK;
 }
-static int check_corpus(const tsm_ctx* c, const tsm_corpus* k) {
-  int rc = check_corpus_head(c, k);
-  if (rc != TSM_OK || k->n_files == 0) return rc;
-  int64_t prev_end = 0;
-  rc = check_files(k, 0, k->n_files, prev_end);
-  if (rc == TSM_OK && prev_end > (int64_t)k->off[k->n_files]) rc = TSM_E_LAYOUT;
-  return rc;
+static int check_files(const tsm_corpus* k, int32_t f0, int32_t f1, bool ext_rule, bool grp_rule) {
+  for (int32_t i = f0; i < f1; ++i) {
+    const int64_t o = k->off[i], l = k->len[i];
+    if (o < 0 || (o & (TSM_ALIGN - 1)) || l < 0 || o + l > (int64_t)k->off[i + 1] || (ext_rule && k->ext && k->ext[i] > TSM_EXT_H))
+      return TSM_E_LAYOUT;
+  }
+  if (f0 < f1 && k->off[f1] > k->off[k->n_files]) return TSM_E_LAYOUT;
+  return grp_rule ? check_groups(k, f0, f1) : TSM_OK;
 }
 
-extern "C" int tsm_upload(tsm_ctx* c, const tsm_corpus* k, void* stream) {
-  if (!c) return TSM_E_ARG;
-  int rc = check_corpus(c, k);
-  if (rc != TSM_OK) return rc;
-  CU(cudaSetDevice(c->device));
-  cudaStream_t st = (cudaStream_t)stream;
+// The file index (off, len, ext, grp; NULL grp = all 0) to the ctx, which takes the corpus' sizes.
+static int upload_index(tsm_ctx* c, const tsm_corpus* k, cudaStream_t st) {
   const int32_t n = k->n_files;
   c->n_files = n;
   c->n_groups = k->n_groups;
   c->arena_bytes = n ? k->off[n] : 0;
   if (n) {
-    CU(cudaMemcpyAsync(c->d_arena, k->arena, (size_t)c->arena_bytes, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(c->d_off, k->off, sizeof(int32_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(c->d_len, k->len, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(c->d_ext, k->ext, (size_t)n, cudaMemcpyHostToDevice, st));
     if (k->grp) CU(cudaMemcpyAsync(c->d_grp, k->grp, sizeof(uint16_t) * (size_t)n, cudaMemcpyHostToDevice, st));
     else CU(cudaMemsetAsync(c->d_grp, 0, sizeof(uint16_t) * (size_t)n, st));
   }
+  return TSM_OK;
+}
+
+extern "C" int tsm_upload(tsm_ctx* c, const tsm_corpus* k, void* stream) {
+  if (!c) return TSM_E_ARG;
+  int rc = check_corpus_head(c, k);
+  if (rc == TSM_OK) rc = check_files(k, 0, k->n_files, true, true);
+  if (rc != TSM_OK) return rc;
+  CU(cudaSetDevice(c->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = upload_index(c, k, st);
+  if (rc != TSM_OK) return rc;
+  if (c->n_files) CU(cudaMemcpyAsync(c->d_arena, k->arena, (size_t)c->arena_bytes, cudaMemcpyHostToDevice, st));
   c->resident = true;
   c->scanned = false;
   return TSM_OK;
@@ -356,8 +364,8 @@ static int ensure_event_buffers(tsm_ctx* c, uint32_t flags) {
   return TSM_OK;
 }
 
-static ScanParams make_params(const tsm_ctx* c, uint32_t flags) {
-  ScanParams p;
+static ScanParams make_params(const tsm_ctx* c, uint32_t flags) {   // the ScanParams of a scan of the ctx's corpus
+  ScanParams p{};
   p.arena = c->d_arena; p.off = c->d_off; p.len = c->d_len; p.ext = c->d_ext; p.grp = c->d_grp;
   p.n_files = c->n_files; p.n_groups = c->n_groups;
   p.unit_file = c->d_unit_file; p.unit_begin = c->d_unit_begin; p.unit_cap = c->unit_cap;
@@ -367,6 +375,17 @@ static ScanParams make_params(const tsm_ctx* c, uint32_t flags) {
   p.aev = c->d_aev; p.aev_cap = (uint32_t)c->max_events;
   p.counts = c->d_counts; p.flags = flags; p.four = 4; p.cls_last = 1;
   return p;
+}
+
+// Resident blocks of k_classify per SM at `smem` bytes of dynamic shared memory (the query is cached for the last size).
+static int classify_per_sm(tsm_ctx* c, size_t smem) {
+  if (c->cls_smem != smem) {
+    int per_sm = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_classify_t<false>, 256, smem) != cudaSuccess || per_sm < 1) per_sm = 4;
+    c->cls_per_sm = per_sm;
+    c->cls_smem = smem;
+  }
+  return c->cls_per_sm;
 }
 
 // One scan = [memsets] + per slab (k_plan, k_scan) + k_classify on `st`.  With host != NULL
@@ -402,18 +421,12 @@ static int launch_scan(tsm_ctx* c, uint32_t flags, cudaStream_t st, const tsm_co
     CU(cudaEventRecord(ev[0], st));
     const int n_slabs = (int)cut.size() - 1;
     const size_t hist = CLS_SMEM_BASE + sizeof(uint32_t) * (c->n_groups <= 16 ? (size_t)c->n_groups * TSM_K : 0);
-    if (c->cls_smem != hist) {                           // one resident wave of k_classify (grid-stride inside)
-      int per_sm = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_classify_t<false>, 256, hist) != cudaSuccess || per_sm < 1) per_sm = 4;
-      c->cls_grid = c->sms * per_sm;
-      c->cls_smem = hist;
-    }
-    int64_t prev_end = 0;
+    const int cls_grid = c->sms * classify_per_sm(c, hist);   // one resident wave of k_classify (grid-stride inside)
     for (int s = 0; s < n_slabs; ++s) {
       const int32_t f0 = cut[(size_t)s], f1 = cut[(size_t)s + 1];
       if (host) {
         if (check_files_here && s == 0) {                  // the first slab's files before anything of them is used ...
-          const int rc0 = check_files(host, f0, f1, prev_end);
+          const int rc0 = check_files(host, f0, f1, true, true);
           if (rc0 != TSM_OK) return rc0;
         }
         const size_t b0 = (size_t)host->off[f0], b1 = (size_t)host->off[f1];
@@ -421,7 +434,7 @@ static int launch_scan(tsm_ctx* c, uint32_t flags, cudaStream_t st, const tsm_co
         CU(cudaEventRecord(c->slab_ev[s], c->copy_stream));
         CU(cudaStreamWaitEvent(st, c->slab_ev[s], 0));
         if (check_files_here && s + 1 < n_slabs) {         // ... the next slab's while this one is on the wire
-          const int rc1 = check_files(host, f1, cut[(size_t)s + 2], prev_end);
+          const int rc1 = check_files(host, f1, cut[(size_t)s + 2], true, true);
           if (rc1 != TSM_OK) { cudaStreamSynchronize(c->copy_stream); cudaStreamSynchronize(st); return rc1; }
         }
       }
@@ -436,16 +449,16 @@ static int launch_scan(tsm_ctx* c, uint32_t flags, cudaStream_t st, const tsm_co
       CU(cudaGetLastError());
       if (s + 1 < n_slabs) {                               // streamed scan: this slab's candidates are classified under the next
         p.cls_last = 0;                                    // slab's copy, so that only the last slab's are left behind the last copy
-        if (flags & TSM_SCAN_REV_B) k_classify_t<true><<<c->cls_grid, 256, hist, st>>>(p);
-        else k_classify_t<false><<<c->cls_grid, 256, hist, st>>>(p);
+        if (flags & TSM_SCAN_REV_B) k_classify_t<true><<<cls_grid, 256, hist, st>>>(p);
+        else k_classify_t<false><<<cls_grid, 256, hist, st>>>(p);
         CU(cudaGetLastError());
         p.cls_last = 1;
       }
     }
     if (n_slabs > 1) CU(cudaEventRecord(ev[1], st));      // per-kernel split is only meaningful for one slab
     CU(cudaEventRecord(ev[2], st));
-    if (flags & TSM_SCAN_REV_B) k_classify_t<true><<<c->cls_grid, 256, hist, st>>>(p);
-    else k_classify_t<false><<<c->cls_grid, 256, hist, st>>>(p);
+    if (flags & TSM_SCAN_REV_B) k_classify_t<true><<<cls_grid, 256, hist, st>>>(p);
+    else k_classify_t<false><<<cls_grid, 256, hist, st>>>(p);
     CU(cudaGetLastError());
     CU(cudaEventRecord(ev[3], st));
     CU(cudaEventRecord(ev[4], st));                           // (slot of the former k_totals, now fused into k_classify)
@@ -549,6 +562,23 @@ static int download_tables(tsm_ctx* c, tsm_result* r, cudaStream_t st) {
   return TSM_OK;
 }
 
+// Events (any order, file < n_files) into the canonical (file, line_off) order: a counting sort by file, then the few events
+// of each file by line_off.  A comparison sort of the whole array costs milliseconds for a C5 batch; this is linear.
+template <typename Event> static void sort_events_by_file(Event* ev, uint32_t m, int32_t n_files) {
+  if (m < 2) return;
+  std::vector<uint32_t> pos((size_t)n_files + 1, 0);
+  for (uint32_t i = 0; i < m; ++i) pos[(size_t)ev[i].file + 1]++;
+  for (int32_t f = 0; f < n_files; ++f) pos[(size_t)f + 1] += pos[(size_t)f];
+  std::vector<Event> tmp(m);
+  std::vector<uint32_t> at(pos.begin(), pos.end() - 1);
+  for (uint32_t i = 0; i < m; ++i) tmp[at[ev[i].file]++] = ev[i];
+  for (int32_t f = 0; f < n_files; ++f)
+    if (pos[(size_t)f + 1] - pos[(size_t)f] > 1)
+      std::sort(tmp.begin() + pos[(size_t)f], tmp.begin() + pos[(size_t)f + 1],
+                [](const Event& a, const Event& b) { return a.line_off < b.line_off; });
+  std::copy(tmp.begin(), tmp.end(), ev);
+}
+
 extern "C" int tsm_download(tsm_ctx* c, tsm_result* r, void* stream) {
   if (!c || !r) return TSM_E_ARG;
   if (!c->scanned) return TSM_E_STATE;
@@ -571,19 +601,17 @@ extern "C" int tsm_download(tsm_ctx* c, tsm_result* r, void* stream) {
     return TSM_E_CAPACITY;
   }
   if (want_aev) {
-    const int64_t m = c->h_ctrl->n_aev;
+    const uint32_t m = c->h_ctrl->n_aev;
     CU(cudaMemcpyAsync(r->aev, c->d_aev, sizeof(tsm_assert_event) * (size_t)m, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    std::sort(r->aev, r->aev + m, [](const tsm_assert_event& a, const tsm_assert_event& b) {
-      return a.file != b.file ? a.file < b.file : a.line_off < b.line_off; });
+    sort_events_by_file(r->aev, m, c->n_files);
     r->n_aev = m;
   } else if (c->last_flags & TSM_SCAN_ASSERT_EVENTS) r->n_aev = c->h_ctrl->n_aev;
   if (want_hev) {
-    const int64_t m = c->h_ctrl->n_hev;
+    const uint32_t m = c->h_ctrl->n_hev;
     CU(cudaMemcpyAsync(r->hev, c->d_hev, sizeof(tsm_header_event) * (size_t)m, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    std::sort(r->hev, r->hev + m, [](const tsm_header_event& a, const tsm_header_event& b) {
-      return a.file != b.file ? a.file < b.file : a.line_off < b.line_off; });
+    sort_events_by_file(r->hev, m, c->n_files);
     r->n_hev = m;
   } else if (c->last_flags & TSM_SCAN_HEADER_EVENTS) r->n_hev = c->h_ctrl->n_hev;
   return TSM_OK;
@@ -596,17 +624,8 @@ extern "C" int tsm_scan(tsm_ctx* c, const tsm_corpus* k, tsm_result* r, uint32_t
   flags &= TSM_SCAN_ASSERT_EVENTS | TSM_SCAN_HEADER_EVENTS | TSM_SCAN_REV_B;
   CU(cudaSetDevice(c->device));
   cudaStream_t st = (cudaStream_t)stream;
-  const int32_t n = k->n_files;
-  c->n_files = n;
-  c->n_groups = k->n_groups;
-  c->arena_bytes = n ? k->off[n] : 0;
-  if (n) {                                                // the index first (small), the arena slab by slab
-    CU(cudaMemcpyAsync(c->d_off, k->off, sizeof(int32_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(c->d_len, k->len, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(c->d_ext, k->ext, (size_t)n, cudaMemcpyHostToDevice, st));
-    if (k->grp) CU(cudaMemcpyAsync(c->d_grp, k->grp, sizeof(uint16_t) * (size_t)n, cudaMemcpyHostToDevice, st));
-    else CU(cudaMemsetAsync(c->d_grp, 0, sizeof(uint16_t) * (size_t)n, st));
-  }
+  rc = upload_index(c, k, st);                            // the index first (small), the arena slab by slab
+  if (rc != TSM_OK) return rc;
   c->resident = true;
   rc = launch_scan(c, flags, st, k, true);
   if (rc != TSM_OK) { c->resident = false; c->scanned = false; return rc; }
@@ -670,6 +689,11 @@ extern "C" void* tsm_host_alloc(int64_t bytes) {
 extern "C" void tsm_host_free(void* p) { if (p) cudaFreeHost(p); }
 
 // ------------------------------------------------------------------------------------- S8 diff
+static float elapsed_ms(cudaEvent_t from, cudaEvent_t to) {   // 0 if the pair cannot be timed
+  float ms = 0;
+  return cudaEventElapsedTime(&ms, from, to) == cudaSuccess ? ms : 0.f;
+}
+
 namespace {
 struct HostSide {                                         // device image of one side of the pairs + its line records
   int32_t n = 0; size_t ab = 0; uint32_t unit_cap = 0;
@@ -684,6 +708,13 @@ struct HostSide {                                         // device image of one
   int launches = 0;
   void drop_staging() { s_hash.reset(); s_end.reset(); s_flag.reset(); }
 };
+
+static ScanParams side_params(const HostSide& h) {        // the ScanParams over an uploaded side: the caller adds the rest
+  ScanParams p{};
+  p.arena = h.arena.as<uint8_t>(); p.off = h.off.as<int32_t>(); p.len = h.len.as<int32_t>(); p.ext = h.ext.as<uint8_t>();
+  p.n_files = h.n; p.four = 4;
+  return p;
+}
 
 // Exclusive scan of n u32 counts into n + 1 u64 (tsm_lines_kernels.cuh); bsum holds n / 1024 + 2 u64.
 static void xscan(const uint32_t* in, uint32_t n, unsigned long long* bsum, unsigned long long* out, cudaStream_t st) {
@@ -768,15 +799,13 @@ int sides_records(tsm_ctx* c, HostSide* const* sides, int ns, cudaStream_t st, f
     HostSide& h = *sides[i];
     const int32_t n = h.n;
     ScanParams& p = ps[i];
-    p = ScanParams{};
-    p.arena = h.arena.as<uint8_t>(); p.off = h.off.as<int32_t>(); p.len = h.len.as<int32_t>(); p.ext = h.ext.as<uint8_t>();
-    p.grp = nullptr; p.n_files = n; p.n_groups = 1;
+    p = side_params(h);
+    p.n_groups = 1;
     p.unit_file = h.unit_file.as<uint32_t>(); p.unit_begin = h.unit_begin.as<uint32_t>(); p.unit_cap = h.unit_cap;
     p.ctrl = reinterpret_cast<Ctrl*>(h.zero.as<uint8_t>()); p.slab = reinterpret_cast<SlabCtl*>(h.zero.as<uint8_t>() + 256);
-    p.f_begin = 0; p.f_end = n; p.unit_base = 0;
+    p.f_end = n;
     p.stats = h.stats.as<tsm_file_stat>();
-    p.cand = nullptr; p.cand_cap = 0; p.hev = nullptr; p.hev_cap = 0; p.aev = nullptr; p.aev_cap = 0; p.counts = nullptr;
-    p.flags = TSM_SCAN_LINE_HASHES; p.four = 4;
+    p.flags = TSM_SCAN_LINE_HASHES;
     p.unit_lines = h.unit_lines.as<uint32_t>(); p.unit_out = h.unit_out.as<uint32_t>();
     // units in (file, chunk) order
     k_file_units<<<(n + 255) / 256, 256, 0, st>>>(p.len, (uint32_t)n, h.cnt.as<uint32_t>());
@@ -790,14 +819,14 @@ int sides_records(tsm_ctx* c, HostSide* const* sides, int ns, cudaStream_t st, f
     HostSide& h = *sides[i];
     const int ev = i ? 6 : 0;
     h.hc = *h.pin_hc; h.total = *h.pin_total;
-    if (scan_ms) { float ms = 0; if (cudaEventElapsedTime(&ms, c->diff_ev[ev], c->diff_ev[ev + 1]) == cudaSuccess) *scan_ms += ms; }
+    if (scan_ms) *scan_ms += elapsed_ms(c->diff_ev[ev], c->diff_ev[ev + 1]);
     if (h.hc.overflow) return TSM_E_CAPACITY;
     if (h.hc.lh_overflow) {                                // more lines than the staging arrays hold: once more, exact size
       const int rc = side_scan_pass(c, h, ps[i], (size_t)h.hc.n_lh + 64, i, st);
       if (rc != TSM_OK) return rc;
       CU(cudaStreamSynchronize(st));
       h.hc = *h.pin_hc; h.total = *h.pin_total;
-      if (scan_ms) { float ms = 0; if (cudaEventElapsedTime(&ms, c->diff_ev[ev], c->diff_ev[ev + 1]) == cudaSuccess) *scan_ms += ms; }
+      if (scan_ms) *scan_ms += elapsed_ms(c->diff_ev[ev], c->diff_ev[ev + 1]);
       if (h.hc.overflow || h.hc.lh_overflow) return TSM_E_CAPACITY;
     }
   }
@@ -844,7 +873,7 @@ int side_records(tsm_ctx* c, HostSide& h, cudaStream_t st, float* scan_ms) {
 }  // namespace
 
 struct HostSidePair {
-  HostSide A, B; int32_t n = 0; bool have_records = false;
+  HostSide A, B; int32_t n = 0;
   int32_t groups_a = 1, groups_b = 1; bool grp_ok = true;  // n_groups of both sides, every grp < n_groups (for the assertion tables)
 };
 
@@ -855,24 +884,27 @@ static void free_res_pair(tsm_ctx* c) {
   c->res_pair = nullptr;
 }
 
-static int check_groups(const tsm_corpus* k) {           // SPEC section 1: every grp below n_groups
-  if (k->n_groups < 1) return TSM_E_ARG;
-  if (k->grp)
-    for (int32_t i = 0; i < k->n_files; ++i)
-      if (k->grp[i] >= k->n_groups) return TSM_E_LAYOUT;
+// The corpora of the diff and line-record calls (n > 0 files each): arena, off and len given, and the per-file layout rules
+// of the scan.  Their grp is not part of it: only the assertion tables use it.
+static int check_sides(std::initializer_list<const tsm_corpus*> sides, int32_t n, bool ext_rule) {
+  for (const tsm_corpus* k : sides) {
+    if (!k->arena || !k->off || !k->len) return TSM_E_ARG;
+    const int rc = check_files(k, 0, n, ext_rule, false);
+    if (rc != TSM_OK) return rc;
+  }
   return TSM_OK;
 }
 
-static int check_pair_layout(const tsm_corpus* olds, const tsm_corpus* news, bool with_ext) {
-  const int32_t n = olds->n_files;
-  for (const tsm_corpus* k : {olds, news}) {              // same layout rules as the scan (SPEC section 1)
-    if (!k->arena || !k->off || !k->len) return TSM_E_ARG;
-    for (int32_t i = 0; i < n; ++i)
-      if (k->off[i] < 0 || (k->off[i] & (TSM_ALIGN - 1)) || k->len[i] < 0 || (int64_t)k->off[i] + k->len[i] > k->off[i + 1] ||
-          (with_ext && k->ext && k->ext[i] > TSM_EXT_H))
-        return TSM_E_LAYOUT;
-  }
-  return TSM_OK;
+// Both sides of the revision pairs to the device (with_grp: their group tags too, for the assertion tables).
+static int pair_upload(const tsm_corpus* olds, const tsm_corpus* news, bool with_grp, HostSidePair& P, cudaStream_t st) {
+  P.n = olds->n_files;
+  P.groups_a = olds->n_groups; P.groups_b = news->n_groups;
+  if (with_grp) P.grp_ok = check_groups(olds, 0, P.n) == TSM_OK && check_groups(news, 0, P.n) == TSM_OK;
+  int rc = side_upload(olds, P.A, st);
+  if (rc == TSM_OK) rc = side_upload(news, P.B, st);
+  if (rc == TSM_OK && with_grp) rc = side_upload_grp(olds, P.A, st);
+  if (rc == TSM_OK && with_grp) rc = side_upload_grp(news, P.B, st);
+  return rc;
 }
 
 // The diff proper over two sides whose line records exist.  k_diff_small finishes the common pairs (distance at most
@@ -936,7 +968,7 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
   CU(cudaStreamSynchronize(st));
   A.drop_staging(); B.drop_staging();
   const uint32_t nt = *pin_nt;
-  { float ms = 0; if (cudaEventElapsedTime(&ms, c->diff_ev[2], c->diff_ev[3]) == cudaSuccess) c->diff_ms[1] = ms; }
+  c->diff_ms[1] = elapsed_ms(c->diff_ev[2], c->diff_ev[3]);
   c->launches = A.launches + B.launches + 4;
   c->diff_ms[2] = 0;
   if (nt == 0) return TSM_OK;
@@ -966,7 +998,7 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
   CU(cudaMemcpyAsync(added, d_add.p, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(removed, d_rem.p, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  { float ms = 0; if (cudaEventElapsedTime(&ms, c->diff_ev[4], c->diff_ev[5]) == cudaSuccess) c->diff_ms[2] += ms; }
+  c->diff_ms[2] += elapsed_ms(c->diff_ev[4], c->diff_ev[5]);
   c->launches++;
   if (!detail) return TSM_OK;
   // ---- their hunks: second search with the rows of V kept; rows sized from the distances just computed,
@@ -1010,7 +1042,7 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
     CU(cudaEventRecord(c->diff_ev[5], st));
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(st));
-    { float ms = 0; if (cudaEventElapsedTime(&ms, c->diff_ev[4], c->diff_ev[5]) == cudaSuccess) c->diff_ms[2] += ms; }
+    c->diff_ms[2] += elapsed_ms(c->diff_ev[4], c->diff_ev[5]);
     c->launches++;
     p0 = p1;
   }
@@ -1022,97 +1054,6 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
     detail[i] = d;
   }
   return TSM_OK;
-}
-
-extern "C" int tsm_diff_pairs_detail(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news,
-                                     int64_t* added, int64_t* removed, tsm_diff_detail* detail, void* stream) {
-  if (!c || !olds || !news || !added || !removed || olds->n_files != news->n_files) return TSM_E_ARG;
-  const int32_t n = olds->n_files;
-  if (n == 0) return TSM_OK;
-  int rc = check_pair_layout(olds, news, detail != nullptr);
-  if (rc != TSM_OK) return rc;
-  CU(cudaSetDevice(c->device));
-  PoolScope pool_scope(&c->pool);
-  cudaStream_t st = (cudaStream_t)stream;
-  HostSide A, B;
-  SyncGuard guard(st);                                     // no buffer goes back to the pool while work on st may still use it
-  c->diff_ms[0] = 0;
-  rc = side_upload(olds, A, st);
-  if (rc == TSM_OK) rc = side_upload(news, B, st);
-  HostSide* both[2] = {&A, &B};
-  if (rc == TSM_OK) rc = sides_records(c, both, 2, st, &c->diff_ms[0], false);
-  if (rc != TSM_OK) return rc;
-  return diff_core(c, A, B, n, added, removed, detail, st);
-}
-
-// Resident variant (what bench.py's `value` times for config C5): the two sides go to HBM once ...
-extern "C" int tsm_diff_upload(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, void* stream) {
-  if (!c || !olds || !news || olds->n_files != news->n_files || olds->n_files <= 0) return TSM_E_ARG;
-  int rc = check_pair_layout(olds, news, true);
-  if (rc != TSM_OK) return rc;
-  CU(cudaSetDevice(c->device));
-  free_res_pair(c);
-  PoolScope pool_scope(&c->pool);
-  cudaStream_t st = (cudaStream_t)stream;
-  SyncGuard guard(st);
-  c->res_pair = new (std::nothrow) HostSidePair;
-  if (!c->res_pair) return TSM_E_NOMEM;
-  HostSidePair& P = *c->res_pair;
-  P.n = olds->n_files;
-  P.groups_a = olds->n_groups; P.groups_b = news->n_groups;
-  P.grp_ok = check_groups(olds) == TSM_OK && check_groups(news) == TSM_OK;
-  rc = side_upload(olds, P.A, st);
-  if (rc == TSM_OK) rc = side_upload(news, P.B, st);
-  if (rc == TSM_OK) rc = side_upload_grp(olds, P.A, st);
-  if (rc == TSM_OK) rc = side_upload_grp(news, P.B, st);
-  if (rc == TSM_OK) rc = cudaStreamSynchronize(st) == cudaSuccess ? TSM_OK : TSM_E_CUDA;
-  if (rc != TSM_OK) { delete c->res_pair; c->res_pair = nullptr; }
-  return rc;
-}
-
-// ... and every call runs the kernels over them: k_scan over both sides (line records), k_myers, k_myers_trace.
-extern "C" int tsm_diff_resident(tsm_ctx* c, int64_t* added, int64_t* removed, tsm_diff_detail* detail, void* stream) {
-  if (!c || !added || !removed) return TSM_E_ARG;
-  if (!c->res_pair) return TSM_E_STATE;
-  CU(cudaSetDevice(c->device));
-  PoolScope pool_scope(&c->pool);
-  cudaStream_t st = (cudaStream_t)stream;
-  SyncGuard guard(st);
-  HostSidePair& P = *c->res_pair;
-  c->diff_ms[0] = 0;
-  P.A.launches = P.B.launches = 0;
-  HostSide* both[2] = {&P.A, &P.B};
-  int rc = sides_records(c, both, 2, st, &c->diff_ms[0], false);
-  if (rc != TSM_OK) return rc;
-  return diff_core(c, P.A, P.B, P.n, added, removed, detail, st);
-}
-
-extern "C" int tsm_diff_last_ms(tsm_ctx* c, float* ms3) {
-  if (!c || !ms3) return TSM_E_ARG;
-  for (int i = 0; i < 3; ++i) ms3[i] = c->diff_ms[i];
-  return TSM_OK;
-}
-
-extern "C" int tsm_diff_pairs(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news,
-                              int64_t* added, int64_t* removed, void* stream) {
-  return tsm_diff_pairs_detail(c, olds, news, added, removed, nullptr, stream);
-}
-
-// Events (any order, file < n_files) into the canonical (file, line_off) order: a counting sort by file, then the few events
-// of each file by line_off.  A comparison sort of the whole array costs milliseconds for a C5 batch; this is linear.
-static void sort_events_by_file(tsm_assert_event* ev, uint32_t m, int32_t n_files) {
-  if (m < 2) return;
-  std::vector<uint32_t> pos((size_t)n_files + 1, 0);
-  for (uint32_t i = 0; i < m; ++i) pos[(size_t)ev[i].file + 1]++;
-  for (int32_t f = 0; f < n_files; ++f) pos[(size_t)f + 1] += pos[(size_t)f];
-  std::vector<tsm_assert_event> tmp(m);
-  std::vector<uint32_t> at(pos.begin(), pos.end() - 1);
-  for (uint32_t i = 0; i < m; ++i) tmp[at[ev[i].file]++] = ev[i];
-  for (int32_t f = 0; f < n_files; ++f)
-    if (pos[(size_t)f + 1] - pos[(size_t)f] > 1)
-      std::sort(tmp.begin() + pos[(size_t)f], tmp.begin() + pos[(size_t)f + 1],
-                [](const tsm_assert_event& a, const tsm_assert_event& b) { return a.line_off < b.line_off; });
-  std::copy(tmp.begin(), tmp.end(), ev);
 }
 
 // Changed assertion lines (docs/SPEC.md section 8): diff_core with the EMIT kernels, then per side ONE k_classify launch
@@ -1148,8 +1089,7 @@ static int diff_asserts(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int32_t
   int64_t* const h_counts[2] = {out->removed_counts, out->added_counts};
   const size_t table = (size_t)(n_groups + 1) * TSM_K;     // [n_groups + 1][K]: k_classify also fills the global row
   const size_t hist = CLS_SMEM_BASE + sizeof(uint32_t) * (n_groups <= 16 ? (size_t)n_groups * TSM_K : 0);
-  int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_classify_t<false>, 256, hist) != cudaSuccess || per_sm < 1) per_sm = 4;
+  const uint32_t cls_wave = (uint32_t)(c->sms * classify_per_sm(c, hist));
   for (int s = 0; s < 2; ++s) {
     if (!d_counts[s].alloc(sizeof(unsigned long long) * table) ||
         (h_ev[s] && !d_aev[s].alloc(sizeof(tsm_assert_event) * (size_t)std::max(nc[s], 1u))))
@@ -1157,15 +1097,14 @@ static int diff_asserts(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int32_t
     CU(cudaMemsetAsync(d_counts[s].p, 0, sizeof(unsigned long long) * table, st));
     if (nc[s] == 0) continue;
     const HostSide& h = *side[s];
-    ScanParams p{};
-    p.arena = h.arena.as<uint8_t>(); p.off = h.off.as<int32_t>(); p.len = h.len.as<int32_t>(); p.ext = h.ext.as<uint8_t>();
-    p.grp = h.grp.as<uint16_t>(); p.n_files = n; p.n_groups = n_groups;
+    ScanParams p = side_params(h);
+    p.grp = h.grp.as<uint16_t>(); p.n_groups = n_groups;
     p.ctrl = ctrl[s];
     p.cand = sink.list[s]; p.cand_cap = sink.cap[s];
     p.aev = d_aev[s].as<tsm_assert_event>(); p.aev_cap = h_ev[s] ? nc[s] : 0;
     p.counts = d_counts[s].as<unsigned long long>();
-    p.flags = h_ev[s] ? TSM_SCAN_ASSERT_EVENTS : 0u; p.four = 4; p.cls_last = 0;
-    k_classify_t<false><<<std::min<uint32_t>((uint32_t)(c->sms * per_sm), (nc[s] + 255) / 256), 256, hist, st>>>(p);
+    p.flags = h_ev[s] ? TSM_SCAN_ASSERT_EVENTS : 0u;
+    k_classify_t<false><<<std::min<uint32_t>(cls_wave, (nc[s] + 255) / 256), 256, hist, st>>>(p);
     CU(cudaGetLastError());
     c->launches++;
   }
@@ -1182,137 +1121,181 @@ static int diff_asserts(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int32_t
   return TSM_OK;
 }
 
+// One diff call over the uploaded sides of P: their line records (diff_ms[0] = k_scan over both), then diff_core, or
+// diff_asserts when `out` is given.  The caller holds the pool scope and the SyncGuard of the call.
+static int pair_run(tsm_ctx* c, HostSidePair& P, int64_t* added, int64_t* removed, tsm_diff_detail* detail,
+                    tsm_diff_asserts* out, cudaStream_t st) {
+  c->diff_ms[0] = 0;
+  P.A.launches = P.B.launches = 0;
+  HostSide* both[2] = {&P.A, &P.B};
+  const int rc = sides_records(c, both, 2, st, &c->diff_ms[0], false);
+  if (rc != TSM_OK) return rc;
+  if (out) return diff_asserts(c, P.A, P.B, P.n, P.groups_a, added, removed, detail, out, st);
+  return diff_core(c, P.A, P.B, P.n, added, removed, detail, st);
+}
+
+extern "C" int tsm_diff_pairs_detail(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news,
+                                     int64_t* added, int64_t* removed, tsm_diff_detail* detail, void* stream) {
+  if (!c || !olds || !news || !added || !removed || olds->n_files != news->n_files) return TSM_E_ARG;
+  if (olds->n_files == 0) return TSM_OK;
+  int rc = check_sides({olds, news}, olds->n_files, detail != nullptr);
+  if (rc != TSM_OK) return rc;
+  CU(cudaSetDevice(c->device));
+  PoolScope pool_scope(&c->pool);
+  cudaStream_t st = (cudaStream_t)stream;
+  HostSidePair P;
+  SyncGuard guard(st);                                     // (after P) no buffer goes back to the pool while work on st may still use it
+  rc = pair_upload(olds, news, false, P, st);
+  return rc != TSM_OK ? rc : pair_run(c, P, added, removed, detail, nullptr, st);
+}
+
+extern "C" int tsm_diff_pairs(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news,
+                              int64_t* added, int64_t* removed, void* stream) {
+  return tsm_diff_pairs_detail(c, olds, news, added, removed, nullptr, stream);
+}
+
 extern "C" int tsm_diff_pairs_asserts(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
                                       tsm_diff_detail* detail, tsm_diff_asserts* out, void* stream) {
   if (!c || !olds || !news || !added || !removed || !out || olds->n_files != news->n_files || olds->n_groups != news->n_groups)
     return TSM_E_ARG;
-  int rc = check_groups(olds);
-  if (rc == TSM_OK) rc = check_groups(news);
-  if (rc != TSM_OK) return rc;
   const int32_t n = olds->n_files;
+  int rc = check_groups(olds, 0, n);
+  if (rc == TSM_OK) rc = check_groups(news, 0, n);
+  if (rc != TSM_OK) return rc;
   out->n_aev = out->n_rev = 0;
   if (n == 0) {
     for (int64_t* t : {out->added_counts, out->removed_counts})
       if (t) memset(t, 0, sizeof(int64_t) * (size_t)olds->n_groups * TSM_K);
     return TSM_OK;
   }
-  rc = check_pair_layout(olds, news, true);
+  rc = check_sides({olds, news}, n, true);
   if (rc != TSM_OK) return rc;
   CU(cudaSetDevice(c->device));
   PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
-  HostSide A, B;
+  HostSidePair P;
   SyncGuard guard(st);
-  c->diff_ms[0] = 0;
-  rc = side_upload(olds, A, st);
-  if (rc == TSM_OK) rc = side_upload(news, B, st);
-  if (rc == TSM_OK) rc = side_upload_grp(olds, A, st);
-  if (rc == TSM_OK) rc = side_upload_grp(news, B, st);
-  HostSide* both[2] = {&A, &B};
-  if (rc == TSM_OK) rc = sides_records(c, both, 2, st, &c->diff_ms[0], false);
+  rc = pair_upload(olds, news, true, P, st);
+  return rc != TSM_OK ? rc : pair_run(c, P, added, removed, detail, out, st);
+}
+
+// Resident variant (what bench.py's `value` times for config C5): the two sides go to HBM once ...
+extern "C" int tsm_diff_upload(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, void* stream) {
+  if (!c || !olds || !news || olds->n_files != news->n_files || olds->n_files <= 0) return TSM_E_ARG;
+  int rc = check_sides({olds, news}, olds->n_files, true);
   if (rc != TSM_OK) return rc;
-  return diff_asserts(c, A, B, n, olds->n_groups, added, removed, detail, out, st);
+  CU(cudaSetDevice(c->device));
+  free_res_pair(c);
+  PoolScope pool_scope(&c->pool);
+  cudaStream_t st = (cudaStream_t)stream;
+  SyncGuard guard(st);
+  c->res_pair = new (std::nothrow) HostSidePair;
+  if (!c->res_pair) return TSM_E_NOMEM;
+  rc = pair_upload(olds, news, true, *c->res_pair, st);    // (a bad grp fails tsm_diff_resident_asserts, not the upload)
+  if (rc == TSM_OK) rc = cudaStreamSynchronize(st) == cudaSuccess ? TSM_OK : TSM_E_CUDA;
+  if (rc != TSM_OK) { delete c->res_pair; c->res_pair = nullptr; }
+  return rc;
+}
+
+// ... and every call runs the kernels over them: k_scan over both sides (line records), k_myers, k_myers_trace.
+extern "C" int tsm_diff_resident(tsm_ctx* c, int64_t* added, int64_t* removed, tsm_diff_detail* detail, void* stream) {
+  if (!c || !added || !removed) return TSM_E_ARG;
+  if (!c->res_pair) return TSM_E_STATE;
+  CU(cudaSetDevice(c->device));
+  PoolScope pool_scope(&c->pool);
+  cudaStream_t st = (cudaStream_t)stream;
+  SyncGuard guard(st);
+  return pair_run(c, *c->res_pair, added, removed, detail, nullptr, st);
 }
 
 extern "C" int tsm_diff_resident_asserts(tsm_ctx* c, int64_t* added, int64_t* removed, tsm_diff_detail* detail,
                                          tsm_diff_asserts* out, void* stream) {
   if (!c || !added || !removed || !out) return TSM_E_ARG;
   if (!c->res_pair) return TSM_E_STATE;
-  HostSidePair& P = *c->res_pair;
-  if (P.groups_a != P.groups_b) return TSM_E_ARG;
-  if (!P.grp_ok) return TSM_E_LAYOUT;
+  if (c->res_pair->groups_a != c->res_pair->groups_b) return TSM_E_ARG;
+  if (!c->res_pair->grp_ok) return TSM_E_LAYOUT;
   out->n_aev = out->n_rev = 0;
   CU(cudaSetDevice(c->device));
   PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
   SyncGuard guard(st);
-  c->diff_ms[0] = 0;
-  P.A.launches = P.B.launches = 0;
-  HostSide* both[2] = {&P.A, &P.B};
-  int rc = sides_records(c, both, 2, st, &c->diff_ms[0], false);
-  if (rc != TSM_OK) return rc;
-  return diff_asserts(c, P.A, P.B, P.n, P.groups_a, added, removed, detail, out, st);
+  return pair_run(c, *c->res_pair, added, removed, detail, out, st);
+}
+
+extern "C" int tsm_diff_last_ms(tsm_ctx* c, float* ms3) {
+  if (!c || !ms3) return TSM_E_ARG;
+  for (int i = 0; i < 3; ++i) ms3[i] = c->diff_ms[i];
+  return TSM_OK;
 }
 
 // ------------------------------------------------------------------------------------- S9 line / n-gram hashes
-extern "C" int tsm_line_hashes(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, uint64_t* line_hash, uint32_t* line_end,
-                               uint8_t* line_flag, int64_t cap, int64_t* n_lines, int32_t ngram_n, uint64_t* ngram_hash,
-                               void* stream) {
-  if (!c || !k || !line_base || !n_lines || cap < 0 || k->n_files < 0 || ngram_n < 0 || (ngram_hash && ngram_n < 1)) return TSM_E_ARG;
+// The front of tsm_line_hashes and tsm_statements: the corpus' line records from one pass of the scan, and line_base[n+1]
+// and *n_lines on the host - also when cap is short of the lines, which returns TSM_E_CAPACITY so that the caller can
+// allocate and call again.  Then tail(S, lines, st), the call's own use of the records, inside the call's SyncGuard.
+template <typename Tail>
+static int line_records(tsm_ctx* c, const tsm_corpus* k, bool ext_rule, int64_t* line_base, int64_t cap, int64_t* n_lines,
+                        void* stream, Tail tail) {
   const int32_t n = k->n_files;
   *n_lines = 0;
   line_base[0] = 0;
   if (n == 0) return TSM_OK;
-  if (!k->arena || !k->off || !k->len) return TSM_E_ARG;
-  for (int32_t i = 0; i < n; ++i)
-    if (k->off[i] < 0 || (k->off[i] & (TSM_ALIGN - 1)) || k->len[i] < 0 || (int64_t)k->off[i] + k->len[i] > k->off[i + 1] ||
-        (k->ext && k->ext[i] > TSM_EXT_H))
-      return TSM_E_LAYOUT;
+  int rc = check_sides({k}, n, ext_rule);
+  if (rc != TSM_OK) return rc;
   CU(cudaSetDevice(c->device));
   PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
   HostSide S;
   SyncGuard guard(st);
-  int rc = side_upload(k, S, st);
+  rc = side_upload(k, S, st);
   if (rc == TSM_OK) rc = side_records(c, S, st, nullptr);
   if (rc != TSM_OK) return rc;
   const unsigned long long total = S.base[(size_t)n];
   for (int32_t i = 0; i <= n; ++i) line_base[i] = (int64_t)S.base[(size_t)i];
   *n_lines = (int64_t)total;
   c->launches = S.launches;
-  if ((unsigned long long)cap < total) return TSM_E_CAPACITY;   // line_base / n_lines are filled: allocate and call again
+  if ((unsigned long long)cap < total) return TSM_E_CAPACITY;
   if (total == 0) return TSM_OK;
-  if (line_hash) CU(cudaMemcpyAsync(line_hash, S.d.line_hash, sizeof(uint64_t) * (size_t)total, cudaMemcpyDeviceToHost, st));
-  if (line_end) CU(cudaMemcpyAsync(line_end, S.d.line_end, sizeof(uint32_t) * (size_t)total, cudaMemcpyDeviceToHost, st));
-  if (line_flag) CU(cudaMemcpyAsync(line_flag, S.d.line_flag, (size_t)total, cudaMemcpyDeviceToHost, st));
-  if (ngram_hash) {
-    DevBuf d_ng;
-    if (!d_ng.alloc(sizeof(unsigned long long) * (size_t)total)) { cudaStreamSynchronize(st); return TSM_E_CUDA; }
-    k_ngrams<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(S.d.line_hash, S.d.line_base, (uint32_t)n, total, (uint32_t)ngram_n,
-                                                               d_ng.as<unsigned long long>());
-    CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(ngram_hash, d_ng.p, sizeof(uint64_t) * (size_t)total, cudaMemcpyDeviceToHost, st));
+  return tail(S, total, st);
+}
+
+extern "C" int tsm_line_hashes(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, uint64_t* line_hash, uint32_t* line_end,
+                               uint8_t* line_flag, int64_t cap, int64_t* n_lines, int32_t ngram_n, uint64_t* ngram_hash,
+                               void* stream) {
+  if (!c || !k || !line_base || !n_lines || cap < 0 || k->n_files < 0 || ngram_n < 0 || (ngram_hash && ngram_n < 1)) return TSM_E_ARG;
+  return line_records(c, k, true, line_base, cap, n_lines, stream, [&](const HostSide& S, unsigned long long total, cudaStream_t st) -> int {
+    if (line_hash) CU(cudaMemcpyAsync(line_hash, S.d.line_hash, sizeof(uint64_t) * (size_t)total, cudaMemcpyDeviceToHost, st));
+    if (line_end) CU(cudaMemcpyAsync(line_end, S.d.line_end, sizeof(uint32_t) * (size_t)total, cudaMemcpyDeviceToHost, st));
+    if (line_flag) CU(cudaMemcpyAsync(line_flag, S.d.line_flag, (size_t)total, cudaMemcpyDeviceToHost, st));
+    if (ngram_hash) {
+      DevBuf d_ng;
+      if (!d_ng.alloc(sizeof(unsigned long long) * (size_t)total)) { cudaStreamSynchronize(st); return TSM_E_CUDA; }
+      k_ngrams<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(S.d.line_hash, S.d.line_base, (uint32_t)S.n, total, (uint32_t)ngram_n,
+                                                                 d_ng.as<unsigned long long>());
+      CU(cudaGetLastError());
+      CU(cudaMemcpyAsync(ngram_hash, d_ng.p, sizeof(uint64_t) * (size_t)total, cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      c->launches++;
+    }
     CU(cudaStreamSynchronize(st));
-    c->launches++;
-  }
-  CU(cudaStreamSynchronize(st));
-  return TSM_OK;
+    return TSM_OK;
+  });
 }
 
 // ------------------------------------------------------------------------------------- SPEC section 10 statements
 extern "C" int tsm_statements(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, uint32_t* line_end,
                               uint8_t* line_kind, int64_t cap, int64_t* n_lines, void* stream) {
   if (!c || !k || !line_base || !n_lines || cap < 0 || k->n_files < 0) return TSM_E_ARG;
-  const int32_t n = k->n_files;
-  *n_lines = 0;
-  line_base[0] = 0;
-  if (n == 0) return TSM_OK;
-  if (!k->arena || !k->off || !k->len) return TSM_E_ARG;
-  for (int32_t i = 0; i < n; ++i)
-    if (k->off[i] < 0 || (k->off[i] & (TSM_ALIGN - 1)) || k->len[i] < 0 || (int64_t)k->off[i] + k->len[i] > k->off[i + 1])
-      return TSM_E_LAYOUT;
-  CU(cudaSetDevice(c->device));
-  PoolScope pool_scope(&c->pool);
-  cudaStream_t st = (cudaStream_t)stream;
-  HostSide S;
-  SyncGuard guard(st);
-  int rc = side_upload(k, S, st);                         // line records from one pass of the scan
-  if (rc == TSM_OK) rc = side_records(c, S, st, nullptr);
-  if (rc != TSM_OK) return rc;
-  const unsigned long long total = S.base[(size_t)n];
-  for (int32_t i = 0; i <= n; ++i) line_base[i] = (int64_t)S.base[(size_t)i];
-  *n_lines = (int64_t)total;
-  if ((unsigned long long)cap < total) return TSM_E_CAPACITY;   // line_base / n_lines are filled: allocate and call again
-  if (total == 0) return TSM_OK;
-  if (!line_end || !line_kind) return TSM_E_ARG;
-  DevBuf d_delta, d_kind;
-  if (!d_delta.alloc(sizeof(int32_t) * (size_t)total) || !d_kind.alloc((size_t)total)) return TSM_E_CUDA;
-  k_line_parens<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(S.d, n, total, d_delta.as<int32_t>(), d_kind.as<uint8_t>());
-  k_stmt_kinds<<<(n * 32 + 127) / 128, 128, 0, st>>>(S.d, n, d_delta.as<int32_t>(), d_kind.as<uint8_t>());
-  CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(line_end, S.d.line_end, sizeof(uint32_t) * (size_t)total, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(line_kind, d_kind.p, (size_t)total, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  c->launches = S.launches + 2;
-  return TSM_OK;
+  return line_records(c, k, false, line_base, cap, n_lines, stream, [&](const HostSide& S, unsigned long long total, cudaStream_t st) -> int {
+    if (!line_end || !line_kind) return TSM_E_ARG;
+    DevBuf d_delta, d_kind;
+    if (!d_delta.alloc(sizeof(int32_t) * (size_t)total) || !d_kind.alloc((size_t)total)) return TSM_E_CUDA;
+    k_line_parens<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(S.d, S.n, total, d_delta.as<int32_t>(), d_kind.as<uint8_t>());
+    k_stmt_kinds<<<(S.n * 32 + 127) / 128, 128, 0, st>>>(S.d, S.n, d_delta.as<int32_t>(), d_kind.as<uint8_t>());
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(line_end, S.d.line_end, sizeof(uint32_t) * (size_t)total, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(line_kind, d_kind.p, (size_t)total, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    c->launches += 2;
+    return TSM_OK;
+  });
 }
