@@ -267,3 +267,73 @@ def score_g1(golden, names, files, events):
 def load_fixture_names(path):
     d = np.load(path)
     return bytes(d["names"]).decode().split("\n")
+
+
+# ---------------------------------------------------------------------------------------------- revision pairs (SPEC section 8)
+# Lines of the tie-heavy pairs: blank lines, braces, CR variants that hash like their LF twins, and assertion lines.
+TIE_LINES = [b"\n", b"\r\n", b"}\n", b"}\r\n", b"  }\n", b"x\n", b"x\r\n", b"assert x\n", b"EXPECT_TRUE(ok);\n",
+             b"self.assertEqual(a, b)\n", b"{\n"]
+
+
+def tie_pair(rng: random.Random, n_lines: int, n_edits: int):
+    """(old, new) over an alphabet of 2-4 lines: a random old file and n_edits random insertions, deletions and
+    replacements of one line.  With so few distinct lines many alignments tie."""
+    alpha = rng.sample(TIE_LINES, rng.randrange(2, 5))
+    old = [rng.choice(alpha) for _ in range(n_lines)]
+    new = list(old)
+    for _ in range(n_edits):
+        i = rng.randrange(len(new) + 1)
+        op = rng.randrange(3)
+        if op == 0 or not new:
+            new.insert(i, rng.choice(alpha))
+        elif op == 1 and i < len(new):
+            del new[i]
+        elif i < len(new):
+            new[i] = rng.choice(alpha)
+    o, n = b"".join(old), b"".join(new)
+    if rng.random() < 0.2 and o.endswith(b"\n"):          # an unterminated last line (equal to its terminated twin)
+        o = o[:-1]
+    return o, n
+
+
+def tie_heavy_pairs(seed: int, scale: int = 1):
+    """Tie-heavy pairs sized for every k_diff_small size and the left-over kernels: (olds, news, exts)."""
+    rng = random.Random(seed)
+    shapes = ([(rng.randrange(8, 200), rng.randrange(1, 12)) for _ in range(40)] +         # middle <= 512, D <= 31
+              [(rng.randrange(300, 480), rng.randrange(12, 26)) for _ in range(16)] +     # <= 1 024 / 63
+              [(rng.randrange(700, 1900), rng.randrange(10, 26)) for _ in range(10)] +    # <= 4 096 / 63
+              [(rng.randrange(700, 1900), rng.randrange(36, 56)) for _ in range(10)] +    # <= 4 096 / 127
+              [(rng.randrange(2200, 2600), rng.randrange(4, 20)) for _ in range(5)] +     # middle > 4 096
+              [(rng.randrange(300, 900), rng.randrange(90, 160)) for _ in range(5)])      # D > 127
+    olds, news, exts = [], [], []
+    for _ in range(scale):
+        for n_lines, n_edits in shapes:
+            o, n = tie_pair(rng, n_lines, n_edits)
+            olds.append(o)
+            news.append(n)
+            exts.append(rng.choice((1, 2, 4)))
+    return olds, news, exts
+
+
+def block_pair(tag: bytes, old_blocks, new_blocks, n_prefix=3, n_suffix=2, assert_every=5):
+    """A pair with a closed-form script: unique old blocks and unique new blocks (sizes old_blocks[i], new_blocks[i]; 0 =
+    none) between unique common lines, behind a common prefix and before a common suffix.  The only LCS is the common
+    lines, so every block pair is one hunk and every block line changes.  Every assert_every-th block line is an assertion
+    line.  Returns (old, new, want) with want = (hunks_add, hunks_del, hunks_mod, deleted, inserted): line indices."""
+    def blk(side, i, k):
+        return [(b"assert %s_%s%d_%d\n" if j % assert_every == 1 else b"%s_%s%d_%d = 1\n") % (tag, side, i, j) for j in range(k)]
+    old = [b"%s_pre%d\n" % (tag, i) for i in range(n_prefix)]
+    new = list(old)
+    deleted, inserted, h = [], [], [0, 0, 0]
+    for i, (ko, kn) in enumerate(zip(old_blocks, new_blocks)):
+        deleted += range(len(old), len(old) + ko)
+        inserted += range(len(new), len(new) + kn)
+        old += blk(b"o", i, ko)
+        new += blk(b"n", i, kn)
+        if ko or kn:
+            h[2 if ko and kn else 0 if kn else 1] += 1
+        common = [b"%s_common%d\n" % (tag, i)]
+        old += common
+        new += common
+    tail = [b"%s_suf%d\n" % (tag, i) for i in range(n_suffix)]
+    return b"".join(old + tail), b"".join(new + tail), (h[0], h[1], h[2], deleted, inserted)

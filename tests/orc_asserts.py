@@ -8,6 +8,7 @@ import hashlib
 import os
 import subprocess
 import tempfile
+import threading
 
 import numpy as np
 
@@ -18,23 +19,25 @@ SRCS = [os.path.join(HERE, "orc_diff_asserts.c"), os.path.join(orc.ORC_DIR, "orc
 DEPS = SRCS + [os.path.join(orc.ORC_DIR, "orc.h"), os.path.join(orc.ORC_DIR, "orc_categories.inc")]
 
 _lib = None
+_lock = threading.Lock()                  # the first call may come from several threads at once
 
 
 def lib():
     global _lib
-    if _lib is None:
-        key = hashlib.sha1(b"".join(open(p, "rb").read() for p in DEPS)).hexdigest()[:16]
-        so = os.path.join(tempfile.gettempdir(), "tosem_orc_asserts_%s_%d.so" % (key, os.getuid()))
-        if not os.path.exists(so):
-            tmp = so + ".%d" % os.getpid()
-            subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-std=c99", "-fPIC", "-shared", "-I", orc.ORC_DIR,
-                                   "-o", tmp] + SRCS)
-            os.replace(tmp, so)
-        L = C.CDLL(so)
-        L.orc_diff_pairs_asserts.restype = C.c_int
-        L.orc_diff_pairs_asserts.argtypes = [C.c_void_p] * 10 + [C.c_int32, C.c_int32] + [C.c_void_p] * 2 + \
-            [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
-        _lib = L
+    with _lock:
+        if _lib is None:
+            key = hashlib.sha1(b"".join(open(p, "rb").read() for p in DEPS)).hexdigest()[:16]
+            so = os.path.join(tempfile.gettempdir(), "tosem_orc_asserts_%s_%d.so" % (key, os.getuid()))
+            if not os.path.exists(so):
+                tmp = so + ".%d" % os.getpid()
+                subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-std=c99", "-fPIC", "-shared", "-I", orc.ORC_DIR,
+                                       "-o", tmp] + SRCS)
+                os.replace(tmp, so)
+            L = C.CDLL(so)
+            L.orc_diff_pairs_asserts.restype = C.c_int
+            L.orc_diff_pairs_asserts.argtypes = [C.c_void_p] * 10 + [C.c_int32, C.c_int32] + [C.c_void_p] * 2 + \
+                [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+            _lib = L
     return _lib
 
 

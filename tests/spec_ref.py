@@ -127,3 +127,82 @@ def py_category_string(t: bytes) -> str:
         s, n = py_ident(t)
         return t[s:s + n].decode("latin-1")
     return CATEGORY_NAMES.get(c, "")
+
+
+def py_diff_script(a, b, fa, fb):
+    """SPEC section 8 as written, for line-hash lists a (old) and b (new) with assertion flags fa, fb.  Returns (added,
+    removed, hunks_add, hunks_del, hunks_mod, added_assert, removed_assert, deleted_idx, inserted_idx): the deleted lines
+    of a and the inserted lines of b as indices into the whole lists, in line order."""
+    n0, m0 = len(a), len(b)
+    pre = 0                                              # step 1: common prefix, then common suffix of the rest
+    while pre < n0 and pre < m0 and a[pre] == b[pre]:
+        pre += 1
+    suf = 0
+    while suf < n0 - pre and suf < m0 - pre and a[n0 - 1 - suf] == b[m0 - 1 - suf]:
+        suf += 1
+    A, B = a[pre:n0 - suf], b[pre:m0 - suf]
+    n, m = len(A), len(B)
+    if n == 0 or m == 0:                                 # the remainder is one pure hunk (or nothing)
+        deleted, inserted = list(range(n)), list(range(m))
+        hunks = [("del" if n else "add")] if n + m else []
+        D = n + m
+    else:
+        V, rows, D = {1: 0}, [], None                    # step 2: rows[d][k] = furthest x on diagonal k after d edits
+        for d in range(n + m + 1):
+            row = {}
+            for k in range(-d, d + 1, 2):
+                if k == -d or (k != d and V[k - 1] < V[k + 1]):
+                    x = V[k + 1]
+                else:
+                    x = V[k - 1] + 1
+                y = x - k
+                while x < n and y < m and A[x] == B[y]:
+                    x += 1
+                    y += 1
+                row[k] = x
+            V.update(row)
+            rows.append(row)
+            if row.get(n - m, -1) >= n:
+                D = d
+                break
+        edits, x, y = [], n, m                           # step 3: (kind, x, y) where each edit starts, last to first
+        for d in range(D, 0, -1):
+            k, P = x - y, rows[d - 1]
+            down = k == -d or (k != d and P[k - 1] < P[k + 1])
+            pk = k + 1 if down else k - 1
+            px = P[pk]
+            py = px - pk
+            edits.append(("ins" if down else "del", px, py))
+            x, y = px, py
+        edits.reverse()
+        deleted = [ex for kind, ex, ey in edits if kind == "del"]
+        inserted = [ey for kind, ex, ey in edits if kind == "ins"]
+        hunks, cur, at = [], set(), None                 # a hunk: edits with no match between them
+        for kind, ex, ey in edits:
+            if at is not None and (ex, ey) != at:
+                hunks.append(cur)
+                cur = set()
+            cur.add(kind)
+            at = (ex + 1, ey) if kind == "del" else (ex, ey + 1)
+        hunks.append(cur)
+        hunks = ["mod" if len(h) == 2 else ("add" if "ins" in h else "del") for h in hunks]
+    lcs = pre + suf + (n + m - D) // 2
+    deleted = [pre + i for i in deleted]
+    inserted = [pre + j for j in inserted]
+    return (m0 - lcs, n0 - lcs, hunks.count("add"), hunks.count("del"), hunks.count("mod"),
+            sum(1 for j in inserted if fb[j]), sum(1 for i in deleted if fa[i]), deleted, inserted)
+
+
+def py_diff_files(old: bytes, new: bytes, ext_old: int, ext_new: int):
+    """py_diff_script of two files, from their line records (SPEC sections 2-4)."""
+    ra, rb = py_line_records(old, ext_old), py_line_records(new, ext_new)
+    return py_diff_script([r[0] for r in ra], [r[0] for r in rb], [r[2] for r in ra], [r[2] for r in rb])
+
+
+def py_line_starts(data: bytes):
+    """File-relative start of every line (the line_off of its events)."""
+    out, pos = [], 0
+    for line in py_lines(data):
+        out.append(pos)
+        pos += len(line) + 1
+    return out

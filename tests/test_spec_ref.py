@@ -102,3 +102,68 @@ def test_py_category_reproduces_golden_g4_with_the_ledger_misses():
             misses.add((r["statement"], r["category"]))
     assert [hit, tot] == [11954, 11981]
     assert misses == {(m["statement"], m["sheet_says"]) for m in ledger["misses"]}
+
+
+def diff_edge_pairs():
+    """The hand-built pairs of the GPU diff tests: empty sides, pure hunks, CR and final-LF twins, reversed and
+    repeated lines, replaced assertion lines."""
+    olds = [b"", b"a\n", b"a\nb\nc\n", b"a\nb\nc", b"x\n" * 100, b"same\n" * 50, b"a\nb\n", b"q\r\nr\n", b"1\n2\n3\n4\n5\n",
+            b"\n\n\n", b"only old\n", b"", b"a\nb\nc\n", b"a\nb\nc\n", b"def t():\n  assert x\n  y = 1\n", b"", b"k\n" * 9,
+            b"EXPECT_EQ(a, b);\nfoo\n", b"x = 1\nself.assertEqual(a, b)\ny = 2\n", b"assert a\n" * 300, b"a\nb\n" * 40]
+    news = [b"", b"a\n", b"a\nc\n", b"a\nb\nc\n", b"y\n" * 70, b"same\n" * 50, b"b\na\n", b"q\nr\r\n", b"5\n4\n3\n2\n1\n",
+            b"\n", b"", b"only new\nsecond\n", b"a\nc\n", b"a\nB\nc\nd\n", b"def t():\n  assert x == 2\n  y = 1\n  assert y\n",
+            b"assert q\n", b"", b"foo\nEXPECT_EQ(a, b);\n", b"x = 1\nself.assertTrue(a)\ny = 2\n", b"", b"b\na\n" * 40]
+    exts = [1] * 17 + [2, 1, 4, 1]
+    return olds, news, exts
+
+
+def check_diff_script(olds, news, exts):
+    """py_diff_script against orc.diff_pairs_detail (added, removed, hunks, assertion counts) and orc_asserts (which lines
+    change: the events of the deleted / inserted assertion lines).  Returns the reference's tuples."""
+    import orc_asserts
+    a, b = orc.pack(olds), orc.pack(news)
+    e = np.array(exts, np.uint8)
+    add, rem, det = orc.diff_pairs_detail(a + (e,), b + (e,))
+    _, _, aev, rev = orc_asserts.diff_pairs_asserts(a + (e,), b + (e,))
+    got_a = {(int(f), int(o)) for f, o in zip(aev["file"], aev["line_off"])}
+    got_r = {(int(f), int(o)) for f, o in zip(rev["file"], rev["line_off"])}
+    want_a, want_r, out = set(), set(), []
+    for i, (o, n, x) in enumerate(zip(olds, news, exts)):
+        r = sr.py_diff_files(o, n, x, x)
+        out.append(r)
+        assert r[:7] == (int(add[i]), int(rem[i]), *(int(det[i][f]) for f in det.dtype.names)), (i, r[:7], add[i], rem[i], det[i])
+        fo, fn = [t[2] for t in sr.py_line_records(o, x)], [t[2] for t in sr.py_line_records(n, x)]
+        so, sn = sr.py_line_starts(o), sr.py_line_starts(n)
+        want_r |= {(i, so[j]) for j in r[7] if fo[j]}
+        want_a |= {(i, sn[j]) for j in r[8] if fn[j]}
+    assert got_a == want_a and got_r == want_r
+    assert len(aev) == len(got_a) and len(rev) == len(got_r)
+    return out
+
+
+def test_py_diff_script_on_the_diff_edge_cases():
+    out = check_diff_script(*diff_edge_pairs())
+    assert out[2][:5] == (0, 1, 0, 1, 0) and out[6][:5] == (1, 1, 1, 1, 0) and out[19][:7] == (0, 300, 0, 1, 0, 0, 300)
+    assert out[3][:2] == (0, 0) and out[7][:2] == (0, 0)          # final-LF and CR twins are the same line
+
+
+def test_py_diff_script_on_tie_heavy_pairs():
+    olds, news, exts = cu.tie_heavy_pairs(31)
+    out = check_diff_script(olds, news, exts)
+    assert sum(r[5] + r[6] for r in out) > 100                    # assertion lines change
+    assert sum(r[4] for r in out) > 50 and sum(r[2] for r in out) > 500 and sum(r[3] for r in out) > 500
+
+
+def test_py_diff_script_on_closed_form_shapes():
+    shapes = [((0, 5, 0), (3, 0, 7)), ((4,), (4,)), ((0,), (9,)), ((9,), (0,)), ((1, 1, 1, 1), (0, 2, 0, 2)),
+              ((40, 0, 13, 2), (0, 17, 5, 0)), ((0, 0), (0, 0))]
+    olds, news, wants = [], [], []
+    for i, (ob, nb) in enumerate(shapes):
+        o, n, want = cu.block_pair(b"s%d" % i, ob, nb, n_prefix=i % 3, n_suffix=(i + 1) % 3)
+        olds.append(o)
+        news.append(n)
+        wants.append(want)
+    out = check_diff_script(olds, news, [1] * len(olds))
+    for r, want, o, n in zip(out, wants, olds, news):
+        assert r[2:5] == want[:3] and r[7] == want[3] and r[8] == want[4]
+        assert (r[0], r[1]) == (len(want[4]), len(want[3]))
