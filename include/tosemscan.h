@@ -173,6 +173,19 @@ int tsm_diff_pairs_asserts(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpu
 int tsm_diff_resident_asserts(tsm_ctx* ctx, int64_t* added, int64_t* removed, tsm_diff_detail* detail, tsm_diff_asserts* out,
                               void* stream);
 
+/* Rename similarity (docs/SPEC.md section 13): common[c] = sum over the line hashes h (section 3) shared by file cand_old[c] of
+ * olds and file cand_new[c] of news of min(W_old(h), W_new(h)), where W_x(h) is the total weight of the lines of x with
+ * hash h and a line weighs its bytes, plus 1 for its LF, minus 1 for the CR of a CRLF (git's diffcore-delta count).  The
+ * host turns it into git's score floor(common * 60000 / max(size_old, size_new)).  The two corpora may have different file
+ * counts; their ext and grp are not used.  An index out of range is TSM_E_ARG; the device needs about 16 B per candidate,
+ * and TSM_E_NOMEM is returned when that does not fit.  n_cand = 0 is legal.  One k_scan pass per side gives the line
+ * records; then per file the sorted distinct (hash, weight) list (shared memory up to 4 096 lines, a tiled sort through
+ * global memory above) and one warp per candidate (persistent warps, binary search of the longer list).
+ * tsm_similarity_last_ms: device time of the last call, ms3 = { k_scan over both sides, sort / merge, k_similarity }. */
+int tsm_similarity(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news, const int32_t* cand_old, const int32_t* cand_new,
+                   int64_t n_cand, int64_t* common, void* stream);
+int tsm_similarity_last_ms(tsm_ctx* ctx, float* ms3);
+
 /* S9 line / n-gram hashes (docs/SPEC.md section 3; SURVEY.md section 8a S9 - a design choice of the north star, attested by no
  * artefact of the package): the records of every line of every file, files in order, from ONE pass of the scan
  * kernel over the source.  line_base[n_files+1] and *n_lines are always filled; line_hash (SPEC section 3), line_end

@@ -15,6 +15,7 @@
 #include "tsm_diff_kernels.cuh"
 #include "tsm_stmt_kernels.cuh"
 #include "tsm_lines_kernels.cuh"
+#include "tsm_similar_kernels.cuh"
 
 using namespace tsm;
 
@@ -90,6 +91,7 @@ struct tsm_ctx {
   cudaEvent_t diff_ev[8] = {};             // around the kernels of the diff path (tsm_diff_last_ms)
   uint8_t* h_diff = nullptr;               // 256 B pinned: what the diff path reads back between its kernels (Ctrl x 2, line totals, todo count)
   float diff_ms[3] = {0, 0, 0};            // k_scan over both sides, k_myers, k_myers_trace of the last diff
+  float sim_ms[3] = {0, 0, 0};             // k_scan over both sides, sort / merge, k_similarity of the last tsm_similarity
   struct HostSidePair* res_pair = nullptr; // sides kept in HBM by tsm_diff_upload
   static constexpr int kMaxSlabs = 64;
   tsm_file_stat* d_stats = nullptr;
@@ -281,7 +283,8 @@ extern "C" int tsm_create(tsm_ctx** out, int device, int64_t max_arena_bytes, in
         cudaMemcpyToSymbol(c_lut_b, lutb, sizeof lutb) != cudaSuccess ||
         cudaFuncSetAttribute(k_scan_t<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN2_SMEM) != cudaSuccess ||
         cudaFuncSetAttribute(k_scan_t<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN2_SMEM_B) != cudaSuccess ||
-        diff_small_smem<false>() != cudaSuccess || diff_small_smem<true>() != cudaSuccess)
+        diff_small_smem<false>() != cudaSuccess || diff_small_smem<true>() != cudaSuccess ||
+        cudaFuncSetAttribute(k_sim_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SIM_SORT_SMEM) != cudaSuccess)
       rc = TSM_E_CUDA;
   }
   if (rc != TSM_OK) {
@@ -1225,6 +1228,98 @@ extern "C" int tsm_diff_resident_asserts(tsm_ctx* c, int64_t* added, int64_t* re
 extern "C" int tsm_diff_last_ms(tsm_ctx* c, float* ms3) {
   if (!c || !ms3) return TSM_E_ARG;
   for (int i = 0; i < 3; ++i) ms3[i] = c->diff_ms[i];
+  return TSM_OK;
+}
+
+// ------------------------------------------------------------------------------------- SPEC section 13 rename similarity
+// Per side with line records: k_sim_sort (distinct (hash, weight) of every file at its line_base), xscan of the list
+// lengths, k_sim_compact (dense CSR).  sim_ms[1] covers both sides.
+namespace {
+struct SimLists { DevBuf wk_key, wk_w, s_key, s_cum, cnt, bsum, base, key, w; };
+
+int sim_lists(const HostSide& h, SimLists& L, cudaStream_t st) {
+  const int32_t n = h.n;
+  const size_t lines = (size_t)h.total;
+  if (!L.wk_key.alloc(sizeof(unsigned long long) * lines) || !L.wk_w.alloc(sizeof(uint32_t) * lines) ||
+      !L.s_key.alloc(sizeof(unsigned long long) * lines) || !L.s_cum.alloc(sizeof(uint32_t) * lines) ||
+      !L.cnt.alloc(sizeof(uint32_t) * (size_t)n) || !L.bsum.alloc(sizeof(unsigned long long) * ((size_t)n / XS_TILE + 4)) ||
+      !L.base.alloc(sizeof(unsigned long long) * ((size_t)n + 1)) || !L.key.alloc(sizeof(unsigned long long) * lines) ||
+      !L.w.alloc(sizeof(uint32_t) * lines))
+    return TSM_E_CUDA;
+  k_sim_sort<<<n, SIM_SORT_THREADS, SIM_SORT_SMEM, st>>>(h.d.arena, h.d.off, h.d.len, h.d.line_base, h.d.line_hash, h.d.line_end,
+                                                        L.wk_key.as<unsigned long long>(), L.wk_w.as<uint32_t>(),
+                                                        L.s_key.as<unsigned long long>(), L.s_cum.as<uint32_t>(), L.cnt.as<uint32_t>());
+  xscan(L.cnt.as<uint32_t>(), (uint32_t)n, L.bsum.as<unsigned long long>(), L.base.as<unsigned long long>(), st);
+  k_sim_compact<<<(unsigned)(((size_t)n * 32 + 255) / 256), 256, 0, st>>>(h.d.line_base, L.cnt.as<uint32_t>(), L.base.as<unsigned long long>(),
+                                                                          (uint32_t)n, L.s_key.as<unsigned long long>(), L.s_cum.as<uint32_t>(),
+                                                                          L.key.as<unsigned long long>(), L.w.as<uint32_t>());
+  CU(cudaGetLastError());
+  return TSM_OK;
+}
+}  // namespace
+
+extern "C" int tsm_similarity(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, const int32_t* cand_old,
+                              const int32_t* cand_new, int64_t n_cand, int64_t* common, void* stream) {
+  if (!c || !olds || !news || n_cand < 0 || (n_cand && (!cand_old || !cand_new || !common))) return TSM_E_ARG;
+  if (olds->n_files < 0 || news->n_files < 0) return TSM_E_ARG;
+  for (float& v : c->sim_ms) v = 0;
+  if (n_cand == 0) return TSM_OK;
+  CU(cudaSetDevice(c->device));
+  {                                                        // the candidates, their indices and results: 16 B each on the device
+    size_t free_b = 0, total_b = 0;
+    CU(cudaMemGetInfo(&free_b, &total_b));
+    if ((uint64_t)n_cand > free_b / 16) return TSM_E_NOMEM;
+  }
+  for (int64_t i = 0; i < n_cand; ++i)
+    if (cand_old[i] < 0 || cand_old[i] >= olds->n_files || cand_new[i] < 0 || cand_new[i] >= news->n_files) return TSM_E_ARG;
+  int rc = check_sides({olds}, olds->n_files, false);
+  if (rc == TSM_OK) rc = check_sides({news}, news->n_files, false);
+  if (rc != TSM_OK) return rc;
+  PoolScope pool_scope(&c->pool);
+  cudaStream_t st = (cudaStream_t)stream;
+  HostSidePair P;
+  SimLists LA, LB;
+  DevBuf d_cand;
+  SyncGuard guard(st);                                     // (after the buffers) nothing goes back to the pool while st may use it
+  rc = side_upload(olds, P.A, st);
+  if (rc == TSM_OK) rc = side_upload(news, P.B, st);
+  if (rc != TSM_OK) return rc;
+  P.A.launches = P.B.launches = 0;
+  HostSide* both[2] = {&P.A, &P.B};
+  rc = sides_records(c, both, 2, st, &c->sim_ms[0], false);
+  if (rc != TSM_OK) return rc;
+  const size_t nc = (size_t)n_cand;
+  if (!d_cand.alloc(16 * nc + 64)) { cudaGetLastError(); return TSM_E_NOMEM; }
+  long long* d_common = d_cand.as<long long>();
+  int32_t* d_old = reinterpret_cast<int32_t*>(d_common + nc);
+  int32_t* d_new = d_old + nc;
+  unsigned long long* d_next = reinterpret_cast<unsigned long long*>(d_new + nc);   // at 16 * nc bytes: 8-byte aligned
+  CU(cudaMemcpyAsync(d_old, cand_old, sizeof(int32_t) * nc, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d_new, cand_new, sizeof(int32_t) * nc, cudaMemcpyHostToDevice, st));
+  CU(cudaMemsetAsync(d_next, 0, sizeof(unsigned long long), st));
+  CU(cudaEventRecord(c->diff_ev[2], st));
+  rc = sim_lists(P.A, LA, st);
+  if (rc == TSM_OK) rc = sim_lists(P.B, LB, st);
+  if (rc != TSM_OK) return rc;
+  CU(cudaEventRecord(c->diff_ev[3], st));
+  const unsigned grid = (unsigned)std::min<size_t>((size_t)c->sms * 8, (nc + 8 * SIM_GRAB - 1) / (8 * SIM_GRAB));
+  k_similarity<<<grid, 256, 0, st>>>(LA.key.as<unsigned long long>(), LA.w.as<uint32_t>(), LA.base.as<unsigned long long>(),
+                                     LB.key.as<unsigned long long>(), LB.w.as<uint32_t>(), LB.base.as<unsigned long long>(),
+                                     d_old, d_new, (unsigned long long)nc, d_next, d_common);
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(c->diff_ev[4], st));
+  CU(cudaMemcpyAsync(common, d_common, sizeof(int64_t) * nc, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  P.A.drop_staging(); P.B.drop_staging();
+  c->sim_ms[1] = elapsed_ms(c->diff_ev[2], c->diff_ev[3]);
+  c->sim_ms[2] = elapsed_ms(c->diff_ev[3], c->diff_ev[4]);
+  c->launches = P.A.launches + P.B.launches + 2 * 5 + 1;   // per side k_sim_sort, xscan (3), k_sim_compact; k_similarity
+  return TSM_OK;
+}
+
+extern "C" int tsm_similarity_last_ms(tsm_ctx* c, float* ms3) {
+  if (!c || !ms3) return TSM_E_ARG;
+  for (int i = 0; i < 3; ++i) ms3[i] = c->sim_ms[i];
   return TSM_OK;
 }
 

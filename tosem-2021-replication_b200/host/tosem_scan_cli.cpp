@@ -17,10 +17,11 @@
 //
 //   tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N]
 //   tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]
-//   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F]
+//   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--find-renames N]
 //   tosem-scan body   <project-root>... [--out F]
 //   tosem-scan releases <snapshot-root>=<tag>... [--out F]   |   releases --git <repository> [<revision>...] [--out F]
 //   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]
+//                      [--find-renames N]
 #include <algorithm>
 #include <atomic>
 #include <cctype>
@@ -1024,6 +1025,141 @@ static int cmd_releases(const std::vector<std::string>& specs_in, const std::str
   return 0;
 }
 
+// ---------------------------------------------------------------------------------- renames (docs/SPEC.md section 13)
+// One group = the deleted and the added files of one commit (history) or of one tree pair (diff), binary files already
+// left out.  find_renames pairs them in three one-to-one steps - exact (identical bytes), base name, matrix - with the
+// inexact scores of every group from ONE tsm_similarity call over the candidates that pass git's size filter.
+struct RenameFile { std::string path; std::vector<uint8_t> bytes; };
+struct RenamePair { size_t del, add; int similarity; bool exact; };
+struct RenameGroup { std::vector<RenameFile> del, add; std::vector<RenamePair> pairs; };
+
+static std::string base_name(const std::string& p) { const size_t s = p.rfind('/'); return s == std::string::npos ? p : p.substr(s + 1); }
+
+static void find_renames(tsm_ctx* ctx, std::vector<RenameGroup>& groups, int min_pct) {
+  const int64_t kMax = 60000, min_score = 600ll * min_pct, base_score = min_score + (kMax - min_score) / 2;
+  struct Cand { size_t g, d, a; };
+  std::vector<Cand> cands;
+  std::vector<std::vector<size_t>> del_order(groups.size()), add_order(groups.size());   // path order of each side
+  std::vector<std::vector<char>> del_used(groups.size()), add_used(groups.size());
+  for (size_t g = 0; g < groups.size(); ++g) {
+    RenameGroup& G = groups[g];
+    G.pairs.clear();
+    auto order = [](const std::vector<RenameFile>& v) {
+      std::vector<size_t> o(v.size());
+      for (size_t i = 0; i < o.size(); ++i) o[i] = i;
+      std::sort(o.begin(), o.end(), [&](size_t x, size_t y) { return v[x].path < v[y].path; });
+      return o;
+    };
+    del_order[g] = order(G.del); add_order[g] = order(G.add);
+    del_used[g].assign(G.del.size(), 0); add_used[g].assign(G.add.size(), 0);
+    // 1. exact: per added file in path order, the unpaired deleted file with the same bytes (same base name first)
+    for (size_t a : add_order[g]) {
+      long best = -1;
+      for (size_t d : del_order[g]) {
+        if (del_used[g][d] || G.del[d].bytes != G.add[a].bytes) continue;
+        if (best < 0) best = (long)d;
+        if (base_name(G.del[d].path) == base_name(G.add[a].path)) { best = (long)d; break; }
+      }
+      if (best < 0) continue;
+      del_used[g][(size_t)best] = add_used[g][a] = 1;
+      G.pairs.push_back({(size_t)best, a, 100, true});
+    }
+    // candidates of the inexact steps: git's size filter (a pair with 100 * min < N * max cannot reach the threshold)
+    for (size_t d = 0; d < G.del.size(); ++d)
+      for (size_t a = 0; a < G.add.size(); ++a) {
+        if (del_used[g][d] || add_used[g][a]) continue;
+        const int64_t x = (int64_t)G.del[d].bytes.size(), y = (int64_t)G.add[a].bytes.size();
+        if (std::max(x, y) == 0 || 100 * std::min(x, y) < (int64_t)min_pct * std::max(x, y)) continue;
+        cands.push_back({g, d, a});
+      }
+  }
+  std::map<std::pair<size_t, size_t>, std::vector<int64_t>> score;   // (group, del) -> score per added file (-1: no candidate)
+  if (!cands.empty()) {
+    std::vector<const std::vector<uint8_t>*> so, sn;                // the files of the candidates, each once per side
+    std::map<std::pair<size_t, size_t>, int32_t> io, in;
+    std::vector<int32_t> co, cn;
+    for (const Cand& c : cands) {
+      auto o = io.emplace(std::make_pair(c.g, c.d), (int32_t)so.size());
+      if (o.second) so.push_back(&groups[c.g].del[c.d].bytes);
+      auto n = in.emplace(std::make_pair(c.g, c.a), (int32_t)sn.size());
+      if (n.second) sn.push_back(&groups[c.g].add[c.a].bytes);
+      co.push_back(o.first->second); cn.push_back(n.first->second);
+    }
+    struct Packed { std::vector<int32_t> off, len; std::vector<uint8_t> arena, ext; };
+    auto pack = [](const std::vector<const std::vector<uint8_t>*>& files, Packed& P) {
+      const size_t n = files.size();
+      P.len.resize(n); P.off.resize(n + 1); P.ext.assign(n, 0);
+      for (size_t i = 0; i < n; ++i) P.len[i] = (int32_t)files[i]->size();
+      const int64_t bytes = tsm_layout(P.len.data(), (int32_t)n, P.off.data());
+      if (bytes < 0) die("rename candidates do not fit one int32-indexed arena");
+      P.arena.assign((size_t)std::max<int64_t>(bytes, 128), 0);
+      for (size_t i = 0; i < n; ++i) if (P.len[i]) memcpy(P.arena.data() + P.off[i], files[i]->data(), files[i]->size());
+    };
+    Packed PO, PN;
+    pack(so, PO); pack(sn, PN);
+    tsm_corpus ko{PO.arena.data(), PO.off.data(), PO.len.data(), PO.ext.data(), nullptr, (int32_t)so.size(), 1};
+    tsm_corpus kn{PN.arena.data(), PN.off.data(), PN.len.data(), PN.ext.data(), nullptr, (int32_t)sn.size(), 1};
+    std::vector<int64_t> common(cands.size());
+    ck(tsm_similarity(ctx, &ko, &kn, co.data(), cn.data(), (int64_t)cands.size(), common.data(), nullptr), "tsm_similarity");
+    for (size_t k = 0; k < cands.size(); ++k) {
+      const Cand& c = cands[k];
+      std::vector<int64_t>& row = score[{c.g, c.d}];
+      row.resize(groups[c.g].add.size(), -1);
+      const int64_t m = (int64_t)std::max(groups[c.g].del[c.d].bytes.size(), groups[c.g].add[c.a].bytes.size());
+      row[c.a] = common[k] * kMax / m;
+    }
+  }
+  auto get = [&](size_t g, size_t d, size_t a) -> int64_t {
+    auto it = score.find({g, d});
+    return it == score.end() ? -1 : it->second[a];
+  };
+  for (size_t g = 0; g < groups.size(); ++g) {
+    RenameGroup& G = groups[g];
+    // 2. base name: a base name that occurs once among the remaining deleted files and once among the remaining added ones
+    std::map<std::string, std::pair<int, size_t>> bd, ba;   // base name -> (count, file)
+    for (size_t d = 0; d < G.del.size(); ++d) if (!del_used[g][d]) { auto& e = bd[base_name(G.del[d].path)]; e.first++; e.second = d; }
+    for (size_t a = 0; a < G.add.size(); ++a) if (!add_used[g][a]) { auto& e = ba[base_name(G.add[a].path)]; e.first++; e.second = a; }
+    for (size_t a : add_order[g]) {
+      if (add_used[g][a]) continue;
+      const auto& ea = ba[base_name(G.add[a].path)];
+      auto it = bd.find(base_name(G.add[a].path));
+      if (ea.first != 1 || it == bd.end() || it->second.first != 1) continue;
+      const size_t d = it->second.second;
+      const int64_t s = get(g, d, a);
+      if (s < base_score) continue;
+      del_used[g][d] = add_used[g][a] = 1;
+      G.pairs.push_back({d, a, (int)(s / 600), false});
+    }
+    // 3. matrix: per added file its 4 best candidates (score, same base name, old path), then all of them greedily
+    struct M { int64_t s; bool same; size_t d, a; };
+    auto better = [&](const M& x, const M& y) {
+      if (x.s != y.s) return x.s > y.s;
+      if (x.same != y.same) return x.same;
+      if (G.del[x.d].path != G.del[y.d].path) return G.del[x.d].path < G.del[y.d].path;
+      return G.add[x.a].path < G.add[y.a].path;
+    };
+    std::vector<M> kept;
+    for (size_t a : add_order[g]) {
+      if (add_used[g][a]) continue;
+      std::vector<M> mine;
+      for (size_t d : del_order[g]) {
+        if (del_used[g][d]) continue;
+        const int64_t s = get(g, d, a);
+        if (s >= min_score && s >= 0) mine.push_back({s, base_name(G.del[d].path) == base_name(G.add[a].path), d, a});
+      }
+      std::sort(mine.begin(), mine.end(), better);
+      if (mine.size() > 4) mine.resize(4);
+      kept.insert(kept.end(), mine.begin(), mine.end());
+    }
+    std::sort(kept.begin(), kept.end(), better);
+    for (const M& m : kept) {
+      if (del_used[g][m.d] || add_used[g][m.a]) continue;
+      del_used[g][m.d] = add_used[g][m.a] = 1;
+      G.pairs.push_back({m.d, m.a, (int)(m.s / 600), false});
+    }
+  }
+}
+
 // ---------------------------------------------------------------------------------- diff (S8)
 // Changed assertion lines (docs/SPEC.md section 8) of one diff call: [n_groups][K] tables by group and the events of both
 // sides (tsm_diff_pairs_asserts), event arrays grown to the counts the library reports when they are too small.
@@ -1068,18 +1204,18 @@ static void churn_rows(std::ostream& os, const std::vector<std::string>& lead, c
 }
 
 static int cmd_diff(const std::string& old_root, const std::string& new_root, const std::string& out_path,
-                    const std::string& asserts_path, const std::string& churn_path) {
+                    const std::string& asserts_path, const std::string& churn_path, int rename_pct) {
   std::vector<FileEntry> a, b;
   walk(old_root, 0, true, a);
   walk(new_root, 0, true, b);
   std::map<std::string, const FileEntry*> bm;
   for (const FileEntry& f : b) bm[f.rel] = &f;
   // pairs by relative path; a file present on one side only is paired with the empty file
-  struct Pair { std::string rel; const FileEntry* o; const FileEntry* n; };
+  struct Pair { std::string rel; const FileEntry* o; const FileEntry* n; std::string old_rel; int similarity; };   // (renames: old path, %)
   std::vector<Pair> pairs;
   std::map<std::string, bool> seen;
-  for (const FileEntry& f : a) { auto it = bm.find(f.rel); pairs.push_back({f.rel, &f, it == bm.end() ? nullptr : it->second}); seen[f.rel] = true; }
-  for (const FileEntry& f : b) if (!seen.count(f.rel)) pairs.push_back({f.rel, nullptr, &f});
+  for (const FileEntry& f : a) { auto it = bm.find(f.rel); pairs.push_back({f.rel, &f, it == bm.end() ? nullptr : it->second, "", -1}); seen[f.rel] = true; }
+  for (const FileEntry& f : b) if (!seen.count(f.rel)) pairs.push_back({f.rel, nullptr, &f, "", -1});
   // git's numstat reports no line counts for binary files: a pair is skipped when either side has a NUL byte in its first 8000
   {
     auto binary = [](const FileEntry* f) {
@@ -1097,6 +1233,45 @@ static int cmd_diff(const std::string& old_root, const std::string& new_root, co
     if (skipped) fprintf(stderr, "tosem-scan: %zu binary file(s) skipped\n", skipped);
     pairs.swap(text);
   }
+  auto read_file = [](const FileEntry* f, uint8_t* dst) {
+    const int fd = open(f->abs.c_str(), O_RDONLY);
+    int64_t got = 0;
+    while (fd >= 0 && got < f->size) {
+      const ssize_t r = read(fd, dst + got, (size_t)(f->size - got));
+      if (r <= 0) break;
+      got += r;
+    }
+    if (fd >= 0) close(fd);
+    if (got != f->size) die("short read: " + f->abs);
+  };
+  tsm_ctx* ctx = nullptr;
+  ck(tsm_create(&ctx, 0, 1 << 20, 16, 1, 0), "tsm_create");
+  if (rename_pct >= 0) {                                   // a deleted and an added file that pair become one pair (old, new)
+    RenameGroup G;
+    std::vector<size_t> di, ai;
+    for (size_t i = 0; i < pairs.size(); ++i) {
+      const FileEntry* f = pairs[i].o ? pairs[i].o : pairs[i].n;
+      if (pairs[i].o && pairs[i].n) continue;
+      RenameFile r{pairs[i].rel, std::vector<uint8_t>((size_t)f->size)};
+      if (f->size) read_file(f, r.bytes.data());
+      if (pairs[i].o) { G.del.push_back(std::move(r)); di.push_back(i); } else { G.add.push_back(std::move(r)); ai.push_back(i); }
+    }
+    std::vector<RenameGroup> groups(1);
+    groups[0] = std::move(G);
+    find_renames(ctx, groups, rename_pct);
+    std::vector<char> drop(pairs.size(), 0);
+    size_t exact = 0;
+    for (const RenamePair& rp : groups[0].pairs) {
+      Pair& p = pairs[ai[rp.add]];
+      p.o = pairs[di[rp.del]].o; p.old_rel = pairs[di[rp.del]].rel; p.similarity = rp.similarity;
+      drop[di[rp.del]] = 1;
+      exact += rp.exact;
+    }
+    std::vector<Pair> kept;
+    for (size_t i = 0; i < pairs.size(); ++i) if (!drop[i]) kept.push_back(pairs[i]);
+    pairs.swap(kept);
+    fprintf(stderr, "tosem-scan: %zu rename(s) found (%zu exact, %zu inexact)\n", groups[0].pairs.size(), exact, groups[0].pairs.size() - exact);
+  }
   auto pack = [&](bool old_side, Batch& B, std::vector<FileEntry>& tmp) {
     for (const Pair& p : pairs) { const FileEntry* f = old_side ? p.o : p.n; tmp.push_back(f ? *f : FileEntry{p.rel, "", 0, 0, 0, nullptr}); }
     const size_t n = tmp.size();
@@ -1109,27 +1284,18 @@ static int cmd_diff(const std::string& old_root, const std::string& new_root, co
     B.arena = (uint8_t*)tsm_host_alloc(std::max<int64_t>(B.bytes, 128));
     if (!B.arena) die("pinned arena allocation failed");
     memset(B.arena, 0, (size_t)std::max<int64_t>(B.bytes, 128));
-    for (size_t i = 0; i < n; ++i) {
-      if (tmp[i].abs.empty() || B.len[i] == 0) continue;
-      const int fd = open(tmp[i].abs.c_str(), O_RDONLY);
-      int64_t got = 0;
-      while (fd >= 0 && got < B.len[i]) {
-        const ssize_t r = read(fd, B.arena + B.off[i] + got, (size_t)(B.len[i] - got));
-        if (r <= 0) break;
-        got += r;
-      }
-      if (fd >= 0) close(fd);
-      if (got != B.len[i]) die("short read: " + tmp[i].abs);
-    }
+    for (size_t i = 0; i < n; ++i)
+      if (!tmp[i].abs.empty() && B.len[i] != 0) read_file(&tmp[i], B.arena + B.off[i]);
   };
   Batch A, N; std::vector<FileEntry> ta, tn;
   pack(true, A, ta); pack(false, N, tn);
-  tsm_ctx* ctx = nullptr;
-  ck(tsm_create(&ctx, 0, 1 << 20, 16, 1, 0), "tsm_create");
   tsm_corpus ca{A.arena, A.off.data(), A.len.data(), A.ext.data(), A.grp.data(), (int32_t)A.count(), 1};
   tsm_corpus cn{N.arena, N.off.data(), N.len.data(), N.ext.data(), N.grp.data(), (int32_t)N.count(), 1};
   // ext tags of both sides feed the assertion-line classification of the changed lines
-  for (size_t i = 0; i < pairs.size(); ++i) { A.ext[i] = (uint8_t)ext_tag(pairs[i].rel); N.ext[i] = A.ext[i]; }
+  for (size_t i = 0; i < pairs.size(); ++i) {
+    N.ext[i] = (uint8_t)ext_tag(pairs[i].rel);
+    A.ext[i] = pairs[i].old_rel.empty() ? N.ext[i] : (uint8_t)ext_tag(pairs[i].old_rel);
+  }
   std::vector<int64_t> added(pairs.size()), removed(pairs.size());
   std::vector<tsm_diff_detail> det(pairs.size());
   ChangedAsserts ch;
@@ -1142,7 +1308,7 @@ static int cmd_diff(const std::string& old_root, const std::string& new_root, co
     csv_row(as, {"fileName", "change", "line", "statement", "category"});
     size_t ka = 0, kr = 0;
     for (size_t i = 0; i < pairs.size(); ++i) {
-      assert_rows(as, {}, pairs[i].rel, A.arena + A.off[i], A.len[i], ch.rev, kr, (uint32_t)i, "-");
+      assert_rows(as, {}, pairs[i].old_rel.empty() ? pairs[i].rel : pairs[i].old_rel, A.arena + A.off[i], A.len[i], ch.rev, kr, (uint32_t)i, "-");
       assert_rows(as, {}, pairs[i].rel, N.arena + N.off[i], N.len[i], ch.aev, ka, (uint32_t)i, "+");
     }
   }
@@ -1154,15 +1320,20 @@ static int cmd_diff(const std::string& old_root, const std::string& new_root, co
   std::ofstream os;
   if (!out_path.empty()) {
     os.open(out_path, std::ios::binary);
-    csv_row(os, {"fileName", "cloc", "added", "removed", "hunks_add", "hunks_del", "hunks_mod", "added_assert", "removed_assert"});
+    std::vector<std::string> head{"fileName", "cloc", "added", "removed", "hunks_add", "hunks_del", "hunks_mod", "added_assert", "removed_assert"};
+    if (rename_pct >= 0) head.insert(head.end(), {"oldFileName", "similarity"});
+    csv_row(os, head);
   }
   int64_t ta_ = 0, tr_ = 0;
   for (size_t i = 0; i < pairs.size(); ++i) {
     ta_ += added[i]; tr_ += removed[i];
-    if (os.is_open() && (added[i] || removed[i]))
-      csv_row(os, {pairs[i].rel, std::to_string(added[i] + removed[i]), std::to_string(added[i]), std::to_string(removed[i]),
-                   std::to_string(det[i].hunks_add), std::to_string(det[i].hunks_del), std::to_string(det[i].hunks_mod),
-                   std::to_string(det[i].added_assert), std::to_string(det[i].removed_assert)});
+    if (os.is_open() && (added[i] || removed[i] || pairs[i].similarity >= 0)) {
+      std::vector<std::string> row{pairs[i].rel, std::to_string(added[i] + removed[i]), std::to_string(added[i]), std::to_string(removed[i]),
+                                   std::to_string(det[i].hunks_add), std::to_string(det[i].hunks_del), std::to_string(det[i].hunks_mod),
+                                   std::to_string(det[i].added_assert), std::to_string(det[i].removed_assert)};
+      if (rename_pct >= 0) row.insert(row.end(), {pairs[i].old_rel, pairs[i].similarity >= 0 ? std::to_string(pairs[i].similarity) : ""});
+      csv_row(os, row);
+    }
   }
   printf("cloc,added,removed\r\n%lld,%lld,%lld\r\n", (long long)(ta_ + tr_), (long long)ta_, (long long)tr_);
   tsm_host_free(A.arena); tsm_host_free(N.arena);
@@ -1175,7 +1346,10 @@ static int cmd_diff(const std::string& old_root, const std::string& new_root, co
 // Host: commit chain, tree diff by object name (only entries whose blob changed are opened), blob inflation into the
 // two pinned arenas.  GPU: line records of both sides + per-pair Myers + hunks + changed assertion lines
 // (tsm_diff_pairs_detail), one call per batch of at most ~512 MiB per side.  Rows: one per (commit, changed file).
-struct BlobChange { std::string path; gitstore::Oid o, n; bool has_o, has_n; };
+struct BlobChange {
+  std::string path; gitstore::Oid o, n; bool has_o, has_n;
+  std::string old_path; int similarity = -1;               // a rename (--find-renames): the deleted file's path and the score in %
+};
 
 static void tree_diff(gitstore::Store& gs, const gitstore::Oid* a, const gitstore::Oid* b, const std::string& prefix,
                       bool all_files, std::vector<BlobChange>& out) {
@@ -1199,7 +1373,7 @@ static void tree_diff(gitstore::Store& gs, const gitstore::Oid* a, const gitstor
     const bool xb = x && x->is_blob(), yb = y && y->is_blob();                     // (symlinks and submodules are not files of the study)
     if (!xb && !yb) continue;
     if (!all_files && (lower(path).find("test") == std::string::npos || ext_tag(path) == TSM_EXT_OTHER)) continue;   // S0, S1
-    BlobChange c{path, {}, {}, xb, yb};
+    BlobChange c{path, {}, {}, xb, yb, "", -1};
     if (xb) c.o = x->oid;
     if (yb) c.n = y->oid;
     out.push_back(c);
@@ -1209,7 +1383,7 @@ static void tree_diff(gitstore::Store& gs, const gitstore::Oid* a, const gitstor
 // --dry-run: no GPU - the rows carry the object names, sizes and an FNV-1a checksum of both blobs instead of the counts
 // (what the CPU tests compare with `git diff-tree` / `git cat-file`).
 static int cmd_history(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files, const std::string& out_path,
-                       bool dry_run, const std::string& asserts_path, const std::string& churn_path) {
+                       bool dry_run, const std::string& asserts_path, const std::string& churn_path, int rename_pct) {
   gitstore::Store gs;
   std::string err;
   if (!gs.open(repo, err)) die(err);
@@ -1236,11 +1410,72 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
     tree_diff(gs, has_parent ? &parent.tree : nullptr, &chain[i].c.tree, "", all_files, ch);
     for (auto& c : ch) rows.push_back({i, c});
   }
+  tsm_ctx* ctx = nullptr;
+  if (!dry_run) ck(tsm_create(&ctx, 0, 1 << 20, 16, 1, 0), "tsm_create");
+  const int64_t kBatch = 512ll << 20;
+  int64_t renames = 0, renames_exact = 0;
+  if (rename_pct >= 0) {
+    // per commit, its deleted and added files (binary ones left out) form a group; groups are paired together until a side
+    // holds kBatch bytes, and a pair's two rows become one row (old blob, new blob) at the added file's place
+    std::vector<char> drop(rows.size(), 0);
+    std::vector<RenameGroup> groups;
+    std::vector<std::vector<size_t>> at_del, at_add;       // row of each file of each group
+    int64_t bytes_d = 0, bytes_a = 0;
+    auto flush = [&]() {
+      find_renames(ctx, groups, rename_pct);
+      for (size_t g = 0; g < groups.size(); ++g)
+        for (const RenamePair& rp : groups[g].pairs) {
+          const BlobChange& d = rows[at_del[g][rp.del]].ch;
+          BlobChange& a = rows[at_add[g][rp.add]].ch;
+          a.o = d.o; a.has_o = true; a.old_path = d.path; a.similarity = rp.similarity;
+          drop[at_del[g][rp.del]] = 1;
+          ++renames; renames_exact += rp.exact;
+        }
+      groups.clear(); at_del.clear(); at_add.clear();
+      bytes_d = bytes_a = 0;
+    };
+    for (size_t r0 = 0, r1 = 0; r0 < rows.size(); r0 = r1) {
+      for (r1 = r0; r1 < rows.size() && rows[r1].step == rows[r0].step; ++r1) {}
+      std::vector<size_t> del, add;
+      for (size_t r = r0; r < r1; ++r) {
+        if (rows[r].ch.has_o && !rows[r].ch.has_n) del.push_back(r);
+        if (!rows[r].ch.has_o && rows[r].ch.has_n) add.push_back(r);
+      }
+      if (del.empty() || add.empty()) continue;
+      RenameGroup G;
+      std::vector<size_t> gd, ga;
+      auto load = [&](const std::vector<size_t>& which, bool old_side, std::vector<RenameFile>& out, std::vector<size_t>& at) {
+        for (size_t r : which) {
+          const gitstore::Oid& id = old_side ? rows[r].ch.o : rows[r].ch.n;
+          gitstore::Object x;
+          if (!gs.read(id, x) || x.type != gitstore::OBJ_BLOB) die("unreadable blob " + id.hex());
+          if (!x.data.empty() && memchr(x.data.data(), 0, std::min<size_t>(x.data.size(), 8000)) != nullptr) continue;   // binary
+          out.push_back({rows[r].ch.path, std::move(x.data)});
+          at.push_back(r);
+        }
+      };
+      load(del, true, G.del, gd);
+      load(add, false, G.add, ga);
+      if (G.del.empty() || G.add.empty()) continue;
+      for (const RenameFile& f : G.del) bytes_d += (int64_t)f.bytes.size() + 256;
+      for (const RenameFile& f : G.add) bytes_a += (int64_t)f.bytes.size() + 256;
+      groups.push_back(std::move(G)); at_del.push_back(gd); at_add.push_back(ga);
+      if (bytes_d >= kBatch || bytes_a >= kBatch) flush();
+    }
+    if (!groups.empty()) flush();
+    std::vector<Row> kept;
+    for (size_t r = 0; r < rows.size(); ++r) if (!drop[r]) kept.push_back(rows[r]);
+    rows.swap(kept);
+  }
   std::ofstream os;
   if (!out_path.empty()) {
     os.open(out_path, std::ios::binary);
     if (dry_run) csv_row(os, {"commit", "parent", "time", "fileName", "old_blob", "new_blob", "old_size", "new_size", "old_fnv", "new_fnv"});
-    else csv_row(os, {"commit", "parent", "time", "fileName", "cloc", "added", "removed", "hunks_add", "hunks_del", "hunks_mod", "added_assert", "removed_assert"});
+    else {
+      std::vector<std::string> head{"commit", "parent", "time", "fileName", "cloc", "added", "removed", "hunks_add", "hunks_del", "hunks_mod", "added_assert", "removed_assert"};
+      if (rename_pct >= 0) head.insert(head.end(), {"oldFileName", "similarity"});
+      csv_row(os, head);
+    }
   }
   const bool want_asserts = !dry_run && (!asserts_path.empty() || !churn_path.empty());
   std::ofstream as;
@@ -1250,11 +1485,8 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
   }
   // per commit with changed assertion lines: its [K] added and removed rows (a commit's files may span two batches)
   std::map<size_t, std::vector<int64_t>> churn;
-  tsm_ctx* ctx = nullptr;
-  if (!dry_run) ck(tsm_create(&ctx, 0, 1 << 20, 16, 1, 0), "tsm_create");
   std::vector<int64_t> per_add(chain.size(), 0), per_rem(chain.size(), 0), per_files(chain.size(), 0);
   int64_t binaries = 0, pairs_done = 0;
-  const int64_t kBatch = 512ll << 20;
   size_t r0 = 0;
   while (r0 < rows.size()) {
     // inflate blobs until a side of the batch is full
@@ -1297,7 +1529,11 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
         for (size_t i = 0; i < n; ++i) if (B.len[i]) memcpy(B.arena + B.off[i], blobs[i].data(), blobs[i].size());
       };
       pack(A, bo); pack(N, bn);
-      for (size_t i = 0; i < n; ++i) { A.ext[i] = (uint8_t)ext_tag(rows[idx[i]].ch.path); N.ext[i] = A.ext[i]; }
+      for (size_t i = 0; i < n; ++i) {
+        const BlobChange& c = rows[idx[i]].ch;
+        N.ext[i] = (uint8_t)ext_tag(c.path);
+        A.ext[i] = c.old_path.empty() ? N.ext[i] : (uint8_t)ext_tag(c.old_path);
+      }
       std::vector<size_t> group_step;                        // group g of the batch = commit group_step[g]
       for (size_t i = 0; want_asserts && i < n; ++i) {
         if (group_step.empty() || group_step.back() != rows[idx[i]].step) group_step.push_back(rows[idx[i]].step);
@@ -1328,7 +1564,7 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
             const Row& r = rows[idx[i]];
             const Step& st = chain[r.step];
             const std::vector<std::string> lead{st.id.hex(), st.c.parents.empty() ? "" : st.c.parents[0].hex(), std::to_string(st.c.time)};
-            assert_rows(as, lead, r.ch.path, A.arena + A.off[i], A.len[i], chg.rev, kr, (uint32_t)i, "-");
+            assert_rows(as, lead, r.ch.old_path.empty() ? r.ch.path : r.ch.old_path, A.arena + A.off[i], A.len[i], chg.rev, kr, (uint32_t)i, "-");
             assert_rows(as, lead, r.ch.path, N.arena + N.off[i], N.len[i], chg.aev, ka, (uint32_t)i, "+");
           }
         }
@@ -1338,10 +1574,12 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
         per_add[r.step] += added[i]; per_rem[r.step] += removed[i]; per_files[r.step]++;
         if (os.is_open()) {
           const Step& st = chain[r.step];
-          csv_row(os, {st.id.hex(), st.c.parents.empty() ? "" : st.c.parents[0].hex(), std::to_string(st.c.time), r.ch.path,
-                       std::to_string(added[i] + removed[i]), std::to_string(added[i]), std::to_string(removed[i]),
-                       std::to_string(det[i].hunks_add), std::to_string(det[i].hunks_del), std::to_string(det[i].hunks_mod),
-                       std::to_string(det[i].added_assert), std::to_string(det[i].removed_assert)});
+          std::vector<std::string> row{st.id.hex(), st.c.parents.empty() ? "" : st.c.parents[0].hex(), std::to_string(st.c.time), r.ch.path,
+                                       std::to_string(added[i] + removed[i]), std::to_string(added[i]), std::to_string(removed[i]),
+                                       std::to_string(det[i].hunks_add), std::to_string(det[i].hunks_del), std::to_string(det[i].hunks_mod),
+                                       std::to_string(det[i].added_assert), std::to_string(det[i].removed_assert)};
+          if (rename_pct >= 0) row.insert(row.end(), {r.ch.old_path, r.ch.similarity >= 0 ? std::to_string(r.ch.similarity) : ""});
+          csv_row(os, row);
         }
       }
       pairs_done += (int64_t)n;
@@ -1364,6 +1602,9 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
   }
   fprintf(stderr, "tosem-scan: history of %s: %zu commits, %lld changed files diffed on the GPU, %lld binary skipped, cloc %lld (+%lld -%lld)\n",
           rev.c_str(), chain.size(), (long long)pairs_done, (long long)binaries, (long long)(ta + tr), (long long)ta, (long long)tr);
+  if (rename_pct >= 0)
+    fprintf(stderr, "tosem-scan: %lld rename(s) found at %d%% (%lld exact, %lld inexact)\n", (long long)renames, rename_pct,
+            (long long)renames_exact, (long long)(renames - renames_exact));
   return 0;
 }
 
@@ -1371,10 +1612,12 @@ static void usage() {
   fprintf(stderr,
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
           "       tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]\n"
-          "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F]\n"
+          "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--find-renames N]\n"
           "       tosem-scan body   <project-root>... [--out F]\n"
           "       tosem-scan releases <snapshot-root>=<tag>... [--out F]   |   releases --git <repository> [<revision>...] [--out F]\n"
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
+          "                          [--find-renames N]\n"
+          "--find-renames N (0..100): pair deleted and added files at least N %% similar, as git -M<N>%% does (docs/SPEC.md section 13).\n"
           "Scans run on the GPU through libtosemscan.so (sm_90a); there is no CPU fallback.\n");
 }
 
@@ -1397,10 +1640,21 @@ int main(int argc, char** argv) {
   if (cmd == "reduce") { if (pos.size() != 1) die("reduce needs the taxonomy csv"); return cmd_reduce(pos[0], opt["--strategy"], opt["--methods"], opt["--properties"], opt["--correlate"], opt["--correlate-tex"], opt["--correlate-counts"], opt["--correlate-merged"]); }
   if (cmd == "releases") { if (pos.empty() && !opt.count("--git")) die("releases needs <root>=<tag>... or --git <repository>"); return cmd_releases(pos, opt["--out"], opt["--git"]); }
   if (cmd == "body") { if (pos.empty()) die("body needs at least one project root"); return cmd_body(pos, opt["--out"]); }
-  if (cmd == "history") { if (pos.size() != 1) die("history needs the repository"); return cmd_history(pos[0], opt.count("--rev") ? opt["--rev"] : "HEAD",
+  int rename_pct = -1;                                     // --find-renames N (docs/SPEC.md section 13); -1 = off
+  if (opt.count("--find-renames")) {
+    std::string v = opt["--find-renames"];
+    if (!v.empty() && v.back() == '%') v.pop_back();
+    char* end = nullptr;
+    const long pct = v.empty() ? -1 : strtol(v.c_str(), &end, 10);
+    if (pct < 0 || pct > 100 || *end) die("--find-renames needs a similarity from 0 to 100");
+    rename_pct = (int)pct;
+  }
+  if (cmd == "history") { if (pos.size() != 1) die("history needs the repository");
+                          if (dry_run && rename_pct >= 0) die("--dry-run and --find-renames cannot be combined (renames need the GPU)");
+                          return cmd_history(pos[0], opt.count("--rev") ? opt["--rev"] : "HEAD",
                                                   opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0, all_files, opt["--out"], dry_run,
-                                                  opt["--asserts"], opt["--assert-churn"]); }
-  if (cmd == "diff") { if (pos.size() != 2) die("diff needs <old-root> <new-root>"); return cmd_diff(pos[0], pos[1], opt["--out"], opt["--asserts"], opt["--assert-churn"]); }
+                                                  opt["--asserts"], opt["--assert-churn"], rename_pct); }
+  if (cmd == "diff") { if (pos.size() != 2) die("diff needs <old-root> <new-root>"); return cmd_diff(pos[0], pos[1], opt["--out"], opt["--asserts"], opt["--assert-churn"], rename_pct); }
   usage();
   return 2;
 }

@@ -35,7 +35,7 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_upload", "tsm_scan_resident", "tsm_download", "tsm_device_counts", "tsm_last_launch_count", "tsm_last_kernel_ms", "tsm_kernel_ms_stats",
            "tsm_diff_pairs", "tsm_diff_pairs_detail", "tsm_statements", "tsm_line_hashes", "tsm_diff_upload", "tsm_diff_resident", "tsm_diff_last_ms",
            "tsm_diff_pairs_asserts", "tsm_diff_resident_asserts", "tsm_reduce", "tsm_host_alloc", "tsm_host_free", "tsm_layout", "tsm_gen_sizes",
-           "tsm_gen_fill", "tsm_gen_edit", "tsm_gen_pair_sizes", "tsm_gen_pair_fill"]
+           "tsm_gen_fill", "tsm_gen_edit", "tsm_gen_pair_sizes", "tsm_gen_pair_fill", "tsm_similarity", "tsm_similarity_last_ms"]
 
 
 class TsmError(RuntimeError):
@@ -141,6 +141,11 @@ def lib():
         L.tsm_diff_resident_asserts.argtypes = [C.c_void_p] * 4 + [C.POINTER(_DiffAsserts), C.c_void_p]
         L.tsm_diff_last_ms.restype = C.c_int
         L.tsm_diff_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 3)]
+        L.tsm_similarity.restype = C.c_int
+        L.tsm_similarity.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus), C.c_void_p, C.c_void_p, C.c_int64,
+                                     C.c_void_p, C.c_void_p]
+        L.tsm_similarity_last_ms.restype = C.c_int
+        L.tsm_similarity_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 3)]
         _lib = L
     return _lib
 
@@ -609,4 +614,24 @@ class Scanner:
         """Device time of the last diff call: [k_scan over both sides, k_diff_small, k_myers + k_myers_trace of the pairs it left over] in ms."""
         ms = (C.c_float * 3)()
         lib().tsm_diff_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
+
+    def similarity(self, olds, news, cand_old, cand_new, stream=None):
+        """Rename similarity (docs/SPEC.md section 13): common[c] of file cand_old[c] of `olds` and file cand_new[c] of `news`
+        as np.int64[n_cand] (git's score is common * 60000 // max(size_old, size_new))."""
+        co = np.ascontiguousarray(cand_old, np.int32).ravel()
+        cn = np.ascontiguousarray(cand_new, np.int32).ravel()
+        if co.size != cn.size:
+            raise ValueError("cand_old and cand_new differ in length")
+        out = np.zeros(max(co.size, 1), np.int64)
+        a, b = olds.c_struct(), news.c_struct()
+        rc = lib().tsm_similarity(self._ctx, C.byref(a), C.byref(b), _p(co), _p(cn), co.size, _p(out), stream)
+        if rc:
+            raise TsmError(rc, "tsm_similarity")
+        return out[:co.size]
+
+    def similarity_last_ms(self):
+        """Device time of the last similarity call: [k_scan over both sides, sort / merge, k_similarity] in ms."""
+        ms = (C.c_float * 3)()
+        lib().tsm_similarity_last_ms(self._ctx, C.byref(ms))
         return [float(x) for x in ms]
