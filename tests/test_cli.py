@@ -285,9 +285,13 @@ def test_diff_trees(tmp_path):
     (new / "fresh.c").write_bytes(b"c\n")
     (old / "same.h").write_bytes(b"s\n")
     (new / "same.h").write_bytes(b"s\n")
+    (old / "blob.py").write_bytes(b"x = 1\n\x00\x01\n")            # binary on one side: skipped, like git's numstat
+    (old / "a" / "tail.py").write_bytes(b"p\nq")                # only the final LF differs: no line changes (SPEC section 2)
+    (new / "a" / "tail.py").write_bytes(b"p\nq\n")
     outp = str(tmp_path / "churn.csv")
     out = subprocess.run([CLI, "diff", str(old), str(new), "--out", outp], capture_output=True, text=True)
     assert out.returncode == 0, out.stderr
+    assert "tosem-scan: 1 binary file(s) skipped" in out.stderr.splitlines()
     assert out.stdout.replace("\r\n", "\n").strip().split("\n") == ["cloc,added,removed", "6,3,3"]
     got = {r[0]: r[1:] for r in read_csv(outp)[1:]}
     # cloc, added, removed, hunks_add, hunks_del, hunks_mod, added_assert, removed_assert

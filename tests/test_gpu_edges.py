@@ -313,12 +313,18 @@ def test_dense_event_corpora(line, ext, rev_b):
         assert np.array_equal(got["header_events"], want["header_events"])
 
 
-def test_dense_events_through_the_cli(tmp_path):
-    """`tosem-scan scan` over a tree whose only file is 2 MB of `assert\\n`."""
-    n = (2 << 20) // 7
+def dense_tree(tmp_path, line):
+    """A project whose only file, tests/test_dense.py, is 2 MB of `line`; returns the number of lines."""
+    n = (2 << 20) // len(line)
     p = tmp_path / "proj" / "tests" / "test_dense.py"
     p.parent.mkdir(parents=True)
-    p.write_bytes(b"assert\n" * n)
+    p.write_bytes(line * n)
+    return n
+
+
+def test_dense_events_through_the_cli(tmp_path):
+    """`tosem-scan scan` over a tree whose only file is 2 MB of `assert\\n`."""
+    n = dense_tree(tmp_path, b"assert\n")
     sum_p = str(tmp_path / "summary.csv")
     out = subprocess.run([CLI, "scan", str(tmp_path / "proj"), "--summary", sum_p], capture_output=True, text=True)
     assert out.returncode == 0, out.stderr
@@ -326,3 +332,22 @@ def test_dense_events_through_the_cli(tmp_path):
     assert {k: int(v) for k, v in agg.items() if int(v)} == {"assertTrue": n}
     rows = open(sum_p, "rb").read().decode().split("\r\n")
     assert rows[1].split(",")[1:3] == ["tests/test_dense.py", str(n)]
+
+
+@pytest.mark.parametrize("cmd", ["body", "releases"])
+def test_dense_events_through_body_and_releases(tmp_path, cmd):
+    """`tosem-scan body` over 2 MB of `def\\n` and `releases` over 2 MB of `assert\\n`: more events than the host arrays of
+    bytes / 8 + 1024 both commands start with, as for `scan` above."""
+    n = dense_tree(tmp_path, b"def\n" if cmd == "body" else b"assert\n")
+    outp = str(tmp_path / "out.csv")
+    proj = str(tmp_path / "proj")
+    out = subprocess.run([CLI, "body", proj, "--out", outp] if cmd == "body" else [CLI, "releases", proj + "=v1", "--out", outp],
+                         capture_output=True, text=True)
+    assert out.returncode == 0, out.stderr
+    rows = open(outp, "rb").read().decode().split("\r\n")
+    if cmd == "body":
+        assert orc.header_kind(1, b"def")                   # every line starts a case; a case header is no statement
+        assert out.stdout.replace("\r\n", "\n").strip().split("\n") == ["files,cases,statements", "1,%d,0" % n]
+        assert len(rows) == n + 2 and rows[-2].split(",")[::3] == [str(n), str(n)]
+    else:
+        assert rows[1].split(",") == ["1", "tests/test_dense.py", "tests/test_dense.py", str(n), "%d:assertTrue" % n]

@@ -248,22 +248,53 @@ def test_assert_rows_of_renamed_files(repo, tmp_path):
     assert got_churn == {k: tuple(v) for k, v in churn.items()}
 
 
+def read_rows(path):
+    return list(csv.reader(open(path, newline="")))
+
+
 def test_diff_of_archives_gives_the_history_rows(repo, tmp_path):
-    table, _ = run_history(repo, tmp_path, 50)
+    """`diff` of two archives equals `history` at that commit with the commit columns removed, with and without renames:
+    --out rows (those that change a line or pair a rename: `history` also lists a changed file whose diff changes no
+    line), --asserts and --assert-churn."""
+    roots = {}
     for k in (1, 2):                                         # the commits whose changed files are all test files
         commit, parent = commits(repo)[k]
-        roots = []
         for rev in (parent, commit):
-            d = tmp_path / ("tree_%d_%s" % (k, rev[:8]))
+            if rev in roots:
+                continue
+            d = tmp_path / ("tree_%s" % rev[:8])
             os.makedirs(d)
             tar = tmp_path / ("t_%s.tar" % rev[:8])
             tar.write_bytes(git(repo, "archive", "--format=tar", rev, text=False))
             with tarfile.open(tar) as t:
                 t.extractall(d, filter="data")
-            roots.append(str(d))
-        out = tmp_path / ("d%d.csv" % k)
-        r = subprocess.run([CLI, "diff", roots[0], roots[1], "--out", str(out), "--find-renames", "50"], capture_output=True, text=True)
+            roots[rev] = str(d)
+    for renames in (["--find-renames", "50"], []):
+        check_diff_against_history(repo, tmp_path / ("r" if renames else "p"), roots, renames)
+
+
+def check_diff_against_history(repo, tmp, roots, renames):
+    os.makedirs(tmp)
+    hist = {p: tmp / ("h_%s.csv" % p) for p in ("out", "asserts", "churn")}
+    r = subprocess.run([CLI, "history", str(repo), "--out", str(hist["out"]), "--asserts", str(hist["asserts"]),
+                        "--assert-churn", str(hist["churn"])] + renames, capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    table = read_rows(hist["out"])
+    for k in (1, 2):
+        commit, parent = commits(repo)[k]
+        mine = {p: tmp / ("d%d_%s.csv" % (k, p)) for p in ("out", "asserts", "churn")}
+        r = subprocess.run([CLI, "diff", roots[parent], roots[commit], "--out", str(mine["out"]), "--asserts", str(mine["asserts"]),
+                            "--assert-churn", str(mine["churn"])] + renames, capture_output=True, text=True)
         assert r.returncode == 0, r.stderr
-        got = sorted(tuple(x) for x in list(csv.reader(open(out, newline="")))[1:])
-        want = sorted(tuple(x[3:]) for x in table[1:] if x[0] == commit)
-        assert got == want and len(want) >= 2
+        got = read_rows(mine["out"])
+        assert got[0] == table[0][3:]
+        want = [x[3:] for x in table[1:] if x[0] == commit and (x[5] != "0" or x[6] != "0" or (renames and x[-1]))]
+        assert sorted(got[1:]) == sorted(want) and len(want) >= 2
+        got = read_rows(mine["asserts"])
+        want = read_rows(hist["asserts"])
+        assert got[0] == want[0][3:]
+        assert sorted(got[1:]) == sorted(x[3:] for x in want[1:] if x[0] == commit) and len(got) > 1
+        got = read_rows(mine["churn"])
+        want = read_rows(hist["churn"])
+        assert got[0] == want[0][1:]
+        assert got[1:] == [x[1:] for x in want[1:] if x[0] == commit] and len(got) > 1

@@ -34,6 +34,7 @@
 #include <unistd.h>
 #include <filesystem>
 #include <fstream>
+#include <functional>
 #include <future>
 #include <map>
 #include <memory>
@@ -112,6 +113,7 @@ static int ext_tag(const std::string& rel) {               // S1
   return TSM_EXT_OTHER;
 }
 static const char* ext_name(int t) { static const char* n[] = {"", "py", "cc", "cpp", "java", "c", "h"}; return n[t]; }
+static std::string base_name(const std::string& p) { const size_t s = p.rfind('/'); return s == std::string::npos ? p : p.substr(s + 1); }
 
 static std::string test_name_tag(const std::string& rel, bool fixture) {   // S2 (mock / Module: parity unpinned, omitted)
   std::string t;
@@ -201,33 +203,43 @@ struct Batch {                                             // one packed arena (
   size_t count() const { return idx.size(); }
 };
 
+// The files of lengths B.len laid out by tsm_layout (B.off, B.bytes) in a zeroed pinned arena, their ext / grp tags zero; the
+// caller fills the bytes and the tags.
+static void alloc_arena(Batch& B) {
+  const size_t n = B.len.size();
+  B.off.resize(n + 1); B.ext.assign(n, 0); B.grp.assign(n, 0);
+  B.bytes = tsm_layout(B.len.data(), (int32_t)n, B.off.data());
+  if (B.bytes < 0) die("batch does not fit an int32-indexed arena");
+  B.arena = (uint8_t*)tsm_host_alloc(std::max<int64_t>(B.bytes, 128));
+  if (!B.arena) die("pinned arena allocation failed (no CUDA device? there is no CPU fallback)");
+  memset(B.arena, 0, (size_t)std::max<int64_t>(B.bytes, 128));
+}
+
+static bool read_file(const std::string& path, uint8_t* dst, int64_t size) {   // false on a short read
+  const int fd = open(path.c_str(), O_RDONLY);
+  int64_t got = 0;
+  while (fd >= 0 && got < size) {
+    const ssize_t r = read(fd, dst + got, (size_t)(size - got));
+    if (r <= 0) break;
+    got += r;
+  }
+  if (fd >= 0) close(fd);
+  return got == size;
+}
+
 static void load_batch(const std::vector<FileEntry>& files, Batch& b) {
   const size_t n = b.count();
-  b.len.resize(n); b.off.resize(n + 1); b.ext.resize(n); b.grp.resize(n);
-  for (size_t i = 0; i < n; ++i) {
-    const FileEntry& f = files[b.idx[i]];
-    b.len[i] = (int32_t)f.size; b.ext[i] = (uint8_t)f.ext; b.grp[i] = (uint16_t)f.grp;
-  }
-  b.bytes = tsm_layout(b.len.data(), (int32_t)n, b.off.data());
-  if (b.bytes < 0) die("batch does not fit an int32-indexed arena");
-  b.arena = (uint8_t*)tsm_host_alloc(std::max<int64_t>(b.bytes, 128));
-  if (!b.arena) die("pinned arena allocation failed (no CUDA device? there is no CPU fallback)");
-  memset(b.arena, 0, (size_t)std::max<int64_t>(b.bytes, 128));
+  b.len.resize(n);
+  for (size_t i = 0; i < n; ++i) b.len[i] = (int32_t)files[b.idx[i]].size;
+  alloc_arena(b);
+  for (size_t i = 0; i < n; ++i) { b.ext[i] = (uint8_t)files[b.idx[i]].ext; b.grp[i] = (uint16_t)files[b.idx[i]].grp; }
   // the reads of a batch run on a few host threads (a source tree is many small files: latency-bound)
   const unsigned nt = std::max(1u, std::min({std::thread::hardware_concurrency(), 32u, (unsigned)((n + 63) / 64)}));
   std::atomic<long> bad{-1};
   auto reader = [&](unsigned t) {
     for (size_t i = t; i < n && bad.load(std::memory_order_relaxed) < 0; i += nt) {
       if (files[b.idx[i]].blob) { if (b.len[i]) memcpy(b.arena + b.off[i], files[b.idx[i]].blob->data(), (size_t)b.len[i]); continue; }
-      const int fd = open(files[b.idx[i]].abs.c_str(), O_RDONLY);
-      int64_t got = 0;
-      while (fd >= 0 && got < b.len[i]) {
-        const ssize_t r = read(fd, b.arena + b.off[i] + got, (size_t)(b.len[i] - got));
-        if (r <= 0) break;
-        got += r;
-      }
-      if (fd >= 0) close(fd);
-      if (got != b.len[i]) bad.store((long)i);
+      if (!read_file(files[b.idx[i]].abs, b.arena + b.off[i], b.len[i])) bad.store((long)i);
     }
   };
   std::vector<std::thread> th;
@@ -237,8 +249,40 @@ static void load_batch(const std::vector<FileEntry>& files, Batch& b) {
   if (bad.load() >= 0) die("short read: " + files[b.idx[(size_t)bad.load()]].abs);
 }
 
+// The files from `first` on that fit one batch of `body` / `releases` (512 MiB of arena, 2^19 files), loaded.
+static Batch next_batch(const std::vector<FileEntry>& files, size_t& first) {
+  Batch B;
+  int64_t cur = 0;
+  while (first < files.size() && (B.count() == 0 || (cur + files[first].size < (1ll << 29) && B.count() < (1u << 19)))) {
+    cur += (files[first].size + 127) / 128 * 128; B.idx.push_back((uint32_t)first); ++first;
+  }
+  load_batch(files, B);
+  return B;
+}
+
 static void cu_ck(cudaError_t e, const char* what) { if (e != cudaSuccess) die(std::string(what) + ": " + cudaGetErrorString(e)); }
 static void nccl_ck(ncclResult_t r, const char* what) { if (r != ncclSuccess) die(std::string(what) + ": " + ncclGetErrorString(r)); }
+
+// tsm_scan of one packed batch of `bytes` with the events `flags` asks for in aev / hev.  The host arrays start at bytes / 8 + 1024
+// entries; a denser batch returns TSM_E_CAPACITY with both counts, and its events are downloaded again into arrays of that size.
+static void scan_events(tsm_ctx* ctx, const tsm_corpus& c, int64_t bytes, tsm_result& r, uint32_t flags, cudaStream_t st,
+                        std::vector<tsm_assert_event>& aev, std::vector<tsm_header_event>& hev) {
+  const bool want_a = flags & TSM_SCAN_ASSERT_EVENTS, want_h = flags & TSM_SCAN_HEADER_EVENTS;
+  auto size = [&](int64_t na, int64_t nh) {
+    aev.resize(want_a ? (size_t)na : 0); hev.resize(want_h ? (size_t)nh : 0);
+    r.aev = want_a ? aev.data() : nullptr; r.aev_cap = (int64_t)aev.size();
+    r.hev = want_h ? hev.data() : nullptr; r.hev_cap = (int64_t)hev.size();
+  };
+  const int64_t cap = std::max<int64_t>(bytes / 8 + 1024, 1024);
+  size(cap, cap);
+  int rc = tsm_scan(ctx, &c, &r, flags, st);
+  if (rc == TSM_E_CAPACITY && (r.n_aev > cap || r.n_hev > cap)) {
+    size(std::max<int64_t>(r.n_aev, 1), std::max<int64_t>(r.n_hev, 1));
+    rc = tsm_download(ctx, &r, st);
+  }
+  ck(rc, "tsm_scan");
+  aev.resize(want_a ? (size_t)r.n_aev : 0); hev.resize(want_h ? (size_t)r.n_hev : 0);
+}
 
 // The statement of an assertion event (the statement may be longer than the 16-bit event field: its end is re-derived on the
 // host if saturated) and its category cell (the verbatim identifier for 127, docs/SPEC.md section 6).
@@ -249,6 +293,13 @@ static std::string event_statement(const uint8_t* base, int32_t size, const tsm_
 }
 static std::string event_category(const uint8_t* base, const tsm_assert_event& ev) {
   return ev.cat == 127 ? std::string((const char*)base + ev.ident_off, ev.ident_len) : std::string(tsm_category_name(ev.cat));
+}
+// The assertion cell of a per-file row, "n:category, ...": the categories in first-seen `order`, stably sorted by count, descending.
+static std::string hist_cell(std::map<std::string, int64_t>& hist, std::vector<std::string> order) {
+  std::stable_sort(order.begin(), order.end(), [&](const std::string& x, const std::string& y) { return hist[x] > hist[y]; });
+  std::string a;
+  for (const std::string& c : order) { if (!a.empty()) a += ", "; a += std::to_string(hist[c]) + ":" + c; }
+  return a;
 }
 
 // The raw rows (fileName, extension, test_name, method, statement, counts, category: ML-Testing-v1.xlsx!apollo_tests:R1) and
@@ -284,11 +335,8 @@ static void render_file(const FileEntry& f, int64_t id, const uint8_t* base, int
     rows_txt = os.str();
   }
   if (want_sum) {
-    std::stable_sort(hist_order.begin(), hist_order.end(), [&](const std::string& x, const std::string& y) { return hist[x] > hist[y]; });
-    std::string a;
-    for (const std::string& c : hist_order) { if (!a.empty()) a += ", "; a += std::to_string(hist[c]) + ":" + c; }
     std::ostringstream os;
-    csv_row(os, {std::to_string(id), f.rel, std::to_string(st.n_assert), a});
+    csv_row(os, {std::to_string(id), f.rel, std::to_string(st.n_assert), hist_cell(hist, hist_order)});
     sum_txt = os.str();
   }
 }
@@ -388,19 +436,9 @@ static int cmd_scan(const std::vector<std::string>& roots, const std::string& ro
       tsm_corpus c{B.arena, B.off.data(), B.len.data(), B.ext.data(), B.grp.data(), (int32_t)B.count(), n_groups};
       stats.resize(B.count());
       group_counts.assign((size_t)n_groups * TSM_NUM_CATEGORIES, 0);
-      const int64_t cap = std::max<int64_t>(B.bytes / 8 + 1024, 1024);
-      aev.resize((size_t)cap); hev.resize((size_t)cap);
       tsm_result r{};
       r.stats = stats.data(); r.group_counts = group_counts.data();
-      r.aev = aev.data(); r.aev_cap = cap; r.hev = hev.data(); r.hev_cap = cap;
-      int rc = tsm_scan(ctx, &c, &r, TSM_SCAN_ASSERT_EVENTS | TSM_SCAN_HEADER_EVENTS | (rev_b ? TSM_SCAN_REV_B : 0u), st);
-      if (rc == TSM_E_CAPACITY && (r.n_aev > cap || r.n_hev > cap)) {   // denser than bytes / 8 events: fetch again at the size
-        aev.resize((size_t)std::max<int64_t>(r.n_aev, 1)); hev.resize((size_t)std::max<int64_t>(r.n_hev, 1));   // tsm_download reports
-        r.aev = aev.data(); r.aev_cap = (int64_t)aev.size(); r.hev = hev.data(); r.hev_cap = (int64_t)hev.size();
-        rc = tsm_download(ctx, &r, st);
-      }
-      ck(rc, "tsm_scan");
-      aev.resize((size_t)r.n_aev); hev.resize((size_t)r.n_hev);
+      scan_events(ctx, c, B.bytes, r, TSM_SCAN_ASSERT_EVENTS | TSM_SCAN_HEADER_EVENTS | (rev_b ? TSM_SCAN_REV_B : 0u), st, aev, hev);
       void* dptr = nullptr; int64_t n64 = 0;
       ck(tsm_device_counts(ctx, &dptr, &n64), "tsm_device_counts");
       h.resize((size_t)n64);
@@ -813,21 +851,14 @@ static int cmd_body(const std::vector<std::string>& roots, const std::string& ou
   int64_t index = 0, cases = 0, file_id = 0, n_stmt = 0;
   size_t first = 0;
   while (first < files.size()) {
-    Batch B;
-    int64_t cur = 0;
-    while (first < files.size() && (B.count() == 0 || (cur + files[first].size < (1ll << 29) && B.count() < (1u << 19)))) {
-      cur += (files[first].size + 127) / 128 * 128; B.idx.push_back((uint32_t)first); ++first;
-    }
-    load_batch(files, B);
+    Batch B = next_batch(files, first);
     tsm_ctx* ctx = nullptr;
     ck(tsm_create(&ctx, 0, B.bytes + 4096, (int32_t)B.count(), (int32_t)std::max<size_t>(roots.size(), 1), 0), "tsm_create");
     tsm_corpus c{B.arena, B.off.data(), B.len.data(), B.ext.data(), B.grp.data(), (int32_t)B.count(), (int32_t)std::max<size_t>(roots.size(), 1)};
-    const int64_t cap = std::max<int64_t>(B.bytes / 8 + 1024, 1024);
-    std::vector<tsm_header_event> hev((size_t)cap);
+    std::vector<tsm_assert_event> aev;
+    std::vector<tsm_header_event> hev;
     tsm_result r{};
-    r.hev = hev.data(); r.hev_cap = cap;
-    ck(tsm_scan(ctx, &c, &r, TSM_SCAN_HEADER_EVENTS, nullptr), "tsm_scan");
-    hev.resize((size_t)r.n_hev);
+    scan_events(ctx, c, B.bytes, r, TSM_SCAN_HEADER_EVENTS, nullptr, aev, hev);
     std::vector<int64_t> base(B.count() + 1);
     int64_t nl = 0;
     int rc = tsm_statements(ctx, &c, base.data(), nullptr, nullptr, 0, &nl, nullptr);
@@ -885,36 +916,26 @@ static std::vector<SnapFile> scan_snapshot(const std::vector<FileEntry>& files) 
   std::vector<SnapFile> out;
   size_t first = 0;
   while (first < files.size()) {
-    Batch B;
-    int64_t cur = 0;
-    while (first < files.size() && (B.count() == 0 || (cur + files[first].size < (1ll << 29) && B.count() < (1u << 19)))) {
-      cur += (files[first].size + 127) / 128 * 128; B.idx.push_back((uint32_t)first); ++first;
-    }
-    load_batch(files, B);
+    Batch B = next_batch(files, first);
     tsm_ctx* ctx = nullptr;
     ck(tsm_create(&ctx, 0, B.bytes + 4096, (int32_t)B.count(), 1, 0), "tsm_create");
     tsm_corpus c{B.arena, B.off.data(), B.len.data(), B.ext.data(), B.grp.data(), (int32_t)B.count(), 1};
-    const int64_t cap = std::max<int64_t>(B.bytes / 8 + 1024, 1024);
     std::vector<tsm_file_stat> stats(B.count());
-    std::vector<tsm_assert_event> aev((size_t)cap);
+    std::vector<tsm_assert_event> aev;
+    std::vector<tsm_header_event> hev;
     tsm_result r{};
-    r.stats = stats.data(); r.aev = aev.data(); r.aev_cap = cap;
-    ck(tsm_scan(ctx, &c, &r, TSM_SCAN_ASSERT_EVENTS, nullptr), "tsm_scan");
+    r.stats = stats.data();
+    scan_events(ctx, c, B.bytes, r, TSM_SCAN_ASSERT_EVENTS, nullptr, aev, hev);
     tsm_destroy(ctx);
     size_t ai = 0;
     for (size_t i = 0; i < B.count(); ++i) {
-      const uint8_t* base = B.arena + B.off[i];
       std::map<std::string, int64_t> hist; std::vector<std::string> order;
-      for (; ai < (size_t)r.n_aev && aev[ai].file == i; ++ai) {
-        const tsm_assert_event& ev = aev[ai];
-        const std::string cat = ev.cat == 127 ? std::string((const char*)base + ev.ident_off, ev.ident_len) : std::string(tsm_category_name(ev.cat));
+      for (; ai < aev.size() && aev[ai].file == i; ++ai) {
+        const std::string cat = event_category(B.arena + B.off[i], aev[ai]);
         if (!hist.count(cat)) order.push_back(cat);
         hist[cat]++;
       }
-      std::stable_sort(order.begin(), order.end(), [&](const std::string& x, const std::string& y) { return hist[x] > hist[y]; });
-      std::string a;
-      for (const std::string& k : order) { if (!a.empty()) a += ", "; a += std::to_string(hist[k]) + ":" + k; }
-      out.push_back({files[B.idx[i]].rel, stats[i].digest, files[B.idx[i]].size, stats[i].n_assert, a});
+      out.push_back({files[B.idx[i]].rel, stats[i].digest, files[B.idx[i]].size, stats[i].n_assert, hist_cell(hist, order)});
     }
     tsm_host_free(B.arena);
   }
@@ -979,7 +1000,6 @@ static int cmd_releases(const std::vector<std::string>& specs_in, const std::str
     }
     const std::vector<SnapFile> snap = scan_snapshot(files);
     std::vector<char> id_taken(ids.size(), 0), f_done(snap.size(), 0);
-    auto base_of = [](const std::string& p) { const size_t s = p.rfind('/'); return s == std::string::npos ? p : p.substr(s + 1); };
     auto bind = [&](size_t fi, size_t id) {
       const SnapFile& f = snap[fi];
       ids[id].path[t] = f.rel; ids[id].cur = f.rel; ids[id].digest = f.digest; ids[id].size = f.size;
@@ -997,7 +1017,7 @@ static int cmd_releases(const std::vector<std::string>& specs_in, const std::str
       if (f_done[fi]) continue;
       int hit = -1, n = 0;
       for (size_t id = 0; id < id_taken.size(); ++id)
-        if (!id_taken[id] && base_of(ids[id].cur) == base_of(snap[fi].rel)) { hit = (int)id; ++n; }
+        if (!id_taken[id] && base_name(ids[id].cur) == base_name(snap[fi].rel)) { hit = (int)id; ++n; }
       if (n == 1) bind(fi, (size_t)hit);
     }
     for (size_t fi = 0; fi < snap.size(); ++fi)                       // new identities, in walk order
@@ -1032,8 +1052,6 @@ static int cmd_releases(const std::vector<std::string>& specs_in, const std::str
 struct RenameFile { std::string path; std::vector<uint8_t> bytes; };
 struct RenamePair { size_t del, add; int similarity; bool exact; };
 struct RenameGroup { std::vector<RenameFile> del, add; std::vector<RenamePair> pairs; };
-
-static std::string base_name(const std::string& p) { const size_t s = p.rfind('/'); return s == std::string::npos ? p : p.substr(s + 1); }
 
 static void find_renames(tsm_ctx* ctx, std::vector<RenameGroup>& groups, int min_pct) {
   const int64_t kMax = 60000, min_score = 600ll * min_pct, base_score = min_score + (kMax - min_score) / 2;
@@ -1085,22 +1103,17 @@ static void find_renames(tsm_ctx* ctx, std::vector<RenameGroup>& groups, int min
       if (n.second) sn.push_back(&groups[c.g].add[c.a].bytes);
       co.push_back(o.first->second); cn.push_back(n.first->second);
     }
-    struct Packed { std::vector<int32_t> off, len; std::vector<uint8_t> arena, ext; };
-    auto pack = [](const std::vector<const std::vector<uint8_t>*>& files, Packed& P) {
-      const size_t n = files.size();
-      P.len.resize(n); P.off.resize(n + 1); P.ext.assign(n, 0);
-      for (size_t i = 0; i < n; ++i) P.len[i] = (int32_t)files[i]->size();
-      const int64_t bytes = tsm_layout(P.len.data(), (int32_t)n, P.off.data());
-      if (bytes < 0) die("rename candidates do not fit one int32-indexed arena");
-      P.arena.assign((size_t)std::max<int64_t>(bytes, 128), 0);
-      for (size_t i = 0; i < n; ++i) if (P.len[i]) memcpy(P.arena.data() + P.off[i], files[i]->data(), files[i]->size());
-    };
-    Packed PO, PN;
-    pack(so, PO); pack(sn, PN);
-    tsm_corpus ko{PO.arena.data(), PO.off.data(), PO.len.data(), PO.ext.data(), nullptr, (int32_t)so.size(), 1};
-    tsm_corpus kn{PN.arena.data(), PN.off.data(), PN.len.data(), PN.ext.data(), nullptr, (int32_t)sn.size(), 1};
+    Batch PO, PN;
+    for (const std::vector<uint8_t>* f : so) PO.len.push_back((int32_t)f->size());
+    for (const std::vector<uint8_t>* f : sn) PN.len.push_back((int32_t)f->size());
+    alloc_arena(PO); alloc_arena(PN);
+    for (size_t i = 0; i < so.size(); ++i) if (PO.len[i]) memcpy(PO.arena + PO.off[i], so[i]->data(), so[i]->size());
+    for (size_t i = 0; i < sn.size(); ++i) if (PN.len[i]) memcpy(PN.arena + PN.off[i], sn[i]->data(), sn[i]->size());
+    tsm_corpus ko{PO.arena, PO.off.data(), PO.len.data(), PO.ext.data(), nullptr, (int32_t)so.size(), 1};
+    tsm_corpus kn{PN.arena, PN.off.data(), PN.len.data(), PN.ext.data(), nullptr, (int32_t)sn.size(), 1};
     std::vector<int64_t> common(cands.size());
     ck(tsm_similarity(ctx, &ko, &kn, co.data(), cn.data(), (int64_t)cands.size(), common.data(), nullptr), "tsm_similarity");
+    tsm_host_free(PO.arena); tsm_host_free(PN.arena);
     for (size_t k = 0; k < cands.size(); ++k) {
       const Cand& c = cands[k];
       std::vector<int64_t>& row = score[{c.g, c.d}];
@@ -1203,140 +1216,222 @@ static void churn_rows(std::ostream& os, const std::vector<std::string>& lead, c
     }
 }
 
+// One changed file of a revision pair.  `step` is its commit (history) or 0 (diff); `o` and `n` name the bytes of the old and
+// the new side for the caller's loader, -1 where that side does not exist.  A rename (--find-renames) moves the deleted file's
+// `o` onto the added file and keeps the deleted file's path and the score in %.
+struct Change { size_t step; std::string path; int64_t o, n; std::string old_path; int similarity; };
+using Loader = std::function<std::vector<uint8_t>(int64_t)>;
+
+// Per step: lines added and removed, files diffed.  Over all steps: binary files skipped, files diffed, renames.
+struct ChangeTotals {
+  std::vector<int64_t> added, removed, files;
+  int64_t binaries = 0, diffed = 0, renames = 0, renames_exact = 0;
+  explicit ChangeTotals(size_t n_steps) : added(n_steps, 0), removed(n_steps, 0), files(n_steps, 0) {}
+};
+
+// Like git's numstat, no line counts for a binary file: one with a NUL byte in its first 8000.
+static bool binary(const std::vector<uint8_t>& v) { return !v.empty() && memchr(v.data(), 0, std::min<size_t>(v.size(), 8000)) != nullptr; }
+
+static const int64_t kBatch = 512ll << 20;                  // bytes per side of one tsm_similarity or diff call
+
+// --find-renames: the deleted and the added files of a step (binary ones left out) form a group; groups are paired together
+// until a side holds kBatch bytes, then every pair's two changes become one (old side of the deleted file, new side of the
+// added one) at the added file's place.
+static void pair_renames(tsm_ctx* ctx, std::vector<Change>& changes, const Loader& load, int pct, ChangeTotals& t) {
+  struct Move { size_t del, add; int similarity; };
+  std::vector<Move> moves;
+  std::vector<RenameGroup> groups;
+  std::vector<std::vector<size_t>> at_del, at_add;        // change of each file of each group
+  int64_t bytes_d = 0, bytes_a = 0;
+  auto flush = [&]() {
+    find_renames(ctx, groups, pct);
+    for (size_t g = 0; g < groups.size(); ++g)
+      for (const RenamePair& rp : groups[g].pairs) {
+        moves.push_back({at_del[g][rp.del], at_add[g][rp.add], rp.similarity});
+        t.renames_exact += rp.exact;
+      }
+    groups.clear(); at_del.clear(); at_add.clear();
+    bytes_d = bytes_a = 0;
+  };
+  for (size_t c0 = 0, c1 = 0; c0 < changes.size(); c0 = c1) {
+    std::vector<size_t> del, add;
+    for (c1 = c0; c1 < changes.size() && changes[c1].step == changes[c0].step; ++c1) {
+      if (changes[c1].o >= 0 && changes[c1].n < 0) del.push_back(c1);
+      if (changes[c1].o < 0 && changes[c1].n >= 0) add.push_back(c1);
+    }
+    if (del.empty() || add.empty()) continue;
+    RenameGroup G;
+    std::vector<size_t> gd, ga;
+    for (size_t c : del) {
+      std::vector<uint8_t> x = load(changes[c].o);
+      if (!binary(x)) { bytes_d += (int64_t)x.size() + 256; G.del.push_back({changes[c].path, std::move(x)}); gd.push_back(c); }
+    }
+    for (size_t c : add) {
+      std::vector<uint8_t> x = load(changes[c].n);
+      if (!binary(x)) { bytes_a += (int64_t)x.size() + 256; G.add.push_back({changes[c].path, std::move(x)}); ga.push_back(c); }
+    }
+    if (G.del.empty() || G.add.empty()) continue;
+    groups.push_back(std::move(G)); at_del.push_back(gd); at_add.push_back(ga);
+    if (bytes_d >= kBatch || bytes_a >= kBatch) flush();
+  }
+  if (!groups.empty()) flush();
+  std::vector<char> drop(changes.size(), 0);
+  for (const Move& m : moves) {
+    Change& a = changes[m.add];
+    a.o = changes[m.del].o; a.old_path = changes[m.del].path; a.similarity = m.similarity;
+    drop[m.del] = 1;
+  }
+  t.renames = (int64_t)moves.size();
+  std::vector<Change> kept;
+  for (size_t c = 0; c < changes.size(); ++c) if (!drop[c]) kept.push_back(std::move(changes[c]));
+  changes.swap(kept);
+}
+
+// The diff of an ordered list of changes of `n_steps` steps, after --find-renames pairing when rename_pct >= 0: binary files
+// skipped, batches of at most kBatch bytes per side (and 65 535 steps, a step being one group of the assertion tables),
+// one tsm_diff_pairs_detail or diff_asserts call per batch.  Every row starts with the `lead(step)` cells named `lead_head`;
+// the --assert-churn rows with the first `churn_lead` of them.  --out has a row for every diffed change when `zero_rows`,
+// else only for those that change a line or pair a rename.
+static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, const Loader& load, int rename_pct, bool zero_rows,
+                                 const std::vector<std::string>& lead_head, size_t churn_lead,
+                                 const std::function<std::vector<std::string>(size_t)>& lead, const std::string& out_path,
+                                 const std::string& asserts_path, const std::string& churn_path) {
+  ChangeTotals t(n_steps);
+  tsm_ctx* ctx = nullptr;
+  ck(tsm_create(&ctx, 0, 1 << 20, 16, 1, 0), "tsm_create");
+  if (rename_pct >= 0) pair_renames(ctx, changes, load, rename_pct, t);
+  std::ofstream os, as;
+  if (!out_path.empty()) {
+    os.open(out_path, std::ios::binary);
+    std::vector<std::string> head = lead_head;
+    head.insert(head.end(), {"fileName", "cloc", "added", "removed", "hunks_add", "hunks_del", "hunks_mod", "added_assert", "removed_assert"});
+    if (rename_pct >= 0) head.insert(head.end(), {"oldFileName", "similarity"});
+    csv_row(os, head);
+  }
+  if (!asserts_path.empty()) {
+    as.open(asserts_path, std::ios::binary);
+    std::vector<std::string> head = lead_head;
+    head.insert(head.end(), {"fileName", "change", "line", "statement", "category"});
+    csv_row(as, head);
+  }
+  const bool want_asserts = !asserts_path.empty() || !churn_path.empty();
+  std::map<size_t, std::vector<int64_t>> churn;            // per step with changed assertion lines: its [K] added and removed rows
+  for (size_t r0 = 0, r1 = 0; r0 < changes.size(); r0 = r1) {
+    // load both sides until a side of the batch is full
+    std::vector<std::vector<uint8_t>> blobs[2];            // old, new
+    std::vector<size_t> idx;
+    int64_t so = 0, sn = 0;
+    size_t steps = 0;
+    for (r1 = r0; r1 < changes.size() && so < kBatch && sn < kBatch; ++r1) {
+      const Change& c = changes[r1];
+      if (want_asserts && (r1 == r0 || c.step != changes[r1 - 1].step) && ++steps > 65535) break;
+      std::vector<uint8_t> x = c.o >= 0 ? load(c.o) : std::vector<uint8_t>(), y = c.n >= 0 ? load(c.n) : std::vector<uint8_t>();
+      if (binary(x) || binary(y)) { ++t.binaries; continue; }
+      if (x.size() > 0x7fff0000u || y.size() > 0x7fff0000u) die("blob too large: " + c.path);
+      so += (int64_t)x.size() + 256; sn += (int64_t)y.size() + 256;
+      blobs[0].push_back(std::move(x)); blobs[1].push_back(std::move(y)); idx.push_back(r1);
+    }
+    const size_t n = idx.size();
+    if (!n) continue;
+    Batch S[2];
+    for (int s = 0; s < 2; ++s) {
+      for (const std::vector<uint8_t>& v : blobs[s]) S[s].len.push_back((int32_t)v.size());
+      alloc_arena(S[s]);
+      for (size_t i = 0; i < n; ++i) if (S[s].len[i]) memcpy(S[s].arena + S[s].off[i], blobs[s][i].data(), blobs[s][i].size());
+    }
+    Batch &A = S[0], &N = S[1];
+    // ext tags of both sides feed the assertion-line classification of the changed lines
+    std::vector<size_t> group_step;                        // group g of the batch = step group_step[g]
+    for (size_t i = 0; i < n; ++i) {
+      const Change& c = changes[idx[i]];
+      N.ext[i] = (uint8_t)ext_tag(c.path);
+      A.ext[i] = c.old_path.empty() ? N.ext[i] : (uint8_t)ext_tag(c.old_path);
+      if (!want_asserts) continue;
+      if (group_step.empty() || group_step.back() != c.step) group_step.push_back(c.step);
+      A.grp[i] = N.grp[i] = (uint16_t)(group_step.size() - 1);
+    }
+    const int32_t n_groups = want_asserts ? (int32_t)group_step.size() : 1;
+    tsm_corpus ca{A.arena, A.off.data(), A.len.data(), A.ext.data(), A.grp.data(), (int32_t)n, n_groups};
+    tsm_corpus cn{N.arena, N.off.data(), N.len.data(), N.ext.data(), N.grp.data(), (int32_t)n, n_groups};
+    std::vector<int64_t> added(n), removed(n);
+    std::vector<tsm_diff_detail> det(n);
+    ChangedAsserts chg;
+    if (!want_asserts) {
+      ck(tsm_diff_pairs_detail(ctx, &ca, &cn, added.data(), removed.data(), det.data(), nullptr), "tsm_diff_pairs_detail");
+    } else {
+      diff_asserts(ctx, ca, cn, added.data(), removed.data(), det.data(), chg);
+      for (size_t g = 0; g < group_step.size(); ++g) {     // a step's files may span two batches
+        const int64_t* ad = chg.added_counts.data() + g * TSM_NUM_CATEGORIES;
+        const int64_t* rm = chg.removed_counts.data() + g * TSM_NUM_CATEGORIES;
+        if (std::all_of(ad, ad + TSM_NUM_CATEGORIES, [](int64_t v) { return v == 0; }) &&
+            std::all_of(rm, rm + TSM_NUM_CATEGORIES, [](int64_t v) { return v == 0; })) continue;
+        std::vector<int64_t>& tab = churn[group_step[g]];
+        tab.resize(2 * TSM_NUM_CATEGORIES, 0);
+        for (int k = 0; k < TSM_NUM_CATEGORIES; ++k) { tab[(size_t)k] += ad[k]; tab[(size_t)(TSM_NUM_CATEGORIES + k)] += rm[k]; }
+      }
+      size_t ka = 0, kr = 0;
+      for (size_t i = 0; as.is_open() && i < n; ++i) {
+        const Change& c = changes[idx[i]];
+        const std::vector<std::string> l = lead(c.step);
+        assert_rows(as, l, c.old_path.empty() ? c.path : c.old_path, A.arena + A.off[i], A.len[i], chg.rev, kr, (uint32_t)i, "-");
+        assert_rows(as, l, c.path, N.arena + N.off[i], N.len[i], chg.aev, ka, (uint32_t)i, "+");
+      }
+    }
+    for (size_t i = 0; i < n; ++i) {
+      const Change& c = changes[idx[i]];
+      t.added[c.step] += added[i]; t.removed[c.step] += removed[i]; t.files[c.step]++;
+      if (!os.is_open() || !(zero_rows || added[i] || removed[i] || c.similarity >= 0)) continue;
+      std::vector<std::string> row = lead(c.step);
+      row.insert(row.end(), {c.path, std::to_string(added[i] + removed[i]), std::to_string(added[i]), std::to_string(removed[i]),
+                             std::to_string(det[i].hunks_add), std::to_string(det[i].hunks_del), std::to_string(det[i].hunks_mod),
+                             std::to_string(det[i].added_assert), std::to_string(det[i].removed_assert)});
+      if (rename_pct >= 0) row.insert(row.end(), {c.old_path, c.similarity >= 0 ? std::to_string(c.similarity) : ""});
+      csv_row(os, row);
+    }
+    t.diffed += (int64_t)n;
+    tsm_host_free(A.arena); tsm_host_free(N.arena);
+  }
+  tsm_destroy(ctx);
+  if (!churn_path.empty()) {
+    std::ofstream cs(churn_path, std::ios::binary);
+    std::vector<std::string> head(lead_head.begin(), lead_head.begin() + (long)churn_lead);
+    head.insert(head.end(), {"category", "added", "removed"});
+    csv_row(cs, head);
+    for (const auto& kv : churn) {
+      std::vector<std::string> l = lead(kv.first);
+      l.resize(churn_lead);
+      churn_rows(cs, l, kv.second.data(), kv.second.data() + TSM_NUM_CATEGORIES);
+    }
+  }
+  return t;
+}
+
 static int cmd_diff(const std::string& old_root, const std::string& new_root, const std::string& out_path,
                     const std::string& asserts_path, const std::string& churn_path, int rename_pct) {
   std::vector<FileEntry> a, b;
   walk(old_root, 0, true, a);
   walk(new_root, 0, true, b);
-  std::map<std::string, const FileEntry*> bm;
-  for (const FileEntry& f : b) bm[f.rel] = &f;
-  // pairs by relative path; a file present on one side only is paired with the empty file
-  struct Pair { std::string rel; const FileEntry* o; const FileEntry* n; std::string old_rel; int similarity; };   // (renames: old path, %)
-  std::vector<Pair> pairs;
-  std::map<std::string, bool> seen;
-  for (const FileEntry& f : a) { auto it = bm.find(f.rel); pairs.push_back({f.rel, &f, it == bm.end() ? nullptr : it->second, "", -1}); seen[f.rel] = true; }
-  for (const FileEntry& f : b) if (!seen.count(f.rel)) pairs.push_back({f.rel, nullptr, &f, "", -1});
-  // git's numstat reports no line counts for binary files: a pair is skipped when either side has a NUL byte in its first 8000
-  {
-    auto binary = [](const FileEntry* f) {
-      if (!f || f->abs.empty() || f->size == 0) return false;
-      char buf[8000];
-      const int fd = open(f->abs.c_str(), O_RDONLY);
-      if (fd < 0) return false;
-      const ssize_t r = read(fd, buf, sizeof buf);
-      close(fd);
-      return r > 0 && memchr(buf, 0, (size_t)r) != nullptr;
-    };
-    std::vector<Pair> text;
-    size_t skipped = 0;
-    for (const Pair& p : pairs) { if (binary(p.o) || binary(p.n)) ++skipped; else text.push_back(p); }
-    if (skipped) fprintf(stderr, "tosem-scan: %zu binary file(s) skipped\n", skipped);
-    pairs.swap(text);
-  }
-  auto read_file = [](const FileEntry* f, uint8_t* dst) {
-    const int fd = open(f->abs.c_str(), O_RDONLY);
-    int64_t got = 0;
-    while (fd >= 0 && got < f->size) {
-      const ssize_t r = read(fd, dst + got, (size_t)(f->size - got));
-      if (r <= 0) break;
-      got += r;
-    }
-    if (fd >= 0) close(fd);
-    if (got != f->size) die("short read: " + f->abs);
+  // pairs by relative path; a file present on one side only is paired with the empty file.  The loader's names: the
+  // files of `a`, then those of `b`.
+  std::map<std::string, int64_t> in_a, in_b;
+  for (size_t i = 0; i < a.size(); ++i) in_a[a[i].rel] = (int64_t)i;
+  for (size_t j = 0; j < b.size(); ++j) in_b[b[j].rel] = (int64_t)(a.size() + j);
+  std::vector<Change> changes;
+  for (const FileEntry& f : a) { auto it = in_b.find(f.rel); changes.push_back({0, f.rel, in_a[f.rel], it == in_b.end() ? -1 : it->second, "", -1}); }
+  for (const FileEntry& f : b) if (!in_a.count(f.rel)) changes.push_back({0, f.rel, -1, in_b[f.rel], "", -1});
+  auto load = [&](int64_t s) {
+    const FileEntry& f = s < (int64_t)a.size() ? a[(size_t)s] : b[(size_t)s - a.size()];
+    std::vector<uint8_t> v((size_t)f.size);
+    if (!read_file(f.abs, v.data(), f.size)) die("short read: " + f.abs);
+    return v;
   };
-  tsm_ctx* ctx = nullptr;
-  ck(tsm_create(&ctx, 0, 1 << 20, 16, 1, 0), "tsm_create");
-  if (rename_pct >= 0) {                                   // a deleted and an added file that pair become one pair (old, new)
-    RenameGroup G;
-    std::vector<size_t> di, ai;
-    for (size_t i = 0; i < pairs.size(); ++i) {
-      const FileEntry* f = pairs[i].o ? pairs[i].o : pairs[i].n;
-      if (pairs[i].o && pairs[i].n) continue;
-      RenameFile r{pairs[i].rel, std::vector<uint8_t>((size_t)f->size)};
-      if (f->size) read_file(f, r.bytes.data());
-      if (pairs[i].o) { G.del.push_back(std::move(r)); di.push_back(i); } else { G.add.push_back(std::move(r)); ai.push_back(i); }
-    }
-    std::vector<RenameGroup> groups(1);
-    groups[0] = std::move(G);
-    find_renames(ctx, groups, rename_pct);
-    std::vector<char> drop(pairs.size(), 0);
-    size_t exact = 0;
-    for (const RenamePair& rp : groups[0].pairs) {
-      Pair& p = pairs[ai[rp.add]];
-      p.o = pairs[di[rp.del]].o; p.old_rel = pairs[di[rp.del]].rel; p.similarity = rp.similarity;
-      drop[di[rp.del]] = 1;
-      exact += rp.exact;
-    }
-    std::vector<Pair> kept;
-    for (size_t i = 0; i < pairs.size(); ++i) if (!drop[i]) kept.push_back(pairs[i]);
-    pairs.swap(kept);
-    fprintf(stderr, "tosem-scan: %zu rename(s) found (%zu exact, %zu inexact)\n", groups[0].pairs.size(), exact, groups[0].pairs.size() - exact);
-  }
-  auto pack = [&](bool old_side, Batch& B, std::vector<FileEntry>& tmp) {
-    for (const Pair& p : pairs) { const FileEntry* f = old_side ? p.o : p.n; tmp.push_back(f ? *f : FileEntry{p.rel, "", 0, 0, 0, nullptr}); }
-    const size_t n = tmp.size();
-    B.idx.resize(n);
-    for (size_t i = 0; i < n; ++i) B.idx[i] = (uint32_t)i;
-    B.len.resize(n); B.off.resize(n + 1); B.ext.assign(n, 0); B.grp.assign(n, 0);
-    for (size_t i = 0; i < n; ++i) B.len[i] = (int32_t)tmp[i].size;
-    B.bytes = tsm_layout(B.len.data(), (int32_t)n, B.off.data());
-    if (B.bytes < 0) die("tree does not fit one int32-indexed arena; diff it per sub-directory");
-    B.arena = (uint8_t*)tsm_host_alloc(std::max<int64_t>(B.bytes, 128));
-    if (!B.arena) die("pinned arena allocation failed");
-    memset(B.arena, 0, (size_t)std::max<int64_t>(B.bytes, 128));
-    for (size_t i = 0; i < n; ++i)
-      if (!tmp[i].abs.empty() && B.len[i] != 0) read_file(&tmp[i], B.arena + B.off[i]);
-  };
-  Batch A, N; std::vector<FileEntry> ta, tn;
-  pack(true, A, ta); pack(false, N, tn);
-  tsm_corpus ca{A.arena, A.off.data(), A.len.data(), A.ext.data(), A.grp.data(), (int32_t)A.count(), 1};
-  tsm_corpus cn{N.arena, N.off.data(), N.len.data(), N.ext.data(), N.grp.data(), (int32_t)N.count(), 1};
-  // ext tags of both sides feed the assertion-line classification of the changed lines
-  for (size_t i = 0; i < pairs.size(); ++i) {
-    N.ext[i] = (uint8_t)ext_tag(pairs[i].rel);
-    A.ext[i] = pairs[i].old_rel.empty() ? N.ext[i] : (uint8_t)ext_tag(pairs[i].old_rel);
-  }
-  std::vector<int64_t> added(pairs.size()), removed(pairs.size());
-  std::vector<tsm_diff_detail> det(pairs.size());
-  ChangedAsserts ch;
-  if (asserts_path.empty() && churn_path.empty())
-    ck(tsm_diff_pairs_detail(ctx, &ca, &cn, added.data(), removed.data(), det.data(), nullptr), "tsm_diff_pairs_detail");
-  else diff_asserts(ctx, ca, cn, added.data(), removed.data(), det.data(), ch);
-  tsm_destroy(ctx);
-  if (!asserts_path.empty()) {
-    std::ofstream as(asserts_path, std::ios::binary);
-    csv_row(as, {"fileName", "change", "line", "statement", "category"});
-    size_t ka = 0, kr = 0;
-    for (size_t i = 0; i < pairs.size(); ++i) {
-      assert_rows(as, {}, pairs[i].old_rel.empty() ? pairs[i].rel : pairs[i].old_rel, A.arena + A.off[i], A.len[i], ch.rev, kr, (uint32_t)i, "-");
-      assert_rows(as, {}, pairs[i].rel, N.arena + N.off[i], N.len[i], ch.aev, ka, (uint32_t)i, "+");
-    }
-  }
-  if (!churn_path.empty()) {
-    std::ofstream cs(churn_path, std::ios::binary);
-    csv_row(cs, {"category", "added", "removed"});
-    churn_rows(cs, {}, ch.added_counts.data(), ch.removed_counts.data());
-  }
-  std::ofstream os;
-  if (!out_path.empty()) {
-    os.open(out_path, std::ios::binary);
-    std::vector<std::string> head{"fileName", "cloc", "added", "removed", "hunks_add", "hunks_del", "hunks_mod", "added_assert", "removed_assert"};
-    if (rename_pct >= 0) head.insert(head.end(), {"oldFileName", "similarity"});
-    csv_row(os, head);
-  }
-  int64_t ta_ = 0, tr_ = 0;
-  for (size_t i = 0; i < pairs.size(); ++i) {
-    ta_ += added[i]; tr_ += removed[i];
-    if (os.is_open() && (added[i] || removed[i] || pairs[i].similarity >= 0)) {
-      std::vector<std::string> row{pairs[i].rel, std::to_string(added[i] + removed[i]), std::to_string(added[i]), std::to_string(removed[i]),
-                                   std::to_string(det[i].hunks_add), std::to_string(det[i].hunks_del), std::to_string(det[i].hunks_mod),
-                                   std::to_string(det[i].added_assert), std::to_string(det[i].removed_assert)};
-      if (rename_pct >= 0) row.insert(row.end(), {pairs[i].old_rel, pairs[i].similarity >= 0 ? std::to_string(pairs[i].similarity) : ""});
-      csv_row(os, row);
-    }
-  }
-  printf("cloc,added,removed\r\n%lld,%lld,%lld\r\n", (long long)(ta_ + tr_), (long long)ta_, (long long)tr_);
-  tsm_host_free(A.arena); tsm_host_free(N.arena);
+  const ChangeTotals t = diff_changes(changes, 1, load, rename_pct, false, {}, 0, [](size_t) { return std::vector<std::string>(); },
+                                      out_path, asserts_path, churn_path);
+  if (t.binaries) fprintf(stderr, "tosem-scan: %lld binary file(s) skipped\n", (long long)t.binaries);
+  if (rename_pct >= 0)
+    fprintf(stderr, "tosem-scan: %lld rename(s) found (%lld exact, %lld inexact)\n", (long long)t.renames, (long long)t.renames_exact,
+            (long long)(t.renames - t.renames_exact));
+  printf("cloc,added,removed\r\n%lld,%lld,%lld\r\n", (long long)(t.added[0] + t.removed[0]), (long long)t.added[0], (long long)t.removed[0]);
   return 0;
 }
 
@@ -1344,15 +1439,11 @@ static int cmd_diff(const std::string& old_root, const std::string& new_root, co
 // `tosem-scan history <repo>`: the churn of the test files along the first-parent history of a revision, read straight
 // from the git object store (host/git_store.hpp: loose objects, packfiles, refs - no `git` process, no checkout).
 // Host: commit chain, tree diff by object name (only entries whose blob changed are opened), blob inflation into the
-// two pinned arenas.  GPU: line records of both sides + per-pair Myers + hunks + changed assertion lines
-// (tsm_diff_pairs_detail), one call per batch of at most ~512 MiB per side.  Rows: one per (commit, changed file).
-struct BlobChange {
-  std::string path; gitstore::Oid o, n; bool has_o, has_n;
-  std::string old_path; int similarity = -1;               // a rename (--find-renames): the deleted file's path and the score in %
-};
+// two pinned arenas.  GPU: diff_changes.  Rows: one per (commit, changed file).
 
-static void tree_diff(gitstore::Store& gs, const gitstore::Oid* a, const gitstore::Oid* b, const std::string& prefix,
-                      bool all_files, std::vector<BlobChange>& out) {
+// The changed blobs under two trees, as changes of `step`; their object names are appended to `objs` (the loader's names).
+static void tree_diff(gitstore::Store& gs, const gitstore::Oid* a, const gitstore::Oid* b, const std::string& prefix, bool all_files,
+                      size_t step, std::vector<gitstore::Oid>& objs, std::vector<Change>& out) {
   std::vector<gitstore::TreeEntry> ea, eb;
   if (a && !gs.tree(*a, ea)) die("unreadable tree " + a->hex());
   if (b && !gs.tree(*b, eb)) die("unreadable tree " + b->hex());
@@ -1369,13 +1460,13 @@ static void tree_diff(gitstore::Store& gs, const gitstore::Oid* a, const gitstor
     if (x && y && x->oid == y->oid && x->is_tree() == y->is_tree()) continue;     // same object: nothing below it changed
     const std::string path = prefix + nm;
     const bool xt = x && x->is_tree(), yt = y && y->is_tree();
-    if (xt || yt) tree_diff(gs, xt ? &x->oid : nullptr, yt ? &y->oid : nullptr, path + "/", all_files, out);
+    if (xt || yt) tree_diff(gs, xt ? &x->oid : nullptr, yt ? &y->oid : nullptr, path + "/", all_files, step, objs, out);
     const bool xb = x && x->is_blob(), yb = y && y->is_blob();                     // (symlinks and submodules are not files of the study)
     if (!xb && !yb) continue;
     if (!all_files && (lower(path).find("test") == std::string::npos || ext_tag(path) == TSM_EXT_OTHER)) continue;   // S0, S1
-    BlobChange c{path, {}, {}, xb, yb, "", -1};
-    if (xb) c.o = x->oid;
-    if (yb) c.n = y->oid;
+    Change c{step, path, -1, -1, "", -1};
+    if (xb) { c.o = (int64_t)objs.size(); objs.push_back(x->oid); }
+    if (yb) { c.n = (int64_t)objs.size(); objs.push_back(y->oid); }
     out.push_back(c);
   }
 }
@@ -1399,212 +1490,57 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
     id = st.c.parents[0];
   }
   std::reverse(chain.begin(), chain.end());                 // oldest first
-  struct Row { size_t step; BlobChange ch; };
-  std::vector<Row> rows;
+  std::vector<gitstore::Oid> objs;
+  std::vector<Change> changes;
   for (size_t i = 0; i < chain.size(); ++i) {
     gitstore::Commit parent;
     const bool has_parent = !chain[i].c.parents.empty();
     if (has_parent && !gs.commit(chain[i].c.parents[0], parent)) die("unreadable commit " + chain[i].c.parents[0].hex());
     if (has_parent && parent.tree == chain[i].c.tree) continue;
-    std::vector<BlobChange> ch;
-    tree_diff(gs, has_parent ? &parent.tree : nullptr, &chain[i].c.tree, "", all_files, ch);
-    for (auto& c : ch) rows.push_back({i, c});
+    tree_diff(gs, has_parent ? &parent.tree : nullptr, &chain[i].c.tree, "", all_files, i, objs, changes);
   }
-  tsm_ctx* ctx = nullptr;
-  if (!dry_run) ck(tsm_create(&ctx, 0, 1 << 20, 16, 1, 0), "tsm_create");
-  const int64_t kBatch = 512ll << 20;
-  int64_t renames = 0, renames_exact = 0;
-  if (rename_pct >= 0) {
-    // per commit, its deleted and added files (binary ones left out) form a group; groups are paired together until a side
-    // holds kBatch bytes, and a pair's two rows become one row (old blob, new blob) at the added file's place
-    std::vector<char> drop(rows.size(), 0);
-    std::vector<RenameGroup> groups;
-    std::vector<std::vector<size_t>> at_del, at_add;       // row of each file of each group
-    int64_t bytes_d = 0, bytes_a = 0;
-    auto flush = [&]() {
-      find_renames(ctx, groups, rename_pct);
-      for (size_t g = 0; g < groups.size(); ++g)
-        for (const RenamePair& rp : groups[g].pairs) {
-          const BlobChange& d = rows[at_del[g][rp.del]].ch;
-          BlobChange& a = rows[at_add[g][rp.add]].ch;
-          a.o = d.o; a.has_o = true; a.old_path = d.path; a.similarity = rp.similarity;
-          drop[at_del[g][rp.del]] = 1;
-          ++renames; renames_exact += rp.exact;
-        }
-      groups.clear(); at_del.clear(); at_add.clear();
-      bytes_d = bytes_a = 0;
-    };
-    for (size_t r0 = 0, r1 = 0; r0 < rows.size(); r0 = r1) {
-      for (r1 = r0; r1 < rows.size() && rows[r1].step == rows[r0].step; ++r1) {}
-      std::vector<size_t> del, add;
-      for (size_t r = r0; r < r1; ++r) {
-        if (rows[r].ch.has_o && !rows[r].ch.has_n) del.push_back(r);
-        if (!rows[r].ch.has_o && rows[r].ch.has_n) add.push_back(r);
-      }
-      if (del.empty() || add.empty()) continue;
-      RenameGroup G;
-      std::vector<size_t> gd, ga;
-      auto load = [&](const std::vector<size_t>& which, bool old_side, std::vector<RenameFile>& out, std::vector<size_t>& at) {
-        for (size_t r : which) {
-          const gitstore::Oid& id = old_side ? rows[r].ch.o : rows[r].ch.n;
-          gitstore::Object x;
-          if (!gs.read(id, x) || x.type != gitstore::OBJ_BLOB) die("unreadable blob " + id.hex());
-          if (!x.data.empty() && memchr(x.data.data(), 0, std::min<size_t>(x.data.size(), 8000)) != nullptr) continue;   // binary
-          out.push_back({rows[r].ch.path, std::move(x.data)});
-          at.push_back(r);
-        }
-      };
-      load(del, true, G.del, gd);
-      load(add, false, G.add, ga);
-      if (G.del.empty() || G.add.empty()) continue;
-      for (const RenameFile& f : G.del) bytes_d += (int64_t)f.bytes.size() + 256;
-      for (const RenameFile& f : G.add) bytes_a += (int64_t)f.bytes.size() + 256;
-      groups.push_back(std::move(G)); at_del.push_back(gd); at_add.push_back(ga);
-      if (bytes_d >= kBatch || bytes_a >= kBatch) flush();
+  auto load = [&](int64_t s) {
+    gitstore::Object x;
+    if (!gs.read(objs[(size_t)s], x) || x.type != gitstore::OBJ_BLOB) die("unreadable blob " + objs[(size_t)s].hex());
+    return std::move(x.data);
+  };
+  auto lead = [&](size_t step) {
+    const Step& st = chain[step];
+    return std::vector<std::string>{st.id.hex(), st.c.parents.empty() ? "" : st.c.parents[0].hex(), std::to_string(st.c.time)};
+  };
+  ChangeTotals t(chain.size());
+  if (dry_run) {
+    std::ofstream os;
+    if (!out_path.empty()) {
+      os.open(out_path, std::ios::binary);
+      csv_row(os, {"commit", "parent", "time", "fileName", "old_blob", "new_blob", "old_size", "new_size", "old_fnv", "new_fnv"});
     }
-    if (!groups.empty()) flush();
-    std::vector<Row> kept;
-    for (size_t r = 0; r < rows.size(); ++r) if (!drop[r]) kept.push_back(rows[r]);
-    rows.swap(kept);
-  }
-  std::ofstream os;
-  if (!out_path.empty()) {
-    os.open(out_path, std::ios::binary);
-    if (dry_run) csv_row(os, {"commit", "parent", "time", "fileName", "old_blob", "new_blob", "old_size", "new_size", "old_fnv", "new_fnv"});
-    else {
-      std::vector<std::string> head{"commit", "parent", "time", "fileName", "cloc", "added", "removed", "hunks_add", "hunks_del", "hunks_mod", "added_assert", "removed_assert"};
-      if (rename_pct >= 0) head.insert(head.end(), {"oldFileName", "similarity"});
-      csv_row(os, head);
+    auto fnv = [](const std::vector<uint8_t>& v) { uint64_t h = 0xcbf29ce484222325ull; for (uint8_t b : v) h = (h ^ b) * 0x100000001b3ull; char buf[24]; snprintf(buf, sizeof buf, "%016llx", (unsigned long long)h); return std::string(buf); };
+    for (const Change& c : changes) {
+      const std::vector<uint8_t> x = c.o >= 0 ? load(c.o) : std::vector<uint8_t>(), y = c.n >= 0 ? load(c.n) : std::vector<uint8_t>();
+      if (os.is_open()) {
+        std::vector<std::string> row = lead(c.step);
+        row.insert(row.end(), {c.path, c.o >= 0 ? objs[(size_t)c.o].hex() : "", c.n >= 0 ? objs[(size_t)c.n].hex() : "",
+                               std::to_string(x.size()), std::to_string(y.size()), fnv(x), fnv(y)});
+        csv_row(os, row);
+      }
+      t.files[c.step]++;
     }
-  }
-  const bool want_asserts = !dry_run && (!asserts_path.empty() || !churn_path.empty());
-  std::ofstream as;
-  if (!dry_run && !asserts_path.empty()) {
-    as.open(asserts_path, std::ios::binary);
-    csv_row(as, {"commit", "parent", "time", "fileName", "change", "line", "statement", "category"});
-  }
-  // per commit with changed assertion lines: its [K] added and removed rows (a commit's files may span two batches)
-  std::map<size_t, std::vector<int64_t>> churn;
-  std::vector<int64_t> per_add(chain.size(), 0), per_rem(chain.size(), 0), per_files(chain.size(), 0);
-  int64_t binaries = 0, pairs_done = 0;
-  size_t r0 = 0;
-  while (r0 < rows.size()) {
-    // inflate blobs until a side of the batch is full
-    std::vector<std::vector<uint8_t>> bo, bn;
-    std::vector<size_t> idx;
-    int64_t so = 0, sn = 0;
-    size_t r1 = r0, commits = 0;                           // with the assertion tables, a commit is a group: at most 65 535 per batch
-    for (; r1 < rows.size() && so < kBatch && sn < kBatch; ++r1) {
-      if (want_asserts && (r1 == r0 || rows[r1].step != rows[r1 - 1].step) && ++commits > 65535) break;
-      const BlobChange& c = rows[r1].ch;
-      gitstore::Object x, y;
-      if (c.has_o && (!gs.read(c.o, x) || x.type != gitstore::OBJ_BLOB)) die("unreadable blob " + c.o.hex());
-      if (c.has_n && (!gs.read(c.n, y) || y.type != gitstore::OBJ_BLOB)) die("unreadable blob " + c.n.hex());
-      auto binary = [](const std::vector<uint8_t>& v) { return !v.empty() && memchr(v.data(), 0, std::min<size_t>(v.size(), 8000)) != nullptr; };
-      if (dry_run) {
-        auto fnv = [](const std::vector<uint8_t>& v) { uint64_t h = 0xcbf29ce484222325ull; for (uint8_t b : v) h = (h ^ b) * 0x100000001b3ull; char buf[24]; snprintf(buf, sizeof buf, "%016llx", (unsigned long long)h); return std::string(buf); };
-        const Step& st = chain[rows[r1].step];
-        if (os.is_open())
-          csv_row(os, {st.id.hex(), st.c.parents.empty() ? "" : st.c.parents[0].hex(), std::to_string(st.c.time), c.path, c.has_o ? c.o.hex() : "", c.has_n ? c.n.hex() : "",
-                       std::to_string(x.data.size()), std::to_string(y.data.size()), fnv(x.data), fnv(y.data)});
-        per_files[rows[r1].step]++;
-        continue;
-      }
-      if (binary(x.data) || binary(y.data)) { ++binaries; continue; }              // like git's numstat: no line counts for binary files
-      if (x.data.size() > 0x7fff0000u || y.data.size() > 0x7fff0000u) die("blob too large: " + c.path);
-      so += (int64_t)x.data.size() + 256; sn += (int64_t)y.data.size() + 256;
-      bo.push_back(std::move(x.data)); bn.push_back(std::move(y.data)); idx.push_back(r1);
-    }
-    const size_t n = idx.size();
-    if (n) {
-      Batch A, N;
-      auto pack = [&](Batch& B, const std::vector<std::vector<uint8_t>>& blobs) {
-        B.len.resize(n); B.off.resize(n + 1); B.ext.assign(n, 0); B.grp.assign(n, 0);
-        for (size_t i = 0; i < n; ++i) B.len[i] = (int32_t)blobs[i].size();
-        B.bytes = tsm_layout(B.len.data(), (int32_t)n, B.off.data());
-        if (B.bytes < 0) die("batch does not fit one int32-indexed arena");
-        B.arena = (uint8_t*)tsm_host_alloc(std::max<int64_t>(B.bytes, 128));
-        if (!B.arena) die("pinned arena allocation failed");
-        memset(B.arena, 0, (size_t)std::max<int64_t>(B.bytes, 128));
-        for (size_t i = 0; i < n; ++i) if (B.len[i]) memcpy(B.arena + B.off[i], blobs[i].data(), blobs[i].size());
-      };
-      pack(A, bo); pack(N, bn);
-      for (size_t i = 0; i < n; ++i) {
-        const BlobChange& c = rows[idx[i]].ch;
-        N.ext[i] = (uint8_t)ext_tag(c.path);
-        A.ext[i] = c.old_path.empty() ? N.ext[i] : (uint8_t)ext_tag(c.old_path);
-      }
-      std::vector<size_t> group_step;                        // group g of the batch = commit group_step[g]
-      for (size_t i = 0; want_asserts && i < n; ++i) {
-        if (group_step.empty() || group_step.back() != rows[idx[i]].step) group_step.push_back(rows[idx[i]].step);
-        A.grp[i] = N.grp[i] = (uint16_t)(group_step.size() - 1);
-      }
-      const int32_t n_groups = want_asserts ? (int32_t)group_step.size() : 1;
-      tsm_corpus ca{A.arena, A.off.data(), A.len.data(), A.ext.data(), A.grp.data(), (int32_t)n, n_groups};
-      tsm_corpus cn{N.arena, N.off.data(), N.len.data(), N.ext.data(), N.grp.data(), (int32_t)n, n_groups};
-      std::vector<int64_t> added(n), removed(n);
-      std::vector<tsm_diff_detail> det(n);
-      ChangedAsserts chg;
-      if (!want_asserts) {
-        ck(tsm_diff_pairs_detail(ctx, &ca, &cn, added.data(), removed.data(), det.data(), nullptr), "tsm_diff_pairs_detail");
-      } else {
-        diff_asserts(ctx, ca, cn, added.data(), removed.data(), det.data(), chg);
-        for (size_t g = 0; g < group_step.size(); ++g) {
-          const int64_t* ad = chg.added_counts.data() + g * TSM_NUM_CATEGORIES;
-          const int64_t* rm = chg.removed_counts.data() + g * TSM_NUM_CATEGORIES;
-          if (std::all_of(ad, ad + TSM_NUM_CATEGORIES, [](int64_t v) { return v == 0; }) &&
-              std::all_of(rm, rm + TSM_NUM_CATEGORIES, [](int64_t v) { return v == 0; })) continue;
-          std::vector<int64_t>& t = churn[group_step[g]];
-          t.resize(2 * TSM_NUM_CATEGORIES, 0);
-          for (int k = 0; k < TSM_NUM_CATEGORIES; ++k) { t[(size_t)k] += ad[k]; t[(size_t)(TSM_NUM_CATEGORIES + k)] += rm[k]; }
-        }
-        if (as.is_open()) {
-          size_t ka = 0, kr = 0;
-          for (size_t i = 0; i < n; ++i) {
-            const Row& r = rows[idx[i]];
-            const Step& st = chain[r.step];
-            const std::vector<std::string> lead{st.id.hex(), st.c.parents.empty() ? "" : st.c.parents[0].hex(), std::to_string(st.c.time)};
-            assert_rows(as, lead, r.ch.old_path.empty() ? r.ch.path : r.ch.old_path, A.arena + A.off[i], A.len[i], chg.rev, kr, (uint32_t)i, "-");
-            assert_rows(as, lead, r.ch.path, N.arena + N.off[i], N.len[i], chg.aev, ka, (uint32_t)i, "+");
-          }
-        }
-      }
-      for (size_t i = 0; i < n; ++i) {
-        const Row& r = rows[idx[i]];
-        per_add[r.step] += added[i]; per_rem[r.step] += removed[i]; per_files[r.step]++;
-        if (os.is_open()) {
-          const Step& st = chain[r.step];
-          std::vector<std::string> row{st.id.hex(), st.c.parents.empty() ? "" : st.c.parents[0].hex(), std::to_string(st.c.time), r.ch.path,
-                                       std::to_string(added[i] + removed[i]), std::to_string(added[i]), std::to_string(removed[i]),
-                                       std::to_string(det[i].hunks_add), std::to_string(det[i].hunks_del), std::to_string(det[i].hunks_mod),
-                                       std::to_string(det[i].added_assert), std::to_string(det[i].removed_assert)};
-          if (rename_pct >= 0) row.insert(row.end(), {r.ch.old_path, r.ch.similarity >= 0 ? std::to_string(r.ch.similarity) : ""});
-          csv_row(os, row);
-        }
-      }
-      pairs_done += (int64_t)n;
-      tsm_host_free(A.arena); tsm_host_free(N.arena);
-    }
-    r0 = r1;
-  }
-  if (ctx) tsm_destroy(ctx);
-  if (want_asserts && !churn_path.empty()) {
-    std::ofstream cs(churn_path, std::ios::binary);
-    csv_row(cs, {"commit", "category", "added", "removed"});
-    for (const auto& kv : churn) churn_rows(cs, {chain[kv.first].id.hex()}, kv.second.data(), kv.second.data() + TSM_NUM_CATEGORIES);
+  } else {
+    t = diff_changes(changes, chain.size(), load, rename_pct, true, {"commit", "parent", "time"}, 1, lead, out_path, asserts_path, churn_path);
   }
   printf("commit,files,cloc,added,removed\r\n");
   int64_t ta = 0, tr = 0;
   for (size_t i = 0; i < chain.size(); ++i) {
-    ta += per_add[i]; tr += per_rem[i];
-    printf("%s,%lld,%lld,%lld,%lld\r\n", chain[i].id.hex().c_str(), (long long)per_files[i], (long long)(per_add[i] + per_rem[i]),
-           (long long)per_add[i], (long long)per_rem[i]);
+    ta += t.added[i]; tr += t.removed[i];
+    printf("%s,%lld,%lld,%lld,%lld\r\n", chain[i].id.hex().c_str(), (long long)t.files[i], (long long)(t.added[i] + t.removed[i]),
+           (long long)t.added[i], (long long)t.removed[i]);
   }
   fprintf(stderr, "tosem-scan: history of %s: %zu commits, %lld changed files diffed on the GPU, %lld binary skipped, cloc %lld (+%lld -%lld)\n",
-          rev.c_str(), chain.size(), (long long)pairs_done, (long long)binaries, (long long)(ta + tr), (long long)ta, (long long)tr);
+          rev.c_str(), chain.size(), (long long)t.diffed, (long long)t.binaries, (long long)(ta + tr), (long long)ta, (long long)tr);
   if (rename_pct >= 0)
-    fprintf(stderr, "tosem-scan: %lld rename(s) found at %d%% (%lld exact, %lld inexact)\n", (long long)renames, rename_pct,
-            (long long)renames_exact, (long long)(renames - renames_exact));
+    fprintf(stderr, "tosem-scan: %lld rename(s) found at %d%% (%lld exact, %lld inexact)\n", (long long)t.renames, rename_pct,
+            (long long)t.renames_exact, (long long)(t.renames - t.renames_exact));
   return 0;
 }
 
