@@ -8,10 +8,18 @@
  *
  * Conventions: plain pointers and sizes, no exceptions, no global state; every call returns
  * TSM_OK (0) or a negative tsm_status; caller owns all host memory; a tsm_ctx owns device memory
- * and is bound to one CUDA device; calls on one ctx must be serialised by the caller, calls on
- * different ctxs are independent (one host thread / process per GPU).  `stream` is a cudaStream_t
- * passed as void* (NULL = the legacy default stream).  There is no CPU fallback: without a usable
- * CUDA device tsm_create() fails with TSM_E_CUDA.
+ * and is bound to one CUDA device; calls on one ctx must be serialised by the caller (one host thread
+ * at a time), calls on different ctxs are independent, also from different host threads on one device.
+ * There is no CPU fallback: without a usable CUDA device tsm_create() fails with TSM_E_CUDA.
+ *
+ * Streams: `stream` is a cudaStream_t passed as void* (NULL = the legacy default stream).  Calls on one
+ * ctx may use different streams: each call's device work is ordered after all earlier device work of
+ * that ctx, whatever stream it was queued on, and tsm_create returns with the device initialised.
+ * tsm_upload and tsm_scan_resident return with their work in flight on `stream`, so the corpus' host
+ * arrays must stay unchanged until that work has run (a synchronisation of `stream`, or any later call
+ * that synchronises); every other call that takes a stream synchronises it before it returns.  A call
+ * that grows the ctx's scratch buffers or event lists frees device memory, which synchronises the device;
+ * a call that allocates nothing waits for no device work other than the ctx's own.
  */
 #ifndef TOSEMSCAN_H
 #define TOSEMSCAN_H
@@ -113,8 +121,10 @@ int tsm_scan_resident(tsm_ctx* ctx, uint32_t flags, void* stream);       /* kern
  * tsm_download again, the scan is not repeated. */
 int tsm_download(tsm_ctx* ctx, tsm_result* result, void* stream);
 /* Device address of the [n_groups+1][K] int64 count table of the last scan (row n_groups = global),
- * for the single multi-GPU allreduce (SURVEY.md section 8e); valid until the next scan.  The table is complete
- * once tsm_download has returned: a scan whose candidate list overflowed is redone there. */
+ * for the single multi-GPU allreduce (SURVEY.md section 8e); valid until the next scan.  When the scan's lists did
+ * not overflow, the table is complete in `stream` order behind tsm_scan_resident: work queued on that stream after
+ * the call reads the final table, and a consumer on another stream orders itself with an event recorded there.  It
+ * is complete in any case once tsm_download has returned: a scan whose candidate list overflowed is redone there. */
 int tsm_device_counts(tsm_ctx* ctx, void** dptr, int64_t* n_int64);
 /* Kernel launches issued by the last tsm_scan / tsm_scan_resident call. */
 int tsm_last_launch_count(tsm_ctx* ctx);

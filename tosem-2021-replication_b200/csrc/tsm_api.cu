@@ -88,6 +88,7 @@ struct tsm_ctx {
   cudaStream_t copy_stream = nullptr;       // H2D of arena slabs, overlapped with the scan of earlier slabs
   cudaEvent_t slab_ev[64] = {};
   cudaEvent_t ready_ev = nullptr;
+  cudaEvent_t order_ev = nullptr;           // recorded behind the device work of every call (CallOrder)
   cudaEvent_t diff_ev[8] = {};             // around the kernels of the diff path (tsm_diff_last_ms)
   uint8_t* h_diff = nullptr;               // 256 B pinned: what the diff path reads back between its kernels (Ctrl x 2, line totals, todo count)
   float diff_ms[3] = {0, 0, 0};            // k_scan over both sides, k_myers, k_myers_trace of the last diff
@@ -114,6 +115,16 @@ struct tsm_ctx {
   int ev_next = 0, ev_last = -1;
   double ms_sum[4] = {0, 0, 0, 0};
   long long ms_n = 0;
+};
+
+// A ctx orders its own work, whatever stream each call is given: a call's stream first waits for the ctx's order event
+// (a wait on an event that was never recorded is a no-op), and the event is recorded on it behind everything the call
+// queued, on every return path.  Declared before the call's DevBufs and SyncGuard, so that it records after them.
+struct CallOrder {
+  tsm_ctx* c; cudaStream_t st;
+  CallOrder(tsm_ctx* ctx, cudaStream_t s) : c(ctx), st(s) {}
+  cudaError_t wait() const { return cudaStreamWaitEvent(st, c->order_ev, 0); }
+  ~CallOrder() { cudaEventRecord(c->order_ev, st); }
 };
 
 // Fold the elapsed times of event set `i` into the running sums (waits for it if still in flight).
@@ -206,6 +217,7 @@ extern "C" void tsm_destroy(tsm_ctx* c) {
   if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
   for (cudaEvent_t e : c->slab_ev) if (e) cudaEventDestroy(e);
   if (c->ready_ev) cudaEventDestroy(c->ready_ev);
+  if (c->order_ev) cudaEventDestroy(c->order_ev);
   for (cudaEvent_t e : c->diff_ev) if (e) cudaEventDestroy(e);
   free_res_pair(c);
   cudaFree(c->d_cand); cudaFree(c->d_hev); cudaFree(c->d_aev);
@@ -259,6 +271,7 @@ extern "C" int tsm_create(tsm_ctx** out, int device, int64_t max_arena_bytes, in
   if (rc == TSM_OK && cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking) != cudaSuccess) rc = TSM_E_CUDA;
   for (cudaEvent_t& e : c->slab_ev) if (rc == TSM_OK && cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess) rc = TSM_E_CUDA;
   if (rc == TSM_OK && cudaEventCreateWithFlags(&c->ready_ev, cudaEventDisableTiming) != cudaSuccess) rc = TSM_E_CUDA;
+  if (rc == TSM_OK && cudaEventCreateWithFlags(&c->order_ev, cudaEventDisableTiming) != cudaSuccess) rc = TSM_E_CUDA;
   for (cudaEvent_t& e : c->diff_ev) if (rc == TSM_OK && cudaEventCreate(&e) != cudaSuccess) rc = TSM_E_CUDA;
   A((void**)&c->d_stats, sizeof(tsm_file_stat) * (size_t)max_files);
   A((void**)&c->d_cand, sizeof(unsigned long long) * (size_t)c->max_events);
@@ -287,6 +300,9 @@ extern "C" int tsm_create(tsm_ctx** out, int device, int64_t max_arena_bytes, in
         cudaFuncSetAttribute(k_sim_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SIM_SORT_SMEM) != cudaSuccess)
       rc = TSM_E_CUDA;
   }
+  // The arena memset runs on the legacy stream and the last constant-table copy may still be in flight: a first call on
+  // a non-blocking stream would not be ordered behind either.
+  if (rc == TSM_OK && cudaDeviceSynchronize() != cudaSuccess) rc = TSM_E_CUDA;
   if (rc != TSM_OK) {
     fprintf(stderr, "tosemscan: tsm_create failed: %s\n", cudaGetErrorString(cudaGetLastError()));
     tsm_destroy(c);
@@ -351,6 +367,8 @@ extern "C" int tsm_upload(tsm_ctx* c, const tsm_corpus* k, void* stream) {
   if (rc != TSM_OK) return rc;
   CU(cudaSetDevice(c->device));
   cudaStream_t st = (cudaStream_t)stream;
+  CallOrder order(c, st);
+  CU(order.wait());
   rc = upload_index(c, k, st);
   if (rc != TSM_OK) return rc;
   if (c->n_files) CU(cudaMemcpyAsync(c->d_arena, k->arena, (size_t)c->arena_bytes, cudaMemcpyHostToDevice, st));
@@ -480,6 +498,8 @@ extern "C" int tsm_scan_resident(tsm_ctx* c, uint32_t flags, void* stream) {
   flags &= TSM_SCAN_ASSERT_EVENTS | TSM_SCAN_HEADER_EVENTS | TSM_SCAN_REV_B;
   if (!c->resident) return TSM_E_STATE;
   CU(cudaSetDevice(c->device));
+  CallOrder order(c, (cudaStream_t)stream);
+  CU(order.wait());
   return launch_scan(c, flags, (cudaStream_t)stream, nullptr);
 }
 
@@ -582,11 +602,8 @@ template <typename Event> static void sort_events_by_file(Event* ev, uint32_t m,
   std::copy(tmp.begin(), tmp.end(), ev);
 }
 
-extern "C" int tsm_download(tsm_ctx* c, tsm_result* r, void* stream) {
-  if (!c || !r) return TSM_E_ARG;
-  if (!c->scanned) return TSM_E_STATE;
-  CU(cudaSetDevice(c->device));
-  cudaStream_t st = (cudaStream_t)stream;
+// tsm_download inside a call that has set the device and ordered st.
+static int download(tsm_ctx* c, tsm_result* r, cudaStream_t st) {
   r->n_aev = 0; r->n_hev = 0;
   int rc = download_tables(c, r, st);
   if (rc != TSM_OK) return rc;
@@ -620,6 +637,15 @@ extern "C" int tsm_download(tsm_ctx* c, tsm_result* r, void* stream) {
   return TSM_OK;
 }
 
+extern "C" int tsm_download(tsm_ctx* c, tsm_result* r, void* stream) {
+  if (!c || !r) return TSM_E_ARG;
+  if (!c->scanned) return TSM_E_STATE;
+  CU(cudaSetDevice(c->device));
+  CallOrder order(c, (cudaStream_t)stream);
+  CU(order.wait());
+  return download(c, r, (cudaStream_t)stream);
+}
+
 extern "C" int tsm_scan(tsm_ctx* c, const tsm_corpus* k, tsm_result* r, uint32_t flags, void* stream) {
   if (!c || !r) return TSM_E_ARG;
   int rc = check_corpus_head(c, k);                       // (the per-file rules are checked slab by slab, under the copies)
@@ -627,12 +653,14 @@ extern "C" int tsm_scan(tsm_ctx* c, const tsm_corpus* k, tsm_result* r, uint32_t
   flags &= TSM_SCAN_ASSERT_EVENTS | TSM_SCAN_HEADER_EVENTS | TSM_SCAN_REV_B;
   CU(cudaSetDevice(c->device));
   cudaStream_t st = (cudaStream_t)stream;
+  CallOrder order(c, st);
+  CU(order.wait());
   rc = upload_index(c, k, st);                            // the index first (small), the arena slab by slab
   if (rc != TSM_OK) return rc;
   c->resident = true;
   rc = launch_scan(c, flags, st, k, true);
   if (rc != TSM_OK) { c->resident = false; c->scanned = false; return rc; }
-  return tsm_download(c, r, stream);
+  return download(c, r, st);
 }
 
 // ------------------------------------------------------------------------------------- S10 reduce
@@ -646,6 +674,8 @@ extern "C" int tsm_reduce(tsm_ctx* c, const uint8_t* flags, const int32_t* repo,
   CU(cudaSetDevice(c->device));
   PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
+  CallOrder order(c, st);
+  CU(order.wait());
   const size_t words = ((size_t)n_cases + 31) / 32;
   const size_t nbits = (size_t)(n_flags + 1) * n_repos * words;
   DevBuf b_flags, b_repo, b_case, b_bits, b_out;          // scratch from the ctx's pool (kept between calls)
@@ -1146,6 +1176,8 @@ extern "C" int tsm_diff_pairs_detail(tsm_ctx* c, const tsm_corpus* olds, const t
   CU(cudaSetDevice(c->device));
   PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
+  CallOrder order(c, st);
+  CU(order.wait());
   HostSidePair P;
   SyncGuard guard(st);                                     // (after P) no buffer goes back to the pool while work on st may still use it
   rc = pair_upload(olds, news, false, P, st);
@@ -1176,6 +1208,8 @@ extern "C" int tsm_diff_pairs_asserts(tsm_ctx* c, const tsm_corpus* olds, const 
   CU(cudaSetDevice(c->device));
   PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
+  CallOrder order(c, st);
+  CU(order.wait());
   HostSidePair P;
   SyncGuard guard(st);
   rc = pair_upload(olds, news, true, P, st);
@@ -1188,9 +1222,11 @@ extern "C" int tsm_diff_upload(tsm_ctx* c, const tsm_corpus* olds, const tsm_cor
   int rc = check_sides({olds, news}, olds->n_files, true);
   if (rc != TSM_OK) return rc;
   CU(cudaSetDevice(c->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  CallOrder order(c, st);
+  CU(order.wait());
   free_res_pair(c);
   PoolScope pool_scope(&c->pool);
-  cudaStream_t st = (cudaStream_t)stream;
   SyncGuard guard(st);
   c->res_pair = new (std::nothrow) HostSidePair;
   if (!c->res_pair) return TSM_E_NOMEM;
@@ -1207,6 +1243,8 @@ extern "C" int tsm_diff_resident(tsm_ctx* c, int64_t* added, int64_t* removed, t
   CU(cudaSetDevice(c->device));
   PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
+  CallOrder order(c, st);
+  CU(order.wait());
   SyncGuard guard(st);
   return pair_run(c, *c->res_pair, added, removed, detail, nullptr, st);
 }
@@ -1221,6 +1259,8 @@ extern "C" int tsm_diff_resident_asserts(tsm_ctx* c, int64_t* added, int64_t* re
   CU(cudaSetDevice(c->device));
   PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
+  CallOrder order(c, st);
+  CU(order.wait());
   SyncGuard guard(st);
   return pair_run(c, *c->res_pair, added, removed, detail, out, st);
 }
@@ -1277,6 +1317,8 @@ extern "C" int tsm_similarity(tsm_ctx* c, const tsm_corpus* olds, const tsm_corp
   if (rc != TSM_OK) return rc;
   PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
+  CallOrder order(c, st);
+  CU(order.wait());
   HostSidePair P;
   SimLists LA, LB;
   DevBuf d_cand;
@@ -1339,6 +1381,8 @@ static int line_records(tsm_ctx* c, const tsm_corpus* k, bool ext_rule, int64_t*
   CU(cudaSetDevice(c->device));
   PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
+  CallOrder order(c, st);
+  CU(order.wait());
   HostSide S;
   SyncGuard guard(st);
   rc = side_upload(k, S, st);
