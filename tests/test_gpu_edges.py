@@ -260,7 +260,7 @@ def test_saturated_statement_fields_and_full_statement_hash(scanner):
 @pytest.mark.parametrize("rev_b", [False, True], ids=["rev_a", "rev_b"])
 def test_triggers_inside_lines_longer_than_the_lookahead(scanner, rev_b):
     """Rev-A and Rev-B triggers at every offset mod 8 inside lines that start in one chunk and end more than 240 B
-    into the next (long_line / revb_trigger_gmem), before, on and behind the chunk edge."""
+    into the next (long_line, the automaton walked from HBM), before, on and behind the chunk edge."""
     trig = [b"assert", b"EXPECT_", b"_CHECK", b"TESTEQUAL", b"FAIL"]
     files = []
     for t in trig:
@@ -275,6 +275,36 @@ def test_triggers_inside_lines_longer_than_the_lookahead(scanner, rev_b):
             f = files[int(e["file"])]
             t = sr.py_statement(f[int(e["line_off"]):].split(b"\n", 1)[0])
             assert int(e["stmt_hash"]) == sr.py_bytes_hash(t) and int(e["cat"]) == sr.py_category(t)
+
+
+LONG_HEADS = [b"class Foo(Base):", b"class", b"def test_x(self):", b"TEST_F(Fix, Name) {", b"TEST_F(Fix, Name)",
+              b"test_case(int x) {", b"void helper(int x) {"]
+
+
+@pytest.mark.parametrize("rev_b", [False, True], ids=["rev_a", "rev_b"])
+@pytest.mark.parametrize("ext", [1, 2, 4, 0], ids=["py", "cc", "java", "none"])
+def test_header_rules_on_lines_longer_than_the_lookahead(scanner, ext, rev_b):
+    """Header and fixture-header lines (`class` + blank + text, `class` + only blanks, `def`, `TEST_F(` with and
+    without `{`, `test ... {`, `void ... {`) that start in one chunk at every offset mod 8 and end more than 240 B
+    into the next (long_line reads them from HBM): behind 0-20 blanks of indentation (runs of spaces, with and
+    without tabs), ended by LF, by CR LF, or unterminated at the end of the file."""
+    indents = [b" " * n for n in range(21)] + [b"\t", b" \t", b"\t" * 9 + b" ", b" " * 7 + b"\t" + b" " * 7,
+                                               b"\t " * 10, b" " * 15 + b"\t"]
+    files = []
+    for h, head in enumerate(LONG_HEADS):
+        pad = b" " * 500 + b"\t" if head == b"class" else b" " + b"z" * 500
+        for i, ind in enumerate(indents):
+            for k in range(8):
+                end = (b"\n", b"\r\n", b"")[(h + i + k) % 3]
+                files.append(filler(4000 + k) + ind + head + pad + end + (b"def tail():\n" if end else b""))
+    c = ts.pack(files, [ext] * len(files))
+    got = check_against_oracle(scanner, c, rev_b=rev_b)
+    if ext:
+        assert int(got["stats"]["n_headers"].sum()) > len(files) // 4 and (ext == 1) == (int(got["stats"]["n_fixture"].sum()) == 0)
+    if not rev_b:                                        # (line records are Rev A's)
+        want = orc.line_records(c.arena, c.off, c.len, c.ext)
+        for a, b in zip(scanner.line_hashes(c), want):
+            assert np.array_equal(a, b)
 
 
 # ---------------------------------------------------------------------------------------- 6. dense events

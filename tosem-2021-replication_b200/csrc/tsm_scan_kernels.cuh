@@ -1,7 +1,7 @@
 // tsm_scan_kernels.cuh - hand-written sm_90a kernels of the corpus scan (docs/SPEC.md, DESIGN.md), part 1:
 //
 //   k_plan      files -> (file, 4 KiB chunk) work units                         [tiny]
-//   (k_scan     the hot kernel: tsm_scan_walk.cuh; this file holds the line helpers it shares with the slow path)
+//   (k_scan     the hot kernel: tsm_scan_walk.cuh; this file holds the small helpers it uses)
 //   k_classify  one thread per candidate: statement, last identifier, category (S5), events, the
 //               cross-file aggregate into a shared-memory privatised [group][category] table, and
 //               the totals of the per-file records.
@@ -9,7 +9,6 @@
 // There is no reference kernel: the reference ships data only (SURVEY.md section 0).  Rules cite
 // docs/SPEC.md, which cites the artefacts.
 #pragma once
-#include <type_traits>
 #include "tsm_device.cuh"
 
 namespace tsm {
@@ -51,7 +50,7 @@ __global__ void k_plan(ScanParams p) {
   }
 }
 
-// ================================================================================= line helpers (k_scan, its slow path)
+// ================================================================================= helpers of k_scan
 // SWAR: 4-bit mask of the bytes equal to '\n' in a 32-bit word.
 __device__ __forceinline__ uint32_t nl_word(uint32_t w) {
   const uint32_t y = w ^ 0x0A0A0A0Au;
@@ -59,52 +58,14 @@ __device__ __forceinline__ uint32_t nl_word(uint32_t w) {
   const uint32_t z = ~(t | y | 0x7F7F7F7Fu);            // 0x80 in every byte that was '\n'
   return (z * 0x00204081u) >> 28;                        // gather the four flag bits: 7+21, 15+14, 23+7, 31+0 -> 28..31
 }
-// Per-lane state of the line currently walked by this lane.
-struct LineState {
-  uint32_t s, e;            // [s, e) = line
-  uint32_t pos;             // next 8-byte block to process
-  uint32_t D, A;            // automaton state / OR of all states
-  unsigned long long B;     // Horner accumulator: B_k = B_{k-1} * 2^-64 + X_k  (mod 2^61-1)
-};
-
-__device__ __forceinline__ void line_init(LineState& L, uint32_t s, uint32_t e) {
-  L.s = s; L.e = e; L.D = 0; L.A = 0; L.B = 0;
-  L.pos = (s == e) ? e : (s & ~7u);
+// number of leading 0x20 bytes among the 8 bytes of w
+__device__ __forceinline__ uint32_t spaces_of(unsigned long long w) {
+  const unsigned long long x = w ^ 0x2020202020202020ull, k7 = 0x7F7F7F7F7F7F7F7Full;
+  const unsigned long long nz = (((x & k7) + k7) | x) & ~k7;             // 0x80 in every byte that is not a space
+  return nz ? ((uint32_t)__ffsll((long long)nz) - 1u) >> 3 : 8u;
 }
-
-// One 8-byte block of a lane-per-line walk (long-line slow path).  Files without a scannable
-// extension run the same code: their pattern ends are simply never looked at.
-__device__ __forceinline__ void line_block(LineState& L, unsigned long long w, const uint32_t* lut, uint32_t first) {
-  const uint32_t pos = L.pos;
-  if (pos < L.s || pos + 8 > L.e) {                      // first / last block: zero the bytes outside the line
-    unsigned long long m = ~0ull;
-    if (pos < L.s) m <<= 8u * (L.s - pos);
-    if (pos + 8 > L.e) m &= ~0ull >> (8u * (pos + 8 - L.e));
-    w &= m;
-  }
-  {
-    const uint32_t lo = (uint32_t)w, hi = (uint32_t)(w >> 32);
-    uint32_t D = L.D, A = L.A;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      D = ((D + D) | first) & lut[__byte_perm(lo, 0, 0x4440 + k)];
-      A |= D;
-    }
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      D = ((D + D) | first) & lut[__byte_perm(hi, 0, 0x4440 + k)];
-      A |= D;
-    }
-    L.D = D; L.A = A;
-  }
-  // B = B * 2^-64 + w  (2^-64 = 2^-3 = 2^58 mod 2^61-1: a rotation by 3 to the right)
-  const unsigned long long b = L.B;
-  const unsigned long long rot = (b >> 3) | ((b & 7ull) << 58);
-  L.B = fold61(fold61(rot + fold61(w)));
-  L.pos = pos + 8;
-}
-
-struct SmemByte {                                        // byte source = the staged chunk
+// Byte sources of the line rules (line_flags2, starts_with8): a byte, the 8 bytes at any alignment, their leading spaces.
+struct SmemByte {                                        // the staged chunk
   const uint8_t* b;
   __device__ __forceinline__ uint32_t operator()(uint32_t i) const { return b[i]; }
   // the 8 bytes at i, any alignment (shared memory is readable 8 bytes past any line of the buffer)
@@ -114,96 +75,23 @@ struct SmemByte {                                        // byte source = the st
     const unsigned long long hi = *reinterpret_cast<const unsigned long long*>(b + a + 8);
     return sh ? (lo >> sh) | (hi << (64u - sh)) : lo;
   }
-  // number of leading 0x20 bytes among the 8 bytes at i
-  __device__ __forceinline__ uint32_t spaces8(uint32_t i) const {
-    const unsigned long long w = load8(i);
-    const unsigned long long x = w ^ 0x2020202020202020ull, k7 = 0x7F7F7F7F7F7F7F7Full;
-    const unsigned long long nz = (((x & k7) + k7) | x) & ~k7;           // 0x80 in every byte that is not a space
-    return nz ? ((uint32_t)__ffsll((long long)nz) - 1u) >> 3 : 8u;
-  }
+  __device__ __forceinline__ uint32_t spaces8(uint32_t i) const { return spaces_of(load8(i)); }
 };
-struct GmemByte {                                        // byte source = the file in HBM (slow path)
+struct HbmByte {                                         // a file in HBM (long lines), b 8-byte aligned
   const uint8_t* b;
   __device__ __forceinline__ uint32_t operator()(uint32_t i) const { return __ldg(b + i); }
+  // the 8 bytes at i from two aligned loads, which read up to byte i + 15, i.e. up to 15 bytes past the line end.  That
+  // is readable: every device arena has 4 096 B of slack behind off[n] (tsm_create allocates max_arena + 4096,
+  // side_upload ab + 4096).
+  __device__ __forceinline__ unsigned long long load8(uint32_t i) const {
+    const unsigned long long* w = reinterpret_cast<const unsigned long long*>(b) + (i >> 3);
+    const uint32_t sh = 8u * (i & 7u);
+    const unsigned long long lo = __ldg(w), hi = __ldg(w + 1);
+    return sh ? (lo >> sh) | (hi << (64u - sh)) : lo;
+  }
+  __device__ __forceinline__ uint32_t spaces8(uint32_t i) const { return spaces_of(load8(i)); }
 };
-
-template <typename LoadByte>
-__device__ __forceinline__ bool starts_with(LoadByte lb, uint32_t s, uint32_t e, const char* pat, int n, bool need_ws) {
-  if constexpr (std::is_same<LoadByte, SmemByte>::value) {  // staged bytes: runs of spaces eight at a time
-    uint32_t r;
-    while (s + 8 <= e && (r = lb.spaces8(s)) != 0) { s += r; if (r < 8) break; }
-  }
-  while (s < e && is_w(lb(s))) ++s;
-  if (s + n + (need_ws ? 1 : 0) > e) return false;
-  for (int k = 0; k < n; ++k)
-    if (lb(s + k) != (uint8_t)pat[k]) return false;
-  if (need_ws) {                                         // the blank must be inside the STRIPPED line:
-    const uint32_t c = lb(s + n);                        // some non-blank byte has to follow it
-    if (c != 0x20 && c != 0x09) return false;
-    for (uint32_t q = s + n + 1; q < e; ++q)
-      if (!is_w(lb(q))) return true;
-    return false;
-  }
-  return true;
-}
-
 struct Accum { uint32_t lines, asserts, hdrs, fixes; unsigned long long digest; };
-
-
-// The four facts pass 3 needs about a line, as one nibble: bit 0 = assertion pattern, bits 1..3 = the
-// language's header patterns (PY: def, class, TEST_F gate; C family: test, one of { class void, TEST_F gate).
-__device__ __forceinline__ uint32_t flag_nibble(uint32_t A, uint32_t g1, uint32_t g2, uint32_t g3) {
-  return ((A & (AF_ASSERT | AF_EXPECT)) ? 1u : 0u) | ((A & g1) ? 2u : 0u) | ((A & g2) ? 4u : 0u) | ((A & g3) ? 8u : 0u);
-}
-__device__ __forceinline__ uint32_t flag_nibble_ext(uint32_t A, int ext) {
-  return ext == TSM_EXT_PY ? flag_nibble(A, PY_G1, PY_G2, 0u) : flag_nibble(A, CJ_G1, CJ_G2, 0u);
-}
-
-// Finish one line: h0 = Mersenne-61 value of its bytes (SPEC section 3, trailing CR still inside), nib = its
-// pattern nibble.  Adds the line to the per-file accumulators and returns its LF_* flags (SPEC sections 4/5).
-template <typename LoadByte>
-__device__ __forceinline__ uint32_t line_finish_h(uint32_t s, uint32_t e, unsigned long long h0, uint32_t nib, int ext,
-                                                  LoadByte lb, Accum& ac) {
-  uint32_t len = e - s;
-  unsigned long long h = 0;
-  if (len) {
-    h = h0;
-    if (lb(e - 1) == 0x0D) {                             // drop one trailing CR: subtract 0x0D * 256^(len-1)
-      --len;
-      const unsigned long long cr = rotl61(0x0Dull, (8u * len) % 61u);
-      h = h >= cr ? h - cr : h + M61 - cr;
-    }                                                    // h0 is canonical (< 2^61 - 1) and the CR step keeps it so
-  }
-  ac.lines++;
-  ac.digest += mix_hash(h, len);
-  if (ext == 0) return 0;
-  uint32_t fl = (nib & 1u) ? LF_CAND : 0;
-  bool hdr;
-  if (ext == TSM_EXT_PY) {
-    hdr = (nib & 2u) != 0;
-    if (!hdr && (nib & 4u)) hdr = starts_with(lb, s, e, "class", 5, true);
-  } else {
-    hdr = (nib & 6u) == 6u;
-  }
-  if (hdr) { fl |= LF_HDR; if (starts_with(lb, s, e, "TEST_F", 6, false)) fl |= LF_FIX; }   // (headers are ~2 % of the lines)
-  ac.asserts += fl & LF_CAND;
-  ac.hdrs += (fl >> 1) & 1u;
-  ac.fixes += (fl >> 2) & 1u;
-  return fl;
-}
-
-// Same, from the raw (A, B) of a lane-per-line walk (the long-line slow path).
-template <typename LoadByte>
-__device__ __forceinline__ uint32_t line_finish(uint32_t s, uint32_t e, uint32_t A, unsigned long long B, int ext,
-                                                LoadByte lb, Accum& ac) {
-  unsigned long long h0 = 0;
-  if (e != s) {
-    // N * 2^(8*lead) = B * 2^(64*(m-1)), m = number of 8-byte blocks the line touches
-    const uint32_t lead = s & 7u, m = ((e - 1) >> 3) - (s >> 3) + 1;
-    h0 = rotl61(canon61(B), (3u * (m - 1) + 61u * 8u - 8u * lead) % 61u);
-  }
-  return line_finish_h(s, e, h0, ext ? flag_nibble_ext(A, ext) : 0u, ext, lb, ac);
-}
 
 // Append `n` list entries with one atomic; returns the base slot (broadcast from lane 0).
 __device__ __forceinline__ uint32_t warp_reserve(uint32_t* counter, uint32_t n, int lane) {
@@ -216,36 +104,6 @@ __device__ __forceinline__ uint32_t warp_reserve(uint32_t* counter, uint32_t n, 
 __device__ __forceinline__ const uint32_t* scan_lut() {
   extern __shared__ __align__(128) uint8_t smem[];
   return reinterpret_cast<const uint32_t*>(smem);
-}
-
-// Slow path: a line that starts in this chunk but ends behind the staged bytes.  Walked by lane 0
-// straight from HBM (correct for any length; lines longer than 240 B past a chunk edge are rare).
-// Everything goes in and out by value: no argument of this call lives in local memory.
-struct LongLine { uint32_t e, fl; Accum ac; };           // file-relative end of the line, its LF_* flags, the accumulators
-__device__ __noinline__ LongLine long_line(const ScanParams& p, const uint32_t* lut, uint32_t first, uint32_t f,
-                                           uint32_t fo, uint32_t size, int ext, uint32_t s, Accum ac) {
-  const uint8_t* g = p.arena + fo;
-  const GmemByte lb{g};
-  uint32_t e = s;
-  while (e < size && lb(e) != '\n') ++e;
-  LineState L;
-  line_init(L, s, e);
-  while (L.pos < L.e) {
-    const unsigned long long w = __ldg(reinterpret_cast<const unsigned long long*>(g + L.pos));
-    line_block(L, w, lut, first);
-  }
-  const uint32_t fl = line_finish(s, e, L.A, L.B, ext, lb, ac);
-  if ((fl & LF_CAND) && p.cand_cap) {
-    const uint32_t slot = atomicAdd(&p.ctrl->n_cand, 1u);
-    if (slot < p.cand_cap) p.cand[slot] = ((unsigned long long)f << 32) | s;
-    else p.ctrl->overflow = 1;
-  }
-  if ((fl & LF_HDR) && (p.flags & TSM_SCAN_HEADER_EVENTS)) {
-    const uint32_t slot = atomicAdd(&p.ctrl->n_hev, 1u);
-    if (slot < p.hev_cap) p.hev[slot] = tsm_header_event{f, s, e - s, (fl >> 2) & 1u};
-    else p.ctrl->overflow = 1;
-  }
-  return LongLine{e, fl, ac};
 }
 
 // Stage the bytes [max(cb-16,0), min(cb+CH+EXT, size)) of a file so that file byte cb sits at buf+PRE.

@@ -93,26 +93,17 @@ constexpr uint32_t B2_FIRST = (1u << 0) | (1u << 6) | (1u << 15), B2_FIN = (1u <
 constexpr uint32_t REVB_BIT = 1u;                        // in the stored ORs: bit 0 (a non-final state of `assert`) = "a Rev-B trigger ended"
 
 // Table entry of byte `idx`.  The address is formed by an integer multiply-add whose factor (4) the compiler
-// cannot see: IMAD runs on the FMA pipe, the LEA it replaces on the ALU pipe.
-#ifndef TSM_PIPE_BALANCE
-#define TSM_PIPE_BALANCE 1
-#endif
-// Both operands come from shared memory (LutRef, written by the kernel prologue), so the compiler keeps them in
-// registers for the whole pass instead of forming the table address again for every word.
+// cannot see: IMAD runs on the FMA pipe, the LEA it replaces on the ALU pipe.  Both operands come from shared memory
+// (LutRef, written by the kernel prologue), so the compiler keeps them in registers for the whole pass instead of
+// forming the table address again for every word.
 struct LutRef { uint32_t four, base; };                  // 4 (from a launch parameter) and the table's shared-window address
 __device__ __forceinline__ LutRef lut_ref() { return LutRef{scan_lut()[256 + 12], scan_lut()[256 + 13]}; }
 template <bool REVB>
 __device__ __forceinline__ void lut_at(uint32_t idx, LutRef t, uint32_t& v, uint32_t& v2) {
-#if TSM_PIPE_BALANCE
   uint32_t addr;
   asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(addr) : "r"(idx), "r"(t.four), "r"(t.base));
   asm("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
   if (REVB) asm("ld.shared.u32 %0, [%1+%2];" : "=r"(v2) : "r"(addr), "n"(O2_LUTB));
-#else
-  (void)t;
-  v = scan_lut()[idx];
-  if (REVB) v2 = scan_lut()[O2_LUTB / 4 + idx];
-#endif
 }
 
 struct Auto { uint32_t D, D2; };                         // automaton state (D2: the Rev-B word, unused otherwise)
@@ -242,13 +233,14 @@ __device__ __forceinline__ void emit_header(const ScanParams& p, uint32_t f, uin
 }
 
 // Does the stripped line [s, e) start with the n <= 7 bytes of `pat` (little-endian in a u64)?  With need_ws the
-// byte behind them must be a blank that lies inside the stripped line (SPEC section 5, `class`).  Staged bytes only.
-__device__ __noinline__ bool starts_with8(SmemByte lb, uint32_t s, uint32_t e, unsigned long long pat, uint32_t n, bool need_ws) {
+// byte behind them must be a blank that lies inside the stripped line (SPEC section 5, `class`).
+template <typename Bytes>
+__device__ __noinline__ bool starts_with8(Bytes lb, uint32_t s, uint32_t e, unsigned long long pat, uint32_t n, bool need_ws) {
   uint32_t r;
   while (s + 8 <= e && (r = lb.spaces8(s)) != 0) { s += r; if (r < 8) break; }
   while (s < e && is_w(lb(s))) ++s;
   if (s + n + (need_ws ? 1u : 0u) > e) return false;
-  const unsigned long long v = lb.load8(s);              // readable 8 bytes past any line of the buffer
+  const unsigned long long v = lb.load8(s);              // readable 8 bytes past any line (SmemByte, HbmByte)
   if ((v & low_mask(n)) != pat) return false;
   if (need_ws) {
     const uint32_t c = (uint32_t)(v >> (8u * n)) & 0xFFu;
@@ -261,8 +253,8 @@ __device__ __noinline__ bool starts_with8(SmemByte lb, uint32_t s, uint32_t e, u
 }
 
 // Flags of a finished line (SPEC sections 4 / 5) from the OR of its automaton states; adds it to the per-file counters.
-template <bool REVB>
-__device__ __forceinline__ uint32_t line_flags2(uint32_t s, uint32_t e, uint32_t A, uint32_t g1, uint32_t g2, int ext, SmemByte lb, Accum& ac) {
+template <bool REVB, typename Bytes>
+__device__ __forceinline__ uint32_t line_flags2(uint32_t s, uint32_t e, uint32_t A, uint32_t g1, uint32_t g2, int ext, Bytes lb, Accum& ac) {
   if (ext == 0) return 0;
   uint32_t fl = (A & (AF_ASSERT | AF_EXPECT | (REVB ? REVB_BIT : 0u))) ? LF_CAND : 0;
   bool hdr;
@@ -277,19 +269,6 @@ __device__ __forceinline__ uint32_t line_flags2(uint32_t s, uint32_t e, uint32_t
   ac.hdrs += (fl >> 1) & 1u;
   ac.fixes += (fl >> 2) & 1u;
   return fl;
-}
-
-// Does the line [s, e) of a file in HBM hold a Rev-B trigger (docs/SPEC.md section 4b)?  Slow path of long lines only.
-__device__ __noinline__ bool revb_trigger_gmem(const uint8_t* g, uint32_t s, uint32_t e) {
-  const char* const pats[3] = {"_CHECK", "TESTEQUAL", "FAIL"};
-  const uint32_t lens[3] = {6, 9, 4};
-  for (int t = 0; t < 3; ++t)
-    for (uint32_t i = s; i + lens[t] <= e; ++i) {
-      uint32_t k = 0;
-      while (k < lens[t] && __ldg(g + i + k) == (uint8_t)pats[t][k]) ++k;
-      if (k == lens[t]) return true;
-    }
-  return false;
 }
 
 struct FinishState {                                     // carried from one window of line records to the next (by value: no local memory)
@@ -402,6 +381,57 @@ __device__ __noinline__ FinishState finish_lines2(const ScanParams& p, uint8_t* 
   fs.prevP = prevP;
   fs.lh_done = lh_done;
   return fs;
+}
+
+// Slow path: the line that starts at file byte s of this chunk but ends behind the staged bytes (rare).  Lane 0 walks
+// it straight from HBM with the walk's automaton step and hash recurrence and finishes it as finish_lines2 does: its
+// candidate, header event and line record are written here.  Everything goes in and out by value: no argument of
+// this call lives in local memory.
+template <bool REVB>
+__device__ __noinline__ Accum long_line(const ScanParams& p, const uint32_t* lc, uint32_t f, uint32_t size, int ext,
+                                        uint32_t s, uint32_t lh_slot, Accum ac) {
+  const HbmByte lb{p.arena + (uint32_t)p.off[f]};
+  uint32_t e = s;
+  while (e < size && lb(e) != '\n') ++e;                 // (e > s: byte s is no newline)
+  const uint32_t k0 = s >> 3, k1 = (e - 1u) >> 3;        // the words the line touches
+  const LutRef t = lut_ref();
+  Auto au{0u, 0u};
+  uint32_t A = 0;
+  unsigned long long R = 0;
+#pragma unroll 1
+  for (uint32_t k = k0; k <= k1; ++k) {                  // bytes outside the line become zeros, as in the staged chunk
+    unsigned long long w = __ldg(reinterpret_cast<const unsigned long long*>(lb.b) + k);
+    if (k == k0) w &= ~0ull << (8u * (s & 7u));
+    if (k == k1) w &= low_mask(e - 8u * k);
+    uint32_t Aw = 0;
+    step8b<REVB>(w, au, Aw, t);
+    A |= Aw;
+    R = ror3_61(R) + fold61(w);
+  }
+  // value of the bytes [s, e): R * 2^(64 (k1 - k0)) / 2^(8 (s & 7))
+  unsigned long long h = rotl61(canon61(R), (3u * (k1 - k0) + 61u * 8u - 8u * (s & 7u)) % 61u);
+  uint32_t len = e - s;
+  if (lb(e - 1u) == 0x0D) {                              // drop one trailing CR: subtract 0x0D * 256^(len-1)
+    --len;
+    const unsigned long long cr = rotl61(0x0Dull, (8u * len) % 61u);
+    h = h >= cr ? h - cr : h + M61 - cr;
+  }
+  const unsigned long long lh = mix_hash(h, len);
+  ac.lines++;
+  ac.digest += lh;
+  const uint32_t fl = line_flags2<REVB>(s, e, A, lc[1], lc[2], ext, lb, ac);
+  if ((fl & LF_CAND) && p.cand_cap) {
+    const uint32_t slot = atomicAdd(&p.ctrl->n_cand, 1u);
+    if (slot < p.cand_cap) p.cand[slot] = ((unsigned long long)f << 32) | s;
+    else p.ctrl->overflow = 1;
+  }
+  if ((fl & LF_HDR) && (p.flags & TSM_SCAN_HEADER_EVENTS)) emit_header(p, f, s, e - s, fl);
+  if ((p.flags & TSM_SCAN_LINE_HASHES) && lh_slot < p.lh_cap) {   // the chunk's last line
+    p.lh_hash[lh_slot] = lh;
+    p.lh_end[lh_slot] = e;
+    p.lh_flag[lh_slot] = (uint8_t)(fl & LF_CAND);
+  }
+  return ac;
 }
 
 template <bool REVB>
@@ -550,28 +580,7 @@ __device__ __forceinline__ void process_chunk2(const ScanParams& p, const uint32
   if (n_rec) fs = finish_lines2<REVB>(p, wb, lc, n_rec, lim, skip_first, f, cb, ext, lane, fs);
   pc.mark(PH_FINISH, lane);
   Accum ac = fs.ac;
-  if (tail_long && lane == 0) {
-    const unsigned long long d0 = ac.digest;
-    const uint32_t ls = cb + tail_start - PRE;
-    const uint32_t fo = (uint32_t)p.off[f];              // (read again here: kept in a register it spilled in the Rev-B kernel)
-    const LongLine ll = long_line(p, scan_lut(), B_FIRST, f, fo, size, ext, ls, ac);
-    const uint32_t e = ll.e;
-    uint32_t fl = ll.fl;
-    ac = ll.ac;
-    if (REVB && ext != 0 && !(fl & LF_CAND) && revb_trigger_gmem(p.arena + fo, ls, e)) {   // Rev-B triggers of a long line: plain search in HBM
-      fl |= LF_CAND;
-      ac.asserts++;
-      if (p.cand_cap) {
-        const uint32_t slot = atomicAdd(&p.ctrl->n_cand, 1u);
-        if (slot < p.cand_cap) p.cand[slot] = ((unsigned long long)f << 32) | ls;
-        else p.ctrl->overflow = 1;
-      }
-    }
-    if (want_lh) {                                       // the chunk's last line
-      const uint32_t slot = fs.lh_base + fs.lh_done;
-      if (slot < p.lh_cap) { p.lh_hash[slot] = ac.digest - d0; p.lh_end[slot] = e; p.lh_flag[slot] = (uint8_t)(fl & LF_CAND); }
-    }
-  }
+  if (tail_long && lane == 0) ac = long_line<REVB>(p, lc, f, size, ext, cb + tail_start - PRE, fs.lh_base + fs.lh_done, ac);
   pc.mark(PH_LONG, lane);
   // ---- per-file counters: warp reduce (the digest as three partial sums: low halves keep their carries),
   //      then one store (single-chunk file) or one atomic per counter
@@ -635,15 +644,8 @@ __global__ void __launch_bounds__(SCAN2_WARPS * 32, SCAN2_CTAS_PER_SM) k_scan_t(
 #if TSM_PHASE_CLOCKS
   pc.t = clock64();
 #endif
-#ifndef TSM_LOCKSTEP2
-#define TSM_LOCKSTEP2 0
-#endif
-#if TSM_LOCKSTEP2
-  while (__syncthreads_or(cur.u < n_units)) {
-    if (cur.u >= n_units) continue;
-#else
   while (cur.u < n_units) {                              // (no CTA-wide chunk start: with the walk as one rolled loop the hot code fits the
-#endif                                                   //  instruction cache and the barrier only costs)
+                                                         //  instruction cache and the barrier only costs)
     fence_proxy_async();                                 // this warp's zero fill and reads of the last chunk come first
     __syncwarp();
     if (lane == 0) issue_load(p, wb, bar, cur.fo, cur.size, cur.cb);
