@@ -196,6 +196,39 @@ int tsm_similarity(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news,
                    int64_t n_cand, int64_t* common, void* stream);
 int tsm_similarity_last_ms(tsm_ctx* ctx, float* ms3);
 
+/* Edit marks (docs/SPEC.md section 14): the lines the canonical edit script of each pair deletes from olds and inserts into
+ * news, one byte per line (1 = deleted / inserted, else 0) in the global line order of each side (line_base: files in order,
+ * SPEC sections 2-3).  A pair tsm_diff_pairs_detail does not trace has its whole middle marked (every line between the common
+ * prefix and suffix), the one hunk its detail reports.  added / removed / detail are those of tsm_diff_pairs_detail (detail
+ * may be NULL).  line_base_old / line_base_new [n_pairs+1] and n_old / n_new are always set; if del_cap < n_old or
+ * ins_cap < n_new the call returns TSM_E_CAPACITY with them set (and no diff run): size the arrays and call again.
+ * Kernels: the DIFF_MARKS variants of k_diff_small (all four sizes) and k_myers_trace. */
+typedef struct tsm_line_marks {
+  int64_t* line_base_old; int64_t* line_base_new;   /* [n_pairs+1] */
+  uint8_t* del; int64_t del_cap; int64_t n_old;     /* [lines of olds] */
+  uint8_t* ins; int64_t ins_cap; int64_t n_new;     /* [lines of news] */
+} tsm_line_marks;
+int tsm_diff_pairs_marks(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                         tsm_diff_detail* detail, tsm_line_marks* marks, void* stream);
+
+/* Line provenance (docs/SPEC.md section 14, `tosem-scan blame`): the origin of every line of every new side.  The pairs form
+ * chains: prev[i] is the pair whose new side is pair i's old side (prev[i] < i; each pair is the prev of at most one pair), or
+ * -1 for a chain head, whose old side's origins are origin_in[in_base[i] .. in_base[i+1]) (in_base [n_pairs+1], ascending;
+ * only the heads' ranges are read).  The k-th line of new that the script does not insert takes the origin of the k-th line of
+ * old that it does not delete; inserted line j (0-based) of pair i gets {label[i], j + 1}.  TSM_E_ARG for a bad prev, or for
+ * a pair whose old side has another line count than its prev's new side or its head range.  line_base_old / line_base_new
+ * [n_pairs+1] (may be NULL) and *n_lines (lines of news) are always set; if cap < *n_lines the call returns TSM_E_CAPACITY
+ * (no diff run): size origin_out and call again.  added / removed / detail as tsm_diff_pairs_detail (detail may be NULL).
+ * Kernels: the diff of tsm_diff_pairs_marks, then k_blame (a warp per chain, longest chains first).
+ * tsm_diff_last_ms after this call: ms3 = { k_scan over both sides, k_diff_small, k_myers + k_myers_trace }; tsm_blame_last_ms:
+ * the k_blame launch. */
+typedef struct tsm_origin { int32_t change, line; } tsm_origin;
+int tsm_blame_pairs(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                    tsm_diff_detail* detail, const int32_t* prev, const int32_t* label, const tsm_origin* origin_in,
+                    const int64_t* in_base, int64_t* line_base_old, int64_t* line_base_new, tsm_origin* origin_out,
+                    int64_t cap, int64_t* n_lines, void* stream);
+int tsm_blame_last_ms(tsm_ctx* ctx, float* ms);
+
 /* S9 line / n-gram hashes (docs/SPEC.md section 3; SURVEY.md section 8a S9 - a design choice of the north star, attested by no
  * artefact of the package): the records of every line of every file, files in order, from ONE pass of the scan
  * kernel over the source.  line_base[n_files+1] and *n_lines are always filled; line_hash (SPEC section 3), line_end

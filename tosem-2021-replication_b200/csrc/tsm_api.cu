@@ -13,6 +13,7 @@
 #include "tsm_scan_walk.cuh"
 #include "tsm_reduce_kernels.cuh"
 #include "tsm_diff_kernels.cuh"
+#include "tsm_blame_kernels.cuh"
 #include "tsm_stmt_kernels.cuh"
 #include "tsm_lines_kernels.cuh"
 #include "tsm_similar_kernels.cuh"
@@ -93,6 +94,8 @@ struct tsm_ctx {
   uint8_t* h_diff = nullptr;               // 256 B pinned: what the diff path reads back between its kernels (Ctrl x 2, line totals, todo count)
   float diff_ms[3] = {0, 0, 0};            // k_scan over both sides, k_myers, k_myers_trace of the last diff
   float sim_ms[3] = {0, 0, 0};             // k_scan over both sides, sort / merge, k_similarity of the last tsm_similarity
+  cudaEvent_t blame_ev[2] = {};            // around k_blame (tsm_blame_last_ms)
+  float blame_ms = 0;
   struct HostSidePair* res_pair = nullptr; // sides kept in HBM by tsm_diff_upload
   static constexpr int kMaxSlabs = 64;
   tsm_file_stat* d_stats = nullptr;
@@ -196,14 +199,14 @@ static void build_elut(uint32_t* lut) {                  // operator patterns of
 
 static void free_res_pair(tsm_ctx* c);
 
-template <bool EMIT> static cudaError_t diff_small_smem() {   // the dynamic shared memory of the four k_diff_small sizes
-  cudaError_t e = cudaFuncSetAttribute(k_diff_small<DS1_HCAP, DS1_DCAP, DS1_WARPS, EMIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+template <int MODE> static cudaError_t diff_small_smem() {   // the dynamic shared memory of the four k_diff_small sizes
+  cudaError_t e = cudaFuncSetAttribute(k_diff_small<DS1_HCAP, DS1_DCAP, DS1_WARPS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)(DS1_WARPS * ds_warp_bytes(DS1_HCAP, DS1_DCAP)));
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_diff_small<DS2_HCAP, DS2_DCAP, DS2_WARPS, EMIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_diff_small<DS2_HCAP, DS2_DCAP, DS2_WARPS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                  (int)(DS2_WARPS * ds_warp_bytes(DS2_HCAP, DS2_DCAP)));
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_diff_small<DS3_HCAP, DS3_DCAP, DS3_WARPS, EMIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_diff_small<DS3_HCAP, DS3_DCAP, DS3_WARPS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                  (int)(DS3_WARPS * ds_warp_bytes(DS3_HCAP, DS3_DCAP)));
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_diff_small<DS4_HCAP, DS4_DCAP, DS4_WARPS, EMIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_diff_small<DS4_HCAP, DS4_DCAP, DS4_WARPS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                  (int)(DS4_WARPS * ds_warp_bytes(DS4_HCAP, DS4_DCAP)));
   return e;
 }
@@ -219,6 +222,7 @@ extern "C" void tsm_destroy(tsm_ctx* c) {
   if (c->ready_ev) cudaEventDestroy(c->ready_ev);
   if (c->order_ev) cudaEventDestroy(c->order_ev);
   for (cudaEvent_t e : c->diff_ev) if (e) cudaEventDestroy(e);
+  for (cudaEvent_t e : c->blame_ev) if (e) cudaEventDestroy(e);
   free_res_pair(c);
   cudaFree(c->d_cand); cudaFree(c->d_hev); cudaFree(c->d_aev);
   if (c->h_ctrl) cudaFreeHost(c->h_ctrl);
@@ -273,6 +277,7 @@ extern "C" int tsm_create(tsm_ctx** out, int device, int64_t max_arena_bytes, in
   if (rc == TSM_OK && cudaEventCreateWithFlags(&c->ready_ev, cudaEventDisableTiming) != cudaSuccess) rc = TSM_E_CUDA;
   if (rc == TSM_OK && cudaEventCreateWithFlags(&c->order_ev, cudaEventDisableTiming) != cudaSuccess) rc = TSM_E_CUDA;
   for (cudaEvent_t& e : c->diff_ev) if (rc == TSM_OK && cudaEventCreate(&e) != cudaSuccess) rc = TSM_E_CUDA;
+  for (cudaEvent_t& e : c->blame_ev) if (rc == TSM_OK && cudaEventCreate(&e) != cudaSuccess) rc = TSM_E_CUDA;
   A((void**)&c->d_stats, sizeof(tsm_file_stat) * (size_t)max_files);
   A((void**)&c->d_cand, sizeof(unsigned long long) * (size_t)c->max_events);
   if (rc == TSM_OK && cudaHostAlloc((void**)&c->h_ctrl, sizeof(Ctrl) + 64, cudaHostAllocDefault) != cudaSuccess) rc = TSM_E_CUDA;
@@ -296,7 +301,8 @@ extern "C" int tsm_create(tsm_ctx** out, int device, int64_t max_arena_bytes, in
         cudaMemcpyToSymbol(c_lut_b, lutb, sizeof lutb) != cudaSuccess ||
         cudaFuncSetAttribute(k_scan_t<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN2_SMEM) != cudaSuccess ||
         cudaFuncSetAttribute(k_scan_t<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN2_SMEM_B) != cudaSuccess ||
-        diff_small_smem<false>() != cudaSuccess || diff_small_smem<true>() != cudaSuccess ||
+        diff_small_smem<DIFF_PLAIN>() != cudaSuccess || diff_small_smem<DIFF_EMIT>() != cudaSuccess ||
+        diff_small_smem<DIFF_MARKS>() != cudaSuccess ||
         cudaFuncSetAttribute(k_sim_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SIM_SORT_SMEM) != cudaSuccess)
       rc = TSM_E_CUDA;
   }
@@ -948,8 +954,9 @@ static int pair_upload(const tsm_corpus* olds, const tsm_corpus* news, bool with
 // assertion lines).  A pair whose distance D needs more than TSM_DIFF_TRACE_MAX_INTS trace entries ((D+1)(D+2)/2) is
 // not traced: it is reported as ONE hunk (add / del / mod by its counts) with added_assert = removed_assert = -1
 // (tosemscan.h).  diff_ms[1] = k_diff_small, diff_ms[2] = the two kernels of the left-over pairs.  With `sink` (needs
-// `detail`) the EMIT variants of k_diff_small and k_myers_trace also list the changed assertion lines.
-template <bool EMIT>
+// `detail`) the DIFF_EMIT variants of k_diff_small and k_myers_trace also list the changed assertion lines, or, when the sink
+// has marks, the DIFF_MARKS variants mark the deleted and inserted lines.
+template <int MODE>
 static void launch_diff_small(tsm_ctx* c, const HostSide& A, const HostSide& B, int32_t n, const uint8_t* fa, const uint8_t* fb,
                               uint32_t* cnt, int32_t* const todo[4], long long* da, long long* dr, tsm_diff_detail* d_det,
                               const AssertSink& sink, cudaStream_t st) {
@@ -958,13 +965,13 @@ static void launch_diff_small(tsm_ctx* c, const HostSide& A, const HostSide& B, 
   static_assert(kSmem1 * 4 + 4 * 1024 <= 233472 && kSmem2 * 6 + 6 * 1024 <= 233472 && kSmem3 * 5 + 5 * 1024 <= 233472 &&
                 kSmem4 * 3 + 3 * 1024 <= 233472, "pairs per SM");
   // (the kernels' dynamic shared memory limits are raised per device in tsm_create)
-  k_diff_small<DS1_HCAP, DS1_DCAP, DS1_WARPS, EMIT><<<std::min((n + DS1_WARPS - 1) / DS1_WARPS, c->sms * 4), DS1_WARPS * 32, kSmem1, st>>>(
+  k_diff_small<DS1_HCAP, DS1_DCAP, DS1_WARPS, MODE><<<std::min((n + DS1_WARPS - 1) / DS1_WARPS, c->sms * 4), DS1_WARPS * 32, kSmem1, st>>>(
       A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, nullptr, nullptr, n, cnt + 4, da, dr, d_det, todo[0], cnt + 0, sink);
-  k_diff_small<DS2_HCAP, DS2_DCAP, DS2_WARPS, EMIT><<<std::min((n + DS2_WARPS - 1) / DS2_WARPS, c->sms * 6), DS2_WARPS * 32, kSmem2, st>>>(
+  k_diff_small<DS2_HCAP, DS2_DCAP, DS2_WARPS, MODE><<<std::min((n + DS2_WARPS - 1) / DS2_WARPS, c->sms * 6), DS2_WARPS * 32, kSmem2, st>>>(
       A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, todo[0], cnt + 0, n, cnt + 5, da, dr, d_det, todo[1], cnt + 1, sink);
-  k_diff_small<DS3_HCAP, DS3_DCAP, DS3_WARPS, EMIT><<<std::min(n, c->sms * 5), DS3_WARPS * 32, kSmem3, st>>>(
+  k_diff_small<DS3_HCAP, DS3_DCAP, DS3_WARPS, MODE><<<std::min(n, c->sms * 5), DS3_WARPS * 32, kSmem3, st>>>(
       A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, todo[1], cnt + 1, n, cnt + 6, da, dr, d_det, todo[2], cnt + 2, sink);
-  k_diff_small<DS4_HCAP, DS4_DCAP, DS4_WARPS, EMIT><<<std::min(n, c->sms * 3), DS4_WARPS * 32, kSmem4, st>>>(
+  k_diff_small<DS4_HCAP, DS4_DCAP, DS4_WARPS, MODE><<<std::min(n, c->sms * 3), DS4_WARPS * 32, kSmem4, st>>>(
       A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, todo[2], cnt + 2, n, cnt + 7, da, dr, d_det, todo[3], cnt + 3, sink);
 }
 
@@ -989,8 +996,10 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
   long long* dr = d_rem.as<long long>();
   int32_t* const todo_lists[4] = {d_todo1.as<int32_t>(), d_todo2.as<int32_t>(), d_todo3.as<int32_t>(), d_todo.as<int32_t>()};
   CU(cudaEventRecord(c->diff_ev[2], st));
-  if (sink) launch_diff_small<true>(c, A, B, n, fa, fb, cnt, todo_lists, da, dr, d_det, *sink, st);
-  else launch_diff_small<false>(c, A, B, n, fa, fb, cnt, todo_lists, da, dr, d_det, AssertSink{}, st);
+  const int mode = !sink ? DIFF_PLAIN : sink->mark[0] ? DIFF_MARKS : DIFF_EMIT;
+  if (mode == DIFF_MARKS) launch_diff_small<DIFF_MARKS>(c, A, B, n, fa, fb, cnt, todo_lists, da, dr, d_det, *sink, st);
+  else if (mode == DIFF_EMIT) launch_diff_small<DIFF_EMIT>(c, A, B, n, fa, fb, cnt, todo_lists, da, dr, d_det, *sink, st);
+  else launch_diff_small<DIFF_PLAIN>(c, A, B, n, fa, fb, cnt, todo_lists, da, dr, d_det, AssertSink{}, st);
   CU(cudaEventRecord(c->diff_ev[3], st));
   CU(cudaGetLastError());
   uint32_t* pin_nt = reinterpret_cast<uint32_t*>(c->h_diff + 80);
@@ -1062,13 +1071,18 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
                        cudaMemcpyHostToDevice, st));
     CU(cudaEventRecord(c->diff_ev[4], st));
     const unsigned grid = ((p1 - p0) * 32 + 127) / 128;
-    if (sink)
-      k_myers_trace<true><<<grid, 128, 0, st>>>(
+    if (mode == DIFF_MARKS)
+      k_myers_trace<DIFF_MARKS><<<grid, 128, 0, st>>>(
+          A.d.line_hash, A.d.line_base, A.d.line_flag, B.d.line_hash, B.d.line_base, B.d.line_flag, (int32_t)p0, (int32_t)(p1 - p0),
+          d_trace.as<int32_t>(), d_tbase.as<unsigned long long>(), d_add.as<long long>(), d_rem.as<long long>(),
+          (long long)TSM_DIFF_TRACE_MAX_D, d_detail.as<tsm_diff_detail>(), d_todo.as<int32_t>(), *sink);
+    else if (mode == DIFF_EMIT)
+      k_myers_trace<DIFF_EMIT><<<grid, 128, 0, st>>>(
           A.d.line_hash, A.d.line_base, A.d.line_flag, B.d.line_hash, B.d.line_base, B.d.line_flag, (int32_t)p0, (int32_t)(p1 - p0),
           d_trace.as<int32_t>(), d_tbase.as<unsigned long long>(), d_add.as<long long>(), d_rem.as<long long>(),
           (long long)TSM_DIFF_TRACE_MAX_D, d_detail.as<tsm_diff_detail>(), d_todo.as<int32_t>(), *sink);
     else
-      k_myers_trace<false><<<grid, 128, 0, st>>>(
+      k_myers_trace<DIFF_PLAIN><<<grid, 128, 0, st>>>(
           A.d.line_hash, A.d.line_base, A.d.line_flag, B.d.line_hash, B.d.line_base, B.d.line_flag, (int32_t)p0, (int32_t)(p1 - p0),
           d_trace.as<int32_t>(), d_tbase.as<unsigned long long>(), d_add.as<long long>(), d_rem.as<long long>(),
           (long long)TSM_DIFF_TRACE_MAX_D, d_detail.as<tsm_diff_detail>(), d_todo.as<int32_t>(), AssertSink{});
@@ -1268,6 +1282,171 @@ extern "C" int tsm_diff_resident_asserts(tsm_ctx* c, int64_t* added, int64_t* re
 extern "C" int tsm_diff_last_ms(tsm_ctx* c, float* ms3) {
   if (!c || !ms3) return TSM_E_ARG;
   for (int i = 0; i < 3; ++i) ms3[i] = c->diff_ms[i];
+  return TSM_OK;
+}
+
+// ------------------------------------------------------------------------------------- SPEC section 14 line provenance
+// The line records of both uploaded sides with line_base on the host (diff_ms[0] = k_scan over both); line_base of each
+// side copied to base_old / base_new when given.
+static int marks_records(tsm_ctx* c, HostSidePair& P, int64_t* base_old, int64_t* base_new, cudaStream_t st) {
+  c->diff_ms[0] = 0;
+  P.A.launches = P.B.launches = 0;
+  HostSide* both[2] = {&P.A, &P.B};
+  const int rc = sides_records(c, both, 2, st, &c->diff_ms[0], true);
+  if (rc != TSM_OK) return rc;
+  const size_t bytes = sizeof(int64_t) * ((size_t)P.n + 1);
+  if (base_old) memcpy(base_old, P.A.base.data(), bytes);
+  if (base_new) memcpy(base_new, P.B.base.data(), bytes);
+  return TSM_OK;
+}
+
+// diff_core with the DIFF_MARKS kernels over two zeroed byte arrays, one per line of each side.  The marks come from the
+// paths of the detail (pure hunks, backtrack), so the detail is computed also when the caller does not want it.
+static int marks_diff(tsm_ctx* c, HostSidePair& P, int64_t* added, int64_t* removed, tsm_diff_detail* detail, DevBuf& del,
+                      DevBuf& ins, cudaStream_t st) {
+  std::vector<tsm_diff_detail> own;
+  if (!detail) { own.resize((size_t)P.n); detail = own.data(); }
+  if (!del.alloc((size_t)P.A.total) || !ins.alloc((size_t)P.B.total)) return TSM_E_CUDA;
+  CU(cudaMemsetAsync(del.p, 0, (size_t)P.A.total, st));
+  CU(cudaMemsetAsync(ins.p, 0, (size_t)P.B.total, st));
+  AssertSink sink{};
+  sink.mark[0] = del.as<uint8_t>(); sink.mark[1] = ins.as<uint8_t>();
+  return diff_core(c, P.A, P.B, P.n, added, removed, detail, st, &sink);
+}
+
+extern "C" int tsm_diff_pairs_marks(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                                    tsm_diff_detail* detail, tsm_line_marks* mk, void* stream) {
+  if (!c || !olds || !news || !added || !removed || !mk || !mk->line_base_old || !mk->line_base_new || olds->n_files != news->n_files)
+    return TSM_E_ARG;
+  const int32_t n = olds->n_files;
+  mk->n_old = mk->n_new = 0;
+  if (n == 0) { mk->line_base_old[0] = mk->line_base_new[0] = 0; return TSM_OK; }
+  int rc = check_sides({olds, news}, n, true);
+  if (rc != TSM_OK) return rc;
+  CU(cudaSetDevice(c->device));
+  PoolScope pool_scope(&c->pool);
+  cudaStream_t st = (cudaStream_t)stream;
+  CallOrder order(c, st);
+  CU(order.wait());
+  HostSidePair P;
+  SyncGuard guard(st);
+  rc = pair_upload(olds, news, false, P, st);
+  if (rc == TSM_OK) rc = marks_records(c, P, mk->line_base_old, mk->line_base_new, st);
+  if (rc != TSM_OK) return rc;
+  mk->n_old = (int64_t)P.A.total; mk->n_new = (int64_t)P.B.total;
+  if (mk->del_cap < mk->n_old || mk->ins_cap < mk->n_new) return TSM_E_CAPACITY;
+  if ((mk->n_old && !mk->del) || (mk->n_new && !mk->ins)) return TSM_E_ARG;
+  DevBuf del, ins;
+  rc = marks_diff(c, P, added, removed, detail, del, ins, st);
+  if (rc != TSM_OK) return rc;
+  if (mk->n_old) CU(cudaMemcpyAsync(mk->del, del.p, (size_t)mk->n_old, cudaMemcpyDeviceToHost, st));
+  if (mk->n_new) CU(cudaMemcpyAsync(mk->ins, ins.p, (size_t)mk->n_new, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TSM_OK;
+}
+
+// Provenance: the checks of prev and the line counts on the host, the marks diff, then ONE k_blame launch over the chains
+// (pair lists in chain order, longest chain first: the long chains are the tail of the launch).
+extern "C" int tsm_blame_pairs(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                               tsm_diff_detail* detail, const int32_t* prev, const int32_t* label, const tsm_origin* origin_in,
+                               const int64_t* in_base, int64_t* line_base_old, int64_t* line_base_new, tsm_origin* origin_out,
+                               int64_t cap, int64_t* n_lines, void* stream) {
+  if (!c || !olds || !news || !added || !removed || !prev || !label || !in_base || !n_lines || olds->n_files != news->n_files)
+    return TSM_E_ARG;
+  const int32_t n = olds->n_files;
+  *n_lines = 0;
+  c->blame_ms = 0;
+  if (n == 0) {
+    if (line_base_old) line_base_old[0] = 0;
+    if (line_base_new) line_base_new[0] = 0;
+    return TSM_OK;
+  }
+  std::vector<int32_t> next((size_t)n, -1);
+  if (in_base[0] < 0) return TSM_E_ARG;
+  for (int32_t i = 0; i < n; ++i) {
+    const int32_t p = prev[i];
+    if (p < -1 || p >= i || in_base[i + 1] < in_base[i]) return TSM_E_ARG;
+    if (p >= 0) {
+      if (next[(size_t)p] != -1) return TSM_E_ARG;         // a new side continues one chain only
+      next[(size_t)p] = i;
+    } else if (in_base[i + 1] > in_base[i] && !origin_in) {
+      return TSM_E_ARG;
+    }
+  }
+  int rc = check_sides({olds, news}, n, true);
+  if (rc != TSM_OK) return rc;
+  CU(cudaSetDevice(c->device));
+  PoolScope pool_scope(&c->pool);
+  cudaStream_t st = (cudaStream_t)stream;
+  CallOrder order(c, st);
+  CU(order.wait());
+  HostSidePair P;
+  SyncGuard guard(st);
+  rc = pair_upload(olds, news, false, P, st);
+  if (rc == TSM_OK) rc = marks_records(c, P, line_base_old, line_base_new, st);
+  if (rc != TSM_OK) return rc;
+  *n_lines = (int64_t)P.B.total;
+  const std::vector<unsigned long long>& la = P.A.base;
+  const std::vector<unsigned long long>& lb = P.B.base;
+  for (int32_t i = 0; i < n; ++i) {                        // old side i = new side prev[i], or the head's range of origin_in
+    const unsigned long long want = prev[i] >= 0 ? lb[(size_t)prev[i] + 1] - lb[(size_t)prev[i]] : (unsigned long long)(in_base[i + 1] - in_base[i]);
+    if (la[(size_t)i + 1] - la[(size_t)i] != want) return TSM_E_ARG;
+  }
+  if (cap < *n_lines) return TSM_E_CAPACITY;
+  if (*n_lines && !origin_out) return TSM_E_ARG;
+  DevBuf del, ins;
+  rc = marks_diff(c, P, added, removed, detail, del, ins, st);
+  if (rc != TSM_OK) return rc;
+  // chains: heads in pair order, then stably by length, longest first
+  std::vector<int32_t> heads, len;
+  for (int32_t i = 0; i < n; ++i)
+    if (prev[i] < 0) {
+      int32_t k = 0;
+      for (int32_t j = i; j >= 0; j = next[(size_t)j]) ++k;
+      heads.push_back(i); len.push_back(k);
+    }
+  std::vector<int32_t> order_h(heads.size());
+  for (size_t h = 0; h < heads.size(); ++h) order_h[h] = (int32_t)h;
+  std::stable_sort(order_h.begin(), order_h.end(), [&](int32_t x, int32_t y) { return len[(size_t)x] > len[(size_t)y]; });
+  const int32_t n_chains = (int32_t)heads.size();
+  std::vector<int32_t> chain_pairs, chain_start;
+  chain_pairs.reserve((size_t)n); chain_start.reserve((size_t)n_chains + 1);
+  for (int32_t h : order_h) {
+    chain_start.push_back((int32_t)chain_pairs.size());
+    for (int32_t j = heads[(size_t)h]; j >= 0; j = next[(size_t)j]) chain_pairs.push_back(j);
+  }
+  chain_start.push_back((int32_t)chain_pairs.size());
+  const size_t n_in = (size_t)in_base[n];
+  DevBuf d_prev, d_label, d_head, d_in_base, d_pairs, d_start, d_work, d_keep, d_out;
+  if (!d_prev.alloc(sizeof(int32_t) * (size_t)n) || !d_label.alloc(sizeof(int32_t) * (size_t)n) ||
+      !d_head.alloc(sizeof(tsm_origin) * n_in) || !d_in_base.alloc(sizeof(int64_t) * ((size_t)n + 1)) ||
+      !d_pairs.alloc(sizeof(int32_t) * (size_t)n) || !d_start.alloc(sizeof(int32_t) * ((size_t)n_chains + 1)) || !d_work.alloc(16) ||
+      !d_keep.alloc(sizeof(tsm_origin) * (size_t)P.A.total) || !d_out.alloc(sizeof(tsm_origin) * (size_t)P.B.total))
+    return TSM_E_CUDA;
+  CU(cudaMemcpyAsync(d_prev.p, prev, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d_label.p, label, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
+  if (n_in) CU(cudaMemcpyAsync(d_head.p, origin_in, sizeof(tsm_origin) * n_in, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d_in_base.p, in_base, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d_pairs.p, chain_pairs.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d_start.p, chain_start.data(), sizeof(int32_t) * ((size_t)n_chains + 1), cudaMemcpyHostToDevice, st));
+  CU(cudaMemsetAsync(d_work.p, 0, 16, st));
+  CU(cudaEventRecord(c->blame_ev[0], st));
+  k_blame<<<std::min((n_chains + 7) / 8, c->sms * 8), 256, 0, st>>>(
+      P.A.d.line_base, P.B.d.line_base, del.as<uint8_t>(), ins.as<uint8_t>(), d_prev.as<int32_t>(), d_label.as<int32_t>(),
+      d_head.as<tsm_origin>(), d_in_base.as<long long>(), d_pairs.as<int32_t>(), d_start.as<int32_t>(), n_chains, d_work.as<uint32_t>(),
+      d_keep.as<tsm_origin>(), d_out.as<tsm_origin>());
+  CU(cudaEventRecord(c->blame_ev[1], st));
+  CU(cudaGetLastError());
+  c->launches++;
+  if (*n_lines) CU(cudaMemcpyAsync(origin_out, d_out.p, sizeof(tsm_origin) * (size_t)*n_lines, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  c->blame_ms = elapsed_ms(c->blame_ev[0], c->blame_ev[1]);
+  return TSM_OK;
+}
+
+extern "C" int tsm_blame_last_ms(tsm_ctx* c, float* ms) {
+  if (!c || !ms) return TSM_E_ARG;
+  *ms = c->blame_ms;
   return TSM_OK;
 }
 

@@ -13,8 +13,9 @@
 //   k_myers         warp per pair: the same search with V in global scratch (any size)
 //   k_myers_trace   the same with one row of V kept per D in global memory, then the backtrack
 //
-// k_diff_small and k_myers_trace have a second variant (EMIT) that also lists the changed assertion lines (SPEC section 8)
-// for k_classify; the variant without it is the same code as before the lists existed.
+// k_diff_small and k_myers_trace have two more variants (DiffMode): DIFF_EMIT also lists the changed assertion lines
+// (SPEC section 8) for k_classify, DIFF_MARKS marks every deleted and inserted line (SPEC section 14) for k_blame.  The
+// variant with neither is the same code as before they existed.
 #pragma once
 #include "tsm_scan_kernels.cuh"
 
@@ -30,15 +31,20 @@ struct DiffSide {                   // one corpus (old or new) on the device
   uint8_t* line_flag;               // [total lines] 1 = assertion line (SPEC section 4); NULL = not wanted
 };
 
-// Where the EMIT variants put the changed assertion lines: side 0 = deleted lines of `old`, side 1 = inserted lines of `new`,
+// Where the DIFF_EMIT variants put the changed assertion lines: side 0 = deleted lines of `old`, side 1 = inserted lines of `new`,
 // each as (pair << 32 | file-relative line start), the candidate format of k_classify.  n[s] is the n_cand of the Ctrl that
 // k_classify reads for side s; it counts every line, also those past cap[s], so that the host sees an overflow.
+// The DIFF_MARKS variants use mark[] only: mark[0][g] = 1 for every deleted line g of `old`, mark[1][g] = 1 for every
+// inserted line g of `new` (global line indices, zeroed by the host).
 struct AssertSink {
   unsigned long long* list[2];
   uint32_t* n[2];
   uint32_t cap[2];
   const uint32_t* line_end[2];      // DiffSide::line_end of each side
+  uint8_t* mark[2];
 };
+
+enum DiffMode { DIFF_PLAIN = 0, DIFF_EMIT = 1, DIFF_MARKS = 2 };
 
 // Candidate of line g (global line index) of pair pr, whose file starts at line `first` of its side.
 __device__ __forceinline__ unsigned long long sink_key(const AssertSink& s, int side, int pr, unsigned long long first,
@@ -61,6 +67,11 @@ __device__ __forceinline__ void sink_run(const AssertSink& s, int side, int pr, 
     const uint32_t slot = base + (uint32_t)__popc(bal & ((1u << lane) - 1u));
     if (f && slot < s.cap[side]) s.list[side][slot] = sink_key(s, side, pr, first, g0 + (unsigned long long)i);
   }
+}
+
+// Mark the run [0, cnt) of p: the whole warp.
+__device__ __forceinline__ void mark_run(uint8_t* p, int cnt, int lane) {
+  for (int i = lane; i < cnt; i += 32) p[i] = 1;
 }
 
 // Follow a diagonal while the lines are equal.  Four positions are compared per round trip to HBM / L2 (the loads
@@ -97,7 +108,7 @@ __host__ __device__ constexpr uint32_t ds_warp_bytes(int hcap, int dcap) { retur
 //     is finished by the whole warp, 32 lines per step: a long unchanged stretch costs a few ballots, not hundreds of
 //     dependent loads;
 //   * the assertion-line flags of the middle are staged next to the hashes: the backtrack reads shared memory only.
-template <int HCAP, int DCAP, bool EMIT>
+template <int HCAP, int DCAP, int MODE>
 __device__ __forceinline__ bool diff_one(uint8_t* mine, int pr, int lane,
     const unsigned long long* ha, const unsigned long long* la, const uint8_t* fa,
     const unsigned long long* hb, const unsigned long long* lb, const uint8_t* fb,
@@ -141,7 +152,7 @@ __device__ __forceinline__ bool diff_one(uint8_t* mine, int pr, int lane,
       for (int k = 16; k; k >>= 1) { ca += __shfl_xor_sync(0xffffffffu, ca, k); cb += __shfl_xor_sync(0xffffffffu, cb, k); }
       if (n) { h_del = 1; r_as = ca; }
       if (m) { h_add = 1; a_as = cb; }
-      if constexpr (EMIT) {
+      if constexpr (MODE == DIFF_EMIT) {
         sink_run(sink, 0, pr, la[pr], la[pr] + pre, qa, n, lane);
         sink_run(sink, 1, pr, lb[pr], lb[pr] + pre, qb, m, lane);
       }
@@ -229,15 +240,33 @@ __device__ __forceinline__ bool diff_one(uint8_t* mine, int pr, int lane,
         in_hunk = true;
         if (down) { has_add = true; a_as += sfb[py] != 0; }
         else { has_del = true; r_as += sfa[px] != 0; }
-        if constexpr (EMIT) {
+        if constexpr (MODE == DIFF_EMIT) {
           if (down && sfb[py]) sink_put(sink, 1, sink_key(sink, 1, pr, lb[pr], lb[pr] + pre + py));
           if (!down && sfa[px]) sink_put(sink, 0, sink_key(sink, 0, pr, la[pr], la[pr] + pre + px));
+        }
+        if constexpr (MODE == DIFF_MARKS) {                // bit 1 of the staged flag, written out by the warp below
+          if (down) sfb[py] |= 2;
+          else sfa[px] |= 2;
         }
         x = px; y = py;
       }
       if (in_hunk) { if (has_add && has_del) ++h_mod; else if (has_add) ++h_add; else ++h_del; }
     }
+    if constexpr (MODE == DIFF_MARKS) {
+      __syncwarp();
+      uint8_t* ma = sink.mark[0] + la[pr] + pre;
+      uint8_t* mb = sink.mark[1] + lb[pr] + pre;
+#pragma unroll 1
+      for (int i = lane; i < n; i += 32) if (sfa[i] & 2) ma[i] = 1;
+#pragma unroll 1
+      for (int i = lane; i < m; i += 32) if (sfb[i] & 2) mb[i] = 1;
+    }
   }
+  if constexpr (MODE == DIFF_MARKS)
+    if (n == 0 || m == 0) {
+      mark_run(sink.mark[0] + la[pr] + pre, n, lane);
+      mark_run(sink.mark[1] + lb[pr] + pre, m, lane);
+    }
   if (lane == 0) {
     const long long lcs = ((long long)(n + m) - D) / 2 + pre + suf;
     removed[pr] = n0 - lcs;
@@ -249,7 +278,7 @@ __device__ __forceinline__ bool diff_one(uint8_t* mine, int pr, int lane,
 
 // Persistent warps, pairs handed out by an atomic counter (their cost varies by two orders of magnitude).  The pairs
 // are todo_in[0 .. *n_in) when todo_in is given, else 0 .. n_all; what this size cannot finish goes to todo_out.
-template <int HCAP, int DCAP, int WARPS, bool EMIT>
+template <int HCAP, int DCAP, int WARPS, int MODE>
 __global__ void __launch_bounds__(WARPS * 32) k_diff_small(
     const unsigned long long* ha, const unsigned long long* la, const uint8_t* fa,
     const unsigned long long* hb, const unsigned long long* lb, const uint8_t* fb,
@@ -265,7 +294,7 @@ __global__ void __launch_bounds__(WARPS * 32) k_diff_small(
     slot = __shfl_sync(0xffffffffu, slot, 0);
     if (slot >= limit) return;
     const int pr = todo_in ? todo_in[slot] : (int)slot;
-    if (!diff_one<HCAP, DCAP, EMIT>(mine, pr, lane, ha, la, fa, hb, lb, fb, added, removed, detail, sink) && lane == 0)
+    if (!diff_one<HCAP, DCAP, MODE>(mine, pr, lane, ha, la, fa, hb, lb, fb, added, removed, detail, sink) && lane == 0)
       todo_out[atomicAdd(n_out, 1u)] = pr;
   }
 }
@@ -333,7 +362,8 @@ __global__ void k_myers(const unsigned long long* ha, const unsigned long long* 
 // Hunks and their classification (docs/SPEC.md section 8): the same search with one row of V kept per D
 // (row d holds the diagonals -d, -d+2, ..., d), then the canonical backtrack by lane 0.
 // trace_base[pr] = first int of pair pr's rows, sized (D+1)(D+2)/2 from the distances of k_myers.
-template <bool EMIT>
+// The DIFF_MARKS variant marks the whole middle (between the common prefix and suffix) of a pair it does not trace.
+template <int MODE>
 __global__ void k_myers_trace(const unsigned long long* ha, const unsigned long long* la, const uint8_t* fa,
                               const unsigned long long* hb, const unsigned long long* lb, const uint8_t* fb,
                               int32_t pair0, int32_t n_pairs, int32_t* trace, const unsigned long long* trace_base,
@@ -342,7 +372,8 @@ __global__ void k_myers_trace(const unsigned long long* ha, const unsigned long 
   const int slot = pair0 + ((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (slot >= pair0 + n_pairs) return;
   const int pr = todo ? todo[slot] : slot;                // trace_base is indexed by slot
-  if (added[pr] + removed[pr] > max_d) return;             // too far apart to keep the rows of V: the host reports one hunk
+  if constexpr (MODE != DIFF_MARKS)
+    if (added[pr] + removed[pr] > max_d) return;           // too far apart to keep the rows of V: the host reports one hunk
   const unsigned long long* a = ha + la[pr];
   const unsigned long long* b = hb + lb[pr];
   const uint8_t* qa = fa + la[pr];
@@ -364,6 +395,12 @@ __global__ void k_myers_trace(const unsigned long long* ha, const unsigned long 
     suf += 32;
   }
   n -= suf; m -= suf;
+  if constexpr (MODE == DIFF_MARKS)
+    if (added[pr] + removed[pr] > max_d) {
+      mark_run(sink.mark[0] + la[pr] + pre, n, lane);
+      mark_run(sink.mark[1] + lb[pr] + pre, m, lane);
+      return;
+    }
   long long h_add = 0, h_del = 0, h_mod = 0, a_as = 0, r_as = 0;
   if (n == 0 || m == 0) {                                 // one pure hunk (or none)
     int ca = 0, cb = 0;
@@ -373,9 +410,13 @@ __global__ void k_myers_trace(const unsigned long long* ha, const unsigned long 
     for (int k = 16; k; k >>= 1) { ca += __shfl_xor_sync(0xffffffffu, ca, k); cb += __shfl_xor_sync(0xffffffffu, cb, k); }
     if (n) { h_del = 1; r_as = ca; }
     if (m) { h_add = 1; a_as = cb; }
-    if constexpr (EMIT) {
+    if constexpr (MODE == DIFF_EMIT) {
       sink_run(sink, 0, pr, la[pr], la[pr] + pre, qa, n, lane);
       sink_run(sink, 1, pr, lb[pr], lb[pr] + pre, qb, m, lane);
+    }
+    if constexpr (MODE == DIFF_MARKS) {
+      mark_run(sink.mark[0] + la[pr] + pre, n, lane);
+      mark_run(sink.mark[1] + lb[pr] + pre, m, lane);
     }
   } else {
     int32_t* R = trace + trace_base[slot];
@@ -418,9 +459,13 @@ __global__ void k_myers_trace(const unsigned long long* ha, const unsigned long 
         in_hunk = true;
         if (down) { has_add = true; a_as += qb[py] != 0; }
         else { has_del = true; r_as += qa[px] != 0; }
-        if constexpr (EMIT) {
+        if constexpr (MODE == DIFF_EMIT) {
           if (down && qb[py]) sink_put(sink, 1, sink_key(sink, 1, pr, lb[pr], lb[pr] + pre + py));
           if (!down && qa[px]) sink_put(sink, 0, sink_key(sink, 0, pr, la[pr], la[pr] + pre + px));
+        }
+        if constexpr (MODE == DIFF_MARKS) {
+          if (down) sink.mark[1][lb[pr] + pre + py] = 1;
+          else sink.mark[0][la[pr] + pre + px] = 1;
         }
         x = px; y = py;
       }

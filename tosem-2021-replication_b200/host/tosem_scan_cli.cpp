@@ -1287,15 +1287,21 @@ static void pair_renames(tsm_ctx* ctx, std::vector<Change>& changes, const Loade
   changes.swap(kept);
 }
 
+// What runs instead of tsm_diff_pairs_detail on a batch (blame): the changes [r0, r1), of which idx were packed (the others are
+// binary and skipped), the two sides, and added / removed / detail to fill.
+using BatchFn = std::function<void(tsm_ctx*, size_t r0, size_t r1, const std::vector<size_t>& idx, const tsm_corpus&, const tsm_corpus&,
+                                   int64_t*, int64_t*, tsm_diff_detail*)>;
+
 // The diff of an ordered list of changes of `n_steps` steps, after --find-renames pairing when rename_pct >= 0: binary files
-// skipped, batches of at most kBatch bytes per side (and 65 535 steps, a step being one group of the assertion tables),
-// one tsm_diff_pairs_detail or diff_asserts call per batch.  Every row starts with the `lead(step)` cells named `lead_head`;
-// the --assert-churn rows with the first `churn_lead` of them.  --out has a row for every diffed change when `zero_rows`,
-// else only for those that change a line or pair a rename.
+// skipped, batches of at most batch_bytes bytes per side (and 65 535 steps, a step being one group of the assertion tables),
+// one tsm_diff_pairs_detail or diff_asserts call per batch (or `pairs`, when given).  Every row starts with the `lead(step)`
+// cells named `lead_head`; the --assert-churn rows with the first `churn_lead` of them.  --out has a row for every diffed change
+// when `zero_rows`, else only for those that change a line or pair a rename.
 static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, const Loader& load, int rename_pct, bool zero_rows,
                                  const std::vector<std::string>& lead_head, size_t churn_lead,
                                  const std::function<std::vector<std::string>(size_t)>& lead, const std::string& out_path,
-                                 const std::string& asserts_path, const std::string& churn_path) {
+                                 const std::string& asserts_path, const std::string& churn_path, int64_t batch_bytes = kBatch,
+                                 const BatchFn* pairs = nullptr) {
   ChangeTotals t(n_steps);
   tsm_ctx* ctx = nullptr;
   ck(tsm_create(&ctx, 0, 1 << 20, 16, 1, 0), "tsm_create");
@@ -1322,7 +1328,7 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
     std::vector<size_t> idx;
     int64_t so = 0, sn = 0;
     size_t steps = 0;
-    for (r1 = r0; r1 < changes.size() && so < kBatch && sn < kBatch; ++r1) {
+    for (r1 = r0; r1 < changes.size() && so < batch_bytes && sn < batch_bytes; ++r1) {
       const Change& c = changes[r1];
       if (want_asserts && (r1 == r0 || c.step != changes[r1 - 1].step) && ++steps > 65535) break;
       std::vector<uint8_t> x = c.o >= 0 ? load(c.o) : std::vector<uint8_t>(), y = c.n >= 0 ? load(c.n) : std::vector<uint8_t>();
@@ -1332,6 +1338,7 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
       blobs[0].push_back(std::move(x)); blobs[1].push_back(std::move(y)); idx.push_back(r1);
     }
     const size_t n = idx.size();
+    if (!n && pairs) (*pairs)(ctx, r0, r1, idx, tsm_corpus{}, tsm_corpus{}, nullptr, nullptr, nullptr);
     if (!n) continue;
     Batch S[2];
     for (int s = 0; s < 2; ++s) {
@@ -1356,7 +1363,9 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
     std::vector<int64_t> added(n), removed(n);
     std::vector<tsm_diff_detail> det(n);
     ChangedAsserts chg;
-    if (!want_asserts) {
+    if (pairs) {
+      (*pairs)(ctx, r0, r1, idx, ca, cn, added.data(), removed.data(), det.data());
+    } else if (!want_asserts) {
       ck(tsm_diff_pairs_detail(ctx, &ca, &cn, added.data(), removed.data(), det.data(), nullptr), "tsm_diff_pairs_detail");
     } else {
       diff_asserts(ctx, ca, cn, added.data(), removed.data(), det.data(), chg);
@@ -1471,17 +1480,13 @@ static void tree_diff(gitstore::Store& gs, const gitstore::Oid* a, const gitstor
   }
 }
 
-// --dry-run: no GPU - the rows carry the object names, sizes and an FNV-1a checksum of both blobs instead of the counts
-// (what the CPU tests compare with `git diff-tree` / `git cat-file`).
-static int cmd_history(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files, const std::string& out_path,
-                       bool dry_run, const std::string& asserts_path, const std::string& churn_path, int rename_pct) {
-  gitstore::Store gs;
-  std::string err;
-  if (!gs.open(repo, err)) die(err);
+// The first-parent chain of `rev` (at most max_commits commits; all when 0), oldest first, and the changed selected files of
+// every commit against its parent, as changes of the commit's place in the chain; `objs` names the blobs of the changes.
+struct Step { gitstore::Oid id; gitstore::Commit c; };
+static void history_walk(gitstore::Store& gs, const std::string& rev, int64_t max_commits, bool all_files, std::vector<Step>& chain,
+                         std::vector<gitstore::Oid>& objs, std::vector<Change>& changes) {
   gitstore::Oid head;
   if (!gs.resolve(rev, head)) die("cannot resolve revision " + rev);
-  struct Step { gitstore::Oid id; gitstore::Commit c; };
-  std::vector<Step> chain;
   for (gitstore::Oid id = head; max_commits <= 0 || (int64_t)chain.size() < max_commits;) {
     Step st{id, {}};
     if (!gs.commit(id, st.c)) die("unreadable commit " + id.hex());
@@ -1490,8 +1495,6 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
     id = st.c.parents[0];
   }
   std::reverse(chain.begin(), chain.end());                 // oldest first
-  std::vector<gitstore::Oid> objs;
-  std::vector<Change> changes;
   for (size_t i = 0; i < chain.size(); ++i) {
     gitstore::Commit parent;
     const bool has_parent = !chain[i].c.parents.empty();
@@ -1499,6 +1502,19 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
     if (has_parent && parent.tree == chain[i].c.tree) continue;
     tree_diff(gs, has_parent ? &parent.tree : nullptr, &chain[i].c.tree, "", all_files, i, objs, changes);
   }
+}
+
+// --dry-run: no GPU - the rows carry the object names, sizes and an FNV-1a checksum of both blobs instead of the counts
+// (what the CPU tests compare with `git diff-tree` / `git cat-file`).
+static int cmd_history(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files, const std::string& out_path,
+                       bool dry_run, const std::string& asserts_path, const std::string& churn_path, int rename_pct) {
+  gitstore::Store gs;
+  std::string err;
+  if (!gs.open(repo, err)) die(err);
+  std::vector<Step> chain;
+  std::vector<gitstore::Oid> objs;
+  std::vector<Change> changes;
+  history_walk(gs, rev, max_commits, all_files, chain, objs, changes);
   auto load = [&](int64_t s) {
     gitstore::Object x;
     if (!gs.read(objs[(size_t)s], x) || x.type != gitstore::OBJ_BLOB) die("unreadable blob " + objs[(size_t)s].hex());
@@ -1544,6 +1560,204 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
   return 0;
 }
 
+// ---------------------------------------------------------------------------------- line provenance (docs/SPEC.md section 14)
+// `tosem-scan blame <repo>`: the commit, path and line that introduced every line of the selected files at a revision.  The
+// walk, the tree diff, the rename pairing and the batch loop are those of `history`; each batch of changes goes through
+// tsm_blame_pairs, a pair continuing the chain of the batch's last pair that wrote its old path, or starting from the origins
+// the host keeps per live path between batches.  An origin's `change` is an index into `owners`: (commit of the window, or -1
+// for the boundary commit P0, and the path in that commit).
+
+static int64_t count_lines(const std::vector<uint8_t>& v) {                 // docs/SPEC.md section 2
+  int64_t n = std::count(v.begin(), v.end(), (uint8_t)'\n');
+  return n + (!v.empty() && v.back() != '\n');
+}
+
+// The origins of one live path: `org`, or (lazy) every line of blob `obj` with the origin (owner, line).
+struct PathState { std::vector<tsm_origin> org; int32_t owner = -1; int64_t obj = -1; };
+
+static int cmd_blame(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files, int rename_pct,
+                     int64_t batch_bytes, const std::string& out_path, const std::string& asserts_path) {
+  gitstore::Store gs;
+  std::string err;
+  if (!gs.open(repo, err)) die(err);
+  std::vector<Step> chain;
+  std::vector<gitstore::Oid> objs;
+  std::vector<Change> changes;
+  history_walk(gs, rev, max_commits, all_files, chain, objs, changes);
+  const bool cut = !chain.empty() && !chain[0].c.parents.empty();          // the window does not reach the root
+  Step p0{};
+  if (cut) { p0.id = chain[0].c.parents[0]; if (!gs.commit(p0.id, p0.c)) die("unreadable commit " + p0.id.hex()); }
+  auto load = [&](int64_t s) {
+    gitstore::Object x;
+    if (!gs.read(objs[(size_t)s], x) || x.type != gitstore::OBJ_BLOB) die("unreadable blob " + objs[(size_t)s].hex());
+    return std::move(x.data);
+  };
+  struct Owner { int64_t step; std::string path; };
+  std::vector<Owner> owners;
+  std::map<std::pair<int64_t, std::string>, int32_t> owner_id;
+  auto owner = [&](int64_t step, const std::string& path) {
+    auto it = owner_id.find({step, path});
+    if (it != owner_id.end()) return it->second;
+    owners.push_back({step, path});
+    return owner_id[{step, path}] = (int32_t)owners.size() - 1;
+  };
+  auto lazy = [&](const PathState& st, const std::vector<uint8_t>* bytes) {   // the origins of a lazy state
+    std::vector<tsm_origin> v;
+    const int64_t n = count_lines(bytes ? *bytes : load(st.obj));
+    for (int64_t j = 0; j < n; ++j) v.push_back({st.owner, (int32_t)(j + 1)});
+    return v;
+  };
+  std::map<std::string, PathState> live;                   // host state between batches
+  int64_t blamed_pairs = 0;
+  BatchFn run = [&](tsm_ctx* ctx, size_t r0, size_t r1, const std::vector<size_t>& idx, const tsm_corpus& ca, const tsm_corpus& cn,
+                    int64_t* added, int64_t* removed, tsm_diff_detail* det) {
+    // the batch's view of every path it touches: the pair that last wrote it, a lazy state (binary change) or gone
+    struct View { int kind; size_t pair; PathState st; };   // kind 0 pair, 1 state, 2 gone
+    std::map<std::string, View> view;
+    const size_t n = idx.size();
+    std::vector<int32_t> prev(n, -1), label(n);
+    std::vector<int64_t> in_base(n + 1, 0);
+    std::vector<tsm_origin> origin_in;
+    for (size_t r = r0, i = 0; r < r1; ++r) {
+      const Change& c = changes[r];
+      const std::string& src = c.old_path.empty() ? c.path : c.old_path;
+      if (i < n && idx[i] == r) {
+        if (c.o >= 0) {
+          auto v = view.find(src);
+          if (v != view.end() && v->second.kind == 0) prev[i] = (int32_t)v->second.pair;
+          else {
+            PathState st;
+            if (v != view.end() && v->second.kind == 1) st = v->second.st;
+            else if (live.count(src)) st = live[src];
+            else if (cut) st.owner = owner(-1, src), st.obj = c.o;          // unchanged since P0: a boundary line
+            else die("no origins for " + src);
+            std::vector<tsm_origin> h = st.org.empty() && st.obj >= 0 ? lazy(st, nullptr) : st.org;
+            origin_in.insert(origin_in.end(), h.begin(), h.end());
+          }
+        }
+        in_base[i + 1] = (int64_t)origin_in.size();
+        label[i] = owner((int64_t)c.step, c.path);
+        if (src != c.path) view[src] = View{2, 0, {}};
+        view[c.path] = c.n >= 0 ? View{0, i, {}} : View{2, 0, {}};
+        ++i;
+      } else {                                              // binary on a side: a text new side takes its lines from this commit
+        if (src != c.path) view[src] = View{2, 0, {}};
+        PathState st;
+        st.owner = owner((int64_t)c.step, c.path); st.obj = c.n;
+        view[c.path] = c.n >= 0 && !binary(load(c.n)) ? View{1, 0, st} : View{2, 0, {}};
+      }
+    }
+    std::vector<tsm_origin> out;
+    std::vector<int64_t> base_new(n + 1, 0);
+    if (n) {
+      int64_t cap = 0, got = 0;
+      if (origin_in.empty()) origin_in.push_back({0, 0});
+      for (;;) {
+        out.resize((size_t)std::max<int64_t>(cap, 1));
+        const int rc = tsm_blame_pairs(ctx, &ca, &cn, added, removed, det, prev.data(), label.data(), origin_in.data(), in_base.data(),
+                                       nullptr, base_new.data(), out.data(), cap, &got, nullptr);
+        if (rc == TSM_E_CAPACITY && got > cap) { cap = got; continue; }
+        ck(rc, "tsm_blame_pairs");
+        break;
+      }
+      blamed_pairs += (int64_t)n;
+    }
+    for (auto& kv : view) {
+      if (kv.second.kind == 2) { live.erase(kv.first); continue; }
+      if (kv.second.kind == 1) { live[kv.first] = kv.second.st; continue; }
+      const size_t i = kv.second.pair;
+      PathState st;
+      st.org.assign(out.begin() + base_new[i], out.begin() + base_new[i + 1]);
+      live[kv.first] = std::move(st);
+    }
+  };
+  const ChangeTotals t = diff_changes(changes, chain.size(), load, rename_pct, true, {}, 0, [](size_t) { return std::vector<std::string>(); },
+                                      "", "", "", batch_bytes, &run);
+  // the selected files at R, path order: their origins (a file untouched by the window is all boundary lines)
+  std::vector<FileEntry> files;
+  if (!chain.empty()) walk_git(gs, chain.back().c.tree, "", all_files, files);
+  std::vector<std::vector<tsm_origin>> org(files.size());
+  for (size_t f = 0; f < files.size(); ++f) {
+    if (binary(*files[f].blob)) continue;
+    auto it = live.find(files[f].rel);
+    if (it != live.end()) org[f] = it->second.org.empty() && it->second.obj >= 0 ? lazy(it->second, files[f].blob.get()) : it->second.org;
+    else if (cut) { PathState st; st.owner = owner(-1, files[f].rel); org[f] = lazy(st, files[f].blob.get()); }
+    if ((int64_t)org[f].size() != count_lines(*files[f].blob)) die("blame: origins and lines of " + files[f].rel + " differ");
+  }
+  auto commit_of = [&](int32_t o) -> const Step& { return owners[(size_t)o].step < 0 ? p0 : chain[(size_t)owners[(size_t)o].step]; };
+  auto cells = [&](const std::string& path, int64_t line, const tsm_origin& g) {
+    const Step& st = commit_of(g.change);
+    return std::vector<std::string>{path, std::to_string(line), st.id.hex(), std::to_string(st.c.time), owners[(size_t)g.change].path,
+                                    std::to_string(g.line), owners[(size_t)g.change].step < 0 ? "1" : "0"};
+  };
+  std::ofstream os;
+  if (!out_path.empty()) {
+    os.open(out_path, std::ios::binary);
+    csv_row(os, {"fileName", "line", "commit", "time", "origFileName", "origLine", "boundary"});
+    for (size_t f = 0; f < files.size(); ++f)
+      for (size_t j = 0; j < org[f].size(); ++j) csv_row(os, cells(files[f].rel, (int64_t)j + 1, org[f][j]));
+  }
+  // the assertion lines at R (SPEC section 4 Rev A, ext of the path at R): one scan with assertion events
+  std::vector<int64_t> lines_of(owners.size(), 0), asserts_of(owners.size(), 0);
+  for (size_t f = 0; f < files.size(); ++f) for (const tsm_origin& g : org[f]) lines_of[(size_t)g.change]++;
+  int64_t n_asserts = 0;
+  if (!files.empty()) {
+    std::ofstream as;
+    if (!asserts_path.empty()) {
+      as.open(asserts_path, std::ios::binary);
+      csv_row(as, {"fileName", "line", "commit", "time", "origFileName", "origLine", "boundary", "statement", "category"});
+    }
+    Batch B;
+    for (size_t f = 0; f < files.size(); ++f) B.idx.push_back((uint32_t)f);
+    load_batch(files, B);
+    tsm_ctx* ctx = nullptr;
+    ck(tsm_create(&ctx, 0, std::max<int64_t>(B.bytes, 1 << 20), (int32_t)files.size(), 1, 0), "tsm_create");
+    tsm_corpus c{B.arena, B.off.data(), B.len.data(), B.ext.data(), B.grp.data(), (int32_t)files.size(), 1};
+    tsm_result r{};
+    std::vector<tsm_assert_event> aev;
+    std::vector<tsm_header_event> hev;
+    scan_events(ctx, c, B.bytes, r, TSM_SCAN_ASSERT_EVENTS, nullptr, aev, hev);
+    tsm_destroy(ctx);
+    size_t k = 0;
+    for (size_t f = 0; f < files.size(); ++f) {
+      const uint8_t* base = B.arena + B.off[f];
+      uint32_t pos = 0;
+      int64_t line = 1;
+      for (; k < aev.size() && aev[k].file == f; ++k) {
+        for (; pos < aev[k].line_off; ++pos) line += base[pos] == '\n';
+        if (org[f].empty()) continue;                        // (binary)
+        const tsm_origin& g = org[f][(size_t)line - 1];
+        asserts_of[(size_t)g.change]++; ++n_asserts;
+        if (!as.is_open()) continue;
+        std::vector<std::string> row = cells(files[f].rel, line, g);
+        row.insert(row.end(), {event_statement(base, B.len[f], aev[k]), event_category(base, aev[k])});
+        csv_row(as, row);
+      }
+    }
+    tsm_host_free(B.arena);
+  }
+  // survival counts per commit that owns a line at R, in window order (the boundary commit first)
+  std::vector<int64_t> cl(chain.size() + 1, 0), ca(chain.size() + 1, 0);
+  for (size_t o = 0; o < owners.size(); ++o) {
+    const size_t s = (size_t)(owners[o].step + 1);
+    cl[s] += lines_of[o]; ca[s] += asserts_of[o];
+  }
+  printf("commit,lines,asserts\r\n");
+  int64_t total = 0;
+  for (size_t s = 0; s <= chain.size(); ++s) {
+    total += cl[s];
+    if (cl[s]) printf("%s,%lld,%lld\r\n", (s ? chain[s - 1].id : p0.id).hex().c_str(), (long long)cl[s], (long long)ca[s]);
+  }
+  fprintf(stderr, "tosem-scan: blame of %s: %zu commits, %lld changed files on the GPU, %lld binary skipped, %zu files, %lld lines, %lld assertion lines\n",
+          rev.c_str(), chain.size(), (long long)blamed_pairs, (long long)t.binaries, files.size(), (long long)total,
+          (long long)n_asserts);
+  if (cut) fprintf(stderr, "tosem-scan: boundary commit %s\n", p0.id.hex().c_str());
+  if (rename_pct >= 0)
+    fprintf(stderr, "tosem-scan: %lld rename(s) found at %d%% (%lld exact, %lld inexact)\n", (long long)t.renames, rename_pct,
+            (long long)t.renames_exact, (long long)(t.renames - t.renames_exact));
+  return 0;
+}
+
 static void usage() {
   fprintf(stderr,
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
@@ -1553,6 +1767,7 @@ static void usage() {
           "       tosem-scan releases <snapshot-root>=<tag>... [--out F]   |   releases --git <repository> [<revision>...] [--out F]\n"
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
           "                          [--find-renames N]\n"
+          "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
           "--find-renames N (0..100): pair deleted and added files at least N %% similar, as git -M<N>%% does (docs/SPEC.md section 13).\n"
           "Scans run on the GPU through libtosemscan.so (sm_90a); there is no CPU fallback.\n");
 }
@@ -1590,6 +1805,11 @@ int main(int argc, char** argv) {
                           return cmd_history(pos[0], opt.count("--rev") ? opt["--rev"] : "HEAD",
                                                   opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0, all_files, opt["--out"], dry_run,
                                                   opt["--asserts"], opt["--assert-churn"], rename_pct); }
+  if (cmd == "blame") { if (pos.size() != 1) die("blame needs the repository");
+                        return cmd_blame(pos[0], opt.count("--rev") ? opt["--rev"] : "HEAD",
+                                         opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0, all_files, rename_pct,
+                                         opt.count("--batch-bytes") ? std::max<int64_t>(1, atoll(opt["--batch-bytes"].c_str())) : kBatch,
+                                         opt["--out"], opt["--asserts"]); }
   if (cmd == "diff") { if (pos.size() != 2) die("diff needs <old-root> <new-root>"); return cmd_diff(pos[0], pos[1], opt["--out"], opt["--asserts"], opt["--assert-churn"], rename_pct); }
   usage();
   return 2;

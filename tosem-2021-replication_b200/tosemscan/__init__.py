@@ -29,13 +29,15 @@ ASSERT_EVENT = np.dtype([("file", "<u4"), ("line_off", "<u4"), ("stmt_off", "<u4
 HEADER_EVENT = np.dtype([("file", "<u4"), ("line_off", "<u4"), ("line_len", "<u4"), ("kind", "<u4")])
 DIFF_DETAIL = np.dtype([("hunks_add", "<i8"), ("hunks_del", "<i8"), ("hunks_mod", "<i8"),
                         ("added_assert", "<i8"), ("removed_assert", "<i8")])
+ORIGIN = np.dtype([("change", "<i4"), ("line", "<i4")])   # tsm_origin: the change that inserted a line, 1-based line there
 
 # every symbol include/tosemscan.h declares (tests check the library exports exactly these)
 SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create", "tsm_destroy", "tsm_scan",
            "tsm_upload", "tsm_scan_resident", "tsm_download", "tsm_device_counts", "tsm_last_launch_count", "tsm_last_kernel_ms", "tsm_kernel_ms_stats",
            "tsm_diff_pairs", "tsm_diff_pairs_detail", "tsm_statements", "tsm_line_hashes", "tsm_diff_upload", "tsm_diff_resident", "tsm_diff_last_ms",
            "tsm_diff_pairs_asserts", "tsm_diff_resident_asserts", "tsm_reduce", "tsm_host_alloc", "tsm_host_free", "tsm_layout", "tsm_gen_sizes",
-           "tsm_gen_fill", "tsm_gen_edit", "tsm_gen_pair_sizes", "tsm_gen_pair_fill", "tsm_similarity", "tsm_similarity_last_ms"]
+           "tsm_gen_fill", "tsm_gen_edit", "tsm_gen_pair_sizes", "tsm_gen_pair_fill", "tsm_similarity", "tsm_similarity_last_ms",
+           "tsm_diff_pairs_marks", "tsm_blame_pairs", "tsm_blame_last_ms"]
 
 
 class TsmError(RuntimeError):
@@ -54,6 +56,12 @@ class _Result(C.Structure):
                 ("aev", C.c_void_p), ("aev_cap", C.c_int64), ("n_aev", C.c_int64),
                 ("hev", C.c_void_p), ("hev_cap", C.c_int64), ("n_hev", C.c_int64),
                 ("totals", C.c_int64 * 4)]
+
+
+class _LineMarks(C.Structure):
+    _fields_ = [("line_base_old", C.c_void_p), ("line_base_new", C.c_void_p),
+                ("dels", C.c_void_p), ("del_cap", C.c_int64), ("n_old", C.c_int64),
+                ("ins", C.c_void_p), ("ins_cap", C.c_int64), ("n_new", C.c_int64)]
 
 
 class _DiffAsserts(C.Structure):
@@ -146,6 +154,14 @@ def lib():
                                      C.c_void_p, C.c_void_p]
         L.tsm_similarity_last_ms.restype = C.c_int
         L.tsm_similarity_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 3)]
+        L.tsm_diff_pairs_marks.restype = C.c_int
+        L.tsm_diff_pairs_marks.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 3 + \
+            [C.POINTER(_LineMarks), C.c_void_p]
+        L.tsm_blame_pairs.restype = C.c_int
+        L.tsm_blame_pairs.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 10 + \
+            [C.c_int64, C.POINTER(C.c_int64), C.c_void_p]
+        L.tsm_blame_last_ms.restype = C.c_int
+        L.tsm_blame_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
         _lib = L
     return _lib
 
@@ -615,6 +631,68 @@ class Scanner:
         ms = (C.c_float * 3)()
         lib().tsm_diff_last_ms(self._ctx, C.byref(ms))
         return [float(x) for x in ms]
+
+    def diff_marks(self, olds, news, stream=None, cap=None):
+        """Edit marks (docs/SPEC.md section 14): (added, removed, detail, line_base_old, line_base_new, dels, ins) - dels[g] = 1
+        for every line g of `olds` the canonical script deletes, ins[g] = 1 for every line g of `news` it inserts (global line
+        order of each side; line_base[i] = first line of file i).  Arrays too small for the lines are sized and the call made
+        again (cap: the first guess)."""
+        n = olds.n_files
+        added, removed, det = np.zeros(n, np.int64), np.zeros(n, np.int64), np.zeros(max(n, 1), DIFF_DETAIL)
+        bo, bn = np.zeros(n + 1, np.int64), np.zeros(n + 1, np.int64)
+        a, b = olds.c_struct(), news.c_struct()
+        co = cn = int(cap if cap is not None else 0)
+        for _ in range(2):
+            dels, ins = np.zeros(max(co, 1), np.uint8), np.zeros(max(cn, 1), np.uint8)
+            mk = _LineMarks(_p(bo), _p(bn), _p(dels), co, 0, _p(ins), cn, 0)
+            rc = lib().tsm_diff_pairs_marks(self._ctx, C.byref(a), C.byref(b), _p(added), _p(removed), _p(det), C.byref(mk), stream)
+            if rc == TSM_E_CAPACITY and (mk.n_old > co or mk.n_new > cn):
+                co, cn = int(mk.n_old), int(mk.n_new)
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_diff_pairs_marks")
+            return added, removed, det[:n], bo, bn, dels[:mk.n_old], ins[:mk.n_new]
+        raise TsmError(TSM_E_CAPACITY, "tsm_diff_pairs_marks")
+
+    def blame_pairs(self, olds, news, prev, label, heads, stream=None, cap=None):
+        """Line provenance (docs/SPEC.md section 14): (added, removed, detail, line_base_new, origins) with origins an ORIGIN array
+        over every line of `news` (line_base_new[i] = first line of file i).  prev[i]: the pair whose new side is pair i's old
+        side, or -1; heads: {pair: ORIGIN array of its old side's lines} for the pairs with prev -1 (a missing head has a file
+        with no lines); label[i]: the change of the lines pair i inserts."""
+        n = olds.n_files
+        prev = np.ascontiguousarray(prev, np.int32)
+        label = np.ascontiguousarray(label, np.int32)
+        in_base = np.zeros(n + 1, np.int64)
+        parts = []
+        for i in range(n):
+            h = heads.get(i) if prev[i] < 0 else None
+            h = np.zeros(0, ORIGIN) if h is None else np.ascontiguousarray(h, ORIGIN)
+            parts.append(h)
+            in_base[i + 1] = in_base[i] + len(h)
+        origin_in = np.concatenate(parts) if parts else np.zeros(0, ORIGIN)
+        origin_in = origin_in if len(origin_in) else np.zeros(1, ORIGIN)
+        added, removed, det = np.zeros(n, np.int64), np.zeros(n, np.int64), np.zeros(max(n, 1), DIFF_DETAIL)
+        bo, bn = np.zeros(n + 1, np.int64), np.zeros(n + 1, np.int64)
+        a, b = olds.c_struct(), news.c_struct()
+        c = int(cap if cap is not None else 0)
+        for _ in range(2):
+            out = np.zeros(max(c, 1), ORIGIN)
+            nl = C.c_int64()
+            rc = lib().tsm_blame_pairs(self._ctx, C.byref(a), C.byref(b), _p(added), _p(removed), _p(det), _p(prev), _p(label),
+                                       _p(origin_in), _p(in_base), _p(bo), _p(bn), _p(out), c, C.byref(nl), stream)
+            if rc == TSM_E_CAPACITY and nl.value > c:
+                c = int(nl.value)
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_blame_pairs")
+            return added, removed, det[:n], bn, out[:nl.value]
+        raise TsmError(TSM_E_CAPACITY, "tsm_blame_pairs")
+
+    def blame_last_ms(self):
+        """Device time of k_blame in the last blame_pairs call, in ms."""
+        ms = C.c_float()
+        lib().tsm_blame_last_ms(self._ctx, C.byref(ms))
+        return float(ms.value)
 
     def similarity(self, olds, news, cand_old, cand_new, stream=None):
         """Rename similarity (docs/SPEC.md section 13): common[c] of file cand_old[c] of `olds` and file cand_new[c] of `news`
