@@ -151,6 +151,7 @@ int tsm_diff_pairs_detail(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus
 /* A pair whose edit distance D is larger than 23 168 lines needs more than 2^28 trace entries ((D+1)(D+2)/2 ints, 1 GiB)
  * for its backtrack: tsm_diff_pairs_detail does not trace it - added / removed are exact, the detail reports ONE hunk
  * (add, del or mod by the counts) and added_assert = removed_assert = -1.  Every other pair of the call is unaffected.
+ * A pure insertion or deletion (after the common prefix and suffix) needs no backtrack: its detail is exact at any D.
  *
  * Resident variant (bench.py's `value` for config C5): tsm_diff_upload copies both sides to HBM once and keeps them in
  * the ctx; every tsm_diff_resident call runs the kernels over them (k_scan over both sides for the line records,

@@ -1,7 +1,7 @@
 """ctypes binding of the CPU reference of the edit marks (tests/orc_diff_marks.c).  TEST INFRASTRUCTURE ONLY.
 
-The C file is compiled into a library in the temporary directory, so that the tests never write into the tree.  diff_marks
-of packed sides takes the line hashes from the oracle (orc.line_records)."""
+The C file is compiled into a library in the temporary directory, so that the tests never write into the tree.  The marks
+of packed sides take the line hashes from the oracle (orc.scan)."""
 import ctypes as C
 import hashlib
 import os
@@ -49,14 +49,54 @@ def diff_marks(a, b):
     return int(d), dl[:a.size], ins[:b.size]
 
 
-def diff_pairs_marks(old, new):
+def line_hashes(side):
+    """(line_base, line_hash) of the packed side (arena, off, len, ext): orc.line_records without the assertion flags."""
+    res = orc.scan(*side, np.zeros(len(side[2]), np.uint16), 1, events=False, line_hashes=True)
+    return res["line_base"], res["line_hash"]
+
+
+def middle(a, b):
+    """(pre, suf) of the line-hash sequences a and b: their common prefix, then the common suffix of what the prefix leaves,
+    as the diff kernels take them.  The middle is a[pre:len(a) - suf] and b[pre:len(b) - suf]."""
+    a, b = np.asarray(a, np.uint64), np.asarray(b, np.uint64)
+    k = min(a.size, b.size)
+    ne = np.flatnonzero(a[:k] != b[:k])
+    pre = int(ne[0]) if ne.size else k
+    k -= pre
+    ne = np.flatnonzero(a[a.size - k:][::-1] != b[b.size - k:][::-1])
+    return pre, int(ne[0]) if ne.size else k
+
+
+def middle_marks(a, b):
+    """(del, ins) with every line of the middle marked: how the device marks a pair it does not trace (D > TRACE_MAX_D)."""
+    pre, suf = middle(a, b)
+    dl, ins = np.zeros(len(a), np.uint8), np.zeros(len(b), np.uint8)
+    dl[pre:len(a) - suf] = 1
+    ins[pre:len(b) - suf] = 1
+    return dl, ins
+
+
+def device_marks(a, b, d=None):
+    """(del, ins) of the line-hash sequences a and b as the device marks them: the serial script of a traced pair, the whole
+    middle of an untraced one.  d: the pair's distance when it is known without a search (corpus_util.block_pair gives it in
+    closed form); the serial search, whose memory grows as D^2, runs only when d is None or at most TRACE_MAX_D.  A pure
+    hunk needs no search: its script is its whole middle, at any distance."""
+    if d is not None and d > TRACE_MAX_D:
+        return middle_marks(a, b)
+    got, dl, ins = diff_marks(a, b)
+    assert d is None or got == d, (got, d)
+    assert got <= TRACE_MAX_D or not dl.any() or not ins.any(), got
+    return dl, ins
+
+
+def diff_pairs_marks(old, new, dist=None):
     """old/new: packed sides (arena, off, len, ext).  (line_base_old, line_base_new, del, ins) over every line of each side,
-    as tsm_diff_pairs_marks gives them; both sides must be within reach of the serial search (no untraced pair)."""
-    ba, ha = orc.line_records(*old)[:2]
-    bb, hb = orc.line_records(*new)[:2]
+    as tsm_diff_pairs_marks gives them (device_marks per pair).  dist: {pair: D} of the pairs whose distance is known in closed
+    form; every other pair must be within reach of the serial search."""
+    ba, ha = line_hashes(old)
+    bb, hb = line_hashes(new)
+    dist = dist or {}
     dl, ins = np.zeros(int(ba[-1]), np.uint8), np.zeros(int(bb[-1]), np.uint8)
     for i in range(len(ba) - 1):
-        d, x, y = diff_marks(ha[ba[i]:ba[i + 1]], hb[bb[i]:bb[i + 1]])
-        assert d <= TRACE_MAX_D
-        dl[ba[i]:ba[i + 1]], ins[bb[i]:bb[i + 1]] = x, y
+        dl[ba[i]:ba[i + 1]], ins[bb[i]:bb[i + 1]] = device_marks(ha[ba[i]:ba[i + 1]], hb[bb[i]:bb[i + 1]], dist.get(i))
     return ba, bb, dl, ins

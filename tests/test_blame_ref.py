@@ -154,6 +154,56 @@ def test_py_blame_window_matches_git(tmp_path, n):
         assert any(b for *_, b in got) == any(b for *_, b in state[path])
 
 
+def block_middle(old_blocks, new_blocks, n_prefix, n_suffix):
+    """(pre, suf) of a corpus_util.block_pair in closed form: leading empty block pairs put their common line in the prefix,
+    the common line behind the last non-empty block pair and those of the empty pairs after it belong to the suffix."""
+    nz = [i for i, (x, y) in enumerate(zip(old_blocks, new_blocks)) if x or y]
+    return n_prefix + nz[0], n_suffix + len(old_blocks) - nz[-1]
+
+
+def hashes(f):
+    return np.array([r[0] for r in sr.py_line_records(f, 1)], np.uint64)
+
+
+def test_untraced_marks_closed_form():
+    """orc_marks.device_marks: on traced block pairs the serial marks, whose distance is the closed form's and whose first and
+    last changed lines bound the closed-form middle; on untraced ones (D > 23 168, no serial search) the whole closed-form
+    middle, common lines inside it included."""
+    rng = random.Random(12)
+    shapes = [(tuple(rng.randrange(0, 30) for _ in range(k)), tuple(rng.randrange(0, 30) for _ in range(k)))
+              for k in (1, 2, 3, 5) for _ in range(8)]
+    shapes += [((0, 7, 0), (0, 0, 0)), ((0, 0, 4), (3, 0, 0)), ((5,), (0,)), ((0,), (6,)), ((0, 2, 0, 0), (0, 0, 9, 0))]
+    n = 0
+    for i, (ob, nb) in enumerate(shapes):
+        if not any(ob) and not any(nb):
+            continue
+        pre, suf = rng.randrange(0, 4), rng.randrange(0, 4)
+        o, nw, w = cu.block_pair(b"m%d" % i, ob, nb, n_prefix=pre, n_suffix=suf)
+        a, b = hashes(o), hashes(nw)
+        p, s = orc_marks.middle(a, b)
+        assert (p, s) == block_middle(ob, nb, pre, suf)
+        d, dl, ins = orc_marks.diff_marks(a, b)
+        assert d == len(w[3]) + len(w[4])
+        assert np.flatnonzero(dl).tolist() == w[3] and np.flatnonzero(ins).tolist() == w[4]
+        marks = ((np.flatnonzero(dl), len(a)), (np.flatnonzero(ins), len(b)))
+        assert all(x.size == 0 or (x[0] >= p and x[-1] < k - s) for x, k in marks)
+        assert any(x.size and x[0] == p for x, _ in marks) and any(x.size and x[-1] == k - s - 1 for x, k in marks)
+        got = orc_marks.device_marks(a, b, d)
+        assert np.array_equal(got[0], dl) and np.array_equal(got[1], ins)
+        n += 1
+    assert n > 30
+    for i, (ob, nb) in enumerate((((11584,), (11585,)), ((6000, 5585), (6000, 5585)), ((23169,), (0,)), ((0, 9, 23161), (1, 0, 0)))):
+        o, nw, w = cu.block_pair(b"u%d" % i, ob, nb, n_prefix=40 + i, n_suffix=30 + i)
+        d = len(w[3]) + len(w[4])
+        assert d > orc_marks.TRACE_MAX_D
+        a, b = hashes(o), hashes(nw)
+        p, s = block_middle(ob, nb, 40 + i, 30 + i)
+        dl, ins = orc_marks.device_marks(a, b, d)
+        assert np.flatnonzero(dl).tolist() == list(range(p, len(a) - s))
+        assert np.flatnonzero(ins).tolist() == list(range(p, len(b) - s))
+        assert set(w[3]) <= set(range(p, len(a) - s)) and set(w[4]) <= set(range(p, len(b) - s))
+
+
 def test_marks_reference_matches_spec_ref():
     olds, news, exts = cu.tie_heavy_pairs(7)
     rng = random.Random(4)

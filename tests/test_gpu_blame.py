@@ -8,7 +8,6 @@ import numpy as np
 import pytest
 
 import corpus_util as cu
-import orc
 import orc_marks
 import spec_ref as sr
 import tosemscan as ts
@@ -92,18 +91,25 @@ def test_marks_trace_limit():
     assert int(dl[bo[4]:bo[5]].sum()) > rem[4]              # the untraced middle holds a common line
 
 
-def ref_blame(a, b, prev, label, heads):
-    """Serial provenance (SPEC section 14) from the reference marks: a list of (change, line) lists, one per pair."""
-    ba, ha = orc.line_records(*a)[:2]
-    bb, hb = orc.line_records(*b)[:2]
+def provenance(ba, bb, dl, ins, prev, label, heads):
+    """Serial provenance (SPEC section 14) from the marks of every pair (orc_marks.diff_pairs_marks): an ORIGIN array per pair."""
     out = []
     for i in range(len(prev)):
-        src = out[prev[i]] if prev[i] >= 0 else [tuple(x) for x in heads.get(i, [])]
-        _, dl, ins = orc_marks.diff_marks(ha[ba[i]:ba[i + 1]], hb[bb[i]:bb[i + 1]])
-        assert len(src) == len(dl)
-        kept = iter([s for s, x in zip(src, dl) if not x])
-        out.append([(int(label[i]), j + 1) if x else next(kept) for j, x in enumerate(ins)])
+        src = out[prev[i]] if prev[i] >= 0 else np.asarray(heads.get(i, np.zeros(0, ts.ORIGIN)), ts.ORIGIN)
+        d, s = dl[ba[i]:ba[i + 1]], ins[bb[i]:bb[i + 1]]
+        assert len(src) == len(d)
+        o = np.zeros(len(s), ts.ORIGIN)
+        new = np.flatnonzero(s)
+        o["change"][new], o["line"][new] = label[i], new + 1
+        o[s == 0] = src[d == 0]
+        out.append(o)
     return out
+
+
+def ref_blame(a, b, prev, label, heads, dist=None):
+    """provenance over the reference marks of the packed sides a, b; dist as orc_marks.diff_pairs_marks (pairs above the trace
+    limit are marked over their whole middle, as the device marks them)."""
+    return provenance(*orc_marks.diff_pairs_marks(a, b, dist), prev, label, heads)
 
 
 def chains(seed, lengths, lam_hi=200.0):
@@ -131,13 +137,43 @@ def chains(seed, lengths, lam_hi=200.0):
     return olds, news, exts, np.array(prev, np.int32), np.array(label, np.int32), heads
 
 
+def chain_order(prev, seed):
+    """A random order of the pairs that keeps every pair behind its prev: order[k] = the pair that goes to place k."""
+    rng = np.random.default_rng(seed)
+    head = np.arange(len(prev))
+    for i, p in enumerate(prev):
+        if p >= 0:
+            head[i] = head[p]
+    key = np.empty(len(prev))
+    idx = np.argsort(head, kind="stable")                  # the pairs chain by chain, each chain in its order
+    cut = np.flatnonzero(np.diff(head[idx])) + 1
+    for members in np.split(idx, cut):
+        key[members] = np.sort(rng.random(len(members)))
+    return np.argsort(key, kind="stable")
+
+
+def reordered(order, olds, news, exts, prev, label, heads):
+    """The batch with pair order[k] at place k, prev / label / heads remapped."""
+    pos = np.empty(len(order), np.int64)
+    pos[order] = np.arange(len(order))
+    nprev = np.array([pos[prev[i]] if prev[i] >= 0 else -1 for i in order], np.int32)
+    assert (nprev < np.arange(len(order))).all()
+    return ([olds[i] for i in order], [news[i] for i in order], [exts[i] for i in order], nprev, label[order].copy(),
+            {int(pos[i]): h for i, h in heads.items()})
+
+
+def same_origins(org, bn, want):
+    """Device origins (every line of every new side) against ref_blame's, origin for origin."""
+    assert len(org) == bn[-1] == sum(len(w) for w in want)
+    for i, w in enumerate(want):
+        assert np.array_equal(org[bn[i]:bn[i + 1]], w), i
+
+
 def check_blame(sc, olds, news, exts, prev, label, heads, stream=None):
     a, b = ts.pack(olds, exts), ts.pack(news, exts)
     add, rem, det, bn, org = sc.blame_pairs(a, b, prev, label, heads, stream=stream)
     want = ref_blame(*sides(a, b), prev, label, heads)
-    for i, w in enumerate(want):
-        got = [tuple(int(v) for v in x) for x in org[bn[i]:bn[i + 1]]]
-        assert got == w, i
+    same_origins(org, bn, want)
     padd, prem, pdet = sc.diff_pairs(a, b, detail=True)
     assert np.array_equal(add, padd) and np.array_equal(rem, prem) and np.array_equal(det, pdet)
     return add, rem

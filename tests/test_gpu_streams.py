@@ -29,8 +29,10 @@ import pytest
 import corpus_util as cu
 import orc
 import orc_asserts
+import orc_marks
 import orc_similarity
 import tosemscan as ts
+from test_gpu_blame import chain_order, chains, ref_blame, reordered, same_origins
 from test_gpu_slabs import check, expected_slabs
 
 pytestmark = pytest.mark.gpu
@@ -200,6 +202,18 @@ def pair_corpora():
     return out
 
 
+@functools.lru_cache(None)
+def blame_chains():
+    """Chains of edited C5-law files (test_gpu_blame.chains) as blame_pairs arguments; the twin has the pairs in another
+    order that keeps each chain's order."""
+    olds, news, exts, prev, label, heads = chains(0x57E0B1, [30, 1, 6, 2, 12, 3, 1, 4, 9, 2])
+    out = []
+    for order in (np.arange(len(prev)), chain_order(prev, 5)):
+        o, n, e, p, lab, h = reordered(order, olds, news, exts, prev, label, heads)
+        out.append((ts.pack(o, e, pinned=True), ts.pack(n, e, pinned=True), p, lab, h))
+    return out
+
+
 def reduce_rows(seed):
     rng = np.random.default_rng(seed)
     n = 20000
@@ -230,6 +244,17 @@ def check_asserts(got, a, b):
     assert len(want[2]) > 50 and len(want[3]) > 50
 
 
+def check_marks(got, a, b):
+    check_diff(got[:3], a, b)
+    same(got[3:], orc_marks.diff_pairs_marks((a.arena, a.off, a.len, a.ext), (b.arena, b.off, b.len, b.ext)))
+
+
+def check_blame(got, x):
+    a, b, prev, label, heads = x
+    check_diff(got[:3], a, b)
+    same_origins(got[4], got[3], ref_blame((a.arena, a.off, a.len, a.ext), (b.arena, b.off, b.len, b.ext), prev, label, heads))
+
+
 def check_lines(got, c):
     base, lh, le, lf = orc.line_records(c.arena, c.off, c.len, c.ext)
     same(got, (base, lh, le, lf, orc.ngram_hashes(lh, base, 3)))
@@ -257,6 +282,14 @@ def a_case(name):
             sc.scan_resident(EV, st)
             return sc.download(EV, st)
         return sc, call, c, twin, lambda r, x: check(r, oracle(x))
+    if name == "diff_pairs_marks":
+        pair, twin = pair_corpora()
+        sc = ts.Scanner(0, 1 << 20, 16, 4)
+        return sc, lambda x, st: sc.diff_marks(*x, st), pair, twin, lambda r, x: check_marks(r, *x)
+    if name == "blame_pairs":
+        x, twin = blame_chains()
+        sc = ts.Scanner(0, 1 << 20, 16, 4)
+        return sc, lambda x, st: sc.blame_pairs(*x, stream=st), x, twin, check_blame
     if name.startswith("diff_"):
         pair, twin = pair_corpora()
         sc = ts.Scanner(0, 1 << 20, 16, 4)
@@ -298,8 +331,8 @@ def a_case(name):
 
 
 A_CASES = ["scan-small-revA", "scan-small-revB", "scan-streamed-revA", "scan-streamed-revB", "resident", "diff_pairs",
-           "diff_pairs_detail", "diff_pairs_asserts", "diff_resident", "diff_resident_asserts", "similarity", "line_hashes",
-           "statements", "reduce"]
+           "diff_pairs_detail", "diff_pairs_asserts", "diff_resident", "diff_resident_asserts", "diff_pairs_marks",
+           "blame_pairs", "similarity", "line_hashes", "statements", "reduce"]
 
 
 @pytest.mark.parametrize("name", A_CASES)
