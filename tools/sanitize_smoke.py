@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Small scan (Rev A and Rev B) + line records + diff + statements + reduce under compute-sanitizer (run: compute-sanitizer --tool memcheck python tools/sanitize_smoke.py)."""
+"""Small scan (Rev A and Rev B) + line records + diff (plain, assertion lines, marks, provenance) + similarity + statements + reduce under compute-sanitizer (run: compute-sanitizer --tool memcheck python tools/sanitize_smoke.py)."""
 import os
 import sys
 
@@ -23,6 +23,17 @@ print(s.diff_pairs(a, b, detail=True))
 far_o = [b"".join(b"o%d\n" % i for i in range(60)), b"head\n" * 10 + b"".join(b"m%d\n" % i for i in range(2500)) + b"tail\n"]
 far_n = [b"".join(b"n%d\n" % i for i in range(50)), b"head\n" * 10 + b"x\n" + b"".join(b"m%d\n" % i for i in range(2500)) + b"y\ntail\n"]
 print(s.diff_pairs(ts.pack(far_o, [1, 1]), ts.pack(far_n, [1, 1]), detail=True))   # the left-over path: D > 31, middle > 4 096 lines
+# the pair calls with their own scratch: changed assertion lines, edit marks, provenance and rename similarity, each also
+# over the far pair so that the EMIT and MARKS variants of the left-over kernels run
+far_o[0] += b"assert x == 1\n"; far_n[0] += b"assertEqual(y, 2)\n"
+fo, fn = ts.pack(far_o, [1, 1], [0, 1], 2), ts.pack(far_n, [1, 1], [1, 0], 2)
+print([x.sum() for x in s.diff_pairs(fo, fn, asserts=True)[3:5]])
+print([int(x.sum()) for x in s.diff_marks(fo, fn)[5:]])
+lines0 = far_o[0].count(b"\n")
+g = s.blame_pairs(ts.pack([far_o[0], far_n[0]], [1, 1]), ts.pack([far_n[0], far_o[0]], [1, 1]), [-1, 0], [1, 2],
+                  {0: np.array([(-1, j + 1) for j in range(lines0)], ts.ORIGIN)})
+print(len(g[4]), g[4][:3])
+print(s.similarity(fo, ts.pack(far_n + [b"m1\nm2\n"], [1, 1, 1]), [0, 1, 1], [0, 1, 2]))
 print([x[:4] for x in s.line_hashes(ts.pack(files[:40], exts[:40]), ngram=3)])
 r4 = s.scan(ts.pack(files, exts, grps, 5), 3 | ts.SCAN_REV_B)
 print(s.statements(c)[0][-1])

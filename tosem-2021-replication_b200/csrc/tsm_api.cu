@@ -5,6 +5,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <new>
+#include <utility>
 #include <vector>
 
 #include "tsm_device.cuh"
@@ -47,9 +48,10 @@ struct ScratchPool {
   void clear() { for (Slot& s : slots) cudaFree(s.p); slots.clear(); }
 };
 static thread_local ScratchPool* t_pool = nullptr;        // pool of the ctx whose call runs on this thread
-struct PoolScope {
-  explicit PoolScope(ScratchPool* p) { t_pool = p; }
-  ~PoolScope() { t_pool = nullptr; }
+struct PoolScope {                                        // (restores the pool it replaced: scopes nest)
+  ScratchPool* prev;
+  explicit PoolScope(ScratchPool* p) : prev(t_pool) { t_pool = p; }
+  ~PoolScope() { t_pool = prev; }
 };
 
 struct DevBuf {                                           // device scratch from the ctx's pool, returned on scope exit
@@ -61,7 +63,7 @@ struct DevBuf {                                           // device scratch from
 };
 
 struct SyncGuard {                                        // error paths: wait for the work queued on st before the DevBufs of the
-  cudaStream_t st;                                        // scope hand their slots back to the pool (the next call may reuse or free them)
+  cudaStream_t st;                                        // call hand their slots back to the pool (see CallScope)
   explicit SyncGuard(cudaStream_t s) : st(s) {}
   ~SyncGuard() { cudaStreamSynchronize(st); }
 };
@@ -89,8 +91,8 @@ struct tsm_ctx {
   cudaStream_t copy_stream = nullptr;       // H2D of arena slabs, overlapped with the scan of earlier slabs
   cudaEvent_t slab_ev[64] = {};
   cudaEvent_t ready_ev = nullptr;
-  cudaEvent_t order_ev = nullptr;           // recorded behind the device work of every call (CallOrder)
-  cudaEvent_t diff_ev[8] = {};             // around the kernels of the diff path (tsm_diff_last_ms)
+  cudaEvent_t order_ev = nullptr;           // recorded behind the device work of every call (CallScope)
+  cudaEvent_t diff_ev[8] = {};             // around the kernels of the diff path (tsm_diff_last_ms): slots EV_*
   uint8_t* h_diff = nullptr;               // 256 B pinned: what the diff path reads back between its kernels (Ctrl x 2, line totals, todo count)
   float diff_ms[3] = {0, 0, 0};            // k_scan over both sides, k_myers, k_myers_trace of the last diff
   float sim_ms[3] = {0, 0, 0};             // k_scan over both sides, sort / merge, k_similarity of the last tsm_similarity
@@ -120,14 +122,34 @@ struct tsm_ctx {
   long long ms_n = 0;
 };
 
-// A ctx orders its own work, whatever stream each call is given: a call's stream first waits for the ctx's order event
-// (a wait on an event that was never recorded is a no-op), and the event is recorded on it behind everything the call
-// queued, on every return path.  Declared before the call's DevBufs and SyncGuard, so that it records after them.
-struct CallOrder {
+// Slots of tsm_ctx::diff_ev.  The line records of a revision pair: k_scan of side s from EV_SCAN[s].from to .to.  The diff:
+// k_diff_small over EV_SMALL, each launch for the pairs it leaves over EV_LEFT.  tsm_similarity: the sorted lists of both
+// sides from EV_SIM_LISTS to EV_SIM_PAIRS, k_similarity from there to EV_SIM_END.
+struct EvSpan { int from, to; };
+constexpr EvSpan EV_SCAN[2] = {{0, 1}, {6, 7}}, EV_SMALL = {2, 3}, EV_LEFT = {4, 5};
+constexpr int EV_SIM_LISTS = 2, EV_SIM_PAIRS = 3, EV_SIM_END = 4;
+
+// The start of every call that queues device work on st: the ctx's device, the ctx's pool for the call's DevBufs, and the
+// order of the ctx's calls.  A ctx orders its own work, whatever stream each call is given: the call's stream first waits
+// for the ctx's order event (a wait on an event that was never recorded is a no-op), and the event is recorded on it
+// behind everything the call queued, on every return path once the device is set.  status = the first failure.
+// Order of a call's objects: this scope, then the DevBufs (and the HostSides that hold them), then a SyncGuard.
+// Destruction runs backwards: the SyncGuard waits for st before any buffer goes back to the pool (the next call may
+// reuse or free it), and the order event is recorded behind all of it.  A helper that takes DevBufs of its own
+// (diff_core, diff_asserts, the tails of line_records) synchronises st before it returns them on success; on an error
+// it returns them at once, but the call then unwinds without allocating again and its SyncGuard waits for st before
+// the call returns.
+struct CallScope {
   tsm_ctx* c; cudaStream_t st;
-  CallOrder(tsm_ctx* ctx, cudaStream_t s) : c(ctx), st(s) {}
-  cudaError_t wait() const { return cudaStreamWaitEvent(st, c->order_ev, 0); }
-  ~CallOrder() { cudaEventRecord(c->order_ev, st); }
+  PoolScope pool;
+  bool on_device;
+  cudaError_t status;
+  CallScope(tsm_ctx* ctx, cudaStream_t s) : c(ctx), st(s), pool(&ctx->pool) {
+    status = cudaSetDevice(c->device);
+    on_device = status == cudaSuccess;
+    if (on_device) status = cudaStreamWaitEvent(st, c->order_ev, 0);
+  }
+  ~CallScope() { if (on_device) cudaEventRecord(c->order_ev, st); }
 };
 
 // Fold the elapsed times of event set `i` into the running sums (waits for it if still in flight).
@@ -199,16 +221,18 @@ static void build_elut(uint32_t* lut) {                  // operator patterns of
 
 static void free_res_pair(tsm_ctx* c);
 
-template <int MODE> static cudaError_t diff_small_smem() {   // the dynamic shared memory of the four k_diff_small sizes
-  cudaError_t e = cudaFuncSetAttribute(k_diff_small<DS1_HCAP, DS1_DCAP, DS1_WARPS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)(DS1_WARPS * ds_warp_bytes(DS1_HCAP, DS1_DCAP)));
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_diff_small<DS2_HCAP, DS2_DCAP, DS2_WARPS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                 (int)(DS2_WARPS * ds_warp_bytes(DS2_HCAP, DS2_DCAP)));
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_diff_small<DS3_HCAP, DS3_DCAP, DS3_WARPS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                 (int)(DS3_WARPS * ds_warp_bytes(DS3_HCAP, DS3_DCAP)));
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_diff_small<DS4_HCAP, DS4_DCAP, DS4_WARPS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                 (int)(DS4_WARPS * ds_warp_bytes(DS4_HCAP, DS4_DCAP)));
-  return e;
+// f(std::integral_constant<int, I>{}) for every size I of k_diff_small (DS_SIZES), in order.
+template <typename F, int... I> static void for_ds_sizes(F&& f, std::integer_sequence<int, I...>) { (f(std::integral_constant<int, I>{}), ...); }
+template <typename F> static void for_ds_sizes(F&& f) { for_ds_sizes(f, std::make_integer_sequence<int, DS_N>()); }
+
+template <int MODE> static bool diff_small_smem() {      // the dynamic shared memory limit of every k_diff_small size
+  bool ok = true;
+  for_ds_sizes([&](auto i) {
+    constexpr DiffSmallSize s = DS_SIZES[decltype(i)::value];
+    ok = ok && cudaFuncSetAttribute(k_diff_small<s.hcap, s.dcap, s.warps, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)s.smem()) == cudaSuccess;
+  });
+  return ok;
 }
 
 extern "C" void tsm_destroy(tsm_ctx* c) {
@@ -301,8 +325,7 @@ extern "C" int tsm_create(tsm_ctx** out, int device, int64_t max_arena_bytes, in
         cudaMemcpyToSymbol(c_lut_b, lutb, sizeof lutb) != cudaSuccess ||
         cudaFuncSetAttribute(k_scan_t<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN2_SMEM) != cudaSuccess ||
         cudaFuncSetAttribute(k_scan_t<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN2_SMEM_B) != cudaSuccess ||
-        diff_small_smem<DIFF_PLAIN>() != cudaSuccess || diff_small_smem<DIFF_EMIT>() != cudaSuccess ||
-        diff_small_smem<DIFF_MARKS>() != cudaSuccess ||
+        !diff_small_smem<DIFF_PLAIN>() || !diff_small_smem<DIFF_EMIT>() || !diff_small_smem<DIFF_MARKS>() ||
         cudaFuncSetAttribute(k_sim_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SIM_SORT_SMEM) != cudaSuccess)
       rc = TSM_E_CUDA;
   }
@@ -371,10 +394,9 @@ extern "C" int tsm_upload(tsm_ctx* c, const tsm_corpus* k, void* stream) {
   int rc = check_corpus_head(c, k);
   if (rc == TSM_OK) rc = check_files(k, 0, k->n_files, true, true);
   if (rc != TSM_OK) return rc;
-  CU(cudaSetDevice(c->device));
   cudaStream_t st = (cudaStream_t)stream;
-  CallOrder order(c, st);
-  CU(order.wait());
+  CallScope call(c, st);
+  CU(call.status);
   rc = upload_index(c, k, st);
   if (rc != TSM_OK) return rc;
   if (c->n_files) CU(cudaMemcpyAsync(c->d_arena, k->arena, (size_t)c->arena_bytes, cudaMemcpyHostToDevice, st));
@@ -404,15 +426,29 @@ static ScanParams make_params(const tsm_ctx* c, uint32_t flags) {   // the ScanP
   return p;
 }
 
-// Resident blocks of k_classify per SM at `smem` bytes of dynamic shared memory (the query is cached for the last size).
-static int classify_per_sm(tsm_ctx* c, size_t smem) {
+// k_scan over the slab of p, with the Rev-B triggers or without.
+static void launch_k_scan(const tsm_ctx* c, const ScanParams& p, bool rev_b, cudaStream_t st) {
+  if (rev_b) k_scan_t<true><<<c->sms * SCAN2_CTAS_PER_SM, SCAN2_WARPS * 32, SCAN2_SMEM_B, st>>>(p);
+  else k_scan_t<false><<<c->sms * SCAN2_CTAS_PER_SM, SCAN2_WARPS * 32, SCAN2_SMEM, st>>>(p);
+}
+
+// The dynamic shared memory of k_classify over n_groups groups (their histogram is kept per block up to 16 groups) and
+// one resident wave of its blocks, which loop over the candidates (the occupancy query is cached for the last size).
+struct ClassifyShape { size_t smem; uint32_t wave; };
+static ClassifyShape classify_shape(tsm_ctx* c, int32_t n_groups) {
+  const size_t smem = CLS_SMEM_BASE + sizeof(uint32_t) * (n_groups <= 16 ? (size_t)n_groups * TSM_K : 0);
   if (c->cls_smem != smem) {
     int per_sm = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_classify_t<false>, 256, smem) != cudaSuccess || per_sm < 1) per_sm = 4;
     c->cls_per_sm = per_sm;
     c->cls_smem = smem;
   }
-  return c->cls_per_sm;
+  return {smem, (uint32_t)(c->sms * c->cls_per_sm)};
+}
+
+static void launch_k_classify(const ScanParams& p, bool rev_b, uint32_t grid, size_t smem, cudaStream_t st) {
+  if (rev_b) k_classify_t<true><<<grid, 256, smem, st>>>(p);
+  else k_classify_t<false><<<grid, 256, smem, st>>>(p);
 }
 
 // One scan = [memsets] + per slab (k_plan, k_scan) + k_classify on `st`.  With host != NULL
@@ -447,8 +483,8 @@ static int launch_scan(tsm_ctx* c, uint32_t flags, cudaStream_t st, const tsm_co
     cudaEvent_t* ev = c->ev[es];
     CU(cudaEventRecord(ev[0], st));
     const int n_slabs = (int)cut.size() - 1;
-    const size_t hist = CLS_SMEM_BASE + sizeof(uint32_t) * (c->n_groups <= 16 ? (size_t)c->n_groups * TSM_K : 0);
-    const int cls_grid = c->sms * classify_per_sm(c, hist);   // one resident wave of k_classify (grid-stride inside)
+    const bool rev_b = flags & TSM_SCAN_REV_B;
+    const ClassifyShape cls = classify_shape(c, c->n_groups);
     for (int s = 0; s < n_slabs; ++s) {
       const int32_t f0 = cut[(size_t)s], f1 = cut[(size_t)s + 1];
       if (host) {
@@ -471,21 +507,18 @@ static int launch_scan(tsm_ctx* c, uint32_t flags, cudaStream_t st, const tsm_co
       k_plan<<<(f1 - f0 + 255) / 256, 256, 0, st>>>(p);
       CU(cudaGetLastError());
       if (s == 0 && n_slabs == 1) CU(cudaEventRecord(ev[1], st));
-      if (flags & TSM_SCAN_REV_B) k_scan_t<true><<<c->sms * SCAN2_CTAS_PER_SM, SCAN2_WARPS * 32, SCAN2_SMEM_B, st>>>(p);
-      else k_scan_t<false><<<c->sms * SCAN2_CTAS_PER_SM, SCAN2_WARPS * 32, SCAN2_SMEM, st>>>(p);
+      launch_k_scan(c, p, rev_b, st);
       CU(cudaGetLastError());
       if (s + 1 < n_slabs) {                               // streamed scan: this slab's candidates are classified under the next
         p.cls_last = 0;                                    // slab's copy, so that only the last slab's are left behind the last copy
-        if (flags & TSM_SCAN_REV_B) k_classify_t<true><<<cls_grid, 256, hist, st>>>(p);
-        else k_classify_t<false><<<cls_grid, 256, hist, st>>>(p);
+        launch_k_classify(p, rev_b, cls.wave, cls.smem, st);
         CU(cudaGetLastError());
         p.cls_last = 1;
       }
     }
     if (n_slabs > 1) CU(cudaEventRecord(ev[1], st));      // per-kernel split is only meaningful for one slab
     CU(cudaEventRecord(ev[2], st));
-    if (flags & TSM_SCAN_REV_B) k_classify_t<true><<<cls_grid, 256, hist, st>>>(p);
-    else k_classify_t<false><<<cls_grid, 256, hist, st>>>(p);
+    launch_k_classify(p, rev_b, cls.wave, cls.smem, st);
     CU(cudaGetLastError());
     CU(cudaEventRecord(ev[3], st));
     CU(cudaEventRecord(ev[4], st));                           // (slot of the former k_totals, now fused into k_classify)
@@ -503,9 +536,8 @@ extern "C" int tsm_scan_resident(tsm_ctx* c, uint32_t flags, void* stream) {
   if (!c) return TSM_E_ARG;
   flags &= TSM_SCAN_ASSERT_EVENTS | TSM_SCAN_HEADER_EVENTS | TSM_SCAN_REV_B;
   if (!c->resident) return TSM_E_STATE;
-  CU(cudaSetDevice(c->device));
-  CallOrder order(c, (cudaStream_t)stream);
-  CU(order.wait());
+  CallScope call(c, (cudaStream_t)stream);
+  CU(call.status);
   return launch_scan(c, flags, (cudaStream_t)stream, nullptr);
 }
 
@@ -646,9 +678,8 @@ static int download(tsm_ctx* c, tsm_result* r, cudaStream_t st) {
 extern "C" int tsm_download(tsm_ctx* c, tsm_result* r, void* stream) {
   if (!c || !r) return TSM_E_ARG;
   if (!c->scanned) return TSM_E_STATE;
-  CU(cudaSetDevice(c->device));
-  CallOrder order(c, (cudaStream_t)stream);
-  CU(order.wait());
+  CallScope call(c, (cudaStream_t)stream);
+  CU(call.status);
   return download(c, r, (cudaStream_t)stream);
 }
 
@@ -657,10 +688,9 @@ extern "C" int tsm_scan(tsm_ctx* c, const tsm_corpus* k, tsm_result* r, uint32_t
   int rc = check_corpus_head(c, k);                       // (the per-file rules are checked slab by slab, under the copies)
   if (rc != TSM_OK) return rc;
   flags &= TSM_SCAN_ASSERT_EVENTS | TSM_SCAN_HEADER_EVENTS | TSM_SCAN_REV_B;
-  CU(cudaSetDevice(c->device));
   cudaStream_t st = (cudaStream_t)stream;
-  CallOrder order(c, st);
-  CU(order.wait());
+  CallScope call(c, st);
+  CU(call.status);
   rc = upload_index(c, k, st);                            // the index first (small), the arena slab by slab
   if (rc != TSM_OK) return rc;
   c->resident = true;
@@ -677,11 +707,9 @@ extern "C" int tsm_reduce(tsm_ctx* c, const uint8_t* flags, const int32_t* repo,
     return TSM_E_ARG;
   for (int32_t i = 0; i < n_rows; ++i)
     if (repo[i] < 0 || repo[i] >= n_repos || case_id[i] < 0 || case_id[i] >= n_cases) return TSM_E_ARG;
-  CU(cudaSetDevice(c->device));
-  PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
-  CallOrder order(c, st);
-  CU(order.wait());
+  CallScope call(c, st);
+  CU(call.status);
   const size_t words = ((size_t)n_cases + 31) / 32;
   const size_t nbits = (size_t)(n_flags + 1) * n_repos * words;
   DevBuf b_flags, b_repo, b_case, b_bits, b_out;          // scratch from the ctx's pool (kept between calls)
@@ -737,6 +765,7 @@ namespace {
 struct HostSide {                                         // device image of one side of the pairs + its line records
   int32_t n = 0; size_t ab = 0; uint32_t unit_cap = 0;
   DevBuf arena, off, len, ext, grp, line_base, line_end, line_hash, line_flag;   // (grp: only for the changed assertion lines)
+  DevBuf line_mark;                                       // 1 = line deleted (old side) / inserted (new side): DIFF_MARKS only
   DevBuf unit_file, unit_begin, cnt, unit_first, bsum, zero, stats, unit_lines, unit_out, unit_line_base, s_hash, s_end, s_flag;
   std::vector<unsigned long long> base;                   // host copy of line_base (only when asked for)
   uint32_t n_units = 0;                                   // (file, chunk) work units: sum of ceil(len / 4 KiB)
@@ -808,7 +837,6 @@ int side_upload_grp(const tsm_corpus* k, HostSide& h, cudaStream_t st) {
 // size (the first pass counted them).  scan_ms adds the device time of the k_scan launches (CUDA events on st).
 // host_base: also copy line_base to the host (HostSide::base).
 static int side_scan_pass(tsm_ctx* c, HostSide& h, ScanParams& p, size_t cap, int side, cudaStream_t st) {
-  const int ev = side ? 6 : 0;
   h.pin_hc = reinterpret_cast<Ctrl*>(c->h_diff + 32 * side);            // pinned: the copies below do not stall the host
   h.pin_total = reinterpret_cast<unsigned long long*>(c->h_diff + 64 + 8 * side);
   const int32_t n = h.n;
@@ -818,9 +846,9 @@ static int side_scan_pass(tsm_ctx* c, HostSide& h, ScanParams& p, size_t cap, in
   p.lh_cap = (uint32_t)cap;
   CU(cudaMemsetAsync(h.zero.p, 0, 256 + sizeof(SlabCtl), st));
   k_plan_det<<<(n + 1 + 255) / 256, 256, 0, st>>>(p, h.unit_first.as<unsigned long long>());
-  CU(cudaEventRecord(c->diff_ev[ev], st));
-  k_scan_t<false><<<c->sms * SCAN2_CTAS_PER_SM, SCAN2_WARPS * 32, SCAN2_SMEM, st>>>(p);
-  CU(cudaEventRecord(c->diff_ev[ev + 1], st));
+  CU(cudaEventRecord(c->diff_ev[EV_SCAN[side].from], st));
+  launch_k_scan(c, p, false, st);
+  CU(cudaEventRecord(c->diff_ev[EV_SCAN[side].to], st));
   CU(cudaGetLastError());
   // lines per unit -> first line of every unit (the unit count is known on the host: units are (file, chunk) in order)
   xscan(p.unit_lines, h.n_units, h.bsum.as<unsigned long long>(), h.unit_line_base.as<unsigned long long>(), st);
@@ -856,16 +884,16 @@ int sides_records(tsm_ctx* c, HostSide* const* sides, int ns, cudaStream_t st, f
   CU(cudaStreamSynchronize(st));
   for (int i = 0; i < ns; ++i) {
     HostSide& h = *sides[i];
-    const int ev = i ? 6 : 0;
+    const EvSpan ev = EV_SCAN[i];
     h.hc = *h.pin_hc; h.total = *h.pin_total;
-    if (scan_ms) *scan_ms += elapsed_ms(c->diff_ev[ev], c->diff_ev[ev + 1]);
+    if (scan_ms) *scan_ms += elapsed_ms(c->diff_ev[ev.from], c->diff_ev[ev.to]);
     if (h.hc.overflow) return TSM_E_CAPACITY;
     if (h.hc.lh_overflow) {                                // more lines than the staging arrays hold: once more, exact size
       const int rc = side_scan_pass(c, h, ps[i], (size_t)h.hc.n_lh + 64, i, st);
       if (rc != TSM_OK) return rc;
       CU(cudaStreamSynchronize(st));
       h.hc = *h.pin_hc; h.total = *h.pin_total;
-      if (scan_ms) *scan_ms += elapsed_ms(c->diff_ev[ev], c->diff_ev[ev + 1]);
+      if (scan_ms) *scan_ms += elapsed_ms(c->diff_ev[ev.from], c->diff_ev[ev.to]);
       if (h.hc.overflow || h.hc.lh_overflow) return TSM_E_CAPACITY;
     }
   }
@@ -934,7 +962,8 @@ static int check_sides(std::initializer_list<const tsm_corpus*> sides, int32_t n
   return TSM_OK;
 }
 
-// Both sides of the revision pairs to the device (with_grp: their group tags too, for the assertion tables).
+// Both sides of the revision pairs to the device (with_grp: their group tags too, for the assertion tables).  Each side
+// is sized from its own corpus: the sides of tsm_similarity may differ in files (P.n is the count of `olds`).
 static int pair_upload(const tsm_corpus* olds, const tsm_corpus* news, bool with_grp, HostSidePair& P, cudaStream_t st) {
   P.n = olds->n_files;
   P.groups_a = olds->n_groups; P.groups_b = news->n_groups;
@@ -946,77 +975,78 @@ static int pair_upload(const tsm_corpus* olds, const tsm_corpus* news, bool with
   return rc;
 }
 
+// The line records of both uploaded sides of P (*scan_ms = k_scan over both; host_base: line_base of each side on the host too).
+static int pair_records(tsm_ctx* c, HostSidePair& P, float* scan_ms, bool host_base, cudaStream_t st) {
+  *scan_ms = 0;
+  P.A.launches = P.B.launches = 0;
+  HostSide* both[2] = {&P.A, &P.B};
+  return sides_records(c, both, 2, st, scan_ms, host_base);
+}
+
 // The diff proper over two sides whose line records exist.  k_diff_small finishes the common pairs (distance at most
 // 127 lines, middle of at most 4 096 lines) start to finish - search in registers, rows of V and backtrack in shared
-// memory - in four sizes (512 lines / D <= 31 at 32 pairs per SM, 1 024 / 63 at 12, 4 096 / 63 at 5, 4 096 / 127 at 3), each
-// fed on the device by the list the size before it leaves.  What all of them leave over (the `todo` list, normally empty) goes through k_myers (edit distance, V in global scratch) and, for `detail`,
+// memory - in the sizes of DS_SIZES, each fed on the device by the list the size before it leaves.  What all of them
+// leave over (the `todo` list, normally empty) goes through k_myers (edit distance, V in global scratch) and, for `detail`,
 // k_myers_trace (rows of V in global memory sized from those distances, then the canonical script: hunks, changed
 // assertion lines).  A pair whose distance D needs more than TSM_DIFF_TRACE_MAX_INTS trace entries ((D+1)(D+2)/2) is
 // not traced: it is reported as ONE hunk (add / del / mod by its counts) with added_assert = removed_assert = -1
-// (tosemscan.h).  diff_ms[1] = k_diff_small, diff_ms[2] = the two kernels of the left-over pairs.  With `sink` (needs
-// `detail`) the DIFF_EMIT variants of k_diff_small and k_myers_trace also list the changed assertion lines, or, when the sink
-// has marks, the DIFF_MARKS variants mark the deleted and inserted lines.
+// (tosemscan.h).  diff_ms[1] = k_diff_small, diff_ms[2] = the two kernels of the left-over pairs.
+// MODE (DiffMode) picks the variant of k_diff_small and k_myers_trace: DIFF_EMIT also lists the changed assertion lines
+// into the caller's sink, DIFF_MARKS marks the deleted and inserted lines into A.line_mark / B.line_mark (one zeroed byte
+// per line of each side).  Both find those lines on the paths that compute the detail (the assertion flags come with it),
+// so they compute it also when the caller passes none.
 template <int MODE>
-static void launch_diff_small(tsm_ctx* c, const HostSide& A, const HostSide& B, int32_t n, const uint8_t* fa, const uint8_t* fb,
-                              uint32_t* cnt, int32_t* const todo[4], long long* da, long long* dr, tsm_diff_detail* d_det,
-                              const AssertSink& sink, cudaStream_t st) {
-  constexpr uint32_t kSmem1 = DS1_WARPS * ds_warp_bytes(DS1_HCAP, DS1_DCAP), kSmem2 = DS2_WARPS * ds_warp_bytes(DS2_HCAP, DS2_DCAP),
-                     kSmem3 = DS3_WARPS * ds_warp_bytes(DS3_HCAP, DS3_DCAP), kSmem4 = DS4_WARPS * ds_warp_bytes(DS4_HCAP, DS4_DCAP);
-  static_assert(kSmem1 * 4 + 4 * 1024 <= 233472 && kSmem2 * 6 + 6 * 1024 <= 233472 && kSmem3 * 5 + 5 * 1024 <= 233472 &&
-                kSmem4 * 3 + 3 * 1024 <= 233472, "pairs per SM");
-  // (the kernels' dynamic shared memory limits are raised per device in tsm_create)
-  k_diff_small<DS1_HCAP, DS1_DCAP, DS1_WARPS, MODE><<<std::min((n + DS1_WARPS - 1) / DS1_WARPS, c->sms * 4), DS1_WARPS * 32, kSmem1, st>>>(
-      A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, nullptr, nullptr, n, cnt + 4, da, dr, d_det, todo[0], cnt + 0, sink);
-  k_diff_small<DS2_HCAP, DS2_DCAP, DS2_WARPS, MODE><<<std::min((n + DS2_WARPS - 1) / DS2_WARPS, c->sms * 6), DS2_WARPS * 32, kSmem2, st>>>(
-      A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, todo[0], cnt + 0, n, cnt + 5, da, dr, d_det, todo[1], cnt + 1, sink);
-  k_diff_small<DS3_HCAP, DS3_DCAP, DS3_WARPS, MODE><<<std::min(n, c->sms * 5), DS3_WARPS * 32, kSmem3, st>>>(
-      A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, todo[1], cnt + 1, n, cnt + 6, da, dr, d_det, todo[2], cnt + 2, sink);
-  k_diff_small<DS4_HCAP, DS4_DCAP, DS4_WARPS, MODE><<<std::min(n, c->sms * 3), DS4_WARPS * 32, kSmem4, st>>>(
-      A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, todo[2], cnt + 2, n, cnt + 7, da, dr, d_det, todo[3], cnt + 3, sink);
-}
-
 static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* added, int64_t* removed,
-                     tsm_diff_detail* detail, cudaStream_t st, const AssertSink* sink = nullptr) {
+                     tsm_diff_detail* detail, cudaStream_t st, AssertSink sink = {}) {
   static_assert(sizeof(long long) == sizeof(int64_t), "int64");
-  DevBuf d_add, d_rem, d_detail, d_todo1, d_todo2, d_todo3, d_todo, d_ntodo;
-  if (!d_add.alloc(sizeof(long long) * (size_t)n) || !d_rem.alloc(sizeof(long long) * (size_t)n) ||
-      !d_todo1.alloc(sizeof(int32_t) * (size_t)n) || !d_todo2.alloc(sizeof(int32_t) * (size_t)n) || !d_todo3.alloc(sizeof(int32_t) * (size_t)n) || !d_todo.alloc(sizeof(int32_t) * (size_t)n) ||
-      !d_ntodo.alloc(64) || (detail && !d_detail.alloc(sizeof(tsm_diff_detail) * (size_t)n)))
-    return TSM_E_CUDA;
-  if (sink && !detail) return TSM_E_ARG;
+  static_assert(2 * DS_N * sizeof(uint32_t) <= 64, "d_ntodo: two counters per size");
+  std::vector<tsm_diff_detail> own;
+  if (MODE != DIFF_PLAIN && !detail) { own.resize((size_t)n); detail = own.data(); }
+  if constexpr (MODE == DIFF_MARKS) {
+    if (!A.line_mark.alloc((size_t)A.total) || !B.line_mark.alloc((size_t)B.total)) return TSM_E_CUDA;
+    CU(cudaMemsetAsync(A.line_mark.p, 0, (size_t)A.total, st));
+    CU(cudaMemsetAsync(B.line_mark.p, 0, (size_t)B.total, st));
+    sink.mark[0] = A.line_mark.as<uint8_t>(); sink.mark[1] = B.line_mark.as<uint8_t>();
+  }
+  DevBuf d_add, d_rem, d_detail, d_todo[DS_N], d_ntodo;
+  bool ok = d_add.alloc(sizeof(long long) * (size_t)n) && d_rem.alloc(sizeof(long long) * (size_t)n);
+  for (DevBuf& t : d_todo) ok = ok && t.alloc(sizeof(int32_t) * (size_t)n);
+  if (!ok || !d_ntodo.alloc(64) || (detail && !d_detail.alloc(sizeof(tsm_diff_detail) * (size_t)n))) return TSM_E_CUDA;
   CU(cudaMemsetAsync(d_ntodo.p, 0, 64, st));
   CU(cudaMemsetAsync(d_add.p, 0, sizeof(long long) * (size_t)n, st));     // (the first copy back covers every pair, also the ones
-  CU(cudaMemsetAsync(d_rem.p, 0, sizeof(long long) * (size_t)n, st));     //  the four sizes leave to k_myers / k_myers_trace)
+  CU(cudaMemsetAsync(d_rem.p, 0, sizeof(long long) * (size_t)n, st));     //  the sizes leave to k_myers / k_myers_trace)
   if (detail) CU(cudaMemsetAsync(d_detail.p, 0, sizeof(tsm_diff_detail) * (size_t)n, st));
-  uint32_t* cnt = d_ntodo.as<uint32_t>();                  // [0..3] pairs each size left over, [4..7] the sizes' work counters
+  uint32_t* cnt = d_ntodo.as<uint32_t>();                  // [I] pairs size I left over, [DS_N + I] size I's work counter
   const uint8_t* fa = detail ? A.d.line_flag : nullptr;
   const uint8_t* fb = detail ? B.d.line_flag : nullptr;
   tsm_diff_detail* d_det = detail ? d_detail.as<tsm_diff_detail>() : nullptr;
-  long long* da = d_add.as<long long>();
-  long long* dr = d_rem.as<long long>();
-  int32_t* const todo_lists[4] = {d_todo1.as<int32_t>(), d_todo2.as<int32_t>(), d_todo3.as<int32_t>(), d_todo.as<int32_t>()};
-  CU(cudaEventRecord(c->diff_ev[2], st));
-  const int mode = !sink ? DIFF_PLAIN : sink->mark[0] ? DIFF_MARKS : DIFF_EMIT;
-  if (mode == DIFF_MARKS) launch_diff_small<DIFF_MARKS>(c, A, B, n, fa, fb, cnt, todo_lists, da, dr, d_det, *sink, st);
-  else if (mode == DIFF_EMIT) launch_diff_small<DIFF_EMIT>(c, A, B, n, fa, fb, cnt, todo_lists, da, dr, d_det, *sink, st);
-  else launch_diff_small<DIFF_PLAIN>(c, A, B, n, fa, fb, cnt, todo_lists, da, dr, d_det, AssertSink{}, st);
-  CU(cudaEventRecord(c->diff_ev[3], st));
+  int32_t* const d_left = d_todo[DS_N - 1].as<int32_t>();  // what the last size leaves over
+  CU(cudaEventRecord(c->diff_ev[EV_SMALL.from], st));
+  for_ds_sizes([&](auto i) {                               // size I: the pairs size I - 1 left over (size 0: all n)
+    constexpr int I = decltype(i)::value;
+    constexpr DiffSmallSize s = DS_SIZES[I];
+    k_diff_small<s.hcap, s.dcap, s.warps, MODE><<<std::min((n + s.warps - 1) / s.warps, c->sms * s.per_sm), s.warps * 32, s.smem(), st>>>(
+        A.d.line_hash, A.d.line_base, fa, B.d.line_hash, B.d.line_base, fb, I ? d_todo[I - 1].as<int32_t>() : nullptr,
+        I ? cnt + I - 1 : nullptr, n, cnt + DS_N + I, d_add.as<long long>(), d_rem.as<long long>(), d_det, d_todo[I].as<int32_t>(),
+        cnt + I, sink);
+  });
+  CU(cudaEventRecord(c->diff_ev[EV_SMALL.to], st));
   CU(cudaGetLastError());
   uint32_t* pin_nt = reinterpret_cast<uint32_t*>(c->h_diff + 80);
-  CU(cudaMemcpyAsync(pin_nt, cnt + 3, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(pin_nt, cnt + DS_N - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(added, d_add.p, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(removed, d_rem.p, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
   if (detail) CU(cudaMemcpyAsync(detail, d_detail.p, sizeof(tsm_diff_detail) * (size_t)n, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   A.drop_staging(); B.drop_staging();
   const uint32_t nt = *pin_nt;
-  c->diff_ms[1] = elapsed_ms(c->diff_ev[2], c->diff_ev[3]);
-  c->launches = A.launches + B.launches + 4;
+  c->diff_ms[1] = elapsed_ms(c->diff_ev[EV_SMALL.from], c->diff_ev[EV_SMALL.to]);
+  c->launches = A.launches + B.launches + DS_N;
   c->diff_ms[2] = 0;
   if (nt == 0) return TSM_OK;
   // ---- the left-over pairs: long middles, far-apart revisions
   std::vector<int32_t> todo(nt);
-  CU(cudaMemcpyAsync(todo.data(), d_todo.p, sizeof(int32_t) * (size_t)nt, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(todo.data(), d_left, sizeof(int32_t) * (size_t)nt, cudaMemcpyDeviceToHost, st));
   for (HostSide* h : {&A, &B})
     if (h->base.empty()) {
       h->base.assign((size_t)n + 1, 0);
@@ -1031,16 +1061,16 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
   DevBuf d_vbase, d_v;
   if (!d_vbase.alloc(sizeof(unsigned long long) * ((size_t)nt + 1)) || !d_v.alloc(sizeof(int32_t) * (size_t)vbase[nt])) return TSM_E_CUDA;
   CU(cudaMemcpyAsync(d_vbase.p, vbase.data(), sizeof(unsigned long long) * ((size_t)nt + 1), cudaMemcpyHostToDevice, st));
-  CU(cudaEventRecord(c->diff_ev[4], st));
+  CU(cudaEventRecord(c->diff_ev[EV_LEFT.from], st));
   k_myers<<<(nt * 32 + 127) / 128, 128, 0, st>>>(A.d.line_hash, A.d.line_base, B.d.line_hash, B.d.line_base, (int32_t)nt,
                                                 d_v.as<int32_t>(), d_vbase.as<unsigned long long>(),
-                                                d_add.as<long long>(), d_rem.as<long long>(), d_todo.as<int32_t>());
-  CU(cudaEventRecord(c->diff_ev[5], st));
+                                                d_add.as<long long>(), d_rem.as<long long>(), d_left);
+  CU(cudaEventRecord(c->diff_ev[EV_LEFT.to], st));
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(added, d_add.p, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(removed, d_rem.p, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  c->diff_ms[2] += elapsed_ms(c->diff_ev[4], c->diff_ev[5]);
+  c->diff_ms[2] += elapsed_ms(c->diff_ev[EV_LEFT.from], c->diff_ev[EV_LEFT.to]);
   c->launches++;
   if (!detail) return TSM_OK;
   // ---- their hunks: second search with the rows of V kept; rows sized from the distances just computed,
@@ -1069,27 +1099,16 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
     if (!d_trace.alloc(sizeof(int32_t) * (size_t)tot)) return TSM_E_CUDA;
     CU(cudaMemcpyAsync(d_tbase.as<unsigned long long>() + p0, tbase.data() + p0, sizeof(unsigned long long) * (size_t)(p1 - p0),
                        cudaMemcpyHostToDevice, st));
-    CU(cudaEventRecord(c->diff_ev[4], st));
+    CU(cudaEventRecord(c->diff_ev[EV_LEFT.from], st));
     const unsigned grid = ((p1 - p0) * 32 + 127) / 128;
-    if (mode == DIFF_MARKS)
-      k_myers_trace<DIFF_MARKS><<<grid, 128, 0, st>>>(
-          A.d.line_hash, A.d.line_base, A.d.line_flag, B.d.line_hash, B.d.line_base, B.d.line_flag, (int32_t)p0, (int32_t)(p1 - p0),
-          d_trace.as<int32_t>(), d_tbase.as<unsigned long long>(), d_add.as<long long>(), d_rem.as<long long>(),
-          (long long)TSM_DIFF_TRACE_MAX_D, d_detail.as<tsm_diff_detail>(), d_todo.as<int32_t>(), *sink);
-    else if (mode == DIFF_EMIT)
-      k_myers_trace<DIFF_EMIT><<<grid, 128, 0, st>>>(
-          A.d.line_hash, A.d.line_base, A.d.line_flag, B.d.line_hash, B.d.line_base, B.d.line_flag, (int32_t)p0, (int32_t)(p1 - p0),
-          d_trace.as<int32_t>(), d_tbase.as<unsigned long long>(), d_add.as<long long>(), d_rem.as<long long>(),
-          (long long)TSM_DIFF_TRACE_MAX_D, d_detail.as<tsm_diff_detail>(), d_todo.as<int32_t>(), *sink);
-    else
-      k_myers_trace<DIFF_PLAIN><<<grid, 128, 0, st>>>(
-          A.d.line_hash, A.d.line_base, A.d.line_flag, B.d.line_hash, B.d.line_base, B.d.line_flag, (int32_t)p0, (int32_t)(p1 - p0),
-          d_trace.as<int32_t>(), d_tbase.as<unsigned long long>(), d_add.as<long long>(), d_rem.as<long long>(),
-          (long long)TSM_DIFF_TRACE_MAX_D, d_detail.as<tsm_diff_detail>(), d_todo.as<int32_t>(), AssertSink{});
-    CU(cudaEventRecord(c->diff_ev[5], st));
+    k_myers_trace<MODE><<<grid, 128, 0, st>>>(
+        A.d.line_hash, A.d.line_base, A.d.line_flag, B.d.line_hash, B.d.line_base, B.d.line_flag, (int32_t)p0, (int32_t)(p1 - p0),
+        d_trace.as<int32_t>(), d_tbase.as<unsigned long long>(), d_add.as<long long>(), d_rem.as<long long>(),
+        (long long)TSM_DIFF_TRACE_MAX_D, d_detail.as<tsm_diff_detail>(), d_left, sink);
+    CU(cudaEventRecord(c->diff_ev[EV_LEFT.to], st));
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(st));
-    c->diff_ms[2] += elapsed_ms(c->diff_ev[4], c->diff_ev[5]);
+    c->diff_ms[2] += elapsed_ms(c->diff_ev[EV_LEFT.from], c->diff_ev[EV_LEFT.to]);
     c->launches++;
     p0 = p1;
   }
@@ -1109,8 +1128,6 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
 // one entry per line of its side, a bound known before the launch that no side can exceed.
 static int diff_asserts(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int32_t n_groups, int64_t* added, int64_t* removed,
                         tsm_diff_detail* detail, tsm_diff_asserts* out, cudaStream_t st) {
-  std::vector<tsm_diff_detail> own;                        // the lists need the assertion flags, which come with the detail
-  if (!detail) { own.resize((size_t)n); detail = own.data(); }
   HostSide* side[2] = {&A, &B};                            // side 0: deleted lines of `old`, side 1: inserted lines of `new`
   DevBuf d_list[2], d_ctrl, d_counts[2], d_aev[2];
   AssertSink sink{};
@@ -1124,7 +1141,7 @@ static int diff_asserts(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int32_t
     sink.line_end[s] = side[s]->d.line_end;
   }
   CU(cudaMemsetAsync(d_ctrl.p, 0, 2 * 64, st));            // n_cand = cls_done = 0
-  int rc = diff_core(c, A, B, n, added, removed, detail, st, &sink);
+  int rc = diff_core<DIFF_EMIT>(c, A, B, n, added, removed, detail, st, sink);
   if (rc != TSM_OK) return rc;
   Ctrl hc[2];
   for (int s = 0; s < 2; ++s) CU(cudaMemcpyAsync(&hc[s], ctrl[s], sizeof(Ctrl), cudaMemcpyDeviceToHost, st));
@@ -1135,8 +1152,7 @@ static int diff_asserts(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int32_t
   const int64_t h_cap[2] = {out->rev_cap, out->aev_cap};
   int64_t* const h_counts[2] = {out->removed_counts, out->added_counts};
   const size_t table = (size_t)(n_groups + 1) * TSM_K;     // [n_groups + 1][K]: k_classify also fills the global row
-  const size_t hist = CLS_SMEM_BASE + sizeof(uint32_t) * (n_groups <= 16 ? (size_t)n_groups * TSM_K : 0);
-  const uint32_t cls_wave = (uint32_t)(c->sms * classify_per_sm(c, hist));
+  const ClassifyShape cls = classify_shape(c, n_groups);
   for (int s = 0; s < 2; ++s) {
     if (!d_counts[s].alloc(sizeof(unsigned long long) * table) ||
         (h_ev[s] && !d_aev[s].alloc(sizeof(tsm_assert_event) * (size_t)std::max(nc[s], 1u))))
@@ -1151,7 +1167,7 @@ static int diff_asserts(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int32_t
     p.aev = d_aev[s].as<tsm_assert_event>(); p.aev_cap = h_ev[s] ? nc[s] : 0;
     p.counts = d_counts[s].as<unsigned long long>();
     p.flags = h_ev[s] ? TSM_SCAN_ASSERT_EVENTS : 0u;
-    k_classify_t<false><<<std::min<uint32_t>(cls_wave, (nc[s] + 255) / 256), 256, hist, st>>>(p);
+    launch_k_classify(p, false, std::min<uint32_t>(cls.wave, (nc[s] + 255) / 256), cls.smem, st);
     CU(cudaGetLastError());
     c->launches++;
   }
@@ -1169,16 +1185,13 @@ static int diff_asserts(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int32_t
 }
 
 // One diff call over the uploaded sides of P: their line records (diff_ms[0] = k_scan over both), then diff_core, or
-// diff_asserts when `out` is given.  The caller holds the pool scope and the SyncGuard of the call.
+// diff_asserts when `out` is given.  The caller holds the CallScope and the SyncGuard of the call.
 static int pair_run(tsm_ctx* c, HostSidePair& P, int64_t* added, int64_t* removed, tsm_diff_detail* detail,
                     tsm_diff_asserts* out, cudaStream_t st) {
-  c->diff_ms[0] = 0;
-  P.A.launches = P.B.launches = 0;
-  HostSide* both[2] = {&P.A, &P.B};
-  const int rc = sides_records(c, both, 2, st, &c->diff_ms[0], false);
+  const int rc = pair_records(c, P, &c->diff_ms[0], false, st);
   if (rc != TSM_OK) return rc;
   if (out) return diff_asserts(c, P.A, P.B, P.n, P.groups_a, added, removed, detail, out, st);
-  return diff_core(c, P.A, P.B, P.n, added, removed, detail, st);
+  return diff_core<DIFF_PLAIN>(c, P.A, P.B, P.n, added, removed, detail, st);
 }
 
 extern "C" int tsm_diff_pairs_detail(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news,
@@ -1187,13 +1200,11 @@ extern "C" int tsm_diff_pairs_detail(tsm_ctx* c, const tsm_corpus* olds, const t
   if (olds->n_files == 0) return TSM_OK;
   int rc = check_sides({olds, news}, olds->n_files, detail != nullptr);
   if (rc != TSM_OK) return rc;
-  CU(cudaSetDevice(c->device));
-  PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
-  CallOrder order(c, st);
-  CU(order.wait());
+  CallScope call(c, st);
+  CU(call.status);
   HostSidePair P;
-  SyncGuard guard(st);                                     // (after P) no buffer goes back to the pool while work on st may still use it
+  SyncGuard guard(st);
   rc = pair_upload(olds, news, false, P, st);
   return rc != TSM_OK ? rc : pair_run(c, P, added, removed, detail, nullptr, st);
 }
@@ -1219,11 +1230,9 @@ extern "C" int tsm_diff_pairs_asserts(tsm_ctx* c, const tsm_corpus* olds, const 
   }
   rc = check_sides({olds, news}, n, true);
   if (rc != TSM_OK) return rc;
-  CU(cudaSetDevice(c->device));
-  PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
-  CallOrder order(c, st);
-  CU(order.wait());
+  CallScope call(c, st);
+  CU(call.status);
   HostSidePair P;
   SyncGuard guard(st);
   rc = pair_upload(olds, news, true, P, st);
@@ -1235,12 +1244,10 @@ extern "C" int tsm_diff_upload(tsm_ctx* c, const tsm_corpus* olds, const tsm_cor
   if (!c || !olds || !news || olds->n_files != news->n_files || olds->n_files <= 0) return TSM_E_ARG;
   int rc = check_sides({olds, news}, olds->n_files, true);
   if (rc != TSM_OK) return rc;
-  CU(cudaSetDevice(c->device));
   cudaStream_t st = (cudaStream_t)stream;
-  CallOrder order(c, st);
-  CU(order.wait());
+  CallScope call(c, st);
+  CU(call.status);
   free_res_pair(c);
-  PoolScope pool_scope(&c->pool);
   SyncGuard guard(st);
   c->res_pair = new (std::nothrow) HostSidePair;
   if (!c->res_pair) return TSM_E_NOMEM;
@@ -1254,11 +1261,9 @@ extern "C" int tsm_diff_upload(tsm_ctx* c, const tsm_corpus* olds, const tsm_cor
 extern "C" int tsm_diff_resident(tsm_ctx* c, int64_t* added, int64_t* removed, tsm_diff_detail* detail, void* stream) {
   if (!c || !added || !removed) return TSM_E_ARG;
   if (!c->res_pair) return TSM_E_STATE;
-  CU(cudaSetDevice(c->device));
-  PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
-  CallOrder order(c, st);
-  CU(order.wait());
+  CallScope call(c, st);
+  CU(call.status);
   SyncGuard guard(st);
   return pair_run(c, *c->res_pair, added, removed, detail, nullptr, st);
 }
@@ -1270,11 +1275,9 @@ extern "C" int tsm_diff_resident_asserts(tsm_ctx* c, int64_t* added, int64_t* re
   if (c->res_pair->groups_a != c->res_pair->groups_b) return TSM_E_ARG;
   if (!c->res_pair->grp_ok) return TSM_E_LAYOUT;
   out->n_aev = out->n_rev = 0;
-  CU(cudaSetDevice(c->device));
-  PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
-  CallOrder order(c, st);
-  CU(order.wait());
+  CallScope call(c, st);
+  CU(call.status);
   SyncGuard guard(st);
   return pair_run(c, *c->res_pair, added, removed, detail, out, st);
 }
@@ -1286,34 +1289,6 @@ extern "C" int tsm_diff_last_ms(tsm_ctx* c, float* ms3) {
 }
 
 // ------------------------------------------------------------------------------------- SPEC section 14 line provenance
-// The line records of both uploaded sides with line_base on the host (diff_ms[0] = k_scan over both); line_base of each
-// side copied to base_old / base_new when given.
-static int marks_records(tsm_ctx* c, HostSidePair& P, int64_t* base_old, int64_t* base_new, cudaStream_t st) {
-  c->diff_ms[0] = 0;
-  P.A.launches = P.B.launches = 0;
-  HostSide* both[2] = {&P.A, &P.B};
-  const int rc = sides_records(c, both, 2, st, &c->diff_ms[0], true);
-  if (rc != TSM_OK) return rc;
-  const size_t bytes = sizeof(int64_t) * ((size_t)P.n + 1);
-  if (base_old) memcpy(base_old, P.A.base.data(), bytes);
-  if (base_new) memcpy(base_new, P.B.base.data(), bytes);
-  return TSM_OK;
-}
-
-// diff_core with the DIFF_MARKS kernels over two zeroed byte arrays, one per line of each side.  The marks come from the
-// paths of the detail (pure hunks, backtrack), so the detail is computed also when the caller does not want it.
-static int marks_diff(tsm_ctx* c, HostSidePair& P, int64_t* added, int64_t* removed, tsm_diff_detail* detail, DevBuf& del,
-                      DevBuf& ins, cudaStream_t st) {
-  std::vector<tsm_diff_detail> own;
-  if (!detail) { own.resize((size_t)P.n); detail = own.data(); }
-  if (!del.alloc((size_t)P.A.total) || !ins.alloc((size_t)P.B.total)) return TSM_E_CUDA;
-  CU(cudaMemsetAsync(del.p, 0, (size_t)P.A.total, st));
-  CU(cudaMemsetAsync(ins.p, 0, (size_t)P.B.total, st));
-  AssertSink sink{};
-  sink.mark[0] = del.as<uint8_t>(); sink.mark[1] = ins.as<uint8_t>();
-  return diff_core(c, P.A, P.B, P.n, added, removed, detail, st, &sink);
-}
-
 extern "C" int tsm_diff_pairs_marks(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
                                     tsm_diff_detail* detail, tsm_line_marks* mk, void* stream) {
   if (!c || !olds || !news || !added || !removed || !mk || !mk->line_base_old || !mk->line_base_new || olds->n_files != news->n_files)
@@ -1323,24 +1298,23 @@ extern "C" int tsm_diff_pairs_marks(tsm_ctx* c, const tsm_corpus* olds, const ts
   if (n == 0) { mk->line_base_old[0] = mk->line_base_new[0] = 0; return TSM_OK; }
   int rc = check_sides({olds, news}, n, true);
   if (rc != TSM_OK) return rc;
-  CU(cudaSetDevice(c->device));
-  PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
-  CallOrder order(c, st);
-  CU(order.wait());
+  CallScope call(c, st);
+  CU(call.status);
   HostSidePair P;
   SyncGuard guard(st);
   rc = pair_upload(olds, news, false, P, st);
-  if (rc == TSM_OK) rc = marks_records(c, P, mk->line_base_old, mk->line_base_new, st);
+  if (rc == TSM_OK) rc = pair_records(c, P, &c->diff_ms[0], true, st);
   if (rc != TSM_OK) return rc;
+  memcpy(mk->line_base_old, P.A.base.data(), sizeof(int64_t) * ((size_t)n + 1));
+  memcpy(mk->line_base_new, P.B.base.data(), sizeof(int64_t) * ((size_t)n + 1));
   mk->n_old = (int64_t)P.A.total; mk->n_new = (int64_t)P.B.total;
   if (mk->del_cap < mk->n_old || mk->ins_cap < mk->n_new) return TSM_E_CAPACITY;
   if ((mk->n_old && !mk->del) || (mk->n_new && !mk->ins)) return TSM_E_ARG;
-  DevBuf del, ins;
-  rc = marks_diff(c, P, added, removed, detail, del, ins, st);
+  rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
   if (rc != TSM_OK) return rc;
-  if (mk->n_old) CU(cudaMemcpyAsync(mk->del, del.p, (size_t)mk->n_old, cudaMemcpyDeviceToHost, st));
-  if (mk->n_new) CU(cudaMemcpyAsync(mk->ins, ins.p, (size_t)mk->n_new, cudaMemcpyDeviceToHost, st));
+  if (mk->n_old) CU(cudaMemcpyAsync(mk->del, P.A.line_mark.p, (size_t)mk->n_old, cudaMemcpyDeviceToHost, st));
+  if (mk->n_new) CU(cudaMemcpyAsync(mk->ins, P.B.line_mark.p, (size_t)mk->n_new, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return TSM_OK;
 }
@@ -1375,16 +1349,17 @@ extern "C" int tsm_blame_pairs(tsm_ctx* c, const tsm_corpus* olds, const tsm_cor
   }
   int rc = check_sides({olds, news}, n, true);
   if (rc != TSM_OK) return rc;
-  CU(cudaSetDevice(c->device));
-  PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
-  CallOrder order(c, st);
-  CU(order.wait());
+  CallScope call(c, st);
+  CU(call.status);
   HostSidePair P;
+  DevBuf d_prev, d_label, d_head, d_in_base, d_pairs, d_start, d_work, d_keep, d_out;
   SyncGuard guard(st);
   rc = pair_upload(olds, news, false, P, st);
-  if (rc == TSM_OK) rc = marks_records(c, P, line_base_old, line_base_new, st);
+  if (rc == TSM_OK) rc = pair_records(c, P, &c->diff_ms[0], true, st);
   if (rc != TSM_OK) return rc;
+  if (line_base_old) memcpy(line_base_old, P.A.base.data(), sizeof(int64_t) * ((size_t)n + 1));
+  if (line_base_new) memcpy(line_base_new, P.B.base.data(), sizeof(int64_t) * ((size_t)n + 1));
   *n_lines = (int64_t)P.B.total;
   const std::vector<unsigned long long>& la = P.A.base;
   const std::vector<unsigned long long>& lb = P.B.base;
@@ -1394,8 +1369,7 @@ extern "C" int tsm_blame_pairs(tsm_ctx* c, const tsm_corpus* olds, const tsm_cor
   }
   if (cap < *n_lines) return TSM_E_CAPACITY;
   if (*n_lines && !origin_out) return TSM_E_ARG;
-  DevBuf del, ins;
-  rc = marks_diff(c, P, added, removed, detail, del, ins, st);
+  rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
   if (rc != TSM_OK) return rc;
   // chains: heads in pair order, then stably by length, longest first
   std::vector<int32_t> heads, len;
@@ -1417,7 +1391,6 @@ extern "C" int tsm_blame_pairs(tsm_ctx* c, const tsm_corpus* olds, const tsm_cor
   }
   chain_start.push_back((int32_t)chain_pairs.size());
   const size_t n_in = (size_t)in_base[n];
-  DevBuf d_prev, d_label, d_head, d_in_base, d_pairs, d_start, d_work, d_keep, d_out;
   if (!d_prev.alloc(sizeof(int32_t) * (size_t)n) || !d_label.alloc(sizeof(int32_t) * (size_t)n) ||
       !d_head.alloc(sizeof(tsm_origin) * n_in) || !d_in_base.alloc(sizeof(int64_t) * ((size_t)n + 1)) ||
       !d_pairs.alloc(sizeof(int32_t) * (size_t)n) || !d_start.alloc(sizeof(int32_t) * ((size_t)n_chains + 1)) || !d_work.alloc(16) ||
@@ -1432,7 +1405,7 @@ extern "C" int tsm_blame_pairs(tsm_ctx* c, const tsm_corpus* olds, const tsm_cor
   CU(cudaMemsetAsync(d_work.p, 0, 16, st));
   CU(cudaEventRecord(c->blame_ev[0], st));
   k_blame<<<std::min((n_chains + 7) / 8, c->sms * 8), 256, 0, st>>>(
-      P.A.d.line_base, P.B.d.line_base, del.as<uint8_t>(), ins.as<uint8_t>(), d_prev.as<int32_t>(), d_label.as<int32_t>(),
+      P.A.d.line_base, P.B.d.line_base, P.A.line_mark.as<uint8_t>(), P.B.line_mark.as<uint8_t>(), d_prev.as<int32_t>(), d_label.as<int32_t>(),
       d_head.as<tsm_origin>(), d_in_base.as<long long>(), d_pairs.as<int32_t>(), d_start.as<int32_t>(), n_chains, d_work.as<uint32_t>(),
       d_keep.as<tsm_origin>(), d_out.as<tsm_origin>());
   CU(cudaEventRecord(c->blame_ev[1], st));
@@ -1494,20 +1467,15 @@ extern "C" int tsm_similarity(tsm_ctx* c, const tsm_corpus* olds, const tsm_corp
   int rc = check_sides({olds}, olds->n_files, false);
   if (rc == TSM_OK) rc = check_sides({news}, news->n_files, false);
   if (rc != TSM_OK) return rc;
-  PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
-  CallOrder order(c, st);
-  CU(order.wait());
+  CallScope call(c, st);
+  CU(call.status);
   HostSidePair P;
   SimLists LA, LB;
   DevBuf d_cand;
-  SyncGuard guard(st);                                     // (after the buffers) nothing goes back to the pool while st may use it
-  rc = side_upload(olds, P.A, st);
-  if (rc == TSM_OK) rc = side_upload(news, P.B, st);
-  if (rc != TSM_OK) return rc;
-  P.A.launches = P.B.launches = 0;
-  HostSide* both[2] = {&P.A, &P.B};
-  rc = sides_records(c, both, 2, st, &c->sim_ms[0], false);
+  SyncGuard guard(st);
+  rc = pair_upload(olds, news, false, P, st);
+  if (rc == TSM_OK) rc = pair_records(c, P, &c->sim_ms[0], false, st);
   if (rc != TSM_OK) return rc;
   const size_t nc = (size_t)n_cand;
   if (!d_cand.alloc(16 * nc + 64)) { cudaGetLastError(); return TSM_E_NOMEM; }
@@ -1518,22 +1486,22 @@ extern "C" int tsm_similarity(tsm_ctx* c, const tsm_corpus* olds, const tsm_corp
   CU(cudaMemcpyAsync(d_old, cand_old, sizeof(int32_t) * nc, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(d_new, cand_new, sizeof(int32_t) * nc, cudaMemcpyHostToDevice, st));
   CU(cudaMemsetAsync(d_next, 0, sizeof(unsigned long long), st));
-  CU(cudaEventRecord(c->diff_ev[2], st));
+  CU(cudaEventRecord(c->diff_ev[EV_SIM_LISTS], st));
   rc = sim_lists(P.A, LA, st);
   if (rc == TSM_OK) rc = sim_lists(P.B, LB, st);
   if (rc != TSM_OK) return rc;
-  CU(cudaEventRecord(c->diff_ev[3], st));
+  CU(cudaEventRecord(c->diff_ev[EV_SIM_PAIRS], st));
   const unsigned grid = (unsigned)std::min<size_t>((size_t)c->sms * 8, (nc + 8 * SIM_GRAB - 1) / (8 * SIM_GRAB));
   k_similarity<<<grid, 256, 0, st>>>(LA.key.as<unsigned long long>(), LA.w.as<uint32_t>(), LA.base.as<unsigned long long>(),
                                      LB.key.as<unsigned long long>(), LB.w.as<uint32_t>(), LB.base.as<unsigned long long>(),
                                      d_old, d_new, (unsigned long long)nc, d_next, d_common);
   CU(cudaGetLastError());
-  CU(cudaEventRecord(c->diff_ev[4], st));
+  CU(cudaEventRecord(c->diff_ev[EV_SIM_END], st));
   CU(cudaMemcpyAsync(common, d_common, sizeof(int64_t) * nc, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   P.A.drop_staging(); P.B.drop_staging();
-  c->sim_ms[1] = elapsed_ms(c->diff_ev[2], c->diff_ev[3]);
-  c->sim_ms[2] = elapsed_ms(c->diff_ev[3], c->diff_ev[4]);
+  c->sim_ms[1] = elapsed_ms(c->diff_ev[EV_SIM_LISTS], c->diff_ev[EV_SIM_PAIRS]);
+  c->sim_ms[2] = elapsed_ms(c->diff_ev[EV_SIM_PAIRS], c->diff_ev[EV_SIM_END]);
   c->launches = P.A.launches + P.B.launches + 2 * 5 + 1;   // per side k_sim_sort, xscan (3), k_sim_compact; k_similarity
   return TSM_OK;
 }
@@ -1557,11 +1525,9 @@ static int line_records(tsm_ctx* c, const tsm_corpus* k, bool ext_rule, int64_t*
   if (n == 0) return TSM_OK;
   int rc = check_sides({k}, n, ext_rule);
   if (rc != TSM_OK) return rc;
-  CU(cudaSetDevice(c->device));
-  PoolScope pool_scope(&c->pool);
   cudaStream_t st = (cudaStream_t)stream;
-  CallOrder order(c, st);
-  CU(order.wait());
+  CallScope call(c, st);
+  CU(call.status);
   HostSide S;
   SyncGuard guard(st);
   rc = side_upload(k, S, st);

@@ -7,7 +7,7 @@
 //   k_diff_small    warp per pair, the common case in ONE kernel: common prefix / suffix trim by ballots, the middle
 //                   hash sequences staged in shared memory, the greedy furthest-reaching D-path search with the
 //                   diagonals of one D across the lanes and V in REGISTERS (neighbour diagonals by shuffle), the rows
-//                   of V kept in shared memory, the canonical backtrack by lane 0.  Four sizes (DS1 .. DS4: staged lines,
+//                   of V kept in shared memory, the canonical backtrack by lane 0.  Four sizes (DS_SIZES: staged lines,
 //                   largest distance, pairs per SM), each fed by the list the size before it leaves; a pair none of
 //                   them holds (middle above 4 096 lines, distance above 127) is left to the two kernels below
 //   k_myers         warp per pair: the same search with V in global scratch (any size)
@@ -90,15 +90,30 @@ __device__ __forceinline__ void snake_gmem(const unsigned long long* a, const un
   }
 }
 
-// Four sizes of the same kernel: <lines of both middles staged per warp, largest distance, warps per block>.  The rows of
-// V ((DCAP+1)(DCAP+2)/2 ints) and the staged middle (9 B per line) fix the shared memory per pair, hence the pairs in
-// flight per SM: most pairs are small, the few large ones decide the tail.
-constexpr int DS1_HCAP = 512, DS1_DCAP = 31, DS1_WARPS = 8;     //  6.6 KB per pair: 32 pairs per SM
-constexpr int DS2_HCAP = 1024, DS2_DCAP = 63, DS2_WARPS = 2;    // 17.3 KB per pair: 12 pairs per SM
-constexpr int DS3_HCAP = 4096, DS3_DCAP = 63, DS3_WARPS = 1;    // 44.3 KB per pair:  5 pairs per SM
-constexpr int DS4_HCAP = 4096, DS4_DCAP = 127, DS4_WARPS = 1;   // 68.3 KB per pair:  3 pairs per SM (a handful of far-apart pairs)
 __host__ __device__ constexpr uint32_t ds_rows(int dcap) { return (uint32_t)((dcap + 1) * (dcap + 2) / 2); }
 __host__ __device__ constexpr uint32_t ds_warp_bytes(int hcap, int dcap) { return (uint32_t)hcap * 8u + ds_rows(dcap) * 4u + (uint32_t)hcap; }
+
+// Four sizes of the same kernel, k_diff_small<hcap, dcap, warps, MODE>, launched in this order: lines of both middles
+// staged per warp, largest distance, warps per block, and the blocks per SM that the launch asks for.  The rows of V
+// ((dcap+1)(dcap+2)/2 ints) and the staged middle (9 B per line) fix the shared memory per pair, hence the pairs in
+// flight per SM: most pairs are small, the few large ones decide the tail.
+struct DiffSmallSize {
+  int hcap, dcap, warps, per_sm;
+  constexpr uint32_t smem() const { return (uint32_t)warps * ds_warp_bytes(hcap, dcap); }   // dynamic shared memory per block
+};
+constexpr DiffSmallSize DS_SIZES[] = {
+    {512, 31, 8, 4},      //  6.6 KB per pair: 32 pairs per SM
+    {1024, 63, 2, 6},     // 17.3 KB per pair: 12 pairs per SM
+    {4096, 63, 1, 5},     // 44.3 KB per pair:  5 pairs per SM
+    {4096, 127, 1, 3},    // 68.3 KB per pair:  3 pairs per SM (a handful of far-apart pairs)
+};
+constexpr int DS_N = (int)(sizeof(DS_SIZES) / sizeof(DS_SIZES[0]));
+constexpr bool ds_sizes_fit() {   // per_sm blocks of each size in the 228 KB of an SM, 1 KB reserved per block
+  for (const DiffSmallSize& s : DS_SIZES)
+    if (s.per_sm * (s.smem() + 1024) > 233472) return false;
+  return true;
+}
+static_assert(ds_sizes_fit(), "pairs per SM");
 
 // One pair start to finish; false = left to the next size (middle longer than HCAP lines or distance above DCAP).
 //   * V of row d lives in REGISTERS: entry j (diagonal k = -d + 2 j) in lane j % 32, register j / 32.  Row d + 1 needs
