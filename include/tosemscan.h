@@ -240,6 +240,28 @@ int tsm_blame_last_ms(tsm_ctx* ctx, float* ms);
 int tsm_line_hashes(tsm_ctx* ctx, const tsm_corpus* corpus, int64_t* line_base, uint64_t* line_hash, uint32_t* line_end,
                     uint8_t* line_flag, int64_t cap, int64_t* n_lines, int32_t ngram_n, uint64_t* ngram_hash, void* stream);
 
+/* Duplicated test code (docs/SPEC.md section 15, `tosem-scan clones`): the maximal classes of windows of min_lines lines (1 to
+ * 1024, else TSM_E_ARG) whose n-gram keys (section 3) are equal, in the global line order of section 3 (files in order).  A class
+ * is its fragments [member[j], member[j] + class_len[c]) for class_base[c] <= j < class_base[c+1]; classes are in ascending
+ * order of their first fragment, fragments in ascending order of start.  file_dup[f] / file_dup_assert[f]: the lines of file f
+ * inside some fragment, and those of them that are assertion lines (section 4, Rev A, by the file's ext).  Any pointer of the
+ * result may be NULL (that output is skipped); n_classes and n_members are always set.  class_base holds class_cap + 1
+ * entries, class_len class_cap, member member_cap: if class_cap < n_classes or member_cap < n_members the call returns
+ * TSM_E_CAPACITY with both counts set: size the arrays and call again (the call is redone).  n_files = 0 is legal.  The
+ * grouping table has 28 B per slot and two to four slots per line of the corpus; TSM_E_NOMEM is returned when it does not fit
+ * the device's free memory.
+ * Kernels: k_scan for the line records, k_ngrams for the keys, then grouping through one open-addressing hash table, the
+ * class lengths by warp ballots, a sort of every class' fragments and the coverage (csrc/tsm_clone_kernels.cuh).
+ * tsm_clones_last_ms: device time of the last call, ms3 = { k_scan, grouping + classes, members + coverage }. */
+typedef struct tsm_clone_result {
+  int64_t* line_base;                                    /* [n_files+1] */
+  uint32_t* file_dup; uint32_t* file_dup_assert;         /* [n_files] */
+  int64_t* class_base; uint32_t* class_len; int64_t class_cap; int64_t n_classes;
+  int64_t* member; int64_t member_cap; int64_t n_members;   /* global first line of each fragment */
+} tsm_clone_result;
+int tsm_clones(tsm_ctx* ctx, const tsm_corpus* corpus, int32_t min_lines, tsm_clone_result* out, void* stream);
+int tsm_clones_last_ms(tsm_ctx* ctx, float* ms3);
+
 /* Body statements (docs/SPEC.md section 10; Important-files/ML-Analysis-v4.xlsx!Apollo:R2-R26, golden G2): the
  * kind of every line of every file - 0 blank, 1 first line of a statement, 2 continuation (lines
  * are joined while the parentheses are open).  line_base[n_files+1] and *n_lines are always filled;

@@ -66,6 +66,8 @@ rec("blame_pairs", list(s.blame_pairs(ts.pack(ob + [nb[0]], ext + [1]), ts.pack(
 co = np.array(list(range(n)) + list(range(n - 1)), np.int32)
 cn = np.array(list(range(n)) + list(range(1, n)), np.int32)
 rec("similarity", s.similarity(A, ts.pack(nb + [b"z\n"], ext + [1]), co, cn))
+cl = s.clones(ts.pack(ob + nb, ext + ext), 3)
+rec("clones", [cl[k] for k in ("line_base", "file_dup", "file_dup_assert", "class_base", "class_len", "member")])
 rec("line_hashes", list(s.line_hashes(A, ngram=3)))
 rec("statements", list(s.statements(A)))
 s.close()

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Small scan (Rev A and Rev B) + line records + diff (plain, assertion lines, marks, provenance) + similarity + statements + reduce under compute-sanitizer (run: compute-sanitizer --tool memcheck python tools/sanitize_smoke.py)."""
+"""Small scan (Rev A and Rev B) + line records + diff (plain, assertion lines, marks, provenance) + similarity + clones + statements + reduce under compute-sanitizer (run: compute-sanitizer --tool memcheck python tools/sanitize_smoke.py)."""
 import os
 import sys
 
@@ -34,6 +34,9 @@ g = s.blame_pairs(ts.pack([far_o[0], far_n[0]], [1, 1]), ts.pack([far_n[0], far_
                   {0: np.array([(-1, j + 1) for j in range(lines0)], ts.ORIGIN)})
 print(len(g[4]), g[4][:3])
 print(s.similarity(fo, ts.pack(far_n + [b"m1\nm2\n"], [1, 1, 1]), [0, 1, 1], [0, 1, 2]))
+lic = b"".join(b"# licence %d\n" % i for i in range(8))    # clone classes: warp-sorted, CTA-sorted and tiled (> 4 096 fragments)
+cl = s.clones(ts.pack(far_o + far_n + [lic + (b"x\n" if i % 50 else b"") + b"f%d\n" % i for i in range(4200)], [1] * 4204), 3)
+print(len(cl["class_len"]), int(cl["file_dup"].sum()), int(cl["class_len"].max()))
 print([x[:4] for x in s.line_hashes(ts.pack(files[:40], exts[:40]), ngram=3)])
 r4 = s.scan(ts.pack(files, exts, grps, 5), 3 | ts.SCAN_REV_B)
 print(s.statements(c)[0][-1])

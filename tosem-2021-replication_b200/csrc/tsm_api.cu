@@ -18,6 +18,7 @@
 #include "tsm_stmt_kernels.cuh"
 #include "tsm_lines_kernels.cuh"
 #include "tsm_similar_kernels.cuh"
+#include "tsm_clone_kernels.cuh"
 
 using namespace tsm;
 
@@ -96,6 +97,7 @@ struct tsm_ctx {
   uint8_t* h_diff = nullptr;               // 256 B pinned: what the diff path reads back between its kernels (Ctrl x 2, line totals, todo count)
   float diff_ms[3] = {0, 0, 0};            // k_scan over both sides, k_myers, k_myers_trace of the last diff
   float sim_ms[3] = {0, 0, 0};             // k_scan over both sides, sort / merge, k_similarity of the last tsm_similarity
+  float clone_ms[3] = {0, 0, 0};           // k_scan, grouping + classes, members + coverage of the last tsm_clones
   cudaEvent_t blame_ev[2] = {};            // around k_blame (tsm_blame_last_ms)
   float blame_ms = 0;
   struct HostSidePair* res_pair = nullptr; // sides kept in HBM by tsm_diff_upload
@@ -124,10 +126,12 @@ struct tsm_ctx {
 
 // Slots of tsm_ctx::diff_ev.  The line records of a revision pair: k_scan of side s from EV_SCAN[s].from to .to.  The diff:
 // k_diff_small over EV_SMALL, each launch for the pairs it leaves over EV_LEFT.  tsm_similarity: the sorted lists of both
-// sides from EV_SIM_LISTS to EV_SIM_PAIRS, k_similarity from there to EV_SIM_END.
+// sides from EV_SIM_LISTS to EV_SIM_PAIRS, k_similarity from there to EV_SIM_END.  tsm_clones: grouping and classes from
+// EV_CLONE_GROUP to EV_CLONE_MEMBERS, members and coverage from there to EV_CLONE_END.
 struct EvSpan { int from, to; };
 constexpr EvSpan EV_SCAN[2] = {{0, 1}, {6, 7}}, EV_SMALL = {2, 3}, EV_LEFT = {4, 5};
 constexpr int EV_SIM_LISTS = 2, EV_SIM_PAIRS = 3, EV_SIM_END = 4;
+constexpr int EV_CLONE_GROUP = 2, EV_CLONE_MEMBERS = 3, EV_CLONE_END = 4;
 
 // The start of every call that queues device work on st: the ctx's device, the ctx's pool for the call's DevBufs, and the
 // order of the ctx's calls.  A ctx orders its own work, whatever stream each call is given: the call's stream first waits
@@ -326,7 +330,8 @@ extern "C" int tsm_create(tsm_ctx** out, int device, int64_t max_arena_bytes, in
         cudaFuncSetAttribute(k_scan_t<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN2_SMEM) != cudaSuccess ||
         cudaFuncSetAttribute(k_scan_t<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN2_SMEM_B) != cudaSuccess ||
         !diff_small_smem<DIFF_PLAIN>() || !diff_small_smem<DIFF_EMIT>() || !diff_small_smem<DIFF_MARKS>() ||
-        cudaFuncSetAttribute(k_sim_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SIM_SORT_SMEM) != cudaSuccess)
+        cudaFuncSetAttribute(k_sim_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SIM_SORT_SMEM) != cudaSuccess ||
+        cudaFuncSetAttribute(k_clone_sort_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SIM_SORT_SMEM) != cudaSuccess)
       rc = TSM_E_CUDA;
   }
   // The arena memset runs on the legacy stream and the last constant-table copy may still be in flight: a first call on
@@ -1516,9 +1521,10 @@ extern "C" int tsm_similarity_last_ms(tsm_ctx* c, float* ms3) {
 // The front of tsm_line_hashes and tsm_statements: the corpus' line records from one pass of the scan, and line_base[n+1]
 // and *n_lines on the host - also when cap is short of the lines, which returns TSM_E_CAPACITY so that the caller can
 // allocate and call again.  Then tail(S, lines, st), the call's own use of the records, inside the call's SyncGuard.
+// scan_ms: the device time of the k_scan launches.
 template <typename Tail>
 static int line_records(tsm_ctx* c, const tsm_corpus* k, bool ext_rule, int64_t* line_base, int64_t cap, int64_t* n_lines,
-                        void* stream, Tail tail) {
+                        void* stream, Tail tail, float* scan_ms = nullptr) {
   const int32_t n = k->n_files;
   *n_lines = 0;
   line_base[0] = 0;
@@ -1531,7 +1537,7 @@ static int line_records(tsm_ctx* c, const tsm_corpus* k, bool ext_rule, int64_t*
   HostSide S;
   SyncGuard guard(st);
   rc = side_upload(k, S, st);
-  if (rc == TSM_OK) rc = side_records(c, S, st, nullptr);
+  if (rc == TSM_OK) rc = side_records(c, S, st, scan_ms);
   if (rc != TSM_OK) return rc;
   const unsigned long long total = S.base[(size_t)n];
   for (int32_t i = 0; i <= n; ++i) line_base[i] = (int64_t)S.base[(size_t)i];
@@ -1582,4 +1588,117 @@ extern "C" int tsm_statements(tsm_ctx* c, const tsm_corpus* k, int64_t* line_bas
     c->launches += 2;
     return TSM_OK;
   });
+}
+
+// ------------------------------------------------------------------------------------- SPEC section 15 clones
+// The line records of the corpus (line_records), then the kernels of tsm_clone_kernels.cuh.  One synchronisation between
+// the grouping and the members reads the class and fragment counts: a short cap returns there, else the fragments are
+// scattered, sorted and copied back with the coverage.
+extern "C" int tsm_clones(tsm_ctx* c, const tsm_corpus* k, int32_t min_lines, tsm_clone_result* out, void* stream) {
+  if (!c || !k || !out || k->n_files < 0 || min_lines < 1 || min_lines > 1024 || out->class_cap < 0 || out->member_cap < 0) return TSM_E_ARG;
+  const int32_t nf = k->n_files;
+  for (float& v : c->clone_ms) v = 0;
+  c->launches = 0;
+  out->n_classes = out->n_members = 0;
+  if (out->class_base) out->class_base[0] = 0;
+  if (out->file_dup) memset(out->file_dup, 0, sizeof(uint32_t) * (size_t)nf);
+  if (out->file_dup_assert) memset(out->file_dup_assert, 0, sizeof(uint32_t) * (size_t)nf);
+  std::vector<int64_t> own_base;
+  int64_t* line_base = out->line_base;
+  if (!line_base) { own_base.resize((size_t)nf + 1); line_base = own_base.data(); }
+  int64_t n_lines = 0;
+  return line_records(c, k, true, line_base, INT64_MAX, &n_lines, stream, [&](const HostSide& S, unsigned long long total, cudaStream_t st) -> int {
+    const uint32_t T = (uint32_t)total, n = (uint32_t)min_lines, nfu = (uint32_t)S.n;
+    size_t slots = 1;                                      // a power of two, at least 2 x the windows (<= lines)
+    while (slots < 2 * (size_t)total) slots <<= 1;
+    const uint32_t mask = (uint32_t)(slots - 1);
+    const size_t table_bytes = (slots + 1) * (sizeof(CloneSlot) + 3 * sizeof(uint32_t));
+    {
+      size_t free_b = 0, total_b = 0;
+      CU(cudaMemGetInfo(&free_b, &total_b));
+      if (table_bytes > free_b) return TSM_E_NOMEM;
+    }
+    const size_t L = (size_t)total, nb = L / XS_TILE + 4;
+    DevBuf d_key, d_slot, d_wflag, d_table, d_plo, d_phi, d_scls, d_dup, d_head, d_ext, d_cidx, d_cover, d_rep, d_size, d_cbase,
+        d_big, d_nbig, d_bsum, d_len, d_cursor, d_member, d_wk, d_fdup;
+    if (!d_key.alloc(8 * L) || !d_slot.alloc(4 * L) || !d_wflag.alloc(L) || !d_table.alloc(sizeof(CloneSlot) * (slots + 1)) ||
+        !d_plo.alloc(4 * (slots + 1)) || !d_phi.alloc(4 * (slots + 1)) || !d_scls.alloc(4 * (slots + 1)) || !d_dup.alloc(4 * L) ||
+        !d_head.alloc(4 * L) || !d_ext.alloc(L) || !d_cidx.alloc(8 * (L + 1)) || !d_cover.alloc(8 * (L + 1)) || !d_rep.alloc(4 * L) ||
+        !d_size.alloc(4 * L) || !d_cbase.alloc(8 * (L + 1)) || !d_big.alloc(4 * L) || !d_nbig.alloc(4) || !d_bsum.alloc(8 * nb) ||
+        !d_len.alloc(4 * L) || !d_fdup.alloc(8 * (size_t)nfu)) {
+      cudaGetLastError();
+      return TSM_E_NOMEM;
+    }
+    CloneSlot* table = d_table.as<CloneSlot>();
+    uint32_t* slot_of = d_slot.as<uint32_t>();
+    const unsigned grid = (unsigned)((L + 255) / 256);
+    CU(cudaEventRecord(c->diff_ev[EV_CLONE_GROUP], st));
+    CU(cudaMemsetAsync(d_table.p, 0, sizeof(CloneSlot) * (slots + 1), st));
+    CU(cudaMemsetAsync(d_plo.p, 0xFF, 4 * (slots + 1), st));
+    CU(cudaMemsetAsync(d_phi.p, 0, 4 * (slots + 1), st));
+    CU(cudaMemsetAsync(d_scls.p, 0xFF, 4 * (slots + 1), st));
+    CU(cudaMemsetAsync(d_size.p, 0, 4 * L, st));
+    CU(cudaMemsetAsync(d_nbig.p, 0, 4, st));
+    k_ngrams<<<grid, 256, 0, st>>>(S.d.line_hash, S.d.line_base, nfu, total, n, d_key.as<unsigned long long>());
+    k_clone_insert<<<grid, 256, 0, st>>>(d_key.as<unsigned long long>(), S.d.line_base, nfu, S.d.line_end, S.d.arena, S.d.off, T, n, table,
+                                         mask, slot_of, d_wflag.as<uint8_t>());
+    k_clone_preds<<<grid, 256, 0, st>>>(table, slot_of, d_wflag.as<uint8_t>(), T, d_plo.as<uint32_t>(), d_phi.as<uint32_t>());
+    k_clone_heads<<<grid, 256, 0, st>>>(table, slot_of, d_plo.as<uint32_t>(), d_phi.as<uint32_t>(), T, d_dup.as<uint32_t>(),
+                                        d_head.as<uint32_t>(), d_ext.as<uint8_t>());
+    xscan(d_head.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), d_cidx.as<unsigned long long>(), st);
+    xscan(d_dup.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), d_cover.as<unsigned long long>(), st);
+    k_clone_classes<<<grid, 256, 0, st>>>(d_head.as<uint32_t>(), d_cidx.as<unsigned long long>(), slot_of, table, T, d_rep.as<uint32_t>(),
+                                          d_size.as<uint32_t>(), d_scls.as<uint32_t>(), d_big.as<uint32_t>(), d_nbig.as<uint32_t>());
+    xscan(d_size.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), d_cbase.as<unsigned long long>(), st);
+    k_clone_length<<<(unsigned)c->sms * 8, 256, 0, st>>>(d_rep.as<uint32_t>(), d_ext.as<uint8_t>(), T, n, d_cidx.as<unsigned long long>() + L,
+                                                         d_len.as<uint32_t>());
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_CLONE_MEMBERS], st));
+    unsigned long long* pin = reinterpret_cast<unsigned long long*>(c->h_diff + 128);   // classes, fragments, large classes
+    CU(cudaMemcpyAsync(pin, d_cidx.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(pin + 1, d_cbase.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(pin + 2, d_nbig.p, 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    c->launches += 15;                                     // k_ngrams, insert, preds, heads, 3 x xscan (3 each), classes, length
+    const uint32_t nc = (uint32_t)pin[0], nbig = (uint32_t)(pin[2] & 0xFFFFFFFFu);
+    const unsigned long long nm = pin[1];
+    out->n_classes = (int64_t)nc;
+    out->n_members = (int64_t)nm;
+    c->clone_ms[1] = elapsed_ms(c->diff_ev[EV_CLONE_GROUP], c->diff_ev[EV_CLONE_MEMBERS]);
+    if ((out->class_cap < (int64_t)nc && (out->class_base || out->class_len)) || (out->member_cap < (int64_t)nm && out->member))
+      return TSM_E_CAPACITY;
+    if (nc) {
+      if (!d_cursor.alloc(4 * (size_t)nc) || !d_member.alloc(8 * nm) || !d_wk.alloc(4 * nm)) { cudaGetLastError(); return TSM_E_NOMEM; }
+      unsigned long long* member = d_member.as<unsigned long long>();
+      CU(cudaMemsetAsync(d_cursor.p, 0, 4 * (size_t)nc, st));
+      k_clone_scatter<<<grid, 256, 0, st>>>(slot_of, d_scls.as<uint32_t>(), d_cbase.as<unsigned long long>(), T, d_cursor.as<uint32_t>(), member);
+      k_clone_sort_warp<<<(unsigned)(((size_t)nc * 32 + 255) / 256), 256, 0, st>>>(d_cbase.as<unsigned long long>(), nc, member);
+      c->launches += 2;
+      if (nbig) {
+        k_clone_sort_cta<<<std::min<unsigned>(nbig, (unsigned)c->sms * 2), SIM_SORT_THREADS, SIM_SORT_SMEM, st>>>(
+            d_cbase.as<unsigned long long>(), d_big.as<uint32_t>(), d_nbig.as<uint32_t>(), member, d_wk.as<uint32_t>());
+        c->launches += 1;
+      }
+      uint32_t* fdup = d_fdup.as<uint32_t>();
+      k_clone_cover<<<(unsigned)(((size_t)nfu * 32 + 255) / 256), 256, 0, st>>>(S.d.line_base, nfu, d_cover.as<unsigned long long>(),
+                                                                              S.d.line_flag, n, fdup, fdup + nfu);
+      c->launches += 1;
+      CU(cudaGetLastError());
+      CU(cudaEventRecord(c->diff_ev[EV_CLONE_END], st));
+      if (out->file_dup) CU(cudaMemcpyAsync(out->file_dup, fdup, 4 * (size_t)nfu, cudaMemcpyDeviceToHost, st));
+      if (out->file_dup_assert) CU(cudaMemcpyAsync(out->file_dup_assert, fdup + nfu, 4 * (size_t)nfu, cudaMemcpyDeviceToHost, st));
+      if (out->class_base) CU(cudaMemcpyAsync(out->class_base, d_cbase.p, 8 * ((size_t)nc + 1), cudaMemcpyDeviceToHost, st));
+      if (out->class_len) CU(cudaMemcpyAsync(out->class_len, d_len.p, 4 * (size_t)nc, cudaMemcpyDeviceToHost, st));
+      if (out->member) CU(cudaMemcpyAsync(out->member, member, 8 * nm, cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      c->clone_ms[2] = elapsed_ms(c->diff_ev[EV_CLONE_MEMBERS], c->diff_ev[EV_CLONE_END]);
+    }
+    return TSM_OK;
+  }, &c->clone_ms[0]);
+}
+
+extern "C" int tsm_clones_last_ms(tsm_ctx* c, float* ms3) {
+  if (!c || !ms3) return TSM_E_ARG;
+  for (int i = 0; i < 3; ++i) ms3[i] = c->clone_ms[i];
+  return TSM_OK;
 }

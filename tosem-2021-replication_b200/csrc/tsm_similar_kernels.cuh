@@ -49,6 +49,24 @@ __device__ __forceinline__ void bitonic_pass(unsigned long long* key, uint32_t* 
 
 __device__ __forceinline__ uint32_t pow2_at_least(uint32_t n) { return n <= 1 ? 1u : 1u << (32 - __clz(n - 1)); }
 
+// The rest of an ascending bitonic sort of gk/gw[0, n) in global memory (n > SIM_SMEM_LINES, n2 = pow2_at_least(n)) whose
+// tiles of SIM_SMEM_LINES are already sorted: the passes of distance >= a tile over global memory, the passes inside a tile
+// in shared memory (sk / sw: one tile).  Called by the whole CTA.
+__device__ __forceinline__ void bitonic_merge_tiles(unsigned long long* gk, uint32_t* gw, uint32_t n, uint32_t n2,
+                                                    unsigned long long* sk, uint32_t* sw) {
+  for (uint32_t k = 2 * SIM_SMEM_LINES; k <= n2; k <<= 1) {
+    for (uint32_t j = k >> 1; j >= SIM_SMEM_LINES; j >>= 1) bitonic_pass(gk, gw, n, n2, k, j);
+    for (uint32_t t0 = 0; t0 < n; t0 += SIM_SMEM_LINES) {   // the passes inside a tile (j < tile, never the mirror pass)
+      const uint32_t m = min(SIM_SMEM_LINES, n - t0);
+      for (uint32_t i = threadIdx.x; i < m; i += blockDim.x) { sk[i] = gk[t0 + i]; sw[i] = gw[t0 + i]; }
+      __syncthreads();
+      for (uint32_t j = SIM_SMEM_LINES >> 1; j; j >>= 1) bitonic_pass(sk, sw, m, SIM_SMEM_LINES, k, j);
+      for (uint32_t i = threadIdx.x; i < m; i += blockDim.x) { gk[t0 + i] = sk[i]; gw[t0 + i] = sw[i]; }
+      __syncthreads();
+    }
+  }
+}
+
 // Inclusive block scan of two u32 per thread (256 threads); tot = the block's totals.
 __device__ __forceinline__ uint2 block_scan2(uint2 v, uint2* sh, uint2& tot) {
   const int lane = threadIdx.x & 31, wi = threadIdx.x >> 5;
@@ -132,17 +150,7 @@ __global__ void __launch_bounds__(SIM_SORT_THREADS) k_sim_sort(const uint8_t* ar
     for (uint32_t i = threadIdx.x; i < m; i += blockDim.x) { gk[t0 + i] = sk[i]; gw[t0 + i] = sw[i]; }
     __syncthreads();
   }
-  for (uint32_t k = 2 * SIM_SMEM_LINES; k <= n2; k <<= 1) {
-    for (uint32_t j = k >> 1; j >= SIM_SMEM_LINES; j >>= 1) bitonic_pass(gk, gw, n, n2, k, j);
-    for (uint32_t t0 = 0; t0 < n; t0 += SIM_SMEM_LINES) {   // the passes inside a tile (j < tile, never the mirror pass)
-      const uint32_t m = min(SIM_SMEM_LINES, n - t0);
-      for (uint32_t i = threadIdx.x; i < m; i += blockDim.x) { sk[i] = gk[t0 + i]; sw[i] = gw[t0 + i]; }
-      __syncthreads();
-      for (uint32_t j = SIM_SMEM_LINES >> 1; j; j >>= 1) bitonic_pass(sk, sw, m, SIM_SMEM_LINES, k, j);
-      for (uint32_t i = threadIdx.x; i < m; i += blockDim.x) { gk[t0 + i] = sk[i]; gw[t0 + i] = sw[i]; }
-      __syncthreads();
-    }
-  }
+  bitonic_merge_tiles(gk, gw, n, n2, sk, sw);
   const uint32_t runs = merge_runs(gk, gw, n, out_key + b0, out_cum + b0, sh);
   if (threadIdx.x == 0) cnt[f] = runs;
 }

@@ -22,6 +22,7 @@
 //   tosem-scan releases <snapshot-root>=<tag>... [--out F]   |   releases --git <repository> [<revision>...] [--out F]
 //   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]
 //                      [--find-renames N]
+//   tosem-scan clones <project-root>... | --git <repository> [--rev R]   [--min-lines N] [--all-files] [--out F]
 #include <algorithm>
 #include <atomic>
 #include <cctype>
@@ -1758,6 +1759,88 @@ static int cmd_blame(const std::string& repo, const std::string& rev, int64_t ma
   return 0;
 }
 
+// ---------------------------------------------------------------------------------- clones (docs/SPEC.md section 15)
+static std::string repo_name(const std::string& path) {
+  std::string s = fs::path(path).lexically_normal().generic_string();
+  while (s.size() > 1 && s.back() == '/') s.pop_back();
+  return base_name(s);
+}
+
+// One tsm_clones call over every selected file (classes cross roots and batches), plus one tsm_scan for the per-file line and
+// assertion-line totals.  stdout: one row per root and an <all> row; --out: one row per fragment, classes numbered from 1 in
+// SPEC order, lines 1-based.
+static int cmd_clones(const std::vector<std::string>& roots, const std::string& git_repo, const std::string& rev, int min_lines,
+                      bool all_files, const std::string& out_path) {
+  std::vector<FileEntry> files;
+  std::vector<std::string> names;
+  if (!git_repo.empty()) {
+    gitstore::Store gs;
+    std::string err;
+    if (!gs.open(git_repo, err)) die(err);
+    gitstore::Oid id; gitstore::Commit cm;
+    if (!gs.resolve(rev, id) || !gs.commit(id, cm)) die("cannot resolve revision " + rev);
+    walk_git(gs, cm.tree, "", all_files, files);
+    names.push_back(repo_name(git_repo));
+  } else {
+    for (size_t g = 0; g < roots.size(); ++g) { walk(roots[g], (int)g, all_files, files); names.push_back(repo_name(roots[g])); }
+  }
+  fprintf(stderr, "tosem-scan: %zu files selected under %zu root(s)\n", files.size(), names.size());
+  int64_t need = 4096;
+  for (const FileEntry& f : files) need += (f.size + 127) / 128 * 128;
+  if (need >= (1ll << 31) || files.size() >= (1u << 31))
+    die("the selected files (" + std::to_string(need) + " bytes of arena) do not fit one int32-indexed arena; clones are found "
+        "across all files at once, so select fewer files");
+  Batch B;
+  for (size_t i = 0; i < files.size(); ++i) B.idx.push_back((uint32_t)i);
+  load_batch(files, B);
+  const int32_t nf = (int32_t)B.count();
+  tsm_ctx* ctx = nullptr;
+  ck(tsm_create(&ctx, 0, B.bytes + 4096, std::max<int32_t>(nf, 1), 1, 0), "tsm_create");
+  tsm_corpus c{B.arena, B.off.data(), B.len.data(), B.ext.data(), nullptr, nf, 1};
+  std::vector<tsm_file_stat> stats((size_t)nf);
+  if (nf) { tsm_result sr{}; sr.stats = stats.data(); ck(tsm_scan(ctx, &c, &sr, 0, nullptr), "tsm_scan"); }
+  std::vector<int64_t> base((size_t)nf + 1), cbase(1), member(1);
+  std::vector<uint32_t> dup((size_t)nf), dupa((size_t)nf), clen(1);
+  tsm_clone_result r{base.data(), dup.data(), dupa.data(), nullptr, nullptr, 0, 0, nullptr, 0, 0};
+  ck(tsm_clones(ctx, &c, min_lines, &r, nullptr), "tsm_clones");  // the counts; the second call fills arrays of that size
+  cbase.resize((size_t)r.n_classes + 1); clen.resize((size_t)std::max<int64_t>(r.n_classes, 1)); member.resize((size_t)std::max<int64_t>(r.n_members, 1));
+  r.class_base = cbase.data(); r.class_len = clen.data(); r.class_cap = r.n_classes; r.member = member.data(); r.member_cap = r.n_members;
+  ck(tsm_clones(ctx, &c, min_lines, &r, nullptr), "tsm_clones");
+  tsm_destroy(ctx);
+  const size_t ng = names.size();
+  std::vector<std::vector<int64_t>> tot(ng + 1, std::vector<int64_t>(6, 0));   // files, lines, dup, asserts, dup asserts, classes
+  for (int32_t i = 0; i < nf; ++i) {
+    const size_t g = (size_t)files[B.idx[(size_t)i]].grp;
+    const int64_t v[5] = {1, (int64_t)stats[(size_t)i].n_lines, dup[(size_t)i], (int64_t)stats[(size_t)i].n_assert, dupa[(size_t)i]};
+    for (int k = 0; k < 5; ++k) { tot[g][(size_t)k] += v[k]; tot[ng][(size_t)k] += v[k]; }
+  }
+  tot[ng][5] = r.n_classes;
+  std::ofstream os;
+  if (!out_path.empty()) { os.open(out_path, std::ios::binary); csv_row(os, {"class", "repository", "fileName", "first_line", "last_line"}); }
+  std::vector<int64_t> seen(ng, -1);                      // the last class counted for each root
+  for (int64_t k = 0; k < r.n_classes; ++k)
+    for (int64_t j = cbase[(size_t)k]; j < cbase[(size_t)k + 1]; ++j) {
+      const int64_t at = member[(size_t)j];
+      const size_t f = (size_t)(std::upper_bound(base.begin(), base.end(), at) - base.begin() - 1);
+      const FileEntry& fe = files[B.idx[f]];
+      if (seen[(size_t)fe.grp] != k) { seen[(size_t)fe.grp] = k; tot[(size_t)fe.grp][5]++; }
+      if (os.is_open()) {
+        const int64_t first = at - base[f] + 1;
+        csv_row(os, {std::to_string(k + 1), names[(size_t)fe.grp], fe.rel, std::to_string(first), std::to_string(first + clen[(size_t)k] - 1)});
+      }
+    }
+  std::ostringstream so;
+  csv_row(so, {"repository", "files", "lines", "duplicated_lines", "assertion_lines", "duplicated_assertion_lines", "classes"});
+  for (size_t g = 0; g <= ng; ++g) {
+    std::vector<std::string> row = {g < ng ? names[g] : "<all>"};
+    for (int64_t v : tot[g]) row.push_back(std::to_string(v));
+    csv_row(so, row);
+  }
+  fputs(so.str().c_str(), stdout);
+  tsm_host_free(B.arena);
+  return 0;
+}
+
 static void usage() {
   fprintf(stderr,
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
@@ -1768,6 +1851,8 @@ static void usage() {
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
           "                          [--find-renames N]\n"
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
+          "       tosem-scan clones <project-root>... [--min-lines N] [--all-files] [--out F]\n"
+          "       tosem-scan clones --git <repository> [--rev R] [--min-lines N] [--all-files] [--out F]\n"
           "--find-renames N (0..100): pair deleted and added files at least N %% similar, as git -M<N>%% does (docs/SPEC.md section 13).\n"
           "Scans run on the GPU through libtosemscan.so (sm_90a); there is no CPU fallback.\n");
 }
@@ -1790,6 +1875,12 @@ int main(int argc, char** argv) {
                                         opt.count("--batch-bytes") ? std::max<int64_t>(4096, atoll(opt["--batch-bytes"].c_str())) : (1ll << 30), rev_b); }
   if (cmd == "reduce") { if (pos.size() != 1) die("reduce needs the taxonomy csv"); return cmd_reduce(pos[0], opt["--strategy"], opt["--methods"], opt["--properties"], opt["--correlate"], opt["--correlate-tex"], opt["--correlate-counts"], opt["--correlate-merged"]); }
   if (cmd == "releases") { if (pos.empty() && !opt.count("--git")) die("releases needs <root>=<tag>... or --git <repository>"); return cmd_releases(pos, opt["--out"], opt["--git"]); }
+  if (cmd == "clones") {
+    if (pos.empty() == !opt.count("--git")) die("clones needs project roots or --git <repository>, not both");
+    const long n = opt.count("--min-lines") ? strtol(opt["--min-lines"].c_str(), nullptr, 10) : 5;
+    if (n < 1 || n > 1024) die("--min-lines needs a number of lines from 1 to 1024");
+    return cmd_clones(pos, opt["--git"], opt.count("--rev") ? opt["--rev"] : "HEAD", (int)n, all_files, opt["--out"]);
+  }
   if (cmd == "body") { if (pos.empty()) die("body needs at least one project root"); return cmd_body(pos, opt["--out"]); }
   int rename_pct = -1;                                     // --find-renames N (docs/SPEC.md section 13); -1 = off
   if (opt.count("--find-renames")) {

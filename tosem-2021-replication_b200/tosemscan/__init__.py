@@ -37,7 +37,7 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_diff_pairs", "tsm_diff_pairs_detail", "tsm_statements", "tsm_line_hashes", "tsm_diff_upload", "tsm_diff_resident", "tsm_diff_last_ms",
            "tsm_diff_pairs_asserts", "tsm_diff_resident_asserts", "tsm_reduce", "tsm_host_alloc", "tsm_host_free", "tsm_layout", "tsm_gen_sizes",
            "tsm_gen_fill", "tsm_gen_edit", "tsm_gen_pair_sizes", "tsm_gen_pair_fill", "tsm_similarity", "tsm_similarity_last_ms",
-           "tsm_diff_pairs_marks", "tsm_blame_pairs", "tsm_blame_last_ms"]
+           "tsm_diff_pairs_marks", "tsm_blame_pairs", "tsm_blame_last_ms", "tsm_clones", "tsm_clones_last_ms"]
 
 
 class TsmError(RuntimeError):
@@ -68,6 +68,12 @@ class _DiffAsserts(C.Structure):
     _fields_ = [("added_counts", C.c_void_p), ("removed_counts", C.c_void_p),
                 ("aev", C.c_void_p), ("aev_cap", C.c_int64), ("n_aev", C.c_int64),
                 ("rev", C.c_void_p), ("rev_cap", C.c_int64), ("n_rev", C.c_int64)]
+
+
+class _CloneResult(C.Structure):
+    _fields_ = [("line_base", C.c_void_p), ("file_dup", C.c_void_p), ("file_dup_assert", C.c_void_p),
+                ("class_base", C.c_void_p), ("class_len", C.c_void_p), ("class_cap", C.c_int64), ("n_classes", C.c_int64),
+                ("member", C.c_void_p), ("member_cap", C.c_int64), ("n_members", C.c_int64)]
 
 
 _lib = None
@@ -162,6 +168,10 @@ def lib():
             [C.c_int64, C.POINTER(C.c_int64), C.c_void_p]
         L.tsm_blame_last_ms.restype = C.c_int
         L.tsm_blame_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float)]
+        L.tsm_clones.restype = C.c_int
+        L.tsm_clones.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_int32, C.POINTER(_CloneResult), C.c_void_p]
+        L.tsm_clones_last_ms.restype = C.c_int
+        L.tsm_clones_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 3)]
         _lib = L
     return _lib
 
@@ -712,4 +722,36 @@ class Scanner:
         """Device time of the last similarity call: [k_scan over both sides, sort / merge, k_similarity] in ms."""
         ms = (C.c_float * 3)()
         lib().tsm_similarity_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
+
+    def clones(self, corpus, min_lines=5, stream=None, cap=None):
+        """Duplicated test code (docs/SPEC.md section 15): a dict of numpy arrays line_base[n_files+1], file_dup[n_files],
+        file_dup_assert[n_files], class_base[n_classes+1], class_len[n_classes] and member[n_members] (the global first line of
+        every fragment; class c is member[class_base[c]:class_base[c+1]], each fragment class_len[c] lines).  Arrays too small
+        for the classes or fragments are sized from the counts and the call is made again (cap: the first guess of both)."""
+        n = corpus.n_files
+        cs = corpus.c_struct()
+        cc = cm = int(cap if cap is not None else 0)
+        for _ in range(2):
+            out = {"line_base": np.zeros(n + 1, np.int64), "file_dup": np.zeros(n, np.uint32), "file_dup_assert": np.zeros(n, np.uint32),
+                   "class_base": np.zeros(cc + 1, np.int64), "class_len": np.zeros(max(cc, 1), np.uint32),
+                   "member": np.zeros(max(cm, 1), np.int64)}
+            r = _CloneResult(*[_p(out[k]) for k in ("line_base", "file_dup", "file_dup_assert", "class_base", "class_len")], cc, 0,
+                             _p(out["member"]), cm, 0)
+            rc = lib().tsm_clones(self._ctx, C.byref(cs), int(min_lines), C.byref(r), stream)
+            if rc == TSM_E_CAPACITY and (r.n_classes > cc or r.n_members > cm):
+                cc, cm = int(r.n_classes), int(r.n_members)
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_clones")
+            out["class_base"] = out["class_base"][:r.n_classes + 1]
+            out["class_len"] = out["class_len"][:r.n_classes]
+            out["member"] = out["member"][:r.n_members]
+            return out
+        raise TsmError(TSM_E_CAPACITY, "tsm_clones")
+
+    def clones_last_ms(self):
+        """Device time of the last clones call: [k_scan, grouping + classes, members + coverage] in ms."""
+        ms = (C.c_float * 3)()
+        lib().tsm_clones_last_ms(self._ctx, C.byref(ms))
         return [float(x) for x in ms]
