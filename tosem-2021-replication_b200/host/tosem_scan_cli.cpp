@@ -18,11 +18,14 @@
 //   tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N]
 //   tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]
 //   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--find-renames N]
-//   tosem-scan body   <project-root>... [--out F]
-//   tosem-scan releases <snapshot-root>=<tag>... [--out F]   |   releases --git <repository> [<revision>...] [--out F]
+//   tosem-scan body   <project-root>... [--batch-bytes N] [--out F]
+//   tosem-scan releases <snapshot-root>=<tag>... | --git <repository> [<revision>...]   [--batch-bytes N] [--out F]
 //   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]
 //                      [--find-renames N]
+//   tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]
 //   tosem-scan clones <project-root>... | --git <repository> [--rev R]   [--min-lines N] [--all-files] [--out F]
+// Every command that scans files does it with scan_batches: batches of at most --batch-bytes of arena (clones: all files in one),
+// one context, the next batch read while the current one is scanned.
 #include <algorithm>
 #include <atomic>
 #include <cctype>
@@ -39,6 +42,7 @@
 #include <future>
 #include <map>
 #include <memory>
+#include <numeric>
 #include <sstream>
 #include <string>
 #include <thread>
@@ -194,14 +198,19 @@ static std::string method_string(int ext, const uint8_t* line, uint32_t len) {  
 }
 
 // ---------------------------------------------------------------------------------- scan
-struct Batch {                                             // one packed arena (<= ~1 GiB) of files of one GPU's share
+struct HostFree { void operator()(uint8_t* p) const { tsm_host_free(p); } };
+
+struct Batch {                                             // one packed arena of files; move-only, it owns its pinned arena
   std::vector<uint32_t> idx;                               // indices into the walk's file list, ascending
   std::vector<int32_t> off, len;
   std::vector<uint8_t> ext;
   std::vector<uint16_t> grp;
-  uint8_t* arena = nullptr;
-  int64_t bytes = 0;
+  std::unique_ptr<uint8_t[], HostFree> arena;
+  int64_t bytes = 0;                                       // arena bytes (padded file sizes)
   size_t count() const { return idx.size(); }
+  tsm_corpus corpus(int32_t n_groups) const {
+    return {arena.get(), off.data(), len.data(), ext.data(), grp.data(), (int32_t)len.size(), n_groups};
+  }
 };
 
 // The files of lengths B.len laid out by tsm_layout (B.off, B.bytes) in a zeroed pinned arena, their ext / grp tags zero; the
@@ -211,9 +220,18 @@ static void alloc_arena(Batch& B) {
   B.off.resize(n + 1); B.ext.assign(n, 0); B.grp.assign(n, 0);
   B.bytes = tsm_layout(B.len.data(), (int32_t)n, B.off.data());
   if (B.bytes < 0) die("batch does not fit an int32-indexed arena");
-  B.arena = (uint8_t*)tsm_host_alloc(std::max<int64_t>(B.bytes, 128));
+  B.arena.reset((uint8_t*)tsm_host_alloc(std::max<int64_t>(B.bytes, 128)));
   if (!B.arena) die("pinned arena allocation failed (no CUDA device? there is no CPU fallback)");
-  memset(B.arena, 0, (size_t)std::max<int64_t>(B.bytes, 128));
+  memset(B.arena.get(), 0, (size_t)std::max<int64_t>(B.bytes, 128));
+}
+
+// Byte strings held in memory, packed into one arena in order (ext / grp tags zero).
+static Batch pack(const std::vector<const std::vector<uint8_t>*>& bytes) {
+  Batch B;
+  for (const std::vector<uint8_t>* v : bytes) B.len.push_back((int32_t)v->size());
+  alloc_arena(B);
+  for (size_t i = 0; i < bytes.size(); ++i) if (B.len[i]) memcpy(B.arena.get() + B.off[i], bytes[i]->data(), bytes[i]->size());
+  return B;
 }
 
 static bool read_file(const std::string& path, uint8_t* dst, int64_t size) {   // false on a short read
@@ -239,8 +257,8 @@ static void load_batch(const std::vector<FileEntry>& files, Batch& b) {
   std::atomic<long> bad{-1};
   auto reader = [&](unsigned t) {
     for (size_t i = t; i < n && bad.load(std::memory_order_relaxed) < 0; i += nt) {
-      if (files[b.idx[i]].blob) { if (b.len[i]) memcpy(b.arena + b.off[i], files[b.idx[i]].blob->data(), (size_t)b.len[i]); continue; }
-      if (!read_file(files[b.idx[i]].abs, b.arena + b.off[i], b.len[i])) bad.store((long)i);
+      if (files[b.idx[i]].blob) { if (b.len[i]) memcpy(b.arena.get() + b.off[i], files[b.idx[i]].blob->data(), (size_t)b.len[i]); continue; }
+      if (!read_file(files[b.idx[i]].abs, b.arena.get() + b.off[i], b.len[i])) bad.store((long)i);
     }
   };
   std::vector<std::thread> th;
@@ -250,16 +268,28 @@ static void load_batch(const std::vector<FileEntry>& files, Batch& b) {
   if (bad.load() >= 0) die("short read: " + files[b.idx[(size_t)bad.load()]].abs);
 }
 
-// The files from `first` on that fit one batch of `body` / `releases` (512 MiB of arena, 2^19 files), loaded.
-static Batch next_batch(const std::vector<FileEntry>& files, size_t& first) {
-  Batch B;
-  int64_t cur = 0;
-  while (first < files.size() && (B.count() == 0 || (cur + files[first].size < (1ll << 29) && B.count() < (1u << 19)))) {
-    cur += (files[first].size + 127) / 128 * 128; B.idx.push_back((uint32_t)first); ++first;
+// The files `indices` (ascending) cut in order into batches of at most max_bytes of arena (128-byte padded sizes) and max_files
+// files; a file larger than max_bytes is a batch of its own.  Not loaded yet: Batch::bytes is the arena load_batch will lay out.
+static std::vector<Batch> plan_batches(const std::vector<FileEntry>& files, const std::vector<uint32_t>& indices, int64_t max_bytes,
+                                       size_t max_files) {
+  std::vector<Batch> out;
+  for (uint32_t i : indices) {
+    const int64_t padded = (files[i].size + 127) / 128 * 128;
+    if (out.empty() || out.back().bytes + padded > max_bytes || out.back().count() >= max_files) out.emplace_back();
+    out.back().idx.push_back(i);
+    out.back().bytes += padded;
   }
-  load_batch(files, B);
-  return B;
+  return out;
 }
+static std::vector<uint32_t> all_of(const std::vector<FileEntry>& files) {
+  std::vector<uint32_t> v(files.size());
+  std::iota(v.begin(), v.end(), 0u);
+  return v;
+}
+// Batches of every command but `scan`: --batch-bytes defaults to kBatch (bytes per side of a diff or tsm_similarity call, arena
+// bytes of a scan), and a scan batch holds at most kBatchFiles files.
+static const int64_t kBatch = 512ll << 20;
+static const size_t kBatchFiles = 1u << 19;
 
 static void cu_ck(cudaError_t e, const char* what) { if (e != cudaSuccess) die(std::string(what) + ": " + cudaGetErrorString(e)); }
 static void nccl_ck(ncclResult_t r, const char* what) { if (r != ncclSuccess) die(std::string(what) + ": " + ncclGetErrorString(r)); }
@@ -285,6 +315,58 @@ static void scan_events(tsm_ctx* ctx, const tsm_corpus& c, int64_t bytes, tsm_re
   aev.resize(want_a ? (size_t)r.n_aev : 0); hev.resize(want_h ? (size_t)r.n_hev : 0);
 }
 
+// One scanned batch: per-file records, the count table ([n_groups][K] by group, [K] over the batch, then the 4 totals of
+// tsm_result), the events `flags` asked for, and the context that holds the batch for more calls on it.
+struct Scanned {
+  const std::vector<tsm_file_stat>& stats;
+  const std::vector<int64_t>& counts;
+  const std::vector<tsm_assert_event>& aev;
+  const std::vector<tsm_header_event>& hev;
+  tsm_ctx* ctx;
+};
+using ScanFn = std::function<void(const Batch&, const Scanned&)>;
+
+// Every batch of `batches` loaded, scanned with `flags` on one context of `device` (sized to the largest batch) and handed to
+// `fn`.  Host pipeline: while the GPU scans batch b (tsm_scan overlaps its H2D slabs with the kernels), a background task
+// already reads the files of batch b + 1 into its pinned arena.  At most two arenas are alive: a batch's arena is freed as soon
+// as `fn` returns.  No batches: no context, `fn` never runs.
+static void scan_batches(const std::vector<FileEntry>& files, std::vector<Batch>& batches, int device, int32_t n_groups, uint32_t flags,
+                         const ScanFn& fn) {
+  if (batches.empty()) return;
+  cu_ck(cudaSetDevice(device), "cudaSetDevice");
+  cudaStream_t st;
+  cu_ck(cudaStreamCreate(&st), "cudaStreamCreate");
+  int64_t max_arena = 1 << 20; int32_t max_files = 16;
+  for (const Batch& b : batches) { max_arena = std::max(max_arena, b.bytes + 4096); max_files = std::max(max_files, (int32_t)b.count()); }
+  tsm_ctx* ctx = nullptr;
+  ck(tsm_create(&ctx, device, max_arena, max_files, n_groups, 0), "tsm_create");
+  auto load = [&](size_t b) {
+    return std::async(std::launch::async, [&files, &batches, b, device] { cudaSetDevice(device); load_batch(files, batches[b]); });
+  };
+  std::future<void> next = load(0);
+  std::vector<tsm_file_stat> stats;
+  std::vector<int64_t> counts;
+  std::vector<tsm_assert_event> aev;
+  std::vector<tsm_header_event> hev;
+  const size_t K = TSM_NUM_CATEGORIES;
+  for (size_t b = 0; b < batches.size(); ++b) {
+    Batch& B = batches[b];
+    next.get();
+    if (b + 1 < batches.size()) next = load(b + 1);
+    stats.resize(B.count());
+    counts.assign((size_t)(n_groups + 1) * K + 4, 0);
+    tsm_result r{};
+    r.stats = stats.data(); r.group_counts = counts.data(); r.global_counts = counts.data() + (size_t)n_groups * K;
+    scan_events(ctx, B.corpus(n_groups), B.bytes, r, flags, st, aev, hev);
+    std::copy(r.totals, r.totals + 4, counts.end() - 4);
+    fn(B, Scanned{stats, counts, aev, hev, ctx});
+    B.arena.reset();
+    std::vector<int32_t>().swap(B.off); std::vector<int32_t>().swap(B.len);
+  }
+  tsm_destroy(ctx);
+  cudaStreamDestroy(st);
+}
+
 // The statement of an assertion event (the statement may be longer than the 16-bit event field: its end is re-derived on the
 // host if saturated) and its category cell (the verbatim identifier for 127, docs/SPEC.md section 6).
 static std::string event_statement(const uint8_t* base, int32_t size, const tsm_assert_event& ev) {
@@ -295,13 +377,26 @@ static std::string event_statement(const uint8_t* base, int32_t size, const tsm_
 static std::string event_category(const uint8_t* base, const tsm_assert_event& ev) {
   return ev.cat == 127 ? std::string((const char*)base + ev.ident_off, ev.ident_len) : std::string(tsm_category_name(ev.cat));
 }
-// The assertion cell of a per-file row, "n:category, ...": the categories in first-seen `order`, stably sorted by count, descending.
-static std::string hist_cell(std::map<std::string, int64_t>& hist, std::vector<std::string> order) {
-  std::stable_sort(order.begin(), order.end(), [&](const std::string& x, const std::string& y) { return hist[x] > hist[y]; });
-  std::string a;
-  for (const std::string& c : order) { if (!a.empty()) a += ", "; a += std::to_string(hist[c]) + ":" + c; }
-  return a;
-}
+// The assertion cell of a per-file row, "n:category, ...": the categories in first-seen order, stably sorted by count, descending.
+struct CategoryHist {
+  std::map<std::string, int64_t> n;
+  std::vector<std::string> order;
+  void add(const std::string& cat) { if (!n.count(cat)) order.push_back(cat); n[cat]++; }
+  std::string cell() {
+    std::stable_sort(order.begin(), order.end(), [&](const std::string& x, const std::string& y) { return n[x] > n[y]; });
+    std::string a;
+    for (const std::string& c : order) { if (!a.empty()) a += ", "; a += std::to_string(n[c]) + ":" + c; }
+    return a;
+  }
+};
+
+// The 1-based line numbers of ascending offsets into one file, counting the newlines from the previous offset on.
+struct LineCounter {
+  const uint8_t* base;
+  uint32_t pos = 0;
+  int64_t line = 1;
+  int64_t at(uint32_t off) { for (; pos < off; ++pos) line += base[pos] == '\n'; return line; }
+};
 
 // The raw rows (fileName, extension, test_name, method, statement, counts, category: ML-Testing-v1.xlsx!apollo_tests:R1) and
 // the summary row (Id, FileName, total assert, assertion: Release-Meta-tpot.csv:1-2) of one file, from its events.
@@ -311,7 +406,7 @@ static void render_file(const FileEntry& f, int64_t id, const uint8_t* base, int
   struct Row { int64_t hdr; std::string stmt; int cat; std::string catname; int64_t count; bool fixture; std::string method; };
   std::vector<Row> rows;
   std::map<std::pair<int64_t, std::string>, size_t> index;
-  std::map<std::string, int64_t> hist; std::vector<std::string> hist_order;
+  CategoryHist hist;
   int64_t cur_hdr = -1; bool cur_fix = false; std::string cur_method = "xxxx";
   while (ai < aev.size() && aev[ai].file == slot) {
     const tsm_assert_event& ev = aev[ai++];
@@ -325,8 +420,7 @@ static void render_file(const FileEntry& f, int64_t id, const uint8_t* base, int
     auto it = index.find(key);
     if (it == index.end()) { index[key] = rows.size(); rows.push_back({cur_hdr, stmt, ev.cat, cat, 1, cur_fix, cur_method}); }
     else rows[it->second].count++;
-    if (!hist.count(cat)) hist_order.push_back(cat);
-    hist[cat]++;
+    hist.add(cat);
   }
   while (hi < hev.size() && hev[hi].file == slot) ++hi;
   if (want_rows && !rows.empty()) {
@@ -337,7 +431,7 @@ static void render_file(const FileEntry& f, int64_t id, const uint8_t* base, int
   }
   if (want_sum) {
     std::ostringstream os;
-    csv_row(os, {std::to_string(id), f.rel, std::to_string(st.n_assert), hist_cell(hist, hist_order)});
+    csv_row(os, {std::to_string(id), f.rel, std::to_string(st.n_assert), hist.cell()});
     sum_txt = os.str();
   }
 }
@@ -372,16 +466,7 @@ static int cmd_scan(const std::vector<std::string>& roots, const std::string& ro
     }
     for (int g = 0; g < gpus; ++g) {
       std::sort(mine[(size_t)g].begin(), mine[(size_t)g].end());
-      int64_t cur = 0;
-      share[(size_t)g].emplace_back();
-      for (uint32_t i : mine[(size_t)g]) {
-        const int64_t padded = (files[i].size + 127) / 128 * 128;
-        Batch* b = &share[(size_t)g].back();
-        if (b->count() && (cur + padded > batch_bytes || b->count() >= (1u << 20))) { share[(size_t)g].emplace_back(); b = &share[(size_t)g].back(); cur = 0; }
-        b->idx.push_back(i);
-        cur += padded;
-      }
-      if (share[(size_t)g].back().count() == 0) share[(size_t)g].pop_back();
+      share[(size_t)g] = plan_batches(files, mine[(size_t)g], batch_bytes, 1u << 20);
     }
   }
   // one host thread per GPU; one ncclAllReduce of the count table at the end
@@ -405,67 +490,29 @@ static int cmd_scan(const std::vector<std::string>& roots, const std::string& ro
   const bool want_rows = !rows_path.empty(), want_sum = !summary_path.empty();
   std::vector<std::string> rows_txt(want_rows ? files.size() : 0), sum_txt(want_sum ? files.size() : 0);   // per file, written in walk order at the end
   auto worker = [&](int g) {
-    std::vector<Batch>& batches = share[(size_t)g];
+    const uint32_t flags = TSM_SCAN_ASSERT_EVENTS | TSM_SCAN_HEADER_EVENTS | (rev_b ? TSM_SCAN_REV_B : 0u);
+    scan_batches(files, share[(size_t)g], g, n_groups, flags, [&](const Batch& B, const Scanned& s) {
+      for (size_t i = 0; i < table; ++i) totals[g][i] += s.counts[i];
+      if (!want_rows && !want_sum) return;
+      size_t ai = 0, hi = 0;
+      std::string none;
+      for (size_t i = 0; i < B.count(); ++i) {
+        const uint32_t fi = B.idx[i];
+        render_file(files[fi], (int64_t)fi + 1, B.arena.get() + B.off[i], B.len[i], (uint32_t)i, s.stats[i], s.aev, ai, s.hev, hi, want_rows,
+                    want_sum, want_rows ? rows_txt[fi] : none, want_sum ? sum_txt[fi] : none);
+      }
+    });
     cu_ck(cudaSetDevice(g), "cudaSetDevice");
     cudaStream_t st;
     cu_ck(cudaStreamCreate(&st), "cudaStreamCreate");
-    int64_t max_arena = 1 << 20; int32_t max_files = 16;
-    for (const Batch& b : batches) {
-      int64_t bytes = 0;
-      for (uint32_t i : b.idx) bytes += (files[i].size + 127) / 128 * 128;
-      max_arena = std::max(max_arena, bytes + 4096);
-      max_files = std::max<int32_t>(max_files, (int32_t)b.count());
-    }
-    tsm_ctx* ctx = nullptr;
-    ck(tsm_create(&ctx, g, max_arena, max_files, std::max(n_groups, 1), 0), "tsm_create");
     int64_t* d_acc = nullptr;                               // this GPU's count table, input and output of the allreduce
     cu_ck(cudaMalloc((void**)&d_acc, table * sizeof(int64_t)), "cudaMalloc");
-    // host pipeline: while the GPU scans batch b (tsm_scan overlaps its H2D slabs with the kernels), a background
-    // task already reads the files of the next batch into its pinned arena.  At most two arenas per GPU are alive:
-    // a batch's rows are rendered and its arena and events are freed as soon as its scan returns.
-    std::future<void> next_load;
-    if (!batches.empty()) next_load = std::async(std::launch::async, [&files, &batches, g] { cudaSetDevice(g); load_batch(files, batches[0]); });
-    std::vector<tsm_file_stat> stats;
-    std::vector<tsm_assert_event> aev;
-    std::vector<tsm_header_event> hev;
-    std::vector<int64_t> group_counts, h;
-    for (size_t b = 0; b < batches.size(); ++b) {
-      Batch& B = batches[b];
-      next_load.get();
-      if (b + 1 < batches.size())
-        next_load = std::async(std::launch::async, [&files, &batches, b, g] { cudaSetDevice(g); load_batch(files, batches[b + 1]); });
-      tsm_corpus c{B.arena, B.off.data(), B.len.data(), B.ext.data(), B.grp.data(), (int32_t)B.count(), n_groups};
-      stats.resize(B.count());
-      group_counts.assign((size_t)n_groups * TSM_NUM_CATEGORIES, 0);
-      tsm_result r{};
-      r.stats = stats.data(); r.group_counts = group_counts.data();
-      scan_events(ctx, c, B.bytes, r, TSM_SCAN_ASSERT_EVENTS | TSM_SCAN_HEADER_EVENTS | (rev_b ? TSM_SCAN_REV_B : 0u), st, aev, hev);
-      void* dptr = nullptr; int64_t n64 = 0;
-      ck(tsm_device_counts(ctx, &dptr, &n64), "tsm_device_counts");
-      h.resize((size_t)n64);
-      cu_ck(cudaMemcpyAsync(h.data(), dptr, (size_t)n64 * sizeof(int64_t), cudaMemcpyDeviceToHost, st), "cudaMemcpyAsync");
-      cu_ck(cudaStreamSynchronize(st), "cudaStreamSynchronize");
-      for (size_t i = 0; i < (size_t)n64 && i < table; ++i) totals[g][i] += h[i];
-      if (want_rows || want_sum) {
-        size_t ai = 0, hi = 0;
-        static std::string none;
-        for (size_t i = 0; i < B.count(); ++i) {
-          const uint32_t fi = B.idx[i];
-          render_file(files[fi], (int64_t)fi + 1, B.arena + B.off[i], B.len[i], (uint32_t)i, stats[i], aev, ai, hev, hi, want_rows, want_sum,
-                      want_rows ? rows_txt[fi] : none, want_sum ? sum_txt[fi] : none);
-        }
-      }
-      tsm_host_free(B.arena);
-      B.arena = nullptr;
-      std::vector<int32_t>().swap(B.off); std::vector<int32_t>().swap(B.len);
-    }
     cu_ck(cudaMemcpyAsync(d_acc, totals[g].data(), table * sizeof(int64_t), cudaMemcpyHostToDevice, st), "cudaMemcpyAsync");
     if (gpus > 1)                                           // the single collective of the path (SURVEY.md section 8e)
       nccl_ck(ncclAllReduce(d_acc, d_acc, table, ncclInt64, ncclSum, comms[g], st), "ncclAllReduce");
     cu_ck(cudaMemcpyAsync(totals[g].data(), d_acc, table * sizeof(int64_t), cudaMemcpyDeviceToHost, st), "cudaMemcpyAsync");
     cu_ck(cudaStreamSynchronize(st), "cudaStreamSynchronize");
     cudaFree(d_acc);
-    tsm_destroy(ctx);
     cudaStreamDestroy(st);
   };
   if (gpus == 1) worker(0);
@@ -685,6 +732,9 @@ static int cmd_reduce(const std::string& path, const std::string& strategy_path,
   ck(tsm_reduce(ctx, flags.data(), repo.data(), cas.data(), n_rows, nF, n_repos, n_cases, out.data(), cpr.data(), nullptr), "tsm_reduce");
   tsm_destroy(ctx);
   int64_t all_cases = 0; for (int64_t c : cpr) all_cases += c;
+  // row order of the property and correlate tables: the shipped one when all nine repositories are present, else that of `repos`
+  std::vector<std::string> order = {"auto_sklearn", "google_automl", "tpot", "autokeras", "Nupic", "Apollo", "nni", "Ray", "DeepSpeech2"};
+  for (auto& r : repos) if (!std::count(order.begin(), order.end(), r)) order.push_back(r);
   if (!strategy_path.empty()) {                             // layout of RQs/RQ3/tests_strategy_rq32.csv
     std::ofstream os(strategy_path, std::ios::binary);
     std::vector<std::string> h = {"Tests"};
@@ -729,9 +779,6 @@ static int cmd_reduce(const std::string& path, const std::string& strategy_path,
     int64_t denom = 0;                                      // one denominator for every row: Apollo's case count (the 216 of
     if (rid.count("Apollo")) denom = cpr[(size_t)rid["Apollo"]];   // the shipped table), else the largest repository
     if (denom == 0) for (int64_t c : cpr) denom = std::max(denom, c);
-    // shipped row order when all nine repositories are present, else the order of `repos`
-    std::vector<std::string> order = {"auto_sklearn", "google_automl", "tpot", "autokeras", "Nupic", "Apollo", "nni", "Ray", "DeepSpeech2"};
-    for (auto& r : repos) if (!std::count(order.begin(), order.end(), r)) order.push_back(r);
     for (auto& name : order) {
       if (!rid.count(name) || cpr[(size_t)rid[name]] == 0) continue;
       const int r = rid[name];
@@ -741,72 +788,52 @@ static int cmd_reduce(const std::string& path, const std::string& strategy_path,
       csv_row(os, row);
     }
   }
-  if (corr) {
-    // three shipped layouts of the same 20 x 21 counts: RQs/RQ3/tests_correlate_rq3.csv ("repo:(p%), " for every repository),
-    // tests_correlate_rq4.csv (LaTeX cells "$repo:p\%$, " of the non-zero repositories) and
-    // tests_combined_correlate_rq3.csv (the distinct cases of all repositories together)
-    for (const CorrRow& cr : kCorrRows) if (!col.count(cr.col)) die(std::string("taxonomy lacks column ") + cr.col);
-    std::vector<std::string> order = {"auto_sklearn", "google_automl", "tpot", "autokeras", "Nupic", "Apollo", "nni", "Ray", "DeepSpeech2"};
-    for (auto& r : repos) if (!std::count(order.begin(), order.end(), r)) order.push_back(r);
-    const size_t c0 = (size_t)(nS + nM + nP);
-    for (int layout = 0; layout < 3; ++layout) {
-      const std::string& outp = layout == 0 ? correlate_path : layout == 1 ? correlate_tex_path : correlate_counts_path;
-      if (outp.empty()) continue;
-      std::ofstream os(outp, std::ios::binary);
-      std::vector<std::string> h = {"Tests"};
-      for (int q = 0; q < nCC; ++q) h.push_back(kCorrCols[q].name);
-      csv_row(os, h);
-      for (int j = 0; j < nCR; ++j) {
-        std::vector<std::string> row = {kCorrRows[j].name};
-        for (int q = 0; q < nCC; ++q) {
-          const int64_t* d = &out[(c0 + (size_t)j * nCC + q) * n_repos];
-          int64_t all = 0;
-          for (int r = 0; r < n_repos; ++r) all += d[r];
-          std::string cellv = "0";                          // a pairing no case has is the bare string "0" in every layout
-          if (layout == 2) cellv = std::to_string(all);
-          else if (all) {
-            cellv.clear();
-            for (auto& name : order) {
-              if (!rid.count(name) || cpr[(size_t)rid[name]] == 0) continue;
-              const int r = rid[name];
-              const std::string pct = fmt_pyfloat2(100.0 * (double)d[r] / (double)cpr[r]);
-              if (layout == 0) cellv += name + ":(" + pct + "%), ";
-              else if (d[r]) cellv += "$" + name + ":" + pct + "\\%$, ";
-            }
-          }
-          row.push_back(cellv);
-        }
-        csv_row(os, row);
-      }
-    }
-  }
-  if (merged) {                                             // the four one-row tables, as four rows of one file
-    std::ofstream os(correlate_merged_path, std::ios::binary);
+  // A table of the correlate layout: 21 property columns, one row per name, the row j counts in the flag columns c0 + j * nCC + q.
+  // Three shipped layouts of the same counts: RQs/RQ3/tests_correlate_rq3.csv (0: "repo:(p%), " for every repository),
+  // tests_correlate_rq4.csv (1: LaTeX cells "$repo:p\%$, " of the non-zero repositories) and tests_combined_correlate_rq3.csv
+  // (2: the distinct cases of all repositories together).
+  auto correlate = [&](const std::string& outp, int layout, size_t c0, const std::vector<std::string>& names) {
+    if (outp.empty()) return;
+    std::ofstream os(outp, std::ios::binary);
     std::vector<std::string> h = {"Tests"};
     for (int q = 0; q < nCC; ++q) h.push_back(kCorrCols[q].name);
     csv_row(os, h);
-    std::vector<std::string> order = {"auto_sklearn", "google_automl", "tpot", "autokeras", "Nupic", "Apollo", "nni", "Ray", "DeepSpeech2"};
-    for (auto& r : repos) if (!std::count(order.begin(), order.end(), r)) order.push_back(r);
-    const size_t c0 = (size_t)(nS + nM + nP + (corr ? nCR * nCC : 0));
-    for (int j = 0; j < nMR; ++j) {
-      std::vector<std::string> row = {kMergedRows[j].name};
+    for (size_t j = 0; j < names.size(); ++j) {
+      std::vector<std::string> row = {names[j]};
       for (int q = 0; q < nCC; ++q) {
-        const int64_t* d = &out[(c0 + (size_t)j * nCC + q) * n_repos];
+        const int64_t* d = &out[(c0 + j * nCC + q) * n_repos];
         int64_t all = 0;
         for (int r = 0; r < n_repos; ++r) all += d[r];
-        std::string cellv = "0";
-        if (all) {
+        std::string cellv = "0";                            // a pairing no case has is the bare string "0" in every layout
+        if (layout == 2) cellv = std::to_string(all);
+        else if (all) {
           cellv.clear();
           for (auto& name : order) {
             if (!rid.count(name) || cpr[(size_t)rid[name]] == 0) continue;
             const int r = rid[name];
-            cellv += name + ":(" + fmt_pyfloat2(100.0 * (double)d[r] / (double)cpr[r]) + "%), ";
+            const std::string pct = fmt_pyfloat2(100.0 * (double)d[r] / (double)cpr[r]);
+            if (layout == 0) cellv += name + ":(" + pct + "%), ";
+            else if (d[r]) cellv += "$" + name + ":" + pct + "\\%$, ";
           }
         }
         row.push_back(cellv);
       }
       csv_row(os, row);
     }
+  };
+  const size_t c0 = (size_t)(nS + nM + nP);
+  if (corr) {
+    for (const CorrRow& cr : kCorrRows) if (!col.count(cr.col)) die(std::string("taxonomy lacks column ") + cr.col);
+    std::vector<std::string> names;
+    for (const CorrRow& cr : kCorrRows) names.push_back(cr.name);
+    correlate(correlate_path, 0, c0, names);
+    correlate(correlate_tex_path, 1, c0, names);
+    correlate(correlate_counts_path, 2, c0, names);
+  }
+  if (merged) {                                             // the four one-row tables, as four rows of one file in layout 0
+    std::vector<std::string> names;
+    for (const MergedRow& mr : kMergedRows) names.push_back(mr.name);
+    correlate(correlate_merged_path, 0, c0 + (corr ? (size_t)(nCR * nCC) : 0), names);
   }
   fprintf(stderr, "tosem-scan: reduce %d rows, %d cases, %d repos\n", n_rows, n_cases, n_repos);
   return 0;
@@ -843,35 +870,29 @@ static std::string case_name(int ext, const uint8_t* line, uint32_t len) {
   return method_string(ext, line, len);
 }
 
-static int cmd_body(const std::vector<std::string>& roots, const std::string& out_path) {
+static int cmd_body(const std::vector<std::string>& roots, const std::string& out_path, int64_t batch_bytes) {
   std::vector<FileEntry> files;
   for (size_t g = 0; g < roots.size(); ++g) walk(roots[g], (int)g, false, files);
   fprintf(stderr, "tosem-scan: %zu files selected under %zu root(s)\n", files.size(), roots.size());
   std::ofstream os;
   if (!out_path.empty()) { os.open(out_path, std::ios::binary); csv_row(os, {"Index", "text", "Category", "cases", "File_ID", "Component"}); }
-  int64_t index = 0, cases = 0, file_id = 0, n_stmt = 0;
-  size_t first = 0;
-  while (first < files.size()) {
-    Batch B = next_batch(files, first);
-    tsm_ctx* ctx = nullptr;
-    ck(tsm_create(&ctx, 0, B.bytes + 4096, (int32_t)B.count(), (int32_t)std::max<size_t>(roots.size(), 1), 0), "tsm_create");
-    tsm_corpus c{B.arena, B.off.data(), B.len.data(), B.ext.data(), B.grp.data(), (int32_t)B.count(), (int32_t)std::max<size_t>(roots.size(), 1)};
-    std::vector<tsm_assert_event> aev;
-    std::vector<tsm_header_event> hev;
-    tsm_result r{};
-    scan_events(ctx, c, B.bytes, r, TSM_SCAN_HEADER_EVENTS, nullptr, aev, hev);
+  int64_t index = 0, cases = 0, file_id = 0, n_stmt = 0;   // carried across batches
+  const int32_t n_groups = (int32_t)roots.size();
+  std::vector<Batch> batches = plan_batches(files, all_of(files), batch_bytes, kBatchFiles);
+  scan_batches(files, batches, 0, n_groups, TSM_SCAN_HEADER_EVENTS, [&](const Batch& B, const Scanned& s) {
+    const tsm_corpus c = B.corpus(n_groups);
+    const std::vector<tsm_header_event>& hev = s.hev;
     std::vector<int64_t> base(B.count() + 1);
     int64_t nl = 0;
-    int rc = tsm_statements(ctx, &c, base.data(), nullptr, nullptr, 0, &nl, nullptr);
+    int rc = tsm_statements(s.ctx, &c, base.data(), nullptr, nullptr, 0, &nl, nullptr);
     if (rc != TSM_OK && rc != TSM_E_CAPACITY) ck(rc, "tsm_statements");
     std::vector<uint32_t> lend((size_t)std::max<int64_t>(nl, 1));
     std::vector<uint8_t> kind((size_t)std::max<int64_t>(nl, 1));
-    ck(tsm_statements(ctx, &c, base.data(), lend.data(), kind.data(), nl, &nl, nullptr), "tsm_statements");
-    tsm_destroy(ctx);
+    ck(tsm_statements(s.ctx, &c, base.data(), lend.data(), kind.data(), nl, &nl, nullptr), "tsm_statements");
     size_t hi = 0;
     for (size_t i = 0; i < B.count(); ++i) {
       const FileEntry& f = files[B.idx[i]];
-      const uint8_t* p = B.arena + B.off[i];
+      const uint8_t* p = B.arena.get() + B.off[i];
       ++file_id;
       bool in_case = false;
       std::string cur_stmt; bool have = false, listed = false;
@@ -903,8 +924,7 @@ static int cmd_body(const std::vector<std::string>& roots, const std::string& ou
       flush();
       while (hi < hev.size() && hev[hi].file == i) ++hi;
     }
-    tsm_host_free(B.arena);
-  }
+  });
   printf("files,cases,statements\r\n%lld,%lld,%lld\r\n", (long long)file_id, (long long)cases, (long long)n_stmt);
   return 0;
 }
@@ -913,33 +933,17 @@ static int cmd_body(const std::vector<std::string>& roots, const std::string& ou
 struct SnapFile { std::string rel; uint64_t digest; int64_t size; uint32_t n_assert; std::string hist; };
 
 // Scan one snapshot: per selected test file its digest, assertion total and "n:category, ..." histogram.
-static std::vector<SnapFile> scan_snapshot(const std::vector<FileEntry>& files) {
+static std::vector<SnapFile> scan_snapshot(const std::vector<FileEntry>& files, int64_t batch_bytes) {
   std::vector<SnapFile> out;
-  size_t first = 0;
-  while (first < files.size()) {
-    Batch B = next_batch(files, first);
-    tsm_ctx* ctx = nullptr;
-    ck(tsm_create(&ctx, 0, B.bytes + 4096, (int32_t)B.count(), 1, 0), "tsm_create");
-    tsm_corpus c{B.arena, B.off.data(), B.len.data(), B.ext.data(), B.grp.data(), (int32_t)B.count(), 1};
-    std::vector<tsm_file_stat> stats(B.count());
-    std::vector<tsm_assert_event> aev;
-    std::vector<tsm_header_event> hev;
-    tsm_result r{};
-    r.stats = stats.data();
-    scan_events(ctx, c, B.bytes, r, TSM_SCAN_ASSERT_EVENTS, nullptr, aev, hev);
-    tsm_destroy(ctx);
+  std::vector<Batch> batches = plan_batches(files, all_of(files), batch_bytes, kBatchFiles);
+  scan_batches(files, batches, 0, 1, TSM_SCAN_ASSERT_EVENTS, [&](const Batch& B, const Scanned& s) {
     size_t ai = 0;
     for (size_t i = 0; i < B.count(); ++i) {
-      std::map<std::string, int64_t> hist; std::vector<std::string> order;
-      for (; ai < aev.size() && aev[ai].file == i; ++ai) {
-        const std::string cat = event_category(B.arena + B.off[i], aev[ai]);
-        if (!hist.count(cat)) order.push_back(cat);
-        hist[cat]++;
-      }
-      out.push_back({files[B.idx[i]].rel, stats[i].digest, files[B.idx[i]].size, stats[i].n_assert, hist_cell(hist, order)});
+      CategoryHist hist;
+      for (; ai < s.aev.size() && s.aev[ai].file == i; ++ai) hist.add(event_category(B.arena.get() + B.off[i], s.aev[ai]));
+      out.push_back({files[B.idx[i]].rel, s.stats[i].digest, files[B.idx[i]].size, s.stats[i].n_assert, hist.cell()});
     }
-    tsm_host_free(B.arena);
-  }
+  });
   return out;
 }
 
@@ -966,7 +970,8 @@ static void walk_git(gitstore::Store& gs, const gitstore::Oid& tree, const std::
 
 // specs: <snapshot-root>=<tag>...; or, with --git <repository>, revisions (tags, branches, object names) in release
 // order - none = every tag of the repository, oldest commit first.
-static int cmd_releases(const std::vector<std::string>& specs_in, const std::string& out_path, const std::string& git_repo) {
+static int cmd_releases(const std::vector<std::string>& specs_in, const std::string& out_path, const std::string& git_repo,
+                        int64_t batch_bytes) {
   std::vector<std::string> specs = specs_in;
   gitstore::Store gs;
   if (!git_repo.empty()) {
@@ -999,7 +1004,7 @@ static int cmd_releases(const std::vector<std::string>& specs_in, const std::str
       tags.push_back(specs[t].substr(eq + 1));
       walk(specs[t].substr(0, eq), 0, false, files);
     }
-    const std::vector<SnapFile> snap = scan_snapshot(files);
+    const std::vector<SnapFile> snap = scan_snapshot(files, batch_bytes);
     std::vector<char> id_taken(ids.size(), 0), f_done(snap.size(), 0);
     auto bind = [&](size_t fi, size_t id) {
       const SnapFile& f = snap[fi];
@@ -1104,17 +1109,12 @@ static void find_renames(tsm_ctx* ctx, std::vector<RenameGroup>& groups, int min
       if (n.second) sn.push_back(&groups[c.g].add[c.a].bytes);
       co.push_back(o.first->second); cn.push_back(n.first->second);
     }
-    Batch PO, PN;
-    for (const std::vector<uint8_t>* f : so) PO.len.push_back((int32_t)f->size());
-    for (const std::vector<uint8_t>* f : sn) PN.len.push_back((int32_t)f->size());
-    alloc_arena(PO); alloc_arena(PN);
-    for (size_t i = 0; i < so.size(); ++i) if (PO.len[i]) memcpy(PO.arena + PO.off[i], so[i]->data(), so[i]->size());
-    for (size_t i = 0; i < sn.size(); ++i) if (PN.len[i]) memcpy(PN.arena + PN.off[i], sn[i]->data(), sn[i]->size());
-    tsm_corpus ko{PO.arena, PO.off.data(), PO.len.data(), PO.ext.data(), nullptr, (int32_t)so.size(), 1};
-    tsm_corpus kn{PN.arena, PN.off.data(), PN.len.data(), PN.ext.data(), nullptr, (int32_t)sn.size(), 1};
     std::vector<int64_t> common(cands.size());
-    ck(tsm_similarity(ctx, &ko, &kn, co.data(), cn.data(), (int64_t)cands.size(), common.data(), nullptr), "tsm_similarity");
-    tsm_host_free(PO.arena); tsm_host_free(PN.arena);
+    {
+      const Batch PO = pack(so), PN = pack(sn);
+      const tsm_corpus ko = PO.corpus(1), kn = PN.corpus(1);
+      ck(tsm_similarity(ctx, &ko, &kn, co.data(), cn.data(), (int64_t)cands.size(), common.data(), nullptr), "tsm_similarity");
+    }
     for (size_t k = 0; k < cands.size(); ++k) {
       const Cand& c = cands[k];
       std::vector<int64_t>& row = score[{c.g, c.d}];
@@ -1197,13 +1197,11 @@ static void diff_asserts(tsm_ctx* ctx, const tsm_corpus& ca, const tsm_corpus& c
 // number in that side's file, statement, category.  `k` walks the side's events (canonical order) across calls.
 static void assert_rows(std::ostream& os, const std::vector<std::string>& lead, const std::string& path, const uint8_t* base,
                         int32_t size, const std::vector<tsm_assert_event>& ev, size_t& k, uint32_t pair, const char* change) {
-  uint32_t pos = 0;
-  int64_t line = 1;
+  LineCounter lc{base};
   for (; k < ev.size() && ev[k].file == pair; ++k) {
     const tsm_assert_event& e = ev[k];
-    for (; pos < e.line_off; ++pos) line += base[pos] == '\n';
     std::vector<std::string> row = lead;
-    row.insert(row.end(), {path, change, std::to_string(line), event_statement(base, size, e), event_category(base, e)});
+    row.insert(row.end(), {path, change, std::to_string(lc.at(e.line_off)), event_statement(base, size, e), event_category(base, e)});
     csv_row(os, row);
   }
 }
@@ -1232,8 +1230,6 @@ struct ChangeTotals {
 
 // Like git's numstat, no line counts for a binary file: one with a NUL byte in its first 8000.
 static bool binary(const std::vector<uint8_t>& v) { return !v.empty() && memchr(v.data(), 0, std::min<size_t>(v.size(), 8000)) != nullptr; }
-
-static const int64_t kBatch = 512ll << 20;                  // bytes per side of one tsm_similarity or diff call
 
 // --find-renames: the deleted and the added files of a step (binary ones left out) form a group; groups are paired together
 // until a side holds kBatch bytes, then every pair's two changes become one (old side of the deleted file, new side of the
@@ -1341,13 +1337,9 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
     const size_t n = idx.size();
     if (!n && pairs) (*pairs)(ctx, r0, r1, idx, tsm_corpus{}, tsm_corpus{}, nullptr, nullptr, nullptr);
     if (!n) continue;
-    Batch S[2];
-    for (int s = 0; s < 2; ++s) {
-      for (const std::vector<uint8_t>& v : blobs[s]) S[s].len.push_back((int32_t)v.size());
-      alloc_arena(S[s]);
-      for (size_t i = 0; i < n; ++i) if (S[s].len[i]) memcpy(S[s].arena + S[s].off[i], blobs[s][i].data(), blobs[s][i].size());
-    }
-    Batch &A = S[0], &N = S[1];
+    std::vector<const std::vector<uint8_t>*> sides[2];
+    for (int s = 0; s < 2; ++s) for (const std::vector<uint8_t>& v : blobs[s]) sides[s].push_back(&v);
+    Batch A = pack(sides[0]), N = pack(sides[1]);
     // ext tags of both sides feed the assertion-line classification of the changed lines
     std::vector<size_t> group_step;                        // group g of the batch = step group_step[g]
     for (size_t i = 0; i < n; ++i) {
@@ -1359,8 +1351,7 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
       A.grp[i] = N.grp[i] = (uint16_t)(group_step.size() - 1);
     }
     const int32_t n_groups = want_asserts ? (int32_t)group_step.size() : 1;
-    tsm_corpus ca{A.arena, A.off.data(), A.len.data(), A.ext.data(), A.grp.data(), (int32_t)n, n_groups};
-    tsm_corpus cn{N.arena, N.off.data(), N.len.data(), N.ext.data(), N.grp.data(), (int32_t)n, n_groups};
+    const tsm_corpus ca = A.corpus(n_groups), cn = N.corpus(n_groups);
     std::vector<int64_t> added(n), removed(n);
     std::vector<tsm_diff_detail> det(n);
     ChangedAsserts chg;
@@ -1383,8 +1374,8 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
       for (size_t i = 0; as.is_open() && i < n; ++i) {
         const Change& c = changes[idx[i]];
         const std::vector<std::string> l = lead(c.step);
-        assert_rows(as, l, c.old_path.empty() ? c.path : c.old_path, A.arena + A.off[i], A.len[i], chg.rev, kr, (uint32_t)i, "-");
-        assert_rows(as, l, c.path, N.arena + N.off[i], N.len[i], chg.aev, ka, (uint32_t)i, "+");
+        assert_rows(as, l, c.old_path.empty() ? c.path : c.old_path, A.arena.get() + A.off[i], A.len[i], chg.rev, kr, (uint32_t)i, "-");
+        assert_rows(as, l, c.path, N.arena.get() + N.off[i], N.len[i], chg.aev, ka, (uint32_t)i, "+");
       }
     }
     for (size_t i = 0; i < n; ++i) {
@@ -1399,7 +1390,6 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
       csv_row(os, row);
     }
     t.diffed += (int64_t)n;
-    tsm_host_free(A.arena); tsm_host_free(N.arena);
   }
   tsm_destroy(ctx);
   if (!churn_path.empty()) {
@@ -1698,45 +1688,34 @@ static int cmd_blame(const std::string& repo, const std::string& rev, int64_t ma
     for (size_t f = 0; f < files.size(); ++f)
       for (size_t j = 0; j < org[f].size(); ++j) csv_row(os, cells(files[f].rel, (int64_t)j + 1, org[f][j]));
   }
-  // the assertion lines at R (SPEC section 4 Rev A, ext of the path at R): one scan with assertion events
+  // the assertion lines at R (SPEC section 4 Rev A, ext of the path at R): a scan with assertion events, in batches
   std::vector<int64_t> lines_of(owners.size(), 0), asserts_of(owners.size(), 0);
   for (size_t f = 0; f < files.size(); ++f) for (const tsm_origin& g : org[f]) lines_of[(size_t)g.change]++;
   int64_t n_asserts = 0;
-  if (!files.empty()) {
-    std::ofstream as;
-    if (!asserts_path.empty()) {
-      as.open(asserts_path, std::ios::binary);
-      csv_row(as, {"fileName", "line", "commit", "time", "origFileName", "origLine", "boundary", "statement", "category"});
-    }
-    Batch B;
-    for (size_t f = 0; f < files.size(); ++f) B.idx.push_back((uint32_t)f);
-    load_batch(files, B);
-    tsm_ctx* ctx = nullptr;
-    ck(tsm_create(&ctx, 0, std::max<int64_t>(B.bytes, 1 << 20), (int32_t)files.size(), 1, 0), "tsm_create");
-    tsm_corpus c{B.arena, B.off.data(), B.len.data(), B.ext.data(), B.grp.data(), (int32_t)files.size(), 1};
-    tsm_result r{};
-    std::vector<tsm_assert_event> aev;
-    std::vector<tsm_header_event> hev;
-    scan_events(ctx, c, B.bytes, r, TSM_SCAN_ASSERT_EVENTS, nullptr, aev, hev);
-    tsm_destroy(ctx);
+  std::ofstream as;
+  if (!asserts_path.empty() && !files.empty()) {
+    as.open(asserts_path, std::ios::binary);
+    csv_row(as, {"fileName", "line", "commit", "time", "origFileName", "origLine", "boundary", "statement", "category"});
+  }
+  std::vector<Batch> batches = plan_batches(files, all_of(files), batch_bytes, kBatchFiles);
+  scan_batches(files, batches, 0, 1, TSM_SCAN_ASSERT_EVENTS, [&](const Batch& B, const Scanned& s) {
     size_t k = 0;
-    for (size_t f = 0; f < files.size(); ++f) {
-      const uint8_t* base = B.arena + B.off[f];
-      uint32_t pos = 0;
-      int64_t line = 1;
-      for (; k < aev.size() && aev[k].file == f; ++k) {
-        for (; pos < aev[k].line_off; ++pos) line += base[pos] == '\n';
+    for (size_t i = 0; i < B.count(); ++i) {
+      const size_t f = B.idx[i];
+      const uint8_t* base = B.arena.get() + B.off[i];
+      LineCounter lc{base};
+      for (; k < s.aev.size() && s.aev[k].file == i; ++k) {
+        const int64_t line = lc.at(s.aev[k].line_off);
         if (org[f].empty()) continue;                        // (binary)
         const tsm_origin& g = org[f][(size_t)line - 1];
         asserts_of[(size_t)g.change]++; ++n_asserts;
         if (!as.is_open()) continue;
         std::vector<std::string> row = cells(files[f].rel, line, g);
-        row.insert(row.end(), {event_statement(base, B.len[f], aev[k]), event_category(base, aev[k])});
+        row.insert(row.end(), {event_statement(base, B.len[i], s.aev[k]), event_category(base, s.aev[k])});
         csv_row(as, row);
       }
     }
-    tsm_host_free(B.arena);
-  }
+  });
   // survival counts per commit that owns a line at R, in window order (the boundary commit first)
   std::vector<int64_t> cl(chain.size() + 1, 0), ca(chain.size() + 1, 0);
   for (size_t o = 0; o < owners.size(); ++o) {
@@ -1785,50 +1764,45 @@ static int cmd_clones(const std::vector<std::string>& roots, const std::string& 
     for (size_t g = 0; g < roots.size(); ++g) { walk(roots[g], (int)g, all_files, files); names.push_back(repo_name(roots[g])); }
   }
   fprintf(stderr, "tosem-scan: %zu files selected under %zu root(s)\n", files.size(), names.size());
+  std::vector<Batch> batches = plan_batches(files, all_of(files), (1ll << 31) - 4097, INT32_MAX);
   int64_t need = 4096;
-  for (const FileEntry& f : files) need += (f.size + 127) / 128 * 128;
-  if (need >= (1ll << 31) || files.size() >= (1u << 31))
+  for (const Batch& b : batches) need += b.bytes;
+  if (batches.size() > 1 || need >= (1ll << 31))           // (one batch over the limit: a single file that large)
     die("the selected files (" + std::to_string(need) + " bytes of arena) do not fit one int32-indexed arena; clones are found "
         "across all files at once, so select fewer files");
-  Batch B;
-  for (size_t i = 0; i < files.size(); ++i) B.idx.push_back((uint32_t)i);
-  load_batch(files, B);
-  const int32_t nf = (int32_t)B.count();
-  tsm_ctx* ctx = nullptr;
-  ck(tsm_create(&ctx, 0, B.bytes + 4096, std::max<int32_t>(nf, 1), 1, 0), "tsm_create");
-  tsm_corpus c{B.arena, B.off.data(), B.len.data(), B.ext.data(), nullptr, nf, 1};
-  std::vector<tsm_file_stat> stats((size_t)nf);
-  if (nf) { tsm_result sr{}; sr.stats = stats.data(); ck(tsm_scan(ctx, &c, &sr, 0, nullptr), "tsm_scan"); }
-  std::vector<int64_t> base((size_t)nf + 1), cbase(1), member(1);
-  std::vector<uint32_t> dup((size_t)nf), dupa((size_t)nf), clen(1);
-  tsm_clone_result r{base.data(), dup.data(), dupa.data(), nullptr, nullptr, 0, 0, nullptr, 0, 0};
-  ck(tsm_clones(ctx, &c, min_lines, &r, nullptr), "tsm_clones");  // the counts; the second call fills arrays of that size
-  cbase.resize((size_t)r.n_classes + 1); clen.resize((size_t)std::max<int64_t>(r.n_classes, 1)); member.resize((size_t)std::max<int64_t>(r.n_members, 1));
-  r.class_base = cbase.data(); r.class_len = clen.data(); r.class_cap = r.n_classes; r.member = member.data(); r.member_cap = r.n_members;
-  ck(tsm_clones(ctx, &c, min_lines, &r, nullptr), "tsm_clones");
-  tsm_destroy(ctx);
   const size_t ng = names.size();
   std::vector<std::vector<int64_t>> tot(ng + 1, std::vector<int64_t>(6, 0));   // files, lines, dup, asserts, dup asserts, classes
-  for (int32_t i = 0; i < nf; ++i) {
-    const size_t g = (size_t)files[B.idx[(size_t)i]].grp;
-    const int64_t v[5] = {1, (int64_t)stats[(size_t)i].n_lines, dup[(size_t)i], (int64_t)stats[(size_t)i].n_assert, dupa[(size_t)i]};
-    for (int k = 0; k < 5; ++k) { tot[g][(size_t)k] += v[k]; tot[ng][(size_t)k] += v[k]; }
-  }
-  tot[ng][5] = r.n_classes;
   std::ofstream os;
   if (!out_path.empty()) { os.open(out_path, std::ios::binary); csv_row(os, {"class", "repository", "fileName", "first_line", "last_line"}); }
-  std::vector<int64_t> seen(ng, -1);                      // the last class counted for each root
-  for (int64_t k = 0; k < r.n_classes; ++k)
-    for (int64_t j = cbase[(size_t)k]; j < cbase[(size_t)k + 1]; ++j) {
-      const int64_t at = member[(size_t)j];
-      const size_t f = (size_t)(std::upper_bound(base.begin(), base.end(), at) - base.begin() - 1);
-      const FileEntry& fe = files[B.idx[f]];
-      if (seen[(size_t)fe.grp] != k) { seen[(size_t)fe.grp] = k; tot[(size_t)fe.grp][5]++; }
-      if (os.is_open()) {
-        const int64_t first = at - base[f] + 1;
-        csv_row(os, {std::to_string(k + 1), names[(size_t)fe.grp], fe.rel, std::to_string(first), std::to_string(first + clen[(size_t)k] - 1)});
-      }
+  scan_batches(files, batches, 0, (int32_t)ng, 0, [&](const Batch& B, const Scanned& s) {
+    const int32_t nf = (int32_t)B.count();
+    const tsm_corpus c = B.corpus((int32_t)ng);
+    std::vector<int64_t> base((size_t)nf + 1), cbase(1), member(1);
+    std::vector<uint32_t> dup((size_t)nf), dupa((size_t)nf), clen(1);
+    tsm_clone_result r{base.data(), dup.data(), dupa.data(), nullptr, nullptr, 0, 0, nullptr, 0, 0};
+    ck(tsm_clones(s.ctx, &c, min_lines, &r, nullptr), "tsm_clones");   // the counts; the second call fills arrays of that size
+    cbase.resize((size_t)r.n_classes + 1); clen.resize((size_t)std::max<int64_t>(r.n_classes, 1)); member.resize((size_t)std::max<int64_t>(r.n_members, 1));
+    r.class_base = cbase.data(); r.class_len = clen.data(); r.class_cap = r.n_classes; r.member = member.data(); r.member_cap = r.n_members;
+    ck(tsm_clones(s.ctx, &c, min_lines, &r, nullptr), "tsm_clones");
+    for (int32_t i = 0; i < nf; ++i) {
+      const size_t g = (size_t)files[B.idx[(size_t)i]].grp;
+      const int64_t v[5] = {1, (int64_t)s.stats[(size_t)i].n_lines, dup[(size_t)i], (int64_t)s.stats[(size_t)i].n_assert, dupa[(size_t)i]};
+      for (int k = 0; k < 5; ++k) { tot[g][(size_t)k] += v[k]; tot[ng][(size_t)k] += v[k]; }
     }
+    tot[ng][5] = r.n_classes;
+    std::vector<int64_t> seen(ng, -1);                    // the last class counted for each root
+    for (int64_t k = 0; k < r.n_classes; ++k)
+      for (int64_t j = cbase[(size_t)k]; j < cbase[(size_t)k + 1]; ++j) {
+        const int64_t at = member[(size_t)j];
+        const size_t f = (size_t)(std::upper_bound(base.begin(), base.end(), at) - base.begin() - 1);
+        const FileEntry& fe = files[B.idx[f]];
+        if (seen[(size_t)fe.grp] != k) { seen[(size_t)fe.grp] = k; tot[(size_t)fe.grp][5]++; }
+        if (os.is_open()) {
+          const int64_t first = at - base[f] + 1;
+          csv_row(os, {std::to_string(k + 1), names[(size_t)fe.grp], fe.rel, std::to_string(first), std::to_string(first + clen[(size_t)k] - 1)});
+        }
+      }
+  });
   std::ostringstream so;
   csv_row(so, {"repository", "files", "lines", "duplicated_lines", "assertion_lines", "duplicated_assertion_lines", "classes"});
   for (size_t g = 0; g <= ng; ++g) {
@@ -1837,7 +1811,6 @@ static int cmd_clones(const std::vector<std::string>& roots, const std::string& 
     csv_row(so, row);
   }
   fputs(so.str().c_str(), stdout);
-  tsm_host_free(B.arena);
   return 0;
 }
 
@@ -1846,14 +1819,16 @@ static void usage() {
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
           "       tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]\n"
           "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--find-renames N]\n"
-          "       tosem-scan body   <project-root>... [--out F]\n"
-          "       tosem-scan releases <snapshot-root>=<tag>... [--out F]   |   releases --git <repository> [<revision>...] [--out F]\n"
+          "       tosem-scan body   <project-root>... [--batch-bytes N] [--out F]\n"
+          "       tosem-scan releases <snapshot-root>=<tag>... [--batch-bytes N] [--out F]\n"
+          "       tosem-scan releases --git <repository> [<revision>...] [--batch-bytes N] [--out F]\n"
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
           "                          [--find-renames N]\n"
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
           "       tosem-scan clones <project-root>... [--min-lines N] [--all-files] [--out F]\n"
           "       tosem-scan clones --git <repository> [--rev R] [--min-lines N] [--all-files] [--out F]\n"
           "--find-renames N (0..100): pair deleted and added files at least N %% similar, as git -M<N>%% does (docs/SPEC.md section 13).\n"
+          "--batch-bytes N: files go to the GPU in batches of at most N bytes (a larger file alone); scan: 1 GiB, else 512 MiB.\n"
           "Scans run on the GPU through libtosemscan.so (sm_90a); there is no CPU fallback.\n");
 }
 
@@ -1871,17 +1846,20 @@ int main(int argc, char** argv) {
     else if (a.rfind("--", 0) == 0) { if (i + 1 >= argc) die("missing value for " + a); opt[a] = argv[++i]; }
     else pos.push_back(a);
   }
+  auto batch_bytes = [&](int64_t dflt, int64_t least) {
+    return opt.count("--batch-bytes") ? std::max<int64_t>(least, atoll(opt["--batch-bytes"].c_str())) : dflt;
+  };
   if (cmd == "scan") { if (pos.empty()) die("scan needs at least one project root"); return cmd_scan(pos, opt["--rows"], opt["--summary"], opt.count("--gpus") ? atoi(opt["--gpus"].c_str()) : 1, all_files,
-                                        opt.count("--batch-bytes") ? std::max<int64_t>(4096, atoll(opt["--batch-bytes"].c_str())) : (1ll << 30), rev_b); }
+                                        batch_bytes(1ll << 30, 4096), rev_b); }
   if (cmd == "reduce") { if (pos.size() != 1) die("reduce needs the taxonomy csv"); return cmd_reduce(pos[0], opt["--strategy"], opt["--methods"], opt["--properties"], opt["--correlate"], opt["--correlate-tex"], opt["--correlate-counts"], opt["--correlate-merged"]); }
-  if (cmd == "releases") { if (pos.empty() && !opt.count("--git")) die("releases needs <root>=<tag>... or --git <repository>"); return cmd_releases(pos, opt["--out"], opt["--git"]); }
+  if (cmd == "releases") { if (pos.empty() && !opt.count("--git")) die("releases needs <root>=<tag>... or --git <repository>"); return cmd_releases(pos, opt["--out"], opt["--git"], batch_bytes(kBatch, 1)); }
   if (cmd == "clones") {
     if (pos.empty() == !opt.count("--git")) die("clones needs project roots or --git <repository>, not both");
     const long n = opt.count("--min-lines") ? strtol(opt["--min-lines"].c_str(), nullptr, 10) : 5;
     if (n < 1 || n > 1024) die("--min-lines needs a number of lines from 1 to 1024");
     return cmd_clones(pos, opt["--git"], opt.count("--rev") ? opt["--rev"] : "HEAD", (int)n, all_files, opt["--out"]);
   }
-  if (cmd == "body") { if (pos.empty()) die("body needs at least one project root"); return cmd_body(pos, opt["--out"]); }
+  if (cmd == "body") { if (pos.empty()) die("body needs at least one project root"); return cmd_body(pos, opt["--out"], batch_bytes(kBatch, 1)); }
   int rename_pct = -1;                                     // --find-renames N (docs/SPEC.md section 13); -1 = off
   if (opt.count("--find-renames")) {
     std::string v = opt["--find-renames"];
@@ -1899,7 +1877,7 @@ int main(int argc, char** argv) {
   if (cmd == "blame") { if (pos.size() != 1) die("blame needs the repository");
                         return cmd_blame(pos[0], opt.count("--rev") ? opt["--rev"] : "HEAD",
                                          opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0, all_files, rename_pct,
-                                         opt.count("--batch-bytes") ? std::max<int64_t>(1, atoll(opt["--batch-bytes"].c_str())) : kBatch,
+                                         batch_bytes(kBatch, 1),
                                          opt["--out"], opt["--asserts"]); }
   if (cmd == "diff") { if (pos.size() != 2) die("diff needs <old-root> <new-root>"); return cmd_diff(pos[0], pos[1], opt["--out"], opt["--asserts"], opt["--assert-churn"], rename_pct); }
   usage();
