@@ -29,6 +29,7 @@ import pytest
 import corpus_util as cu
 import orc
 import orc_asserts
+import orc_clones
 import orc_marks
 import orc_similarity
 import tosemscan as ts
@@ -317,6 +318,14 @@ def a_case(name):
             want = orc_similarity.similarity(x[0], x[1], co, cn)
             assert np.array_equal(r, want) and int((want > 0).sum()) > 1000
         return sc, lambda x, st: sc.similarity(x[0], x[1], co, cn, st), pair, twin, chk
+    if name == "clones":
+        c, twin = line_corpora()
+        sc = ts.Scanner(0, 1 << 20, 16, 4)
+
+        def chk(r, x):
+            orc_clones.assert_equal(r, orc_clones.clones(x, 5))
+            assert len(r["class_len"]) > 100 and (np.diff(r["class_base"]) > 32).any()
+        return sc, lambda x, st: sc.clones(x, 5, stream=st), c, twin, chk
     if name in ("line_hashes", "statements"):
         c, twin = line_corpora()
         sc = ts.Scanner(0, 1 << 20, 16, 4)
@@ -332,7 +341,7 @@ def a_case(name):
 
 A_CASES = ["scan-small-revA", "scan-small-revB", "scan-streamed-revA", "scan-streamed-revB", "resident", "diff_pairs",
            "diff_pairs_detail", "diff_pairs_asserts", "diff_resident", "diff_resident_asserts", "diff_pairs_marks",
-           "blame_pairs", "similarity", "line_hashes", "statements", "reduce"]
+           "blame_pairs", "similarity", "clones", "line_hashes", "statements", "reduce"]
 
 
 @pytest.mark.parametrize("name", A_CASES)
