@@ -212,6 +212,26 @@ typedef struct tsm_line_marks {
 int tsm_diff_pairs_marks(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
                          tsm_diff_detail* detail, tsm_line_marks* marks, void* stream);
 
+/* Test-case churn (docs/SPEC.md section 16): the cases of every old and every new side in global line order (files in order).
+ * A case starts at a header line (section 5, by the side's ext) and runs to the next header line of its file or to the file's
+ * end.  pair = the pair index; line = the 0-based header line in that file; n_lines; n_assert = its assertion lines (section 4,
+ * Rev A); n_changed = its lines that the canonical script of section 8 deletes (old side) or inserts (new side) - every line of
+ * the middle for a pair tsm_diff_pairs_detail does not trace; n_changed_assert = those that are assertion lines.  match (new
+ * cases only, else -1): when the case's header line is not inserted and the old line it corresponds to (the k-th line of new
+ * that is not inserted corresponds to the k-th line of old that is not deleted, section 14) is a header line, the index of the
+ * old case that starts there; else -1.  Matching by case name is left to the host.  n_old and n_new are always set; if
+ * old_cap < n_old or new_cap < n_new the call returns TSM_E_CAPACITY with both set (and no diff run): size the arrays and call
+ * again.  added / removed / detail are those of tsm_diff_pairs_detail (detail may be NULL).
+ * Kernels: k_scan with header events, the diff of tsm_diff_pairs_marks, then per side k_case_heads, k_case_kept, two
+ * exclusive scans, k_case_lines and k_case_reduce (csrc/tsm_case_kernels.cuh). */
+typedef struct tsm_case { int32_t pair, line, n_lines, n_assert, n_changed, n_changed_assert, match; } tsm_case;
+typedef struct tsm_diff_cases {
+  tsm_case* old_cases; int64_t old_cap; int64_t n_old;
+  tsm_case* new_cases; int64_t new_cap; int64_t n_new;
+} tsm_diff_cases;
+int tsm_diff_pairs_cases(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                         tsm_diff_detail* detail, tsm_diff_cases* out, void* stream);
+
 /* Line provenance (docs/SPEC.md section 14, `tosem-scan blame`): the origin of every line of every new side.  The pairs form
  * chains: prev[i] is the pair whose new side is pair i's old side (prev[i] < i; each pair is the prev of at most one pair), or
  * -1 for a chain head, whose old side's origins are origin_in[in_base[i] .. in_base[i+1]) (in_base [n_pairs+1], ascending;

@@ -19,6 +19,7 @@
 #include "tsm_lines_kernels.cuh"
 #include "tsm_similar_kernels.cuh"
 #include "tsm_clone_kernels.cuh"
+#include "tsm_case_kernels.cuh"
 
 using namespace tsm;
 
@@ -771,6 +772,7 @@ struct HostSide {                                         // device image of one
   int32_t n = 0; size_t ab = 0; uint32_t unit_cap = 0;
   DevBuf arena, off, len, ext, grp, line_base, line_end, line_hash, line_flag;   // (grp: only for the changed assertion lines)
   DevBuf line_mark;                                       // 1 = line deleted (old side) / inserted (new side): DIFF_MARKS only
+  DevBuf hev;                                             // header events of the scan, when asked for (test-case churn only)
   DevBuf unit_file, unit_begin, cnt, unit_first, bsum, zero, stats, unit_lines, unit_out, unit_line_base, s_hash, s_end, s_flag;
   std::vector<unsigned long long> base;                   // host copy of line_base (only when asked for)
   uint32_t n_units = 0;                                   // (file, chunk) work units: sum of ceil(len / 4 KiB)
@@ -840,7 +842,8 @@ int side_upload_grp(const tsm_corpus* k, HostSide& h, cudaStream_t st) {
 // host looks at anything: ONE synchronisation (capacity flags + line totals) per call instead of four per side.  The
 // staging arrays are sized for 8-byte lines; a side with more lines than that is scanned a second time with the exact
 // size (the first pass counted them).  scan_ms adds the device time of the k_scan launches (CUDA events on st).
-// host_base: also copy line_base to the host (HostSide::base).
+// host_base: also copy line_base to the host (HostSide::base).  flags: TSM_SCAN_HEADER_EVENTS also lists the header events
+// into HostSide::hev (hc.n_hev of them), sized like the staging arrays: a side has no more headers than lines.
 static int side_scan_pass(tsm_ctx* c, HostSide& h, ScanParams& p, size_t cap, int side, cudaStream_t st) {
   h.pin_hc = reinterpret_cast<Ctrl*>(c->h_diff + 32 * side);            // pinned: the copies below do not stall the host
   h.pin_total = reinterpret_cast<unsigned long long*>(c->h_diff + 64 + 8 * side);
@@ -849,6 +852,10 @@ static int side_scan_pass(tsm_ctx* c, HostSide& h, ScanParams& p, size_t cap, in
   if (!h.s_hash.alloc(sizeof(unsigned long long) * cap) || !h.s_end.alloc(sizeof(uint32_t) * cap) || !h.s_flag.alloc(cap)) return TSM_E_CUDA;
   p.lh_hash = h.s_hash.as<unsigned long long>(); p.lh_end = h.s_end.as<uint32_t>(); p.lh_flag = h.s_flag.as<uint8_t>();
   p.lh_cap = (uint32_t)cap;
+  if (p.flags & TSM_SCAN_HEADER_EVENTS) {
+    if (!h.hev.alloc(sizeof(tsm_header_event) * cap)) return TSM_E_CUDA;
+    p.hev = h.hev.as<tsm_header_event>(); p.hev_cap = (uint32_t)cap;
+  }
   CU(cudaMemsetAsync(h.zero.p, 0, 256 + sizeof(SlabCtl), st));
   k_plan_det<<<(n + 1 + 255) / 256, 256, 0, st>>>(p, h.unit_first.as<unsigned long long>());
   CU(cudaEventRecord(c->diff_ev[EV_SCAN[side].from], st));
@@ -863,7 +870,7 @@ static int side_scan_pass(tsm_ctx* c, HostSide& h, ScanParams& p, size_t cap, in
   return TSM_OK;
 }
 
-int sides_records(tsm_ctx* c, HostSide* const* sides, int ns, cudaStream_t st, float* scan_ms, bool host_base) {
+int sides_records(tsm_ctx* c, HostSide* const* sides, int ns, cudaStream_t st, float* scan_ms, bool host_base, uint32_t flags = 0) {
   if (ns < 1 || ns > 2) return TSM_E_ARG;
   ScanParams ps[2];
   size_t caps[2];
@@ -877,7 +884,7 @@ int sides_records(tsm_ctx* c, HostSide* const* sides, int ns, cudaStream_t st, f
     p.ctrl = reinterpret_cast<Ctrl*>(h.zero.as<uint8_t>()); p.slab = reinterpret_cast<SlabCtl*>(h.zero.as<uint8_t>() + 256);
     p.f_end = n;
     p.stats = h.stats.as<tsm_file_stat>();
-    p.flags = TSM_SCAN_LINE_HASHES;
+    p.flags = TSM_SCAN_LINE_HASHES | flags;
     p.unit_lines = h.unit_lines.as<uint32_t>(); p.unit_out = h.unit_out.as<uint32_t>();
     // units in (file, chunk) order
     k_file_units<<<(n + 255) / 256, 256, 0, st>>>(p.len, (uint32_t)n, h.cnt.as<uint32_t>());
@@ -892,7 +899,7 @@ int sides_records(tsm_ctx* c, HostSide* const* sides, int ns, cudaStream_t st, f
     const EvSpan ev = EV_SCAN[i];
     h.hc = *h.pin_hc; h.total = *h.pin_total;
     if (scan_ms) *scan_ms += elapsed_ms(c->diff_ev[ev.from], c->diff_ev[ev.to]);
-    if (h.hc.overflow) return TSM_E_CAPACITY;
+    if (h.hc.overflow && !h.hc.lh_overflow) return TSM_E_CAPACITY;   // (header events overflow only with the lines that bound them)
     if (h.hc.lh_overflow) {                                // more lines than the staging arrays hold: once more, exact size
       const int rc = side_scan_pass(c, h, ps[i], (size_t)h.hc.n_lh + 64, i, st);
       if (rc != TSM_OK) return rc;
@@ -980,12 +987,13 @@ static int pair_upload(const tsm_corpus* olds, const tsm_corpus* news, bool with
   return rc;
 }
 
-// The line records of both uploaded sides of P (*scan_ms = k_scan over both; host_base: line_base of each side on the host too).
-static int pair_records(tsm_ctx* c, HostSidePair& P, float* scan_ms, bool host_base, cudaStream_t st) {
+// The line records of both uploaded sides of P (*scan_ms = k_scan over both; host_base: line_base of each side on the host too;
+// flags: TSM_SCAN_HEADER_EVENTS for their header events too).
+static int pair_records(tsm_ctx* c, HostSidePair& P, float* scan_ms, bool host_base, cudaStream_t st, uint32_t flags = 0) {
   *scan_ms = 0;
   P.A.launches = P.B.launches = 0;
   HostSide* both[2] = {&P.A, &P.B};
-  return sides_records(c, both, 2, st, scan_ms, host_base);
+  return sides_records(c, both, 2, st, scan_ms, host_base, flags);
 }
 
 // The diff proper over two sides whose line records exist.  k_diff_small finishes the common pairs (distance at most
@@ -1321,6 +1329,83 @@ extern "C" int tsm_diff_pairs_marks(tsm_ctx* c, const tsm_corpus* olds, const ts
   if (mk->n_old) CU(cudaMemcpyAsync(mk->del, P.A.line_mark.p, (size_t)mk->n_old, cudaMemcpyDeviceToHost, st));
   if (mk->n_new) CU(cudaMemcpyAsync(mk->ins, P.B.line_mark.p, (size_t)mk->n_new, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
+  return TSM_OK;
+}
+
+// ------------------------------------------------------------------------------------- SPEC section 16 test-case churn
+// The line records of both sides with their header events (the case counts, so the capacity check comes before the diff),
+// k_case_heads per side, the marks diff, then per side k_case_kept, xscan of the heads and of the kept lines, k_case_lines
+// (old side first: the new side's k_case_reduce reads old_by_rank) and k_case_reduce (csrc/tsm_case_kernels.cuh).
+extern "C" int tsm_diff_pairs_cases(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                                    tsm_diff_detail* detail, tsm_diff_cases* out, void* stream) {
+  if (!c || !olds || !news || !added || !removed || !out || olds->n_files != news->n_files) return TSM_E_ARG;
+  const int32_t n = olds->n_files;
+  out->n_old = out->n_new = 0;
+  if (n == 0) return TSM_OK;
+  int rc = check_sides({olds, news}, n, true);
+  if (rc != TSM_OK) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  CallScope call(c, st);
+  CU(call.status);
+  HostSidePair P;
+  DevBuf d_head[2], d_kept[2], d_case_of[2], d_rank[2], d_first[2], d_cases[2], d_by_rank, d_bsum;
+  SyncGuard guard(st);
+  rc = pair_upload(olds, news, false, P, st);
+  if (rc == TSM_OK) rc = pair_records(c, P, &c->diff_ms[0], false, st, TSM_SCAN_HEADER_EVENTS);
+  if (rc != TSM_OK) return rc;
+  out->n_old = P.A.hc.n_hev; out->n_new = P.B.hc.n_hev;
+  if (out->old_cap < out->n_old || out->new_cap < out->n_new) return TSM_E_CAPACITY;
+  if ((out->n_old && !out->old_cases) || (out->n_new && !out->new_cases)) return TSM_E_ARG;
+  HostSide* side[2] = {&P.A, &P.B};
+  tsm_case* const h_out[2] = {out->old_cases, out->new_cases};
+  int launches = 0;
+  for (int s = 0; s < 2; ++s) {
+    const HostSide& h = *side[s];
+    const size_t total = (size_t)h.total, ne = h.hc.n_hev;
+    if (!d_head[s].alloc(sizeof(uint32_t) * total) || !d_kept[s].alloc(sizeof(uint32_t) * total) ||
+        !d_case_of[s].alloc(sizeof(unsigned long long) * (total + 1)) || !d_rank[s].alloc(sizeof(unsigned long long) * (total + 1)) ||
+        !d_first[s].alloc(sizeof(uint32_t) * ne) || !d_cases[s].alloc(sizeof(tsm_case) * ne))
+      return TSM_E_CUDA;
+    CU(cudaMemsetAsync(d_head[s].p, 0, sizeof(uint32_t) * total, st));
+    if (ne) {
+      k_case_heads<<<(unsigned)((ne + 255) / 256), 256, 0, st>>>(h.hev.as<tsm_header_event>(), (uint32_t)ne, h.d.line_base, h.d.line_end,
+                                                                 d_head[s].as<uint32_t>());
+      ++launches;
+    }
+  }
+  CU(cudaGetLastError());
+  if (!d_by_rank.alloc(sizeof(uint32_t) * (size_t)P.A.total) ||
+      !d_bsum.alloc(sizeof(unsigned long long) * ((size_t)std::max(P.A.total, P.B.total) / XS_TILE + 4)))
+    return TSM_E_CUDA;
+  rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
+  if (rc != TSM_OK) return rc;
+  for (int s = 0; s < 2; ++s) {
+    const HostSide& h = *side[s];
+    const uint32_t total = (uint32_t)h.total;
+    if (total) k_case_kept<<<(total + 255) / 256, 256, 0, st>>>(h.line_mark.as<uint8_t>(), total, d_kept[s].as<uint32_t>());
+    xscan(d_head[s].as<uint32_t>(), total, d_bsum.as<unsigned long long>(), d_case_of[s].as<unsigned long long>(), st);
+    xscan(d_kept[s].as<uint32_t>(), total, d_bsum.as<unsigned long long>(), d_rank[s].as<unsigned long long>(), st);
+    if (total)
+      k_case_lines<<<(total + 255) / 256, 256, 0, st>>>(d_head[s].as<uint32_t>(), d_kept[s].as<uint32_t>(), d_case_of[s].as<unsigned long long>(),
+                                                        d_rank[s].as<unsigned long long>(), total, d_first[s].as<uint32_t>(),
+                                                        s == 0 ? d_by_rank.as<uint32_t>() : nullptr);
+    launches += total ? 8 : 0;
+  }
+  for (int s = 0; s < 2; ++s) {
+    const HostSide& h = *side[s];
+    const uint32_t ne = h.hc.n_hev;
+    if (!ne) continue;
+    const CaseSide cs{h.d.line_base, (uint32_t)n, h.d.line_flag, h.line_mark.as<uint8_t>(), d_first[s].as<uint32_t>(), ne};
+    const bool nw = s == 1;
+    k_case_reduce<<<std::min((ne + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(
+        cs, d_rank[s].as<unsigned long long>(), nw ? d_by_rank.as<uint32_t>() : nullptr, nw ? d_head[0].as<uint32_t>() : nullptr,
+        nw ? d_case_of[0].as<unsigned long long>() : nullptr, d_cases[s].as<tsm_case>());
+    ++launches;
+    CU(cudaMemcpyAsync(h_out[s], d_cases[s].p, sizeof(tsm_case) * ne, cudaMemcpyDeviceToHost, st));
+  }
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(st));
+  c->launches += launches;
   return TSM_OK;
 }
 

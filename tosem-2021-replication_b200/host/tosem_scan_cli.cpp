@@ -17,10 +17,10 @@
 //
 //   tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N]
 //   tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]
-//   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--find-renames N]
+//   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--find-renames N]
 //   tosem-scan body   <project-root>... [--batch-bytes N] [--out F]
 //   tosem-scan releases <snapshot-root>=<tag>... | --git <repository> [<revision>...]   [--batch-bytes N] [--out F]
-//   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]
+//   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F] [--cases F]
 //                      [--find-renames N]
 //   tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]
 //   tosem-scan clones <project-root>... | --git <repository> [--rev R]   [--min-lines N] [--all-files] [--out F]
@@ -1215,6 +1215,77 @@ static void churn_rows(std::ostream& os, const std::vector<std::string>& lead, c
     }
 }
 
+// Test-case churn (docs/SPEC.md section 16) of one diff call: the case records of both sides (tsm_diff_pairs_cases), arrays
+// grown to the counts the library reports when they are too small.
+struct CaseLists { std::vector<tsm_case> olds, news; };
+static void diff_cases(tsm_ctx* ctx, const tsm_corpus& ca, const tsm_corpus& cn, int64_t* added, int64_t* removed,
+                       tsm_diff_detail* det, CaseLists& r) {
+  int64_t co = (int64_t)ca.off[ca.n_files] / 512 + 64, cc = (int64_t)cn.off[cn.n_files] / 512 + 64;
+  for (;;) {
+    r.olds.resize((size_t)co); r.news.resize((size_t)cc);
+    tsm_diff_cases o{r.olds.data(), co, 0, r.news.data(), cc, 0};
+    const int rc = tsm_diff_pairs_cases(ctx, &ca, &cn, added, removed, det, &o, nullptr);
+    if (rc == TSM_E_CAPACITY && (o.n_old > co || o.n_new > cc)) { co = std::max(co, o.n_old); cc = std::max(cc, o.n_new); continue; }
+    ck(rc, "tsm_diff_pairs_cases");
+    r.olds.resize((size_t)o.n_old); r.news.resize((size_t)o.n_new);
+    return;
+  }
+}
+
+// The case name (docs/SPEC.md section 10) of every case of one side of a pair, from the header lines of the side's bytes.
+static std::vector<std::string> case_names(const uint8_t* base, int32_t size, int ext, const tsm_case* cs, size_t n) {
+  std::vector<std::string> out;
+  int32_t line = 0, pos = 0;
+  for (size_t k = 0; k < n; ++k) {                          // cases in line order: one walk over the bytes
+    for (; line < cs[k].line; ++line) pos = (int32_t)((const uint8_t*)memchr(base + pos, '\n', (size_t)(size - pos)) - base) + 1;
+    const uint8_t* lf = (const uint8_t*)memchr(base + pos, '\n', (size_t)(size - pos));
+    out.push_back(case_name(ext, base + pos, (uint32_t)((lf ? (int32_t)(lf - base) : size) - pos)));
+  }
+  return out;
+}
+
+// The --cases rows of one pair (docs/SPEC.md section 16) from its old cases oc[0, no) and new cases nc[0, nn), old case
+// index o_first being oc[0]: matches by kept header line come with the records, matches by name (once among the unmatched
+// cases of each side) are made here; then the D rows in old line order and the A and M rows in new line order.
+struct CaseSide { const uint8_t* base; int32_t size; int ext; const std::string* path; };
+static void case_rows(std::ostream& os, std::vector<std::string> lead, const CaseSide& o, const CaseSide& nw, const std::string* old_path,
+                      const tsm_case* oc, size_t no, const tsm_case* nc, size_t nn, size_t o_first) {
+  const std::vector<std::string> na = case_names(o.base, o.size, o.ext, oc, no), nb = case_names(nw.base, nw.size, nw.ext, nc, nn);
+  std::vector<int64_t> match(nn, -1);
+  std::vector<char> used(no, 0);
+  for (size_t j = 0; j < nn; ++j)
+    if (nc[j].match >= 0) { match[j] = nc[j].match - (int64_t)o_first; used[(size_t)match[j]] = 1; }
+  std::map<std::string, int64_t> cnt_new, cnt_old, old_of;
+  for (size_t j = 0; j < nn; ++j) if (match[j] < 0) ++cnt_new[nb[j]];
+  for (size_t k = 0; k < no; ++k) if (!used[k]) { ++cnt_old[na[k]]; old_of[na[k]] = (int64_t)k; }
+  for (size_t j = 0; j < nn; ++j)
+    if (match[j] < 0 && cnt_new[nb[j]] == 1 && cnt_old[nb[j]] == 1) { match[j] = old_of[nb[j]]; used[(size_t)match[j]] = 1; }
+  auto num = [](int64_t v) { return std::to_string(v); };
+  auto row = [&](const std::string& path, std::vector<std::string> cells) {
+    std::vector<std::string> r = lead;
+    r.push_back(path);
+    r.insert(r.end(), cells.begin(), cells.end());
+    if (old_path) r.push_back(*old_path);
+    csv_row(os, r);
+  };
+  for (size_t k = 0; k < no; ++k) {
+    if (used[k]) continue;
+    const tsm_case& c = oc[k];
+    row(*o.path, {na[k], "D", "", num(c.line + 1), "", num(c.n_lines), "", num(c.n_assert), "", num(c.n_changed), "", num(c.n_changed_assert)});
+  }
+  for (size_t j = 0; j < nn; ++j) {
+    const tsm_case& c = nc[j];
+    if (match[j] < 0) {
+      row(*nw.path, {nb[j], "A", num(c.line + 1), "", num(c.n_lines), "", num(c.n_assert), "", num(c.n_changed), "", num(c.n_changed_assert), ""});
+      continue;
+    }
+    const tsm_case& d = oc[(size_t)match[j]];
+    if (c.n_changed || d.n_changed || c.n_lines != d.n_lines)
+      row(*nw.path, {nb[j], "M", num(c.line + 1), num(d.line + 1), num(c.n_lines), num(d.n_lines), num(c.n_assert), num(d.n_assert),
+                     num(c.n_changed), num(d.n_changed), num(c.n_changed_assert), num(d.n_changed_assert)});
+  }
+}
+
 // One changed file of a revision pair.  `step` is its commit (history) or 0 (diff); `o` and `n` name the bytes of the old and
 // the new side for the caller's loader, -1 where that side does not exist.  A rename (--find-renames) moves the deleted file's
 // `o` onto the added file and keeps the deleted file's path and the score in %.
@@ -1297,13 +1368,13 @@ using BatchFn = std::function<void(tsm_ctx*, size_t r0, size_t r1, const std::ve
 static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, const Loader& load, int rename_pct, bool zero_rows,
                                  const std::vector<std::string>& lead_head, size_t churn_lead,
                                  const std::function<std::vector<std::string>(size_t)>& lead, const std::string& out_path,
-                                 const std::string& asserts_path, const std::string& churn_path, int64_t batch_bytes = kBatch,
-                                 const BatchFn* pairs = nullptr) {
+                                 const std::string& asserts_path, const std::string& churn_path, const std::string& cases_path,
+                                 int64_t batch_bytes = kBatch, const BatchFn* pairs = nullptr) {
   ChangeTotals t(n_steps);
   tsm_ctx* ctx = nullptr;
   ck(tsm_create(&ctx, 0, 1 << 20, 16, 1, 0), "tsm_create");
   if (rename_pct >= 0) pair_renames(ctx, changes, load, rename_pct, t);
-  std::ofstream os, as;
+  std::ofstream os, as, cs;
   if (!out_path.empty()) {
     os.open(out_path, std::ios::binary);
     std::vector<std::string> head = lead_head;
@@ -1316,6 +1387,14 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
     std::vector<std::string> head = lead_head;
     head.insert(head.end(), {"fileName", "change", "line", "statement", "category"});
     csv_row(as, head);
+  }
+  if (!cases_path.empty()) {
+    cs.open(cases_path, std::ios::binary);
+    std::vector<std::string> head = lead_head;
+    head.insert(head.end(), {"fileName", "case", "change", "line", "oldLine", "lines", "oldLines", "asserts", "oldAsserts", "insertedLines",
+                             "deletedLines", "insertedAsserts", "deletedAsserts"});
+    if (rename_pct >= 0) head.push_back("oldFileName");
+    csv_row(cs, head);
   }
   const bool want_asserts = !asserts_path.empty() || !churn_path.empty();
   std::map<size_t, std::vector<int64_t>> churn;            // per step with changed assertion lines: its [K] added and removed rows
@@ -1355,10 +1434,12 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
     std::vector<int64_t> added(n), removed(n);
     std::vector<tsm_diff_detail> det(n);
     ChangedAsserts chg;
+    CaseLists cases;
     if (pairs) {
       (*pairs)(ctx, r0, r1, idx, ca, cn, added.data(), removed.data(), det.data());
     } else if (!want_asserts) {
-      ck(tsm_diff_pairs_detail(ctx, &ca, &cn, added.data(), removed.data(), det.data(), nullptr), "tsm_diff_pairs_detail");
+      if (cs.is_open()) diff_cases(ctx, ca, cn, added.data(), removed.data(), det.data(), cases);
+      else ck(tsm_diff_pairs_detail(ctx, &ca, &cn, added.data(), removed.data(), det.data(), nullptr), "tsm_diff_pairs_detail");
     } else {
       diff_asserts(ctx, ca, cn, added.data(), removed.data(), det.data(), chg);
       for (size_t g = 0; g < group_step.size(); ++g) {     // a step's files may span two batches
@@ -1377,6 +1458,21 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
         assert_rows(as, l, c.old_path.empty() ? c.path : c.old_path, A.arena.get() + A.off[i], A.len[i], chg.rev, kr, (uint32_t)i, "-");
         assert_rows(as, l, c.path, N.arena.get() + N.off[i], N.len[i], chg.aev, ka, (uint32_t)i, "+");
       }
+      if (cs.is_open()) {                                  // a second call: the assertion tables and the cases are separate diffs
+        std::vector<int64_t> a2(n), r2(n);
+        diff_cases(ctx, ca, cn, a2.data(), r2.data(), nullptr, cases);
+      }
+    }
+    for (size_t i = 0, ko = 0, kn = 0; cs.is_open() && i < n; ++i) {
+      const Change& c = changes[idx[i]];
+      const size_t o0 = ko, n0 = kn;
+      while (ko < cases.olds.size() && cases.olds[ko].pair == (int32_t)i) ++ko;
+      while (kn < cases.news.size() && cases.news[kn].pair == (int32_t)i) ++kn;
+      if (ko == o0 && kn == n0) continue;
+      const std::string& old_path = c.old_path.empty() ? c.path : c.old_path;
+      case_rows(cs, lead(c.step), CaseSide{A.arena.get() + A.off[i], A.len[i], A.ext[i], &old_path},
+                CaseSide{N.arena.get() + N.off[i], N.len[i], N.ext[i], &c.path}, rename_pct >= 0 ? &c.old_path : nullptr,
+                cases.olds.data() + o0, ko - o0, cases.news.data() + n0, kn - n0, o0);
     }
     for (size_t i = 0; i < n; ++i) {
       const Change& c = changes[idx[i]];
@@ -1407,7 +1503,7 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
 }
 
 static int cmd_diff(const std::string& old_root, const std::string& new_root, const std::string& out_path,
-                    const std::string& asserts_path, const std::string& churn_path, int rename_pct) {
+                    const std::string& asserts_path, const std::string& churn_path, const std::string& cases_path, int rename_pct) {
   std::vector<FileEntry> a, b;
   walk(old_root, 0, true, a);
   walk(new_root, 0, true, b);
@@ -1426,7 +1522,7 @@ static int cmd_diff(const std::string& old_root, const std::string& new_root, co
     return v;
   };
   const ChangeTotals t = diff_changes(changes, 1, load, rename_pct, false, {}, 0, [](size_t) { return std::vector<std::string>(); },
-                                      out_path, asserts_path, churn_path);
+                                      out_path, asserts_path, churn_path, cases_path);
   if (t.binaries) fprintf(stderr, "tosem-scan: %lld binary file(s) skipped\n", (long long)t.binaries);
   if (rename_pct >= 0)
     fprintf(stderr, "tosem-scan: %lld rename(s) found (%lld exact, %lld inexact)\n", (long long)t.renames, (long long)t.renames_exact,
@@ -1498,7 +1594,8 @@ static void history_walk(gitstore::Store& gs, const std::string& rev, int64_t ma
 // --dry-run: no GPU - the rows carry the object names, sizes and an FNV-1a checksum of both blobs instead of the counts
 // (what the CPU tests compare with `git diff-tree` / `git cat-file`).
 static int cmd_history(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files, const std::string& out_path,
-                       bool dry_run, const std::string& asserts_path, const std::string& churn_path, int rename_pct) {
+                       bool dry_run, const std::string& asserts_path, const std::string& churn_path, const std::string& cases_path,
+                       int rename_pct) {
   gitstore::Store gs;
   std::string err;
   if (!gs.open(repo, err)) die(err);
@@ -1534,7 +1631,7 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
       t.files[c.step]++;
     }
   } else {
-    t = diff_changes(changes, chain.size(), load, rename_pct, true, {"commit", "parent", "time"}, 1, lead, out_path, asserts_path, churn_path);
+    t = diff_changes(changes, chain.size(), load, rename_pct, true, {"commit", "parent", "time"}, 1, lead, out_path, asserts_path, churn_path, cases_path);
   }
   printf("commit,files,cloc,added,removed\r\n");
   int64_t ta = 0, tr = 0;
@@ -1663,7 +1760,7 @@ static int cmd_blame(const std::string& repo, const std::string& rev, int64_t ma
     }
   };
   const ChangeTotals t = diff_changes(changes, chain.size(), load, rename_pct, true, {}, 0, [](size_t) { return std::vector<std::string>(); },
-                                      "", "", "", batch_bytes, &run);
+                                      "", "", "", "", batch_bytes, &run);
   // the selected files at R, path order: their origins (a file untouched by the window is all boundary lines)
   std::vector<FileEntry> files;
   if (!chain.empty()) walk_git(gs, chain.back().c.tree, "", all_files, files);
@@ -1818,16 +1915,17 @@ static void usage() {
   fprintf(stderr,
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
           "       tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]\n"
-          "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--find-renames N]\n"
+          "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--find-renames N]\n"
           "       tosem-scan body   <project-root>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases <snapshot-root>=<tag>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases --git <repository> [<revision>...] [--batch-bytes N] [--out F]\n"
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
-          "                          [--find-renames N]\n"
+          "                          [--cases F] [--find-renames N]\n"
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
           "       tosem-scan clones <project-root>... [--min-lines N] [--all-files] [--out F]\n"
           "       tosem-scan clones --git <repository> [--rev R] [--min-lines N] [--all-files] [--out F]\n"
           "--find-renames N (0..100): pair deleted and added files at least N %% similar, as git -M<N>%% does (docs/SPEC.md section 13).\n"
+          "--cases F: one row per test case that a revision adds (A), deletes (D) or modifies (M) (docs/SPEC.md section 16).\n"
           "--batch-bytes N: files go to the GPU in batches of at most N bytes (a larger file alone); scan: 1 GiB, else 512 MiB.\n"
           "Scans run on the GPU through libtosemscan.so (sm_90a); there is no CPU fallback.\n");
 }
@@ -1873,13 +1971,13 @@ int main(int argc, char** argv) {
                           if (dry_run && rename_pct >= 0) die("--dry-run and --find-renames cannot be combined (renames need the GPU)");
                           return cmd_history(pos[0], opt.count("--rev") ? opt["--rev"] : "HEAD",
                                                   opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0, all_files, opt["--out"], dry_run,
-                                                  opt["--asserts"], opt["--assert-churn"], rename_pct); }
+                                                  opt["--asserts"], opt["--assert-churn"], opt["--cases"], rename_pct); }
   if (cmd == "blame") { if (pos.size() != 1) die("blame needs the repository");
                         return cmd_blame(pos[0], opt.count("--rev") ? opt["--rev"] : "HEAD",
                                          opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0, all_files, rename_pct,
                                          batch_bytes(kBatch, 1),
                                          opt["--out"], opt["--asserts"]); }
-  if (cmd == "diff") { if (pos.size() != 2) die("diff needs <old-root> <new-root>"); return cmd_diff(pos[0], pos[1], opt["--out"], opt["--asserts"], opt["--assert-churn"], rename_pct); }
+  if (cmd == "diff") { if (pos.size() != 2) die("diff needs <old-root> <new-root>"); return cmd_diff(pos[0], pos[1], opt["--out"], opt["--asserts"], opt["--assert-churn"], opt["--cases"], rename_pct); }
   usage();
   return 2;
 }

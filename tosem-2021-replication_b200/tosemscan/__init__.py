@@ -30,6 +30,8 @@ HEADER_EVENT = np.dtype([("file", "<u4"), ("line_off", "<u4"), ("line_len", "<u4
 DIFF_DETAIL = np.dtype([("hunks_add", "<i8"), ("hunks_del", "<i8"), ("hunks_mod", "<i8"),
                         ("added_assert", "<i8"), ("removed_assert", "<i8")])
 ORIGIN = np.dtype([("change", "<i4"), ("line", "<i4")])   # tsm_origin: the change that inserted a line, 1-based line there
+CASE = np.dtype([("pair", "<i4"), ("line", "<i4"), ("n_lines", "<i4"), ("n_assert", "<i4"), ("n_changed", "<i4"),
+                 ("n_changed_assert", "<i4"), ("match", "<i4")])   # tsm_case: one test case of one side of a revision pair
 
 # every symbol include/tosemscan.h declares (tests check the library exports exactly these)
 SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create", "tsm_destroy", "tsm_scan",
@@ -37,7 +39,8 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_diff_pairs", "tsm_diff_pairs_detail", "tsm_statements", "tsm_line_hashes", "tsm_diff_upload", "tsm_diff_resident", "tsm_diff_last_ms",
            "tsm_diff_pairs_asserts", "tsm_diff_resident_asserts", "tsm_reduce", "tsm_host_alloc", "tsm_host_free", "tsm_layout", "tsm_gen_sizes",
            "tsm_gen_fill", "tsm_gen_edit", "tsm_gen_pair_sizes", "tsm_gen_pair_fill", "tsm_similarity", "tsm_similarity_last_ms",
-           "tsm_diff_pairs_marks", "tsm_blame_pairs", "tsm_blame_last_ms", "tsm_clones", "tsm_clones_last_ms"]
+           "tsm_diff_pairs_marks", "tsm_blame_pairs", "tsm_blame_last_ms", "tsm_clones", "tsm_clones_last_ms",
+           "tsm_diff_pairs_cases"]
 
 
 class TsmError(RuntimeError):
@@ -68,6 +71,11 @@ class _DiffAsserts(C.Structure):
     _fields_ = [("added_counts", C.c_void_p), ("removed_counts", C.c_void_p),
                 ("aev", C.c_void_p), ("aev_cap", C.c_int64), ("n_aev", C.c_int64),
                 ("rev", C.c_void_p), ("rev_cap", C.c_int64), ("n_rev", C.c_int64)]
+
+
+class _DiffCases(C.Structure):
+    _fields_ = [("old_cases", C.c_void_p), ("old_cap", C.c_int64), ("n_old", C.c_int64),
+                ("new_cases", C.c_void_p), ("new_cap", C.c_int64), ("n_new", C.c_int64)]
 
 
 class _CloneResult(C.Structure):
@@ -163,6 +171,9 @@ def lib():
         L.tsm_diff_pairs_marks.restype = C.c_int
         L.tsm_diff_pairs_marks.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 3 + \
             [C.POINTER(_LineMarks), C.c_void_p]
+        L.tsm_diff_pairs_cases.restype = C.c_int
+        L.tsm_diff_pairs_cases.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 3 + \
+            [C.POINTER(_DiffCases), C.c_void_p]
         L.tsm_blame_pairs.restype = C.c_int
         L.tsm_blame_pairs.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 10 + \
             [C.c_int64, C.POINTER(C.c_int64), C.c_void_p]
@@ -663,6 +674,27 @@ class Scanner:
                 raise TsmError(rc, "tsm_diff_pairs_marks")
             return added, removed, det[:n], bo, bn, dels[:mk.n_old], ins[:mk.n_new]
         raise TsmError(TSM_E_CAPACITY, "tsm_diff_pairs_marks")
+
+    def diff_cases(self, olds, news, stream=None, cap=None):
+        """Test-case churn (docs/SPEC.md section 16): (added, removed, detail, old_cases, new_cases) with the cases of every old
+        and every new side as CASE arrays in global line order (pair, 0-based header line, lines, assertion lines, deleted or
+        inserted lines, deleted or inserted assertion lines, and for new cases the index of the old case matched by its kept
+        header line, else -1).  Arrays too small for the cases are sized and the call made again (cap: the first guess)."""
+        n = olds.n_files
+        added, removed, det = np.zeros(n, np.int64), np.zeros(n, np.int64), np.zeros(max(n, 1), DIFF_DETAIL)
+        a, b = olds.c_struct(), news.c_struct()
+        co = cn = int(cap if cap is not None else 0)
+        for _ in range(2):
+            oc, nc = np.zeros(max(co, 1), CASE), np.zeros(max(cn, 1), CASE)
+            r = _DiffCases(_p(oc), co, 0, _p(nc), cn, 0)
+            rc = lib().tsm_diff_pairs_cases(self._ctx, C.byref(a), C.byref(b), _p(added), _p(removed), _p(det), C.byref(r), stream)
+            if rc == TSM_E_CAPACITY and (r.n_old > co or r.n_new > cn):
+                co, cn = int(r.n_old), int(r.n_new)
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_diff_pairs_cases")
+            return added, removed, det[:n], oc[:r.n_old], nc[:r.n_new]
+        raise TsmError(TSM_E_CAPACITY, "tsm_diff_pairs_cases")
 
     def blame_pairs(self, olds, news, prev, label, heads, stream=None, cap=None):
         """Line provenance (docs/SPEC.md section 14): (added, removed, detail, line_base_new, origins) with origins an ORIGIN array
