@@ -1,15 +1,24 @@
-"""The batch loop every file-scanning command of `tosem-scan` shares: on the C1 test files (tests/golden/c1_testfiles.npz) in nine
-roots, `scan`, `body` and `releases` give byte-identical stdout and files with the default batch size and with a `--batch-bytes`
-that cuts the tree into dozens of batches (counters and walk order carried across batches, one context per command); and every
-command prints its empty result for a tree with no selected file."""
+"""The batch loops of `tosem-scan`.  Scans: on the C1 test files (tests/golden/c1_testfiles.npz) in nine roots, `scan`, `body` and
+`releases` give byte-identical stdout and files with the default batch size and with a `--batch-bytes` that cuts the tree into
+dozens of batches (counters and walk order carried across batches, one context per command); and every command prints its empty
+result for a tree with no selected file.  Revision pairs: `history` and `diff` with every output and rename pairing give the same
+bytes whether their pairs go in one batch, a few or one per batch, and a history of more than 65 535 commits gives the same
+assertion churn when its batches are cut at the group limit as when they are cut every few hundred commits."""
+import csv
 import os
+import shutil
 import subprocess
+import tarfile
 
 import pytest
 
 import corpus_util as cu
+import test_history_cases
+import test_history_renames
+from test_history import git
 
 pytestmark = pytest.mark.gpu
+needs_git = pytest.mark.skipif(shutil.which("git") is None, reason="needs the git command line")
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 CLI = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tosem-2021-replication_b200", "tosemscan", "tosem-scan")
@@ -46,13 +55,15 @@ def run(args, outs):
     return p.stdout, p.stderr.decode().strip().split("\n")[-1], [open(o, "rb").read() for o in outs]
 
 
-def default_and_small(tmp_path, cmd, args, flags):
+def default_and_small(tmp_path, cmd, args, flags, sizes=(SMALL,)):
+    """One run with the default batch size and one per `--batch-bytes` of `sizes`: all give the same bytes."""
     got = []
-    for tag, extra in (("default", []), ("small", ["--batch-bytes", SMALL])):
+    for tag, extra in [("default", [])] + [("b%s" % s, ["--batch-bytes", s]) for s in sizes]:
         outs = [str(tmp_path / ("%s_%s.csv" % (tag, f.lstrip("-")))) for f in flags]
         opts = [x for f, o in zip(flags, outs) for x in (f, o)]
         got.append(run([cmd] + args + opts + extra, outs))
-    assert got[0] == got[1]
+    for g in got[1:]:
+        assert g == got[0]
     return got[0]
 
 
@@ -113,3 +124,69 @@ def test_empty_selection(tmp_path, empty):
     assert stdout == (b"repository,files,lines,duplicated_lines,assertion_lines,duplicated_assertion_lines,classes\r\n"
                       b"proj,0,0,0,0,0,0\r\n<all>,0,0,0,0,0,0\r\n")
     assert files == [b"class,repository,fileName,first_line,last_line\r\n"]
+
+
+PAIR_FLAGS = ["--out", "--asserts", "--assert-churn", "--cases"]
+PAIR_SIZES = ("1", "3000")                                 # one pair per batch; a few pairs per batch
+
+
+@pytest.fixture(scope="module", params=["renames", "cases"])
+def history_repo(request, tmp_path_factory):
+    """The repositories of test_history_renames.py (pure, edited and base-name moves) and test_history_cases.py (cases added,
+    deleted, edited and moved)."""
+    build = {"renames": test_history_renames.build, "cases": test_history_cases.build}[request.param]
+    return build(tmp_path_factory.mktemp(request.param))
+
+
+@needs_git
+def test_history_pair_batches(tmp_path, history_repo):
+    stdout, last, files = default_and_small(tmp_path, "history", [str(history_repo), "--find-renames", "50"], PAIR_FLAGS, PAIR_SIZES)
+    assert stdout.count(b"\r\n") == 1 + len(git(history_repo, "rev-list", "HEAD").split())
+    assert last.startswith("tosem-scan: ") and "rename(s) found at 50%" in last
+    assert all(f.count(b"\r\n") > 1 for f in files[:3])     # (the renames repository has no test case headers)
+
+
+@needs_git
+def test_diff_pair_batches(tmp_path, history_repo):
+    """`diff` of `git archive` checkouts of the first and the last commit."""
+    revs = git(history_repo, "rev-list", "--first-parent", "--reverse", "HEAD").split()
+    roots = []
+    for rev in (revs[0], revs[-1]):
+        d = tmp_path / ("tree_" + rev[:8])
+        os.makedirs(d)
+        tar = tmp_path / ("t_%s.tar" % rev[:8])
+        tar.write_bytes(git(history_repo, "archive", "--format=tar", rev, text=False))
+        with tarfile.open(tar) as t:
+            t.extractall(d, filter="data")
+        roots.append(str(d))
+    stdout, last, files = default_and_small(tmp_path, "diff", roots + ["--find-renames", "50"], PAIR_FLAGS, PAIR_SIZES)
+    assert stdout.startswith(b"cloc,added,removed\r\n") and "rename(s) found (" in last
+    assert all(f.count(b"\r\n") > 1 for f in files[:3])
+
+
+@needs_git
+def test_history_past_the_group_limit(tmp_path):
+    """65 540 commits, each rewriting the assertion line of one test file: the default batch size cuts the history at 65 535
+    commits (a batch's assertion tables have u16 groups), --batch-bytes 100000 every 300 or so.  The churn must not depend on the
+    cuts and must have the row of every commit."""
+    n = 65540
+    repo = tmp_path / "repo"
+    os.makedirs(repo)
+    git(repo, "init", "-q", ".")
+    stream = []
+    for i in range(n):
+        data = b"def test_a(self):\n    self.assertEqual(x, %d)\n" % i
+        stream.append(b"commit refs/heads/t\ncommitter c <c@example.org> %d +0000\ndata 1\nc\nM 100644 inline tests/test_a.py\n"
+                      b"data %d\n%s\n" % (1600000000 + i, len(data), data))
+    subprocess.run(["git", "-C", str(repo), "fast-import", "--quiet"], input=b"".join(stream), capture_output=True, check=True,
+                   env=dict(os.environ, GIT_CONFIG_NOSYSTEM="1", HOME=str(repo)))
+    git(repo, "symbolic-ref", "HEAD", "refs/heads/t")
+    got = []
+    for extra in ([], ["--batch-bytes", "100000"]):
+        churn, out = tmp_path / ("churn%d.csv" % len(extra)), tmp_path / ("out%d.csv" % len(extra))
+        got.append(run(["history", str(repo), "--assert-churn", str(churn), "--out", str(out)] + extra, [churn, out]))
+    assert got[0] == got[1]
+    stdout, _, (churn, _) = got[0]
+    commits = [row.split(",")[0] for row in stdout.decode().split("\r\n")[1:] if row]
+    assert len(commits) == n
+    assert [r[0] for r in csv.reader(churn.decode().split("\r\n")[1:]) if r] == commits   # one category per commit

@@ -17,15 +17,16 @@
 //
 //   tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N]
 //   tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]
-//   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--find-renames N]
+//   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--find-renames N] [--batch-bytes N]
 //   tosem-scan body   <project-root>... [--batch-bytes N] [--out F]
 //   tosem-scan releases <snapshot-root>=<tag>... | --git <repository> [<revision>...]   [--batch-bytes N] [--out F]
 //   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F] [--cases F]
-//                      [--find-renames N]
+//                      [--find-renames N] [--batch-bytes N]
 //   tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]
 //   tosem-scan clones <project-root>... | --git <repository> [--rev R]   [--min-lines N] [--all-files] [--out F]
 // Every command that scans files does it with scan_batches: batches of at most --batch-bytes of arena (clones: all files in one),
-// one context, the next batch read while the current one is scanned.
+// one context, the next batch read while the current one is scanned.  Every command that diffs revision pairs (diff, history,
+// blame) does it with pair_batches: batches of at most --batch-bytes per side, one context shared with the rename pairing.
 #include <algorithm>
 #include <atomic>
 #include <cctype>
@@ -199,6 +200,13 @@ static std::string method_string(int ext, const uint8_t* line, uint32_t len) {  
 
 // ---------------------------------------------------------------------------------- scan
 struct HostFree { void operator()(uint8_t* p) const { tsm_host_free(p); } };
+struct CtxFree { void operator()(tsm_ctx* c) const { tsm_destroy(c); } };
+// A context at the smallest size, for calls that grow it to what they need (reduce, rename pairing, the diffs of revision pairs).
+static std::unique_ptr<tsm_ctx, CtxFree> small_context() {
+  tsm_ctx* ctx = nullptr;
+  ck(tsm_create(&ctx, 0, 1 << 20, 16, 1, 0), "tsm_create");
+  return std::unique_ptr<tsm_ctx, CtxFree>(ctx);
+}
 
 struct Batch {                                             // one packed arena of files; move-only, it owns its pinned arena
   std::vector<uint32_t> idx;                               // indices into the walk's file list, ascending
@@ -286,8 +294,8 @@ static std::vector<uint32_t> all_of(const std::vector<FileEntry>& files) {
   std::iota(v.begin(), v.end(), 0u);
   return v;
 }
-// Batches of every command but `scan`: --batch-bytes defaults to kBatch (bytes per side of a diff or tsm_similarity call, arena
-// bytes of a scan), and a scan batch holds at most kBatchFiles files.
+// Batches of every command but `scan`: --batch-bytes defaults to kBatch (bytes per side of a diff or of the tsm_similarity call
+// of rename pairing, arena bytes of a scan), and a scan batch holds at most kBatchFiles files.
 static const int64_t kBatch = 512ll << 20;
 static const size_t kBatchFiles = 1u << 19;
 
@@ -726,11 +734,9 @@ static int cmd_reduce(const std::string& path, const std::string& strategy_path,
       }
   }
   const int n_rows = (int)repo.size(), n_repos = (int)repos.size(), n_cases = (int)cid.size();
-  tsm_ctx* ctx = nullptr;
-  ck(tsm_create(&ctx, 0, 1 << 20, 16, 1, 0), "tsm_create");
   std::vector<int64_t> out((size_t)nF * n_repos), cpr((size_t)n_repos);
-  ck(tsm_reduce(ctx, flags.data(), repo.data(), cas.data(), n_rows, nF, n_repos, n_cases, out.data(), cpr.data(), nullptr), "tsm_reduce");
-  tsm_destroy(ctx);
+  ck(tsm_reduce(small_context().get(), flags.data(), repo.data(), cas.data(), n_rows, nF, n_repos, n_cases, out.data(), cpr.data(), nullptr),
+     "tsm_reduce");
   int64_t all_cases = 0; for (int64_t c : cpr) all_cases += c;
   // row order of the property and correlate tables: the shipped one when all nine repositories are present, else that of `repos`
   std::vector<std::string> order = {"auto_sklearn", "google_automl", "tpot", "autokeras", "Nupic", "Apollo", "nni", "Ray", "DeepSpeech2"};
@@ -1303,9 +1309,9 @@ struct ChangeTotals {
 static bool binary(const std::vector<uint8_t>& v) { return !v.empty() && memchr(v.data(), 0, std::min<size_t>(v.size(), 8000)) != nullptr; }
 
 // --find-renames: the deleted and the added files of a step (binary ones left out) form a group; groups are paired together
-// until a side holds kBatch bytes, then every pair's two changes become one (old side of the deleted file, new side of the
-// added one) at the added file's place.
-static void pair_renames(tsm_ctx* ctx, std::vector<Change>& changes, const Loader& load, int pct, ChangeTotals& t) {
+// until a side holds batch_bytes bytes (a group is never split, so the pairs do not depend on where that is), then every pair's
+// two changes become one (old side of the deleted file, new side of the added one) at the added file's place.
+static void pair_renames(tsm_ctx* ctx, std::vector<Change>& changes, const Loader& load, int pct, int64_t batch_bytes, ChangeTotals& t) {
   struct Move { size_t del, add; int similarity; };
   std::vector<Move> moves;
   std::vector<RenameGroup> groups;
@@ -1340,7 +1346,7 @@ static void pair_renames(tsm_ctx* ctx, std::vector<Change>& changes, const Loade
     }
     if (G.del.empty() || G.add.empty()) continue;
     groups.push_back(std::move(G)); at_del.push_back(gd); at_add.push_back(ga);
-    if (bytes_d >= kBatch || bytes_a >= kBatch) flush();
+    if (bytes_d >= batch_bytes || bytes_a >= batch_bytes) flush();
   }
   if (!groups.empty()) flush();
   std::vector<char> drop(changes.size(), 0);
@@ -1355,155 +1361,156 @@ static void pair_renames(tsm_ctx* ctx, std::vector<Change>& changes, const Loade
   changes.swap(kept);
 }
 
-// What runs instead of tsm_diff_pairs_detail on a batch (blame): the changes [r0, r1), of which idx were packed (the others are
-// binary and skipped), the two sides, and added / removed / detail to fill.
-using BatchFn = std::function<void(tsm_ctx*, size_t r0, size_t r1, const std::vector<size_t>& idx, const tsm_corpus&, const tsm_corpus&,
-                                   int64_t*, int64_t*, tsm_diff_detail*)>;
+// One batch of revision pairs: the changes [r0, r1), of which those at `idx` (ascending) are packed into the two sides, pair i
+// being change idx[i]; the others are binary on a side and skipped.  With grouped steps, group g of both sides is step
+// group_step[g]; else every pair is in group 0.
+struct PairBatch {
+  size_t r0, r1;
+  std::vector<size_t> idx;
+  Batch olds, news;
+  std::vector<size_t> group_step;
+  tsm_ctx* ctx;
+  int32_t n_groups() const { return group_step.empty() ? 1 : (int32_t)group_step.size(); }
+};
 
-// The diff of an ordered list of changes of `n_steps` steps, after --find-renames pairing when rename_pct >= 0: binary files
-// skipped, batches of at most batch_bytes bytes per side (and 65 535 steps, a step being one group of the assertion tables),
-// one tsm_diff_pairs_detail or diff_asserts call per batch (or `pairs`, when given).  Every row starts with the `lead(step)`
-// cells named `lead_head`; the --assert-churn rows with the first `churn_lead` of them.  --out has a row for every diffed change
-// when `zero_rows`, else only for those that change a line or pair a rename.
-static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, const Loader& load, int rename_pct, bool zero_rows,
-                                 const std::vector<std::string>& lead_head, size_t churn_lead,
-                                 const std::function<std::vector<std::string>(size_t)>& lead, const std::string& out_path,
-                                 const std::string& asserts_path, const std::string& churn_path, const std::string& cases_path,
-                                 int64_t batch_bytes = kBatch, const BatchFn* pairs = nullptr) {
-  ChangeTotals t(n_steps);
-  tsm_ctx* ctx = nullptr;
-  ck(tsm_create(&ctx, 0, 1 << 20, 16, 1, 0), "tsm_create");
-  if (rename_pct >= 0) pair_renames(ctx, changes, load, rename_pct, t);
-  std::ofstream os, as, cs;
-  if (!out_path.empty()) {
-    os.open(out_path, std::ios::binary);
-    std::vector<std::string> head = lead_head;
-    head.insert(head.end(), {"fileName", "cloc", "added", "removed", "hunks_add", "hunks_del", "hunks_mod", "added_assert", "removed_assert"});
-    if (rename_pct >= 0) head.insert(head.end(), {"oldFileName", "similarity"});
-    csv_row(os, head);
-  }
-  if (!asserts_path.empty()) {
-    as.open(asserts_path, std::ios::binary);
-    std::vector<std::string> head = lead_head;
-    head.insert(head.end(), {"fileName", "change", "line", "statement", "category"});
-    csv_row(as, head);
-  }
-  if (!cases_path.empty()) {
-    cs.open(cases_path, std::ios::binary);
-    std::vector<std::string> head = lead_head;
-    head.insert(head.end(), {"fileName", "case", "change", "line", "oldLine", "lines", "oldLines", "asserts", "oldAsserts", "insertedLines",
-                             "deletedLines", "insertedAsserts", "deletedAsserts"});
-    if (rename_pct >= 0) head.push_back("oldFileName");
-    csv_row(cs, head);
-  }
-  const bool want_asserts = !asserts_path.empty() || !churn_path.empty();
-  std::map<size_t, std::vector<int64_t>> churn;            // per step with changed assertion lines: its [K] added and removed rows
+// The changes cut in order into batches, each handed to `fn`, one whose changes are all binary too (with an empty idx).  Both
+// sides are loaded until one holds batch_bytes bytes; with group_steps (the assertion tables: a group is a u16) a batch also
+// holds at most 65 535 steps, binary-only steps counted.  t.binaries and t.diffed count the skipped and the packed changes.
+static void pair_batches(tsm_ctx* ctx, const std::vector<Change>& changes, const Loader& load, int64_t batch_bytes, bool group_steps,
+                         ChangeTotals& t, const std::function<void(const PairBatch&)>& fn) {
   for (size_t r0 = 0, r1 = 0; r0 < changes.size(); r0 = r1) {
-    // load both sides until a side of the batch is full
+    PairBatch b{r0, r0, {}, {}, {}, {}, ctx};
     std::vector<std::vector<uint8_t>> blobs[2];            // old, new
-    std::vector<size_t> idx;
     int64_t so = 0, sn = 0;
     size_t steps = 0;
     for (r1 = r0; r1 < changes.size() && so < batch_bytes && sn < batch_bytes; ++r1) {
       const Change& c = changes[r1];
-      if (want_asserts && (r1 == r0 || c.step != changes[r1 - 1].step) && ++steps > 65535) break;
+      if (group_steps && (r1 == r0 || c.step != changes[r1 - 1].step) && ++steps > 65535) break;
       std::vector<uint8_t> x = c.o >= 0 ? load(c.o) : std::vector<uint8_t>(), y = c.n >= 0 ? load(c.n) : std::vector<uint8_t>();
       if (binary(x) || binary(y)) { ++t.binaries; continue; }
       if (x.size() > 0x7fff0000u || y.size() > 0x7fff0000u) die("blob too large: " + c.path);
       so += (int64_t)x.size() + 256; sn += (int64_t)y.size() + 256;
-      blobs[0].push_back(std::move(x)); blobs[1].push_back(std::move(y)); idx.push_back(r1);
+      blobs[0].push_back(std::move(x)); blobs[1].push_back(std::move(y)); b.idx.push_back(r1);
     }
-    const size_t n = idx.size();
-    if (!n && pairs) (*pairs)(ctx, r0, r1, idx, tsm_corpus{}, tsm_corpus{}, nullptr, nullptr, nullptr);
-    if (!n) continue;
+    b.r1 = r1;
     std::vector<const std::vector<uint8_t>*> sides[2];
     for (int s = 0; s < 2; ++s) for (const std::vector<uint8_t>& v : blobs[s]) sides[s].push_back(&v);
-    Batch A = pack(sides[0]), N = pack(sides[1]);
+    b.olds = pack(sides[0]); b.news = pack(sides[1]);
     // ext tags of both sides feed the assertion-line classification of the changed lines
-    std::vector<size_t> group_step;                        // group g of the batch = step group_step[g]
-    for (size_t i = 0; i < n; ++i) {
-      const Change& c = changes[idx[i]];
-      N.ext[i] = (uint8_t)ext_tag(c.path);
-      A.ext[i] = c.old_path.empty() ? N.ext[i] : (uint8_t)ext_tag(c.old_path);
-      if (!want_asserts) continue;
-      if (group_step.empty() || group_step.back() != c.step) group_step.push_back(c.step);
-      A.grp[i] = N.grp[i] = (uint16_t)(group_step.size() - 1);
+    for (size_t i = 0; i < b.idx.size(); ++i) {
+      const Change& c = changes[b.idx[i]];
+      b.news.ext[i] = (uint8_t)ext_tag(c.path);
+      b.olds.ext[i] = c.old_path.empty() ? b.news.ext[i] : (uint8_t)ext_tag(c.old_path);
+      if (!group_steps) continue;
+      if (b.group_step.empty() || b.group_step.back() != c.step) b.group_step.push_back(c.step);
+      b.olds.grp[i] = b.news.grp[i] = (uint16_t)(b.group_step.size() - 1);
     }
-    const int32_t n_groups = want_asserts ? (int32_t)group_step.size() : 1;
-    const tsm_corpus ca = A.corpus(n_groups), cn = N.corpus(n_groups);
-    std::vector<int64_t> added(n), removed(n);
-    std::vector<tsm_diff_detail> det(n);
-    ChangedAsserts chg;
-    CaseLists cases;
-    if (pairs) {
-      (*pairs)(ctx, r0, r1, idx, ca, cn, added.data(), removed.data(), det.data());
-    } else if (!want_asserts) {
-      if (cs.is_open()) diff_cases(ctx, ca, cn, added.data(), removed.data(), det.data(), cases);
-      else ck(tsm_diff_pairs_detail(ctx, &ca, &cn, added.data(), removed.data(), det.data(), nullptr), "tsm_diff_pairs_detail");
-    } else {
-      diff_asserts(ctx, ca, cn, added.data(), removed.data(), det.data(), chg);
-      for (size_t g = 0; g < group_step.size(); ++g) {     // a step's files may span two batches
-        const int64_t* ad = chg.added_counts.data() + g * TSM_NUM_CATEGORIES;
-        const int64_t* rm = chg.removed_counts.data() + g * TSM_NUM_CATEGORIES;
-        if (std::all_of(ad, ad + TSM_NUM_CATEGORIES, [](int64_t v) { return v == 0; }) &&
-            std::all_of(rm, rm + TSM_NUM_CATEGORIES, [](int64_t v) { return v == 0; })) continue;
-        std::vector<int64_t>& tab = churn[group_step[g]];
-        tab.resize(2 * TSM_NUM_CATEGORIES, 0);
-        for (int k = 0; k < TSM_NUM_CATEGORIES; ++k) { tab[(size_t)k] += ad[k]; tab[(size_t)(TSM_NUM_CATEGORIES + k)] += rm[k]; }
-      }
-      size_t ka = 0, kr = 0;
-      for (size_t i = 0; as.is_open() && i < n; ++i) {
-        const Change& c = changes[idx[i]];
-        const std::vector<std::string> l = lead(c.step);
-        assert_rows(as, l, c.old_path.empty() ? c.path : c.old_path, A.arena.get() + A.off[i], A.len[i], chg.rev, kr, (uint32_t)i, "-");
-        assert_rows(as, l, c.path, N.arena.get() + N.off[i], N.len[i], chg.aev, ka, (uint32_t)i, "+");
-      }
-      if (cs.is_open()) {                                  // a second call: the assertion tables and the cases are separate diffs
-        std::vector<int64_t> a2(n), r2(n);
-        diff_cases(ctx, ca, cn, a2.data(), r2.data(), nullptr, cases);
-      }
+    t.diffed += (int64_t)b.idx.size();
+    fn(b);
+  }
+}
+
+// What `diff` and `history` write.  Every row starts with the `lead(step)` cells named `lead_head`; the --assert-churn rows with
+// the first `churn_lead` of them.  --out has a row for every diffed change when `zero_rows`, else only for those that change a
+// line or pair a rename.  An empty path is an output not asked for; rename_pct -1 is no rename pairing.
+struct DiffOptions {
+  int rename_pct = -1;
+  int64_t batch_bytes = kBatch;
+  std::string out, asserts, churn, cases;
+  bool zero_rows = false;
+  std::vector<std::string> lead_head;
+  size_t churn_lead = 0;
+  std::function<std::vector<std::string>(size_t)> lead = [](size_t) { return std::vector<std::string>(); };
+};
+
+// The diff of one batch: per pair the lines added and removed and the detail; with `asserts` the changed assertion lines and
+// the [group][K] tables, with `cases` the case records.
+struct PairDiff { std::vector<int64_t> added, removed; std::vector<tsm_diff_detail> det; ChangedAsserts chg; CaseLists cases; };
+static PairDiff diff_batch(const PairBatch& b, bool asserts, bool cases) {
+  const size_t n = b.idx.size();
+  PairDiff d{std::vector<int64_t>(n), std::vector<int64_t>(n), std::vector<tsm_diff_detail>(n), {}, {}};
+  const tsm_corpus ca = b.olds.corpus(b.n_groups()), cn = b.news.corpus(b.n_groups());
+  if (asserts) diff_asserts(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.chg);
+  else if (cases) diff_cases(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.cases);
+  else ck(tsm_diff_pairs_detail(b.ctx, &ca, &cn, d.added.data(), d.removed.data(), d.det.data(), nullptr), "tsm_diff_pairs_detail");
+  if (asserts && cases) {                                  // a second call: the assertion tables and the cases are separate diffs
+    std::vector<int64_t> a2(n), r2(n);
+    diff_cases(b.ctx, ca, cn, a2.data(), r2.data(), nullptr, d.cases);
+  }
+  return d;
+}
+
+// The diff of an ordered list of changes of `n_steps` steps, after --find-renames pairing: one diff_batch per batch of
+// pair_batches, its steps grouped when the assertion tables are asked for, then the rows.
+static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, const Loader& load, const DiffOptions& o) {
+  ChangeTotals t(n_steps);
+  const bool renames = o.rename_pct >= 0;
+  const auto ctx = small_context();
+  if (renames) pair_renames(ctx.get(), changes, load, o.rename_pct, o.batch_bytes, t);
+  std::ofstream os, as, cs, ch;                            // --out, --asserts, --cases, --assert-churn
+  auto open = [&](std::ofstream& f, const std::string& path, size_t n_lead, std::vector<std::string> head) {
+    if (path.empty()) return;
+    f.open(path, std::ios::binary);
+    head.insert(head.begin(), o.lead_head.begin(), o.lead_head.begin() + (long)n_lead);
+    csv_row(f, head);
+  };
+  std::vector<std::string> out_head = {"fileName", "cloc", "added", "removed", "hunks_add", "hunks_del", "hunks_mod", "added_assert", "removed_assert"};
+  std::vector<std::string> case_head = {"fileName", "case", "change", "line", "oldLine", "lines", "oldLines", "asserts", "oldAsserts",
+                                        "insertedLines", "deletedLines", "insertedAsserts", "deletedAsserts"};
+  if (renames) out_head.insert(out_head.end(), {"oldFileName", "similarity"});
+  if (renames) case_head.push_back("oldFileName");
+  open(os, o.out, o.lead_head.size(), out_head);
+  open(as, o.asserts, o.lead_head.size(), {"fileName", "change", "line", "statement", "category"});
+  open(cs, o.cases, o.lead_head.size(), case_head);
+  open(ch, o.churn, o.churn_lead, {"category", "added", "removed"});
+  const bool want_asserts = !o.asserts.empty() || !o.churn.empty();
+  std::map<size_t, std::vector<int64_t>> churn;            // per step with changed assertion lines: its [K] added and removed rows
+  pair_batches(ctx.get(), changes, load, o.batch_bytes, want_asserts, t, [&](const PairBatch& b) {
+    const size_t n = b.idx.size();
+    if (!n) return;
+    const PairDiff d = diff_batch(b, want_asserts, cs.is_open());
+    for (size_t g = 0; ch.is_open() && g < b.group_step.size(); ++g) {   // a step's files may span two batches
+      const int64_t* ad = d.chg.added_counts.data() + g * TSM_NUM_CATEGORIES;
+      const int64_t* rm = d.chg.removed_counts.data() + g * TSM_NUM_CATEGORIES;
+      if (std::all_of(ad, ad + TSM_NUM_CATEGORIES, [](int64_t v) { return v == 0; }) &&
+          std::all_of(rm, rm + TSM_NUM_CATEGORIES, [](int64_t v) { return v == 0; })) continue;
+      std::vector<int64_t>& tab = churn[b.group_step[g]];
+      tab.resize(2 * TSM_NUM_CATEGORIES, 0);
+      for (int k = 0; k < TSM_NUM_CATEGORIES; ++k) { tab[(size_t)k] += ad[k]; tab[(size_t)(TSM_NUM_CATEGORIES + k)] += rm[k]; }
     }
-    for (size_t i = 0, ko = 0, kn = 0; cs.is_open() && i < n; ++i) {
-      const Change& c = changes[idx[i]];
-      const size_t o0 = ko, n0 = kn;
-      while (ko < cases.olds.size() && cases.olds[ko].pair == (int32_t)i) ++ko;
-      while (kn < cases.news.size() && cases.news[kn].pair == (int32_t)i) ++kn;
-      if (ko == o0 && kn == n0) continue;
+    for (size_t i = 0, ka = 0, kr = 0, ko = 0, kn = 0; i < n; ++i) {   // ka, kr, ko, kn: pair i's first event and case of each side
+      const Change& c = changes[b.idx[i]];
       const std::string& old_path = c.old_path.empty() ? c.path : c.old_path;
-      case_rows(cs, lead(c.step), CaseSide{A.arena.get() + A.off[i], A.len[i], A.ext[i], &old_path},
-                CaseSide{N.arena.get() + N.off[i], N.len[i], N.ext[i], &c.path}, rename_pct >= 0 ? &c.old_path : nullptr,
-                cases.olds.data() + o0, ko - o0, cases.news.data() + n0, kn - n0, o0);
-    }
-    for (size_t i = 0; i < n; ++i) {
-      const Change& c = changes[idx[i]];
-      t.added[c.step] += added[i]; t.removed[c.step] += removed[i]; t.files[c.step]++;
-      if (!os.is_open() || !(zero_rows || added[i] || removed[i] || c.similarity >= 0)) continue;
-      std::vector<std::string> row = lead(c.step);
-      row.insert(row.end(), {c.path, std::to_string(added[i] + removed[i]), std::to_string(added[i]), std::to_string(removed[i]),
-                             std::to_string(det[i].hunks_add), std::to_string(det[i].hunks_del), std::to_string(det[i].hunks_mod),
-                             std::to_string(det[i].added_assert), std::to_string(det[i].removed_assert)});
-      if (rename_pct >= 0) row.insert(row.end(), {c.old_path, c.similarity >= 0 ? std::to_string(c.similarity) : ""});
+      const CaseSide olds{b.olds.arena.get() + b.olds.off[i], b.olds.len[i], b.olds.ext[i], &old_path};
+      const CaseSide news{b.news.arena.get() + b.news.off[i], b.news.len[i], b.news.ext[i], &c.path};
+      if (as.is_open()) {
+        assert_rows(as, o.lead(c.step), old_path, olds.base, olds.size, d.chg.rev, kr, (uint32_t)i, "-");
+        assert_rows(as, o.lead(c.step), c.path, news.base, news.size, d.chg.aev, ka, (uint32_t)i, "+");
+      }
+      const size_t o0 = ko, n0 = kn;
+      while (ko < d.cases.olds.size() && d.cases.olds[ko].pair == (int32_t)i) ++ko;
+      while (kn < d.cases.news.size() && d.cases.news[kn].pair == (int32_t)i) ++kn;
+      if (ko > o0 || kn > n0)
+        case_rows(cs, o.lead(c.step), olds, news, renames ? &c.old_path : nullptr, d.cases.olds.data() + o0, ko - o0, d.cases.news.data() + n0,
+                  kn - n0, o0);
+      t.added[c.step] += d.added[i]; t.removed[c.step] += d.removed[i]; t.files[c.step]++;
+      if (!os.is_open() || !(o.zero_rows || d.added[i] || d.removed[i] || c.similarity >= 0)) continue;
+      std::vector<std::string> row = o.lead(c.step);
+      row.insert(row.end(), {c.path, std::to_string(d.added[i] + d.removed[i]), std::to_string(d.added[i]), std::to_string(d.removed[i]),
+                             std::to_string(d.det[i].hunks_add), std::to_string(d.det[i].hunks_del), std::to_string(d.det[i].hunks_mod),
+                             std::to_string(d.det[i].added_assert), std::to_string(d.det[i].removed_assert)});
+      if (renames) row.insert(row.end(), {c.old_path, c.similarity >= 0 ? std::to_string(c.similarity) : ""});
       csv_row(os, row);
     }
-    t.diffed += (int64_t)n;
-  }
-  tsm_destroy(ctx);
-  if (!churn_path.empty()) {
-    std::ofstream cs(churn_path, std::ios::binary);
-    std::vector<std::string> head(lead_head.begin(), lead_head.begin() + (long)churn_lead);
-    head.insert(head.end(), {"category", "added", "removed"});
-    csv_row(cs, head);
-    for (const auto& kv : churn) {
-      std::vector<std::string> l = lead(kv.first);
-      l.resize(churn_lead);
-      churn_rows(cs, l, kv.second.data(), kv.second.data() + TSM_NUM_CATEGORIES);
-    }
+  });
+  for (const auto& kv : churn) {
+    const std::vector<std::string> l = o.lead(kv.first);
+    churn_rows(ch, {l.begin(), l.begin() + (long)o.churn_lead}, kv.second.data(), kv.second.data() + TSM_NUM_CATEGORIES);
   }
   return t;
 }
 
-static int cmd_diff(const std::string& old_root, const std::string& new_root, const std::string& out_path,
-                    const std::string& asserts_path, const std::string& churn_path, const std::string& cases_path, int rename_pct) {
+static int cmd_diff(const std::string& old_root, const std::string& new_root, const DiffOptions& o) {
   std::vector<FileEntry> a, b;
   walk(old_root, 0, true, a);
   walk(new_root, 0, true, b);
@@ -1521,10 +1528,9 @@ static int cmd_diff(const std::string& old_root, const std::string& new_root, co
     if (!read_file(f.abs, v.data(), f.size)) die("short read: " + f.abs);
     return v;
   };
-  const ChangeTotals t = diff_changes(changes, 1, load, rename_pct, false, {}, 0, [](size_t) { return std::vector<std::string>(); },
-                                      out_path, asserts_path, churn_path, cases_path);
+  const ChangeTotals t = diff_changes(changes, 1, load, o);
   if (t.binaries) fprintf(stderr, "tosem-scan: %lld binary file(s) skipped\n", (long long)t.binaries);
-  if (rename_pct >= 0)
+  if (o.rename_pct >= 0)
     fprintf(stderr, "tosem-scan: %lld rename(s) found (%lld exact, %lld inexact)\n", (long long)t.renames, (long long)t.renames_exact,
             (long long)(t.renames - t.renames_exact));
   printf("cloc,added,removed\r\n%lld,%lld,%lld\r\n", (long long)(t.added[0] + t.removed[0]), (long long)t.added[0], (long long)t.removed[0]);
@@ -1567,83 +1573,84 @@ static void tree_diff(gitstore::Store& gs, const gitstore::Oid* a, const gitstor
   }
 }
 
-// The first-parent chain of `rev` (at most max_commits commits; all when 0), oldest first, and the changed selected files of
-// every commit against its parent, as changes of the commit's place in the chain; `objs` names the blobs of the changes.
+// The first-parent chain of `rev` in the repository at `repo` (at most max_commits commits; all when 0), oldest first, and the
+// changed selected files of every commit against its parent, as changes of the commit's place in the chain; `load` reads the
+// blobs of the changes, which `objs` names.
 struct Step { gitstore::Oid id; gitstore::Commit c; };
-static void history_walk(gitstore::Store& gs, const std::string& rev, int64_t max_commits, bool all_files, std::vector<Step>& chain,
-                         std::vector<gitstore::Oid>& objs, std::vector<Change>& changes) {
-  gitstore::Oid head;
-  if (!gs.resolve(rev, head)) die("cannot resolve revision " + rev);
-  for (gitstore::Oid id = head; max_commits <= 0 || (int64_t)chain.size() < max_commits;) {
-    Step st{id, {}};
-    if (!gs.commit(id, st.c)) die("unreadable commit " + id.hex());
-    chain.push_back(st);
-    if (st.c.parents.empty()) break;
-    id = st.c.parents[0];
-  }
-  std::reverse(chain.begin(), chain.end());                 // oldest first
-  for (size_t i = 0; i < chain.size(); ++i) {
-    gitstore::Commit parent;
-    const bool has_parent = !chain[i].c.parents.empty();
-    if (has_parent && !gs.commit(chain[i].c.parents[0], parent)) die("unreadable commit " + chain[i].c.parents[0].hex());
-    if (has_parent && parent.tree == chain[i].c.tree) continue;
-    tree_diff(gs, has_parent ? &parent.tree : nullptr, &chain[i].c.tree, "", all_files, i, objs, changes);
-  }
-}
-
-// --dry-run: no GPU - the rows carry the object names, sizes and an FNV-1a checksum of both blobs instead of the counts
-// (what the CPU tests compare with `git diff-tree` / `git cat-file`).
-static int cmd_history(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files, const std::string& out_path,
-                       bool dry_run, const std::string& asserts_path, const std::string& churn_path, const std::string& cases_path,
-                       int rename_pct) {
+struct History {
   gitstore::Store gs;
-  std::string err;
-  if (!gs.open(repo, err)) die(err);
   std::vector<Step> chain;
   std::vector<gitstore::Oid> objs;
   std::vector<Change> changes;
-  history_walk(gs, rev, max_commits, all_files, chain, objs, changes);
-  auto load = [&](int64_t s) {
+  const Loader load = [this](int64_t s) {
     gitstore::Object x;
     if (!gs.read(objs[(size_t)s], x) || x.type != gitstore::OBJ_BLOB) die("unreadable blob " + objs[(size_t)s].hex());
     return std::move(x.data);
   };
-  auto lead = [&](size_t step) {
-    const Step& st = chain[step];
+  History(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files) {
+    std::string err;
+    if (!gs.open(repo, err)) die(err);
+    gitstore::Oid head;
+    if (!gs.resolve(rev, head)) die("cannot resolve revision " + rev);
+    for (gitstore::Oid id = head; max_commits <= 0 || (int64_t)chain.size() < max_commits;) {
+      Step st{id, {}};
+      if (!gs.commit(id, st.c)) die("unreadable commit " + id.hex());
+      chain.push_back(st);
+      if (st.c.parents.empty()) break;
+      id = st.c.parents[0];
+    }
+    std::reverse(chain.begin(), chain.end());               // oldest first
+    for (size_t i = 0; i < chain.size(); ++i) {
+      gitstore::Commit parent;
+      const bool has_parent = !chain[i].c.parents.empty();
+      if (has_parent && !gs.commit(chain[i].c.parents[0], parent)) die("unreadable commit " + chain[i].c.parents[0].hex());
+      if (has_parent && parent.tree == chain[i].c.tree) continue;
+      tree_diff(gs, has_parent ? &parent.tree : nullptr, &chain[i].c.tree, "", all_files, i, objs, changes);
+    }
+  }
+};
+
+// --dry-run: no GPU - the rows carry the object names, sizes and an FNV-1a checksum of both blobs instead of the counts
+// (what the CPU tests compare with `git diff-tree` / `git cat-file`).
+static int cmd_history(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files, bool dry_run, DiffOptions o) {
+  History h(repo, rev, max_commits, all_files);
+  o.lead = [&](size_t step) {
+    const Step& st = h.chain[step];
     return std::vector<std::string>{st.id.hex(), st.c.parents.empty() ? "" : st.c.parents[0].hex(), std::to_string(st.c.time)};
   };
-  ChangeTotals t(chain.size());
+  ChangeTotals t(h.chain.size());
   if (dry_run) {
     std::ofstream os;
-    if (!out_path.empty()) {
-      os.open(out_path, std::ios::binary);
+    if (!o.out.empty()) {
+      os.open(o.out, std::ios::binary);
       csv_row(os, {"commit", "parent", "time", "fileName", "old_blob", "new_blob", "old_size", "new_size", "old_fnv", "new_fnv"});
     }
     auto fnv = [](const std::vector<uint8_t>& v) { uint64_t h = 0xcbf29ce484222325ull; for (uint8_t b : v) h = (h ^ b) * 0x100000001b3ull; char buf[24]; snprintf(buf, sizeof buf, "%016llx", (unsigned long long)h); return std::string(buf); };
-    for (const Change& c : changes) {
-      const std::vector<uint8_t> x = c.o >= 0 ? load(c.o) : std::vector<uint8_t>(), y = c.n >= 0 ? load(c.n) : std::vector<uint8_t>();
+    for (const Change& c : h.changes) {
+      const std::vector<uint8_t> x = c.o >= 0 ? h.load(c.o) : std::vector<uint8_t>(), y = c.n >= 0 ? h.load(c.n) : std::vector<uint8_t>();
       if (os.is_open()) {
-        std::vector<std::string> row = lead(c.step);
-        row.insert(row.end(), {c.path, c.o >= 0 ? objs[(size_t)c.o].hex() : "", c.n >= 0 ? objs[(size_t)c.n].hex() : "",
+        std::vector<std::string> row = o.lead(c.step);
+        row.insert(row.end(), {c.path, c.o >= 0 ? h.objs[(size_t)c.o].hex() : "", c.n >= 0 ? h.objs[(size_t)c.n].hex() : "",
                                std::to_string(x.size()), std::to_string(y.size()), fnv(x), fnv(y)});
         csv_row(os, row);
       }
       t.files[c.step]++;
     }
   } else {
-    t = diff_changes(changes, chain.size(), load, rename_pct, true, {"commit", "parent", "time"}, 1, lead, out_path, asserts_path, churn_path, cases_path);
+    o.zero_rows = true; o.lead_head = {"commit", "parent", "time"}; o.churn_lead = 1;
+    t = diff_changes(h.changes, h.chain.size(), h.load, o);
   }
   printf("commit,files,cloc,added,removed\r\n");
   int64_t ta = 0, tr = 0;
-  for (size_t i = 0; i < chain.size(); ++i) {
+  for (size_t i = 0; i < h.chain.size(); ++i) {
     ta += t.added[i]; tr += t.removed[i];
-    printf("%s,%lld,%lld,%lld,%lld\r\n", chain[i].id.hex().c_str(), (long long)t.files[i], (long long)(t.added[i] + t.removed[i]),
+    printf("%s,%lld,%lld,%lld,%lld\r\n", h.chain[i].id.hex().c_str(), (long long)t.files[i], (long long)(t.added[i] + t.removed[i]),
            (long long)t.added[i], (long long)t.removed[i]);
   }
   fprintf(stderr, "tosem-scan: history of %s: %zu commits, %lld changed files diffed on the GPU, %lld binary skipped, cloc %lld (+%lld -%lld)\n",
-          rev.c_str(), chain.size(), (long long)t.diffed, (long long)t.binaries, (long long)(ta + tr), (long long)ta, (long long)tr);
-  if (rename_pct >= 0)
-    fprintf(stderr, "tosem-scan: %lld rename(s) found at %d%% (%lld exact, %lld inexact)\n", (long long)t.renames, rename_pct,
+          rev.c_str(), h.chain.size(), (long long)t.diffed, (long long)t.binaries, (long long)(ta + tr), (long long)ta, (long long)tr);
+  if (o.rename_pct >= 0)
+    fprintf(stderr, "tosem-scan: %lld rename(s) found at %d%% (%lld exact, %lld inexact)\n", (long long)t.renames, o.rename_pct,
             (long long)t.renames_exact, (long long)(t.renames - t.renames_exact));
   return 0;
 }
@@ -1665,21 +1672,11 @@ struct PathState { std::vector<tsm_origin> org; int32_t owner = -1; int64_t obj 
 
 static int cmd_blame(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files, int rename_pct,
                      int64_t batch_bytes, const std::string& out_path, const std::string& asserts_path) {
-  gitstore::Store gs;
-  std::string err;
-  if (!gs.open(repo, err)) die(err);
-  std::vector<Step> chain;
-  std::vector<gitstore::Oid> objs;
-  std::vector<Change> changes;
-  history_walk(gs, rev, max_commits, all_files, chain, objs, changes);
+  History h(repo, rev, max_commits, all_files);
+  const std::vector<Step>& chain = h.chain;
   const bool cut = !chain.empty() && !chain[0].c.parents.empty();          // the window does not reach the root
   Step p0{};
-  if (cut) { p0.id = chain[0].c.parents[0]; if (!gs.commit(p0.id, p0.c)) die("unreadable commit " + p0.id.hex()); }
-  auto load = [&](int64_t s) {
-    gitstore::Object x;
-    if (!gs.read(objs[(size_t)s], x) || x.type != gitstore::OBJ_BLOB) die("unreadable blob " + objs[(size_t)s].hex());
-    return std::move(x.data);
-  };
+  if (cut) { p0.id = chain[0].c.parents[0]; if (!h.gs.commit(p0.id, p0.c)) die("unreadable commit " + p0.id.hex()); }
   struct Owner { int64_t step; std::string path; };
   std::vector<Owner> owners;
   std::map<std::pair<int64_t, std::string>, int32_t> owner_id;
@@ -1691,25 +1688,26 @@ static int cmd_blame(const std::string& repo, const std::string& rev, int64_t ma
   };
   auto lazy = [&](const PathState& st, const std::vector<uint8_t>* bytes) {   // the origins of a lazy state
     std::vector<tsm_origin> v;
-    const int64_t n = count_lines(bytes ? *bytes : load(st.obj));
+    const int64_t n = count_lines(bytes ? *bytes : h.load(st.obj));
     for (int64_t j = 0; j < n; ++j) v.push_back({st.owner, (int32_t)(j + 1)});
     return v;
   };
   std::map<std::string, PathState> live;                   // host state between batches
-  int64_t blamed_pairs = 0;
-  BatchFn run = [&](tsm_ctx* ctx, size_t r0, size_t r1, const std::vector<size_t>& idx, const tsm_corpus& ca, const tsm_corpus& cn,
-                    int64_t* added, int64_t* removed, tsm_diff_detail* det) {
+  ChangeTotals t(chain.size());
+  auto ctx = small_context();
+  if (rename_pct >= 0) pair_renames(ctx.get(), h.changes, h.load, rename_pct, batch_bytes, t);
+  pair_batches(ctx.get(), h.changes, h.load, batch_bytes, false, t, [&](const PairBatch& b) {
     // the batch's view of every path it touches: the pair that last wrote it, a lazy state (binary change) or gone
     struct View { int kind; size_t pair; PathState st; };   // kind 0 pair, 1 state, 2 gone
     std::map<std::string, View> view;
-    const size_t n = idx.size();
+    const size_t n = b.idx.size();
     std::vector<int32_t> prev(n, -1), label(n);
     std::vector<int64_t> in_base(n + 1, 0);
     std::vector<tsm_origin> origin_in;
-    for (size_t r = r0, i = 0; r < r1; ++r) {
-      const Change& c = changes[r];
+    for (size_t r = b.r0, i = 0; r < b.r1; ++r) {
+      const Change& c = h.changes[r];
       const std::string& src = c.old_path.empty() ? c.path : c.old_path;
-      if (i < n && idx[i] == r) {
+      if (i < n && b.idx[i] == r) {
         if (c.o >= 0) {
           auto v = view.find(src);
           if (v != view.end() && v->second.kind == 0) prev[i] = (int32_t)v->second.pair;
@@ -1719,8 +1717,8 @@ static int cmd_blame(const std::string& repo, const std::string& rev, int64_t ma
             else if (live.count(src)) st = live[src];
             else if (cut) st.owner = owner(-1, src), st.obj = c.o;          // unchanged since P0: a boundary line
             else die("no origins for " + src);
-            std::vector<tsm_origin> h = st.org.empty() && st.obj >= 0 ? lazy(st, nullptr) : st.org;
-            origin_in.insert(origin_in.end(), h.begin(), h.end());
+            std::vector<tsm_origin> head = st.org.empty() && st.obj >= 0 ? lazy(st, nullptr) : st.org;
+            origin_in.insert(origin_in.end(), head.begin(), head.end());
           }
         }
         in_base[i + 1] = (int64_t)origin_in.size();
@@ -1732,23 +1730,25 @@ static int cmd_blame(const std::string& repo, const std::string& rev, int64_t ma
         if (src != c.path) view[src] = View{2, 0, {}};
         PathState st;
         st.owner = owner((int64_t)c.step, c.path); st.obj = c.n;
-        view[c.path] = c.n >= 0 && !binary(load(c.n)) ? View{1, 0, st} : View{2, 0, {}};
+        view[c.path] = c.n >= 0 && !binary(h.load(c.n)) ? View{1, 0, st} : View{2, 0, {}};
       }
     }
     std::vector<tsm_origin> out;
     std::vector<int64_t> base_new(n + 1, 0);
     if (n) {
+      const tsm_corpus ca = b.olds.corpus(1), cn = b.news.corpus(1);
+      std::vector<int64_t> added(n), removed(n);
+      std::vector<tsm_diff_detail> det(n);
       int64_t cap = 0, got = 0;
       if (origin_in.empty()) origin_in.push_back({0, 0});
       for (;;) {
         out.resize((size_t)std::max<int64_t>(cap, 1));
-        const int rc = tsm_blame_pairs(ctx, &ca, &cn, added, removed, det, prev.data(), label.data(), origin_in.data(), in_base.data(),
-                                       nullptr, base_new.data(), out.data(), cap, &got, nullptr);
+        const int rc = tsm_blame_pairs(b.ctx, &ca, &cn, added.data(), removed.data(), det.data(), prev.data(), label.data(), origin_in.data(),
+                                       in_base.data(), nullptr, base_new.data(), out.data(), cap, &got, nullptr);
         if (rc == TSM_E_CAPACITY && got > cap) { cap = got; continue; }
         ck(rc, "tsm_blame_pairs");
         break;
       }
-      blamed_pairs += (int64_t)n;
     }
     for (auto& kv : view) {
       if (kv.second.kind == 2) { live.erase(kv.first); continue; }
@@ -1758,12 +1758,11 @@ static int cmd_blame(const std::string& repo, const std::string& rev, int64_t ma
       st.org.assign(out.begin() + base_new[i], out.begin() + base_new[i + 1]);
       live[kv.first] = std::move(st);
     }
-  };
-  const ChangeTotals t = diff_changes(changes, chain.size(), load, rename_pct, true, {}, 0, [](size_t) { return std::vector<std::string>(); },
-                                      "", "", "", "", batch_bytes, &run);
+  });
+  ctx.reset();                                             // the assertion scan below has a context of its own
   // the selected files at R, path order: their origins (a file untouched by the window is all boundary lines)
   std::vector<FileEntry> files;
-  if (!chain.empty()) walk_git(gs, chain.back().c.tree, "", all_files, files);
+  if (!chain.empty()) walk_git(h.gs, chain.back().c.tree, "", all_files, files);
   std::vector<std::vector<tsm_origin>> org(files.size());
   for (size_t f = 0; f < files.size(); ++f) {
     if (binary(*files[f].blob)) continue;
@@ -1826,7 +1825,7 @@ static int cmd_blame(const std::string& repo, const std::string& rev, int64_t ma
     if (cl[s]) printf("%s,%lld,%lld\r\n", (s ? chain[s - 1].id : p0.id).hex().c_str(), (long long)cl[s], (long long)ca[s]);
   }
   fprintf(stderr, "tosem-scan: blame of %s: %zu commits, %lld changed files on the GPU, %lld binary skipped, %zu files, %lld lines, %lld assertion lines\n",
-          rev.c_str(), chain.size(), (long long)blamed_pairs, (long long)t.binaries, files.size(), (long long)total,
+          rev.c_str(), chain.size(), (long long)t.diffed, (long long)t.binaries, files.size(), (long long)total,
           (long long)n_asserts);
   if (cut) fprintf(stderr, "tosem-scan: boundary commit %s\n", p0.id.hex().c_str());
   if (rename_pct >= 0)
@@ -1915,18 +1914,18 @@ static void usage() {
   fprintf(stderr,
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
           "       tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]\n"
-          "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--find-renames N]\n"
+          "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan body   <project-root>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases <snapshot-root>=<tag>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases --git <repository> [<revision>...] [--batch-bytes N] [--out F]\n"
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
-          "                          [--cases F] [--find-renames N]\n"
+          "                          [--cases F] [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
           "       tosem-scan clones <project-root>... [--min-lines N] [--all-files] [--out F]\n"
           "       tosem-scan clones --git <repository> [--rev R] [--min-lines N] [--all-files] [--out F]\n"
           "--find-renames N (0..100): pair deleted and added files at least N %% similar, as git -M<N>%% does (docs/SPEC.md section 13).\n"
           "--cases F: one row per test case that a revision adds (A), deletes (D) or modifies (M) (docs/SPEC.md section 16).\n"
-          "--batch-bytes N: files go to the GPU in batches of at most N bytes (a larger file alone); scan: 1 GiB, else 512 MiB.\n"
+          "--batch-bytes N: files go to the GPU in batches of at most N bytes (per side of a diff; a larger file alone); scan: 1 GiB, else 512 MiB.\n"
           "Scans run on the GPU through libtosemscan.so (sm_90a); there is no CPU fallback.\n");
 }
 
@@ -1967,17 +1966,17 @@ int main(int argc, char** argv) {
     if (pct < 0 || pct > 100 || *end) die("--find-renames needs a similarity from 0 to 100");
     rename_pct = (int)pct;
   }
+  DiffOptions d;                                           // diff and history
+  d.rename_pct = rename_pct; d.batch_bytes = batch_bytes(kBatch, 1);
+  d.out = opt["--out"]; d.asserts = opt["--asserts"]; d.churn = opt["--assert-churn"]; d.cases = opt["--cases"];
+  const std::string rev = opt.count("--rev") ? opt["--rev"] : "HEAD";
+  const int64_t max_commits = opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0;
   if (cmd == "history") { if (pos.size() != 1) die("history needs the repository");
                           if (dry_run && rename_pct >= 0) die("--dry-run and --find-renames cannot be combined (renames need the GPU)");
-                          return cmd_history(pos[0], opt.count("--rev") ? opt["--rev"] : "HEAD",
-                                                  opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0, all_files, opt["--out"], dry_run,
-                                                  opt["--asserts"], opt["--assert-churn"], opt["--cases"], rename_pct); }
+                          return cmd_history(pos[0], rev, max_commits, all_files, dry_run, d); }
   if (cmd == "blame") { if (pos.size() != 1) die("blame needs the repository");
-                        return cmd_blame(pos[0], opt.count("--rev") ? opt["--rev"] : "HEAD",
-                                         opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0, all_files, rename_pct,
-                                         batch_bytes(kBatch, 1),
-                                         opt["--out"], opt["--asserts"]); }
-  if (cmd == "diff") { if (pos.size() != 2) die("diff needs <old-root> <new-root>"); return cmd_diff(pos[0], pos[1], opt["--out"], opt["--asserts"], opt["--assert-churn"], opt["--cases"], rename_pct); }
+                        return cmd_blame(pos[0], rev, max_commits, all_files, rename_pct, d.batch_bytes, d.out, d.asserts); }
+  if (cmd == "diff") { if (pos.size() != 2) die("diff needs <old-root> <new-root>"); return cmd_diff(pos[0], pos[1], d); }
   usage();
   return 2;
 }
