@@ -232,6 +232,26 @@ typedef struct tsm_diff_cases {
 int tsm_diff_pairs_cases(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
                          tsm_diff_detail* detail, tsm_diff_cases* out, void* stream);
 
+/* Assertion edits (docs/SPEC.md section 17): which deleted assertion line of a pair became which inserted one.  chg is filled
+ * exactly as tsm_diff_pairs_asserts fills it (same tables, same events in the same order, same capacity rule), except that
+ * both event arrays are required here (else TSM_E_ARG).  An edit pairs deleted line chg->rev[rev] with inserted line
+ * chg->aev[aev] of the same hunk (both changed assertion lines of a traced pair with the same number of kept lines before
+ * them); score = floor(120000 * lcs / (|a| + |b|)) over the stripped lines a, b (section 2), lcs = the length of their longest
+ * common byte subsequence.  Per hunk, the candidates with score >= 30000 are taken greedily by score (descending), then rev,
+ * then aev (ascending), each line in at most one edit.  Edits are ordered by aev; n_edits <= min(n_aev, n_rev).  n_aev,
+ * n_rev and n_edits are always set; if an event cap or edit_cap is smaller than its count, the call returns TSM_E_CAPACITY
+ * with all three set: size the arrays and call again.  added / removed / detail are those of tsm_diff_pairs_detail (detail
+ * may be NULL).  n_files = 0 is legal.
+ * Kernels: the diff of tsm_diff_pairs_marks, then per side k_case_kept, k_edit_flag, two exclusive scans and k_edit_compact,
+ * k_classify over the compacted lines, k_edit_ranges, k_edit_score (patterns up to 256 bytes) and k_edit_score_long
+ * (csrc/tsm_edit_kernels.cuh); the pairing runs on the host.  tsm_assert_edits_last_ms: ms3 = { k_scan over both sides (device),
+ * the diff kernels (device), compact to pairing (host clock, k_classify and the copies included) } of the last call. */
+typedef struct tsm_assert_edit { int64_t rev, aev; int32_t score, _pad; } tsm_assert_edit;   /* indices into chg->rev / chg->aev */
+int tsm_diff_pairs_assert_edits(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                                tsm_diff_detail* detail, tsm_diff_asserts* chg, tsm_assert_edit* edits, int64_t edit_cap,
+                                int64_t* n_edits, void* stream);
+int tsm_assert_edits_last_ms(tsm_ctx* ctx, float* ms3);
+
 /* Line provenance (docs/SPEC.md section 14, `tosem-scan blame`): the origin of every line of every new side.  The pairs form
  * chains: prev[i] is the pair whose new side is pair i's old side (prev[i] < i; each pair is the prev of at most one pair), or
  * -1 for a chain head, whose old side's origins are origin_in[in_base[i] .. in_base[i+1]) (in_base [n_pairs+1], ascending;

@@ -4,6 +4,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <chrono>
 #include <new>
 #include <utility>
 #include <vector>
@@ -20,6 +21,7 @@
 #include "tsm_similar_kernels.cuh"
 #include "tsm_clone_kernels.cuh"
 #include "tsm_case_kernels.cuh"
+#include "tsm_edit_kernels.cuh"
 
 using namespace tsm;
 
@@ -99,6 +101,7 @@ struct tsm_ctx {
   float diff_ms[3] = {0, 0, 0};            // k_scan over both sides, k_myers, k_myers_trace of the last diff
   float sim_ms[3] = {0, 0, 0};             // k_scan over both sides, sort / merge, k_similarity of the last tsm_similarity
   float clone_ms[3] = {0, 0, 0};           // k_scan, grouping + classes, members + coverage of the last tsm_clones
+  float edit_ms[3] = {0, 0, 0};            // k_scan, the diff, compact to pairing (host clock) of the last assertion-edit call
   cudaEvent_t blame_ev[2] = {};            // around k_blame (tsm_blame_last_ms)
   float blame_ms = 0;
   struct HostSidePair* res_pair = nullptr; // sides kept in HBM by tsm_diff_upload
@@ -1139,10 +1142,12 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
 // over the list they filled, with a ScanParams over that side's arena, tags and groups and a Ctrl of its own whose n_cand
 // is the list's counter - a changed line is classified by the code, and so with the result, of a scan.  Each list holds
 // one entry per line of its side, a bound known before the launch that no side can exceed.
+static int classify_changed(tsm_ctx* c, HostSide* const side[2], unsigned long long* const list[2], Ctrl* const ctrl[2],
+                            const uint32_t nc[2], int32_t n, int32_t n_groups, tsm_diff_asserts* out, cudaStream_t st);
 static int diff_asserts(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int32_t n_groups, int64_t* added, int64_t* removed,
                         tsm_diff_detail* detail, tsm_diff_asserts* out, cudaStream_t st) {
   HostSide* side[2] = {&A, &B};                            // side 0: deleted lines of `old`, side 1: inserted lines of `new`
-  DevBuf d_list[2], d_ctrl, d_counts[2], d_aev[2];
+  DevBuf d_list[2], d_ctrl;
   AssertSink sink{};
   if (!d_ctrl.alloc(2 * 64)) return TSM_E_CUDA;
   Ctrl* ctrl[2] = {d_ctrl.as<Ctrl>(), reinterpret_cast<Ctrl*>(d_ctrl.as<uint8_t>() + 64)};
@@ -1161,6 +1166,14 @@ static int diff_asserts(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int32_t
   CU(cudaStreamSynchronize(st));
   const uint32_t nc[2] = {hc[0].n_cand, hc[1].n_cand};
   if (nc[0] > sink.cap[0] || nc[1] > sink.cap[1]) return TSM_E_CAPACITY;   // (more changed lines than lines: never)
+  return classify_changed(c, side, sink.list, ctrl, nc, n, n_groups, out, st);
+}
+
+// The second half of diff_asserts: per side ONE k_classify launch over the nc[s] candidates list[s] (whose Ctrl ctrl[s] has
+// n_cand = nc[s], cls_done = 0), then the tables and the events (sorted into canonical order) to `out`.
+static int classify_changed(tsm_ctx* c, HostSide* const side[2], unsigned long long* const list[2], Ctrl* const ctrl[2],
+                            const uint32_t nc[2], int32_t n, int32_t n_groups, tsm_diff_asserts* out, cudaStream_t st) {
+  DevBuf d_counts[2], d_aev[2];
   tsm_assert_event* const h_ev[2] = {out->rev, out->aev};
   const int64_t h_cap[2] = {out->rev_cap, out->aev_cap};
   int64_t* const h_counts[2] = {out->removed_counts, out->added_counts};
@@ -1176,7 +1189,7 @@ static int diff_asserts(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int32_t
     ScanParams p = side_params(h);
     p.grp = h.grp.as<uint16_t>(); p.n_groups = n_groups;
     p.ctrl = ctrl[s];
-    p.cand = sink.list[s]; p.cand_cap = sink.cap[s];
+    p.cand = list[s]; p.cand_cap = nc[s];
     p.aev = d_aev[s].as<tsm_assert_event>(); p.aev_cap = h_ev[s] ? nc[s] : 0;
     p.counts = d_counts[s].as<unsigned long long>();
     p.flags = h_ev[s] ? TSM_SCAN_ASSERT_EVENTS : 0u;
@@ -1406,6 +1419,208 @@ extern "C" int tsm_diff_pairs_cases(tsm_ctx* c, const tsm_corpus* olds, const ts
   CU(cudaGetLastError());
   CU(cudaStreamSynchronize(st));
   c->launches += launches;
+  return TSM_OK;
+}
+
+// ------------------------------------------------------------------------------------- SPEC section 17 assertion edits
+// The marks diff, then per side k_case_kept + xscan (kept ranks), k_edit_flag + xscan (entry index) and k_edit_compact: the
+// changed assertion lines of the traced pairs in line order, with their hunk keys and k_classify candidates.  Those lists are
+// the ones tsm_diff_pairs_asserts classifies (diff_asserts gets them from the EMIT diff), so classify_changed gives the same
+// tables and events, event k of a side being its entry k.  Then k_edit_ranges, the score kernels (patterns of up to 256
+// bytes in one launch, longer ones in launches whose global slots stay under kEditScratch words) and the greedy pairing on
+// the host, hunk by hunk (the old entries of a hunk are one run of equal keys): its candidates sorted by score, old entry, new
+// entry, then taken greedily.
+static constexpr unsigned long long kEditScratch = 1ull << 25;   // 256 MiB of Peq and V slots per launch of the long path
+
+// kept: the candidates that pass; pat: the old entries (their keys name the hunks).
+static int edit_scores(tsm_ctx* c, const DevBuf* lines, const uint32_t ne[2], const uint8_t* arena_old, const uint8_t* arena_new,
+                       std::vector<EditCand>& kept, std::vector<EditLine>& pat, cudaStream_t st) {
+  const uint32_t no = ne[0], nn = ne[1];
+  DevBuf d_range, d_ids, d_slot, d_kept, d_nk, d_scratch;
+  if (!d_range.alloc(sizeof(uint2) * no)) return TSM_E_CUDA;
+  k_edit_ranges<<<(no + 255) / 256, 256, 0, st>>>(lines[0].as<EditLine>(), no, lines[1].as<EditLine>(), nn, d_range.as<uint2>());
+  CU(cudaGetLastError());
+  std::vector<uint2> range(no);
+  pat.resize(no);
+  CU(cudaMemcpyAsync(range.data(), d_range.p, sizeof(uint2) * no, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(pat.data(), lines[0].p, sizeof(EditLine) * no, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  std::vector<uint32_t> ids;                               // short patterns, then long ones
+  std::vector<unsigned long long> slot;                    // per long pattern: its slot in the scratch of its launch
+  std::vector<std::pair<uint32_t, uint32_t>> launches;     // long launches: [first, end) of the long ids
+  for (uint32_t i = 0; i < no; ++i)
+    if (range[i].y > range[i].x && pat[i].len <= 64 * EDIT_SHORT_WORDS) ids.push_back(i);
+  const uint32_t n_short = (uint32_t)ids.size();
+  unsigned long long top = 0, need = 0;
+  for (uint32_t i = 0; i < no; ++i) {
+    if (range[i].y == range[i].x || pat[i].len <= 64 * EDIT_SHORT_WORDS) continue;
+    const unsigned long long words = 288ull * ((pat[i].len + 63) / 64);
+    if (launches.empty() || (top + words > kEditScratch && top)) { launches.push_back({(uint32_t)ids.size() - n_short, 0}); top = 0; }
+    ids.push_back(i); slot.push_back(top);
+    top += words;
+    need = std::max(need, top);
+    launches.back().second = (uint32_t)ids.size() - n_short;
+  }
+  if (ids.empty()) return TSM_OK;
+  if (!d_ids.alloc(sizeof(uint32_t) * ids.size()) || !d_nk.alloc(sizeof(uint32_t)) ||
+      (!slot.empty() && (!d_slot.alloc(sizeof(unsigned long long) * slot.size()) || !d_scratch.alloc(sizeof(unsigned long long) * need))))
+    return TSM_E_CUDA;
+  CU(cudaMemcpyAsync(d_ids.p, ids.data(), sizeof(uint32_t) * ids.size(), cudaMemcpyHostToDevice, st));
+  if (!slot.empty()) CU(cudaMemcpyAsync(d_slot.p, slot.data(), sizeof(unsigned long long) * slot.size(), cudaMemcpyHostToDevice, st));
+  uint32_t cap = std::max<uint32_t>(4096, no + nn), nk = 0;
+  for (int attempt = 0; attempt < 2; ++attempt) {          // a second run when more candidates pass than the first list holds
+    if (!d_kept.alloc(sizeof(EditCand) * cap)) return TSM_E_CUDA;
+    CU(cudaMemsetAsync(d_nk.p, 0, sizeof(uint32_t), st));
+    if (n_short)
+      k_edit_score<<<std::min<uint32_t>((n_short + EDIT_WARPS - 1) / EDIT_WARPS, (uint32_t)c->sms * 16), EDIT_WARPS * 32, 0, st>>>(
+          d_ids.as<uint32_t>(), n_short, lines[0].as<EditLine>(), lines[1].as<EditLine>(), d_range.as<uint2>(), arena_old, arena_new,
+          d_kept.as<EditCand>(), cap, d_nk.as<uint32_t>());
+    for (const auto& L : launches) {
+      const uint32_t cnt = L.second - L.first;
+      const unsigned long long words = slot[L.second - 1] + 288ull * ((pat[ids[n_short + L.second - 1]].len + 63) / 64);
+      CU(cudaMemsetAsync(d_scratch.p, 0, sizeof(unsigned long long) * words, st));
+      k_edit_score_long<<<(cnt * 32 + 127) / 128, 128, 0, st>>>(
+          d_ids.as<uint32_t>() + n_short + L.first, d_slot.as<unsigned long long>() + L.first, cnt, lines[0].as<EditLine>(),
+          lines[1].as<EditLine>(), d_range.as<uint2>(), arena_old, arena_new, d_scratch.as<unsigned long long>(), d_kept.as<EditCand>(), cap,
+          d_nk.as<uint32_t>());
+    }
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(&nk, d_nk.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    c->launches += (n_short ? 1 : 0) + (int)launches.size();
+    if (nk <= cap) break;
+    cap = nk;
+  }
+  if (nk > cap) return TSM_E_CAPACITY;                     // (the second run holds every candidate of the first)
+  kept.resize(nk);
+  if (nk) CU(cudaMemcpyAsync(kept.data(), d_kept.p, sizeof(EditCand) * nk, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TSM_OK;
+}
+
+extern "C" int tsm_diff_pairs_assert_edits(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                                           tsm_diff_detail* detail, tsm_diff_asserts* chg, tsm_assert_edit* edits, int64_t edit_cap,
+                                           int64_t* n_edits, void* stream) {
+  if (!c || !olds || !news || !added || !removed || !chg || !chg->aev || !chg->rev || !n_edits || edit_cap < 0 ||
+      olds->n_files != news->n_files || olds->n_groups != news->n_groups)
+    return TSM_E_ARG;
+  const int32_t n = olds->n_files;
+  int rc = check_groups(olds, 0, n);
+  if (rc == TSM_OK) rc = check_groups(news, 0, n);
+  if (rc != TSM_OK) return rc;
+  chg->n_aev = chg->n_rev = 0;
+  *n_edits = 0;
+  for (float& ms : c->edit_ms) ms = 0;
+  if (n == 0) {
+    for (int64_t* t : {chg->added_counts, chg->removed_counts})
+      if (t) memset(t, 0, sizeof(int64_t) * (size_t)olds->n_groups * TSM_K);
+    return TSM_OK;
+  }
+  rc = check_sides({olds, news}, n, true);
+  if (rc != TSM_OK) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  CallScope call(c, st);
+  CU(call.status);
+  HostSidePair P;
+  DevBuf d_traced, d_flag[2], d_pos[2], d_kept[2], d_rank[2], d_lines[2], d_cand[2], d_bsum, d_ctrl;
+  SyncGuard guard(st);
+  rc = pair_upload(olds, news, true, P, st);
+  if (rc == TSM_OK) rc = pair_records(c, P, &c->edit_ms[0], false, st);
+  if (rc != TSM_OK) return rc;
+  std::vector<tsm_diff_detail> own;
+  if (!detail) { own.resize((size_t)n); detail = own.data(); }
+  rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
+  if (rc != TSM_OK) return rc;
+  c->edit_ms[1] = c->diff_ms[1] + c->diff_ms[2];
+  const auto t0 = std::chrono::steady_clock::now();
+  std::vector<uint8_t> traced((size_t)n);
+  for (int32_t i = 0; i < n; ++i) traced[(size_t)i] = detail[i].added_assert >= 0;
+  HostSide* side[2] = {&P.A, &P.B};
+  if (!d_traced.alloc((size_t)n) || !d_ctrl.alloc(2 * 64) ||
+      !d_bsum.alloc(sizeof(unsigned long long) * ((size_t)std::max(P.A.total, P.B.total) / XS_TILE + 4)))
+    return TSM_E_CUDA;
+  CU(cudaMemcpyAsync(d_traced.p, traced.data(), (size_t)n, cudaMemcpyHostToDevice, st));
+  unsigned long long cnt[2] = {0, 0};
+  EditSide es[2];
+  for (int s = 0; s < 2; ++s) {
+    const HostSide& h = *side[s];
+    const uint32_t total = (uint32_t)h.total;
+    if (!d_flag[s].alloc(sizeof(uint32_t) * total) || !d_kept[s].alloc(sizeof(uint32_t) * total) ||
+        !d_pos[s].alloc(sizeof(unsigned long long) * ((size_t)total + 1)) || !d_rank[s].alloc(sizeof(unsigned long long) * ((size_t)total + 1)))
+      return TSM_E_CUDA;
+    es[s] = EditSide{h.d.arena, h.d.off, h.d.line_base, (uint32_t)n, h.d.line_end, h.d.line_flag, h.line_mark.as<uint8_t>(), d_traced.as<uint8_t>()};
+    if (total) {
+      k_case_kept<<<(total + 255) / 256, 256, 0, st>>>(es[s].mark, total, d_kept[s].as<uint32_t>());
+      k_edit_flag<<<(total + 255) / 256, 256, 0, st>>>(es[s], total, d_flag[s].as<uint32_t>());
+    }
+    xscan(d_kept[s].as<uint32_t>(), total, d_bsum.as<unsigned long long>(), d_rank[s].as<unsigned long long>(), st);
+    xscan(d_flag[s].as<uint32_t>(), total, d_bsum.as<unsigned long long>(), d_pos[s].as<unsigned long long>(), st);
+    CU(cudaMemcpyAsync(&cnt[s], d_pos[s].as<unsigned long long>() + total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    c->launches += total ? 8 : 0;
+  }
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(st));
+  const uint32_t ne[2] = {(uint32_t)cnt[0], (uint32_t)cnt[1]};
+  Ctrl hc[2] = {};
+  unsigned long long* list[2];
+  for (int s = 0; s < 2; ++s) {
+    const uint32_t total = (uint32_t)side[s]->total;
+    if (!d_lines[s].alloc(sizeof(EditLine) * std::max(ne[s], 1u)) || !d_cand[s].alloc(sizeof(unsigned long long) * std::max(ne[s], 1u)))
+      return TSM_E_CUDA;
+    list[s] = d_cand[s].as<unsigned long long>();
+    hc[s].n_cand = ne[s];
+    if (total)
+      k_edit_compact<<<(total + 255) / 256, 256, 0, st>>>(es[s], total, d_flag[s].as<uint32_t>(), d_pos[s].as<unsigned long long>(),
+                                                          d_rank[s].as<unsigned long long>(), d_lines[s].as<EditLine>(), list[s]);
+    c->launches += total ? 1 : 0;
+  }
+  CU(cudaGetLastError());
+  Ctrl* ctrl[2] = {d_ctrl.as<Ctrl>(), reinterpret_cast<Ctrl*>(d_ctrl.as<uint8_t>() + 64)};
+  for (int s = 0; s < 2; ++s) CU(cudaMemcpyAsync(ctrl[s], &hc[s], sizeof(Ctrl), cudaMemcpyHostToDevice, st));
+  const int cls_rc = classify_changed(c, side, list, ctrl, ne, n, P.groups_a, chg, st);
+  if (cls_rc != TSM_OK && cls_rc != TSM_E_CAPACITY) return cls_rc;
+  std::vector<EditCand> kept;
+  std::vector<EditLine> pat;
+  if (ne[0] && ne[1]) {
+    rc = edit_scores(c, d_lines, ne, P.A.d.arena, P.B.d.arena, kept, pat, st);
+    if (rc != TSM_OK) return rc;
+  }
+  // greedy pairing per hunk: candidates bucketed by old entry (counting sort), then each hunk's run sorted by score
+  // (descending), old entry, new entry and taken in that order; each entry in at most one edit
+  std::vector<uint32_t> at((size_t)ne[0] + 1, 0);
+  for (const EditCand& k : kept) ++at[(size_t)k.old_e + 1];
+  for (uint32_t i = 0; i < ne[0]; ++i) at[(size_t)i + 1] += at[i];
+  std::vector<EditCand> by_old(kept.size());
+  {
+    std::vector<uint32_t> put(at.begin(), at.end() - 1);
+    for (const EditCand& k : kept) by_old[put[k.old_e]++] = k;
+  }
+  std::vector<char> used_old(ne[0], 0), used_new(ne[1], 0);
+  std::vector<tsm_assert_edit> got;
+  for (uint32_t h0 = 0, h1 = 0; h0 < (uint32_t)pat.size(); h0 = h1) {
+    for (h1 = h0 + 1; h1 < (uint32_t)pat.size() && pat[h1].key == pat[h0].key; ++h1) {}
+    const auto b = by_old.begin() + at[h0], e = by_old.begin() + at[h1];
+    std::sort(b, e, [](const EditCand& x, const EditCand& y) {
+      return x.score != y.score ? x.score > y.score : (x.old_e != y.old_e ? x.old_e < y.old_e : x.new_e < y.new_e);
+    });
+    for (auto k = b; k != e; ++k)
+      if (!used_old[k->old_e] && !used_new[k->new_e]) {
+        used_old[k->old_e] = used_new[k->new_e] = 1;
+        got.push_back(tsm_assert_edit{(int64_t)k->old_e, (int64_t)k->new_e, (int32_t)k->score, 0});
+      }
+  }
+  std::sort(got.begin(), got.end(), [](const tsm_assert_edit& x, const tsm_assert_edit& y) { return x.aev < y.aev; });
+  c->edit_ms[2] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  *n_edits = (int64_t)got.size();
+  if (cls_rc == TSM_E_CAPACITY || *n_edits > edit_cap) return TSM_E_CAPACITY;   // all three counts set: size and call again
+  if (*n_edits && !edits) return TSM_E_ARG;
+  if (*n_edits) memcpy(edits, got.data(), sizeof(tsm_assert_edit) * got.size());
+  return TSM_OK;
+}
+
+extern "C" int tsm_assert_edits_last_ms(tsm_ctx* c, float* ms3) {
+  if (!c || !ms3) return TSM_E_ARG;
+  for (int i = 0; i < 3; ++i) ms3[i] = c->edit_ms[i];
   return TSM_OK;
 }
 

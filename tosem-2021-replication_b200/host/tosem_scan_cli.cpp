@@ -17,11 +17,12 @@
 //
 //   tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N]
 //   tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]
-//   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--find-renames N] [--batch-bytes N]
+//   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--find-renames N]
+//                     [--batch-bytes N]
 //   tosem-scan body   <project-root>... [--batch-bytes N] [--out F]
 //   tosem-scan releases <snapshot-root>=<tag>... | --git <repository> [<revision>...]   [--batch-bytes N] [--out F]
 //   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F] [--cases F]
-//                      [--find-renames N] [--batch-bytes N]
+//                      [--assert-edits F] [--find-renames N] [--batch-bytes N]
 //   tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]
 //   tosem-scan clones <project-root>... | --git <repository> [--rev R]   [--min-lines N] [--all-files] [--out F]
 // Every command that scans files does it with scan_batches: batches of at most --batch-bytes of arena (clones: all files in one),
@@ -1199,6 +1200,27 @@ static void diff_asserts(tsm_ctx* ctx, const tsm_corpus& ca, const tsm_corpus& c
     return;
   }
 }
+// The same with the assertion edits of docs/SPEC.md section 17 (tsm_diff_pairs_assert_edits, one call for both): `chg` is
+// filled as diff_asserts fills it, `edits` pairs its events.  Event and edit arrays grow to the counts the library reports.
+static void diff_assert_edits(tsm_ctx* ctx, const tsm_corpus& ca, const tsm_corpus& cn, int64_t* added, int64_t* removed,
+                              tsm_diff_detail* det, ChangedAsserts& r, std::vector<tsm_assert_edit>& edits) {
+  const size_t table = (size_t)ca.n_groups * TSM_NUM_CATEGORIES;
+  r.added_counts.assign(table, 0); r.removed_counts.assign(table, 0);
+  int64_t cap = ((int64_t)ca.off[ca.n_files] + cn.off[cn.n_files]) / 64 + 1024, ecap = cap;
+  for (;;) {
+    r.aev.resize((size_t)cap); r.rev.resize((size_t)cap); edits.resize((size_t)ecap);
+    tsm_diff_asserts o{r.added_counts.data(), r.removed_counts.data(), r.aev.data(), cap, 0, r.rev.data(), cap, 0};
+    int64_t ne = 0;
+    const int rc = tsm_diff_pairs_assert_edits(ctx, &ca, &cn, added, removed, det, &o, edits.data(), ecap, &ne, nullptr);
+    if (rc == TSM_E_CAPACITY && (std::max(o.n_aev, o.n_rev) > cap || ne > ecap)) {
+      cap = std::max(cap, std::max(o.n_aev, o.n_rev)); ecap = std::max(ecap, ne);
+      continue;
+    }
+    ck(rc, "tsm_diff_pairs_assert_edits");
+    r.aev.resize((size_t)o.n_aev); r.rev.resize((size_t)o.n_rev); edits.resize((size_t)ne);
+    return;
+  }
+}
 // The --asserts rows of pair `pair` on one side: `lead` cells, fileName, change ('+' new side, '-' old side), 1-based line
 // number in that side's file, statement, category.  `k` walks the side's events (canonical order) across calls.
 static void assert_rows(std::ostream& os, const std::vector<std::string>& lead, const std::string& path, const uint8_t* base,
@@ -1289,6 +1311,27 @@ static void case_rows(std::ostream& os, std::vector<std::string> lead, const Cas
     if (c.n_changed || d.n_changed || c.n_lines != d.n_lines)
       row(*nw.path, {nb[j], "M", num(c.line + 1), num(d.line + 1), num(c.n_lines), num(d.n_lines), num(c.n_assert), num(d.n_assert),
                      num(c.n_changed), num(d.n_changed), num(c.n_changed_assert), num(d.n_changed_assert)});
+  }
+}
+
+// The --assert-edits rows of pair `pair` (docs/SPEC.md section 17), in new line order: `lead` cells, fileName (the new path),
+// 1-based oldLine and line, similarity in %, statement and category of both lines, then oldFileName when old_path is given.
+// `ke` walks the edits (aev order) and `kr` the deleted-line events across calls.
+static void edit_rows(std::ostream& os, const std::vector<std::string>& lead, const CaseSide& o, const CaseSide& nw, const std::string* old_path,
+                      const ChangedAsserts& chg, const std::vector<tsm_assert_edit>& ed, size_t& ke, size_t& kr, uint32_t pair) {
+  const size_t r0 = kr;
+  LineCounter lo{o.base}, ln{nw.base};
+  std::vector<int64_t> old_line;                           // line of each deleted-line event of the pair (events in line order)
+  for (; kr < chg.rev.size() && chg.rev[kr].file == pair; ++kr) old_line.push_back(lo.at(chg.rev[kr].line_off));
+  for (; ke < ed.size() && chg.aev[(size_t)ed[ke].aev].file == pair; ++ke) {
+    const tsm_assert_edit& e = ed[ke];
+    const tsm_assert_event &a = chg.rev[(size_t)e.rev], &b = chg.aev[(size_t)e.aev];
+    std::vector<std::string> row = lead;
+    row.insert(row.end(), {*nw.path, std::to_string(old_line[(size_t)e.rev - r0]), std::to_string(ln.at(b.line_off)), std::to_string(e.score / 600),
+                           event_statement(o.base, o.size, a), event_statement(nw.base, nw.size, b), event_category(o.base, a),
+                           event_category(nw.base, b)});
+    if (old_path) row.push_back(*old_path);
+    csv_row(os, row);
   }
 }
 
@@ -1416,7 +1459,7 @@ static void pair_batches(tsm_ctx* ctx, const std::vector<Change>& changes, const
 struct DiffOptions {
   int rename_pct = -1;
   int64_t batch_bytes = kBatch;
-  std::string out, asserts, churn, cases;
+  std::string out, asserts, churn, cases, edits;
   bool zero_rows = false;
   std::vector<std::string> lead_head;
   size_t churn_lead = 0;
@@ -1424,13 +1467,16 @@ struct DiffOptions {
 };
 
 // The diff of one batch: per pair the lines added and removed and the detail; with `asserts` the changed assertion lines and
-// the [group][K] tables, with `cases` the case records.
-struct PairDiff { std::vector<int64_t> added, removed; std::vector<tsm_diff_detail> det; ChangedAsserts chg; CaseLists cases; };
-static PairDiff diff_batch(const PairBatch& b, bool asserts, bool cases) {
+// the [group][K] tables, with `edits` also the assertion edits (the same call), with `cases` the case records.
+struct PairDiff {
+  std::vector<int64_t> added, removed; std::vector<tsm_diff_detail> det; ChangedAsserts chg; CaseLists cases; std::vector<tsm_assert_edit> edits;
+};
+static PairDiff diff_batch(const PairBatch& b, bool asserts, bool cases, bool edits) {
   const size_t n = b.idx.size();
-  PairDiff d{std::vector<int64_t>(n), std::vector<int64_t>(n), std::vector<tsm_diff_detail>(n), {}, {}};
+  PairDiff d{std::vector<int64_t>(n), std::vector<int64_t>(n), std::vector<tsm_diff_detail>(n), {}, {}, {}};
   const tsm_corpus ca = b.olds.corpus(b.n_groups()), cn = b.news.corpus(b.n_groups());
-  if (asserts) diff_asserts(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.chg);
+  if (edits) diff_assert_edits(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.chg, d.edits);
+  else if (asserts) diff_asserts(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.chg);
   else if (cases) diff_cases(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.cases);
   else ck(tsm_diff_pairs_detail(b.ctx, &ca, &cn, d.added.data(), d.removed.data(), d.det.data(), nullptr), "tsm_diff_pairs_detail");
   if (asserts && cases) {                                  // a second call: the assertion tables and the cases are separate diffs
@@ -1447,7 +1493,7 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
   const bool renames = o.rename_pct >= 0;
   const auto ctx = small_context();
   if (renames) pair_renames(ctx.get(), changes, load, o.rename_pct, o.batch_bytes, t);
-  std::ofstream os, as, cs, ch;                            // --out, --asserts, --cases, --assert-churn
+  std::ofstream os, as, cs, ch, es;                        // --out, --asserts, --cases, --assert-churn, --assert-edits
   auto open = [&](std::ofstream& f, const std::string& path, size_t n_lead, std::vector<std::string> head) {
     if (path.empty()) return;
     f.open(path, std::ios::binary);
@@ -1459,16 +1505,19 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
                                         "insertedLines", "deletedLines", "insertedAsserts", "deletedAsserts"};
   if (renames) out_head.insert(out_head.end(), {"oldFileName", "similarity"});
   if (renames) case_head.push_back("oldFileName");
+  std::vector<std::string> edit_head = {"fileName", "oldLine", "line", "similarity", "oldStatement", "statement", "oldCategory", "category"};
+  if (renames) edit_head.push_back("oldFileName");
   open(os, o.out, o.lead_head.size(), out_head);
   open(as, o.asserts, o.lead_head.size(), {"fileName", "change", "line", "statement", "category"});
   open(cs, o.cases, o.lead_head.size(), case_head);
   open(ch, o.churn, o.churn_lead, {"category", "added", "removed"});
-  const bool want_asserts = !o.asserts.empty() || !o.churn.empty();
+  open(es, o.edits, o.lead_head.size(), edit_head);
+  const bool want_asserts = !o.asserts.empty() || !o.churn.empty() || es.is_open();
   std::map<size_t, std::vector<int64_t>> churn;            // per step with changed assertion lines: its [K] added and removed rows
   pair_batches(ctx.get(), changes, load, o.batch_bytes, want_asserts, t, [&](const PairBatch& b) {
     const size_t n = b.idx.size();
     if (!n) return;
-    const PairDiff d = diff_batch(b, want_asserts, cs.is_open());
+    const PairDiff d = diff_batch(b, want_asserts, cs.is_open(), es.is_open());
     for (size_t g = 0; ch.is_open() && g < b.group_step.size(); ++g) {   // a step's files may span two batches
       const int64_t* ad = d.chg.added_counts.data() + g * TSM_NUM_CATEGORIES;
       const int64_t* rm = d.chg.removed_counts.data() + g * TSM_NUM_CATEGORIES;
@@ -1478,7 +1527,8 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
       tab.resize(2 * TSM_NUM_CATEGORIES, 0);
       for (int k = 0; k < TSM_NUM_CATEGORIES; ++k) { tab[(size_t)k] += ad[k]; tab[(size_t)(TSM_NUM_CATEGORIES + k)] += rm[k]; }
     }
-    for (size_t i = 0, ka = 0, kr = 0, ko = 0, kn = 0; i < n; ++i) {   // ka, kr, ko, kn: pair i's first event and case of each side
+    // ka, kr, ko, kn: pair i's first event and case of each side; ke, ker: its first edit and the deleted-line event edit_rows is at
+    for (size_t i = 0, ka = 0, kr = 0, ko = 0, kn = 0, ke = 0, ker = 0; i < n; ++i) {
       const Change& c = changes[b.idx[i]];
       const std::string& old_path = c.old_path.empty() ? c.path : c.old_path;
       const CaseSide olds{b.olds.arena.get() + b.olds.off[i], b.olds.len[i], b.olds.ext[i], &old_path};
@@ -1487,6 +1537,7 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
         assert_rows(as, o.lead(c.step), old_path, olds.base, olds.size, d.chg.rev, kr, (uint32_t)i, "-");
         assert_rows(as, o.lead(c.step), c.path, news.base, news.size, d.chg.aev, ka, (uint32_t)i, "+");
       }
+      if (es.is_open()) edit_rows(es, o.lead(c.step), olds, news, renames ? &c.old_path : nullptr, d.chg, d.edits, ke, ker, (uint32_t)i);
       const size_t o0 = ko, n0 = kn;
       while (ko < d.cases.olds.size() && d.cases.olds[ko].pair == (int32_t)i) ++ko;
       while (kn < d.cases.news.size() && d.cases.news[kn].pair == (int32_t)i) ++kn;
@@ -1914,17 +1965,20 @@ static void usage() {
   fprintf(stderr,
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
           "       tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]\n"
-          "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--find-renames N] [--batch-bytes N]\n"
+          "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--find-renames N]\n"
+          "                         [--batch-bytes N]\n"
           "       tosem-scan body   <project-root>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases <snapshot-root>=<tag>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases --git <repository> [<revision>...] [--batch-bytes N] [--out F]\n"
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
-          "                          [--cases F] [--find-renames N] [--batch-bytes N]\n"
+          "                          [--cases F] [--assert-edits F] [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
           "       tosem-scan clones <project-root>... [--min-lines N] [--all-files] [--out F]\n"
           "       tosem-scan clones --git <repository> [--rev R] [--min-lines N] [--all-files] [--out F]\n"
           "--find-renames N (0..100): pair deleted and added files at least N %% similar, as git -M<N>%% does (docs/SPEC.md section 13).\n"
           "--cases F: one row per test case that a revision adds (A), deletes (D) or modifies (M) (docs/SPEC.md section 16).\n"
+          "--assert-edits F: one row per deleted assertion line that an inserted one of the same hunk replaces, with their similarity\n"
+          "                  (docs/SPEC.md section 17).\n"
           "--batch-bytes N: files go to the GPU in batches of at most N bytes (per side of a diff; a larger file alone); scan: 1 GiB, else 512 MiB.\n"
           "Scans run on the GPU through libtosemscan.so (sm_90a); there is no CPU fallback.\n");
 }
@@ -1969,6 +2023,7 @@ int main(int argc, char** argv) {
   DiffOptions d;                                           // diff and history
   d.rename_pct = rename_pct; d.batch_bytes = batch_bytes(kBatch, 1);
   d.out = opt["--out"]; d.asserts = opt["--asserts"]; d.churn = opt["--assert-churn"]; d.cases = opt["--cases"];
+  d.edits = opt["--assert-edits"];
   const std::string rev = opt.count("--rev") ? opt["--rev"] : "HEAD";
   const int64_t max_commits = opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0;
   if (cmd == "history") { if (pos.size() != 1) die("history needs the repository");

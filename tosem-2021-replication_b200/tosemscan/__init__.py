@@ -32,6 +32,7 @@ DIFF_DETAIL = np.dtype([("hunks_add", "<i8"), ("hunks_del", "<i8"), ("hunks_mod"
 ORIGIN = np.dtype([("change", "<i4"), ("line", "<i4")])   # tsm_origin: the change that inserted a line, 1-based line there
 CASE = np.dtype([("pair", "<i4"), ("line", "<i4"), ("n_lines", "<i4"), ("n_assert", "<i4"), ("n_changed", "<i4"),
                  ("n_changed_assert", "<i4"), ("match", "<i4")])   # tsm_case: one test case of one side of a revision pair
+ASSERT_EDIT = np.dtype([("rev", "<i8"), ("aev", "<i8"), ("score", "<i4"), ("_pad", "<i4")])   # tsm_assert_edit: event indices
 
 # every symbol include/tosemscan.h declares (tests check the library exports exactly these)
 SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create", "tsm_destroy", "tsm_scan",
@@ -40,7 +41,7 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_diff_pairs_asserts", "tsm_diff_resident_asserts", "tsm_reduce", "tsm_host_alloc", "tsm_host_free", "tsm_layout", "tsm_gen_sizes",
            "tsm_gen_fill", "tsm_gen_edit", "tsm_gen_pair_sizes", "tsm_gen_pair_fill", "tsm_similarity", "tsm_similarity_last_ms",
            "tsm_diff_pairs_marks", "tsm_blame_pairs", "tsm_blame_last_ms", "tsm_clones", "tsm_clones_last_ms",
-           "tsm_diff_pairs_cases"]
+           "tsm_diff_pairs_cases", "tsm_diff_pairs_assert_edits", "tsm_assert_edits_last_ms"]
 
 
 class TsmError(RuntimeError):
@@ -174,6 +175,9 @@ def lib():
         L.tsm_diff_pairs_cases.restype = C.c_int
         L.tsm_diff_pairs_cases.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 3 + \
             [C.POINTER(_DiffCases), C.c_void_p]
+        L.tsm_diff_pairs_assert_edits.restype = C.c_int
+        L.tsm_diff_pairs_assert_edits.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 3 + \
+            [C.POINTER(_DiffAsserts), C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p]
         L.tsm_blame_pairs.restype = C.c_int
         L.tsm_blame_pairs.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 10 + \
             [C.c_int64, C.POINTER(C.c_int64), C.c_void_p]
@@ -695,6 +699,39 @@ class Scanner:
                 raise TsmError(rc, "tsm_diff_pairs_cases")
             return added, removed, det[:n], oc[:r.n_old], nc[:r.n_new]
         raise TsmError(TSM_E_CAPACITY, "tsm_diff_pairs_cases")
+
+    def diff_assert_edits(self, olds, news, stream=None, cap=None):
+        """Assertion edits (docs/SPEC.md section 17): diff_pairs(asserts=True)'s (added, removed, detail, added_counts,
+        removed_counts, added_events, removed_events) plus an ASSERT_EDIT array: per edit the index of the deleted line in
+        removed_events (rev), of the inserted line in added_events (aev) and the score (similarity in % = score // 600),
+        ordered by aev.  Arrays too small for the events or the edits are sized and the call made again (cap: the first guess
+        for each)."""
+        n = olds.n_files
+        added, removed, det = np.zeros(n, np.int64), np.zeros(n, np.int64), np.zeros(max(n, 1), DIFF_DETAIL)
+        a, b = olds.c_struct(), news.c_struct()
+        ce = int(cap if cap is not None else (olds.source_bytes + news.source_bytes) // 1024 + 4096)
+        ck = ce
+        for _ in range(2):
+            ac, rc_ = np.zeros((olds.n_groups, K), np.int64), np.zeros((olds.n_groups, K), np.int64)
+            aev, rev, ed = np.zeros(max(ce, 1), ASSERT_EVENT), np.zeros(max(ce, 1), ASSERT_EVENT), np.zeros(max(ck, 1), ASSERT_EDIT)
+            r = _DiffAsserts(_p(ac), _p(rc_), _p(aev), ce, 0, _p(rev), ce, 0)
+            ne = C.c_int64(0)
+            rc = lib().tsm_diff_pairs_assert_edits(self._ctx, C.byref(a), C.byref(b), _p(added), _p(removed), _p(det), C.byref(r),
+                                                   _p(ed), ck, C.byref(ne), stream)
+            if rc == TSM_E_CAPACITY and (max(r.n_aev, r.n_rev) > ce or ne.value > ck):
+                ce, ck = max(ce, int(r.n_aev), int(r.n_rev)), max(ck, int(ne.value))
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_diff_pairs_assert_edits")
+            return added, removed, det[:n], ac, rc_, aev[:r.n_aev], rev[:r.n_rev], ed[:ne.value]
+        raise TsmError(TSM_E_CAPACITY, "tsm_diff_pairs_assert_edits")
+
+    def assert_edits_last_ms(self):
+        """Phases of the last diff_assert_edits call in ms: [k_scan over both sides, the diff kernels, compact to pairing
+        (host clock)]."""
+        ms = (C.c_float * 3)()
+        lib().tsm_assert_edits_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
 
     def blame_pairs(self, olds, news, prev, label, heads, stream=None, cap=None):
         """Line provenance (docs/SPEC.md section 14): (added, removed, detail, line_base_new, origins) with origins an ORIGIN array
