@@ -28,7 +28,9 @@ import pytest
 
 import corpus_util as cu
 import orc
+import orc_assert_edits
 import orc_asserts
+import orc_cases
 import orc_clones
 import orc_marks
 import orc_similarity
@@ -204,6 +206,20 @@ def pair_corpora():
 
 
 @functools.lru_cache(None)
+def edit_corpora():
+    """pair_corpora's pairs, and each of their old sides against itself with every assertion line edited (a byte inserted
+    before its last one): hunks of changed assertion lines that pair up; and the twin."""
+    (a, b), _ = pair_corpora()
+    olds = [a.file_bytes(i) for i in range(a.n_files)]
+    news = [b.file_bytes(i) for i in range(b.n_files)]
+    edited = [b"\n".join(x[:-1] + b"0" + x[-1:] if b"assert" in x.lower() else x for x in o.split(b"\n")) for o in olds]
+    olds, news = olds + olds, news + edited
+    n = len(olds)
+    exts, grp = np.concatenate([a.ext, a.ext]), np.concatenate([a.grp, a.grp])
+    return [(pinned(olds, exts, grp, 3, order), pinned(news, exts, grp, 3, order)) for order in (np.arange(n), shuffled(n, 6))]
+
+
+@functools.lru_cache(None)
 def blame_chains():
     """Chains of edited C5-law files (test_gpu_blame.chains) as blame_pairs arguments; the twin has the pairs in another
     order that keeps each chain's order."""
@@ -243,6 +259,18 @@ def check_asserts(got, a, b):
     for x, y in zip(got[3:], want):
         assert np.array_equal(x, y)
     assert len(want[2]) > 50 and len(want[3]) > 50
+
+
+def check_edits(got, a, b):
+    check_asserts(got[:7], a, b)
+    want = orc_assert_edits.assert_edits((a.arena, a.off, a.len, a.ext), (b.arena, b.off, b.len, b.ext))
+    assert np.array_equal(got[7], want) and len(want) > 1000
+
+
+def check_cases(got, a, b):
+    check_diff(got[:3], a, b)
+    same(got[3:], orc_cases.diff_cases((a.arena, a.off, a.len, a.ext), (b.arena, b.off, b.len, b.ext)))
+    assert len(got[3]) > 100 and (got[4]["match"] >= 0).sum() > 100
 
 
 def check_marks(got, a, b):
@@ -287,6 +315,11 @@ def a_case(name):
         pair, twin = pair_corpora()
         sc = ts.Scanner(0, 1 << 20, 16, 4)
         return sc, lambda x, st: sc.diff_marks(*x, st), pair, twin, lambda r, x: check_marks(r, *x)
+    if name in ("diff_assert_edits", "diff_cases"):
+        pair, twin = edit_corpora() if name == "diff_assert_edits" else pair_corpora()
+        sc = ts.Scanner(0, 1 << 20, 16, 4)
+        fn, chk = (sc.diff_assert_edits, check_edits) if name == "diff_assert_edits" else (sc.diff_cases, check_cases)
+        return sc, lambda x, st: fn(*x, st), pair, twin, lambda r, x: chk(r, *x)
     if name == "blame_pairs":
         x, twin = blame_chains()
         sc = ts.Scanner(0, 1 << 20, 16, 4)
@@ -341,7 +374,7 @@ def a_case(name):
 
 A_CASES = ["scan-small-revA", "scan-small-revB", "scan-streamed-revA", "scan-streamed-revB", "resident", "diff_pairs",
            "diff_pairs_detail", "diff_pairs_asserts", "diff_resident", "diff_resident_asserts", "diff_pairs_marks",
-           "blame_pairs", "similarity", "clones", "line_hashes", "statements", "reduce"]
+           "diff_assert_edits", "diff_cases", "blame_pairs", "similarity", "clones", "line_hashes", "statements", "reduce"]
 
 
 @pytest.mark.parametrize("name", A_CASES)
@@ -557,6 +590,8 @@ def round_of(sc, inp, st):
     sc.scan_resident(EV | REV_B, st)
     out["resident"] = sc.download(EV | REV_B, st)
     out["asserts"] = sc.diff_pairs(a, b, st, asserts=True)
+    out["edits"] = sc.diff_assert_edits(a, b, st)
+    out["cases"] = sc.diff_cases(a, b, st)
     out["similarity"] = sc.similarity(a, b, co, cn, st)
     out["lines"] = sc.line_hashes(small, 3, st)
     out["statements"] = sc.statements(small, st)
