@@ -302,6 +302,31 @@ typedef struct tsm_clone_result {
 int tsm_clones(tsm_ctx* ctx, const tsm_corpus* corpus, int32_t min_lines, tsm_clone_result* out, void* stream);
 int tsm_clones_last_ms(tsm_ctx* ctx, float* ms3);
 
+/* Test smells (docs/SPEC.md section 18, `tosem-scan smells`): the tests of every file (section-16 cases whose header opens a test
+ * by the rule of its family), their bodies and the nine smells below, as one record per test in global line order (files in
+ * order, then header line) and the smell bits of every line (its instances; 0 outside test bodies).  Bit k of `smells` and of
+ * line_smell[l] is smell k of the TSM_SMELL_* list.  The test-level smells `empty` and `assertion_free`, and `ignored` found on
+ * the decorators or the header, are instances on the header line.
+ *   file          index of the file in the corpus
+ *   line          0-based header line inside the file
+ *   body_lines    lines of the body, header line included (section 18's body end)
+ *   n_assert      assertion lines of the test (header statement and code lines only: no comment or docstring line)
+ *   smells        OR of the smell bits of the test
+ *   n_instances   instance lines of the test, one per (line, smell) pair: the sum of popcount(line_smell) over its body
+ * line_base[n_files+1] and line_smell hold the lines of every file (line_cap of them), tests test_cap records.  Any output
+ * pointer may be NULL (it is skipped); *n_lines and *n_tests are always set.  If line_smell is given with line_cap < *n_lines,
+ * or tests with test_cap < *n_tests, the call returns TSM_E_CAPACITY: size the arrays and call again.  n_files = 0 is legal.
+ * Kernels: k_scan with the header events, k_line_parens + k_stmt_kinds (section 10), k_case_heads + xscan + k_case_lines (the
+ * case spans), k_smell_lines and k_smell_tests (csrc/tsm_smell_kernels.cuh).
+ * tsm_smells_last_ms: device time of the last call, ms4 = { k_scan, kinds + case spans, k_smell_lines, k_smell_tests }. */
+enum { TSM_SMELL_EMPTY = 0, TSM_SMELL_ASSERTION_FREE = 1, TSM_SMELL_DUPLICATE_ASSERT = 2, TSM_SMELL_REDUNDANT_ASSERT = 3,
+       TSM_SMELL_CONDITIONAL_LOGIC = 4, TSM_SMELL_EXCEPTION_HANDLING = 5, TSM_SMELL_SLEEPY = 6, TSM_SMELL_PRINT = 7,
+       TSM_SMELL_IGNORED = 8, TSM_N_SMELLS = 9 };
+typedef struct tsm_smell_test { int32_t file, line, body_lines, n_assert; uint32_t smells; int32_t n_instances; } tsm_smell_test;
+int tsm_smells(tsm_ctx* ctx, const tsm_corpus* corpus, int64_t* line_base, uint16_t* line_smell, int64_t line_cap, int64_t* n_lines,
+               tsm_smell_test* tests, int64_t test_cap, int64_t* n_tests, void* stream);
+int tsm_smells_last_ms(tsm_ctx* ctx, float* ms4);
+
 /* Body statements (docs/SPEC.md section 10; Important-files/ML-Analysis-v4.xlsx!Apollo:R2-R26, golden G2): the
  * kind of every line of every file - 0 blank, 1 first line of a statement, 2 continuation (lines
  * are joined while the parentheses are open).  line_base[n_files+1] and *n_lines are always filled;

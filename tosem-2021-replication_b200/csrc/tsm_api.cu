@@ -22,6 +22,7 @@
 #include "tsm_clone_kernels.cuh"
 #include "tsm_case_kernels.cuh"
 #include "tsm_edit_kernels.cuh"
+#include "tsm_smell_kernels.cuh"
 
 using namespace tsm;
 
@@ -101,6 +102,7 @@ struct tsm_ctx {
   float diff_ms[3] = {0, 0, 0};            // k_scan over both sides, k_myers, k_myers_trace of the last diff
   float sim_ms[3] = {0, 0, 0};             // k_scan over both sides, sort / merge, k_similarity of the last tsm_similarity
   float clone_ms[3] = {0, 0, 0};           // k_scan, grouping + classes, members + coverage of the last tsm_clones
+  float smell_ms[4] = {0, 0, 0, 0};        // k_scan, kinds + case spans, k_smell_lines, k_smell_tests of the last tsm_smells
   float edit_ms[3] = {0, 0, 0};            // k_scan, the diff, compact to pairing (host clock) of the last assertion-edit call
   cudaEvent_t blame_ev[2] = {};            // around k_blame (tsm_blame_last_ms)
   float blame_ms = 0;
@@ -136,6 +138,7 @@ struct EvSpan { int from, to; };
 constexpr EvSpan EV_SCAN[2] = {{0, 1}, {6, 7}}, EV_SMALL = {2, 3}, EV_LEFT = {4, 5};
 constexpr int EV_SIM_LISTS = 2, EV_SIM_PAIRS = 3, EV_SIM_END = 4;
 constexpr int EV_CLONE_GROUP = 2, EV_CLONE_MEMBERS = 3, EV_CLONE_END = 4;
+constexpr int EV_SMELL_KINDS = 2, EV_SMELL_LINES = 3, EV_SMELL_TESTS = 4, EV_SMELL_END = 5;
 
 // The start of every call that queues device work on st: the ctx's device, the ctx's pool for the call's DevBufs, and the
 // order of the ctx's calls.  A ctx orders its own work, whatever stream each call is given: the call's stream first waits
@@ -948,9 +951,9 @@ int sides_records(tsm_ctx* c, HostSide* const* sides, int ns, cudaStream_t st, f
   return TSM_OK;                                           //  the gather queued above still reads them)
 }
 
-int side_records(tsm_ctx* c, HostSide& h, cudaStream_t st, float* scan_ms) {
+int side_records(tsm_ctx* c, HostSide& h, cudaStream_t st, float* scan_ms, uint32_t flags = 0) {
   HostSide* one[1] = {&h};
-  return sides_records(c, one, 1, st, scan_ms, true);
+  return sides_records(c, one, 1, st, scan_ms, true, flags);
 }
 }  // namespace
 
@@ -1821,10 +1824,10 @@ extern "C" int tsm_similarity_last_ms(tsm_ctx* c, float* ms3) {
 // The front of tsm_line_hashes and tsm_statements: the corpus' line records from one pass of the scan, and line_base[n+1]
 // and *n_lines on the host - also when cap is short of the lines, which returns TSM_E_CAPACITY so that the caller can
 // allocate and call again.  Then tail(S, lines, st), the call's own use of the records, inside the call's SyncGuard.
-// scan_ms: the device time of the k_scan launches.
+// scan_ms: the device time of the k_scan launches; flags: TSM_SCAN_HEADER_EVENTS also lists the header events (S.hev).
 template <typename Tail>
 static int line_records(tsm_ctx* c, const tsm_corpus* k, bool ext_rule, int64_t* line_base, int64_t cap, int64_t* n_lines,
-                        void* stream, Tail tail, float* scan_ms = nullptr) {
+                        void* stream, Tail tail, float* scan_ms = nullptr, uint32_t flags = 0) {
   const int32_t n = k->n_files;
   *n_lines = 0;
   line_base[0] = 0;
@@ -1837,7 +1840,7 @@ static int line_records(tsm_ctx* c, const tsm_corpus* k, bool ext_rule, int64_t*
   HostSide S;
   SyncGuard guard(st);
   rc = side_upload(k, S, st);
-  if (rc == TSM_OK) rc = side_records(c, S, st, scan_ms);
+  if (rc == TSM_OK) rc = side_records(c, S, st, scan_ms, flags);
   if (rc != TSM_OK) return rc;
   const unsigned long long total = S.base[(size_t)n];
   for (int32_t i = 0; i <= n; ++i) line_base[i] = (int64_t)S.base[(size_t)i];
@@ -2000,5 +2003,75 @@ extern "C" int tsm_clones(tsm_ctx* c, const tsm_corpus* k, int32_t min_lines, ts
 extern "C" int tsm_clones_last_ms(tsm_ctx* c, float* ms3) {
   if (!c || !ms3) return TSM_E_ARG;
   for (int i = 0; i < 3; ++i) ms3[i] = c->clone_ms[i];
+  return TSM_OK;
+}
+
+// ------------------------------------------------------------------------------------- SPEC section 18 test smells
+// The line records of the corpus with its header events (line_records), then the section-10 kinds (k_line_parens, k_stmt_kinds),
+// the case spans (k_case_heads, xscan of the heads, k_case_lines), k_smell_lines (with the test flag of every case), xscan of
+// the test flags (dense test numbers) and k_smell_tests.  One synchronisation at the end reads the test count; the outputs are
+// copied when they fit.
+extern "C" int tsm_smells(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, uint16_t* line_smell, int64_t line_cap, int64_t* n_lines,
+                          tsm_smell_test* tests, int64_t test_cap, int64_t* n_tests, void* stream) {
+  if (!c || !k || !n_lines || !n_tests || line_cap < 0 || test_cap < 0 || k->n_files < 0) return TSM_E_ARG;
+  const int32_t nf = k->n_files;
+  for (float& v : c->smell_ms) v = 0;
+  c->launches = 0;
+  *n_tests = 0;
+  std::vector<int64_t> own_base;
+  if (!line_base) { own_base.resize((size_t)nf + 1); line_base = own_base.data(); }
+  return line_records(c, k, true, line_base, INT64_MAX, n_lines, stream, [&](const HostSide& S, unsigned long long total, cudaStream_t st) -> int {
+    const uint32_t T = (uint32_t)total, ne = S.hc.n_hev;
+    const size_t L = (size_t)total;
+    DevBuf d_delta, d_kind, d_head, d_case_of, d_first, d_tflag, d_tidx, d_bsum, d_lines, d_hash, d_aline, d_smell, d_tests;
+    if (!d_delta.alloc(4 * L) || !d_kind.alloc(L) || !d_head.alloc(4 * L) || !d_case_of.alloc(8 * (L + 1)) || !d_first.alloc(4 * ((size_t)ne + 1)) ||
+        !d_tflag.alloc(4 * ((size_t)ne + 1)) || !d_tidx.alloc(8 * ((size_t)ne + 1)) || !d_bsum.alloc(8 * (L / XS_TILE + 4)) ||
+        !d_lines.alloc(sizeof(SmellLine) * L) || !d_hash.alloc(8 * L) || !d_aline.alloc(4 * L) || !d_smell.alloc(2 * L) ||
+        !d_tests.alloc(sizeof(tsm_smell_test) * ((size_t)ne + 1)))
+      return TSM_E_CUDA;
+    const unsigned grid = (unsigned)((L + 255) / 256);
+    CU(cudaEventRecord(c->diff_ev[EV_SMELL_KINDS], st));
+    CU(cudaMemsetAsync(d_head.p, 0, 4 * L, st));
+    CU(cudaMemsetAsync(d_smell.p, 0, 2 * L, st));
+    k_line_parens<<<grid, 256, 0, st>>>(S.d, S.n, total, d_delta.as<int32_t>(), d_kind.as<uint8_t>());
+    k_stmt_kinds<<<(S.n * 32 + 127) / 128, 128, 0, st>>>(S.d, S.n, d_delta.as<int32_t>(), d_kind.as<uint8_t>());
+    if (ne)
+      k_case_heads<<<(ne + 255) / 256, 256, 0, st>>>(S.hev.as<tsm_header_event>(), ne, S.d.line_base, S.d.line_end, d_head.as<uint32_t>());
+    xscan(d_head.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), d_case_of.as<unsigned long long>(), st);
+    k_case_lines<<<grid, 256, 0, st>>>(d_head.as<uint32_t>(), nullptr, d_case_of.as<unsigned long long>(), nullptr, T,
+                                       d_first.as<uint32_t>(), nullptr);
+    CU(cudaEventRecord(c->diff_ev[EV_SMELL_LINES], st));
+    k_smell_lines<<<grid, 256, 0, st>>>(S.d, S.n, total, d_head.as<uint32_t>(), d_case_of.as<unsigned long long>(), d_lines.as<SmellLine>(),
+                                        d_tflag.as<uint32_t>());
+    CU(cudaEventRecord(c->diff_ev[EV_SMELL_TESTS], st));
+    xscan(d_tflag.as<uint32_t>(), ne, d_bsum.as<unsigned long long>(), d_tidx.as<unsigned long long>(), st);
+    if (ne) {
+      const SmellArgs a{S.d.line_base, (uint32_t)S.n, S.d.ext, d_kind.as<uint8_t>(), d_head.as<uint32_t>(), d_first.as<uint32_t>(), ne,
+                        d_tflag.as<uint32_t>(), d_tidx.as<unsigned long long>(), d_lines.as<SmellLine>(), d_hash.as<unsigned long long>(),
+                        d_aline.as<uint32_t>(), d_smell.as<uint16_t>(), d_tests.as<tsm_smell_test>()};
+      k_smell_tests<<<std::min((ne + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(a);
+    }
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_SMELL_END], st));
+    unsigned long long* pin = reinterpret_cast<unsigned long long*>(c->h_diff + 128);
+    CU(cudaMemcpyAsync(pin, d_tidx.as<unsigned long long>() + ne, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    c->launches += 10 + (ne ? 2 : 0);                      // parens, kinds, 2 x xscan (3 each), case lines, smell lines; heads, tests
+    const unsigned long long nt = *pin;
+    *n_tests = (int64_t)nt;
+    c->smell_ms[1] = elapsed_ms(c->diff_ev[EV_SMELL_KINDS], c->diff_ev[EV_SMELL_LINES]);
+    c->smell_ms[2] = elapsed_ms(c->diff_ev[EV_SMELL_LINES], c->diff_ev[EV_SMELL_TESTS]);
+    c->smell_ms[3] = elapsed_ms(c->diff_ev[EV_SMELL_TESTS], c->diff_ev[EV_SMELL_END]);
+    if ((line_smell && line_cap < (int64_t)total) || (tests && test_cap < (int64_t)nt)) return TSM_E_CAPACITY;
+    if (line_smell) CU(cudaMemcpyAsync(line_smell, d_smell.p, 2 * L, cudaMemcpyDeviceToHost, st));
+    if (tests && nt) CU(cudaMemcpyAsync(tests, d_tests.p, sizeof(tsm_smell_test) * nt, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    return TSM_OK;
+  }, &c->smell_ms[0], TSM_SCAN_HEADER_EVENTS);
+}
+
+extern "C" int tsm_smells_last_ms(tsm_ctx* c, float* ms4) {
+  if (!c || !ms4) return TSM_E_ARG;
+  for (int i = 0; i < 4; ++i) ms4[i] = c->smell_ms[i];
   return TSM_OK;
 }

@@ -1961,6 +1961,91 @@ static int cmd_clones(const std::vector<std::string>& roots, const std::string& 
   return 0;
 }
 
+// Test smells (docs/SPEC.md section 18): tsm_smells per batch (tests never cross files, so batches are independent).  stdout: per
+// root the files and the tests with each smell, and an <all> row; --out: one row per instance line, in file, header line, instance
+// line and smell order, lines 1-based; the statement is the stripped instance line (empty for the test-level smells).
+static int cmd_smells(const std::vector<std::string>& roots, const std::string& git_repo, const std::string& rev, bool all_files,
+                      const std::string& out_path, int64_t batch_bytes) {
+  static const char* const kSmellNames[TSM_N_SMELLS] = {"empty", "assertion_free", "duplicate_assert", "redundant_assert",
+                                                        "conditional_logic", "exception_handling", "sleepy", "print", "ignored"};
+  std::vector<FileEntry> files;
+  std::vector<std::string> names;
+  if (!git_repo.empty()) {
+    gitstore::Store gs;
+    std::string err;
+    if (!gs.open(git_repo, err)) die(err);
+    gitstore::Oid id; gitstore::Commit cm;
+    if (!gs.resolve(rev, id) || !gs.commit(id, cm)) die("cannot resolve revision " + rev);
+    walk_git(gs, cm.tree, "", all_files, files);
+    names.push_back(repo_name(git_repo));
+  } else {
+    for (size_t g = 0; g < roots.size(); ++g) { walk(roots[g], (int)g, all_files, files); names.push_back(repo_name(roots[g])); }
+  }
+  fprintf(stderr, "tosem-scan: %zu files selected under %zu root(s)\n", files.size(), names.size());
+  const size_t ng = names.size();
+  std::vector<std::vector<int64_t>> tot(ng + 1, std::vector<int64_t>(2 + TSM_N_SMELLS, 0));   // files, tests, tests per smell
+  std::ofstream os;
+  if (!out_path.empty()) { os.open(out_path, std::ios::binary); csv_row(os, {"repository", "fileName", "test", "line", "smell", "smellLine", "statement"}); }
+  std::vector<Batch> batches = plan_batches(files, all_of(files), batch_bytes, kBatchFiles);
+  scan_batches(files, batches, 0, (int32_t)ng, TSM_SCAN_HEADER_EVENTS, [&](const Batch& B, const Scanned& s) {
+    const int32_t nf = (int32_t)B.count();
+    const tsm_corpus c = B.corpus((int32_t)ng);
+    std::vector<int64_t> base((size_t)nf + 1);
+    int64_t lines = 0, nl = 0, nt = 0;                     // the batch's scan bounds both outputs: its lines, and its header
+    for (int32_t i = 0; i < nf; ++i) lines += s.stats[(size_t)i].n_lines;   // lines (each test starts at one), so one call fills them
+    std::vector<uint16_t> smell((size_t)std::max<int64_t>(lines, 1));
+    std::vector<tsm_smell_test> tests(std::max<size_t>(s.hev.size(), 1));
+    ck(tsm_smells(s.ctx, &c, base.data(), smell.data(), lines, &nl, tests.data(), (int64_t)s.hev.size(), &nt, nullptr), "tsm_smells");
+    for (int32_t i = 0; i < nf; ++i) { tot[(size_t)files[B.idx[(size_t)i]].grp][0]++; tot[ng][0]++; }
+    int32_t at_file = -1;
+    std::vector<uint32_t> start;                           // byte offset of every line of file at_file
+    for (int64_t t = 0; t < nt; ++t) {
+      const tsm_smell_test& r = tests[(size_t)t];
+      const FileEntry& fe = files[B.idx[(size_t)r.file]];
+      for (size_t g : {(size_t)fe.grp, ng}) {
+        tot[g][1]++;
+        for (int k = 0; k < TSM_N_SMELLS; ++k) tot[g][2 + (size_t)k] += (r.smells >> k) & 1;
+      }
+      if (!os.is_open() || !r.smells) continue;
+      const uint8_t* p = B.arena.get() + B.off[(size_t)r.file];
+      const uint32_t len = (uint32_t)B.len[(size_t)r.file];
+      if (at_file != r.file) {
+        at_file = r.file; start.assign(1, 0);
+        for (uint32_t q = 0; q < len; ++q) if (p[q] == '\n') start.push_back(q + 1);
+      }
+      auto line_end = [&](int64_t l) { return (size_t)l + 1 < start.size() ? start[(size_t)l + 1] - 1 : len; };
+      auto stripped = [&](int64_t l) {
+        uint32_t b = start[(size_t)l], z = line_end(l);
+        while (b < z && is_w(p[b])) ++b;
+        while (z > b && is_w(p[z - 1])) --z;
+        return std::string((const char*)p + b, z - b);
+      };
+      const std::string name = case_name(fe.ext, p + start[(size_t)r.line], line_end(r.line) - start[(size_t)r.line]);
+      const int64_t g0 = base[(size_t)r.file] + r.line;
+      for (int64_t l = r.line; l < (int64_t)r.line + r.body_lines; ++l) {
+        const uint16_t bits = smell[(size_t)(g0 + l - r.line)];
+        for (int k = 0; k < TSM_N_SMELLS; ++k)
+          if ((bits >> k) & 1) {
+            const bool test_level = k == TSM_SMELL_EMPTY || k == TSM_SMELL_ASSERTION_FREE;
+            csv_row(os, {names[(size_t)fe.grp], fe.rel, name, std::to_string(r.line + 1), kSmellNames[k], std::to_string(l + 1),
+                         test_level ? std::string() : stripped(l)});
+          }
+      }
+    }
+  });
+  std::ostringstream so;
+  std::vector<std::string> head = {"repository", "files", "tests"};
+  for (const char* n : kSmellNames) head.push_back(n);
+  csv_row(so, head);
+  for (size_t g = 0; g <= ng; ++g) {
+    std::vector<std::string> row = {g < ng ? names[g] : "<all>"};
+    for (int64_t v : tot[g]) row.push_back(std::to_string(v));
+    csv_row(so, row);
+  }
+  fputs(so.str().c_str(), stdout);
+  return 0;
+}
+
 static void usage() {
   fprintf(stderr,
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
@@ -1975,6 +2060,9 @@ static void usage() {
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
           "       tosem-scan clones <project-root>... [--min-lines N] [--all-files] [--out F]\n"
           "       tosem-scan clones --git <repository> [--rev R] [--min-lines N] [--all-files] [--out F]\n"
+          "       tosem-scan smells <project-root>... [--all-files] [--batch-bytes N] [--out F]\n"
+          "       tosem-scan smells --git <repository> [--rev R] [--all-files] [--batch-bytes N] [--out F]\n"
+          "smells: per root the tests with each of nine test smells; --out F: one row per instance line (docs/SPEC.md section 18).\n"
           "--find-renames N (0..100): pair deleted and added files at least N %% similar, as git -M<N>%% does (docs/SPEC.md section 13).\n"
           "--cases F: one row per test case that a revision adds (A), deletes (D) or modifies (M) (docs/SPEC.md section 16).\n"
           "--assert-edits F: one row per deleted assertion line that an inserted one of the same hunk replaces, with their similarity\n"
@@ -2009,6 +2097,10 @@ int main(int argc, char** argv) {
     const long n = opt.count("--min-lines") ? strtol(opt["--min-lines"].c_str(), nullptr, 10) : 5;
     if (n < 1 || n > 1024) die("--min-lines needs a number of lines from 1 to 1024");
     return cmd_clones(pos, opt["--git"], opt.count("--rev") ? opt["--rev"] : "HEAD", (int)n, all_files, opt["--out"]);
+  }
+  if (cmd == "smells") {
+    if (pos.empty() == !opt.count("--git")) die("smells needs project roots or --git <repository>, not both");
+    return cmd_smells(pos, opt["--git"], opt.count("--rev") ? opt["--rev"] : "HEAD", all_files, opt["--out"], batch_bytes(kBatch, 1));
   }
   if (cmd == "body") { if (pos.empty()) die("body needs at least one project root"); return cmd_body(pos, opt["--out"], batch_bytes(kBatch, 1)); }
   int rename_pct = -1;                                     // --find-renames N (docs/SPEC.md section 13); -1 = off

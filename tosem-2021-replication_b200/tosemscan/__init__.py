@@ -32,6 +32,10 @@ DIFF_DETAIL = np.dtype([("hunks_add", "<i8"), ("hunks_del", "<i8"), ("hunks_mod"
 ORIGIN = np.dtype([("change", "<i4"), ("line", "<i4")])   # tsm_origin: the change that inserted a line, 1-based line there
 CASE = np.dtype([("pair", "<i4"), ("line", "<i4"), ("n_lines", "<i4"), ("n_assert", "<i4"), ("n_changed", "<i4"),
                  ("n_changed_assert", "<i4"), ("match", "<i4")])   # tsm_case: one test case of one side of a revision pair
+SMELL_TEST = np.dtype([("file", "<i4"), ("line", "<i4"), ("body_lines", "<i4"), ("n_assert", "<i4"), ("smells", "<u4"),
+                       ("n_instances", "<i4")])   # tsm_smell_test: one test of the corpus (docs/SPEC.md section 18)
+SMELLS = ["empty", "assertion_free", "duplicate_assert", "redundant_assert", "conditional_logic", "exception_handling", "sleepy",
+          "print", "ignored"]                   # bit k of tsm_smell_test.smells and of line_smell is SMELLS[k]
 ASSERT_EDIT = np.dtype([("rev", "<i8"), ("aev", "<i8"), ("score", "<i4"), ("_pad", "<i4")])   # tsm_assert_edit: event indices
 
 # every symbol include/tosemscan.h declares (tests check the library exports exactly these)
@@ -41,7 +45,7 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_diff_pairs_asserts", "tsm_diff_resident_asserts", "tsm_reduce", "tsm_host_alloc", "tsm_host_free", "tsm_layout", "tsm_gen_sizes",
            "tsm_gen_fill", "tsm_gen_edit", "tsm_gen_pair_sizes", "tsm_gen_pair_fill", "tsm_similarity", "tsm_similarity_last_ms",
            "tsm_diff_pairs_marks", "tsm_blame_pairs", "tsm_blame_last_ms", "tsm_clones", "tsm_clones_last_ms",
-           "tsm_diff_pairs_cases", "tsm_diff_pairs_assert_edits", "tsm_assert_edits_last_ms"]
+           "tsm_diff_pairs_cases", "tsm_diff_pairs_assert_edits", "tsm_assert_edits_last_ms", "tsm_smells", "tsm_smells_last_ms"]
 
 
 class TsmError(RuntimeError):
@@ -187,6 +191,11 @@ def lib():
         L.tsm_clones.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_int32, C.POINTER(_CloneResult), C.c_void_p]
         L.tsm_clones_last_ms.restype = C.c_int
         L.tsm_clones_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 3)]
+        L.tsm_smells.restype = C.c_int
+        L.tsm_smells.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
+                                 C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p]
+        L.tsm_smells_last_ms.restype = C.c_int
+        L.tsm_smells_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
         _lib = L
     return _lib
 
@@ -818,6 +827,33 @@ class Scanner:
             out["member"] = out["member"][:r.n_members]
             return out
         raise TsmError(TSM_E_CAPACITY, "tsm_clones")
+
+    def smells(self, corpus, stream=None, cap=None):
+        """Test smells (docs/SPEC.md section 18): a dict of numpy arrays line_base[n_files+1], line_smell[n_lines] (the smell bits
+        of every line: bit k is SMELLS[k]) and tests[n_tests] (SMELL_TEST records in global line order).  Arrays too small for
+        the lines or tests are sized from the counts and the call is made again (cap: the first guess of both)."""
+        n = corpus.n_files
+        cs = corpus.c_struct()
+        cl = ct = int(cap if cap is not None else 0)
+        for _ in range(2):
+            base = np.zeros(n + 1, np.int64)
+            smell = np.zeros(max(cl, 1), np.uint16)
+            tests = np.zeros(max(ct, 1), SMELL_TEST)
+            nl, nt = C.c_int64(), C.c_int64()
+            rc = lib().tsm_smells(self._ctx, C.byref(cs), _p(base), _p(smell), cl, C.byref(nl), _p(tests), ct, C.byref(nt), stream)
+            if rc == TSM_E_CAPACITY and (nl.value > cl or nt.value > ct):
+                cl, ct = int(nl.value), int(nt.value)
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_smells")
+            return {"line_base": base, "line_smell": smell[:nl.value], "tests": tests[:nt.value]}
+        raise TsmError(TSM_E_CAPACITY, "tsm_smells")
+
+    def smells_last_ms(self):
+        """Device time of the last smells call: [k_scan, kinds + case spans, k_smell_lines, k_smell_tests] in ms."""
+        ms = (C.c_float * 4)()
+        lib().tsm_smells_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
 
     def clones_last_ms(self):
         """Device time of the last clones call: [k_scan, grouping + classes, members + coverage] in ms."""
