@@ -327,6 +327,31 @@ int tsm_smells(tsm_ctx* ctx, const tsm_corpus* corpus, int64_t* line_base, uint1
                tsm_smell_test* tests, int64_t test_cap, int64_t* n_tests, void* stream);
 int tsm_smells_last_ms(tsm_ctx* ctx, float* ms4);
 
+/* Test-smell churn (docs/SPEC.md section 19): the section-16 cases and the section-18 tests of both sides of every revision pair,
+ * and per test how many of its smell instances the revision adds (new side) or removes (old side).  cases is filled exactly as
+ * tsm_diff_pairs_cases fills it.  old_tests / new_tests are the tsm_smell_test records of tsm_smells over each side's corpus
+ * alone, with file = the pair index; old_churn / new_churn hold one tsm_test_churn per test, in the same order:
+ *   case_idx      index of the test's case among the cases of its side (the case that starts at its header line)
+ *   instances[k]  body lines of the test with smell bit k (their sum is n_instances)
+ *   churned[k]    those of them that are added instances (new side) or removed instances (old side): the line is inserted
+ *                 (deleted), or it is kept and the corresponding line of the other side (section 14) lacks bit k.
+ * Any output pointer may be NULL (it is skipped).  cases.n_old / n_new, n_old_tests and n_new_tests are always set; if a given
+ * output's cap is smaller than its count, the call returns TSM_E_CAPACITY with all four set (and no diff run): size the arrays
+ * and call again.  added / removed / detail are those of tsm_diff_pairs_detail (detail may be NULL).  n_files = 0 is legal.
+ * Kernels: k_scan with header events, per side the case spans and the smell stage of tsm_smells, the diff of
+ * tsm_diff_pairs_marks, the case kernels of tsm_diff_pairs_cases and k_smell_churn per side (csrc/tsm_smell_kernels.cuh).
+ * tsm_diff_smells_last_ms: device time of the last call, ms4 = { k_scan over both sides, the smell stage of both sides (case
+ * spans included), k_diff_small + k_myers + k_myers_trace, case records + k_smell_churn }. */
+typedef struct tsm_test_churn { int32_t case_idx; int32_t instances[TSM_N_SMELLS]; int32_t churned[TSM_N_SMELLS]; } tsm_test_churn;
+typedef struct tsm_diff_smells {
+  tsm_diff_cases cases;
+  tsm_smell_test* old_tests; tsm_test_churn* old_churn; int64_t old_test_cap; int64_t n_old_tests;
+  tsm_smell_test* new_tests; tsm_test_churn* new_churn; int64_t new_test_cap; int64_t n_new_tests;
+} tsm_diff_smells;
+int tsm_diff_pairs_smells(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                          tsm_diff_detail* detail, tsm_diff_smells* out, void* stream);
+int tsm_diff_smells_last_ms(tsm_ctx* ctx, float* ms4);
+
 /* Body statements (docs/SPEC.md section 10; Important-files/ML-Analysis-v4.xlsx!Apollo:R2-R26, golden G2): the
  * kind of every line of every file - 0 blank, 1 first line of a statement, 2 continuation (lines
  * are joined while the parentheses are open).  line_base[n_files+1] and *n_lines are always filled;

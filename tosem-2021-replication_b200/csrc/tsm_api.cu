@@ -103,6 +103,7 @@ struct tsm_ctx {
   float sim_ms[3] = {0, 0, 0};             // k_scan over both sides, sort / merge, k_similarity of the last tsm_similarity
   float clone_ms[3] = {0, 0, 0};           // k_scan, grouping + classes, members + coverage of the last tsm_clones
   float smell_ms[4] = {0, 0, 0, 0};        // k_scan, kinds + case spans, k_smell_lines, k_smell_tests of the last tsm_smells
+  float churn_ms[4] = {0, 0, 0, 0};        // k_scan, smell stages, the diff, case records + k_smell_churn of the last tsm_diff_pairs_smells
   float edit_ms[3] = {0, 0, 0};            // k_scan, the diff, compact to pairing (host clock) of the last assertion-edit call
   cudaEvent_t blame_ev[2] = {};            // around k_blame (tsm_blame_last_ms)
   float blame_ms = 0;
@@ -1349,9 +1350,74 @@ extern "C" int tsm_diff_pairs_marks(tsm_ctx* c, const tsm_corpus* olds, const ts
 }
 
 // ------------------------------------------------------------------------------------- SPEC section 16 test-case churn
+// The case spans of one side whose line records and header events exist: k_case_heads (head[l] = 1 on header lines), xscan
+// of the heads (case_of: the case of every header line, cases numbered in line order) and k_case_lines (first[case] = its
+// header line).  bsum holds total / XS_TILE + 4 u64.
+struct CaseSpans { DevBuf head, case_of, first; uint32_t n_cases = 0; };
+
+static int case_spans(const HostSide& h, CaseSpans& sp, DevBuf& bsum, int& launches, cudaStream_t st) {
+  const uint32_t T = (uint32_t)h.total, ne = h.hc.n_hev;
+  const size_t L = (size_t)h.total;
+  sp.n_cases = ne;
+  if (!sp.head.alloc(4 * L) || !sp.case_of.alloc(8 * (L + 1)) || !sp.first.alloc(4 * ((size_t)ne + 1))) return TSM_E_CUDA;
+  CU(cudaMemsetAsync(sp.head.p, 0, 4 * L, st));
+  if (ne)
+    k_case_heads<<<(ne + 255) / 256, 256, 0, st>>>(h.hev.as<tsm_header_event>(), ne, h.d.line_base, h.d.line_end, sp.head.as<uint32_t>());
+  xscan(sp.head.as<uint32_t>(), T, bsum.as<unsigned long long>(), sp.case_of.as<unsigned long long>(), st);
+  if (T)
+    k_case_lines<<<(T + 255) / 256, 256, 0, st>>>(sp.head.as<uint32_t>(), nullptr, sp.case_of.as<unsigned long long>(), nullptr, T,
+                                                  sp.first.as<uint32_t>(), nullptr);
+  CU(cudaGetLastError());
+  launches += (ne ? 1 : 0) + (T ? 4 : 0);
+  return TSM_OK;
+}
+
+// The cases of both sides of the revision pairs: their spans before the marks diff (pair_case_spans), their records behind it
+// (case_records): per side k_case_kept and xscan of the kept lines (rank: the kept rank of every line), k_case_lines for
+// by_rank (the kept line of every rank: the old side's always, the new side's when asked for) and k_case_reduce (the new
+// side's step-1 match reads the old side's by_rank, head and case_of).
+struct PairCases { CaseSpans sp[2]; DevBuf kept[2], rank[2], by_rank[2], cases[2], bsum; };
+
+static int pair_case_spans(const HostSidePair& P, PairCases& pc, int& launches, cudaStream_t st) {
+  if (!pc.bsum.alloc(sizeof(unsigned long long) * ((size_t)std::max(P.A.total, P.B.total) / XS_TILE + 4))) return TSM_E_CUDA;
+  const int rc = case_spans(P.A, pc.sp[0], pc.bsum, launches, st);
+  return rc == TSM_OK ? case_spans(P.B, pc.sp[1], pc.bsum, launches, st) : rc;
+}
+
+static int case_records(tsm_ctx* c, const HostSidePair& P, PairCases& pc, bool new_by_rank, int& launches, cudaStream_t st) {
+  const HostSide* side[2] = {&P.A, &P.B};
+  for (int s = 0; s < 2; ++s) {
+    const HostSide& h = *side[s];
+    const uint32_t total = (uint32_t)h.total;
+    const bool by_rank = s == 0 || new_by_rank;
+    if (!pc.kept[s].alloc(sizeof(uint32_t) * (size_t)total) || !pc.rank[s].alloc(sizeof(unsigned long long) * ((size_t)total + 1)) ||
+        !pc.cases[s].alloc(sizeof(tsm_case) * (size_t)pc.sp[s].n_cases) || (by_rank && !pc.by_rank[s].alloc(sizeof(uint32_t) * (size_t)total)))
+      return TSM_E_CUDA;
+    if (total) k_case_kept<<<(total + 255) / 256, 256, 0, st>>>(h.line_mark.as<uint8_t>(), total, pc.kept[s].as<uint32_t>());
+    xscan(pc.kept[s].as<uint32_t>(), total, pc.bsum.as<unsigned long long>(), pc.rank[s].as<unsigned long long>(), st);
+    if (total && by_rank)
+      k_case_lines<<<(total + 255) / 256, 256, 0, st>>>(pc.sp[s].head.as<uint32_t>(), pc.kept[s].as<uint32_t>(),
+                                                        pc.sp[s].case_of.as<unsigned long long>(), pc.rank[s].as<unsigned long long>(),
+                                                        total, pc.sp[s].first.as<uint32_t>(), pc.by_rank[s].as<uint32_t>());
+    launches += total ? 4 + (by_rank ? 1 : 0) : 0;
+  }
+  for (int s = 0; s < 2; ++s) {
+    const HostSide& h = *side[s];
+    const uint32_t ne = pc.sp[s].n_cases;
+    if (!ne) continue;
+    const CaseSide cs{h.d.line_base, (uint32_t)P.n, h.d.line_flag, h.line_mark.as<uint8_t>(), pc.sp[s].first.as<uint32_t>(), ne};
+    const bool nw = s == 1;
+    k_case_reduce<<<std::min((ne + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(
+        cs, pc.rank[s].as<unsigned long long>(), nw ? pc.by_rank[0].as<uint32_t>() : nullptr, nw ? pc.sp[0].head.as<uint32_t>() : nullptr,
+        nw ? pc.sp[0].case_of.as<unsigned long long>() : nullptr, pc.cases[s].as<tsm_case>());
+    ++launches;
+  }
+  CU(cudaGetLastError());
+  return TSM_OK;
+}
+
 // The line records of both sides with their header events (the case counts, so the capacity check comes before the diff),
-// k_case_heads per side, the marks diff, then per side k_case_kept, xscan of the heads and of the kept lines, k_case_lines
-// (old side first: the new side's k_case_reduce reads old_by_rank) and k_case_reduce (csrc/tsm_case_kernels.cuh).
+// the case spans, the marks diff and the case records (csrc/tsm_case_kernels.cuh).
 extern "C" int tsm_diff_pairs_cases(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
                                     tsm_diff_detail* detail, tsm_diff_cases* out, void* stream) {
   if (!c || !olds || !news || !added || !removed || !out || olds->n_files != news->n_files) return TSM_E_ARG;
@@ -1364,7 +1430,7 @@ extern "C" int tsm_diff_pairs_cases(tsm_ctx* c, const tsm_corpus* olds, const ts
   CallScope call(c, st);
   CU(call.status);
   HostSidePair P;
-  DevBuf d_head[2], d_kept[2], d_case_of[2], d_rank[2], d_first[2], d_cases[2], d_by_rank, d_bsum;
+  PairCases pc;
   SyncGuard guard(st);
   rc = pair_upload(olds, news, false, P, st);
   if (rc == TSM_OK) rc = pair_records(c, P, &c->diff_ms[0], false, st, TSM_SCAN_HEADER_EVENTS);
@@ -1372,54 +1438,14 @@ extern "C" int tsm_diff_pairs_cases(tsm_ctx* c, const tsm_corpus* olds, const ts
   out->n_old = P.A.hc.n_hev; out->n_new = P.B.hc.n_hev;
   if (out->old_cap < out->n_old || out->new_cap < out->n_new) return TSM_E_CAPACITY;
   if ((out->n_old && !out->old_cases) || (out->n_new && !out->new_cases)) return TSM_E_ARG;
-  HostSide* side[2] = {&P.A, &P.B};
-  tsm_case* const h_out[2] = {out->old_cases, out->new_cases};
   int launches = 0;
-  for (int s = 0; s < 2; ++s) {
-    const HostSide& h = *side[s];
-    const size_t total = (size_t)h.total, ne = h.hc.n_hev;
-    if (!d_head[s].alloc(sizeof(uint32_t) * total) || !d_kept[s].alloc(sizeof(uint32_t) * total) ||
-        !d_case_of[s].alloc(sizeof(unsigned long long) * (total + 1)) || !d_rank[s].alloc(sizeof(unsigned long long) * (total + 1)) ||
-        !d_first[s].alloc(sizeof(uint32_t) * ne) || !d_cases[s].alloc(sizeof(tsm_case) * ne))
-      return TSM_E_CUDA;
-    CU(cudaMemsetAsync(d_head[s].p, 0, sizeof(uint32_t) * total, st));
-    if (ne) {
-      k_case_heads<<<(unsigned)((ne + 255) / 256), 256, 0, st>>>(h.hev.as<tsm_header_event>(), (uint32_t)ne, h.d.line_base, h.d.line_end,
-                                                                 d_head[s].as<uint32_t>());
-      ++launches;
-    }
-  }
-  CU(cudaGetLastError());
-  if (!d_by_rank.alloc(sizeof(uint32_t) * (size_t)P.A.total) ||
-      !d_bsum.alloc(sizeof(unsigned long long) * ((size_t)std::max(P.A.total, P.B.total) / XS_TILE + 4)))
-    return TSM_E_CUDA;
-  rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
+  rc = pair_case_spans(P, pc, launches, st);
+  if (rc == TSM_OK) rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
+  if (rc == TSM_OK) rc = case_records(c, P, pc, false, launches, st);
   if (rc != TSM_OK) return rc;
-  for (int s = 0; s < 2; ++s) {
-    const HostSide& h = *side[s];
-    const uint32_t total = (uint32_t)h.total;
-    if (total) k_case_kept<<<(total + 255) / 256, 256, 0, st>>>(h.line_mark.as<uint8_t>(), total, d_kept[s].as<uint32_t>());
-    xscan(d_head[s].as<uint32_t>(), total, d_bsum.as<unsigned long long>(), d_case_of[s].as<unsigned long long>(), st);
-    xscan(d_kept[s].as<uint32_t>(), total, d_bsum.as<unsigned long long>(), d_rank[s].as<unsigned long long>(), st);
-    if (total)
-      k_case_lines<<<(total + 255) / 256, 256, 0, st>>>(d_head[s].as<uint32_t>(), d_kept[s].as<uint32_t>(), d_case_of[s].as<unsigned long long>(),
-                                                        d_rank[s].as<unsigned long long>(), total, d_first[s].as<uint32_t>(),
-                                                        s == 0 ? d_by_rank.as<uint32_t>() : nullptr);
-    launches += total ? 8 : 0;
-  }
-  for (int s = 0; s < 2; ++s) {
-    const HostSide& h = *side[s];
-    const uint32_t ne = h.hc.n_hev;
-    if (!ne) continue;
-    const CaseSide cs{h.d.line_base, (uint32_t)n, h.d.line_flag, h.line_mark.as<uint8_t>(), d_first[s].as<uint32_t>(), ne};
-    const bool nw = s == 1;
-    k_case_reduce<<<std::min((ne + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(
-        cs, d_rank[s].as<unsigned long long>(), nw ? d_by_rank.as<uint32_t>() : nullptr, nw ? d_head[0].as<uint32_t>() : nullptr,
-        nw ? d_case_of[0].as<unsigned long long>() : nullptr, d_cases[s].as<tsm_case>());
-    ++launches;
-    CU(cudaMemcpyAsync(h_out[s], d_cases[s].p, sizeof(tsm_case) * ne, cudaMemcpyDeviceToHost, st));
-  }
-  CU(cudaGetLastError());
+  tsm_case* const h_out[2] = {out->old_cases, out->new_cases};
+  for (int s = 0; s < 2; ++s)
+    if (pc.sp[s].n_cases) CU(cudaMemcpyAsync(h_out[s], pc.cases[s].p, sizeof(tsm_case) * pc.sp[s].n_cases, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   c->launches += launches;
   return TSM_OK;
@@ -2007,10 +2033,46 @@ extern "C" int tsm_clones_last_ms(tsm_ctx* c, float* ms3) {
 }
 
 // ------------------------------------------------------------------------------------- SPEC section 18 test smells
-// The line records of the corpus with its header events (line_records), then the section-10 kinds (k_line_parens, k_stmt_kinds),
-// the case spans (k_case_heads, xscan of the heads, k_case_lines), k_smell_lines (with the test flag of every case), xscan of
-// the test flags (dense test numbers) and k_smell_tests.  One synchronisation at the end reads the test count; the outputs are
-// copied when they fit.
+// The smell stage over one side whose line records (with header events) and case spans exist: the section-10 kinds
+// (k_line_parens, k_stmt_kinds), k_smell_lines (with the test flag of every case), xscan of the test flags (dense test numbers;
+// the test count lands at tidx[n_cases]) and k_smell_tests.  Events EV_SMELL_LINES, EV_SMELL_TESTS and EV_SMELL_END mark its
+// parts.  bsum holds total / XS_TILE + 4 u64.
+struct SmellBufs { DevBuf delta, kind, tflag, tidx, lines, hash, aline, smell, tests; };
+
+static int smell_stage(tsm_ctx* c, const HostSide& S, const CaseSpans& sp, DevBuf& bsum, SmellBufs& m, int& launches, cudaStream_t st) {
+  const unsigned long long total = S.total;
+  const size_t L = (size_t)total;
+  const uint32_t ne = sp.n_cases;
+  if (!m.delta.alloc(4 * L) || !m.kind.alloc(L) || !m.tflag.alloc(4 * ((size_t)ne + 1)) || !m.tidx.alloc(8 * ((size_t)ne + 1)) ||
+      !m.lines.alloc(sizeof(SmellLine) * L) || !m.hash.alloc(8 * L) || !m.aline.alloc(4 * L) || !m.smell.alloc(2 * L) ||
+      !m.tests.alloc(sizeof(tsm_smell_test) * ((size_t)ne + 1)))
+    return TSM_E_CUDA;
+  const unsigned grid = (unsigned)((L + 255) / 256);
+  CU(cudaMemsetAsync(m.smell.p, 0, 2 * L, st));
+  if (L) {
+    k_line_parens<<<grid, 256, 0, st>>>(S.d, S.n, total, m.delta.as<int32_t>(), m.kind.as<uint8_t>());
+    k_stmt_kinds<<<(S.n * 32 + 127) / 128, 128, 0, st>>>(S.d, S.n, m.delta.as<int32_t>(), m.kind.as<uint8_t>());
+  }
+  CU(cudaEventRecord(c->diff_ev[EV_SMELL_LINES], st));
+  if (L)
+    k_smell_lines<<<grid, 256, 0, st>>>(S.d, S.n, total, sp.head.as<uint32_t>(), sp.case_of.as<unsigned long long>(), m.lines.as<SmellLine>(),
+                                        m.tflag.as<uint32_t>());
+  CU(cudaEventRecord(c->diff_ev[EV_SMELL_TESTS], st));
+  xscan(m.tflag.as<uint32_t>(), ne, bsum.as<unsigned long long>(), m.tidx.as<unsigned long long>(), st);
+  if (ne) {
+    const SmellArgs a{S.d.line_base, (uint32_t)S.n, S.d.ext, m.kind.as<uint8_t>(), sp.head.as<uint32_t>(), sp.first.as<uint32_t>(), ne,
+                      m.tflag.as<uint32_t>(), m.tidx.as<unsigned long long>(), m.lines.as<SmellLine>(), m.hash.as<unsigned long long>(),
+                      m.aline.as<uint32_t>(), m.smell.as<uint16_t>(), m.tests.as<tsm_smell_test>()};
+    k_smell_tests<<<std::min((ne + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(a);
+  }
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(c->diff_ev[EV_SMELL_END], st));
+  launches += (L ? 6 : 3) + (ne ? 1 : 0);                 // parens, kinds, smell lines, xscan (3); tests
+  return TSM_OK;
+}
+
+// The line records of the corpus with its header events (line_records), then the case spans and the smell stage.  One
+// synchronisation at the end reads the test count; the outputs are copied when they fit.
 extern "C" int tsm_smells(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, uint16_t* line_smell, int64_t line_cap, int64_t* n_lines,
                           tsm_smell_test* tests, int64_t test_cap, int64_t* n_tests, void* stream) {
   if (!c || !k || !n_lines || !n_tests || line_cap < 0 || test_cap < 0 || k->n_files < 0) return TSM_E_ARG;
@@ -2021,50 +2083,28 @@ extern "C" int tsm_smells(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, u
   std::vector<int64_t> own_base;
   if (!line_base) { own_base.resize((size_t)nf + 1); line_base = own_base.data(); }
   return line_records(c, k, true, line_base, INT64_MAX, n_lines, stream, [&](const HostSide& S, unsigned long long total, cudaStream_t st) -> int {
-    const uint32_t T = (uint32_t)total, ne = S.hc.n_hev;
     const size_t L = (size_t)total;
-    DevBuf d_delta, d_kind, d_head, d_case_of, d_first, d_tflag, d_tidx, d_bsum, d_lines, d_hash, d_aline, d_smell, d_tests;
-    if (!d_delta.alloc(4 * L) || !d_kind.alloc(L) || !d_head.alloc(4 * L) || !d_case_of.alloc(8 * (L + 1)) || !d_first.alloc(4 * ((size_t)ne + 1)) ||
-        !d_tflag.alloc(4 * ((size_t)ne + 1)) || !d_tidx.alloc(8 * ((size_t)ne + 1)) || !d_bsum.alloc(8 * (L / XS_TILE + 4)) ||
-        !d_lines.alloc(sizeof(SmellLine) * L) || !d_hash.alloc(8 * L) || !d_aline.alloc(4 * L) || !d_smell.alloc(2 * L) ||
-        !d_tests.alloc(sizeof(tsm_smell_test) * ((size_t)ne + 1)))
-      return TSM_E_CUDA;
-    const unsigned grid = (unsigned)((L + 255) / 256);
+    CaseSpans sp;
+    SmellBufs m;
+    DevBuf d_bsum;
+    if (!d_bsum.alloc(8 * (L / XS_TILE + 4))) return TSM_E_CUDA;
+    int launches = 0;
     CU(cudaEventRecord(c->diff_ev[EV_SMELL_KINDS], st));
-    CU(cudaMemsetAsync(d_head.p, 0, 4 * L, st));
-    CU(cudaMemsetAsync(d_smell.p, 0, 2 * L, st));
-    k_line_parens<<<grid, 256, 0, st>>>(S.d, S.n, total, d_delta.as<int32_t>(), d_kind.as<uint8_t>());
-    k_stmt_kinds<<<(S.n * 32 + 127) / 128, 128, 0, st>>>(S.d, S.n, d_delta.as<int32_t>(), d_kind.as<uint8_t>());
-    if (ne)
-      k_case_heads<<<(ne + 255) / 256, 256, 0, st>>>(S.hev.as<tsm_header_event>(), ne, S.d.line_base, S.d.line_end, d_head.as<uint32_t>());
-    xscan(d_head.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), d_case_of.as<unsigned long long>(), st);
-    k_case_lines<<<grid, 256, 0, st>>>(d_head.as<uint32_t>(), nullptr, d_case_of.as<unsigned long long>(), nullptr, T,
-                                       d_first.as<uint32_t>(), nullptr);
-    CU(cudaEventRecord(c->diff_ev[EV_SMELL_LINES], st));
-    k_smell_lines<<<grid, 256, 0, st>>>(S.d, S.n, total, d_head.as<uint32_t>(), d_case_of.as<unsigned long long>(), d_lines.as<SmellLine>(),
-                                        d_tflag.as<uint32_t>());
-    CU(cudaEventRecord(c->diff_ev[EV_SMELL_TESTS], st));
-    xscan(d_tflag.as<uint32_t>(), ne, d_bsum.as<unsigned long long>(), d_tidx.as<unsigned long long>(), st);
-    if (ne) {
-      const SmellArgs a{S.d.line_base, (uint32_t)S.n, S.d.ext, d_kind.as<uint8_t>(), d_head.as<uint32_t>(), d_first.as<uint32_t>(), ne,
-                        d_tflag.as<uint32_t>(), d_tidx.as<unsigned long long>(), d_lines.as<SmellLine>(), d_hash.as<unsigned long long>(),
-                        d_aline.as<uint32_t>(), d_smell.as<uint16_t>(), d_tests.as<tsm_smell_test>()};
-      k_smell_tests<<<std::min((ne + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(a);
-    }
-    CU(cudaGetLastError());
-    CU(cudaEventRecord(c->diff_ev[EV_SMELL_END], st));
+    int rc = case_spans(S, sp, d_bsum, launches, st);
+    if (rc == TSM_OK) rc = smell_stage(c, S, sp, d_bsum, m, launches, st);
+    if (rc != TSM_OK) return rc;
     unsigned long long* pin = reinterpret_cast<unsigned long long*>(c->h_diff + 128);
-    CU(cudaMemcpyAsync(pin, d_tidx.as<unsigned long long>() + ne, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(pin, m.tidx.as<unsigned long long>() + sp.n_cases, 8, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    c->launches += 10 + (ne ? 2 : 0);                      // parens, kinds, 2 x xscan (3 each), case lines, smell lines; heads, tests
+    c->launches += launches;
     const unsigned long long nt = *pin;
     *n_tests = (int64_t)nt;
     c->smell_ms[1] = elapsed_ms(c->diff_ev[EV_SMELL_KINDS], c->diff_ev[EV_SMELL_LINES]);
     c->smell_ms[2] = elapsed_ms(c->diff_ev[EV_SMELL_LINES], c->diff_ev[EV_SMELL_TESTS]);
     c->smell_ms[3] = elapsed_ms(c->diff_ev[EV_SMELL_TESTS], c->diff_ev[EV_SMELL_END]);
     if ((line_smell && line_cap < (int64_t)total) || (tests && test_cap < (int64_t)nt)) return TSM_E_CAPACITY;
-    if (line_smell) CU(cudaMemcpyAsync(line_smell, d_smell.p, 2 * L, cudaMemcpyDeviceToHost, st));
-    if (tests && nt) CU(cudaMemcpyAsync(tests, d_tests.p, sizeof(tsm_smell_test) * nt, cudaMemcpyDeviceToHost, st));
+    if (line_smell) CU(cudaMemcpyAsync(line_smell, m.smell.p, 2 * L, cudaMemcpyDeviceToHost, st));
+    if (tests && nt) CU(cudaMemcpyAsync(tests, m.tests.p, sizeof(tsm_smell_test) * nt, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     return TSM_OK;
   }, &c->smell_ms[0], TSM_SCAN_HEADER_EVENTS);
@@ -2073,5 +2113,91 @@ extern "C" int tsm_smells(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, u
 extern "C" int tsm_smells_last_ms(tsm_ctx* c, float* ms4) {
   if (!c || !ms4) return TSM_E_ARG;
   for (int i = 0; i < 4; ++i) ms4[i] = c->smell_ms[i];
+  return TSM_OK;
+}
+
+// ------------------------------------------------------------------------------------- SPEC section 19 test-smell churn
+// The line records of both sides with their header events, per side the case spans and the smell stage, one synchronisation
+// for the case and test counts (the capacity check comes before the diff), the marks diff, the case records (with the new
+// side's by_rank) and k_smell_churn per side.  Slots 0 and 1 of diff_ev (those of the old side's scan, already read) time the
+// smell stages and, behind the diff, the case records and churn.
+extern "C" int tsm_diff_pairs_smells(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                                     tsm_diff_detail* detail, tsm_diff_smells* out, void* stream) {
+  if (!c || !olds || !news || !added || !removed || !out || olds->n_files != news->n_files || out->cases.old_cap < 0 ||
+      out->cases.new_cap < 0 || out->old_test_cap < 0 || out->new_test_cap < 0)
+    return TSM_E_ARG;
+  const int32_t n = olds->n_files;
+  for (float& v : c->churn_ms) v = 0;
+  out->cases.n_old = out->cases.n_new = out->n_old_tests = out->n_new_tests = 0;
+  if (n == 0) return TSM_OK;
+  int rc = check_sides({olds, news}, n, true);
+  if (rc != TSM_OK) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  CallScope call(c, st);
+  CU(call.status);
+  HostSidePair P;
+  PairCases pc;
+  SmellBufs sb[2];
+  DevBuf d_churn[2];
+  SyncGuard guard(st);
+  rc = pair_upload(olds, news, false, P, st);
+  if (rc == TSM_OK) rc = pair_records(c, P, &c->diff_ms[0], false, st, TSM_SCAN_HEADER_EVENTS);
+  if (rc != TSM_OK) return rc;
+  c->churn_ms[0] = c->diff_ms[0];
+  const HostSide* side[2] = {&P.A, &P.B};
+  int launches = 0;
+  CU(cudaEventRecord(c->diff_ev[0], st));
+  rc = pair_case_spans(P, pc, launches, st);
+  for (int s = 0; s < 2 && rc == TSM_OK; ++s) rc = smell_stage(c, *side[s], pc.sp[s], pc.bsum, sb[s], launches, st);
+  if (rc != TSM_OK) return rc;
+  CU(cudaEventRecord(c->diff_ev[1], st));
+  unsigned long long* pin = reinterpret_cast<unsigned long long*>(c->h_diff + 128);
+  for (int s = 0; s < 2; ++s)
+    CU(cudaMemcpyAsync(pin + s, sb[s].tidx.as<unsigned long long>() + pc.sp[s].n_cases, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  c->churn_ms[1] = elapsed_ms(c->diff_ev[0], c->diff_ev[1]);
+  const uint32_t nt[2] = {(uint32_t)pin[0], (uint32_t)pin[1]};
+  out->cases.n_old = pc.sp[0].n_cases; out->cases.n_new = pc.sp[1].n_cases;
+  out->n_old_tests = nt[0]; out->n_new_tests = nt[1];
+  if ((out->cases.old_cases && out->cases.old_cap < out->cases.n_old) || (out->cases.new_cases && out->cases.new_cap < out->cases.n_new) ||
+      ((out->old_tests || out->old_churn) && out->old_test_cap < (int64_t)nt[0]) ||
+      ((out->new_tests || out->new_churn) && out->new_test_cap < (int64_t)nt[1]))
+    return TSM_E_CAPACITY;
+  rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
+  if (rc != TSM_OK) return rc;
+  c->churn_ms[2] = c->diff_ms[1] + c->diff_ms[2];
+  CU(cudaEventRecord(c->diff_ev[0], st));
+  rc = case_records(c, P, pc, true, launches, st);
+  if (rc != TSM_OK) return rc;
+  for (int s = 0; s < 2; ++s) {
+    if (!d_churn[s].alloc(sizeof(tsm_test_churn) * (size_t)nt[s])) return TSM_E_CUDA;
+    if (!nt[s]) continue;
+    const int o = 1 - s;
+    const ChurnSide cs{side[s]->d.line_base, sb[s].tests.as<tsm_smell_test>(), nt[s], sb[s].smell.as<uint16_t>(),
+                       side[s]->line_mark.as<uint8_t>(), pc.rank[s].as<unsigned long long>(), pc.sp[s].case_of.as<unsigned long long>(),
+                       sb[o].smell.as<uint16_t>(), pc.by_rank[o].as<uint32_t>(), d_churn[s].as<tsm_test_churn>()};
+    k_smell_churn<<<std::min((nt[s] + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(cs);
+    ++launches;
+  }
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(c->diff_ev[1], st));
+  tsm_case* const h_cases[2] = {out->cases.old_cases, out->cases.new_cases};
+  tsm_smell_test* const h_tests[2] = {out->old_tests, out->new_tests};
+  tsm_test_churn* const h_churn[2] = {out->old_churn, out->new_churn};
+  for (int s = 0; s < 2; ++s) {
+    if (h_cases[s] && pc.sp[s].n_cases)
+      CU(cudaMemcpyAsync(h_cases[s], pc.cases[s].p, sizeof(tsm_case) * pc.sp[s].n_cases, cudaMemcpyDeviceToHost, st));
+    if (h_tests[s] && nt[s]) CU(cudaMemcpyAsync(h_tests[s], sb[s].tests.p, sizeof(tsm_smell_test) * nt[s], cudaMemcpyDeviceToHost, st));
+    if (h_churn[s] && nt[s]) CU(cudaMemcpyAsync(h_churn[s], d_churn[s].p, sizeof(tsm_test_churn) * nt[s], cudaMemcpyDeviceToHost, st));
+  }
+  CU(cudaStreamSynchronize(st));
+  c->churn_ms[3] = elapsed_ms(c->diff_ev[0], c->diff_ev[1]);
+  c->launches += launches;
+  return TSM_OK;
+}
+
+extern "C" int tsm_diff_smells_last_ms(tsm_ctx* c, float* ms4) {
+  if (!c || !ms4) return TSM_E_ARG;
+  for (int i = 0; i < 4; ++i) ms4[i] = c->churn_ms[i];
   return TSM_OK;
 }

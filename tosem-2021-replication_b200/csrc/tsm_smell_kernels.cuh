@@ -10,6 +10,8 @@
 //                   the brace deltas), the docstring state by a parity scan of ballots, the line-level instances, then the
 //                   duplicate assertions by comparing every assertion hash with every earlier one of the test through
 //                   shuffles, 32 x 32 per tile pair (O(A^2 / 32) per test); lane 0 walks the '@' lines above the header.
+//   k_smell_churn   persistent warps, one test of one side of revision pairs at a time, 32 body lines per round: per smell the
+//                   instance lines and those the revision adds or removes (docs/SPEC.md section 19), by ballots.
 #pragma once
 #include "tsm_device.cuh"
 #include "tsm_diff_kernels.cuh"
@@ -358,6 +360,40 @@ __global__ void __launch_bounds__(256) k_smell_tests(SmellArgs a) {
       a.out[a.tidx[c]] = tsm_smell_test{(int32_t)lo, (int32_t)(b - fb), (int32_t)(bend - b), (int32_t)na, smells,
                                         (int32_t)(ninst + ndup + __popc(hb))};
     }
+  }
+}
+
+// Smell churn of one side of the revision pairs (docs/SPEC.md section 19).  mark / rank: this side's edit marks and kept ranks;
+// other_smell / other_by_rank: the line_smell of the other side and its kept line of every rank.
+struct ChurnSide {
+  const unsigned long long* line_base; const tsm_smell_test* tests; uint32_t n_tests;
+  const uint16_t* line_smell; const uint8_t* mark; const unsigned long long* rank; const unsigned long long* case_of;
+  const uint16_t* other_smell; const uint32_t* other_by_rank; tsm_test_churn* out;
+};
+
+// Persistent warps, one test at a time, 32 body lines per round: the instances of a line are its smell bits, its churned
+// instances the bits the corresponding line of the other side lacks (all of them on a deleted or inserted line).  Lane k < 9
+// counts smell k from one ballot per smell and kind.
+__global__ void __launch_bounds__(256) k_smell_churn(ChurnSide s) {
+  const uint32_t lane = threadIdx.x & 31, warps = gridDim.x * (blockDim.x >> 5);
+  for (uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; t < s.n_tests; t += warps) {
+    const tsm_smell_test r = s.tests[t];
+    const uint32_t b = (uint32_t)s.line_base[r.file] + (uint32_t)r.line, e = b + (uint32_t)r.body_lines;
+    uint32_t ni = 0, nc = 0;
+    for (uint32_t base = b; base < e; base += 32) {
+      const uint32_t l = base + lane;
+      uint32_t bits = 0, churn = 0;
+      if (l < e && (bits = s.line_smell[l]) != 0)
+        churn = s.mark[l] ? bits : bits & ~(uint32_t)s.other_smell[s.other_by_rank[s.rank[l]]];
+#pragma unroll
+      for (uint32_t k = 0; k < TSM_N_SMELLS; ++k) {
+        const uint32_t mi = __ballot_sync(0xffffffffu, (bits >> k) & 1u), mc = __ballot_sync(0xffffffffu, (churn >> k) & 1u);
+        if (lane == k) { ni += __popc(mi); nc += __popc(mc); }
+      }
+    }
+    tsm_test_churn* o = s.out + t;
+    if (lane == 0) o->case_idx = (int32_t)s.case_of[b];
+    if (lane < TSM_N_SMELLS) { o->instances[lane] = (int32_t)ni; o->churned[lane] = (int32_t)nc; }
   }
 }
 

@@ -17,12 +17,12 @@
 //
 //   tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N]
 //   tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]
-//   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--find-renames N]
-//                     [--batch-bytes N]
+//   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--smells F]
+//                     [--find-renames N] [--batch-bytes N]
 //   tosem-scan body   <project-root>... [--batch-bytes N] [--out F]
 //   tosem-scan releases <snapshot-root>=<tag>... | --git <repository> [<revision>...]   [--batch-bytes N] [--out F]
 //   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F] [--cases F]
-//                      [--assert-edits F] [--find-renames N] [--batch-bytes N]
+//                      [--assert-edits F] [--smells F] [--find-renames N] [--batch-bytes N]
 //   tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]
 //   tosem-scan clones <project-root>... | --git <repository> [--rev R]   [--min-lines N] [--all-files] [--out F]
 // Every command that scans files does it with scan_batches: batches of at most --batch-bytes of arena (clones: all files in one),
@@ -1260,6 +1260,33 @@ static void diff_cases(tsm_ctx* ctx, const tsm_corpus& ca, const tsm_corpus& cn,
   }
 }
 
+// Test-smell churn (docs/SPEC.md section 19) of one diff call: the case records (as diff_cases), the tests of both sides and their
+// churn records (tsm_diff_pairs_smells), arrays grown to the counts the library reports when they are too small.
+struct SmellLists { std::vector<tsm_smell_test> olds, news; std::vector<tsm_test_churn> old_churn, new_churn; };
+static void diff_smells(tsm_ctx* ctx, const tsm_corpus& ca, const tsm_corpus& cn, int64_t* added, int64_t* removed,
+                        tsm_diff_detail* det, CaseLists& c, SmellLists& r) {
+  int64_t co = (int64_t)ca.off[ca.n_files] / 512 + 64, cc = (int64_t)cn.off[cn.n_files] / 512 + 64, to = co, tn = cc;
+  for (;;) {
+    c.olds.resize((size_t)co); c.news.resize((size_t)cc);
+    r.olds.resize((size_t)to); r.old_churn.resize((size_t)to); r.news.resize((size_t)tn); r.new_churn.resize((size_t)tn);
+    tsm_diff_smells o{{c.olds.data(), co, 0, c.news.data(), cc, 0}, r.olds.data(), r.old_churn.data(), to, 0,
+                      r.news.data(), r.new_churn.data(), tn, 0};
+    const int rc = tsm_diff_pairs_smells(ctx, &ca, &cn, added, removed, det, &o, nullptr);
+    if (rc == TSM_E_CAPACITY && (o.cases.n_old > co || o.cases.n_new > cc || o.n_old_tests > to || o.n_new_tests > tn)) {
+      co = std::max(co, o.cases.n_old); cc = std::max(cc, o.cases.n_new); to = std::max(to, o.n_old_tests); tn = std::max(tn, o.n_new_tests);
+      continue;
+    }
+    ck(rc, "tsm_diff_pairs_smells");
+    c.olds.resize((size_t)o.cases.n_old); c.news.resize((size_t)o.cases.n_new);
+    r.olds.resize((size_t)o.n_old_tests); r.old_churn.resize((size_t)o.n_old_tests);
+    r.news.resize((size_t)o.n_new_tests); r.new_churn.resize((size_t)o.n_new_tests);
+    return;
+  }
+}
+
+static const char* const kSmellNames[TSM_N_SMELLS] = {"empty", "assertion_free", "duplicate_assert", "redundant_assert",
+                                                      "conditional_logic", "exception_handling", "sleepy", "print", "ignored"};
+
 // The case name (docs/SPEC.md section 10) of every case of one side of a pair, from the header lines of the side's bytes.
 static std::vector<std::string> case_names(const uint8_t* base, int32_t size, int ext, const tsm_case* cs, size_t n) {
   std::vector<std::string> out;
@@ -1272,22 +1299,31 @@ static std::vector<std::string> case_names(const uint8_t* base, int32_t size, in
   return out;
 }
 
-// The --cases rows of one pair (docs/SPEC.md section 16) from its old cases oc[0, no) and new cases nc[0, nn), old case
-// index o_first being oc[0]: matches by kept header line come with the records, matches by name (once among the unmatched
-// cases of each side) are made here; then the D rows in old line order and the A and M rows in new line order.
+// The cases of one pair (docs/SPEC.md section 16): its old cases oc[0, no) and new cases nc[0, nn), old case index o_first being
+// oc[0], their names, and per new case the old case it matches (-1: none) and per old case whether one matches it.  Matches by
+// kept header line come with the records, matches by name (once among the unmatched cases of each side) are made here.
 struct CaseSide { const uint8_t* base; int32_t size; int ext; const std::string* path; };
+struct PairCaseMatch {
+  std::vector<std::string> na, nb; std::vector<int64_t> match; std::vector<char> used;
+  PairCaseMatch(const CaseSide& o, const CaseSide& nw, const tsm_case* oc, size_t no, const tsm_case* nc, size_t nn, size_t o_first)
+      : na(case_names(o.base, o.size, o.ext, oc, no)), nb(case_names(nw.base, nw.size, nw.ext, nc, nn)), match(nn, -1), used(no, 0) {
+    for (size_t j = 0; j < nn; ++j)
+      if (nc[j].match >= 0) { match[j] = nc[j].match - (int64_t)o_first; used[(size_t)match[j]] = 1; }
+    std::map<std::string, int64_t> cnt_new, cnt_old, old_of;
+    for (size_t j = 0; j < nn; ++j) if (match[j] < 0) ++cnt_new[nb[j]];
+    for (size_t k = 0; k < no; ++k) if (!used[k]) { ++cnt_old[na[k]]; old_of[na[k]] = (int64_t)k; }
+    for (size_t j = 0; j < nn; ++j)
+      if (match[j] < 0 && cnt_new[nb[j]] == 1 && cnt_old[nb[j]] == 1) { match[j] = old_of[nb[j]]; used[(size_t)match[j]] = 1; }
+  }
+};
+
+// The --cases rows of one pair (docs/SPEC.md section 16): the D rows in old line order, then the A and M rows in new line order.
 static void case_rows(std::ostream& os, std::vector<std::string> lead, const CaseSide& o, const CaseSide& nw, const std::string* old_path,
                       const tsm_case* oc, size_t no, const tsm_case* nc, size_t nn, size_t o_first) {
-  const std::vector<std::string> na = case_names(o.base, o.size, o.ext, oc, no), nb = case_names(nw.base, nw.size, nw.ext, nc, nn);
-  std::vector<int64_t> match(nn, -1);
-  std::vector<char> used(no, 0);
-  for (size_t j = 0; j < nn; ++j)
-    if (nc[j].match >= 0) { match[j] = nc[j].match - (int64_t)o_first; used[(size_t)match[j]] = 1; }
-  std::map<std::string, int64_t> cnt_new, cnt_old, old_of;
-  for (size_t j = 0; j < nn; ++j) if (match[j] < 0) ++cnt_new[nb[j]];
-  for (size_t k = 0; k < no; ++k) if (!used[k]) { ++cnt_old[na[k]]; old_of[na[k]] = (int64_t)k; }
-  for (size_t j = 0; j < nn; ++j)
-    if (match[j] < 0 && cnt_new[nb[j]] == 1 && cnt_old[nb[j]] == 1) { match[j] = old_of[nb[j]]; used[(size_t)match[j]] = 1; }
+  const PairCaseMatch pm(o, nw, oc, no, nc, nn, o_first);
+  const std::vector<std::string>&na = pm.na, &nb = pm.nb;
+  const std::vector<int64_t>& match = pm.match;
+  const std::vector<char>& used = pm.used;
   auto num = [](int64_t v) { return std::to_string(v); };
   auto row = [&](const std::string& path, std::vector<std::string> cells) {
     std::vector<std::string> r = lead;
@@ -1311,6 +1347,58 @@ static void case_rows(std::ostream& os, std::vector<std::string> lead, const Cas
     if (c.n_changed || d.n_changed || c.n_lines != d.n_lines)
       row(*nw.path, {nb[j], "M", num(c.line + 1), num(d.line + 1), num(c.n_lines), num(d.n_lines), num(c.n_assert), num(d.n_assert),
                      num(c.n_changed), num(d.n_changed), num(c.n_changed_assert), num(d.n_changed_assert)});
+  }
+}
+
+// The --smells rows of one pair (docs/SPEC.md section 19) from its cases (as case_rows, new case index n_first being nc[0]) and
+// its tests ot / nt with their churn records och / nch: two tests match when their cases do.  D tests in old line order, then A
+// and M tests in new line order, each test's rows in smell order.
+static void smell_rows(std::ostream& os, const std::vector<std::string>& lead, const CaseSide& o, const CaseSide& nw, const std::string* old_path,
+                       const tsm_case* oc, size_t no, const tsm_case* nc, size_t nn, size_t o_first, size_t n_first,
+                       const tsm_smell_test* ot, const tsm_test_churn* och, size_t nto, const tsm_smell_test* nt, const tsm_test_churn* nch,
+                       size_t ntn) {
+  const PairCaseMatch pm(o, nw, oc, no, nc, nn, o_first);
+  std::vector<int64_t> test_of_case(no, -1), pair_of(ntn, -1);   // old test of each old case; matched old test of each new test
+  std::vector<char> old_matched(nto, 0);
+  for (size_t t = 0; t < nto; ++t) test_of_case[(size_t)och[t].case_idx - o_first] = (int64_t)t;
+  for (size_t t = 0; t < ntn; ++t) {
+    const int64_t m = pm.match[(size_t)nch[t].case_idx - n_first];
+    if (m >= 0 && test_of_case[(size_t)m] >= 0) { pair_of[t] = test_of_case[(size_t)m]; old_matched[(size_t)pair_of[t]] = 1; }
+  }
+  auto num = [](int64_t v) { return std::to_string(v); };
+  auto row = [&](const std::string& path, const std::string& test, std::vector<std::string> cells) {
+    std::vector<std::string> r = lead;
+    r.insert(r.end(), {path, test});
+    r.insert(r.end(), cells.begin(), cells.end());
+    if (old_path) r.push_back(*old_path);
+    csv_row(os, r);
+  };
+  for (size_t t = 0; t < nto; ++t) {
+    if (old_matched[t]) continue;
+    const std::string& name = pm.na[(size_t)och[t].case_idx - o_first];
+    for (int k = 0; k < TSM_N_SMELLS; ++k)
+      if (ot[t].smells >> k & 1u)
+        row(*o.path, name, {"D", "", num(ot[t].line + 1), kSmellNames[k], "removed", "", num(och[t].instances[k]), "", num(och[t].churned[k])});
+  }
+  for (size_t t = 0; t < ntn; ++t) {
+    const std::string& name = pm.nb[(size_t)nch[t].case_idx - n_first];
+    const tsm_smell_test& x = nt[t];
+    const tsm_test_churn& c = nch[t];
+    if (pair_of[t] < 0) {
+      for (int k = 0; k < TSM_N_SMELLS; ++k)
+        if (x.smells >> k & 1u)
+          row(*nw.path, name, {"A", num(x.line + 1), "", kSmellNames[k], "introduced", num(c.instances[k]), "", num(c.churned[k]), ""});
+      continue;
+    }
+    const tsm_smell_test& y = ot[(size_t)pair_of[t]];
+    const tsm_test_churn& d = och[(size_t)pair_of[t]];
+    for (int k = 0; k < TSM_N_SMELLS; ++k) {
+      const bool hn = x.smells >> k & 1u, ho = y.smells >> k & 1u;
+      const char* ev = hn && !ho ? "introduced" : ho && !hn ? "removed" : hn && ho && (c.churned[k] || d.churned[k]) ? "changed" : nullptr;
+      if (ev)
+        row(*nw.path, name, {"M", num(x.line + 1), num(y.line + 1), kSmellNames[k], ev, num(c.instances[k]), num(d.instances[k]),
+                             num(c.churned[k]), num(d.churned[k])});
+    }
   }
 }
 
@@ -1459,7 +1547,7 @@ static void pair_batches(tsm_ctx* ctx, const std::vector<Change>& changes, const
 struct DiffOptions {
   int rename_pct = -1;
   int64_t batch_bytes = kBatch;
-  std::string out, asserts, churn, cases, edits;
+  std::string out, asserts, churn, cases, edits, smells;
   bool zero_rows = false;
   std::vector<std::string> lead_head;
   size_t churn_lead = 0;
@@ -1467,21 +1555,25 @@ struct DiffOptions {
 };
 
 // The diff of one batch: per pair the lines added and removed and the detail; with `asserts` the changed assertion lines and
-// the [group][K] tables, with `edits` also the assertion edits (the same call), with `cases` the case records.
+// the [group][K] tables, with `edits` also the assertion edits (the same call), with `cases` the case records, with `smells`
+// the case records, the tests and their smell churn (one call, which also serves `cases`).
 struct PairDiff {
   std::vector<int64_t> added, removed; std::vector<tsm_diff_detail> det; ChangedAsserts chg; CaseLists cases; std::vector<tsm_assert_edit> edits;
+  SmellLists smells;
 };
-static PairDiff diff_batch(const PairBatch& b, bool asserts, bool cases, bool edits) {
+static PairDiff diff_batch(const PairBatch& b, bool asserts, bool cases, bool edits, bool smells) {
   const size_t n = b.idx.size();
-  PairDiff d{std::vector<int64_t>(n), std::vector<int64_t>(n), std::vector<tsm_diff_detail>(n), {}, {}, {}};
+  PairDiff d{std::vector<int64_t>(n), std::vector<int64_t>(n), std::vector<tsm_diff_detail>(n), {}, {}, {}, {}};
   const tsm_corpus ca = b.olds.corpus(b.n_groups()), cn = b.news.corpus(b.n_groups());
   if (edits) diff_assert_edits(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.chg, d.edits);
   else if (asserts) diff_asserts(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.chg);
+  else if (smells) diff_smells(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.cases, d.smells);
   else if (cases) diff_cases(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.cases);
   else ck(tsm_diff_pairs_detail(b.ctx, &ca, &cn, d.added.data(), d.removed.data(), d.det.data(), nullptr), "tsm_diff_pairs_detail");
-  if (asserts && cases) {                                  // a second call: the assertion tables and the cases are separate diffs
+  if (asserts && (cases || smells)) {                      // a second call: the assertion tables and the cases are separate diffs
     std::vector<int64_t> a2(n), r2(n);
-    diff_cases(b.ctx, ca, cn, a2.data(), r2.data(), nullptr, d.cases);
+    if (smells) diff_smells(b.ctx, ca, cn, a2.data(), r2.data(), nullptr, d.cases, d.smells);
+    else diff_cases(b.ctx, ca, cn, a2.data(), r2.data(), nullptr, d.cases);
   }
   return d;
 }
@@ -1493,7 +1585,7 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
   const bool renames = o.rename_pct >= 0;
   const auto ctx = small_context();
   if (renames) pair_renames(ctx.get(), changes, load, o.rename_pct, o.batch_bytes, t);
-  std::ofstream os, as, cs, ch, es;                        // --out, --asserts, --cases, --assert-churn, --assert-edits
+  std::ofstream os, as, cs, ch, es, ss;                    // --out, --asserts, --cases, --assert-churn, --assert-edits, --smells
   auto open = [&](std::ofstream& f, const std::string& path, size_t n_lead, std::vector<std::string> head) {
     if (path.empty()) return;
     f.open(path, std::ios::binary);
@@ -1507,17 +1599,21 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
   if (renames) case_head.push_back("oldFileName");
   std::vector<std::string> edit_head = {"fileName", "oldLine", "line", "similarity", "oldStatement", "statement", "oldCategory", "category"};
   if (renames) edit_head.push_back("oldFileName");
+  std::vector<std::string> smell_head = {"fileName", "test", "change", "line", "oldLine", "smell", "event", "instances", "oldInstances",
+                                         "addedInstances", "removedInstances"};
+  if (renames) smell_head.push_back("oldFileName");
   open(os, o.out, o.lead_head.size(), out_head);
   open(as, o.asserts, o.lead_head.size(), {"fileName", "change", "line", "statement", "category"});
   open(cs, o.cases, o.lead_head.size(), case_head);
   open(ch, o.churn, o.churn_lead, {"category", "added", "removed"});
   open(es, o.edits, o.lead_head.size(), edit_head);
+  open(ss, o.smells, o.lead_head.size(), smell_head);
   const bool want_asserts = !o.asserts.empty() || !o.churn.empty() || es.is_open();
   std::map<size_t, std::vector<int64_t>> churn;            // per step with changed assertion lines: its [K] added and removed rows
   pair_batches(ctx.get(), changes, load, o.batch_bytes, want_asserts, t, [&](const PairBatch& b) {
     const size_t n = b.idx.size();
     if (!n) return;
-    const PairDiff d = diff_batch(b, want_asserts, cs.is_open(), es.is_open());
+    const PairDiff d = diff_batch(b, want_asserts, cs.is_open(), es.is_open(), ss.is_open());
     for (size_t g = 0; ch.is_open() && g < b.group_step.size(); ++g) {   // a step's files may span two batches
       const int64_t* ad = d.chg.added_counts.data() + g * TSM_NUM_CATEGORIES;
       const int64_t* rm = d.chg.removed_counts.data() + g * TSM_NUM_CATEGORIES;
@@ -1527,8 +1623,9 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
       tab.resize(2 * TSM_NUM_CATEGORIES, 0);
       for (int k = 0; k < TSM_NUM_CATEGORIES; ++k) { tab[(size_t)k] += ad[k]; tab[(size_t)(TSM_NUM_CATEGORIES + k)] += rm[k]; }
     }
-    // ka, kr, ko, kn: pair i's first event and case of each side; ke, ker: its first edit and the deleted-line event edit_rows is at
-    for (size_t i = 0, ka = 0, kr = 0, ko = 0, kn = 0, ke = 0, ker = 0; i < n; ++i) {
+    // ka, kr, ko, kn, to, tn: pair i's first event, case and test of each side; ke, ker: its first edit and the deleted-line event
+    // edit_rows is at
+    for (size_t i = 0, ka = 0, kr = 0, ko = 0, kn = 0, to = 0, tn = 0, ke = 0, ker = 0; i < n; ++i) {
       const Change& c = changes[b.idx[i]];
       const std::string& old_path = c.old_path.empty() ? c.path : c.old_path;
       const CaseSide olds{b.olds.arena.get() + b.olds.off[i], b.olds.len[i], b.olds.ext[i], &old_path};
@@ -1541,9 +1638,16 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
       const size_t o0 = ko, n0 = kn;
       while (ko < d.cases.olds.size() && d.cases.olds[ko].pair == (int32_t)i) ++ko;
       while (kn < d.cases.news.size() && d.cases.news[kn].pair == (int32_t)i) ++kn;
-      if (ko > o0 || kn > n0)
+      if (cs.is_open() && (ko > o0 || kn > n0))
         case_rows(cs, o.lead(c.step), olds, news, renames ? &c.old_path : nullptr, d.cases.olds.data() + o0, ko - o0, d.cases.news.data() + n0,
                   kn - n0, o0);
+      const size_t to0 = to, tn0 = tn;
+      while (to < d.smells.olds.size() && d.smells.olds[to].file == (int32_t)i) ++to;
+      while (tn < d.smells.news.size() && d.smells.news[tn].file == (int32_t)i) ++tn;
+      if (to > to0 || tn > tn0)
+        smell_rows(ss, o.lead(c.step), olds, news, renames ? &c.old_path : nullptr, d.cases.olds.data() + o0, ko - o0, d.cases.news.data() + n0,
+                   kn - n0, o0, n0, d.smells.olds.data() + to0, d.smells.old_churn.data() + to0, to - to0, d.smells.news.data() + tn0,
+                   d.smells.new_churn.data() + tn0, tn - tn0);
       t.added[c.step] += d.added[i]; t.removed[c.step] += d.removed[i]; t.files[c.step]++;
       if (!os.is_open() || !(o.zero_rows || d.added[i] || d.removed[i] || c.similarity >= 0)) continue;
       std::vector<std::string> row = o.lead(c.step);
@@ -1966,8 +2070,6 @@ static int cmd_clones(const std::vector<std::string>& roots, const std::string& 
 // line and smell order, lines 1-based; the statement is the stripped instance line (empty for the test-level smells).
 static int cmd_smells(const std::vector<std::string>& roots, const std::string& git_repo, const std::string& rev, bool all_files,
                       const std::string& out_path, int64_t batch_bytes) {
-  static const char* const kSmellNames[TSM_N_SMELLS] = {"empty", "assertion_free", "duplicate_assert", "redundant_assert",
-                                                        "conditional_logic", "exception_handling", "sleepy", "print", "ignored"};
   std::vector<FileEntry> files;
   std::vector<std::string> names;
   if (!git_repo.empty()) {
@@ -2050,13 +2152,13 @@ static void usage() {
   fprintf(stderr,
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
           "       tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]\n"
-          "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--find-renames N]\n"
-          "                         [--batch-bytes N]\n"
+          "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--smells F]\n"
+          "                         [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan body   <project-root>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases <snapshot-root>=<tag>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases --git <repository> [<revision>...] [--batch-bytes N] [--out F]\n"
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
-          "                          [--cases F] [--assert-edits F] [--find-renames N] [--batch-bytes N]\n"
+          "                          [--cases F] [--assert-edits F] [--smells F] [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
           "       tosem-scan clones <project-root>... [--min-lines N] [--all-files] [--out F]\n"
           "       tosem-scan clones --git <repository> [--rev R] [--min-lines N] [--all-files] [--out F]\n"
@@ -2067,6 +2169,8 @@ static void usage() {
           "--cases F: one row per test case that a revision adds (A), deletes (D) or modifies (M) (docs/SPEC.md section 16).\n"
           "--assert-edits F: one row per deleted assertion line that an inserted one of the same hunk replaces, with their similarity\n"
           "                  (docs/SPEC.md section 17).\n"
+          "--smells F: one row per (test, smell) that a revision introduces, removes or changes, with the smell's instances and the\n"
+          "            instance lines it adds and removes (docs/SPEC.md section 19).\n"
           "--batch-bytes N: files go to the GPU in batches of at most N bytes (per side of a diff; a larger file alone); scan: 1 GiB, else 512 MiB.\n"
           "Scans run on the GPU through libtosemscan.so (sm_90a); there is no CPU fallback.\n");
 }
@@ -2115,7 +2219,7 @@ int main(int argc, char** argv) {
   DiffOptions d;                                           // diff and history
   d.rename_pct = rename_pct; d.batch_bytes = batch_bytes(kBatch, 1);
   d.out = opt["--out"]; d.asserts = opt["--asserts"]; d.churn = opt["--assert-churn"]; d.cases = opt["--cases"];
-  d.edits = opt["--assert-edits"];
+  d.edits = opt["--assert-edits"]; d.smells = opt["--smells"];
   const std::string rev = opt.count("--rev") ? opt["--rev"] : "HEAD";
   const int64_t max_commits = opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0;
   if (cmd == "history") { if (pos.size() != 1) die("history needs the repository");

@@ -36,6 +36,7 @@ SMELL_TEST = np.dtype([("file", "<i4"), ("line", "<i4"), ("body_lines", "<i4"), 
                        ("n_instances", "<i4")])   # tsm_smell_test: one test of the corpus (docs/SPEC.md section 18)
 SMELLS = ["empty", "assertion_free", "duplicate_assert", "redundant_assert", "conditional_logic", "exception_handling", "sleepy",
           "print", "ignored"]                   # bit k of tsm_smell_test.smells and of line_smell is SMELLS[k]
+TEST_CHURN = np.dtype([("case_idx", "<i4"), ("instances", "<i4", (9,)), ("churned", "<i4", (9,))])   # tsm_test_churn (section 19)
 ASSERT_EDIT = np.dtype([("rev", "<i8"), ("aev", "<i8"), ("score", "<i4"), ("_pad", "<i4")])   # tsm_assert_edit: event indices
 
 # every symbol include/tosemscan.h declares (tests check the library exports exactly these)
@@ -45,7 +46,8 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_diff_pairs_asserts", "tsm_diff_resident_asserts", "tsm_reduce", "tsm_host_alloc", "tsm_host_free", "tsm_layout", "tsm_gen_sizes",
            "tsm_gen_fill", "tsm_gen_edit", "tsm_gen_pair_sizes", "tsm_gen_pair_fill", "tsm_similarity", "tsm_similarity_last_ms",
            "tsm_diff_pairs_marks", "tsm_blame_pairs", "tsm_blame_last_ms", "tsm_clones", "tsm_clones_last_ms",
-           "tsm_diff_pairs_cases", "tsm_diff_pairs_assert_edits", "tsm_assert_edits_last_ms", "tsm_smells", "tsm_smells_last_ms"]
+           "tsm_diff_pairs_cases", "tsm_diff_pairs_assert_edits", "tsm_assert_edits_last_ms", "tsm_smells", "tsm_smells_last_ms",
+           "tsm_diff_pairs_smells", "tsm_diff_smells_last_ms"]
 
 
 class TsmError(RuntimeError):
@@ -81,6 +83,12 @@ class _DiffAsserts(C.Structure):
 class _DiffCases(C.Structure):
     _fields_ = [("old_cases", C.c_void_p), ("old_cap", C.c_int64), ("n_old", C.c_int64),
                 ("new_cases", C.c_void_p), ("new_cap", C.c_int64), ("n_new", C.c_int64)]
+
+
+class _DiffSmells(C.Structure):
+    _fields_ = [("cases", _DiffCases),
+                ("old_tests", C.c_void_p), ("old_churn", C.c_void_p), ("old_test_cap", C.c_int64), ("n_old_tests", C.c_int64),
+                ("new_tests", C.c_void_p), ("new_churn", C.c_void_p), ("new_test_cap", C.c_int64), ("n_new_tests", C.c_int64)]
 
 
 class _CloneResult(C.Structure):
@@ -196,6 +204,11 @@ def lib():
                                  C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p]
         L.tsm_smells_last_ms.restype = C.c_int
         L.tsm_smells_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
+        L.tsm_diff_pairs_smells.restype = C.c_int
+        L.tsm_diff_pairs_smells.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 3 + \
+            [C.POINTER(_DiffSmells), C.c_void_p]
+        L.tsm_diff_smells_last_ms.restype = C.c_int
+        L.tsm_diff_smells_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
         _lib = L
     return _lib
 
@@ -848,6 +861,40 @@ class Scanner:
                 raise TsmError(rc, "tsm_smells")
             return {"line_base": base, "line_smell": smell[:nl.value], "tests": tests[:nt.value]}
         raise TsmError(TSM_E_CAPACITY, "tsm_smells")
+
+    def diff_smells(self, olds, news, stream=None, cap=None):
+        """Test-smell churn (docs/SPEC.md section 19): a dict of added, removed, detail (tsm_diff_pairs_detail's), old_cases and
+        new_cases (diff_cases' CASE arrays), old_tests and new_tests (SMELL_TEST records of each side, file = the pair) and
+        old_churn and new_churn (one TEST_CHURN record per test: its case index, and per smell its instances and those that the
+        revision removes (old side) or adds (new side)).  Arrays too small for the cases or tests are sized from the counts and
+        the call is made again (cap: the first guess of each)."""
+        n = olds.n_files
+        added, removed, det = np.zeros(n, np.int64), np.zeros(n, np.int64), np.zeros(max(n, 1), DIFF_DETAIL)
+        a, b = olds.c_struct(), news.c_struct()
+        co = cn = to = tn = int(cap if cap is not None else 0)
+        for _ in range(2):
+            oc, nc = np.zeros(max(co, 1), CASE), np.zeros(max(cn, 1), CASE)
+            ot, nt = np.zeros(max(to, 1), SMELL_TEST), np.zeros(max(tn, 1), SMELL_TEST)
+            och, nch = np.zeros(max(to, 1), TEST_CHURN), np.zeros(max(tn, 1), TEST_CHURN)
+            r = _DiffSmells(_DiffCases(_p(oc), co, 0, _p(nc), cn, 0), _p(ot), _p(och), to, 0, _p(nt), _p(nch), tn, 0)
+            rc = lib().tsm_diff_pairs_smells(self._ctx, C.byref(a), C.byref(b), _p(added), _p(removed), _p(det), C.byref(r), stream)
+            k = r.cases
+            if rc == TSM_E_CAPACITY and (k.n_old > co or k.n_new > cn or r.n_old_tests > to or r.n_new_tests > tn):
+                co, cn, to, tn = int(k.n_old), int(k.n_new), int(r.n_old_tests), int(r.n_new_tests)
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_diff_pairs_smells")
+            return {"added": added, "removed": removed, "detail": det[:n], "old_cases": oc[:k.n_old], "new_cases": nc[:k.n_new],
+                    "old_tests": ot[:r.n_old_tests], "new_tests": nt[:r.n_new_tests], "old_churn": och[:r.n_old_tests],
+                    "new_churn": nch[:r.n_new_tests]}
+        raise TsmError(TSM_E_CAPACITY, "tsm_diff_pairs_smells")
+
+    def diff_smells_last_ms(self):
+        """Device time of the last diff_smells call: [k_scan over both sides, smell stages, the diff, case records +
+        k_smell_churn] in ms."""
+        ms = (C.c_float * 4)()
+        lib().tsm_diff_smells_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
 
     def smells_last_ms(self):
         """Device time of the last smells call: [k_scan, kinds + case spans, k_smell_lines, k_smell_tests] in ms."""
