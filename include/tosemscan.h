@@ -352,6 +352,34 @@ int tsm_diff_pairs_smells(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus
                           tsm_diff_detail* detail, tsm_diff_smells* out, void* stream);
 int tsm_diff_smells_last_ms(tsm_ctx* ctx, float* ms4);
 
+/* Moved code (docs/SPEC.md section 20, git's `--color-moved=blocks`): the blocks of changed lines that a step moves.  A pair's
+ * step is its grp; it must be the same on both sides and below olds->n_groups (grp NULL: every pair in step 0), else TSM_E_ARG.
+ * Deleted and inserted lines of one step match when their line hashes (section 3) are equal; a block is a stretch of a run
+ * (maximal changed lines of one file on one side) that follows one matching diagonal as far as both runs allow, with at least 20
+ * alphanumeric bytes.  old_blocks / new_blocks hold the blocks of each side in ascending line order:
+ *   line      global line of the block's first line on its side (marks.line_base_* give the files)
+ *   partner   global line on the other side of the first line it matches (the smallest of the longest reach)
+ *   n_lines   lines of the block
+ *   n_assert  its assertion lines (section 4, Rev A, by the side's ext)
+ * marks is filled as tsm_diff_pairs_marks fills it, except that a moved line has bit 1 set too (value 3).  Any output pointer may
+ * be NULL (it is skipped); marks.n_old / n_new, n_old_blocks and n_new_blocks are always set.  If a given output's cap is smaller
+ * than its count, the call returns TSM_E_CAPACITY with all four set: size the arrays and call again.  added / removed / detail
+ * are those of tsm_diff_pairs_detail (detail may be NULL).  n_files = 0 is legal.
+ * Kernels: the diff of tsm_diff_pairs_marks, then k_move_lines, k_move_compact, k_move_insert, k_move_scatter, k_move_reach,
+ * k_move_starts, k_move_runs and k_move_mark (csrc/tsm_move_kernels.cuh).  The reach costs one comparison per matching (deleted, inserted)
+ * pair of a step: quadratic in a line that repeats on both sides of one step.
+ * tsm_moves_last_ms: device time of the last call, ms4 = { k_scan over both sides, k_diff_small + k_myers + k_myers_trace,
+ * k_move_lines to k_move_reach (the join and the reach), k_move_starts + k_move_runs + k_move_mark (the blocks) }. */
+typedef struct tsm_move_block { int64_t line, partner; int32_t n_lines, n_assert; } tsm_move_block;
+typedef struct tsm_diff_moves {
+  tsm_line_marks marks;
+  tsm_move_block* old_blocks; int64_t old_cap; int64_t n_old_blocks;
+  tsm_move_block* new_blocks; int64_t new_cap; int64_t n_new_blocks;
+} tsm_diff_moves;
+int tsm_diff_pairs_moves(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                         tsm_diff_detail* detail, tsm_diff_moves* out, void* stream);
+int tsm_moves_last_ms(tsm_ctx* ctx, float* ms4);
+
 /* Body statements (docs/SPEC.md section 10; Important-files/ML-Analysis-v4.xlsx!Apollo:R2-R26, golden G2): the
  * kind of every line of every file - 0 blank, 1 first line of a statement, 2 continuation (lines
  * are joined while the parentheses are open).  line_base[n_files+1] and *n_lines are always filled;

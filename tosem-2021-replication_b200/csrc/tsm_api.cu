@@ -23,6 +23,7 @@
 #include "tsm_case_kernels.cuh"
 #include "tsm_edit_kernels.cuh"
 #include "tsm_smell_kernels.cuh"
+#include "tsm_move_kernels.cuh"
 
 using namespace tsm;
 
@@ -105,6 +106,7 @@ struct tsm_ctx {
   float smell_ms[4] = {0, 0, 0, 0};        // k_scan, kinds + case spans, k_smell_lines, k_smell_tests of the last tsm_smells
   float churn_ms[4] = {0, 0, 0, 0};        // k_scan, smell stages, the diff, case records + k_smell_churn of the last tsm_diff_pairs_smells
   float edit_ms[3] = {0, 0, 0};            // k_scan, the diff, compact to pairing (host clock) of the last assertion-edit call
+  float move_ms[4] = {0, 0, 0, 0};         // k_scan, the diff, line flags to k_move_reach, k_move_starts to k_move_mark of the last tsm_diff_pairs_moves
   cudaEvent_t blame_ev[2] = {};            // around k_blame (tsm_blame_last_ms)
   float blame_ms = 0;
   struct HostSidePair* res_pair = nullptr; // sides kept in HBM by tsm_diff_upload
@@ -2199,5 +2201,193 @@ extern "C" int tsm_diff_pairs_smells(tsm_ctx* c, const tsm_corpus* olds, const t
 extern "C" int tsm_diff_smells_last_ms(tsm_ctx* c, float* ms4) {
   if (!c || !ms4) return TSM_E_ARG;
   for (int i = 0; i < 4; ++i) ms4[i] = c->churn_ms[i];
+  return TSM_OK;
+}
+
+// ------------------------------------------------------------------------------------- SPEC section 20 moved code
+// The line records of both sides, the marks diff, then per side k_move_lines and three exclusive scans (alnum prefix, entry and
+// run numbers); one synchronisation reads the entry and run counts, which size the join.  k_move_compact, the (step, hash) table
+// (k_move_insert, xscan of each side's slot counts, k_move_scatter) and k_move_reach; per side the list of block starts
+// (k_move_starts twice around an xscan) and k_move_runs twice around an xscan of the block counts; a second synchronisation reads the block counts for k_move_mark.  Slots 0-1 and 2-3 of diff_ev time the
+// flags and the join with the reach, 4-5 and 6-7 the runs and the marks (the diff's own slots have been read by then).
+struct MoveBufs { DevBuf flag, alnum, chg, head, apre, eidx, ridx, best, ent, run_first, run_end, cnt, base, cursor, slot_of, seg, seg_slot,
+                  start, sidx, starts, rcnt, rbase, blocks; };
+
+extern "C" int tsm_diff_pairs_moves(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                                    tsm_diff_detail* detail, tsm_diff_moves* out, void* stream) {
+  if (!c || !olds || !news || !added || !removed || !out || olds->n_files != news->n_files || out->marks.del_cap < 0 ||
+      out->marks.ins_cap < 0 || out->old_cap < 0 || out->new_cap < 0)
+    return TSM_E_ARG;
+  const int32_t n = olds->n_files;
+  for (int32_t i = 0; i < n; ++i) {                        // a pair's step: the same grp on both sides, below n_groups
+    const uint16_t go = olds->grp ? olds->grp[i] : 0, gn = news->grp ? news->grp[i] : 0;
+    if (go != gn || go >= olds->n_groups || gn >= news->n_groups) return TSM_E_ARG;
+  }
+  for (float& v : c->move_ms) v = 0;
+  tsm_line_marks& mk = out->marks;
+  mk.n_old = mk.n_new = 0;
+  out->n_old_blocks = out->n_new_blocks = 0;
+  if (n == 0) {
+    if (mk.line_base_old) mk.line_base_old[0] = 0;
+    if (mk.line_base_new) mk.line_base_new[0] = 0;
+    return TSM_OK;
+  }
+  int rc = check_sides({olds, news}, n, true);
+  if (rc != TSM_OK) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  CallScope call(c, st);
+  CU(call.status);
+  HostSidePair P;
+  MoveBufs mb[2];
+  DevBuf d_bsum, d_slot_bsum, d_table;
+  SyncGuard guard(st);
+  rc = pair_upload(olds, news, true, P, st);
+  if (rc == TSM_OK) rc = pair_records(c, P, &c->diff_ms[0], true, st);
+  if (rc != TSM_OK) return rc;
+  c->move_ms[0] = c->diff_ms[0];
+  rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
+  if (rc != TSM_OK) return rc;
+  c->move_ms[1] = c->diff_ms[1] + c->diff_ms[2];
+  HostSide* const side[2] = {&P.A, &P.B};
+  const uint32_t T[2] = {(uint32_t)P.A.total, (uint32_t)P.B.total};
+  int launches = 0;
+  if (!d_bsum.alloc(8 * ((size_t)std::max(T[0], T[1]) / XS_TILE + 4))) return TSM_E_CUDA;
+  unsigned long long* const bsum = d_bsum.as<unsigned long long>();
+  CU(cudaEventRecord(c->diff_ev[0], st));
+  for (int s = 0; s < 2; ++s) {
+    MoveBufs& m = mb[s];
+    const size_t L = T[s];
+    if (!m.flag.alloc(L) || !m.alnum.alloc(4 * L) || !m.chg.alloc(4 * L) || !m.head.alloc(4 * L) || !m.apre.alloc(8 * (L + 1)) ||
+        !m.eidx.alloc(8 * (L + 1)) || !m.ridx.alloc(8 * (L + 1)) || !m.best.alloc(8 * L))
+      return TSM_E_CUDA;
+    CU(cudaMemsetAsync(m.best.p, 0, 8 * L, st));
+    if (L) k_move_lines<<<(unsigned)((L + 255) / 256), 256, 0, st>>>(side[s]->d, n, T[s], side[s]->line_mark.as<uint8_t>(), m.flag.as<uint8_t>(),
+                                                                      m.alnum.as<uint32_t>(), m.chg.as<uint32_t>(), m.head.as<uint32_t>());
+    xscan(m.alnum.as<uint32_t>(), T[s], bsum, m.apre.as<unsigned long long>(), st);
+    xscan(m.chg.as<uint32_t>(), T[s], bsum, m.eidx.as<unsigned long long>(), st);
+    xscan(m.head.as<uint32_t>(), T[s], bsum, m.ridx.as<unsigned long long>(), st);
+    launches += (L ? 1 : 0) + 9;
+  }
+  CU(cudaGetLastError());
+  unsigned long long* pin = reinterpret_cast<unsigned long long*>(c->h_diff + 128);
+  for (int s = 0; s < 2; ++s) {
+    CU(cudaMemcpyAsync(pin + 2 * s, mb[s].eidx.as<unsigned long long>() + T[s], 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(pin + 2 * s + 1, mb[s].ridx.as<unsigned long long>() + T[s], 8, cudaMemcpyDeviceToHost, st));
+  }
+  CU(cudaStreamSynchronize(st));
+  const uint32_t ne[2] = {(uint32_t)pin[0], (uint32_t)pin[2]}, nr[2] = {(uint32_t)pin[1], (uint32_t)pin[3]};
+  for (int s = 0; s < 2; ++s) {
+    MoveBufs& m = mb[s];
+    if (!m.ent.alloc(4 * (size_t)ne[s]) || !m.run_first.alloc(4 * (size_t)nr[s]) || !m.run_end.alloc(4 * (size_t)nr[s])) return TSM_E_CUDA;
+    if (T[s])
+      k_move_compact<<<(T[s] + 255) / 256, 256, 0, st>>>(m.flag.as<uint8_t>(), T[s], m.eidx.as<unsigned long long>(), m.ridx.as<unsigned long long>(),
+                                                          m.ent.as<uint32_t>(), m.run_first.as<uint32_t>(), m.run_end.as<uint32_t>());
+  }
+  CU(cudaEventRecord(c->diff_ev[1], st));
+  // ---- the join: one table over the entries of both sides, at most half full
+  const unsigned long long tot = (unsigned long long)ne[0] + ne[1];
+  unsigned long long cap = 1024;
+  while (cap < 2 * tot) cap <<= 1;
+  if (cap > (1ull << 31)) return TSM_E_NOMEM;
+  const uint32_t mask = (uint32_t)cap - 1;
+  if (!d_table.alloc(sizeof(MoveKey) * cap)) return TSM_E_CUDA;
+  CU(cudaEventRecord(c->diff_ev[2], st));
+  CU(cudaMemsetAsync(d_table.p, 0, sizeof(MoveKey) * cap, st));
+  for (int s = 0; s < 2; ++s) {
+    MoveBufs& m = mb[s];
+    if (!m.cnt.alloc(4 * cap) || !m.cursor.alloc(4 * cap) || !m.base.alloc(8 * (cap + 1)) || !m.slot_of.alloc(4 * (size_t)ne[s]) ||
+        !m.seg.alloc(4 * (size_t)ne[s]) || (s == 0 && !m.seg_slot.alloc(4 * (size_t)ne[s])))
+      return TSM_E_CUDA;
+    CU(cudaMemsetAsync(m.cnt.p, 0, 4 * cap, st));
+    CU(cudaMemsetAsync(m.cursor.p, 0, 4 * cap, st));
+    if (ne[s])
+      k_move_insert<<<(ne[s] + 255) / 256, 256, 0, st>>>(m.ent.as<uint32_t>(), ne[s], side[s]->d.line_hash, side[s]->d.line_base, n,
+                                                          side[s]->grp.as<uint16_t>(), d_table.as<MoveKey>(), mask, m.cnt.as<uint32_t>(),
+                                                          m.slot_of.as<uint32_t>());
+  }
+  if (!d_slot_bsum.alloc(8 * (cap / XS_TILE + 4))) return TSM_E_CUDA;
+  for (int s = 0; s < 2; ++s) {
+    MoveBufs& m = mb[s];
+    xscan(m.cnt.as<uint32_t>(), (uint32_t)cap, d_slot_bsum.as<unsigned long long>(), m.base.as<unsigned long long>(), st);
+    if (ne[s])
+      k_move_scatter<<<(ne[s] + 255) / 256, 256, 0, st>>>(m.ent.as<uint32_t>(), m.slot_of.as<uint32_t>(), ne[s], m.base.as<unsigned long long>(),
+                                                           m.cursor.as<uint32_t>(), m.seg.as<uint32_t>(), s == 0 ? m.seg_slot.as<uint32_t>() : nullptr);
+    launches += 3 + (ne[s] ? 2 : 0);
+  }
+  MoveSide ms[2];
+  for (int s = 0; s < 2; ++s)
+    ms[s] = MoveSide{side[s]->d.line_hash, mb[s].flag.as<uint8_t>(), mb[s].ridx.as<unsigned long long>(), mb[s].run_end.as<uint32_t>(),
+                     mb[s].best.as<unsigned long long>()};
+  if (ne[0] && ne[1]) {
+    k_move_reach<<<std::min((ne[0] + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(ms[0], ms[1], mb[0].seg.as<uint32_t>(), mb[0].seg_slot.as<uint32_t>(),
+                                                                               ne[0], mb[1].seg.as<uint32_t>(), mb[1].base.as<unsigned long long>());
+    ++launches;
+  }
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(c->diff_ev[3], st));
+  // ---- the blocks of every run, in line order
+  CU(cudaEventRecord(c->diff_ev[4], st));
+  for (int s = 0; s < 2; ++s) {
+    MoveBufs& m = mb[s];
+    if (!m.start.alloc(4 * (size_t)ne[s]) || !m.sidx.alloc(8 * ((size_t)ne[s] + 1)) || !m.starts.alloc(4 * (size_t)ne[s]) ||
+        !m.rcnt.alloc(4 * (size_t)nr[s]) || !m.rbase.alloc(8 * ((size_t)nr[s] + 1)) || !m.blocks.alloc(sizeof(tsm_move_block) * (size_t)ne[s]))
+      return TSM_E_CUDA;
+    const unsigned ge = (ne[s] + 255) / 256, g = (nr[s] + 255) / 256;
+    const uint32_t* ent = m.ent.as<uint32_t>();
+    const unsigned long long* best = m.best.as<unsigned long long>();
+    if (ne[s])
+      k_move_starts<0><<<ge, 256, 0, st>>>(ent, ne[s], best, m.apre.as<unsigned long long>(), m.start.as<uint32_t>(), nullptr, nullptr);
+    xscan(m.start.as<uint32_t>(), ne[s], bsum, m.sidx.as<unsigned long long>(), st);
+    if (ne[s])
+      k_move_starts<1><<<ge, 256, 0, st>>>(ent, ne[s], best, nullptr, m.start.as<uint32_t>(), m.sidx.as<unsigned long long>(),
+                                           m.starts.as<uint32_t>());
+    if (nr[s])
+      k_move_runs<0><<<g, 256, 0, st>>>(m.run_first.as<uint32_t>(), m.run_end.as<uint32_t>(), nr[s], best, m.eidx.as<unsigned long long>(),
+                                        m.sidx.as<unsigned long long>(), ne[s], m.starts.as<uint32_t>(), m.rcnt.as<uint32_t>(), nullptr, nullptr);
+    xscan(m.rcnt.as<uint32_t>(), nr[s], bsum, m.rbase.as<unsigned long long>(), st);
+    if (nr[s])
+      k_move_runs<1><<<g, 256, 0, st>>>(m.run_first.as<uint32_t>(), m.run_end.as<uint32_t>(), nr[s], best, m.eidx.as<unsigned long long>(),
+                                        m.sidx.as<unsigned long long>(), ne[s], m.starts.as<uint32_t>(), nullptr,
+                                        m.rbase.as<unsigned long long>(), m.blocks.as<tsm_move_block>());
+    CU(cudaMemcpyAsync(pin + s, m.rbase.as<unsigned long long>() + nr[s], 8, cudaMemcpyDeviceToHost, st));
+    launches += 6 + (ne[s] ? 2 : 0) + (nr[s] ? 2 : 0);
+  }
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(c->diff_ev[5], st));
+  CU(cudaStreamSynchronize(st));
+  const uint32_t nb[2] = {(uint32_t)pin[0], (uint32_t)pin[1]};
+  CU(cudaEventRecord(c->diff_ev[6], st));
+  for (int s = 0; s < 2; ++s)
+    if (nb[s]) {
+      k_move_mark<<<(ne[s] + 255) / 256, 256, 0, st>>>(mb[s].ent.as<uint32_t>(), ne[s], mb[s].blocks.as<tsm_move_block>(), nb[s],
+                                                        side[s]->d.line_flag, side[s]->line_mark.as<uint8_t>());
+      ++launches;
+    }
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(c->diff_ev[7], st));
+  mk.n_old = (int64_t)T[0]; mk.n_new = (int64_t)T[1];
+  out->n_old_blocks = nb[0]; out->n_new_blocks = nb[1];
+  if (mk.line_base_old) memcpy(mk.line_base_old, P.A.base.data(), sizeof(int64_t) * ((size_t)n + 1));
+  if (mk.line_base_new) memcpy(mk.line_base_new, P.B.base.data(), sizeof(int64_t) * ((size_t)n + 1));
+  CU(cudaStreamSynchronize(st));
+  c->move_ms[2] = elapsed_ms(c->diff_ev[0], c->diff_ev[1]) + elapsed_ms(c->diff_ev[2], c->diff_ev[3]);
+  c->move_ms[3] = elapsed_ms(c->diff_ev[4], c->diff_ev[5]) + elapsed_ms(c->diff_ev[6], c->diff_ev[7]);
+  c->launches += launches;
+  if ((mk.del && mk.del_cap < mk.n_old) || (mk.ins && mk.ins_cap < mk.n_new) || (out->old_blocks && out->old_cap < (int64_t)nb[0]) ||
+      (out->new_blocks && out->new_cap < (int64_t)nb[1]))
+    return TSM_E_CAPACITY;
+  uint8_t* const h_mark[2] = {mk.del, mk.ins};
+  tsm_move_block* const h_blocks[2] = {out->old_blocks, out->new_blocks};
+  for (int s = 0; s < 2; ++s) {
+    if (h_mark[s] && T[s]) CU(cudaMemcpyAsync(h_mark[s], side[s]->line_mark.p, T[s], cudaMemcpyDeviceToHost, st));
+    if (h_blocks[s] && nb[s]) CU(cudaMemcpyAsync(h_blocks[s], mb[s].blocks.p, sizeof(tsm_move_block) * nb[s], cudaMemcpyDeviceToHost, st));
+  }
+  CU(cudaStreamSynchronize(st));
+  return TSM_OK;
+}
+
+extern "C" int tsm_moves_last_ms(tsm_ctx* c, float* ms4) {
+  if (!c || !ms4) return TSM_E_ARG;
+  for (int i = 0; i < 4; ++i) ms4[i] = c->move_ms[i];
   return TSM_OK;
 }

@@ -18,16 +18,17 @@
 //   tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N]
 //   tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]
 //   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--smells F]
-//                     [--find-renames N] [--batch-bytes N]
+//                     [--moves F] [--find-renames N] [--batch-bytes N]
 //   tosem-scan body   <project-root>... [--batch-bytes N] [--out F]
 //   tosem-scan releases <snapshot-root>=<tag>... | --git <repository> [<revision>...]   [--batch-bytes N] [--out F]
 //   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F] [--cases F]
-//                      [--assert-edits F] [--smells F] [--find-renames N] [--batch-bytes N]
+//                      [--assert-edits F] [--smells F] [--moves F] [--find-renames N] [--batch-bytes N]
 //   tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]
 //   tosem-scan clones <project-root>... | --git <repository> [--rev R]   [--min-lines N] [--all-files] [--out F]
 // Every command that scans files does it with scan_batches: batches of at most --batch-bytes of arena (clones: all files in one),
 // one context, the next batch read while the current one is scanned.  Every command that diffs revision pairs (diff, history,
-// blame) does it with pair_batches: batches of at most --batch-bytes per side, one context shared with the rename pairing.
+// blame) does it with pair_batches: batches of at most --batch-bytes per side (with --moves: whole steps), one context shared
+// with the rename pairing.
 #include <algorithm>
 #include <atomic>
 #include <cctype>
@@ -45,6 +46,7 @@
 #include <map>
 #include <memory>
 #include <numeric>
+#include <optional>
 #include <sstream>
 #include <string>
 #include <thread>
@@ -1423,6 +1425,47 @@ static void edit_rows(std::ostream& os, const std::vector<std::string>& lead, co
   }
 }
 
+// Moved code (docs/SPEC.md section 20) of one diff call: the first global line of every pair on each side and the moved blocks of
+// both sides (tsm_diff_pairs_moves, the batch's groups being its steps), block arrays grown to the counts the library reports.
+struct MoveLists { std::vector<int64_t> base[2]; std::vector<tsm_move_block> blocks[2]; };
+static void diff_moves(tsm_ctx* ctx, const tsm_corpus& ca, const tsm_corpus& cn, MoveLists& r) {
+  const size_t n = (size_t)ca.n_files;
+  std::vector<int64_t> added(n), removed(n);
+  for (std::vector<int64_t>& b : r.base) b.assign(n + 1, 0);
+  int64_t cap[2] = {1024, 1024};
+  for (;;) {
+    for (int s = 0; s < 2; ++s) r.blocks[s].resize((size_t)cap[s]);
+    tsm_diff_moves o{{r.base[0].data(), r.base[1].data(), nullptr, 0, 0, nullptr, 0, 0}, r.blocks[0].data(), cap[0], 0, r.blocks[1].data(), cap[1], 0};
+    const int rc = tsm_diff_pairs_moves(ctx, &ca, &cn, added.data(), removed.data(), nullptr, &o, nullptr);
+    if (rc == TSM_E_CAPACITY && (o.n_old_blocks > cap[0] || o.n_new_blocks > cap[1])) {
+      cap[0] = std::max(cap[0], o.n_old_blocks); cap[1] = std::max(cap[1], o.n_new_blocks);
+      continue;
+    }
+    ck(rc, "tsm_diff_pairs_moves");
+    r.blocks[0].resize((size_t)o.n_old_blocks); r.blocks[1].resize((size_t)o.n_new_blocks);
+    return;
+  }
+}
+
+// The --moves rows of pair i (docs/SPEC.md section 20): `lead` cells, fileName, change ('-' a block moved away, old side; '+' a
+// block moved here, new side), 1-based line, lines, asserts, then otherFileName and the 1-based otherLine of the block's partner
+// on the other side.  The '-' rows in old line order, then the '+' rows in new line order.  k[s] walks the blocks of side s
+// across calls; path(s, j) is the path of pair j on side s.
+static void move_rows(std::ostream& os, const std::vector<std::string>& lead, const MoveLists& m, size_t i, size_t k[2],
+                      const std::function<const std::string&(int, size_t)>& path) {
+  for (int s = 0; s < 2; ++s) {
+    const std::vector<int64_t>&here = m.base[s], &there = m.base[1 - s];
+    for (; k[s] < m.blocks[s].size() && m.blocks[s][k[s]].line < here[i + 1]; ++k[s]) {
+      const tsm_move_block& b = m.blocks[s][k[s]];
+      const size_t j = (size_t)(std::upper_bound(there.begin(), there.end(), b.partner) - there.begin()) - 1;
+      std::vector<std::string> row = lead;
+      row.insert(row.end(), {path(s, i), s ? "+" : "-", std::to_string(b.line - here[i] + 1), std::to_string(b.n_lines),
+                             std::to_string(b.n_assert), path(1 - s, j), std::to_string(b.partner - there[j] + 1)});
+      csv_row(os, row);
+    }
+  }
+}
+
 // One changed file of a revision pair.  `step` is its commit (history) or 0 (diff); `o` and `n` name the bytes of the old and
 // the new side for the caller's loader, -1 where that side does not exist.  A rename (--find-renames) moves the deleted file's
 // `o` onto the added file and keeps the deleted file's path and the score in %.
@@ -1505,23 +1548,64 @@ struct PairBatch {
 };
 
 // The changes cut in order into batches, each handed to `fn`, one whose changes are all binary too (with an empty idx).  Both
-// sides are loaded until one holds batch_bytes bytes; with group_steps (the assertion tables: a group is a u16) a batch also
-// holds at most 65 535 steps, binary-only steps counted.  t.binaries and t.diffed count the skipped and the packed changes.
+// sides are loaded until one holds batch_bytes bytes; with group_steps (the assertion tables and the moves: a group is a u16) a
+// batch also holds at most 65 535 steps, binary-only steps counted.  With whole_steps (the moves, which cross the files of a
+// step) a batch takes whole steps: a step joins it only while both sides stay within batch_bytes and the int32-indexed arena, so
+// a step larger than that is a batch of its own (and one larger than the arena is refused).  A step loaded but not taken is kept
+// for the next batch.  t.binaries and t.diffed count the skipped and the packed changes.
 static void pair_batches(tsm_ctx* ctx, const std::vector<Change>& changes, const Loader& load, int64_t batch_bytes, bool group_steps,
-                         ChangeTotals& t, const std::function<void(const PairBatch&)>& fn) {
+                         bool whole_steps, ChangeTotals& t, const std::function<void(const PairBatch&)>& fn) {
+  struct StepLoad { size_t s1 = 0; std::vector<size_t> idx; std::vector<std::vector<uint8_t>> x, y; int64_t so = 0, sn = 0, binaries = 0; };
+  auto load_pair = [&](size_t r, std::vector<uint8_t>& x, std::vector<uint8_t>& y) {   // false: binary on a side
+    const Change& c = changes[r];
+    x = c.o >= 0 ? load(c.o) : std::vector<uint8_t>(); y = c.n >= 0 ? load(c.n) : std::vector<uint8_t>();
+    if (binary(x) || binary(y)) return false;
+    if (x.size() > 0x7fff0000u || y.size() > 0x7fff0000u) die("blob too large: " + c.path);
+    return true;
+  };
+  auto load_step = [&](size_t r1) {                        // the changes of the step that starts at r1
+    StepLoad S;
+    for (S.s1 = r1; S.s1 < changes.size() && changes[S.s1].step == changes[r1].step; ++S.s1) {
+      std::vector<uint8_t> x, y;
+      if (!load_pair(S.s1, x, y)) { ++S.binaries; continue; }
+      S.so += (int64_t)x.size() + 256; S.sn += (int64_t)y.size() + 256;
+      S.x.push_back(std::move(x)); S.y.push_back(std::move(y)); S.idx.push_back(S.s1);
+    }
+    return S;
+  };
+  const int64_t arena_max = (1ll << 31) - 4097;
+  std::optional<StepLoad> carry;                           // whole_steps: the loaded step the previous batch did not take
   for (size_t r0 = 0, r1 = 0; r0 < changes.size(); r0 = r1) {
     PairBatch b{r0, r0, {}, {}, {}, {}, ctx};
     std::vector<std::vector<uint8_t>> blobs[2];            // old, new
     int64_t so = 0, sn = 0;
     size_t steps = 0;
-    for (r1 = r0; r1 < changes.size() && so < batch_bytes && sn < batch_bytes; ++r1) {
-      const Change& c = changes[r1];
-      if (group_steps && (r1 == r0 || c.step != changes[r1 - 1].step) && ++steps > 65535) break;
-      std::vector<uint8_t> x = c.o >= 0 ? load(c.o) : std::vector<uint8_t>(), y = c.n >= 0 ? load(c.n) : std::vector<uint8_t>();
-      if (binary(x) || binary(y)) { ++t.binaries; continue; }
-      if (x.size() > 0x7fff0000u || y.size() > 0x7fff0000u) die("blob too large: " + c.path);
-      so += (int64_t)x.size() + 256; sn += (int64_t)y.size() + 256;
-      blobs[0].push_back(std::move(x)); blobs[1].push_back(std::move(y)); b.idx.push_back(r1);
+    if (whole_steps) {
+      const int64_t limit = std::min(batch_bytes, arena_max);
+      for (r1 = r0; r1 < changes.size();) {
+        StepLoad S = carry ? std::move(*carry) : load_step(r1);
+        carry.reset();
+        if (r1 > r0 && (so + S.so > limit || sn + S.sn > limit || (group_steps && steps + 1 > 65535))) { carry = std::move(S); break; }
+        ++steps;
+        t.binaries += S.binaries;
+        for (size_t k = 0; k < S.idx.size(); ++k) {
+          blobs[0].push_back(std::move(S.x[k])); blobs[1].push_back(std::move(S.y[k])); b.idx.push_back(S.idx[k]);
+        }
+        so += S.so; sn += S.sn;
+        r1 = S.s1;
+      }
+      if (std::max(so, sn) > arena_max)
+        die("--moves keeps every step in one batch, and a side of step " + std::to_string(changes[r0].step) +
+            " does not fit an int32-indexed arena (2 GiB)");
+    } else {
+      for (r1 = r0; r1 < changes.size() && so < batch_bytes && sn < batch_bytes; ++r1) {
+        const Change& c = changes[r1];
+        if (group_steps && (r1 == r0 || c.step != changes[r1 - 1].step) && ++steps > 65535) break;
+        std::vector<uint8_t> x, y;
+        if (!load_pair(r1, x, y)) { ++t.binaries; continue; }
+        so += (int64_t)x.size() + 256; sn += (int64_t)y.size() + 256;
+        blobs[0].push_back(std::move(x)); blobs[1].push_back(std::move(y)); b.idx.push_back(r1);
+      }
     }
     b.r1 = r1;
     std::vector<const std::vector<uint8_t>*> sides[2];
@@ -1547,7 +1631,7 @@ static void pair_batches(tsm_ctx* ctx, const std::vector<Change>& changes, const
 struct DiffOptions {
   int rename_pct = -1;
   int64_t batch_bytes = kBatch;
-  std::string out, asserts, churn, cases, edits, smells;
+  std::string out, asserts, churn, cases, edits, smells, moves;
   bool zero_rows = false;
   std::vector<std::string> lead_head;
   size_t churn_lead = 0;
@@ -1556,14 +1640,15 @@ struct DiffOptions {
 
 // The diff of one batch: per pair the lines added and removed and the detail; with `asserts` the changed assertion lines and
 // the [group][K] tables, with `edits` also the assertion edits (the same call), with `cases` the case records, with `smells`
-// the case records, the tests and their smell churn (one call, which also serves `cases`).
+// the case records, the tests and their smell churn (one call, which also serves `cases`), with `moves` the moved blocks (a call
+// of its own).
 struct PairDiff {
   std::vector<int64_t> added, removed; std::vector<tsm_diff_detail> det; ChangedAsserts chg; CaseLists cases; std::vector<tsm_assert_edit> edits;
-  SmellLists smells;
+  SmellLists smells; MoveLists moves;
 };
-static PairDiff diff_batch(const PairBatch& b, bool asserts, bool cases, bool edits, bool smells) {
+static PairDiff diff_batch(const PairBatch& b, bool asserts, bool cases, bool edits, bool smells, bool moves) {
   const size_t n = b.idx.size();
-  PairDiff d{std::vector<int64_t>(n), std::vector<int64_t>(n), std::vector<tsm_diff_detail>(n), {}, {}, {}, {}};
+  PairDiff d{std::vector<int64_t>(n), std::vector<int64_t>(n), std::vector<tsm_diff_detail>(n), {}, {}, {}, {}, {}};
   const tsm_corpus ca = b.olds.corpus(b.n_groups()), cn = b.news.corpus(b.n_groups());
   if (edits) diff_assert_edits(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.chg, d.edits);
   else if (asserts) diff_asserts(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.chg);
@@ -1575,6 +1660,7 @@ static PairDiff diff_batch(const PairBatch& b, bool asserts, bool cases, bool ed
     if (smells) diff_smells(b.ctx, ca, cn, a2.data(), r2.data(), nullptr, d.cases, d.smells);
     else diff_cases(b.ctx, ca, cn, a2.data(), r2.data(), nullptr, d.cases);
   }
+  if (moves) diff_moves(b.ctx, ca, cn, d.moves);
   return d;
 }
 
@@ -1585,7 +1671,7 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
   const bool renames = o.rename_pct >= 0;
   const auto ctx = small_context();
   if (renames) pair_renames(ctx.get(), changes, load, o.rename_pct, o.batch_bytes, t);
-  std::ofstream os, as, cs, ch, es, ss;                    // --out, --asserts, --cases, --assert-churn, --assert-edits, --smells
+  std::ofstream os, as, cs, ch, es, ss, ms;                // --out, --asserts, --cases, --assert-churn, --assert-edits, --smells, --moves
   auto open = [&](std::ofstream& f, const std::string& path, size_t n_lead, std::vector<std::string> head) {
     if (path.empty()) return;
     f.open(path, std::ios::binary);
@@ -1608,12 +1694,18 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
   open(ch, o.churn, o.churn_lead, {"category", "added", "removed"});
   open(es, o.edits, o.lead_head.size(), edit_head);
   open(ss, o.smells, o.lead_head.size(), smell_head);
+  open(ms, o.moves, o.lead_head.size(), {"fileName", "change", "line", "lines", "asserts", "otherFileName", "otherLine"});
   const bool want_asserts = !o.asserts.empty() || !o.churn.empty() || es.is_open();
   std::map<size_t, std::vector<int64_t>> churn;            // per step with changed assertion lines: its [K] added and removed rows
-  pair_batches(ctx.get(), changes, load, o.batch_bytes, want_asserts, t, [&](const PairBatch& b) {
+  pair_batches(ctx.get(), changes, load, o.batch_bytes, want_asserts || ms.is_open(), ms.is_open(), t, [&](const PairBatch& b) {
     const size_t n = b.idx.size();
     if (!n) return;
-    const PairDiff d = diff_batch(b, want_asserts, cs.is_open(), es.is_open(), ss.is_open());
+    const PairDiff d = diff_batch(b, want_asserts, cs.is_open(), es.is_open(), ss.is_open(), ms.is_open());
+    auto path = [&](int s, size_t j) -> const std::string& {  // the path of pair j on side s (0 old, 1 new)
+      const Change& c = changes[b.idx[j]];
+      return s == 0 && !c.old_path.empty() ? c.old_path : c.path;
+    };
+    size_t km[2] = {0, 0};                                 // the first block of each side of pair i
     for (size_t g = 0; ch.is_open() && g < b.group_step.size(); ++g) {   // a step's files may span two batches
       const int64_t* ad = d.chg.added_counts.data() + g * TSM_NUM_CATEGORIES;
       const int64_t* rm = d.chg.removed_counts.data() + g * TSM_NUM_CATEGORIES;
@@ -1648,6 +1740,7 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
         smell_rows(ss, o.lead(c.step), olds, news, renames ? &c.old_path : nullptr, d.cases.olds.data() + o0, ko - o0, d.cases.news.data() + n0,
                    kn - n0, o0, n0, d.smells.olds.data() + to0, d.smells.old_churn.data() + to0, to - to0, d.smells.news.data() + tn0,
                    d.smells.new_churn.data() + tn0, tn - tn0);
+      if (ms.is_open()) move_rows(ms, o.lead(c.step), d.moves, i, km, path);
       t.added[c.step] += d.added[i]; t.removed[c.step] += d.removed[i]; t.files[c.step]++;
       if (!os.is_open() || !(o.zero_rows || d.added[i] || d.removed[i] || c.similarity >= 0)) continue;
       std::vector<std::string> row = o.lead(c.step);
@@ -1851,7 +1944,7 @@ static int cmd_blame(const std::string& repo, const std::string& rev, int64_t ma
   ChangeTotals t(chain.size());
   auto ctx = small_context();
   if (rename_pct >= 0) pair_renames(ctx.get(), h.changes, h.load, rename_pct, batch_bytes, t);
-  pair_batches(ctx.get(), h.changes, h.load, batch_bytes, false, t, [&](const PairBatch& b) {
+  pair_batches(ctx.get(), h.changes, h.load, batch_bytes, false, false, t, [&](const PairBatch& b) {
     // the batch's view of every path it touches: the pair that last wrote it, a lazy state (binary change) or gone
     struct View { int kind; size_t pair; PathState st; };   // kind 0 pair, 1 state, 2 gone
     std::map<std::string, View> view;
@@ -2153,12 +2246,12 @@ static void usage() {
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
           "       tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]\n"
           "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--smells F]\n"
-          "                         [--find-renames N] [--batch-bytes N]\n"
+          "                         [--moves F] [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan body   <project-root>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases <snapshot-root>=<tag>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases --git <repository> [<revision>...] [--batch-bytes N] [--out F]\n"
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
-          "                          [--cases F] [--assert-edits F] [--smells F] [--find-renames N] [--batch-bytes N]\n"
+          "                          [--cases F] [--assert-edits F] [--smells F] [--moves F] [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
           "       tosem-scan clones <project-root>... [--min-lines N] [--all-files] [--out F]\n"
           "       tosem-scan clones --git <repository> [--rev R] [--min-lines N] [--all-files] [--out F]\n"
@@ -2171,6 +2264,9 @@ static void usage() {
           "                  (docs/SPEC.md section 17).\n"
           "--smells F: one row per (test, smell) that a revision introduces, removes or changes, with the smell's instances and the\n"
           "            instance lines it adds and removes (docs/SPEC.md section 19).\n"
+          "--moves F: one row per block of changed lines that a commit moves, within or across its files, as git diff\n"
+          "           --color-moved=blocks finds them (docs/SPEC.md section 20); a commit is never split across batches, and one\n"
+          "           larger than --batch-bytes is a batch of its own.\n"
           "--batch-bytes N: files go to the GPU in batches of at most N bytes (per side of a diff; a larger file alone); scan: 1 GiB, else 512 MiB.\n"
           "Scans run on the GPU through libtosemscan.so (sm_90a); there is no CPU fallback.\n");
 }
@@ -2219,7 +2315,7 @@ int main(int argc, char** argv) {
   DiffOptions d;                                           // diff and history
   d.rename_pct = rename_pct; d.batch_bytes = batch_bytes(kBatch, 1);
   d.out = opt["--out"]; d.asserts = opt["--asserts"]; d.churn = opt["--assert-churn"]; d.cases = opt["--cases"];
-  d.edits = opt["--assert-edits"]; d.smells = opt["--smells"];
+  d.edits = opt["--assert-edits"]; d.smells = opt["--smells"]; d.moves = opt["--moves"];
   const std::string rev = opt.count("--rev") ? opt["--rev"] : "HEAD";
   const int64_t max_commits = opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0;
   if (cmd == "history") { if (pos.size() != 1) die("history needs the repository");

@@ -37,6 +37,8 @@ SMELL_TEST = np.dtype([("file", "<i4"), ("line", "<i4"), ("body_lines", "<i4"), 
 SMELLS = ["empty", "assertion_free", "duplicate_assert", "redundant_assert", "conditional_logic", "exception_handling", "sleepy",
           "print", "ignored"]                   # bit k of tsm_smell_test.smells and of line_smell is SMELLS[k]
 TEST_CHURN = np.dtype([("case_idx", "<i4"), ("instances", "<i4", (9,)), ("churned", "<i4", (9,))])   # tsm_test_churn (section 19)
+MOVE_BLOCK = np.dtype([("line", "<i8"), ("partner", "<i8"), ("n_lines", "<i4"),
+                       ("n_assert", "<i4")])   # tsm_move_block: one moved block of one side (docs/SPEC.md section 20)
 ASSERT_EDIT = np.dtype([("rev", "<i8"), ("aev", "<i8"), ("score", "<i4"), ("_pad", "<i4")])   # tsm_assert_edit: event indices
 
 # every symbol include/tosemscan.h declares (tests check the library exports exactly these)
@@ -47,7 +49,7 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_gen_fill", "tsm_gen_edit", "tsm_gen_pair_sizes", "tsm_gen_pair_fill", "tsm_similarity", "tsm_similarity_last_ms",
            "tsm_diff_pairs_marks", "tsm_blame_pairs", "tsm_blame_last_ms", "tsm_clones", "tsm_clones_last_ms",
            "tsm_diff_pairs_cases", "tsm_diff_pairs_assert_edits", "tsm_assert_edits_last_ms", "tsm_smells", "tsm_smells_last_ms",
-           "tsm_diff_pairs_smells", "tsm_diff_smells_last_ms"]
+           "tsm_diff_pairs_smells", "tsm_diff_smells_last_ms", "tsm_diff_pairs_moves", "tsm_moves_last_ms"]
 
 
 class TsmError(RuntimeError):
@@ -89,6 +91,12 @@ class _DiffSmells(C.Structure):
     _fields_ = [("cases", _DiffCases),
                 ("old_tests", C.c_void_p), ("old_churn", C.c_void_p), ("old_test_cap", C.c_int64), ("n_old_tests", C.c_int64),
                 ("new_tests", C.c_void_p), ("new_churn", C.c_void_p), ("new_test_cap", C.c_int64), ("n_new_tests", C.c_int64)]
+
+
+class _DiffMoves(C.Structure):
+    _fields_ = [("marks", _LineMarks),
+                ("old_blocks", C.c_void_p), ("old_cap", C.c_int64), ("n_old_blocks", C.c_int64),
+                ("new_blocks", C.c_void_p), ("new_cap", C.c_int64), ("n_new_blocks", C.c_int64)]
 
 
 class _CloneResult(C.Structure):
@@ -209,6 +217,11 @@ def lib():
             [C.POINTER(_DiffSmells), C.c_void_p]
         L.tsm_diff_smells_last_ms.restype = C.c_int
         L.tsm_diff_smells_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
+        L.tsm_diff_pairs_moves.restype = C.c_int
+        L.tsm_diff_pairs_moves.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 3 + \
+            [C.POINTER(_DiffMoves), C.c_void_p]
+        L.tsm_moves_last_ms.restype = C.c_int
+        L.tsm_moves_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
         _lib = L
     return _lib
 
@@ -894,6 +907,39 @@ class Scanner:
         k_smell_churn] in ms."""
         ms = (C.c_float * 4)()
         lib().tsm_diff_smells_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
+
+    def diff_moves(self, olds, news, stream=None, cap=None):
+        """Moved code (docs/SPEC.md section 20): a dict of added, removed, detail (tsm_diff_pairs_detail's), line_base_old and
+        line_base_new, dels and ins (diff_marks' marks with bit 1 set on every moved line, so a moved line is 3) and old_blocks and
+        new_blocks (MOVE_BLOCK arrays in line order: global first line, the partner's global line on the other side, lines and
+        assertion lines).  A pair's step is its grp: olds and news must carry the same grp per pair.  Arrays too small for the
+        lines or blocks are sized from the counts and the call is made again (cap: the first guess of each)."""
+        n = olds.n_files
+        added, removed, det = np.zeros(n, np.int64), np.zeros(n, np.int64), np.zeros(max(n, 1), DIFF_DETAIL)
+        bo, bn = np.zeros(n + 1, np.int64), np.zeros(n + 1, np.int64)
+        a, b = olds.c_struct(), news.c_struct()
+        co = cn = bko = bkn = int(cap if cap is not None else 0)
+        for _ in range(2):
+            dels, ins = np.zeros(max(co, 1), np.uint8), np.zeros(max(cn, 1), np.uint8)
+            ob, nb = np.zeros(max(bko, 1), MOVE_BLOCK), np.zeros(max(bkn, 1), MOVE_BLOCK)
+            r = _DiffMoves(_LineMarks(_p(bo), _p(bn), _p(dels), co, 0, _p(ins), cn, 0), _p(ob), bko, 0, _p(nb), bkn, 0)
+            rc = lib().tsm_diff_pairs_moves(self._ctx, C.byref(a), C.byref(b), _p(added), _p(removed), _p(det), C.byref(r), stream)
+            mk = r.marks
+            if rc == TSM_E_CAPACITY and (mk.n_old > co or mk.n_new > cn or r.n_old_blocks > bko or r.n_new_blocks > bkn):
+                co, cn, bko, bkn = int(mk.n_old), int(mk.n_new), int(r.n_old_blocks), int(r.n_new_blocks)
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_diff_pairs_moves")
+            return {"added": added, "removed": removed, "detail": det[:n], "line_base_old": bo, "line_base_new": bn,
+                    "dels": dels[:mk.n_old], "ins": ins[:mk.n_new], "old_blocks": ob[:r.n_old_blocks], "new_blocks": nb[:r.n_new_blocks]}
+        raise TsmError(TSM_E_CAPACITY, "tsm_diff_pairs_moves")
+
+    def moves_last_ms(self):
+        """Device time of the last diff_moves call: [k_scan over both sides, the diff, line flags + join + k_move_reach,
+        k_move_starts + k_move_runs + k_move_mark] in ms."""
+        ms = (C.c_float * 4)()
+        lib().tsm_moves_last_ms(self._ctx, C.byref(ms))
         return [float(x) for x in ms]
 
     def smells_last_ms(self):
