@@ -1,7 +1,9 @@
 #!/usr/bin/env python3
-"""tsm_last_launch_count and an output digest (sha256 of the returned arrays) after one call of every pair and line-records
-entry point, plus the scan and reduce calls, on a fixed small input: 300 gen_pairs revision pairs and two far-apart pairs
-that go to k_myers / k_myers_trace.  Two builds of the library that launch and compute the same print the same object.
+"""tsm_last_launch_count, an output digest (sha256 of the returned arrays) and which phase times are zero after one call of
+every pair and line-records entry point, plus the scan and reduce calls, on a fixed small input: 300 gen_pairs revision pairs,
+two far-apart pairs that go to k_myers / k_myers_trace and two planted test files (cases, smells, a moved block).  The phase
+times are every *_last_ms getter after the call, one character per entry: 0 for zero, + for non-zero.  Two builds of the
+library that launch, compute and time the same phases print the same object.
 
     python tools/launch_counts.py [TREE]      (TREE: the repository whose build is used; default this one)"""
 import hashlib
@@ -36,12 +38,25 @@ nb.append(b"head\n" * 10 + b"x\n" + b"".join(b"m%d\n" % i for i in range(2500)) 
 n = len(ob)
 ext = [1] * n
 A, B = ts.pack(ob, ext, [i % 3 for i in range(n)], 3), ts.pack(nb, ext, [(i + 1) % 3 for i in range(n)], 3)
+# planted tests for the case, smell and move calls: a sleepy test with a duplicate assertion that loses it, a new print test,
+# an edited assertion and a test that moves to the other file of its step
+body = b"    x = compute_the_value(1, 2)\n    assert x == 3\n"
+to = [b"import time\n\ndef test_sleepy():\n    time.sleep(1)\n    assert f(1) == 2\n    assert f(1) == 2\n\ndef test_moved():\n" + body,
+      b"class T:\n    def test_kept(self):\n        self.assertEqual(g(), 1)\n"]
+tn = [b"import time\n\ndef test_sleepy():\n    time.sleep(1)\n    assert f(1) == 2\n\ndef test_new():\n    print(1)\n",
+      b"class T:\n    def test_kept(self):\n        self.assertEqual(g(), 2)\n    def test_moved():\n" + body]
+AT, BT = ts.pack(ob + to, ext + [1, 1]), ts.pack(nb + tn, ext + [1, 1])
+steps = [i * 16 // (n + 2) for i in range(n + 2)]            # moves: 16 steps of consecutive pairs, the same tag on both sides
+AM, BM = ts.pack(ob + to, ext + [1, 1], steps, 16), ts.pack(nb + tn, ext + [1, 1], steps, 16)
 s = ts.Scanner(0, 1 << 24, 4096, 16)
 out = {}
+TIMES = ("diff_last_ms", "similarity_last_ms", "clones_last_ms", "smells_last_ms", "diff_smells_last_ms", "assert_edits_last_ms",
+         "moves_last_ms", "blame_last_ms")
 
 
 def rec(name, res):
-    out[name] = {"launches": s.last_launch_count(), "digest": h(res)}
+    ms = {t: "".join("+" if v else "0" for v in np.atleast_1d(getattr(s, t)())) for t in TIMES}
+    out[name] = {"launches": s.last_launch_count(), "digest": h(res), "ms": ms}
 
 
 c = ts.gen_corpus(0x5EED0002, 400, 1, n_groups=4, pinned=False)
@@ -70,5 +85,13 @@ cl = s.clones(ts.pack(ob + nb, ext + ext), 3)
 rec("clones", [cl[k] for k in ("line_base", "file_dup", "file_dup_assert", "class_base", "class_len", "member")])
 rec("line_hashes", list(s.line_hashes(A, ngram=3)))
 rec("statements", list(s.statements(A)))
+rec("diff_cases", list(s.diff_cases(AT, BT)))
+rec("diff_assert_edits", list(s.diff_assert_edits(AT, BT)))
+r = s.smells(AT)
+rec("smells", [r["line_base"], r["line_smell"], r["tests"]])
+r = s.diff_smells(AT, BT)
+rec("diff_smells", [r[k] for k in sorted(r)])
+r = s.diff_moves(AM, BM)
+rec("diff_moves", [r[k] for k in sorted(r)])
 s.close()
 print(json.dumps(out, sort_keys=True))

@@ -1,5 +1,7 @@
 #!/usr/bin/env python3
-"""Small scan (Rev A and Rev B) + line records + diff (plain, assertion lines, marks, provenance) + similarity + clones + statements + reduce under compute-sanitizer (run: compute-sanitizer --tool memcheck python tools/sanitize_smoke.py)."""
+"""Small scan (Rev A and Rev B) + line records + diff (plain, assertion lines, marks, provenance, test cases, assertion edits,
+smell churn, moved code) + similarity + clones + smells + statements + reduce under compute-sanitizer (run: compute-sanitizer
+--tool memcheck python tools/sanitize_smoke.py)."""
 import os
 import sys
 
@@ -34,6 +36,18 @@ g = s.blame_pairs(ts.pack([far_o[0], far_n[0]], [1, 1]), ts.pack([far_n[0], far_
                   {0: np.array([(-1, j + 1) for j in range(lines0)], ts.ORIGIN)})
 print(len(g[4]), g[4][:3])
 print(s.similarity(fo, ts.pack(far_n + [b"m1\nm2\n"], [1, 1, 1]), [0, 1, 1], [0, 1, 2]))
+# the case, assertion-edit, smell and move calls over the far pair and a test file with cases, smells, an edited assertion
+# and a block that moves between the files of its step
+body = b"    x = compute_the_value(1, 2)\n    assert x == 3\n"
+to = [far_o[0], b"import time\n\ndef test_a():\n    time.sleep(1)\n    assert f(1) == 2\n    assert f(1) == 2\n\ndef test_m():\n" + body]
+tn = [far_n[0] + b"def test_m():\n" + body, b"import time\n\ndef test_a():\n    time.sleep(1)\n    assert f(1) == 3\n"]
+to_, tn_ = ts.pack(to, [1, 1], [0, 0], 1), ts.pack(tn, [1, 1], [0, 0], 1)
+print([len(x) for x in s.diff_cases(to_, tn_)[3:]])
+print(len(s.diff_assert_edits(to_, tn_)[7]))
+print(len(s.smells(to_)["tests"]))
+print({k: len(v) for k, v in s.diff_smells(to_, tn_).items()})
+mv = s.diff_moves(to_, tn_)
+print(len(mv["old_blocks"]), len(mv["new_blocks"]))
 lic = b"".join(b"# licence %d\n" % i for i in range(8))    # clone classes: warp-sorted, CTA-sorted and tiled (> 4 096 fragments)
 cl = s.clones(ts.pack(far_o + far_n + [lic + (b"x\n" if i % 50 else b"") + b"f%d\n" % i for i in range(4200)], [1] * 4204), 3)
 print(len(cl["class_len"]), int(cl["file_dup"].sum()), int(cl["class_len"].max()))

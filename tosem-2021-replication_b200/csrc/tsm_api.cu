@@ -1,6 +1,7 @@
 // tsm_api.cu - the extern "C" boundary of libtosemscan.so (include/tosemscan.h): context, device
 // memory, H2D/D2H staging and kernel launches.  No torch types, no CPU fallback.
 #include <algorithm>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -74,6 +75,31 @@ struct SyncGuard {                                        // error paths: wait f
   ~SyncGuard() { cudaStreamSynchronize(st); }
 };
 
+// The timed calls: tsm_ctx::last_ms[MS_*] holds the phases of the last call of each, which its tsm_*_last_ms returns.
+enum Timed {
+  MS_DIFF,    // k_scan over both sides, k_diff_small, k_myers + k_myers_trace of the last pair call (whose k_scan time is
+              // its own row's for tsm_similarity and tsm_diff_pairs_assert_edits)
+  MS_SIM,     // k_scan over both sides, sort / merge, k_similarity of the last tsm_similarity
+  MS_CLONE,   // k_scan, grouping + classes, members + coverage of the last tsm_clones
+  MS_SMELL,   // k_scan, kinds + case spans, k_smell_lines, k_smell_tests of the last tsm_smells
+  MS_CHURN,   // k_scan, smell stages, the diff, case records + k_smell_churn of the last tsm_diff_pairs_smells
+  MS_EDIT,    // k_scan, the diff, compact to pairing (host clock) of the last tsm_diff_pairs_assert_edits
+  MS_MOVE,    // k_scan, the diff, line flags to k_move_reach, k_move_starts to k_move_mark of the last tsm_diff_pairs_moves
+  MS_BLAME,   // k_blame of the last tsm_blame_pairs
+  N_TIMED
+};
+
+// tsm_ctx::h_rb: the counts a call reads back between its kernels, at fixed offsets in 256 B of pinned memory.
+struct alignas(32) SideCtrl { Ctrl v; };
+struct Readback {
+  SideCtrl ctrl[2];                        // the Ctrl of each side's scan (line records)
+  unsigned long long total[2];             // the line total of each side
+  uint32_t n_todo;                         // the pairs k_diff_small leaves to k_myers
+  alignas(64) unsigned long long u64[4];   // the counts of the call's own stages (clones, smells, smell churn, moves)
+};
+static_assert(offsetof(Readback, ctrl[1]) == 32 && offsetof(Readback, total) == 64 && offsetof(Readback, n_todo) == 80 &&
+              offsetof(Readback, u64) == 128 && sizeof(Readback) <= 256, "Readback: the 256 B block");
+
 struct tsm_ctx {
   int device = 0;
   ScratchPool pool;
@@ -98,17 +124,10 @@ struct tsm_ctx {
   cudaEvent_t slab_ev[64] = {};
   cudaEvent_t ready_ev = nullptr;
   cudaEvent_t order_ev = nullptr;           // recorded behind the device work of every call (CallScope)
-  cudaEvent_t diff_ev[8] = {};             // around the kernels of the diff path (tsm_diff_last_ms): slots EV_*
-  uint8_t* h_diff = nullptr;               // 256 B pinned: what the diff path reads back between its kernels (Ctrl x 2, line totals, todo count)
-  float diff_ms[3] = {0, 0, 0};            // k_scan over both sides, k_myers, k_myers_trace of the last diff
-  float sim_ms[3] = {0, 0, 0};             // k_scan over both sides, sort / merge, k_similarity of the last tsm_similarity
-  float clone_ms[3] = {0, 0, 0};           // k_scan, grouping + classes, members + coverage of the last tsm_clones
-  float smell_ms[4] = {0, 0, 0, 0};        // k_scan, kinds + case spans, k_smell_lines, k_smell_tests of the last tsm_smells
-  float churn_ms[4] = {0, 0, 0, 0};        // k_scan, smell stages, the diff, case records + k_smell_churn of the last tsm_diff_pairs_smells
-  float edit_ms[3] = {0, 0, 0};            // k_scan, the diff, compact to pairing (host clock) of the last assertion-edit call
-  float move_ms[4] = {0, 0, 0, 0};         // k_scan, the diff, line flags to k_move_reach, k_move_starts to k_move_mark of the last tsm_diff_pairs_moves
-  cudaEvent_t blame_ev[2] = {};            // around k_blame (tsm_blame_last_ms)
-  float blame_ms = 0;
+  static constexpr int kEvSlots = 8;
+  cudaEvent_t diff_ev[kEvSlots] = {};      // around the kernels of the pair and line-record calls: slots EV_*
+  Readback* h_rb = nullptr;                // 256 B pinned: what those calls read back between their kernels
+  float last_ms[N_TIMED][4] = {};          // phases of the last call of each timed kind (MS_*)
   struct HostSidePair* res_pair = nullptr; // sides kept in HBM by tsm_diff_upload
   static constexpr int kMaxSlabs = 64;
   tsm_file_stat* d_stats = nullptr;
@@ -133,15 +152,28 @@ struct tsm_ctx {
   long long ms_n = 0;
 };
 
-// Slots of tsm_ctx::diff_ev.  The line records of a revision pair: k_scan of side s from EV_SCAN[s].from to .to.  The diff:
-// k_diff_small over EV_SMALL, each launch for the pairs it leaves over EV_LEFT.  tsm_similarity: the sorted lists of both
-// sides from EV_SIM_LISTS to EV_SIM_PAIRS, k_similarity from there to EV_SIM_END.  tsm_clones: grouping and classes from
-// EV_CLONE_GROUP to EV_CLONE_MEMBERS, members and coverage from there to EV_CLONE_END.
+// Slots of tsm_ctx::diff_ev, by call and phase.  Each phase reads its slots behind a synchronisation of its own, and a later
+// phase records a slot again only after that: the rows below a call's line-record row reuse slots that have been read.
+//
+//   phase                                  0       1       2       3       4       5       6       7       read
+//   line records of side 0 / 1 (k_scan)    SCAN[0] SCAN[0]                                 SCAN[1] SCAN[1] sides_records
+//   diff_core                                              SMALL   SMALL   LEFT    LEFT                    diff_core, per launch
+//   tsm_similarity                                         LISTS   PAIRS   END                             at the end
+//   tsm_clones                                             GROUP   MEMBERS END                             at the members / end
+//   tsm_smells (smell_stage: LINES - END)                  KINDS   LINES   TESTS   END                     at the end
+//   tsm_diff_pairs_smells: smell stages    CHURN_SMELLS            LINES*  TESTS*  END*                    before the diff
+//     case records + churn, behind diff    CHURN_CASES                                                     at the end
+//   tsm_diff_pairs_moves, behind the diff  MOVE_FLAGS      MOVE_JOIN       MOVE_RUNS       MOVE_MARK       at the end
+//   tsm_blame_pairs, behind the diff       BLAME                                                           at the end
+//   (* recorded by smell_stage, and not read in this call)
 struct EvSpan { int from, to; };
 constexpr EvSpan EV_SCAN[2] = {{0, 1}, {6, 7}}, EV_SMALL = {2, 3}, EV_LEFT = {4, 5};
 constexpr int EV_SIM_LISTS = 2, EV_SIM_PAIRS = 3, EV_SIM_END = 4;
 constexpr int EV_CLONE_GROUP = 2, EV_CLONE_MEMBERS = 3, EV_CLONE_END = 4;
 constexpr int EV_SMELL_KINDS = 2, EV_SMELL_LINES = 3, EV_SMELL_TESTS = 4, EV_SMELL_END = 5;
+constexpr EvSpan EV_CHURN_SMELLS = {0, 1}, EV_CHURN_CASES = {0, 1};   // the old side's scan slots, then the same again
+constexpr EvSpan EV_MOVE_FLAGS = {0, 1}, EV_MOVE_JOIN = {2, 3}, EV_MOVE_RUNS = {4, 5}, EV_MOVE_MARK = {6, 7};
+constexpr EvSpan EV_BLAME = {0, 1};
 
 // The start of every call that queues device work on st: the ctx's device, the ctx's pool for the call's DevBufs, and the
 // order of the ctx's calls.  A ctx orders its own work, whatever stream each call is given: the call's stream first waits
@@ -150,9 +182,9 @@ constexpr int EV_SMELL_KINDS = 2, EV_SMELL_LINES = 3, EV_SMELL_TESTS = 4, EV_SME
 // Order of a call's objects: this scope, then the DevBufs (and the HostSides that hold them), then a SyncGuard.
 // Destruction runs backwards: the SyncGuard waits for st before any buffer goes back to the pool (the next call may
 // reuse or free it), and the order event is recorded behind all of it.  A helper that takes DevBufs of its own
-// (diff_core, diff_asserts, the tails of line_records) synchronises st before it returns them on success; on an error
-// it returns them at once, but the call then unwinds without allocating again and its SyncGuard waits for st before
-// the call returns.
+// (diff_core, diff_asserts, the tails of line_records and pair_call) synchronises st before it returns them on success;
+// on an error it returns them at once, but the call then unwinds without allocating again and its SyncGuard waits for
+// st before the call returns.
 struct CallScope {
   tsm_ctx* c; cudaStream_t st;
   PoolScope pool;
@@ -260,11 +292,10 @@ extern "C" void tsm_destroy(tsm_ctx* c) {
   if (c->ready_ev) cudaEventDestroy(c->ready_ev);
   if (c->order_ev) cudaEventDestroy(c->order_ev);
   for (cudaEvent_t e : c->diff_ev) if (e) cudaEventDestroy(e);
-  for (cudaEvent_t e : c->blame_ev) if (e) cudaEventDestroy(e);
   free_res_pair(c);
   cudaFree(c->d_cand); cudaFree(c->d_hev); cudaFree(c->d_aev);
   if (c->h_ctrl) cudaFreeHost(c->h_ctrl);
-  if (c->h_diff) cudaFreeHost(c->h_diff);
+  if (c->h_rb) cudaFreeHost(c->h_rb);
   for (auto& set : c->ev) for (cudaEvent_t e : set) if (e) cudaEventDestroy(e);
   delete c;
 }
@@ -315,11 +346,10 @@ extern "C" int tsm_create(tsm_ctx** out, int device, int64_t max_arena_bytes, in
   if (rc == TSM_OK && cudaEventCreateWithFlags(&c->ready_ev, cudaEventDisableTiming) != cudaSuccess) rc = TSM_E_CUDA;
   if (rc == TSM_OK && cudaEventCreateWithFlags(&c->order_ev, cudaEventDisableTiming) != cudaSuccess) rc = TSM_E_CUDA;
   for (cudaEvent_t& e : c->diff_ev) if (rc == TSM_OK && cudaEventCreate(&e) != cudaSuccess) rc = TSM_E_CUDA;
-  for (cudaEvent_t& e : c->blame_ev) if (rc == TSM_OK && cudaEventCreate(&e) != cudaSuccess) rc = TSM_E_CUDA;
   A((void**)&c->d_stats, sizeof(tsm_file_stat) * (size_t)max_files);
   A((void**)&c->d_cand, sizeof(unsigned long long) * (size_t)c->max_events);
   if (rc == TSM_OK && cudaHostAlloc((void**)&c->h_ctrl, sizeof(Ctrl) + 64, cudaHostAllocDefault) != cudaSuccess) rc = TSM_E_CUDA;
-  if (rc == TSM_OK && cudaHostAlloc((void**)&c->h_diff, 256, cudaHostAllocDefault) != cudaSuccess) rc = TSM_E_CUDA;
+  if (rc == TSM_OK && cudaHostAlloc((void**)&c->h_rb, 256, cudaHostAllocDefault) != cudaSuccess) rc = TSM_E_CUDA;
   for (auto& set : c->ev) for (cudaEvent_t& e : set) if (rc == TSM_OK && cudaEventCreate(&e) != cudaSuccess) rc = TSM_E_CUDA;
   if (rc == TSM_OK) {
     uint32_t lut[256];
@@ -775,6 +805,15 @@ static float elapsed_ms(cudaEvent_t from, cudaEvent_t to) {   // 0 if the pair c
   float ms = 0;
   return cudaEventElapsedTime(&ms, from, to) == cudaSuccess ? ms : 0.f;
 }
+static float span_ms(const tsm_ctx* c, EvSpan s) { return elapsed_ms(c->diff_ev[s.from], c->diff_ev[s.to]); }
+
+// The phase times of the timed call t: cleared at the start of the call, copied out by its tsm_*_last_ms (n of them).
+static float* clear_ms(tsm_ctx* c, Timed t) { std::fill_n(c->last_ms[t], 4, 0.f); return c->last_ms[t]; }
+static int copy_ms(const tsm_ctx* c, Timed t, float* out, int n) {
+  if (!c || !out) return TSM_E_ARG;
+  std::copy_n(c->last_ms[t], n, out);
+  return TSM_OK;
+}
 
 namespace {
 struct HostSide {                                         // device image of one side of the pairs + its line records
@@ -787,7 +826,6 @@ struct HostSide {                                         // device image of one
   uint32_t n_units = 0;                                   // (file, chunk) work units: sum of ceil(len / 4 KiB)
   Ctrl hc{};                                              // read back behind the scan: capacity flags, lines written
   unsigned long long total = 0;                           // lines of the side
-  Ctrl* pin_hc = nullptr; unsigned long long* pin_total = nullptr;   // where they land (pinned, in the ctx)
   DiffSide d{};
   int launches = 0;
   void drop_staging() { s_hash.reset(); s_end.reset(); s_flag.reset(); }
@@ -854,8 +892,6 @@ int side_upload_grp(const tsm_corpus* k, HostSide& h, cudaStream_t st) {
 // host_base: also copy line_base to the host (HostSide::base).  flags: TSM_SCAN_HEADER_EVENTS also lists the header events
 // into HostSide::hev (hc.n_hev of them), sized like the staging arrays: a side has no more headers than lines.
 static int side_scan_pass(tsm_ctx* c, HostSide& h, ScanParams& p, size_t cap, int side, cudaStream_t st) {
-  h.pin_hc = reinterpret_cast<Ctrl*>(c->h_diff + 32 * side);            // pinned: the copies below do not stall the host
-  h.pin_total = reinterpret_cast<unsigned long long*>(c->h_diff + 64 + 8 * side);
   const int32_t n = h.n;
   if (cap > 0xFFFFFFF0ull) return TSM_E_CAPACITY;
   if (!h.s_hash.alloc(sizeof(unsigned long long) * cap) || !h.s_end.alloc(sizeof(uint32_t) * cap) || !h.s_flag.alloc(cap)) return TSM_E_CUDA;
@@ -873,8 +909,9 @@ static int side_scan_pass(tsm_ctx* c, HostSide& h, ScanParams& p, size_t cap, in
   CU(cudaGetLastError());
   // lines per unit -> first line of every unit (the unit count is known on the host: units are (file, chunk) in order)
   xscan(p.unit_lines, h.n_units, h.bsum.as<unsigned long long>(), h.unit_line_base.as<unsigned long long>(), st);
-  CU(cudaMemcpyAsync(h.pin_hc, p.ctrl, sizeof(Ctrl), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(h.pin_total, h.unit_line_base.as<unsigned long long>() + h.n_units, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(&c->h_rb->ctrl[side].v, p.ctrl, sizeof(Ctrl), cudaMemcpyDeviceToHost, st));   // pinned: no host stall
+  CU(cudaMemcpyAsync(&c->h_rb->total[side], h.unit_line_base.as<unsigned long long>() + h.n_units, sizeof(unsigned long long),
+                     cudaMemcpyDeviceToHost, st));
   h.launches += 6;
   return TSM_OK;
 }
@@ -905,16 +942,15 @@ int sides_records(tsm_ctx* c, HostSide* const* sides, int ns, cudaStream_t st, f
   CU(cudaStreamSynchronize(st));
   for (int i = 0; i < ns; ++i) {
     HostSide& h = *sides[i];
-    const EvSpan ev = EV_SCAN[i];
-    h.hc = *h.pin_hc; h.total = *h.pin_total;
-    if (scan_ms) *scan_ms += elapsed_ms(c->diff_ev[ev.from], c->diff_ev[ev.to]);
+    h.hc = c->h_rb->ctrl[i].v; h.total = c->h_rb->total[i];
+    if (scan_ms) *scan_ms += span_ms(c, EV_SCAN[i]);
     if (h.hc.overflow && !h.hc.lh_overflow) return TSM_E_CAPACITY;   // (header events overflow only with the lines that bound them)
     if (h.hc.lh_overflow) {                                // more lines than the staging arrays hold: once more, exact size
       const int rc = side_scan_pass(c, h, ps[i], (size_t)h.hc.n_lh + 64, i, st);
       if (rc != TSM_OK) return rc;
       CU(cudaStreamSynchronize(st));
-      h.hc = *h.pin_hc; h.total = *h.pin_total;
-      if (scan_ms) *scan_ms += elapsed_ms(c->diff_ev[ev.from], c->diff_ev[ev.to]);
+      h.hc = c->h_rb->ctrl[i].v; h.total = c->h_rb->total[i];
+      if (scan_ms) *scan_ms += span_ms(c, EV_SCAN[i]);
       if (h.hc.overflow || h.hc.lh_overflow) return TSM_E_CAPACITY;
     }
   }
@@ -972,12 +1008,12 @@ static void free_res_pair(tsm_ctx* c) {
   c->res_pair = nullptr;
 }
 
-// The corpora of the diff and line-record calls (n > 0 files each): arena, off and len given, and the per-file layout rules
+// The corpora of the diff and line-record calls (n_files > 0 each): arena, off and len given, and the per-file layout rules
 // of the scan.  Their grp is not part of it: only the assertion tables use it.
-static int check_sides(std::initializer_list<const tsm_corpus*> sides, int32_t n, bool ext_rule) {
+static int check_sides(std::initializer_list<const tsm_corpus*> sides, bool ext_rule) {
   for (const tsm_corpus* k : sides) {
     if (!k->arena || !k->off || !k->len) return TSM_E_ARG;
-    const int rc = check_files(k, 0, n, ext_rule, false);
+    const int rc = check_files(k, 0, k->n_files, ext_rule, false);
     if (rc != TSM_OK) return rc;
   }
   return TSM_OK;
@@ -1005,6 +1041,33 @@ static int pair_records(tsm_ctx* c, HostSidePair& P, float* scan_ms, bool host_b
   return sides_records(c, both, 2, st, scan_ms, host_base, flags);
 }
 
+// What a revision-pair call asks of pair_call, beside the TSM_SCAN_* flags of the line records (TSM_SCAN_HEADER_EVENTS).
+enum : uint32_t {
+  PAIR_ANY_EXT = 1u << 16,                                 // no ext <= TSM_EXT_H rule in check_sides
+  PAIR_GRP = 1u << 17,                                     // the group tags of both sides too (pair_upload's with_grp)
+  PAIR_HOST_BASE = 1u << 18,                               // line_base of each side on the host too (HostSide::base)
+};
+static_assert((TSM_SCAN_ASSERT_EVENTS | TSM_SCAN_HEADER_EVENTS | TSM_SCAN_LINE_HASHES | TSM_SCAN_REV_B) < PAIR_ANY_EXT, "PAIR_*");
+
+// The front of every call over uploaded revision pairs (n_files > 0 on both sides; the caller checks its own arguments and
+// returns early for none): check_sides, the CallScope, both sides to the device, their line records (*scan_ms = k_scan over
+// both), then tail(P, st), the call's own use of them, inside the call's SyncGuard.  The tail keeps the rule of CallScope:
+// it synchronises st before it returns on success, and on an error it returns without allocating again.
+template <typename Tail>
+static int pair_call(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, uint32_t opts, float* scan_ms, void* stream,
+                     Tail tail) {
+  int rc = check_sides({olds, news}, !(opts & PAIR_ANY_EXT));
+  if (rc != TSM_OK) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  CallScope call(c, st);
+  CU(call.status);
+  HostSidePair P;
+  SyncGuard guard(st);
+  rc = pair_upload(olds, news, opts & PAIR_GRP, P, st);
+  if (rc == TSM_OK) rc = pair_records(c, P, scan_ms, opts & PAIR_HOST_BASE, st, opts & TSM_SCAN_HEADER_EVENTS);
+  return rc != TSM_OK ? rc : tail(P, st);
+}
+
 // The diff proper over two sides whose line records exist.  k_diff_small finishes the common pairs (distance at most
 // 127 lines, middle of at most 4 096 lines) start to finish - search in registers, rows of V and backtrack in shared
 // memory - in the sizes of DS_SIZES, each fed on the device by the list the size before it leaves.  What all of them
@@ -1012,7 +1075,7 @@ static int pair_records(tsm_ctx* c, HostSidePair& P, float* scan_ms, bool host_b
 // k_myers_trace (rows of V in global memory sized from those distances, then the canonical script: hunks, changed
 // assertion lines).  A pair whose distance D needs more than TSM_DIFF_TRACE_MAX_INTS trace entries ((D+1)(D+2)/2) is
 // not traced: it is reported as ONE hunk (add / del / mod by its counts) with added_assert = removed_assert = -1
-// (tosemscan.h).  diff_ms[1] = k_diff_small, diff_ms[2] = the two kernels of the left-over pairs.
+// (tosemscan.h).  last_ms[MS_DIFF][1] = k_diff_small, [2] = the two kernels of the left-over pairs.
 // MODE (DiffMode) picks the variant of k_diff_small and k_myers_trace: DIFF_EMIT also lists the changed assertion lines
 // into the caller's sink, DIFF_MARKS marks the deleted and inserted lines into A.line_mark / B.line_mark (one zeroed byte
 // per line of each side).  Both find those lines on the paths that compute the detail (the assertion flags come with it),
@@ -1054,7 +1117,7 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
   });
   CU(cudaEventRecord(c->diff_ev[EV_SMALL.to], st));
   CU(cudaGetLastError());
-  uint32_t* pin_nt = reinterpret_cast<uint32_t*>(c->h_diff + 80);
+  uint32_t* pin_nt = &c->h_rb->n_todo;
   CU(cudaMemcpyAsync(pin_nt, cnt + DS_N - 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(added, d_add.p, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(removed, d_rem.p, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
@@ -1062,9 +1125,10 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
   CU(cudaStreamSynchronize(st));
   A.drop_staging(); B.drop_staging();
   const uint32_t nt = *pin_nt;
-  c->diff_ms[1] = elapsed_ms(c->diff_ev[EV_SMALL.from], c->diff_ev[EV_SMALL.to]);
+  float* const ms = c->last_ms[MS_DIFF];
+  ms[1] = span_ms(c, EV_SMALL);
   c->launches = A.launches + B.launches + DS_N;
-  c->diff_ms[2] = 0;
+  ms[2] = 0;
   if (nt == 0) return TSM_OK;
   // ---- the left-over pairs: long middles, far-apart revisions
   std::vector<int32_t> todo(nt);
@@ -1092,7 +1156,7 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
   CU(cudaMemcpyAsync(added, d_add.p, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(removed, d_rem.p, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  c->diff_ms[2] += elapsed_ms(c->diff_ev[EV_LEFT.from], c->diff_ev[EV_LEFT.to]);
+  ms[2] += span_ms(c, EV_LEFT);
   c->launches++;
   if (!detail) return TSM_OK;
   // ---- their hunks: second search with the rows of V kept; rows sized from the distances just computed,
@@ -1130,7 +1194,7 @@ static int diff_core(tsm_ctx* c, HostSide& A, HostSide& B, int32_t n, int64_t* a
     CU(cudaEventRecord(c->diff_ev[EV_LEFT.to], st));
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(st));
-    c->diff_ms[2] += elapsed_ms(c->diff_ev[EV_LEFT.from], c->diff_ev[EV_LEFT.to]);
+    ms[2] += span_ms(c, EV_LEFT);
     c->launches++;
     p0 = p1;
   }
@@ -1216,12 +1280,9 @@ static int classify_changed(tsm_ctx* c, HostSide* const side[2], unsigned long l
   return TSM_OK;
 }
 
-// One diff call over the uploaded sides of P: their line records (diff_ms[0] = k_scan over both), then diff_core, or
-// diff_asserts when `out` is given.  The caller holds the CallScope and the SyncGuard of the call.
+// The plain and the assertion diff behind the line records of P: diff_core, or diff_asserts when `out` is given.
 static int pair_run(tsm_ctx* c, HostSidePair& P, int64_t* added, int64_t* removed, tsm_diff_detail* detail,
                     tsm_diff_asserts* out, cudaStream_t st) {
-  const int rc = pair_records(c, P, &c->diff_ms[0], false, st);
-  if (rc != TSM_OK) return rc;
   if (out) return diff_asserts(c, P.A, P.B, P.n, P.groups_a, added, removed, detail, out, st);
   return diff_core<DIFF_PLAIN>(c, P.A, P.B, P.n, added, removed, detail, st);
 }
@@ -1230,15 +1291,9 @@ extern "C" int tsm_diff_pairs_detail(tsm_ctx* c, const tsm_corpus* olds, const t
                                      int64_t* added, int64_t* removed, tsm_diff_detail* detail, void* stream) {
   if (!c || !olds || !news || !added || !removed || olds->n_files != news->n_files) return TSM_E_ARG;
   if (olds->n_files == 0) return TSM_OK;
-  int rc = check_sides({olds, news}, olds->n_files, detail != nullptr);
-  if (rc != TSM_OK) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  CallScope call(c, st);
-  CU(call.status);
-  HostSidePair P;
-  SyncGuard guard(st);
-  rc = pair_upload(olds, news, false, P, st);
-  return rc != TSM_OK ? rc : pair_run(c, P, added, removed, detail, nullptr, st);
+  return pair_call(c, olds, news, detail ? 0u : PAIR_ANY_EXT, &c->last_ms[MS_DIFF][0], stream, [&](HostSidePair& P, cudaStream_t st) {
+    return pair_run(c, P, added, removed, detail, nullptr, st);
+  });
 }
 
 extern "C" int tsm_diff_pairs(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news,
@@ -1260,21 +1315,15 @@ extern "C" int tsm_diff_pairs_asserts(tsm_ctx* c, const tsm_corpus* olds, const 
       if (t) memset(t, 0, sizeof(int64_t) * (size_t)olds->n_groups * TSM_K);
     return TSM_OK;
   }
-  rc = check_sides({olds, news}, n, true);
-  if (rc != TSM_OK) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  CallScope call(c, st);
-  CU(call.status);
-  HostSidePair P;
-  SyncGuard guard(st);
-  rc = pair_upload(olds, news, true, P, st);
-  return rc != TSM_OK ? rc : pair_run(c, P, added, removed, detail, out, st);
+  return pair_call(c, olds, news, PAIR_GRP, &c->last_ms[MS_DIFF][0], stream, [&](HostSidePair& P, cudaStream_t st) {
+    return pair_run(c, P, added, removed, detail, out, st);
+  });
 }
 
 // Resident variant (what bench.py's `value` times for config C5): the two sides go to HBM once ...
 extern "C" int tsm_diff_upload(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, void* stream) {
   if (!c || !olds || !news || olds->n_files != news->n_files || olds->n_files <= 0) return TSM_E_ARG;
-  int rc = check_sides({olds, news}, olds->n_files, true);
+  int rc = check_sides({olds, news}, true);
   if (rc != TSM_OK) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   CallScope call(c, st);
@@ -1290,14 +1339,19 @@ extern "C" int tsm_diff_upload(tsm_ctx* c, const tsm_corpus* olds, const tsm_cor
 }
 
 // ... and every call runs the kernels over them: k_scan over both sides (line records), k_myers, k_myers_trace.
-extern "C" int tsm_diff_resident(tsm_ctx* c, int64_t* added, int64_t* removed, tsm_diff_detail* detail, void* stream) {
-  if (!c || !added || !removed) return TSM_E_ARG;
-  if (!c->res_pair) return TSM_E_STATE;
+static int resident_run(tsm_ctx* c, int64_t* added, int64_t* removed, tsm_diff_detail* detail, tsm_diff_asserts* out, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   CallScope call(c, st);
   CU(call.status);
   SyncGuard guard(st);
-  return pair_run(c, *c->res_pair, added, removed, detail, nullptr, st);
+  const int rc = pair_records(c, *c->res_pair, &c->last_ms[MS_DIFF][0], false, st);
+  return rc != TSM_OK ? rc : pair_run(c, *c->res_pair, added, removed, detail, out, st);
+}
+
+extern "C" int tsm_diff_resident(tsm_ctx* c, int64_t* added, int64_t* removed, tsm_diff_detail* detail, void* stream) {
+  if (!c || !added || !removed) return TSM_E_ARG;
+  if (!c->res_pair) return TSM_E_STATE;
+  return resident_run(c, added, removed, detail, nullptr, stream);
 }
 
 extern "C" int tsm_diff_resident_asserts(tsm_ctx* c, int64_t* added, int64_t* removed, tsm_diff_detail* detail,
@@ -1307,18 +1361,10 @@ extern "C" int tsm_diff_resident_asserts(tsm_ctx* c, int64_t* added, int64_t* re
   if (c->res_pair->groups_a != c->res_pair->groups_b) return TSM_E_ARG;
   if (!c->res_pair->grp_ok) return TSM_E_LAYOUT;
   out->n_aev = out->n_rev = 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  CallScope call(c, st);
-  CU(call.status);
-  SyncGuard guard(st);
-  return pair_run(c, *c->res_pair, added, removed, detail, out, st);
+  return resident_run(c, added, removed, detail, out, stream);
 }
 
-extern "C" int tsm_diff_last_ms(tsm_ctx* c, float* ms3) {
-  if (!c || !ms3) return TSM_E_ARG;
-  for (int i = 0; i < 3; ++i) ms3[i] = c->diff_ms[i];
-  return TSM_OK;
-}
+extern "C" int tsm_diff_last_ms(tsm_ctx* c, float* ms3) { return copy_ms(c, MS_DIFF, ms3, 3); }
 
 // ------------------------------------------------------------------------------------- SPEC section 14 line provenance
 extern "C" int tsm_diff_pairs_marks(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
@@ -1328,27 +1374,19 @@ extern "C" int tsm_diff_pairs_marks(tsm_ctx* c, const tsm_corpus* olds, const ts
   const int32_t n = olds->n_files;
   mk->n_old = mk->n_new = 0;
   if (n == 0) { mk->line_base_old[0] = mk->line_base_new[0] = 0; return TSM_OK; }
-  int rc = check_sides({olds, news}, n, true);
-  if (rc != TSM_OK) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  CallScope call(c, st);
-  CU(call.status);
-  HostSidePair P;
-  SyncGuard guard(st);
-  rc = pair_upload(olds, news, false, P, st);
-  if (rc == TSM_OK) rc = pair_records(c, P, &c->diff_ms[0], true, st);
-  if (rc != TSM_OK) return rc;
-  memcpy(mk->line_base_old, P.A.base.data(), sizeof(int64_t) * ((size_t)n + 1));
-  memcpy(mk->line_base_new, P.B.base.data(), sizeof(int64_t) * ((size_t)n + 1));
-  mk->n_old = (int64_t)P.A.total; mk->n_new = (int64_t)P.B.total;
-  if (mk->del_cap < mk->n_old || mk->ins_cap < mk->n_new) return TSM_E_CAPACITY;
-  if ((mk->n_old && !mk->del) || (mk->n_new && !mk->ins)) return TSM_E_ARG;
-  rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
-  if (rc != TSM_OK) return rc;
-  if (mk->n_old) CU(cudaMemcpyAsync(mk->del, P.A.line_mark.p, (size_t)mk->n_old, cudaMemcpyDeviceToHost, st));
-  if (mk->n_new) CU(cudaMemcpyAsync(mk->ins, P.B.line_mark.p, (size_t)mk->n_new, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  return TSM_OK;
+  return pair_call(c, olds, news, PAIR_HOST_BASE, &c->last_ms[MS_DIFF][0], stream, [&](HostSidePair& P, cudaStream_t st) -> int {
+    memcpy(mk->line_base_old, P.A.base.data(), sizeof(int64_t) * ((size_t)n + 1));
+    memcpy(mk->line_base_new, P.B.base.data(), sizeof(int64_t) * ((size_t)n + 1));
+    mk->n_old = (int64_t)P.A.total; mk->n_new = (int64_t)P.B.total;
+    if (mk->del_cap < mk->n_old || mk->ins_cap < mk->n_new) return TSM_E_CAPACITY;
+    if ((mk->n_old && !mk->del) || (mk->n_new && !mk->ins)) return TSM_E_ARG;
+    const int rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
+    if (rc != TSM_OK) return rc;
+    if (mk->n_old) CU(cudaMemcpyAsync(mk->del, P.A.line_mark.p, (size_t)mk->n_old, cudaMemcpyDeviceToHost, st));
+    if (mk->n_new) CU(cudaMemcpyAsync(mk->ins, P.B.line_mark.p, (size_t)mk->n_new, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    return TSM_OK;
+  });
 }
 
 // ------------------------------------------------------------------------------------- SPEC section 16 test-case churn
@@ -1374,10 +1412,17 @@ static int case_spans(const HostSide& h, CaseSpans& sp, DevBuf& bsum, int& launc
   return TSM_OK;
 }
 
+// The kept rank of every line of a side behind the marks diff: k_case_kept (kept[l] = 1 on the lines the diff keeps) and its
+// xscan (rank[l] = the kept lines before l; rank[total] = all of them).  kept holds total u32, rank total + 1 u64.
+static void kept_ranks(const HostSide& h, DevBuf& kept, DevBuf& rank, DevBuf& bsum, cudaStream_t st) {
+  const uint32_t total = (uint32_t)h.total;
+  if (total) k_case_kept<<<(total + 255) / 256, 256, 0, st>>>(h.line_mark.as<uint8_t>(), total, kept.as<uint32_t>());
+  xscan(kept.as<uint32_t>(), total, bsum.as<unsigned long long>(), rank.as<unsigned long long>(), st);
+}
+
 // The cases of both sides of the revision pairs: their spans before the marks diff (pair_case_spans), their records behind it
-// (case_records): per side k_case_kept and xscan of the kept lines (rank: the kept rank of every line), k_case_lines for
-// by_rank (the kept line of every rank: the old side's always, the new side's when asked for) and k_case_reduce (the new
-// side's step-1 match reads the old side's by_rank, head and case_of).
+// (case_records): per side kept_ranks, k_case_lines for by_rank (the kept line of every rank: the old side's always, the new
+// side's when asked for) and k_case_reduce (the new side's step-1 match reads the old side's by_rank, head and case_of).
 struct PairCases { CaseSpans sp[2]; DevBuf kept[2], rank[2], by_rank[2], cases[2], bsum; };
 
 static int pair_case_spans(const HostSidePair& P, PairCases& pc, int& launches, cudaStream_t st) {
@@ -1395,8 +1440,7 @@ static int case_records(tsm_ctx* c, const HostSidePair& P, PairCases& pc, bool n
     if (!pc.kept[s].alloc(sizeof(uint32_t) * (size_t)total) || !pc.rank[s].alloc(sizeof(unsigned long long) * ((size_t)total + 1)) ||
         !pc.cases[s].alloc(sizeof(tsm_case) * (size_t)pc.sp[s].n_cases) || (by_rank && !pc.by_rank[s].alloc(sizeof(uint32_t) * (size_t)total)))
       return TSM_E_CUDA;
-    if (total) k_case_kept<<<(total + 255) / 256, 256, 0, st>>>(h.line_mark.as<uint8_t>(), total, pc.kept[s].as<uint32_t>());
-    xscan(pc.kept[s].as<uint32_t>(), total, pc.bsum.as<unsigned long long>(), pc.rank[s].as<unsigned long long>(), st);
+    kept_ranks(h, pc.kept[s], pc.rank[s], pc.bsum, st);
     if (total && by_rank)
       k_case_lines<<<(total + 255) / 256, 256, 0, st>>>(pc.sp[s].head.as<uint32_t>(), pc.kept[s].as<uint32_t>(),
                                                         pc.sp[s].case_of.as<unsigned long long>(), pc.rank[s].as<unsigned long long>(),
@@ -1426,31 +1470,23 @@ extern "C" int tsm_diff_pairs_cases(tsm_ctx* c, const tsm_corpus* olds, const ts
   const int32_t n = olds->n_files;
   out->n_old = out->n_new = 0;
   if (n == 0) return TSM_OK;
-  int rc = check_sides({olds, news}, n, true);
-  if (rc != TSM_OK) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  CallScope call(c, st);
-  CU(call.status);
-  HostSidePair P;
-  PairCases pc;
-  SyncGuard guard(st);
-  rc = pair_upload(olds, news, false, P, st);
-  if (rc == TSM_OK) rc = pair_records(c, P, &c->diff_ms[0], false, st, TSM_SCAN_HEADER_EVENTS);
-  if (rc != TSM_OK) return rc;
-  out->n_old = P.A.hc.n_hev; out->n_new = P.B.hc.n_hev;
-  if (out->old_cap < out->n_old || out->new_cap < out->n_new) return TSM_E_CAPACITY;
-  if ((out->n_old && !out->old_cases) || (out->n_new && !out->new_cases)) return TSM_E_ARG;
-  int launches = 0;
-  rc = pair_case_spans(P, pc, launches, st);
-  if (rc == TSM_OK) rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
-  if (rc == TSM_OK) rc = case_records(c, P, pc, false, launches, st);
-  if (rc != TSM_OK) return rc;
-  tsm_case* const h_out[2] = {out->old_cases, out->new_cases};
-  for (int s = 0; s < 2; ++s)
-    if (pc.sp[s].n_cases) CU(cudaMemcpyAsync(h_out[s], pc.cases[s].p, sizeof(tsm_case) * pc.sp[s].n_cases, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  c->launches += launches;
-  return TSM_OK;
+  return pair_call(c, olds, news, TSM_SCAN_HEADER_EVENTS, &c->last_ms[MS_DIFF][0], stream, [&](HostSidePair& P, cudaStream_t st) -> int {
+    out->n_old = P.A.hc.n_hev; out->n_new = P.B.hc.n_hev;
+    if (out->old_cap < out->n_old || out->new_cap < out->n_new) return TSM_E_CAPACITY;
+    if ((out->n_old && !out->old_cases) || (out->n_new && !out->new_cases)) return TSM_E_ARG;
+    PairCases pc;
+    int launches = 0;
+    int rc = pair_case_spans(P, pc, launches, st);
+    if (rc == TSM_OK) rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
+    if (rc == TSM_OK) rc = case_records(c, P, pc, false, launches, st);
+    if (rc != TSM_OK) return rc;
+    tsm_case* const h_out[2] = {out->old_cases, out->new_cases};
+    for (int s = 0; s < 2; ++s)
+      if (pc.sp[s].n_cases) CU(cudaMemcpyAsync(h_out[s], pc.cases[s].p, sizeof(tsm_case) * pc.sp[s].n_cases, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    c->launches += launches;
+    return TSM_OK;
+  });
 }
 
 // ------------------------------------------------------------------------------------- SPEC section 17 assertion edits
@@ -1541,119 +1577,104 @@ extern "C" int tsm_diff_pairs_assert_edits(tsm_ctx* c, const tsm_corpus* olds, c
   if (rc != TSM_OK) return rc;
   chg->n_aev = chg->n_rev = 0;
   *n_edits = 0;
-  for (float& ms : c->edit_ms) ms = 0;
+  float* const ms = clear_ms(c, MS_EDIT);
   if (n == 0) {
     for (int64_t* t : {chg->added_counts, chg->removed_counts})
       if (t) memset(t, 0, sizeof(int64_t) * (size_t)olds->n_groups * TSM_K);
     return TSM_OK;
   }
-  rc = check_sides({olds, news}, n, true);
-  if (rc != TSM_OK) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  CallScope call(c, st);
-  CU(call.status);
-  HostSidePair P;
-  DevBuf d_traced, d_flag[2], d_pos[2], d_kept[2], d_rank[2], d_lines[2], d_cand[2], d_bsum, d_ctrl;
-  SyncGuard guard(st);
-  rc = pair_upload(olds, news, true, P, st);
-  if (rc == TSM_OK) rc = pair_records(c, P, &c->edit_ms[0], false, st);
-  if (rc != TSM_OK) return rc;
-  std::vector<tsm_diff_detail> own;
-  if (!detail) { own.resize((size_t)n); detail = own.data(); }
-  rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
-  if (rc != TSM_OK) return rc;
-  c->edit_ms[1] = c->diff_ms[1] + c->diff_ms[2];
-  const auto t0 = std::chrono::steady_clock::now();
-  std::vector<uint8_t> traced((size_t)n);
-  for (int32_t i = 0; i < n; ++i) traced[(size_t)i] = detail[i].added_assert >= 0;
-  HostSide* side[2] = {&P.A, &P.B};
-  if (!d_traced.alloc((size_t)n) || !d_ctrl.alloc(2 * 64) ||
-      !d_bsum.alloc(sizeof(unsigned long long) * ((size_t)std::max(P.A.total, P.B.total) / XS_TILE + 4)))
-    return TSM_E_CUDA;
-  CU(cudaMemcpyAsync(d_traced.p, traced.data(), (size_t)n, cudaMemcpyHostToDevice, st));
-  unsigned long long cnt[2] = {0, 0};
-  EditSide es[2];
-  for (int s = 0; s < 2; ++s) {
-    const HostSide& h = *side[s];
-    const uint32_t total = (uint32_t)h.total;
-    if (!d_flag[s].alloc(sizeof(uint32_t) * total) || !d_kept[s].alloc(sizeof(uint32_t) * total) ||
-        !d_pos[s].alloc(sizeof(unsigned long long) * ((size_t)total + 1)) || !d_rank[s].alloc(sizeof(unsigned long long) * ((size_t)total + 1)))
-      return TSM_E_CUDA;
-    es[s] = EditSide{h.d.arena, h.d.off, h.d.line_base, (uint32_t)n, h.d.line_end, h.d.line_flag, h.line_mark.as<uint8_t>(), d_traced.as<uint8_t>()};
-    if (total) {
-      k_case_kept<<<(total + 255) / 256, 256, 0, st>>>(es[s].mark, total, d_kept[s].as<uint32_t>());
-      k_edit_flag<<<(total + 255) / 256, 256, 0, st>>>(es[s], total, d_flag[s].as<uint32_t>());
-    }
-    xscan(d_kept[s].as<uint32_t>(), total, d_bsum.as<unsigned long long>(), d_rank[s].as<unsigned long long>(), st);
-    xscan(d_flag[s].as<uint32_t>(), total, d_bsum.as<unsigned long long>(), d_pos[s].as<unsigned long long>(), st);
-    CU(cudaMemcpyAsync(&cnt[s], d_pos[s].as<unsigned long long>() + total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    c->launches += total ? 8 : 0;
-  }
-  CU(cudaGetLastError());
-  CU(cudaStreamSynchronize(st));
-  const uint32_t ne[2] = {(uint32_t)cnt[0], (uint32_t)cnt[1]};
-  Ctrl hc[2] = {};
-  unsigned long long* list[2];
-  for (int s = 0; s < 2; ++s) {
-    const uint32_t total = (uint32_t)side[s]->total;
-    if (!d_lines[s].alloc(sizeof(EditLine) * std::max(ne[s], 1u)) || !d_cand[s].alloc(sizeof(unsigned long long) * std::max(ne[s], 1u)))
-      return TSM_E_CUDA;
-    list[s] = d_cand[s].as<unsigned long long>();
-    hc[s].n_cand = ne[s];
-    if (total)
-      k_edit_compact<<<(total + 255) / 256, 256, 0, st>>>(es[s], total, d_flag[s].as<uint32_t>(), d_pos[s].as<unsigned long long>(),
-                                                          d_rank[s].as<unsigned long long>(), d_lines[s].as<EditLine>(), list[s]);
-    c->launches += total ? 1 : 0;
-  }
-  CU(cudaGetLastError());
-  Ctrl* ctrl[2] = {d_ctrl.as<Ctrl>(), reinterpret_cast<Ctrl*>(d_ctrl.as<uint8_t>() + 64)};
-  for (int s = 0; s < 2; ++s) CU(cudaMemcpyAsync(ctrl[s], &hc[s], sizeof(Ctrl), cudaMemcpyHostToDevice, st));
-  const int cls_rc = classify_changed(c, side, list, ctrl, ne, n, P.groups_a, chg, st);
-  if (cls_rc != TSM_OK && cls_rc != TSM_E_CAPACITY) return cls_rc;
-  std::vector<EditCand> kept;
-  std::vector<EditLine> pat;
-  if (ne[0] && ne[1]) {
-    rc = edit_scores(c, d_lines, ne, P.A.d.arena, P.B.d.arena, kept, pat, st);
+  return pair_call(c, olds, news, PAIR_GRP, &ms[0], stream, [&](HostSidePair& P, cudaStream_t st) -> int {
+    std::vector<tsm_diff_detail> own;
+    if (!detail) { own.resize((size_t)n); detail = own.data(); }
+    int rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
     if (rc != TSM_OK) return rc;
-  }
-  // greedy pairing per hunk: candidates bucketed by old entry (counting sort), then each hunk's run sorted by score
-  // (descending), old entry, new entry and taken in that order; each entry in at most one edit
-  std::vector<uint32_t> at((size_t)ne[0] + 1, 0);
-  for (const EditCand& k : kept) ++at[(size_t)k.old_e + 1];
-  for (uint32_t i = 0; i < ne[0]; ++i) at[(size_t)i + 1] += at[i];
-  std::vector<EditCand> by_old(kept.size());
-  {
-    std::vector<uint32_t> put(at.begin(), at.end() - 1);
-    for (const EditCand& k : kept) by_old[put[k.old_e]++] = k;
-  }
-  std::vector<char> used_old(ne[0], 0), used_new(ne[1], 0);
-  std::vector<tsm_assert_edit> got;
-  for (uint32_t h0 = 0, h1 = 0; h0 < (uint32_t)pat.size(); h0 = h1) {
-    for (h1 = h0 + 1; h1 < (uint32_t)pat.size() && pat[h1].key == pat[h0].key; ++h1) {}
-    const auto b = by_old.begin() + at[h0], e = by_old.begin() + at[h1];
-    std::sort(b, e, [](const EditCand& x, const EditCand& y) {
-      return x.score != y.score ? x.score > y.score : (x.old_e != y.old_e ? x.old_e < y.old_e : x.new_e < y.new_e);
-    });
-    for (auto k = b; k != e; ++k)
-      if (!used_old[k->old_e] && !used_new[k->new_e]) {
-        used_old[k->old_e] = used_new[k->new_e] = 1;
-        got.push_back(tsm_assert_edit{(int64_t)k->old_e, (int64_t)k->new_e, (int32_t)k->score, 0});
-      }
-  }
-  std::sort(got.begin(), got.end(), [](const tsm_assert_edit& x, const tsm_assert_edit& y) { return x.aev < y.aev; });
-  c->edit_ms[2] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  *n_edits = (int64_t)got.size();
-  if (cls_rc == TSM_E_CAPACITY || *n_edits > edit_cap) return TSM_E_CAPACITY;   // all three counts set: size and call again
-  if (*n_edits && !edits) return TSM_E_ARG;
-  if (*n_edits) memcpy(edits, got.data(), sizeof(tsm_assert_edit) * got.size());
-  return TSM_OK;
+    ms[1] = c->last_ms[MS_DIFF][1] + c->last_ms[MS_DIFF][2];
+    const auto t0 = std::chrono::steady_clock::now();
+    std::vector<uint8_t> traced((size_t)n);
+    for (int32_t i = 0; i < n; ++i) traced[(size_t)i] = detail[i].added_assert >= 0;
+    HostSide* side[2] = {&P.A, &P.B};
+    DevBuf d_traced, d_flag[2], d_pos[2], d_kept[2], d_rank[2], d_lines[2], d_cand[2], d_bsum, d_ctrl;
+    if (!d_traced.alloc((size_t)n) || !d_ctrl.alloc(2 * 64) ||
+        !d_bsum.alloc(sizeof(unsigned long long) * ((size_t)std::max(P.A.total, P.B.total) / XS_TILE + 4)))
+      return TSM_E_CUDA;
+    CU(cudaMemcpyAsync(d_traced.p, traced.data(), (size_t)n, cudaMemcpyHostToDevice, st));
+    unsigned long long cnt[2] = {0, 0};
+    EditSide es[2];
+    for (int s = 0; s < 2; ++s) {
+      const HostSide& h = *side[s];
+      const uint32_t total = (uint32_t)h.total;
+      if (!d_flag[s].alloc(sizeof(uint32_t) * total) || !d_kept[s].alloc(sizeof(uint32_t) * total) ||
+          !d_pos[s].alloc(sizeof(unsigned long long) * ((size_t)total + 1)) || !d_rank[s].alloc(sizeof(unsigned long long) * ((size_t)total + 1)))
+        return TSM_E_CUDA;
+      es[s] = EditSide{h.d.arena, h.d.off, h.d.line_base, (uint32_t)n, h.d.line_end, h.d.line_flag, h.line_mark.as<uint8_t>(), d_traced.as<uint8_t>()};
+      kept_ranks(h, d_kept[s], d_rank[s], d_bsum, st);
+      if (total) k_edit_flag<<<(total + 255) / 256, 256, 0, st>>>(es[s], total, d_flag[s].as<uint32_t>());
+      xscan(d_flag[s].as<uint32_t>(), total, d_bsum.as<unsigned long long>(), d_pos[s].as<unsigned long long>(), st);
+      CU(cudaMemcpyAsync(&cnt[s], d_pos[s].as<unsigned long long>() + total, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+      c->launches += total ? 8 : 0;
+    }
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(st));
+    const uint32_t ne[2] = {(uint32_t)cnt[0], (uint32_t)cnt[1]};
+    Ctrl hc[2] = {};
+    unsigned long long* list[2];
+    for (int s = 0; s < 2; ++s) {
+      const uint32_t total = (uint32_t)side[s]->total;
+      if (!d_lines[s].alloc(sizeof(EditLine) * std::max(ne[s], 1u)) || !d_cand[s].alloc(sizeof(unsigned long long) * std::max(ne[s], 1u)))
+        return TSM_E_CUDA;
+      list[s] = d_cand[s].as<unsigned long long>();
+      hc[s].n_cand = ne[s];
+      if (total)
+        k_edit_compact<<<(total + 255) / 256, 256, 0, st>>>(es[s], total, d_flag[s].as<uint32_t>(), d_pos[s].as<unsigned long long>(),
+                                                            d_rank[s].as<unsigned long long>(), d_lines[s].as<EditLine>(), list[s]);
+      c->launches += total ? 1 : 0;
+    }
+    CU(cudaGetLastError());
+    Ctrl* ctrl[2] = {d_ctrl.as<Ctrl>(), reinterpret_cast<Ctrl*>(d_ctrl.as<uint8_t>() + 64)};
+    for (int s = 0; s < 2; ++s) CU(cudaMemcpyAsync(ctrl[s], &hc[s], sizeof(Ctrl), cudaMemcpyHostToDevice, st));
+    const int cls_rc = classify_changed(c, side, list, ctrl, ne, n, P.groups_a, chg, st);
+    if (cls_rc != TSM_OK && cls_rc != TSM_E_CAPACITY) return cls_rc;
+    std::vector<EditCand> kept;
+    std::vector<EditLine> pat;
+    if (ne[0] && ne[1]) {
+      rc = edit_scores(c, d_lines, ne, P.A.d.arena, P.B.d.arena, kept, pat, st);
+      if (rc != TSM_OK) return rc;
+    }
+    // greedy pairing per hunk: candidates bucketed by old entry (counting sort), then each hunk's run sorted by score
+    // (descending), old entry, new entry and taken in that order; each entry in at most one edit
+    std::vector<uint32_t> at((size_t)ne[0] + 1, 0);
+    for (const EditCand& k : kept) ++at[(size_t)k.old_e + 1];
+    for (uint32_t i = 0; i < ne[0]; ++i) at[(size_t)i + 1] += at[i];
+    std::vector<EditCand> by_old(kept.size());
+    {
+      std::vector<uint32_t> put(at.begin(), at.end() - 1);
+      for (const EditCand& k : kept) by_old[put[k.old_e]++] = k;
+    }
+    std::vector<char> used_old(ne[0], 0), used_new(ne[1], 0);
+    std::vector<tsm_assert_edit> got;
+    for (uint32_t h0 = 0, h1 = 0; h0 < (uint32_t)pat.size(); h0 = h1) {
+      for (h1 = h0 + 1; h1 < (uint32_t)pat.size() && pat[h1].key == pat[h0].key; ++h1) {}
+      const auto b = by_old.begin() + at[h0], e = by_old.begin() + at[h1];
+      std::sort(b, e, [](const EditCand& x, const EditCand& y) {
+        return x.score != y.score ? x.score > y.score : (x.old_e != y.old_e ? x.old_e < y.old_e : x.new_e < y.new_e);
+      });
+      for (auto k = b; k != e; ++k)
+        if (!used_old[k->old_e] && !used_new[k->new_e]) {
+          used_old[k->old_e] = used_new[k->new_e] = 1;
+          got.push_back(tsm_assert_edit{(int64_t)k->old_e, (int64_t)k->new_e, (int32_t)k->score, 0});
+        }
+    }
+    std::sort(got.begin(), got.end(), [](const tsm_assert_edit& x, const tsm_assert_edit& y) { return x.aev < y.aev; });
+    ms[2] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    *n_edits = (int64_t)got.size();
+    if (cls_rc == TSM_E_CAPACITY || *n_edits > edit_cap) return TSM_E_CAPACITY;   // all three counts set: size and call again
+    if (*n_edits && !edits) return TSM_E_ARG;
+    if (*n_edits) memcpy(edits, got.data(), sizeof(tsm_assert_edit) * got.size());
+    return TSM_OK;
+  });
 }
 
-extern "C" int tsm_assert_edits_last_ms(tsm_ctx* c, float* ms3) {
-  if (!c || !ms3) return TSM_E_ARG;
-  for (int i = 0; i < 3; ++i) ms3[i] = c->edit_ms[i];
-  return TSM_OK;
-}
+extern "C" int tsm_assert_edits_last_ms(tsm_ctx* c, float* ms3) { return copy_ms(c, MS_EDIT, ms3, 3); }
 
 // Provenance: the checks of prev and the line counts on the host, the marks diff, then ONE k_blame launch over the chains
 // (pair lists in chain order, longest chain first: the long chains are the tail of the launch).
@@ -1665,7 +1686,7 @@ extern "C" int tsm_blame_pairs(tsm_ctx* c, const tsm_corpus* olds, const tsm_cor
     return TSM_E_ARG;
   const int32_t n = olds->n_files;
   *n_lines = 0;
-  c->blame_ms = 0;
+  float* const ms = clear_ms(c, MS_BLAME);
   if (n == 0) {
     if (line_base_old) line_base_old[0] = 0;
     if (line_base_new) line_base_new[0] = 0;
@@ -1683,85 +1704,73 @@ extern "C" int tsm_blame_pairs(tsm_ctx* c, const tsm_corpus* olds, const tsm_cor
       return TSM_E_ARG;
     }
   }
-  int rc = check_sides({olds, news}, n, true);
-  if (rc != TSM_OK) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  CallScope call(c, st);
-  CU(call.status);
-  HostSidePair P;
-  DevBuf d_prev, d_label, d_head, d_in_base, d_pairs, d_start, d_work, d_keep, d_out;
-  SyncGuard guard(st);
-  rc = pair_upload(olds, news, false, P, st);
-  if (rc == TSM_OK) rc = pair_records(c, P, &c->diff_ms[0], true, st);
-  if (rc != TSM_OK) return rc;
-  if (line_base_old) memcpy(line_base_old, P.A.base.data(), sizeof(int64_t) * ((size_t)n + 1));
-  if (line_base_new) memcpy(line_base_new, P.B.base.data(), sizeof(int64_t) * ((size_t)n + 1));
-  *n_lines = (int64_t)P.B.total;
-  const std::vector<unsigned long long>& la = P.A.base;
-  const std::vector<unsigned long long>& lb = P.B.base;
-  for (int32_t i = 0; i < n; ++i) {                        // old side i = new side prev[i], or the head's range of origin_in
-    const unsigned long long want = prev[i] >= 0 ? lb[(size_t)prev[i] + 1] - lb[(size_t)prev[i]] : (unsigned long long)(in_base[i + 1] - in_base[i]);
-    if (la[(size_t)i + 1] - la[(size_t)i] != want) return TSM_E_ARG;
-  }
-  if (cap < *n_lines) return TSM_E_CAPACITY;
-  if (*n_lines && !origin_out) return TSM_E_ARG;
-  rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
-  if (rc != TSM_OK) return rc;
-  // chains: heads in pair order, then stably by length, longest first
-  std::vector<int32_t> heads, len;
-  for (int32_t i = 0; i < n; ++i)
-    if (prev[i] < 0) {
-      int32_t k = 0;
-      for (int32_t j = i; j >= 0; j = next[(size_t)j]) ++k;
-      heads.push_back(i); len.push_back(k);
+  return pair_call(c, olds, news, PAIR_HOST_BASE, &c->last_ms[MS_DIFF][0], stream, [&](HostSidePair& P, cudaStream_t st) -> int {
+    if (line_base_old) memcpy(line_base_old, P.A.base.data(), sizeof(int64_t) * ((size_t)n + 1));
+    if (line_base_new) memcpy(line_base_new, P.B.base.data(), sizeof(int64_t) * ((size_t)n + 1));
+    *n_lines = (int64_t)P.B.total;
+    const std::vector<unsigned long long>& la = P.A.base;
+    const std::vector<unsigned long long>& lb = P.B.base;
+    for (int32_t i = 0; i < n; ++i) {                        // old side i = new side prev[i], or the head's range of origin_in
+      const unsigned long long want = prev[i] >= 0 ? lb[(size_t)prev[i] + 1] - lb[(size_t)prev[i]] : (unsigned long long)(in_base[i + 1] - in_base[i]);
+      if (la[(size_t)i + 1] - la[(size_t)i] != want) return TSM_E_ARG;
     }
-  std::vector<int32_t> order_h(heads.size());
-  for (size_t h = 0; h < heads.size(); ++h) order_h[h] = (int32_t)h;
-  std::stable_sort(order_h.begin(), order_h.end(), [&](int32_t x, int32_t y) { return len[(size_t)x] > len[(size_t)y]; });
-  const int32_t n_chains = (int32_t)heads.size();
-  std::vector<int32_t> chain_pairs, chain_start;
-  chain_pairs.reserve((size_t)n); chain_start.reserve((size_t)n_chains + 1);
-  for (int32_t h : order_h) {
+    if (cap < *n_lines) return TSM_E_CAPACITY;
+    if (*n_lines && !origin_out) return TSM_E_ARG;
+    const int rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
+    if (rc != TSM_OK) return rc;
+    // chains: heads in pair order, then stably by length, longest first
+    std::vector<int32_t> heads, len;
+    for (int32_t i = 0; i < n; ++i)
+      if (prev[i] < 0) {
+        int32_t k = 0;
+        for (int32_t j = i; j >= 0; j = next[(size_t)j]) ++k;
+        heads.push_back(i); len.push_back(k);
+      }
+    std::vector<int32_t> order_h(heads.size());
+    for (size_t h = 0; h < heads.size(); ++h) order_h[h] = (int32_t)h;
+    std::stable_sort(order_h.begin(), order_h.end(), [&](int32_t x, int32_t y) { return len[(size_t)x] > len[(size_t)y]; });
+    const int32_t n_chains = (int32_t)heads.size();
+    std::vector<int32_t> chain_pairs, chain_start;
+    chain_pairs.reserve((size_t)n); chain_start.reserve((size_t)n_chains + 1);
+    for (int32_t h : order_h) {
+      chain_start.push_back((int32_t)chain_pairs.size());
+      for (int32_t j = heads[(size_t)h]; j >= 0; j = next[(size_t)j]) chain_pairs.push_back(j);
+    }
     chain_start.push_back((int32_t)chain_pairs.size());
-    for (int32_t j = heads[(size_t)h]; j >= 0; j = next[(size_t)j]) chain_pairs.push_back(j);
-  }
-  chain_start.push_back((int32_t)chain_pairs.size());
-  const size_t n_in = (size_t)in_base[n];
-  if (!d_prev.alloc(sizeof(int32_t) * (size_t)n) || !d_label.alloc(sizeof(int32_t) * (size_t)n) ||
-      !d_head.alloc(sizeof(tsm_origin) * n_in) || !d_in_base.alloc(sizeof(int64_t) * ((size_t)n + 1)) ||
-      !d_pairs.alloc(sizeof(int32_t) * (size_t)n) || !d_start.alloc(sizeof(int32_t) * ((size_t)n_chains + 1)) || !d_work.alloc(16) ||
-      !d_keep.alloc(sizeof(tsm_origin) * (size_t)P.A.total) || !d_out.alloc(sizeof(tsm_origin) * (size_t)P.B.total))
-    return TSM_E_CUDA;
-  CU(cudaMemcpyAsync(d_prev.p, prev, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(d_label.p, label, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
-  if (n_in) CU(cudaMemcpyAsync(d_head.p, origin_in, sizeof(tsm_origin) * n_in, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(d_in_base.p, in_base, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(d_pairs.p, chain_pairs.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(d_start.p, chain_start.data(), sizeof(int32_t) * ((size_t)n_chains + 1), cudaMemcpyHostToDevice, st));
-  CU(cudaMemsetAsync(d_work.p, 0, 16, st));
-  CU(cudaEventRecord(c->blame_ev[0], st));
-  k_blame<<<std::min((n_chains + 7) / 8, c->sms * 8), 256, 0, st>>>(
-      P.A.d.line_base, P.B.d.line_base, P.A.line_mark.as<uint8_t>(), P.B.line_mark.as<uint8_t>(), d_prev.as<int32_t>(), d_label.as<int32_t>(),
-      d_head.as<tsm_origin>(), d_in_base.as<long long>(), d_pairs.as<int32_t>(), d_start.as<int32_t>(), n_chains, d_work.as<uint32_t>(),
-      d_keep.as<tsm_origin>(), d_out.as<tsm_origin>());
-  CU(cudaEventRecord(c->blame_ev[1], st));
-  CU(cudaGetLastError());
-  c->launches++;
-  if (*n_lines) CU(cudaMemcpyAsync(origin_out, d_out.p, sizeof(tsm_origin) * (size_t)*n_lines, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  c->blame_ms = elapsed_ms(c->blame_ev[0], c->blame_ev[1]);
-  return TSM_OK;
+    const size_t n_in = (size_t)in_base[n];
+    DevBuf d_prev, d_label, d_head, d_in_base, d_pairs, d_start, d_work, d_keep, d_out;
+    if (!d_prev.alloc(sizeof(int32_t) * (size_t)n) || !d_label.alloc(sizeof(int32_t) * (size_t)n) ||
+        !d_head.alloc(sizeof(tsm_origin) * n_in) || !d_in_base.alloc(sizeof(int64_t) * ((size_t)n + 1)) ||
+        !d_pairs.alloc(sizeof(int32_t) * (size_t)n) || !d_start.alloc(sizeof(int32_t) * ((size_t)n_chains + 1)) || !d_work.alloc(16) ||
+        !d_keep.alloc(sizeof(tsm_origin) * (size_t)P.A.total) || !d_out.alloc(sizeof(tsm_origin) * (size_t)P.B.total))
+      return TSM_E_CUDA;
+    CU(cudaMemcpyAsync(d_prev.p, prev, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_label.p, label, sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
+    if (n_in) CU(cudaMemcpyAsync(d_head.p, origin_in, sizeof(tsm_origin) * n_in, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_in_base.p, in_base, sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_pairs.p, chain_pairs.data(), sizeof(int32_t) * (size_t)n, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_start.p, chain_start.data(), sizeof(int32_t) * ((size_t)n_chains + 1), cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync(d_work.p, 0, 16, st));
+    CU(cudaEventRecord(c->diff_ev[EV_BLAME.from], st));
+    k_blame<<<std::min((n_chains + 7) / 8, c->sms * 8), 256, 0, st>>>(
+        P.A.d.line_base, P.B.d.line_base, P.A.line_mark.as<uint8_t>(), P.B.line_mark.as<uint8_t>(), d_prev.as<int32_t>(), d_label.as<int32_t>(),
+        d_head.as<tsm_origin>(), d_in_base.as<long long>(), d_pairs.as<int32_t>(), d_start.as<int32_t>(), n_chains, d_work.as<uint32_t>(),
+        d_keep.as<tsm_origin>(), d_out.as<tsm_origin>());
+    CU(cudaEventRecord(c->diff_ev[EV_BLAME.to], st));
+    CU(cudaGetLastError());
+    c->launches++;
+    if (*n_lines) CU(cudaMemcpyAsync(origin_out, d_out.p, sizeof(tsm_origin) * (size_t)*n_lines, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    ms[0] = span_ms(c, EV_BLAME);
+    return TSM_OK;
+  });
 }
 
-extern "C" int tsm_blame_last_ms(tsm_ctx* c, float* ms) {
-  if (!c || !ms) return TSM_E_ARG;
-  *ms = c->blame_ms;
-  return TSM_OK;
-}
+extern "C" int tsm_blame_last_ms(tsm_ctx* c, float* ms) { return copy_ms(c, MS_BLAME, ms, 1); }
 
 // ------------------------------------------------------------------------------------- SPEC section 13 rename similarity
 // Per side with line records: k_sim_sort (distinct (hash, weight) of every file at its line_base), xscan of the list
-// lengths, k_sim_compact (dense CSR).  sim_ms[1] covers both sides.
+// lengths, k_sim_compact (dense CSR).  last_ms[MS_SIM][1] covers both sides.
 namespace {
 struct SimLists { DevBuf wk_key, wk_w, s_key, s_cum, cnt, bsum, base, key, w; };
 
@@ -1790,7 +1799,7 @@ extern "C" int tsm_similarity(tsm_ctx* c, const tsm_corpus* olds, const tsm_corp
                               const int32_t* cand_new, int64_t n_cand, int64_t* common, void* stream) {
   if (!c || !olds || !news || n_cand < 0 || (n_cand && (!cand_old || !cand_new || !common))) return TSM_E_ARG;
   if (olds->n_files < 0 || news->n_files < 0) return TSM_E_ARG;
-  for (float& v : c->sim_ms) v = 0;
+  float* const ms = clear_ms(c, MS_SIM);
   if (n_cand == 0) return TSM_OK;
   CU(cudaSetDevice(c->device));
   {                                                        // the candidates, their indices and results: 16 B each on the device
@@ -1800,53 +1809,40 @@ extern "C" int tsm_similarity(tsm_ctx* c, const tsm_corpus* olds, const tsm_corp
   }
   for (int64_t i = 0; i < n_cand; ++i)
     if (cand_old[i] < 0 || cand_old[i] >= olds->n_files || cand_new[i] < 0 || cand_new[i] >= news->n_files) return TSM_E_ARG;
-  int rc = check_sides({olds}, olds->n_files, false);
-  if (rc == TSM_OK) rc = check_sides({news}, news->n_files, false);
-  if (rc != TSM_OK) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  CallScope call(c, st);
-  CU(call.status);
-  HostSidePair P;
-  SimLists LA, LB;
-  DevBuf d_cand;
-  SyncGuard guard(st);
-  rc = pair_upload(olds, news, false, P, st);
-  if (rc == TSM_OK) rc = pair_records(c, P, &c->sim_ms[0], false, st);
-  if (rc != TSM_OK) return rc;
-  const size_t nc = (size_t)n_cand;
-  if (!d_cand.alloc(16 * nc + 64)) { cudaGetLastError(); return TSM_E_NOMEM; }
-  long long* d_common = d_cand.as<long long>();
-  int32_t* d_old = reinterpret_cast<int32_t*>(d_common + nc);
-  int32_t* d_new = d_old + nc;
-  unsigned long long* d_next = reinterpret_cast<unsigned long long*>(d_new + nc);   // at 16 * nc bytes: 8-byte aligned
-  CU(cudaMemcpyAsync(d_old, cand_old, sizeof(int32_t) * nc, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(d_new, cand_new, sizeof(int32_t) * nc, cudaMemcpyHostToDevice, st));
-  CU(cudaMemsetAsync(d_next, 0, sizeof(unsigned long long), st));
-  CU(cudaEventRecord(c->diff_ev[EV_SIM_LISTS], st));
-  rc = sim_lists(P.A, LA, st);
-  if (rc == TSM_OK) rc = sim_lists(P.B, LB, st);
-  if (rc != TSM_OK) return rc;
-  CU(cudaEventRecord(c->diff_ev[EV_SIM_PAIRS], st));
-  const unsigned grid = (unsigned)std::min<size_t>((size_t)c->sms * 8, (nc + 8 * SIM_GRAB - 1) / (8 * SIM_GRAB));
-  k_similarity<<<grid, 256, 0, st>>>(LA.key.as<unsigned long long>(), LA.w.as<uint32_t>(), LA.base.as<unsigned long long>(),
-                                     LB.key.as<unsigned long long>(), LB.w.as<uint32_t>(), LB.base.as<unsigned long long>(),
-                                     d_old, d_new, (unsigned long long)nc, d_next, d_common);
-  CU(cudaGetLastError());
-  CU(cudaEventRecord(c->diff_ev[EV_SIM_END], st));
-  CU(cudaMemcpyAsync(common, d_common, sizeof(int64_t) * nc, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  P.A.drop_staging(); P.B.drop_staging();
-  c->sim_ms[1] = elapsed_ms(c->diff_ev[EV_SIM_LISTS], c->diff_ev[EV_SIM_PAIRS]);
-  c->sim_ms[2] = elapsed_ms(c->diff_ev[EV_SIM_PAIRS], c->diff_ev[EV_SIM_END]);
-  c->launches = P.A.launches + P.B.launches + 2 * 5 + 1;   // per side k_sim_sort, xscan (3), k_sim_compact; k_similarity
-  return TSM_OK;
+  return pair_call(c, olds, news, PAIR_ANY_EXT, &ms[0], stream, [&](HostSidePair& P, cudaStream_t st) -> int {
+    const size_t nc = (size_t)n_cand;
+    SimLists LA, LB;
+    DevBuf d_cand;
+    if (!d_cand.alloc(16 * nc + 64)) { cudaGetLastError(); return TSM_E_NOMEM; }
+    long long* d_common = d_cand.as<long long>();
+    int32_t* d_old = reinterpret_cast<int32_t*>(d_common + nc);
+    int32_t* d_new = d_old + nc;
+    unsigned long long* d_next = reinterpret_cast<unsigned long long*>(d_new + nc);   // at 16 * nc bytes: 8-byte aligned
+    CU(cudaMemcpyAsync(d_old, cand_old, sizeof(int32_t) * nc, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_new, cand_new, sizeof(int32_t) * nc, cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync(d_next, 0, sizeof(unsigned long long), st));
+    CU(cudaEventRecord(c->diff_ev[EV_SIM_LISTS], st));
+    int rc = sim_lists(P.A, LA, st);
+    if (rc == TSM_OK) rc = sim_lists(P.B, LB, st);
+    if (rc != TSM_OK) return rc;
+    CU(cudaEventRecord(c->diff_ev[EV_SIM_PAIRS], st));
+    const unsigned grid = (unsigned)std::min<size_t>((size_t)c->sms * 8, (nc + 8 * SIM_GRAB - 1) / (8 * SIM_GRAB));
+    k_similarity<<<grid, 256, 0, st>>>(LA.key.as<unsigned long long>(), LA.w.as<uint32_t>(), LA.base.as<unsigned long long>(),
+                                       LB.key.as<unsigned long long>(), LB.w.as<uint32_t>(), LB.base.as<unsigned long long>(),
+                                       d_old, d_new, (unsigned long long)nc, d_next, d_common);
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_SIM_END], st));
+    CU(cudaMemcpyAsync(common, d_common, sizeof(int64_t) * nc, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    P.A.drop_staging(); P.B.drop_staging();
+    ms[1] = elapsed_ms(c->diff_ev[EV_SIM_LISTS], c->diff_ev[EV_SIM_PAIRS]);
+    ms[2] = elapsed_ms(c->diff_ev[EV_SIM_PAIRS], c->diff_ev[EV_SIM_END]);
+    c->launches = P.A.launches + P.B.launches + 2 * 5 + 1;   // per side k_sim_sort, xscan (3), k_sim_compact; k_similarity
+    return TSM_OK;
+  });
 }
 
-extern "C" int tsm_similarity_last_ms(tsm_ctx* c, float* ms3) {
-  if (!c || !ms3) return TSM_E_ARG;
-  for (int i = 0; i < 3; ++i) ms3[i] = c->sim_ms[i];
-  return TSM_OK;
-}
+extern "C" int tsm_similarity_last_ms(tsm_ctx* c, float* ms3) { return copy_ms(c, MS_SIM, ms3, 3); }
 
 // ------------------------------------------------------------------------------------- S9 line / n-gram hashes
 // The front of tsm_line_hashes and tsm_statements: the corpus' line records from one pass of the scan, and line_base[n+1]
@@ -1860,7 +1856,7 @@ static int line_records(tsm_ctx* c, const tsm_corpus* k, bool ext_rule, int64_t*
   *n_lines = 0;
   line_base[0] = 0;
   if (n == 0) return TSM_OK;
-  int rc = check_sides({k}, n, ext_rule);
+  int rc = check_sides({k}, ext_rule);
   if (rc != TSM_OK) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   CallScope call(c, st);
@@ -1928,7 +1924,7 @@ extern "C" int tsm_statements(tsm_ctx* c, const tsm_corpus* k, int64_t* line_bas
 extern "C" int tsm_clones(tsm_ctx* c, const tsm_corpus* k, int32_t min_lines, tsm_clone_result* out, void* stream) {
   if (!c || !k || !out || k->n_files < 0 || min_lines < 1 || min_lines > 1024 || out->class_cap < 0 || out->member_cap < 0) return TSM_E_ARG;
   const int32_t nf = k->n_files;
-  for (float& v : c->clone_ms) v = 0;
+  float* const ms = clear_ms(c, MS_CLONE);
   c->launches = 0;
   out->n_classes = out->n_members = 0;
   if (out->class_base) out->class_base[0] = 0;
@@ -1985,7 +1981,7 @@ extern "C" int tsm_clones(tsm_ctx* c, const tsm_corpus* k, int32_t min_lines, ts
                                                          d_len.as<uint32_t>());
     CU(cudaGetLastError());
     CU(cudaEventRecord(c->diff_ev[EV_CLONE_MEMBERS], st));
-    unsigned long long* pin = reinterpret_cast<unsigned long long*>(c->h_diff + 128);   // classes, fragments, large classes
+    unsigned long long* pin = c->h_rb->u64;                 // classes, fragments, large classes
     CU(cudaMemcpyAsync(pin, d_cidx.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(pin + 1, d_cbase.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(pin + 2, d_nbig.p, 4, cudaMemcpyDeviceToHost, st));
@@ -1995,7 +1991,7 @@ extern "C" int tsm_clones(tsm_ctx* c, const tsm_corpus* k, int32_t min_lines, ts
     const unsigned long long nm = pin[1];
     out->n_classes = (int64_t)nc;
     out->n_members = (int64_t)nm;
-    c->clone_ms[1] = elapsed_ms(c->diff_ev[EV_CLONE_GROUP], c->diff_ev[EV_CLONE_MEMBERS]);
+    ms[1] = elapsed_ms(c->diff_ev[EV_CLONE_GROUP], c->diff_ev[EV_CLONE_MEMBERS]);
     if ((out->class_cap < (int64_t)nc && (out->class_base || out->class_len)) || (out->member_cap < (int64_t)nm && out->member))
       return TSM_E_CAPACITY;
     if (nc) {
@@ -2022,17 +2018,13 @@ extern "C" int tsm_clones(tsm_ctx* c, const tsm_corpus* k, int32_t min_lines, ts
       if (out->class_len) CU(cudaMemcpyAsync(out->class_len, d_len.p, 4 * (size_t)nc, cudaMemcpyDeviceToHost, st));
       if (out->member) CU(cudaMemcpyAsync(out->member, member, 8 * nm, cudaMemcpyDeviceToHost, st));
       CU(cudaStreamSynchronize(st));
-      c->clone_ms[2] = elapsed_ms(c->diff_ev[EV_CLONE_MEMBERS], c->diff_ev[EV_CLONE_END]);
+      ms[2] = elapsed_ms(c->diff_ev[EV_CLONE_MEMBERS], c->diff_ev[EV_CLONE_END]);
     }
     return TSM_OK;
-  }, &c->clone_ms[0]);
+  }, &ms[0]);
 }
 
-extern "C" int tsm_clones_last_ms(tsm_ctx* c, float* ms3) {
-  if (!c || !ms3) return TSM_E_ARG;
-  for (int i = 0; i < 3; ++i) ms3[i] = c->clone_ms[i];
-  return TSM_OK;
-}
+extern "C" int tsm_clones_last_ms(tsm_ctx* c, float* ms3) { return copy_ms(c, MS_CLONE, ms3, 3); }
 
 // ------------------------------------------------------------------------------------- SPEC section 18 test smells
 // The smell stage over one side whose line records (with header events) and case spans exist: the section-10 kinds
@@ -2079,7 +2071,7 @@ extern "C" int tsm_smells(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, u
                           tsm_smell_test* tests, int64_t test_cap, int64_t* n_tests, void* stream) {
   if (!c || !k || !n_lines || !n_tests || line_cap < 0 || test_cap < 0 || k->n_files < 0) return TSM_E_ARG;
   const int32_t nf = k->n_files;
-  for (float& v : c->smell_ms) v = 0;
+  float* const ms = clear_ms(c, MS_SMELL);
   c->launches = 0;
   *n_tests = 0;
   std::vector<int64_t> own_base;
@@ -2095,121 +2087,107 @@ extern "C" int tsm_smells(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, u
     int rc = case_spans(S, sp, d_bsum, launches, st);
     if (rc == TSM_OK) rc = smell_stage(c, S, sp, d_bsum, m, launches, st);
     if (rc != TSM_OK) return rc;
-    unsigned long long* pin = reinterpret_cast<unsigned long long*>(c->h_diff + 128);
+    unsigned long long* pin = c->h_rb->u64;
     CU(cudaMemcpyAsync(pin, m.tidx.as<unsigned long long>() + sp.n_cases, 8, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     c->launches += launches;
     const unsigned long long nt = *pin;
     *n_tests = (int64_t)nt;
-    c->smell_ms[1] = elapsed_ms(c->diff_ev[EV_SMELL_KINDS], c->diff_ev[EV_SMELL_LINES]);
-    c->smell_ms[2] = elapsed_ms(c->diff_ev[EV_SMELL_LINES], c->diff_ev[EV_SMELL_TESTS]);
-    c->smell_ms[3] = elapsed_ms(c->diff_ev[EV_SMELL_TESTS], c->diff_ev[EV_SMELL_END]);
+    ms[1] = elapsed_ms(c->diff_ev[EV_SMELL_KINDS], c->diff_ev[EV_SMELL_LINES]);
+    ms[2] = elapsed_ms(c->diff_ev[EV_SMELL_LINES], c->diff_ev[EV_SMELL_TESTS]);
+    ms[3] = elapsed_ms(c->diff_ev[EV_SMELL_TESTS], c->diff_ev[EV_SMELL_END]);
     if ((line_smell && line_cap < (int64_t)total) || (tests && test_cap < (int64_t)nt)) return TSM_E_CAPACITY;
     if (line_smell) CU(cudaMemcpyAsync(line_smell, m.smell.p, 2 * L, cudaMemcpyDeviceToHost, st));
     if (tests && nt) CU(cudaMemcpyAsync(tests, m.tests.p, sizeof(tsm_smell_test) * nt, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     return TSM_OK;
-  }, &c->smell_ms[0], TSM_SCAN_HEADER_EVENTS);
+  }, &ms[0], TSM_SCAN_HEADER_EVENTS);
 }
 
-extern "C" int tsm_smells_last_ms(tsm_ctx* c, float* ms4) {
-  if (!c || !ms4) return TSM_E_ARG;
-  for (int i = 0; i < 4; ++i) ms4[i] = c->smell_ms[i];
-  return TSM_OK;
-}
+extern "C" int tsm_smells_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_SMELL, ms4, 4); }
 
 // ------------------------------------------------------------------------------------- SPEC section 19 test-smell churn
 // The line records of both sides with their header events, per side the case spans and the smell stage, one synchronisation
 // for the case and test counts (the capacity check comes before the diff), the marks diff, the case records (with the new
-// side's by_rank) and k_smell_churn per side.  Slots 0 and 1 of diff_ev (those of the old side's scan, already read) time the
-// smell stages and, behind the diff, the case records and churn.
+// side's by_rank) and k_smell_churn per side.  EV_CHURN_SMELLS times the smell stages, and EV_CHURN_CASES, the same slots
+// again once read, the case records and churn behind the diff.
 extern "C" int tsm_diff_pairs_smells(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
                                      tsm_diff_detail* detail, tsm_diff_smells* out, void* stream) {
   if (!c || !olds || !news || !added || !removed || !out || olds->n_files != news->n_files || out->cases.old_cap < 0 ||
       out->cases.new_cap < 0 || out->old_test_cap < 0 || out->new_test_cap < 0)
     return TSM_E_ARG;
   const int32_t n = olds->n_files;
-  for (float& v : c->churn_ms) v = 0;
+  float* const ms = clear_ms(c, MS_CHURN);
   out->cases.n_old = out->cases.n_new = out->n_old_tests = out->n_new_tests = 0;
   if (n == 0) return TSM_OK;
-  int rc = check_sides({olds, news}, n, true);
-  if (rc != TSM_OK) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  CallScope call(c, st);
-  CU(call.status);
-  HostSidePair P;
-  PairCases pc;
-  SmellBufs sb[2];
-  DevBuf d_churn[2];
-  SyncGuard guard(st);
-  rc = pair_upload(olds, news, false, P, st);
-  if (rc == TSM_OK) rc = pair_records(c, P, &c->diff_ms[0], false, st, TSM_SCAN_HEADER_EVENTS);
-  if (rc != TSM_OK) return rc;
-  c->churn_ms[0] = c->diff_ms[0];
-  const HostSide* side[2] = {&P.A, &P.B};
-  int launches = 0;
-  CU(cudaEventRecord(c->diff_ev[0], st));
-  rc = pair_case_spans(P, pc, launches, st);
-  for (int s = 0; s < 2 && rc == TSM_OK; ++s) rc = smell_stage(c, *side[s], pc.sp[s], pc.bsum, sb[s], launches, st);
-  if (rc != TSM_OK) return rc;
-  CU(cudaEventRecord(c->diff_ev[1], st));
-  unsigned long long* pin = reinterpret_cast<unsigned long long*>(c->h_diff + 128);
-  for (int s = 0; s < 2; ++s)
-    CU(cudaMemcpyAsync(pin + s, sb[s].tidx.as<unsigned long long>() + pc.sp[s].n_cases, 8, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  c->churn_ms[1] = elapsed_ms(c->diff_ev[0], c->diff_ev[1]);
-  const uint32_t nt[2] = {(uint32_t)pin[0], (uint32_t)pin[1]};
-  out->cases.n_old = pc.sp[0].n_cases; out->cases.n_new = pc.sp[1].n_cases;
-  out->n_old_tests = nt[0]; out->n_new_tests = nt[1];
-  if ((out->cases.old_cases && out->cases.old_cap < out->cases.n_old) || (out->cases.new_cases && out->cases.new_cap < out->cases.n_new) ||
-      ((out->old_tests || out->old_churn) && out->old_test_cap < (int64_t)nt[0]) ||
-      ((out->new_tests || out->new_churn) && out->new_test_cap < (int64_t)nt[1]))
-    return TSM_E_CAPACITY;
-  rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
-  if (rc != TSM_OK) return rc;
-  c->churn_ms[2] = c->diff_ms[1] + c->diff_ms[2];
-  CU(cudaEventRecord(c->diff_ev[0], st));
-  rc = case_records(c, P, pc, true, launches, st);
-  if (rc != TSM_OK) return rc;
-  for (int s = 0; s < 2; ++s) {
-    if (!d_churn[s].alloc(sizeof(tsm_test_churn) * (size_t)nt[s])) return TSM_E_CUDA;
-    if (!nt[s]) continue;
-    const int o = 1 - s;
-    const ChurnSide cs{side[s]->d.line_base, sb[s].tests.as<tsm_smell_test>(), nt[s], sb[s].smell.as<uint16_t>(),
-                       side[s]->line_mark.as<uint8_t>(), pc.rank[s].as<unsigned long long>(), pc.sp[s].case_of.as<unsigned long long>(),
-                       sb[o].smell.as<uint16_t>(), pc.by_rank[o].as<uint32_t>(), d_churn[s].as<tsm_test_churn>()};
-    k_smell_churn<<<std::min((nt[s] + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(cs);
-    ++launches;
-  }
-  CU(cudaGetLastError());
-  CU(cudaEventRecord(c->diff_ev[1], st));
-  tsm_case* const h_cases[2] = {out->cases.old_cases, out->cases.new_cases};
-  tsm_smell_test* const h_tests[2] = {out->old_tests, out->new_tests};
-  tsm_test_churn* const h_churn[2] = {out->old_churn, out->new_churn};
-  for (int s = 0; s < 2; ++s) {
-    if (h_cases[s] && pc.sp[s].n_cases)
-      CU(cudaMemcpyAsync(h_cases[s], pc.cases[s].p, sizeof(tsm_case) * pc.sp[s].n_cases, cudaMemcpyDeviceToHost, st));
-    if (h_tests[s] && nt[s]) CU(cudaMemcpyAsync(h_tests[s], sb[s].tests.p, sizeof(tsm_smell_test) * nt[s], cudaMemcpyDeviceToHost, st));
-    if (h_churn[s] && nt[s]) CU(cudaMemcpyAsync(h_churn[s], d_churn[s].p, sizeof(tsm_test_churn) * nt[s], cudaMemcpyDeviceToHost, st));
-  }
-  CU(cudaStreamSynchronize(st));
-  c->churn_ms[3] = elapsed_ms(c->diff_ev[0], c->diff_ev[1]);
-  c->launches += launches;
-  return TSM_OK;
+  float* const dm = c->last_ms[MS_DIFF];
+  return pair_call(c, olds, news, TSM_SCAN_HEADER_EVENTS, &dm[0], stream, [&](HostSidePair& P, cudaStream_t st) -> int {
+    ms[0] = dm[0];
+    const HostSide* side[2] = {&P.A, &P.B};
+    PairCases pc;
+    SmellBufs sb[2];
+    DevBuf d_churn[2];
+    int launches = 0;
+    CU(cudaEventRecord(c->diff_ev[EV_CHURN_SMELLS.from], st));
+    int rc = pair_case_spans(P, pc, launches, st);
+    for (int s = 0; s < 2 && rc == TSM_OK; ++s) rc = smell_stage(c, *side[s], pc.sp[s], pc.bsum, sb[s], launches, st);
+    if (rc != TSM_OK) return rc;
+    CU(cudaEventRecord(c->diff_ev[EV_CHURN_SMELLS.to], st));
+    unsigned long long* pin = c->h_rb->u64;
+    for (int s = 0; s < 2; ++s)
+      CU(cudaMemcpyAsync(pin + s, sb[s].tidx.as<unsigned long long>() + pc.sp[s].n_cases, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    ms[1] = span_ms(c, EV_CHURN_SMELLS);
+    const uint32_t nt[2] = {(uint32_t)pin[0], (uint32_t)pin[1]};
+    out->cases.n_old = pc.sp[0].n_cases; out->cases.n_new = pc.sp[1].n_cases;
+    out->n_old_tests = nt[0]; out->n_new_tests = nt[1];
+    if ((out->cases.old_cases && out->cases.old_cap < out->cases.n_old) || (out->cases.new_cases && out->cases.new_cap < out->cases.n_new) ||
+        ((out->old_tests || out->old_churn) && out->old_test_cap < (int64_t)nt[0]) ||
+        ((out->new_tests || out->new_churn) && out->new_test_cap < (int64_t)nt[1]))
+      return TSM_E_CAPACITY;
+    rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
+    if (rc != TSM_OK) return rc;
+    ms[2] = dm[1] + dm[2];
+    CU(cudaEventRecord(c->diff_ev[EV_CHURN_CASES.from], st));
+    rc = case_records(c, P, pc, true, launches, st);
+    if (rc != TSM_OK) return rc;
+    for (int s = 0; s < 2; ++s) {
+      if (!d_churn[s].alloc(sizeof(tsm_test_churn) * (size_t)nt[s])) return TSM_E_CUDA;
+      if (!nt[s]) continue;
+      const int o = 1 - s;
+      const ChurnSide cs{side[s]->d.line_base, sb[s].tests.as<tsm_smell_test>(), nt[s], sb[s].smell.as<uint16_t>(),
+                         side[s]->line_mark.as<uint8_t>(), pc.rank[s].as<unsigned long long>(), pc.sp[s].case_of.as<unsigned long long>(),
+                         sb[o].smell.as<uint16_t>(), pc.by_rank[o].as<uint32_t>(), d_churn[s].as<tsm_test_churn>()};
+      k_smell_churn<<<std::min((nt[s] + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(cs);
+      ++launches;
+    }
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_CHURN_CASES.to], st));
+    tsm_case* const h_cases[2] = {out->cases.old_cases, out->cases.new_cases};
+    tsm_smell_test* const h_tests[2] = {out->old_tests, out->new_tests};
+    tsm_test_churn* const h_churn[2] = {out->old_churn, out->new_churn};
+    for (int s = 0; s < 2; ++s) {
+      if (h_cases[s] && pc.sp[s].n_cases)
+        CU(cudaMemcpyAsync(h_cases[s], pc.cases[s].p, sizeof(tsm_case) * pc.sp[s].n_cases, cudaMemcpyDeviceToHost, st));
+      if (h_tests[s] && nt[s]) CU(cudaMemcpyAsync(h_tests[s], sb[s].tests.p, sizeof(tsm_smell_test) * nt[s], cudaMemcpyDeviceToHost, st));
+      if (h_churn[s] && nt[s]) CU(cudaMemcpyAsync(h_churn[s], d_churn[s].p, sizeof(tsm_test_churn) * nt[s], cudaMemcpyDeviceToHost, st));
+    }
+    CU(cudaStreamSynchronize(st));
+    ms[3] = span_ms(c, EV_CHURN_CASES);
+    c->launches += launches;
+    return TSM_OK;
+  });
 }
 
-extern "C" int tsm_diff_smells_last_ms(tsm_ctx* c, float* ms4) {
-  if (!c || !ms4) return TSM_E_ARG;
-  for (int i = 0; i < 4; ++i) ms4[i] = c->churn_ms[i];
-  return TSM_OK;
-}
+extern "C" int tsm_diff_smells_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_CHURN, ms4, 4); }
 
 // ------------------------------------------------------------------------------------- SPEC section 20 moved code
 // The line records of both sides, the marks diff, then per side k_move_lines and three exclusive scans (alnum prefix, entry and
 // run numbers); one synchronisation reads the entry and run counts, which size the join.  k_move_compact, the (step, hash) table
 // (k_move_insert, xscan of each side's slot counts, k_move_scatter) and k_move_reach; per side the list of block starts
-// (k_move_starts twice around an xscan) and k_move_runs twice around an xscan of the block counts; a second synchronisation reads the block counts for k_move_mark.  Slots 0-1 and 2-3 of diff_ev time the
-// flags and the join with the reach, 4-5 and 6-7 the runs and the marks (the diff's own slots have been read by then).
+// (k_move_starts twice around an xscan) and k_move_runs twice around an xscan of the block counts; a second synchronisation
+// reads the block counts for k_move_mark.  EV_MOVE_FLAGS and EV_MOVE_JOIN time the flags and the join with the reach,
+// EV_MOVE_RUNS and EV_MOVE_MARK the runs and the marks: every slot again, the diff's own having been read by then.
 struct MoveBufs { DevBuf flag, alnum, chg, head, apre, eidx, ridx, best, ent, run_first, run_end, cnt, base, cursor, slot_of, seg, seg_slot,
                   start, sidx, starts, rcnt, rbase, blocks; };
 
@@ -2223,7 +2201,7 @@ extern "C" int tsm_diff_pairs_moves(tsm_ctx* c, const tsm_corpus* olds, const ts
     const uint16_t go = olds->grp ? olds->grp[i] : 0, gn = news->grp ? news->grp[i] : 0;
     if (go != gn || go >= olds->n_groups || gn >= news->n_groups) return TSM_E_ARG;
   }
-  for (float& v : c->move_ms) v = 0;
+  float* const mt = clear_ms(c, MS_MOVE);
   tsm_line_marks& mk = out->marks;
   mk.n_old = mk.n_new = 0;
   out->n_old_blocks = out->n_new_blocks = 0;
@@ -2232,162 +2210,151 @@ extern "C" int tsm_diff_pairs_moves(tsm_ctx* c, const tsm_corpus* olds, const ts
     if (mk.line_base_new) mk.line_base_new[0] = 0;
     return TSM_OK;
   }
-  int rc = check_sides({olds, news}, n, true);
-  if (rc != TSM_OK) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  CallScope call(c, st);
-  CU(call.status);
-  HostSidePair P;
-  MoveBufs mb[2];
-  DevBuf d_bsum, d_slot_bsum, d_table;
-  SyncGuard guard(st);
-  rc = pair_upload(olds, news, true, P, st);
-  if (rc == TSM_OK) rc = pair_records(c, P, &c->diff_ms[0], true, st);
-  if (rc != TSM_OK) return rc;
-  c->move_ms[0] = c->diff_ms[0];
-  rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
-  if (rc != TSM_OK) return rc;
-  c->move_ms[1] = c->diff_ms[1] + c->diff_ms[2];
-  HostSide* const side[2] = {&P.A, &P.B};
-  const uint32_t T[2] = {(uint32_t)P.A.total, (uint32_t)P.B.total};
-  int launches = 0;
-  if (!d_bsum.alloc(8 * ((size_t)std::max(T[0], T[1]) / XS_TILE + 4))) return TSM_E_CUDA;
-  unsigned long long* const bsum = d_bsum.as<unsigned long long>();
-  CU(cudaEventRecord(c->diff_ev[0], st));
-  for (int s = 0; s < 2; ++s) {
-    MoveBufs& m = mb[s];
-    const size_t L = T[s];
-    if (!m.flag.alloc(L) || !m.alnum.alloc(4 * L) || !m.chg.alloc(4 * L) || !m.head.alloc(4 * L) || !m.apre.alloc(8 * (L + 1)) ||
-        !m.eidx.alloc(8 * (L + 1)) || !m.ridx.alloc(8 * (L + 1)) || !m.best.alloc(8 * L))
-      return TSM_E_CUDA;
-    CU(cudaMemsetAsync(m.best.p, 0, 8 * L, st));
-    if (L) k_move_lines<<<(unsigned)((L + 255) / 256), 256, 0, st>>>(side[s]->d, n, T[s], side[s]->line_mark.as<uint8_t>(), m.flag.as<uint8_t>(),
-                                                                      m.alnum.as<uint32_t>(), m.chg.as<uint32_t>(), m.head.as<uint32_t>());
-    xscan(m.alnum.as<uint32_t>(), T[s], bsum, m.apre.as<unsigned long long>(), st);
-    xscan(m.chg.as<uint32_t>(), T[s], bsum, m.eidx.as<unsigned long long>(), st);
-    xscan(m.head.as<uint32_t>(), T[s], bsum, m.ridx.as<unsigned long long>(), st);
-    launches += (L ? 1 : 0) + 9;
-  }
-  CU(cudaGetLastError());
-  unsigned long long* pin = reinterpret_cast<unsigned long long*>(c->h_diff + 128);
-  for (int s = 0; s < 2; ++s) {
-    CU(cudaMemcpyAsync(pin + 2 * s, mb[s].eidx.as<unsigned long long>() + T[s], 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(pin + 2 * s + 1, mb[s].ridx.as<unsigned long long>() + T[s], 8, cudaMemcpyDeviceToHost, st));
-  }
-  CU(cudaStreamSynchronize(st));
-  const uint32_t ne[2] = {(uint32_t)pin[0], (uint32_t)pin[2]}, nr[2] = {(uint32_t)pin[1], (uint32_t)pin[3]};
-  for (int s = 0; s < 2; ++s) {
-    MoveBufs& m = mb[s];
-    if (!m.ent.alloc(4 * (size_t)ne[s]) || !m.run_first.alloc(4 * (size_t)nr[s]) || !m.run_end.alloc(4 * (size_t)nr[s])) return TSM_E_CUDA;
-    if (T[s])
-      k_move_compact<<<(T[s] + 255) / 256, 256, 0, st>>>(m.flag.as<uint8_t>(), T[s], m.eidx.as<unsigned long long>(), m.ridx.as<unsigned long long>(),
-                                                          m.ent.as<uint32_t>(), m.run_first.as<uint32_t>(), m.run_end.as<uint32_t>());
-  }
-  CU(cudaEventRecord(c->diff_ev[1], st));
-  // ---- the join: one table over the entries of both sides, at most half full
-  const unsigned long long tot = (unsigned long long)ne[0] + ne[1];
-  unsigned long long cap = 1024;
-  while (cap < 2 * tot) cap <<= 1;
-  if (cap > (1ull << 31)) return TSM_E_NOMEM;
-  const uint32_t mask = (uint32_t)cap - 1;
-  if (!d_table.alloc(sizeof(MoveKey) * cap)) return TSM_E_CUDA;
-  CU(cudaEventRecord(c->diff_ev[2], st));
-  CU(cudaMemsetAsync(d_table.p, 0, sizeof(MoveKey) * cap, st));
-  for (int s = 0; s < 2; ++s) {
-    MoveBufs& m = mb[s];
-    if (!m.cnt.alloc(4 * cap) || !m.cursor.alloc(4 * cap) || !m.base.alloc(8 * (cap + 1)) || !m.slot_of.alloc(4 * (size_t)ne[s]) ||
-        !m.seg.alloc(4 * (size_t)ne[s]) || (s == 0 && !m.seg_slot.alloc(4 * (size_t)ne[s])))
-      return TSM_E_CUDA;
-    CU(cudaMemsetAsync(m.cnt.p, 0, 4 * cap, st));
-    CU(cudaMemsetAsync(m.cursor.p, 0, 4 * cap, st));
-    if (ne[s])
-      k_move_insert<<<(ne[s] + 255) / 256, 256, 0, st>>>(m.ent.as<uint32_t>(), ne[s], side[s]->d.line_hash, side[s]->d.line_base, n,
-                                                          side[s]->grp.as<uint16_t>(), d_table.as<MoveKey>(), mask, m.cnt.as<uint32_t>(),
-                                                          m.slot_of.as<uint32_t>());
-  }
-  if (!d_slot_bsum.alloc(8 * (cap / XS_TILE + 4))) return TSM_E_CUDA;
-  for (int s = 0; s < 2; ++s) {
-    MoveBufs& m = mb[s];
-    xscan(m.cnt.as<uint32_t>(), (uint32_t)cap, d_slot_bsum.as<unsigned long long>(), m.base.as<unsigned long long>(), st);
-    if (ne[s])
-      k_move_scatter<<<(ne[s] + 255) / 256, 256, 0, st>>>(m.ent.as<uint32_t>(), m.slot_of.as<uint32_t>(), ne[s], m.base.as<unsigned long long>(),
-                                                           m.cursor.as<uint32_t>(), m.seg.as<uint32_t>(), s == 0 ? m.seg_slot.as<uint32_t>() : nullptr);
-    launches += 3 + (ne[s] ? 2 : 0);
-  }
-  MoveSide ms[2];
-  for (int s = 0; s < 2; ++s)
-    ms[s] = MoveSide{side[s]->d.line_hash, mb[s].flag.as<uint8_t>(), mb[s].ridx.as<unsigned long long>(), mb[s].run_end.as<uint32_t>(),
-                     mb[s].best.as<unsigned long long>()};
-  if (ne[0] && ne[1]) {
-    k_move_reach<<<std::min((ne[0] + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(ms[0], ms[1], mb[0].seg.as<uint32_t>(), mb[0].seg_slot.as<uint32_t>(),
-                                                                               ne[0], mb[1].seg.as<uint32_t>(), mb[1].base.as<unsigned long long>());
-    ++launches;
-  }
-  CU(cudaGetLastError());
-  CU(cudaEventRecord(c->diff_ev[3], st));
-  // ---- the blocks of every run, in line order
-  CU(cudaEventRecord(c->diff_ev[4], st));
-  for (int s = 0; s < 2; ++s) {
-    MoveBufs& m = mb[s];
-    if (!m.start.alloc(4 * (size_t)ne[s]) || !m.sidx.alloc(8 * ((size_t)ne[s] + 1)) || !m.starts.alloc(4 * (size_t)ne[s]) ||
-        !m.rcnt.alloc(4 * (size_t)nr[s]) || !m.rbase.alloc(8 * ((size_t)nr[s] + 1)) || !m.blocks.alloc(sizeof(tsm_move_block) * (size_t)ne[s]))
-      return TSM_E_CUDA;
-    const unsigned ge = (ne[s] + 255) / 256, g = (nr[s] + 255) / 256;
-    const uint32_t* ent = m.ent.as<uint32_t>();
-    const unsigned long long* best = m.best.as<unsigned long long>();
-    if (ne[s])
-      k_move_starts<0><<<ge, 256, 0, st>>>(ent, ne[s], best, m.apre.as<unsigned long long>(), m.start.as<uint32_t>(), nullptr, nullptr);
-    xscan(m.start.as<uint32_t>(), ne[s], bsum, m.sidx.as<unsigned long long>(), st);
-    if (ne[s])
-      k_move_starts<1><<<ge, 256, 0, st>>>(ent, ne[s], best, nullptr, m.start.as<uint32_t>(), m.sidx.as<unsigned long long>(),
-                                           m.starts.as<uint32_t>());
-    if (nr[s])
-      k_move_runs<0><<<g, 256, 0, st>>>(m.run_first.as<uint32_t>(), m.run_end.as<uint32_t>(), nr[s], best, m.eidx.as<unsigned long long>(),
-                                        m.sidx.as<unsigned long long>(), ne[s], m.starts.as<uint32_t>(), m.rcnt.as<uint32_t>(), nullptr, nullptr);
-    xscan(m.rcnt.as<uint32_t>(), nr[s], bsum, m.rbase.as<unsigned long long>(), st);
-    if (nr[s])
-      k_move_runs<1><<<g, 256, 0, st>>>(m.run_first.as<uint32_t>(), m.run_end.as<uint32_t>(), nr[s], best, m.eidx.as<unsigned long long>(),
-                                        m.sidx.as<unsigned long long>(), ne[s], m.starts.as<uint32_t>(), nullptr,
-                                        m.rbase.as<unsigned long long>(), m.blocks.as<tsm_move_block>());
-    CU(cudaMemcpyAsync(pin + s, m.rbase.as<unsigned long long>() + nr[s], 8, cudaMemcpyDeviceToHost, st));
-    launches += 6 + (ne[s] ? 2 : 0) + (nr[s] ? 2 : 0);
-  }
-  CU(cudaGetLastError());
-  CU(cudaEventRecord(c->diff_ev[5], st));
-  CU(cudaStreamSynchronize(st));
-  const uint32_t nb[2] = {(uint32_t)pin[0], (uint32_t)pin[1]};
-  CU(cudaEventRecord(c->diff_ev[6], st));
-  for (int s = 0; s < 2; ++s)
-    if (nb[s]) {
-      k_move_mark<<<(ne[s] + 255) / 256, 256, 0, st>>>(mb[s].ent.as<uint32_t>(), ne[s], mb[s].blocks.as<tsm_move_block>(), nb[s],
-                                                        side[s]->d.line_flag, side[s]->line_mark.as<uint8_t>());
+  float* const dm = c->last_ms[MS_DIFF];
+  return pair_call(c, olds, news, PAIR_GRP | PAIR_HOST_BASE, &dm[0], stream, [&](HostSidePair& P, cudaStream_t st) -> int {
+    mt[0] = dm[0];
+    const int rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
+    if (rc != TSM_OK) return rc;
+    mt[1] = dm[1] + dm[2];
+    MoveBufs mb[2];
+    DevBuf d_bsum, d_slot_bsum, d_table;
+    HostSide* const side[2] = {&P.A, &P.B};
+    const uint32_t T[2] = {(uint32_t)P.A.total, (uint32_t)P.B.total};
+    int launches = 0;
+    if (!d_bsum.alloc(8 * ((size_t)std::max(T[0], T[1]) / XS_TILE + 4))) return TSM_E_CUDA;
+    unsigned long long* const bsum = d_bsum.as<unsigned long long>();
+    CU(cudaEventRecord(c->diff_ev[EV_MOVE_FLAGS.from], st));
+    for (int s = 0; s < 2; ++s) {
+      MoveBufs& m = mb[s];
+      const size_t L = T[s];
+      if (!m.flag.alloc(L) || !m.alnum.alloc(4 * L) || !m.chg.alloc(4 * L) || !m.head.alloc(4 * L) || !m.apre.alloc(8 * (L + 1)) ||
+          !m.eidx.alloc(8 * (L + 1)) || !m.ridx.alloc(8 * (L + 1)) || !m.best.alloc(8 * L))
+        return TSM_E_CUDA;
+      CU(cudaMemsetAsync(m.best.p, 0, 8 * L, st));
+      if (L) k_move_lines<<<(unsigned)((L + 255) / 256), 256, 0, st>>>(side[s]->d, n, T[s], side[s]->line_mark.as<uint8_t>(), m.flag.as<uint8_t>(),
+                                                                        m.alnum.as<uint32_t>(), m.chg.as<uint32_t>(), m.head.as<uint32_t>());
+      xscan(m.alnum.as<uint32_t>(), T[s], bsum, m.apre.as<unsigned long long>(), st);
+      xscan(m.chg.as<uint32_t>(), T[s], bsum, m.eidx.as<unsigned long long>(), st);
+      xscan(m.head.as<uint32_t>(), T[s], bsum, m.ridx.as<unsigned long long>(), st);
+      launches += (L ? 1 : 0) + 9;
+    }
+    CU(cudaGetLastError());
+    unsigned long long* pin = c->h_rb->u64;
+    for (int s = 0; s < 2; ++s) {
+      CU(cudaMemcpyAsync(pin + 2 * s, mb[s].eidx.as<unsigned long long>() + T[s], 8, cudaMemcpyDeviceToHost, st));
+      CU(cudaMemcpyAsync(pin + 2 * s + 1, mb[s].ridx.as<unsigned long long>() + T[s], 8, cudaMemcpyDeviceToHost, st));
+    }
+    CU(cudaStreamSynchronize(st));
+    const uint32_t ne[2] = {(uint32_t)pin[0], (uint32_t)pin[2]}, nr[2] = {(uint32_t)pin[1], (uint32_t)pin[3]};
+    for (int s = 0; s < 2; ++s) {
+      MoveBufs& m = mb[s];
+      if (!m.ent.alloc(4 * (size_t)ne[s]) || !m.run_first.alloc(4 * (size_t)nr[s]) || !m.run_end.alloc(4 * (size_t)nr[s])) return TSM_E_CUDA;
+      if (T[s])
+        k_move_compact<<<(T[s] + 255) / 256, 256, 0, st>>>(m.flag.as<uint8_t>(), T[s], m.eidx.as<unsigned long long>(), m.ridx.as<unsigned long long>(),
+                                                            m.ent.as<uint32_t>(), m.run_first.as<uint32_t>(), m.run_end.as<uint32_t>());
+    }
+    CU(cudaEventRecord(c->diff_ev[EV_MOVE_FLAGS.to], st));
+    // ---- the join: one table over the entries of both sides, at most half full
+    const unsigned long long tot = (unsigned long long)ne[0] + ne[1];
+    unsigned long long cap = 1024;
+    while (cap < 2 * tot) cap <<= 1;
+    if (cap > (1ull << 31)) return TSM_E_NOMEM;
+    const uint32_t mask = (uint32_t)cap - 1;
+    if (!d_table.alloc(sizeof(MoveKey) * cap)) return TSM_E_CUDA;
+    CU(cudaEventRecord(c->diff_ev[EV_MOVE_JOIN.from], st));
+    CU(cudaMemsetAsync(d_table.p, 0, sizeof(MoveKey) * cap, st));
+    for (int s = 0; s < 2; ++s) {
+      MoveBufs& m = mb[s];
+      if (!m.cnt.alloc(4 * cap) || !m.cursor.alloc(4 * cap) || !m.base.alloc(8 * (cap + 1)) || !m.slot_of.alloc(4 * (size_t)ne[s]) ||
+          !m.seg.alloc(4 * (size_t)ne[s]) || (s == 0 && !m.seg_slot.alloc(4 * (size_t)ne[s])))
+        return TSM_E_CUDA;
+      CU(cudaMemsetAsync(m.cnt.p, 0, 4 * cap, st));
+      CU(cudaMemsetAsync(m.cursor.p, 0, 4 * cap, st));
+      if (ne[s])
+        k_move_insert<<<(ne[s] + 255) / 256, 256, 0, st>>>(m.ent.as<uint32_t>(), ne[s], side[s]->d.line_hash, side[s]->d.line_base, n,
+                                                            side[s]->grp.as<uint16_t>(), d_table.as<MoveKey>(), mask, m.cnt.as<uint32_t>(),
+                                                            m.slot_of.as<uint32_t>());
+    }
+    if (!d_slot_bsum.alloc(8 * (cap / XS_TILE + 4))) return TSM_E_CUDA;
+    for (int s = 0; s < 2; ++s) {
+      MoveBufs& m = mb[s];
+      xscan(m.cnt.as<uint32_t>(), (uint32_t)cap, d_slot_bsum.as<unsigned long long>(), m.base.as<unsigned long long>(), st);
+      if (ne[s])
+        k_move_scatter<<<(ne[s] + 255) / 256, 256, 0, st>>>(m.ent.as<uint32_t>(), m.slot_of.as<uint32_t>(), ne[s], m.base.as<unsigned long long>(),
+                                                             m.cursor.as<uint32_t>(), m.seg.as<uint32_t>(), s == 0 ? m.seg_slot.as<uint32_t>() : nullptr);
+      launches += 3 + (ne[s] ? 2 : 0);
+    }
+    MoveSide ms[2];
+    for (int s = 0; s < 2; ++s)
+      ms[s] = MoveSide{side[s]->d.line_hash, mb[s].flag.as<uint8_t>(), mb[s].ridx.as<unsigned long long>(), mb[s].run_end.as<uint32_t>(),
+                       mb[s].best.as<unsigned long long>()};
+    if (ne[0] && ne[1]) {
+      k_move_reach<<<std::min((ne[0] + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(ms[0], ms[1], mb[0].seg.as<uint32_t>(), mb[0].seg_slot.as<uint32_t>(),
+                                                                                 ne[0], mb[1].seg.as<uint32_t>(), mb[1].base.as<unsigned long long>());
       ++launches;
     }
-  CU(cudaGetLastError());
-  CU(cudaEventRecord(c->diff_ev[7], st));
-  mk.n_old = (int64_t)T[0]; mk.n_new = (int64_t)T[1];
-  out->n_old_blocks = nb[0]; out->n_new_blocks = nb[1];
-  if (mk.line_base_old) memcpy(mk.line_base_old, P.A.base.data(), sizeof(int64_t) * ((size_t)n + 1));
-  if (mk.line_base_new) memcpy(mk.line_base_new, P.B.base.data(), sizeof(int64_t) * ((size_t)n + 1));
-  CU(cudaStreamSynchronize(st));
-  c->move_ms[2] = elapsed_ms(c->diff_ev[0], c->diff_ev[1]) + elapsed_ms(c->diff_ev[2], c->diff_ev[3]);
-  c->move_ms[3] = elapsed_ms(c->diff_ev[4], c->diff_ev[5]) + elapsed_ms(c->diff_ev[6], c->diff_ev[7]);
-  c->launches += launches;
-  if ((mk.del && mk.del_cap < mk.n_old) || (mk.ins && mk.ins_cap < mk.n_new) || (out->old_blocks && out->old_cap < (int64_t)nb[0]) ||
-      (out->new_blocks && out->new_cap < (int64_t)nb[1]))
-    return TSM_E_CAPACITY;
-  uint8_t* const h_mark[2] = {mk.del, mk.ins};
-  tsm_move_block* const h_blocks[2] = {out->old_blocks, out->new_blocks};
-  for (int s = 0; s < 2; ++s) {
-    if (h_mark[s] && T[s]) CU(cudaMemcpyAsync(h_mark[s], side[s]->line_mark.p, T[s], cudaMemcpyDeviceToHost, st));
-    if (h_blocks[s] && nb[s]) CU(cudaMemcpyAsync(h_blocks[s], mb[s].blocks.p, sizeof(tsm_move_block) * nb[s], cudaMemcpyDeviceToHost, st));
-  }
-  CU(cudaStreamSynchronize(st));
-  return TSM_OK;
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_MOVE_JOIN.to], st));
+    // ---- the blocks of every run, in line order
+    CU(cudaEventRecord(c->diff_ev[EV_MOVE_RUNS.from], st));
+    for (int s = 0; s < 2; ++s) {
+      MoveBufs& m = mb[s];
+      if (!m.start.alloc(4 * (size_t)ne[s]) || !m.sidx.alloc(8 * ((size_t)ne[s] + 1)) || !m.starts.alloc(4 * (size_t)ne[s]) ||
+          !m.rcnt.alloc(4 * (size_t)nr[s]) || !m.rbase.alloc(8 * ((size_t)nr[s] + 1)) || !m.blocks.alloc(sizeof(tsm_move_block) * (size_t)ne[s]))
+        return TSM_E_CUDA;
+      const unsigned ge = (ne[s] + 255) / 256, g = (nr[s] + 255) / 256;
+      const uint32_t* ent = m.ent.as<uint32_t>();
+      const unsigned long long* best = m.best.as<unsigned long long>();
+      if (ne[s])
+        k_move_starts<0><<<ge, 256, 0, st>>>(ent, ne[s], best, m.apre.as<unsigned long long>(), m.start.as<uint32_t>(), nullptr, nullptr);
+      xscan(m.start.as<uint32_t>(), ne[s], bsum, m.sidx.as<unsigned long long>(), st);
+      if (ne[s])
+        k_move_starts<1><<<ge, 256, 0, st>>>(ent, ne[s], best, nullptr, m.start.as<uint32_t>(), m.sidx.as<unsigned long long>(),
+                                             m.starts.as<uint32_t>());
+      if (nr[s])
+        k_move_runs<0><<<g, 256, 0, st>>>(m.run_first.as<uint32_t>(), m.run_end.as<uint32_t>(), nr[s], best, m.eidx.as<unsigned long long>(),
+                                          m.sidx.as<unsigned long long>(), ne[s], m.starts.as<uint32_t>(), m.rcnt.as<uint32_t>(), nullptr, nullptr);
+      xscan(m.rcnt.as<uint32_t>(), nr[s], bsum, m.rbase.as<unsigned long long>(), st);
+      if (nr[s])
+        k_move_runs<1><<<g, 256, 0, st>>>(m.run_first.as<uint32_t>(), m.run_end.as<uint32_t>(), nr[s], best, m.eidx.as<unsigned long long>(),
+                                          m.sidx.as<unsigned long long>(), ne[s], m.starts.as<uint32_t>(), nullptr,
+                                          m.rbase.as<unsigned long long>(), m.blocks.as<tsm_move_block>());
+      CU(cudaMemcpyAsync(pin + s, m.rbase.as<unsigned long long>() + nr[s], 8, cudaMemcpyDeviceToHost, st));
+      launches += 6 + (ne[s] ? 2 : 0) + (nr[s] ? 2 : 0);
+    }
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_MOVE_RUNS.to], st));
+    CU(cudaStreamSynchronize(st));
+    const uint32_t nb[2] = {(uint32_t)pin[0], (uint32_t)pin[1]};
+    CU(cudaEventRecord(c->diff_ev[EV_MOVE_MARK.from], st));
+    for (int s = 0; s < 2; ++s)
+      if (nb[s]) {
+        k_move_mark<<<(ne[s] + 255) / 256, 256, 0, st>>>(mb[s].ent.as<uint32_t>(), ne[s], mb[s].blocks.as<tsm_move_block>(), nb[s],
+                                                          side[s]->d.line_flag, side[s]->line_mark.as<uint8_t>());
+        ++launches;
+      }
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_MOVE_MARK.to], st));
+    mk.n_old = (int64_t)T[0]; mk.n_new = (int64_t)T[1];
+    out->n_old_blocks = nb[0]; out->n_new_blocks = nb[1];
+    if (mk.line_base_old) memcpy(mk.line_base_old, P.A.base.data(), sizeof(int64_t) * ((size_t)n + 1));
+    if (mk.line_base_new) memcpy(mk.line_base_new, P.B.base.data(), sizeof(int64_t) * ((size_t)n + 1));
+    CU(cudaStreamSynchronize(st));
+    mt[2] = span_ms(c, EV_MOVE_FLAGS) + span_ms(c, EV_MOVE_JOIN);
+    mt[3] = span_ms(c, EV_MOVE_RUNS) + span_ms(c, EV_MOVE_MARK);
+    c->launches += launches;
+    if ((mk.del && mk.del_cap < mk.n_old) || (mk.ins && mk.ins_cap < mk.n_new) || (out->old_blocks && out->old_cap < (int64_t)nb[0]) ||
+        (out->new_blocks && out->new_cap < (int64_t)nb[1]))
+      return TSM_E_CAPACITY;
+    uint8_t* const h_mark[2] = {mk.del, mk.ins};
+    tsm_move_block* const h_blocks[2] = {out->old_blocks, out->new_blocks};
+    for (int s = 0; s < 2; ++s) {
+      if (h_mark[s] && T[s]) CU(cudaMemcpyAsync(h_mark[s], side[s]->line_mark.p, T[s], cudaMemcpyDeviceToHost, st));
+      if (h_blocks[s] && nb[s]) CU(cudaMemcpyAsync(h_blocks[s], mb[s].blocks.p, sizeof(tsm_move_block) * nb[s], cudaMemcpyDeviceToHost, st));
+    }
+    CU(cudaStreamSynchronize(st));
+    return TSM_OK;
+  });
 }
 
-extern "C" int tsm_moves_last_ms(tsm_ctx* c, float* ms4) {
-  if (!c || !ms4) return TSM_E_ARG;
-  for (int i = 0; i < 4; ++i) ms4[i] = c->move_ms[i];
-  return TSM_OK;
-}
+extern "C" int tsm_moves_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_MOVE, ms4, 4); }
