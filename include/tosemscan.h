@@ -302,6 +302,32 @@ typedef struct tsm_clone_result {
 int tsm_clones(tsm_ctx* ctx, const tsm_corpus* corpus, int32_t min_lines, tsm_clone_result* out, void* stream);
 int tsm_clones_last_ms(tsm_ctx* ctx, float* ms3);
 
+/* Near-miss duplicated test code (docs/SPEC.md section 21, `tosem-scan clones --blind`): the classes of section 15 over the kept
+ * lines of the corpus, whose windows are compared by the blind form of their lines - identifiers, numbers and literals
+ * replaced by placeholders, keywords and punctuation kept, whitespace and comments dropped, by a lexer that knows where
+ * comments and strings (also those spanning lines) begin and end.  A line is kept when its blind form is not empty; kept lines
+ * are numbered globally, files in order.  `out` means what it means for tsm_clones, over kept lines: member and class_len are in
+ * kept numbering, file_dup / file_dup_assert count kept lines, and out->line_base is the line_base of section 3.  `blind`
+ * (may be NULL): kept_base[f] = the kept lines before file f, kept_line / blind_hash the original global line and the
+ * bytes_hash of the blind form of each kept line (kept_cap entries each), file_kept_assert[f] = the kept assertion lines of
+ * file f; n_kept is always set.  Any pointer may be NULL; a short kept_cap (with kept_line or blind_hash given), class_cap or
+ * member_cap returns TSM_E_CAPACITY with all counts set.  Arguments, streams and memory errors as for tsm_clones.
+ * Kernels: k_scan for the line records; k_blind_state (per-line transfer functions of the cross-line lexer states),
+ * k_blind_scan (per-file scan of them), k_blind_lines (the blind hash of every line), the compaction of the kept lines
+ * (csrc/tsm_blind_kernels.cuh); then the kernels of tsm_clones over the kept lines.
+ * tsm_clones_blind_last_ms: device time of the last call, ms4 = { k_scan, lexing + compaction, grouping + classes, members +
+ * coverage }. */
+typedef struct tsm_blind_result {
+  int64_t* kept_base;                                    /* [n_files+1] kept lines before each file (global kept numbering) */
+  int64_t* kept_line;                                    /* [kept_cap]  original global line (section 3) of each kept line */
+  uint64_t* blind_hash;                                  /* [kept_cap]  bytes_hash of each kept line's blind form */
+  uint32_t* file_kept_assert;                            /* [n_files]   kept lines of the file that are assertion lines */
+  int64_t kept_cap; int64_t n_kept;
+} tsm_blind_result;
+int tsm_clones_blind(tsm_ctx* ctx, const tsm_corpus* corpus, int32_t min_lines, tsm_blind_result* blind, tsm_clone_result* out,
+                     void* stream);
+int tsm_clones_blind_last_ms(tsm_ctx* ctx, float* ms4);
+
 /* Test smells (docs/SPEC.md section 18, `tosem-scan smells`): the tests of every file (section-16 cases whose header opens a test
  * by the rule of its family), their bodies and the nine smells below, as one record per test in global line order (files in
  * order, then header line) and the smell bits of every line (its instances; 0 outside test bodies).  Bit k of `smells` and of

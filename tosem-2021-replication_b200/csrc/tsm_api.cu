@@ -21,6 +21,7 @@
 #include "tsm_lines_kernels.cuh"
 #include "tsm_similar_kernels.cuh"
 #include "tsm_clone_kernels.cuh"
+#include "tsm_blind_kernels.cuh"
 #include "tsm_case_kernels.cuh"
 #include "tsm_edit_kernels.cuh"
 #include "tsm_smell_kernels.cuh"
@@ -81,6 +82,7 @@ enum Timed {
               // its own row's for tsm_similarity and tsm_diff_pairs_assert_edits)
   MS_SIM,     // k_scan over both sides, sort / merge, k_similarity of the last tsm_similarity
   MS_CLONE,   // k_scan, grouping + classes, members + coverage of the last tsm_clones
+  MS_BLIND,   // k_scan, lexing + compaction, grouping + classes, members + coverage of the last tsm_clones_blind
   MS_SMELL,   // k_scan, kinds + case spans, k_smell_lines, k_smell_tests of the last tsm_smells
   MS_CHURN,   // k_scan, smell stages, the diff, case records + k_smell_churn of the last tsm_diff_pairs_smells
   MS_EDIT,    // k_scan, the diff, compact to pairing (host clock) of the last tsm_diff_pairs_assert_edits
@@ -160,6 +162,8 @@ struct tsm_ctx {
 //   diff_core                                              SMALL   SMALL   LEFT    LEFT                    diff_core, per launch
 //   tsm_similarity                                         LISTS   PAIRS   END                             at the end
 //   tsm_clones                                             GROUP   MEMBERS END                             at the members / end
+//   tsm_clones_blind                                       GROUP   MEMBERS END     LEX     LEX_END         at the kept count /
+//                                                                                                         the members / end
 //   tsm_smells (smell_stage: LINES - END)                  KINDS   LINES   TESTS   END                     at the end
 //   tsm_diff_pairs_smells: smell stages    CHURN_SMELLS            LINES*  TESTS*  END*                    before the diff
 //     case records + churn, behind diff    CHURN_CASES                                                     at the end
@@ -170,6 +174,7 @@ struct EvSpan { int from, to; };
 constexpr EvSpan EV_SCAN[2] = {{0, 1}, {6, 7}}, EV_SMALL = {2, 3}, EV_LEFT = {4, 5};
 constexpr int EV_SIM_LISTS = 2, EV_SIM_PAIRS = 3, EV_SIM_END = 4;
 constexpr int EV_CLONE_GROUP = 2, EV_CLONE_MEMBERS = 3, EV_CLONE_END = 4;
+constexpr int EV_BLIND_LEX = 5, EV_BLIND_LEX_END = 6;
 constexpr int EV_SMELL_KINDS = 2, EV_SMELL_LINES = 3, EV_SMELL_TESTS = 4, EV_SMELL_END = 5;
 constexpr EvSpan EV_CHURN_SMELLS = {0, 1}, EV_CHURN_CASES = {0, 1};   // the old side's scan slots, then the same again
 constexpr EvSpan EV_MOVE_FLAGS = {0, 1}, EV_MOVE_JOIN = {2, 3}, EV_MOVE_RUNS = {4, 5}, EV_MOVE_MARK = {6, 7};
@@ -360,6 +365,9 @@ extern "C" int tsm_create(tsm_ctx** out, int device, int64_t max_arena_bytes, in
     uint32_t elut[256], lutb[256];
     build_elut(elut);
     build_lut_b(lutb);
+    BlindKw bkw[BLIND_KW_SLOTS];
+    uint8_t bkind[BLIND_KW_SLOTS];
+    blind_keyword_table(bkw, bkind);
     if (cudaMemcpyToSymbol(c_lut, lut, sizeof lut) != cudaSuccess ||
         cudaMemcpyToSymbol(c_elut, elut, sizeof elut) != cudaSuccess ||
         cudaMemcpyToSymbol(c_cat_slot, slot, sizeof slot) != cudaSuccess ||
@@ -367,6 +375,8 @@ extern "C" int tsm_create(tsm_ctx** out, int device, int64_t max_arena_bytes, in
         cudaMemcpyToSymbol(c_cat_blob, blob, TSM_CAT_BLOB_LEN + 1) != cudaSuccess ||
         cudaMemset(c->d_arena, 0, (size_t)c->max_arena + 4096) != cudaSuccess ||
         cudaMemcpyToSymbol(c_lut_b, lutb, sizeof lutb) != cudaSuccess ||
+        cudaMemcpyToSymbol(c_blind_kw, bkw, sizeof bkw) != cudaSuccess ||
+        cudaMemcpyToSymbol(c_blind_kind, bkind, sizeof bkind) != cudaSuccess ||
         cudaFuncSetAttribute(k_scan_t<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN2_SMEM) != cudaSuccess ||
         cudaFuncSetAttribute(k_scan_t<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCAN2_SMEM_B) != cudaSuccess ||
         !diff_small_smem<DIFF_PLAIN>() || !diff_small_smem<DIFF_EMIT>() || !diff_small_smem<DIFF_MARKS>() ||
@@ -1918,9 +1928,103 @@ extern "C" int tsm_statements(tsm_ctx* c, const tsm_corpus* k, int64_t* line_bas
 }
 
 // ------------------------------------------------------------------------------------- SPEC section 15 clones
-// The line records of the corpus (line_records), then the kernels of tsm_clone_kernels.cuh.  One synchronisation between
-// the grouping and the members reads the class and fragment counts: a short cap returns there, else the fragments are
-// scattered, sorted and copied back with the coverage.
+// Section 15 over T lines (T > 0) of nfu files: their hashes, per-file bases line_base[nfu + 1] and assertion flags on the
+// device; with SKIP_EMPTY the window test reads the lines' bytes (arena, off, line_end).  The kernels of tsm_clone_kernels.cuh,
+// with one synchronisation between the grouping and the members that reads the class and fragment counts: a short cap returns
+// there, else the fragments are scattered, sorted and copied back with the coverage.  ms[0] / ms[1]: grouping + classes, members
+// + coverage.
+template <bool SKIP_EMPTY>
+static int clone_classes(tsm_ctx* c, const unsigned long long* hash, const unsigned long long* line_base, uint32_t nfu, uint32_t T,
+                         const uint8_t* line_flag, const uint32_t* line_end, const uint8_t* arena, const int32_t* off, uint32_t n,
+                         tsm_clone_result* out, float* ms, cudaStream_t st) {
+  size_t slots = 1;                                      // a power of two, at least 2 x the windows (<= lines)
+  while (slots < 2 * (size_t)T) slots <<= 1;
+  const uint32_t mask = (uint32_t)(slots - 1);
+  const size_t table_bytes = (slots + 1) * (sizeof(CloneSlot) + 3 * sizeof(uint32_t));
+  {
+    size_t free_b = 0, total_b = 0;
+    CU(cudaMemGetInfo(&free_b, &total_b));
+    if (table_bytes > free_b) return TSM_E_NOMEM;
+  }
+  const size_t L = (size_t)T, nb = L / XS_TILE + 4;
+  DevBuf d_key, d_slot, d_wflag, d_table, d_plo, d_phi, d_scls, d_dup, d_head, d_ext, d_cidx, d_cover, d_rep, d_size, d_cbase,
+      d_big, d_nbig, d_bsum, d_len, d_cursor, d_member, d_wk, d_fdup;
+  if (!d_key.alloc(8 * L) || !d_slot.alloc(4 * L) || !d_wflag.alloc(L) || !d_table.alloc(sizeof(CloneSlot) * (slots + 1)) ||
+      !d_plo.alloc(4 * (slots + 1)) || !d_phi.alloc(4 * (slots + 1)) || !d_scls.alloc(4 * (slots + 1)) || !d_dup.alloc(4 * L) ||
+      !d_head.alloc(4 * L) || !d_ext.alloc(L) || !d_cidx.alloc(8 * (L + 1)) || !d_cover.alloc(8 * (L + 1)) || !d_rep.alloc(4 * L) ||
+      !d_size.alloc(4 * L) || !d_cbase.alloc(8 * (L + 1)) || !d_big.alloc(4 * L) || !d_nbig.alloc(4) || !d_bsum.alloc(8 * nb) ||
+      !d_len.alloc(4 * L) || !d_fdup.alloc(8 * (size_t)nfu)) {
+    cudaGetLastError();
+    return TSM_E_NOMEM;
+  }
+  CloneSlot* table = d_table.as<CloneSlot>();
+  uint32_t* slot_of = d_slot.as<uint32_t>();
+  const unsigned grid = (unsigned)((L + 255) / 256);
+  CU(cudaEventRecord(c->diff_ev[EV_CLONE_GROUP], st));
+  CU(cudaMemsetAsync(d_table.p, 0, sizeof(CloneSlot) * (slots + 1), st));
+  CU(cudaMemsetAsync(d_plo.p, 0xFF, 4 * (slots + 1), st));
+  CU(cudaMemsetAsync(d_phi.p, 0, 4 * (slots + 1), st));
+  CU(cudaMemsetAsync(d_scls.p, 0xFF, 4 * (slots + 1), st));
+  CU(cudaMemsetAsync(d_size.p, 0, 4 * L, st));
+  CU(cudaMemsetAsync(d_nbig.p, 0, 4, st));
+  k_ngrams<<<grid, 256, 0, st>>>(hash, line_base, nfu, T, n, d_key.as<unsigned long long>());
+  k_clone_insert<SKIP_EMPTY><<<grid, 256, 0, st>>>(d_key.as<unsigned long long>(), line_base, nfu, line_end, arena, off, T, n, table,
+                                       mask, slot_of, d_wflag.as<uint8_t>());
+  k_clone_preds<<<grid, 256, 0, st>>>(table, slot_of, d_wflag.as<uint8_t>(), T, d_plo.as<uint32_t>(), d_phi.as<uint32_t>());
+  k_clone_heads<<<grid, 256, 0, st>>>(table, slot_of, d_plo.as<uint32_t>(), d_phi.as<uint32_t>(), T, d_dup.as<uint32_t>(),
+                                      d_head.as<uint32_t>(), d_ext.as<uint8_t>());
+  xscan(d_head.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), d_cidx.as<unsigned long long>(), st);
+  xscan(d_dup.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), d_cover.as<unsigned long long>(), st);
+  k_clone_classes<<<grid, 256, 0, st>>>(d_head.as<uint32_t>(), d_cidx.as<unsigned long long>(), slot_of, table, T, d_rep.as<uint32_t>(),
+                                        d_size.as<uint32_t>(), d_scls.as<uint32_t>(), d_big.as<uint32_t>(), d_nbig.as<uint32_t>());
+  xscan(d_size.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), d_cbase.as<unsigned long long>(), st);
+  k_clone_length<<<(unsigned)c->sms * 8, 256, 0, st>>>(d_rep.as<uint32_t>(), d_ext.as<uint8_t>(), T, n, d_cidx.as<unsigned long long>() + L,
+                                                       d_len.as<uint32_t>());
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(c->diff_ev[EV_CLONE_MEMBERS], st));
+  unsigned long long* pin = c->h_rb->u64;                 // classes, fragments, large classes
+  CU(cudaMemcpyAsync(pin, d_cidx.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(pin + 1, d_cbase.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(pin + 2, d_nbig.p, 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  c->launches += 15;                                     // k_ngrams, insert, preds, heads, 3 x xscan (3 each), classes, length
+  const uint32_t nc = (uint32_t)pin[0], nbig = (uint32_t)(pin[2] & 0xFFFFFFFFu);
+  const unsigned long long nm = pin[1];
+  out->n_classes = (int64_t)nc;
+  out->n_members = (int64_t)nm;
+  ms[0] = elapsed_ms(c->diff_ev[EV_CLONE_GROUP], c->diff_ev[EV_CLONE_MEMBERS]);
+  if ((out->class_cap < (int64_t)nc && (out->class_base || out->class_len)) || (out->member_cap < (int64_t)nm && out->member))
+    return TSM_E_CAPACITY;
+  if (nc) {
+    if (!d_cursor.alloc(4 * (size_t)nc) || !d_member.alloc(8 * nm) || !d_wk.alloc(4 * nm)) { cudaGetLastError(); return TSM_E_NOMEM; }
+    unsigned long long* member = d_member.as<unsigned long long>();
+    CU(cudaMemsetAsync(d_cursor.p, 0, 4 * (size_t)nc, st));
+    k_clone_scatter<<<grid, 256, 0, st>>>(slot_of, d_scls.as<uint32_t>(), d_cbase.as<unsigned long long>(), T, d_cursor.as<uint32_t>(), member);
+    k_clone_sort_warp<<<(unsigned)(((size_t)nc * 32 + 255) / 256), 256, 0, st>>>(d_cbase.as<unsigned long long>(), nc, member);
+    c->launches += 2;
+    if (nbig) {
+      k_clone_sort_cta<<<std::min<unsigned>(nbig, (unsigned)c->sms * 2), SIM_SORT_THREADS, SIM_SORT_SMEM, st>>>(
+          d_cbase.as<unsigned long long>(), d_big.as<uint32_t>(), d_nbig.as<uint32_t>(), member, d_wk.as<uint32_t>());
+      c->launches += 1;
+    }
+    uint32_t* fdup = d_fdup.as<uint32_t>();
+    k_clone_cover<<<(unsigned)(((size_t)nfu * 32 + 255) / 256), 256, 0, st>>>(line_base, nfu, d_cover.as<unsigned long long>(),
+                                                                            line_flag, n, fdup, fdup + nfu);
+    c->launches += 1;
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_CLONE_END], st));
+    if (out->file_dup) CU(cudaMemcpyAsync(out->file_dup, fdup, 4 * (size_t)nfu, cudaMemcpyDeviceToHost, st));
+    if (out->file_dup_assert) CU(cudaMemcpyAsync(out->file_dup_assert, fdup + nfu, 4 * (size_t)nfu, cudaMemcpyDeviceToHost, st));
+    if (out->class_base) CU(cudaMemcpyAsync(out->class_base, d_cbase.p, 8 * ((size_t)nc + 1), cudaMemcpyDeviceToHost, st));
+    if (out->class_len) CU(cudaMemcpyAsync(out->class_len, d_len.p, 4 * (size_t)nc, cudaMemcpyDeviceToHost, st));
+    if (out->member) CU(cudaMemcpyAsync(out->member, member, 8 * nm, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    ms[1] = elapsed_ms(c->diff_ev[EV_CLONE_MEMBERS], c->diff_ev[EV_CLONE_END]);
+  }
+  return TSM_OK;
+}
+
+// The line records of the corpus (line_records), then clone_classes over them.
 extern "C" int tsm_clones(tsm_ctx* c, const tsm_corpus* k, int32_t min_lines, tsm_clone_result* out, void* stream) {
   if (!c || !k || !out || k->n_files < 0 || min_lines < 1 || min_lines > 1024 || out->class_cap < 0 || out->member_cap < 0) return TSM_E_ARG;
   const int32_t nf = k->n_files;
@@ -1935,96 +2039,84 @@ extern "C" int tsm_clones(tsm_ctx* c, const tsm_corpus* k, int32_t min_lines, ts
   if (!line_base) { own_base.resize((size_t)nf + 1); line_base = own_base.data(); }
   int64_t n_lines = 0;
   return line_records(c, k, true, line_base, INT64_MAX, &n_lines, stream, [&](const HostSide& S, unsigned long long total, cudaStream_t st) -> int {
-    const uint32_t T = (uint32_t)total, n = (uint32_t)min_lines, nfu = (uint32_t)S.n;
-    size_t slots = 1;                                      // a power of two, at least 2 x the windows (<= lines)
-    while (slots < 2 * (size_t)total) slots <<= 1;
-    const uint32_t mask = (uint32_t)(slots - 1);
-    const size_t table_bytes = (slots + 1) * (sizeof(CloneSlot) + 3 * sizeof(uint32_t));
-    {
-      size_t free_b = 0, total_b = 0;
-      CU(cudaMemGetInfo(&free_b, &total_b));
-      if (table_bytes > free_b) return TSM_E_NOMEM;
-    }
-    const size_t L = (size_t)total, nb = L / XS_TILE + 4;
-    DevBuf d_key, d_slot, d_wflag, d_table, d_plo, d_phi, d_scls, d_dup, d_head, d_ext, d_cidx, d_cover, d_rep, d_size, d_cbase,
-        d_big, d_nbig, d_bsum, d_len, d_cursor, d_member, d_wk, d_fdup;
-    if (!d_key.alloc(8 * L) || !d_slot.alloc(4 * L) || !d_wflag.alloc(L) || !d_table.alloc(sizeof(CloneSlot) * (slots + 1)) ||
-        !d_plo.alloc(4 * (slots + 1)) || !d_phi.alloc(4 * (slots + 1)) || !d_scls.alloc(4 * (slots + 1)) || !d_dup.alloc(4 * L) ||
-        !d_head.alloc(4 * L) || !d_ext.alloc(L) || !d_cidx.alloc(8 * (L + 1)) || !d_cover.alloc(8 * (L + 1)) || !d_rep.alloc(4 * L) ||
-        !d_size.alloc(4 * L) || !d_cbase.alloc(8 * (L + 1)) || !d_big.alloc(4 * L) || !d_nbig.alloc(4) || !d_bsum.alloc(8 * nb) ||
-        !d_len.alloc(4 * L) || !d_fdup.alloc(8 * (size_t)nfu)) {
-      cudaGetLastError();
-      return TSM_E_NOMEM;
-    }
-    CloneSlot* table = d_table.as<CloneSlot>();
-    uint32_t* slot_of = d_slot.as<uint32_t>();
-    const unsigned grid = (unsigned)((L + 255) / 256);
-    CU(cudaEventRecord(c->diff_ev[EV_CLONE_GROUP], st));
-    CU(cudaMemsetAsync(d_table.p, 0, sizeof(CloneSlot) * (slots + 1), st));
-    CU(cudaMemsetAsync(d_plo.p, 0xFF, 4 * (slots + 1), st));
-    CU(cudaMemsetAsync(d_phi.p, 0, 4 * (slots + 1), st));
-    CU(cudaMemsetAsync(d_scls.p, 0xFF, 4 * (slots + 1), st));
-    CU(cudaMemsetAsync(d_size.p, 0, 4 * L, st));
-    CU(cudaMemsetAsync(d_nbig.p, 0, 4, st));
-    k_ngrams<<<grid, 256, 0, st>>>(S.d.line_hash, S.d.line_base, nfu, total, n, d_key.as<unsigned long long>());
-    k_clone_insert<<<grid, 256, 0, st>>>(d_key.as<unsigned long long>(), S.d.line_base, nfu, S.d.line_end, S.d.arena, S.d.off, T, n, table,
-                                         mask, slot_of, d_wflag.as<uint8_t>());
-    k_clone_preds<<<grid, 256, 0, st>>>(table, slot_of, d_wflag.as<uint8_t>(), T, d_plo.as<uint32_t>(), d_phi.as<uint32_t>());
-    k_clone_heads<<<grid, 256, 0, st>>>(table, slot_of, d_plo.as<uint32_t>(), d_phi.as<uint32_t>(), T, d_dup.as<uint32_t>(),
-                                        d_head.as<uint32_t>(), d_ext.as<uint8_t>());
-    xscan(d_head.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), d_cidx.as<unsigned long long>(), st);
-    xscan(d_dup.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), d_cover.as<unsigned long long>(), st);
-    k_clone_classes<<<grid, 256, 0, st>>>(d_head.as<uint32_t>(), d_cidx.as<unsigned long long>(), slot_of, table, T, d_rep.as<uint32_t>(),
-                                          d_size.as<uint32_t>(), d_scls.as<uint32_t>(), d_big.as<uint32_t>(), d_nbig.as<uint32_t>());
-    xscan(d_size.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), d_cbase.as<unsigned long long>(), st);
-    k_clone_length<<<(unsigned)c->sms * 8, 256, 0, st>>>(d_rep.as<uint32_t>(), d_ext.as<uint8_t>(), T, n, d_cidx.as<unsigned long long>() + L,
-                                                         d_len.as<uint32_t>());
-    CU(cudaGetLastError());
-    CU(cudaEventRecord(c->diff_ev[EV_CLONE_MEMBERS], st));
-    unsigned long long* pin = c->h_rb->u64;                 // classes, fragments, large classes
-    CU(cudaMemcpyAsync(pin, d_cidx.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(pin + 1, d_cbase.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(pin + 2, d_nbig.p, 4, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    c->launches += 15;                                     // k_ngrams, insert, preds, heads, 3 x xscan (3 each), classes, length
-    const uint32_t nc = (uint32_t)pin[0], nbig = (uint32_t)(pin[2] & 0xFFFFFFFFu);
-    const unsigned long long nm = pin[1];
-    out->n_classes = (int64_t)nc;
-    out->n_members = (int64_t)nm;
-    ms[1] = elapsed_ms(c->diff_ev[EV_CLONE_GROUP], c->diff_ev[EV_CLONE_MEMBERS]);
-    if ((out->class_cap < (int64_t)nc && (out->class_base || out->class_len)) || (out->member_cap < (int64_t)nm && out->member))
-      return TSM_E_CAPACITY;
-    if (nc) {
-      if (!d_cursor.alloc(4 * (size_t)nc) || !d_member.alloc(8 * nm) || !d_wk.alloc(4 * nm)) { cudaGetLastError(); return TSM_E_NOMEM; }
-      unsigned long long* member = d_member.as<unsigned long long>();
-      CU(cudaMemsetAsync(d_cursor.p, 0, 4 * (size_t)nc, st));
-      k_clone_scatter<<<grid, 256, 0, st>>>(slot_of, d_scls.as<uint32_t>(), d_cbase.as<unsigned long long>(), T, d_cursor.as<uint32_t>(), member);
-      k_clone_sort_warp<<<(unsigned)(((size_t)nc * 32 + 255) / 256), 256, 0, st>>>(d_cbase.as<unsigned long long>(), nc, member);
-      c->launches += 2;
-      if (nbig) {
-        k_clone_sort_cta<<<std::min<unsigned>(nbig, (unsigned)c->sms * 2), SIM_SORT_THREADS, SIM_SORT_SMEM, st>>>(
-            d_cbase.as<unsigned long long>(), d_big.as<uint32_t>(), d_nbig.as<uint32_t>(), member, d_wk.as<uint32_t>());
-        c->launches += 1;
-      }
-      uint32_t* fdup = d_fdup.as<uint32_t>();
-      k_clone_cover<<<(unsigned)(((size_t)nfu * 32 + 255) / 256), 256, 0, st>>>(S.d.line_base, nfu, d_cover.as<unsigned long long>(),
-                                                                              S.d.line_flag, n, fdup, fdup + nfu);
-      c->launches += 1;
-      CU(cudaGetLastError());
-      CU(cudaEventRecord(c->diff_ev[EV_CLONE_END], st));
-      if (out->file_dup) CU(cudaMemcpyAsync(out->file_dup, fdup, 4 * (size_t)nfu, cudaMemcpyDeviceToHost, st));
-      if (out->file_dup_assert) CU(cudaMemcpyAsync(out->file_dup_assert, fdup + nfu, 4 * (size_t)nfu, cudaMemcpyDeviceToHost, st));
-      if (out->class_base) CU(cudaMemcpyAsync(out->class_base, d_cbase.p, 8 * ((size_t)nc + 1), cudaMemcpyDeviceToHost, st));
-      if (out->class_len) CU(cudaMemcpyAsync(out->class_len, d_len.p, 4 * (size_t)nc, cudaMemcpyDeviceToHost, st));
-      if (out->member) CU(cudaMemcpyAsync(out->member, member, 8 * nm, cudaMemcpyDeviceToHost, st));
-      CU(cudaStreamSynchronize(st));
-      ms[2] = elapsed_ms(c->diff_ev[EV_CLONE_MEMBERS], c->diff_ev[EV_CLONE_END]);
-    }
-    return TSM_OK;
+    return clone_classes<true>(c, S.d.line_hash, S.d.line_base, (uint32_t)S.n, (uint32_t)total, S.d.line_flag, S.d.line_end, S.d.arena,
+                               S.d.off, (uint32_t)min_lines, out, ms + 1, st);
   }, &ms[0]);
 }
 
 extern "C" int tsm_clones_last_ms(tsm_ctx* c, float* ms3) { return copy_ms(c, MS_CLONE, ms3, 3); }
+
+// ------------------------------------------------------------------------------------- SPEC section 21 blind clones
+// The line records of the corpus (line_records), the lexer of tsm_blind_kernels.cuh (line states, blind hashes, compaction of
+// the kept lines), one synchronisation that reads the kept count, then clone_classes over the kept lines.  A short kept_cap
+// still runs the grouping, so that every count is set when the call returns TSM_E_CAPACITY.
+extern "C" int tsm_clones_blind(tsm_ctx* c, const tsm_corpus* k, int32_t min_lines, tsm_blind_result* blind, tsm_clone_result* out,
+                                void* stream) {
+  if (!c || !k || !out || k->n_files < 0 || min_lines < 1 || min_lines > 1024 || out->class_cap < 0 || out->member_cap < 0 ||
+      (blind && blind->kept_cap < 0))
+    return TSM_E_ARG;
+  const int32_t nf = k->n_files;
+  float* const ms = clear_ms(c, MS_BLIND);
+  c->launches = 0;
+  out->n_classes = out->n_members = 0;
+  if (out->class_base) out->class_base[0] = 0;
+  if (out->file_dup) memset(out->file_dup, 0, sizeof(uint32_t) * (size_t)nf);
+  if (out->file_dup_assert) memset(out->file_dup_assert, 0, sizeof(uint32_t) * (size_t)nf);
+  tsm_blind_result none{nullptr, nullptr, nullptr, nullptr, 0, 0};
+  tsm_blind_result* const b = blind ? blind : &none;
+  b->n_kept = 0;
+  if (b->kept_base) memset(b->kept_base, 0, sizeof(int64_t) * ((size_t)nf + 1));
+  if (b->file_kept_assert) memset(b->file_kept_assert, 0, sizeof(uint32_t) * (size_t)nf);
+  std::vector<int64_t> own_base;
+  int64_t* line_base = out->line_base;
+  if (!line_base) { own_base.resize((size_t)nf + 1); line_base = own_base.data(); }
+  int64_t n_lines = 0;
+  return line_records(c, k, true, line_base, INT64_MAX, &n_lines, stream, [&](const HostSide& S, unsigned long long total, cudaStream_t st) -> int {
+    const uint32_t T = (uint32_t)total, nfu = (uint32_t)S.n;
+    const size_t L = (size_t)total;
+    DevBuf d_state, d_hash, d_kept, d_rank, d_bsum, d_kline, d_khash, d_kflag, d_kbase, d_kassert;
+    if (!d_state.alloc(L) || !d_hash.alloc(8 * L) || !d_kept.alloc(4 * L) || !d_rank.alloc(8 * (L + 1)) || !d_bsum.alloc(8 * (L / XS_TILE + 4)) ||
+        !d_kline.alloc(8 * L) || !d_khash.alloc(8 * L) || !d_kflag.alloc(L) || !d_kbase.alloc(8 * ((size_t)nfu + 1)) ||
+        !d_kassert.alloc(4 * (size_t)nfu)) {
+      cudaGetLastError();
+      return TSM_E_NOMEM;
+    }
+    const unsigned grid = (unsigned)((L + 255) / 256), fgrid = (unsigned)(((size_t)nfu * 32 + 255) / 256);
+    unsigned long long* rank = d_rank.as<unsigned long long>();
+    CU(cudaEventRecord(c->diff_ev[EV_BLIND_LEX], st));
+    k_blind_state<<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>());
+    k_blind_scan<<<fgrid, 256, 0, st>>>(S.d.line_base, nfu, d_state.as<uint8_t>());
+    k_blind_lines<<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>(), d_hash.as<unsigned long long>(), d_kept.as<uint32_t>());
+    xscan(d_kept.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), rank, st);
+    k_blind_compact<<<grid, 256, 0, st>>>(d_kept.as<uint32_t>(), rank, d_hash.as<unsigned long long>(), S.d.line_flag, total,
+                                          d_kline.as<unsigned long long>(), d_khash.as<unsigned long long>(), d_kflag.as<uint8_t>());
+    k_blind_files<<<(unsigned)(((size_t)nfu * 32 + 32 + 255) / 256), 256, 0, st>>>(S.d.line_base, nfu, rank, d_kflag.as<uint8_t>(),
+                                                                                    d_kbase.as<unsigned long long>(), d_kassert.as<uint32_t>());
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_BLIND_LEX_END], st));
+    c->launches += 8;                                      // state, scan, lines, xscan (3), compact, files
+    unsigned long long* pin = c->h_rb->u64;
+    CU(cudaMemcpyAsync(pin + 3, rank + L, 8, cudaMemcpyDeviceToHost, st));
+    if (b->kept_base) CU(cudaMemcpyAsync(b->kept_base, d_kbase.p, 8 * ((size_t)nfu + 1), cudaMemcpyDeviceToHost, st));
+    if (b->file_kept_assert) CU(cudaMemcpyAsync(b->file_kept_assert, d_kassert.p, 4 * (size_t)nfu, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const unsigned long long nk = pin[3];
+    b->n_kept = (int64_t)nk;
+    ms[1] = elapsed_ms(c->diff_ev[EV_BLIND_LEX], c->diff_ev[EV_BLIND_LEX_END]);
+    const bool kept_short = b->kept_cap < (int64_t)nk && (b->kept_line || b->blind_hash);
+    if (!kept_short) {
+      if (b->kept_line) CU(cudaMemcpyAsync(b->kept_line, d_kline.p, 8 * nk, cudaMemcpyDeviceToHost, st));
+      if (b->blind_hash) CU(cudaMemcpyAsync(b->blind_hash, d_khash.p, 8 * nk, cudaMemcpyDeviceToHost, st));
+    }
+    int rc = TSM_OK;
+    if (nk) rc = clone_classes<false>(c, d_khash.as<unsigned long long>(), d_kbase.as<unsigned long long>(), nfu, (uint32_t)nk,
+                                      d_kflag.as<uint8_t>(), nullptr, nullptr, nullptr, (uint32_t)min_lines, out, ms + 2, st);
+    CU(cudaStreamSynchronize(st));
+    return rc == TSM_OK && kept_short ? TSM_E_CAPACITY : rc;
+  }, &ms[0]);
+}
+
+extern "C" int tsm_clones_blind_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_BLIND, ms4, 4); }
 
 // ------------------------------------------------------------------------------------- SPEC section 18 test smells
 // The smell stage over one side whose line records (with header events) and case spans exist: the section-10 kinds

@@ -40,6 +40,9 @@ __device__ __forceinline__ bool line_empty(const uint8_t* file, const uint32_t* 
   return end == start || (end == start + 1 && file[start] == 0x0D);
 }
 
+// SKIP_EMPTY: a window of n empty lines is no window (read from arena, off and line_end).  The blind clones
+// (tsm_blind_kernels.cuh) group compacted kept lines, none of them empty, and pass no bytes.
+template <bool SKIP_EMPTY>
 __global__ void __launch_bounds__(256) k_clone_insert(const unsigned long long* key, const unsigned long long* line_base, uint32_t n_files,
                                                       const uint32_t* line_end, const uint8_t* arena, const int32_t* off, uint32_t total,
                                                       uint32_t n, CloneSlot* table, uint32_t mask, uint32_t* slot_of, uint8_t* wflag) {
@@ -50,9 +53,11 @@ __global__ void __launch_bounds__(256) k_clone_insert(const unsigned long long* 
   const unsigned long long b = line_base[lo], e = line_base[lo + 1];
   uint32_t s = CLONE_NONE;
   if ((unsigned long long)p + n <= e) {
-    const uint8_t* file = arena + off[lo];
-    bool empty = true;
-    for (uint32_t k = 0; k < n && empty; ++k) empty = line_empty(file, line_end, b, (unsigned long long)p + k);
+    bool empty = SKIP_EMPTY;
+    if (SKIP_EMPTY) {
+      const uint8_t* file = arena + off[lo];
+      for (uint32_t k = 0; k < n && empty; ++k) empty = line_empty(file, line_end, b, (unsigned long long)p + k);
+    }
     if (!empty) {
       const unsigned long long k = key[p];
       if (k == 0) s = mask + 1;

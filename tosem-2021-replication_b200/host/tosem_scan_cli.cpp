@@ -24,7 +24,7 @@
 //   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F] [--cases F]
 //                      [--assert-edits F] [--smells F] [--moves F] [--find-renames N] [--batch-bytes N]
 //   tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]
-//   tosem-scan clones <project-root>... | --git <repository> [--rev R]   [--min-lines N] [--all-files] [--out F]
+//   tosem-scan clones <project-root>... | --git <repository> [--rev R]   [--min-lines N] [--blind] [--all-files] [--out F]
 // Every command that scans files does it with scan_batches: batches of at most --batch-bytes of arena (clones: all files in one),
 // one context, the next batch read while the current one is scanned.  Every command that diffs revision pairs (diff, history,
 // blame) does it with pair_batches: batches of at most --batch-bytes per side (with --moves: whole steps), one context shared
@@ -2091,9 +2091,10 @@ static std::string repo_name(const std::string& path) {
 
 // One tsm_clones call over every selected file (classes cross roots and batches), plus one tsm_scan for the per-file line and
 // assertion-line totals.  stdout: one row per root and an <all> row; --out: one row per fragment, classes numbered from 1 in
-// SPEC order, lines 1-based.
+// SPEC order, lines 1-based.  --blind: one tsm_clones_blind call instead (docs/SPEC.md section 21); lines and assertion lines
+// count kept lines, and a fragment's first / last line are those of its first and last kept line.
 static int cmd_clones(const std::vector<std::string>& roots, const std::string& git_repo, const std::string& rev, int min_lines,
-                      bool all_files, const std::string& out_path) {
+                      bool blind, bool all_files, const std::string& out_path) {
   std::vector<FileEntry> files;
   std::vector<std::string> names;
   if (!git_repo.empty()) {
@@ -2121,16 +2122,26 @@ static int cmd_clones(const std::vector<std::string>& roots, const std::string& 
   scan_batches(files, batches, 0, (int32_t)ng, 0, [&](const Batch& B, const Scanned& s) {
     const int32_t nf = (int32_t)B.count();
     const tsm_corpus c = B.corpus((int32_t)ng);
-    std::vector<int64_t> base((size_t)nf + 1), cbase(1), member(1);
-    std::vector<uint32_t> dup((size_t)nf), dupa((size_t)nf), clen(1);
+    std::vector<int64_t> base((size_t)nf + 1), cbase(1), member(1), kbase((size_t)nf + 1), kline(1);
+    std::vector<uint32_t> dup((size_t)nf), dupa((size_t)nf), clen(1), kassert((size_t)nf);
     tsm_clone_result r{base.data(), dup.data(), dupa.data(), nullptr, nullptr, 0, 0, nullptr, 0, 0};
-    ck(tsm_clones(s.ctx, &c, min_lines, &r, nullptr), "tsm_clones");   // the counts; the second call fills arrays of that size
+    tsm_blind_result kr{kbase.data(), nullptr, nullptr, kassert.data(), 0, 0};
+    auto call = [&] {
+      if (blind) ck(tsm_clones_blind(s.ctx, &c, min_lines, &kr, &r, nullptr), "tsm_clones_blind");
+      else ck(tsm_clones(s.ctx, &c, min_lines, &r, nullptr), "tsm_clones");
+    };
+    call();                                                // the counts; the second call fills arrays of that size
     cbase.resize((size_t)r.n_classes + 1); clen.resize((size_t)std::max<int64_t>(r.n_classes, 1)); member.resize((size_t)std::max<int64_t>(r.n_members, 1));
     r.class_base = cbase.data(); r.class_len = clen.data(); r.class_cap = r.n_classes; r.member = member.data(); r.member_cap = r.n_members;
-    ck(tsm_clones(s.ctx, &c, min_lines, &r, nullptr), "tsm_clones");
+    kline.resize((size_t)std::max<int64_t>(kr.n_kept, 1));
+    kr.kept_line = kline.data(); kr.kept_cap = kr.n_kept;
+    call();
+    const std::vector<int64_t>& fbase = blind ? kbase : base;   // the numbering of member
     for (int32_t i = 0; i < nf; ++i) {
       const size_t g = (size_t)files[B.idx[(size_t)i]].grp;
-      const int64_t v[5] = {1, (int64_t)s.stats[(size_t)i].n_lines, dup[(size_t)i], (int64_t)s.stats[(size_t)i].n_assert, dupa[(size_t)i]};
+      const int64_t lines = blind ? kbase[(size_t)i + 1] - kbase[(size_t)i] : (int64_t)s.stats[(size_t)i].n_lines;
+      const int64_t asserts = blind ? (int64_t)kassert[(size_t)i] : (int64_t)s.stats[(size_t)i].n_assert;
+      const int64_t v[5] = {1, lines, dup[(size_t)i], asserts, dupa[(size_t)i]};
       for (int k = 0; k < 5; ++k) { tot[g][(size_t)k] += v[k]; tot[ng][(size_t)k] += v[k]; }
     }
     tot[ng][5] = r.n_classes;
@@ -2138,12 +2149,13 @@ static int cmd_clones(const std::vector<std::string>& roots, const std::string& 
     for (int64_t k = 0; k < r.n_classes; ++k)
       for (int64_t j = cbase[(size_t)k]; j < cbase[(size_t)k + 1]; ++j) {
         const int64_t at = member[(size_t)j];
-        const size_t f = (size_t)(std::upper_bound(base.begin(), base.end(), at) - base.begin() - 1);
+        const size_t f = (size_t)(std::upper_bound(fbase.begin(), fbase.end(), at) - fbase.begin() - 1);
         const FileEntry& fe = files[B.idx[f]];
         if (seen[(size_t)fe.grp] != k) { seen[(size_t)fe.grp] = k; tot[(size_t)fe.grp][5]++; }
         if (os.is_open()) {
-          const int64_t first = at - base[f] + 1;
-          csv_row(os, {std::to_string(k + 1), names[(size_t)fe.grp], fe.rel, std::to_string(first), std::to_string(first + clen[(size_t)k] - 1)});
+          const int64_t last = at + clen[(size_t)k] - 1;
+          const int64_t first = (blind ? kline[(size_t)at] : at) - base[f] + 1, end = (blind ? kline[(size_t)last] : last) - base[f] + 1;
+          csv_row(os, {std::to_string(k + 1), names[(size_t)fe.grp], fe.rel, std::to_string(first), std::to_string(end)});
         }
       }
   });
@@ -2253,11 +2265,13 @@ static void usage() {
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
           "                          [--cases F] [--assert-edits F] [--smells F] [--moves F] [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
-          "       tosem-scan clones <project-root>... [--min-lines N] [--all-files] [--out F]\n"
-          "       tosem-scan clones --git <repository> [--rev R] [--min-lines N] [--all-files] [--out F]\n"
+          "       tosem-scan clones <project-root>... [--min-lines N] [--blind] [--all-files] [--out F]\n"
+          "       tosem-scan clones --git <repository> [--rev R] [--min-lines N] [--blind] [--all-files] [--out F]\n"
           "       tosem-scan smells <project-root>... [--all-files] [--batch-bytes N] [--out F]\n"
           "       tosem-scan smells --git <repository> [--rev R] [--all-files] [--batch-bytes N] [--out F]\n"
           "smells: per root the tests with each of nine test smells; --out F: one row per instance line (docs/SPEC.md section 18).\n"
+          "--blind (clones): near-miss copies - lines compared with identifiers, literals, whitespace and comments blinded, over the\n"
+          "                  lines that keep a token (docs/SPEC.md section 21).\n"
           "--find-renames N (0..100): pair deleted and added files at least N %% similar, as git -M<N>%% does (docs/SPEC.md section 13).\n"
           "--cases F: one row per test case that a revision adds (A), deletes (D) or modifies (M) (docs/SPEC.md section 16).\n"
           "--assert-edits F: one row per deleted assertion line that an inserted one of the same hunk replaces, with their similarity\n"
@@ -2276,12 +2290,13 @@ int main(int argc, char** argv) {
   const std::string cmd = argv[1];
   std::vector<std::string> pos;
   std::map<std::string, std::string> opt;
-  bool all_files = false, rev_b = false, dry_run = false;
+  bool all_files = false, rev_b = false, dry_run = false, blind = false;
   for (int i = 2; i < argc; ++i) {
     const std::string a = argv[i];
     if (a == "--all-files") all_files = true;
     else if (a == "--rev-b") rev_b = true;
     else if (a == "--dry-run") dry_run = true;
+    else if (a == "--blind") blind = true;
     else if (a.rfind("--", 0) == 0) { if (i + 1 >= argc) die("missing value for " + a); opt[a] = argv[++i]; }
     else pos.push_back(a);
   }
@@ -2296,7 +2311,7 @@ int main(int argc, char** argv) {
     if (pos.empty() == !opt.count("--git")) die("clones needs project roots or --git <repository>, not both");
     const long n = opt.count("--min-lines") ? strtol(opt["--min-lines"].c_str(), nullptr, 10) : 5;
     if (n < 1 || n > 1024) die("--min-lines needs a number of lines from 1 to 1024");
-    return cmd_clones(pos, opt["--git"], opt.count("--rev") ? opt["--rev"] : "HEAD", (int)n, all_files, opt["--out"]);
+    return cmd_clones(pos, opt["--git"], opt.count("--rev") ? opt["--rev"] : "HEAD", (int)n, blind, all_files, opt["--out"]);
   }
   if (cmd == "smells") {
     if (pos.empty() == !opt.count("--git")) die("smells needs project roots or --git <repository>, not both");

@@ -49,7 +49,8 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_gen_fill", "tsm_gen_edit", "tsm_gen_pair_sizes", "tsm_gen_pair_fill", "tsm_similarity", "tsm_similarity_last_ms",
            "tsm_diff_pairs_marks", "tsm_blame_pairs", "tsm_blame_last_ms", "tsm_clones", "tsm_clones_last_ms",
            "tsm_diff_pairs_cases", "tsm_diff_pairs_assert_edits", "tsm_assert_edits_last_ms", "tsm_smells", "tsm_smells_last_ms",
-           "tsm_diff_pairs_smells", "tsm_diff_smells_last_ms", "tsm_diff_pairs_moves", "tsm_moves_last_ms"]
+           "tsm_diff_pairs_smells", "tsm_diff_smells_last_ms", "tsm_diff_pairs_moves", "tsm_moves_last_ms", "tsm_clones_blind",
+           "tsm_clones_blind_last_ms"]
 
 
 class TsmError(RuntimeError):
@@ -103,6 +104,11 @@ class _CloneResult(C.Structure):
     _fields_ = [("line_base", C.c_void_p), ("file_dup", C.c_void_p), ("file_dup_assert", C.c_void_p),
                 ("class_base", C.c_void_p), ("class_len", C.c_void_p), ("class_cap", C.c_int64), ("n_classes", C.c_int64),
                 ("member", C.c_void_p), ("member_cap", C.c_int64), ("n_members", C.c_int64)]
+
+
+class _BlindResult(C.Structure):
+    _fields_ = [("kept_base", C.c_void_p), ("kept_line", C.c_void_p), ("blind_hash", C.c_void_p), ("file_kept_assert", C.c_void_p),
+                ("kept_cap", C.c_int64), ("n_kept", C.c_int64)]
 
 
 _lib = None
@@ -207,6 +213,11 @@ def lib():
         L.tsm_clones.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_int32, C.POINTER(_CloneResult), C.c_void_p]
         L.tsm_clones_last_ms.restype = C.c_int
         L.tsm_clones_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 3)]
+        L.tsm_clones_blind.restype = C.c_int
+        L.tsm_clones_blind.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_int32, C.POINTER(_BlindResult), C.POINTER(_CloneResult),
+                                       C.c_void_p]
+        L.tsm_clones_blind_last_ms.restype = C.c_int
+        L.tsm_clones_blind_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
         L.tsm_smells.restype = C.c_int
         L.tsm_smells.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
                                  C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p]
@@ -828,31 +839,47 @@ class Scanner:
         lib().tsm_similarity_last_ms(self._ctx, C.byref(ms))
         return [float(x) for x in ms]
 
-    def clones(self, corpus, min_lines=5, stream=None, cap=None):
+    def clones(self, corpus, min_lines=5, blind=False, stream=None, cap=None):
         """Duplicated test code (docs/SPEC.md section 15): a dict of numpy arrays line_base[n_files+1], file_dup[n_files],
         file_dup_assert[n_files], class_base[n_classes+1], class_len[n_classes] and member[n_members] (the global first line of
         every fragment; class c is member[class_base[c]:class_base[c+1]], each fragment class_len[c] lines).  Arrays too small
-        for the classes or fragments are sized from the counts and the call is made again (cap: the first guess of both)."""
+        for the classes or fragments are sized from the counts and the call is made again (cap: the first guess of both).
+        blind=True: the near-miss clones of section 21 (tsm_clones_blind) over the kept lines, member, class_len, file_dup and
+        file_dup_assert in kept lines, plus kept_base[n_files+1], kept_line[n_kept] (the global line of every kept line),
+        blind_hash[n_kept] and file_kept_assert[n_files]."""
         n = corpus.n_files
         cs = corpus.c_struct()
-        cc = cm = int(cap if cap is not None else 0)
+        cc = cm = ck = int(cap if cap is not None else 0)
+        what = "tsm_clones_blind" if blind else "tsm_clones"
         for _ in range(2):
             out = {"line_base": np.zeros(n + 1, np.int64), "file_dup": np.zeros(n, np.uint32), "file_dup_assert": np.zeros(n, np.uint32),
                    "class_base": np.zeros(cc + 1, np.int64), "class_len": np.zeros(max(cc, 1), np.uint32),
                    "member": np.zeros(max(cm, 1), np.int64)}
             r = _CloneResult(*[_p(out[k]) for k in ("line_base", "file_dup", "file_dup_assert", "class_base", "class_len")], cc, 0,
                              _p(out["member"]), cm, 0)
-            rc = lib().tsm_clones(self._ctx, C.byref(cs), int(min_lines), C.byref(r), stream)
-            if rc == TSM_E_CAPACITY and (r.n_classes > cc or r.n_members > cm):
+            if blind:
+                out.update(kept_base=np.zeros(n + 1, np.int64), kept_line=np.zeros(max(ck, 1), np.int64),
+                           blind_hash=np.zeros(max(ck, 1), np.uint64), file_kept_assert=np.zeros(n, np.uint32))
+                b = _BlindResult(*[_p(out[k]) for k in ("kept_base", "kept_line", "blind_hash", "file_kept_assert")], ck, 0)
+                rc = lib().tsm_clones_blind(self._ctx, C.byref(cs), int(min_lines), C.byref(b), C.byref(r), stream)
+                short_kept = b.n_kept > ck
+            else:
+                rc = lib().tsm_clones(self._ctx, C.byref(cs), int(min_lines), C.byref(r), stream)
+                short_kept = False
+            if rc == TSM_E_CAPACITY and (r.n_classes > cc or r.n_members > cm or short_kept):
                 cc, cm = int(r.n_classes), int(r.n_members)
+                if blind:
+                    ck = int(b.n_kept)
                 continue
             if rc:
-                raise TsmError(rc, "tsm_clones")
+                raise TsmError(rc, what)
             out["class_base"] = out["class_base"][:r.n_classes + 1]
             out["class_len"] = out["class_len"][:r.n_classes]
             out["member"] = out["member"][:r.n_members]
+            if blind:
+                out["kept_line"], out["blind_hash"] = out["kept_line"][:b.n_kept], out["blind_hash"][:b.n_kept]
             return out
-        raise TsmError(TSM_E_CAPACITY, "tsm_clones")
+        raise TsmError(TSM_E_CAPACITY, what)
 
     def smells(self, corpus, stream=None, cap=None):
         """Test smells (docs/SPEC.md section 18): a dict of numpy arrays line_base[n_files+1], line_smell[n_lines] (the smell bits
@@ -952,4 +979,11 @@ class Scanner:
         """Device time of the last clones call: [k_scan, grouping + classes, members + coverage] in ms."""
         ms = (C.c_float * 3)()
         lib().tsm_clones_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
+
+    def clones_blind_last_ms(self):
+        """Device time of the last clones call with blind=True: [k_scan, lexing + compaction, grouping + classes, members +
+        coverage] in ms."""
+        ms = (C.c_float * 4)()
+        lib().tsm_clones_blind_last_ms(self._ctx, C.byref(ms))
         return [float(x) for x in ms]
