@@ -328,6 +328,43 @@ int tsm_clones_blind(tsm_ctx* ctx, const tsm_corpus* corpus, int32_t min_lines, 
                      void* stream);
 int tsm_clones_blind_last_ms(tsm_ctx* ctx, float* ms4);
 
+/* Clone churn along a revision history (docs/SPEC.md section 22): which fragments of the clone classes of two revisions a step
+ * edits.  old_rev / new_rev are the two revisions (n_files = 0 is legal); pair k pairs file pair_old[k] of old_rev with file
+ * pair_new[k] of new_rev, either -1 for none (a deletion or an addition).  A file in no pair is unchanged.  The pairs' edit
+ * marks are those of tsm_diff_pairs_marks.  Per side (old_side: old_rev, new_side: new_rev):
+ *   clones, blind    what tsm_clones (blind = 0) or tsm_clones_blind (blind != 0; `blind` is read only then) gives for that
+ *                    revision alone at min_lines, with the same pointer and capacity rules
+ *   changed          [member_cap] per fragment, its marked units (lines, or kept lines with blind): deleted lines on the old
+ *                    side, inserted lines on the new side; changed_assert those of them that are assertion lines
+ *   state            [member_cap] TSM_FRAG_KEPT (changed = 0), TSM_FRAG_WHOLE (changed = class_len) or TSM_FRAG_EDITED
+ *   class_counts     [class_cap][3] per class its kept, edited and whole fragments
+ *   status           [class_cap] TSM_CLONE_UNTOUCHED when every fragment is kept, else the first rule that holds:
+ *                    old side  REMOVED (every fragment whole), DIVERGED (a kept and an edited one), DROPPED (a kept one), CHANGED
+ *                    new side  CREATED (every fragment whole), COPIED (a kept and a whole one), JOINED (a kept one), CHANGED
+ * Any output pointer may be NULL (it is skipped); the counts of both sides are always set.  A short class_cap, member_cap or
+ * kept_cap (for a given output sized by it) returns TSM_E_CAPACITY with all counts set: size the arrays and call again.
+ * TSM_E_ARG for min_lines outside 1..1024, a file index out of range, a file in two pairs of one side or a pair (-1, -1);
+ * n_pairs = 0 is legal (nothing is touched).  Memory errors as for tsm_clones.
+ * Kernels: k_scan over both revisions; per pair side a view of its revision's line records (k_churn_gather) and the diff of
+ * tsm_diff_pairs_marks over the views; k_churn_marks onto the revision lines; per revision the kernels of tsm_clones (or
+ * tsm_clones_blind), then k_churn_units, two exclusive scans, k_churn_frags and k_churn_classes
+ * (csrc/tsm_clone_churn_kernels.cuh).
+ * tsm_clone_churn_last_ms: device time of the last call, ms4 = { k_scan over both revisions, classes of both (lexing included),
+ * k_churn_gather + the marks diff, k_churn_marks + the churn kernels of both sides }. */
+enum { TSM_FRAG_KEPT = 0, TSM_FRAG_EDITED = 1, TSM_FRAG_WHOLE = 2 };
+enum { TSM_CLONE_UNTOUCHED = 0, TSM_CLONE_CHANGED = 1, TSM_CLONE_REMOVED = 2, TSM_CLONE_DIVERGED = 3, TSM_CLONE_DROPPED = 4,
+       TSM_CLONE_CREATED = 5, TSM_CLONE_COPIED = 6, TSM_CLONE_JOINED = 7 };
+typedef struct tsm_clone_churn_side {
+  tsm_clone_result clones;
+  tsm_blind_result blind;
+  uint32_t* changed; uint32_t* changed_assert; uint8_t* state;   /* [clones.member_cap] */
+  uint32_t* class_counts; uint8_t* status;                       /* [clones.class_cap][3], [clones.class_cap] */
+} tsm_clone_churn_side;
+int tsm_clone_churn(tsm_ctx* ctx, const tsm_corpus* old_rev, const tsm_corpus* new_rev, const int32_t* pair_old,
+                    const int32_t* pair_new, int64_t n_pairs, int32_t min_lines, int32_t blind, tsm_clone_churn_side* old_side,
+                    tsm_clone_churn_side* new_side, void* stream);
+int tsm_clone_churn_last_ms(tsm_ctx* ctx, float* ms4);
+
 /* Test smells (docs/SPEC.md section 18, `tosem-scan smells`): the tests of every file (section-16 cases whose header opens a test
  * by the rule of its family), their bodies and the nine smells below, as one record per test in global line order (files in
  * order, then header line) and the smell bits of every line (its instances; 0 outside test bodies).  Bit k of `smells` and of

@@ -26,6 +26,7 @@
 #include "tsm_edit_kernels.cuh"
 #include "tsm_smell_kernels.cuh"
 #include "tsm_move_kernels.cuh"
+#include "tsm_clone_churn_kernels.cuh"
 
 using namespace tsm;
 
@@ -88,6 +89,7 @@ enum Timed {
   MS_EDIT,    // k_scan, the diff, compact to pairing (host clock) of the last tsm_diff_pairs_assert_edits
   MS_MOVE,    // k_scan, the diff, line flags to k_move_reach, k_move_starts to k_move_mark of the last tsm_diff_pairs_moves
   MS_BLAME,   // k_blame of the last tsm_blame_pairs
+  MS_CCHURN,  // k_scan of both revisions, classes of both, the marks diff, the churn kernels of the last tsm_clone_churn
   N_TIMED
 };
 
@@ -169,6 +171,8 @@ struct tsm_ctx {
 //     case records + churn, behind diff    CHURN_CASES                                                     at the end
 //   tsm_diff_pairs_moves, behind the diff  MOVE_FLAGS      MOVE_JOIN       MOVE_RUNS       MOVE_MARK       at the end
 //   tsm_blame_pairs, behind the diff       BLAME                                                           at the end
+//   tsm_clone_churn: gather, behind scans  CCHURN                                                          behind the diff
+//     marks, then per side behind classes  CCHURN                                                          at each end
 //   (* recorded by smell_stage, and not read in this call)
 struct EvSpan { int from, to; };
 constexpr EvSpan EV_SCAN[2] = {{0, 1}, {6, 7}}, EV_SMALL = {2, 3}, EV_LEFT = {4, 5};
@@ -179,6 +183,7 @@ constexpr int EV_SMELL_KINDS = 2, EV_SMELL_LINES = 3, EV_SMELL_TESTS = 4, EV_SME
 constexpr EvSpan EV_CHURN_SMELLS = {0, 1}, EV_CHURN_CASES = {0, 1};   // the old side's scan slots, then the same again
 constexpr EvSpan EV_MOVE_FLAGS = {0, 1}, EV_MOVE_JOIN = {2, 3}, EV_MOVE_RUNS = {4, 5}, EV_MOVE_MARK = {6, 7};
 constexpr EvSpan EV_BLAME = {0, 1};
+constexpr EvSpan EV_CCHURN = {0, 1};
 
 // The start of every call that queues device work on st: the ctx's device, the ctx's pool for the call's DevBufs, and the
 // order of the ctx's calls.  A ctx orders its own work, whatever stream each call is given: the call's stream first waits
@@ -1932,11 +1937,22 @@ extern "C" int tsm_statements(tsm_ctx* c, const tsm_corpus* k, int64_t* line_bas
 // device; with SKIP_EMPTY the window test reads the lines' bytes (arena, off, line_end).  The kernels of tsm_clone_kernels.cuh,
 // with one synchronisation between the grouping and the members that reads the class and fragment counts: a short cap returns
 // there, else the fragments are scattered, sorted and copied back with the coverage.  ms[0] / ms[1]: grouping + classes, members
-// + coverage.
-template <bool SKIP_EMPTY>
+// + coverage.  Then then(dev, st), the caller's use of the classes on the device (CloneDev), before their buffers go back to the
+// pool; it is not called when there is no class.  class_out / member_out: the caller has outputs of its own sized by class_cap /
+// member_cap, which the capacity rule then counts as given.
+struct CloneDev {
+  const unsigned long long* class_base; const uint32_t* class_len; const unsigned long long* member;   // [nc + 1], [nc], [nm]
+  uint32_t nc; unsigned long long nm;
+  uint32_t n_units;                                        // the lines (or kept lines) the classes are numbered in
+  const unsigned long long* unit_line;                     // the line of every unit (blind: kept_line), NULL = unit u is line u
+  const uint8_t* unit_flag;                                // the assertion flag of every unit
+};
+struct NoThen { int operator()(const CloneDev&, cudaStream_t) const { return TSM_OK; } };
+template <bool SKIP_EMPTY, typename Then = NoThen>
 static int clone_classes(tsm_ctx* c, const unsigned long long* hash, const unsigned long long* line_base, uint32_t nfu, uint32_t T,
                          const uint8_t* line_flag, const uint32_t* line_end, const uint8_t* arena, const int32_t* off, uint32_t n,
-                         tsm_clone_result* out, float* ms, cudaStream_t st) {
+                         tsm_clone_result* out, float* ms, cudaStream_t st, Then then = {}, bool class_out = false,
+                         bool member_out = false) {
   size_t slots = 1;                                      // a power of two, at least 2 x the windows (<= lines)
   while (slots < 2 * (size_t)T) slots <<= 1;
   const uint32_t mask = (uint32_t)(slots - 1);
@@ -1993,7 +2009,7 @@ static int clone_classes(tsm_ctx* c, const unsigned long long* hash, const unsig
   out->n_classes = (int64_t)nc;
   out->n_members = (int64_t)nm;
   ms[0] = elapsed_ms(c->diff_ev[EV_CLONE_GROUP], c->diff_ev[EV_CLONE_MEMBERS]);
-  if ((out->class_cap < (int64_t)nc && (out->class_base || out->class_len)) || (out->member_cap < (int64_t)nm && out->member))
+  if ((out->class_cap < (int64_t)nc && (class_out || out->class_base || out->class_len)) || (out->member_cap < (int64_t)nm && (member_out || out->member)))
     return TSM_E_CAPACITY;
   if (nc) {
     if (!d_cursor.alloc(4 * (size_t)nc) || !d_member.alloc(8 * nm) || !d_wk.alloc(4 * nm)) { cudaGetLastError(); return TSM_E_NOMEM; }
@@ -2020,6 +2036,7 @@ static int clone_classes(tsm_ctx* c, const unsigned long long* hash, const unsig
     if (out->member) CU(cudaMemcpyAsync(out->member, member, 8 * nm, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     ms[1] = elapsed_ms(c->diff_ev[EV_CLONE_MEMBERS], c->diff_ev[EV_CLONE_END]);
+    return then(CloneDev{d_cbase.as<unsigned long long>(), d_len.as<uint32_t>(), member, nc, nm, T, nullptr, line_flag}, st);
   }
   return TSM_OK;
 }
@@ -2047,9 +2064,60 @@ extern "C" int tsm_clones(tsm_ctx* c, const tsm_corpus* k, int32_t min_lines, ts
 extern "C" int tsm_clones_last_ms(tsm_ctx* c, float* ms3) { return copy_ms(c, MS_CLONE, ms3, 3); }
 
 // ------------------------------------------------------------------------------------- SPEC section 21 blind clones
-// The line records of the corpus (line_records), the lexer of tsm_blind_kernels.cuh (line states, blind hashes, compaction of
-// the kept lines), one synchronisation that reads the kept count, then clone_classes over the kept lines.  A short kept_cap
-// still runs the grouping, so that every count is set when the call returns TSM_E_CAPACITY.
+// The section-21 front over one side whose line records exist (S, total lines > 0): the lexer of tsm_blind_kernels.cuh (line
+// states, blind hashes, compaction of the kept lines), one synchronisation that reads the kept count, then clone_classes over
+// the kept lines, with then, class_out and member_out as there (CloneDev::unit_line = the kept lines' lines).  A short kept_cap
+// still runs the grouping, so that every count is set when it returns TSM_E_CAPACITY.  ms[0]: lexing + compaction, ms[1] / ms[2]:
+// those of clone_classes.
+template <typename Then = NoThen>
+static int blind_classes(tsm_ctx* c, const HostSide& S, unsigned long long total, uint32_t min_lines, tsm_blind_result* b,
+                         tsm_clone_result* out, float* ms, cudaStream_t st, Then then = {}, bool class_out = false, bool member_out = false) {
+  const uint32_t T = (uint32_t)total, nfu = (uint32_t)S.n;
+  const size_t L = (size_t)total;
+  DevBuf d_state, d_hash, d_kept, d_rank, d_bsum, d_kline, d_khash, d_kflag, d_kbase, d_kassert;
+  if (!d_state.alloc(L) || !d_hash.alloc(8 * L) || !d_kept.alloc(4 * L) || !d_rank.alloc(8 * (L + 1)) || !d_bsum.alloc(8 * (L / XS_TILE + 4)) ||
+      !d_kline.alloc(8 * L) || !d_khash.alloc(8 * L) || !d_kflag.alloc(L) || !d_kbase.alloc(8 * ((size_t)nfu + 1)) ||
+      !d_kassert.alloc(4 * (size_t)nfu)) {
+    cudaGetLastError();
+    return TSM_E_NOMEM;
+  }
+  const unsigned grid = (unsigned)((L + 255) / 256), fgrid = (unsigned)(((size_t)nfu * 32 + 255) / 256);
+  unsigned long long* rank = d_rank.as<unsigned long long>();
+  CU(cudaEventRecord(c->diff_ev[EV_BLIND_LEX], st));
+  k_blind_state<<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>());
+  k_blind_scan<<<fgrid, 256, 0, st>>>(S.d.line_base, nfu, d_state.as<uint8_t>());
+  k_blind_lines<<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>(), d_hash.as<unsigned long long>(), d_kept.as<uint32_t>());
+  xscan(d_kept.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), rank, st);
+  k_blind_compact<<<grid, 256, 0, st>>>(d_kept.as<uint32_t>(), rank, d_hash.as<unsigned long long>(), S.d.line_flag, total,
+                                        d_kline.as<unsigned long long>(), d_khash.as<unsigned long long>(), d_kflag.as<uint8_t>());
+  k_blind_files<<<(unsigned)(((size_t)nfu * 32 + 32 + 255) / 256), 256, 0, st>>>(S.d.line_base, nfu, rank, d_kflag.as<uint8_t>(),
+                                                                                  d_kbase.as<unsigned long long>(), d_kassert.as<uint32_t>());
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(c->diff_ev[EV_BLIND_LEX_END], st));
+  c->launches += 8;                                      // state, scan, lines, xscan (3), compact, files
+  unsigned long long* pin = c->h_rb->u64;
+  CU(cudaMemcpyAsync(pin + 3, rank + L, 8, cudaMemcpyDeviceToHost, st));
+  if (b->kept_base) CU(cudaMemcpyAsync(b->kept_base, d_kbase.p, 8 * ((size_t)nfu + 1), cudaMemcpyDeviceToHost, st));
+  if (b->file_kept_assert) CU(cudaMemcpyAsync(b->file_kept_assert, d_kassert.p, 4 * (size_t)nfu, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const unsigned long long nk = pin[3];
+  b->n_kept = (int64_t)nk;
+  ms[0] = elapsed_ms(c->diff_ev[EV_BLIND_LEX], c->diff_ev[EV_BLIND_LEX_END]);
+  const bool kept_short = b->kept_cap < (int64_t)nk && (b->kept_line || b->blind_hash);
+  if (!kept_short) {
+    if (b->kept_line) CU(cudaMemcpyAsync(b->kept_line, d_kline.p, 8 * nk, cudaMemcpyDeviceToHost, st));
+    if (b->blind_hash) CU(cudaMemcpyAsync(b->blind_hash, d_khash.p, 8 * nk, cudaMemcpyDeviceToHost, st));
+  }
+  int rc = TSM_OK;
+  const unsigned long long* kline = d_kline.as<unsigned long long>();
+  if (nk) rc = clone_classes<false>(c, d_khash.as<unsigned long long>(), d_kbase.as<unsigned long long>(), nfu, (uint32_t)nk,
+                                    d_kflag.as<uint8_t>(), nullptr, nullptr, nullptr, min_lines, out, ms + 1, st,
+                                    [&](CloneDev d, cudaStream_t s2) { d.unit_line = kline; return then(d, s2); }, class_out, member_out);
+  CU(cudaStreamSynchronize(st));
+  return rc == TSM_OK && kept_short ? TSM_E_CAPACITY : rc;
+}
+
+// The line records of the corpus (line_records), then blind_classes over them.
 extern "C" int tsm_clones_blind(tsm_ctx* c, const tsm_corpus* k, int32_t min_lines, tsm_blind_result* blind, tsm_clone_result* out,
                                 void* stream) {
   if (!c || !k || !out || k->n_files < 0 || min_lines < 1 || min_lines > 1024 || out->class_cap < 0 || out->member_cap < 0 ||
@@ -2072,51 +2140,199 @@ extern "C" int tsm_clones_blind(tsm_ctx* c, const tsm_corpus* k, int32_t min_lin
   if (!line_base) { own_base.resize((size_t)nf + 1); line_base = own_base.data(); }
   int64_t n_lines = 0;
   return line_records(c, k, true, line_base, INT64_MAX, &n_lines, stream, [&](const HostSide& S, unsigned long long total, cudaStream_t st) -> int {
-    const uint32_t T = (uint32_t)total, nfu = (uint32_t)S.n;
-    const size_t L = (size_t)total;
-    DevBuf d_state, d_hash, d_kept, d_rank, d_bsum, d_kline, d_khash, d_kflag, d_kbase, d_kassert;
-    if (!d_state.alloc(L) || !d_hash.alloc(8 * L) || !d_kept.alloc(4 * L) || !d_rank.alloc(8 * (L + 1)) || !d_bsum.alloc(8 * (L / XS_TILE + 4)) ||
-        !d_kline.alloc(8 * L) || !d_khash.alloc(8 * L) || !d_kflag.alloc(L) || !d_kbase.alloc(8 * ((size_t)nfu + 1)) ||
-        !d_kassert.alloc(4 * (size_t)nfu)) {
-      cudaGetLastError();
-      return TSM_E_NOMEM;
-    }
-    const unsigned grid = (unsigned)((L + 255) / 256), fgrid = (unsigned)(((size_t)nfu * 32 + 255) / 256);
-    unsigned long long* rank = d_rank.as<unsigned long long>();
-    CU(cudaEventRecord(c->diff_ev[EV_BLIND_LEX], st));
-    k_blind_state<<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>());
-    k_blind_scan<<<fgrid, 256, 0, st>>>(S.d.line_base, nfu, d_state.as<uint8_t>());
-    k_blind_lines<<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>(), d_hash.as<unsigned long long>(), d_kept.as<uint32_t>());
-    xscan(d_kept.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), rank, st);
-    k_blind_compact<<<grid, 256, 0, st>>>(d_kept.as<uint32_t>(), rank, d_hash.as<unsigned long long>(), S.d.line_flag, total,
-                                          d_kline.as<unsigned long long>(), d_khash.as<unsigned long long>(), d_kflag.as<uint8_t>());
-    k_blind_files<<<(unsigned)(((size_t)nfu * 32 + 32 + 255) / 256), 256, 0, st>>>(S.d.line_base, nfu, rank, d_kflag.as<uint8_t>(),
-                                                                                    d_kbase.as<unsigned long long>(), d_kassert.as<uint32_t>());
-    CU(cudaGetLastError());
-    CU(cudaEventRecord(c->diff_ev[EV_BLIND_LEX_END], st));
-    c->launches += 8;                                      // state, scan, lines, xscan (3), compact, files
-    unsigned long long* pin = c->h_rb->u64;
-    CU(cudaMemcpyAsync(pin + 3, rank + L, 8, cudaMemcpyDeviceToHost, st));
-    if (b->kept_base) CU(cudaMemcpyAsync(b->kept_base, d_kbase.p, 8 * ((size_t)nfu + 1), cudaMemcpyDeviceToHost, st));
-    if (b->file_kept_assert) CU(cudaMemcpyAsync(b->file_kept_assert, d_kassert.p, 4 * (size_t)nfu, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    const unsigned long long nk = pin[3];
-    b->n_kept = (int64_t)nk;
-    ms[1] = elapsed_ms(c->diff_ev[EV_BLIND_LEX], c->diff_ev[EV_BLIND_LEX_END]);
-    const bool kept_short = b->kept_cap < (int64_t)nk && (b->kept_line || b->blind_hash);
-    if (!kept_short) {
-      if (b->kept_line) CU(cudaMemcpyAsync(b->kept_line, d_kline.p, 8 * nk, cudaMemcpyDeviceToHost, st));
-      if (b->blind_hash) CU(cudaMemcpyAsync(b->blind_hash, d_khash.p, 8 * nk, cudaMemcpyDeviceToHost, st));
-    }
-    int rc = TSM_OK;
-    if (nk) rc = clone_classes<false>(c, d_khash.as<unsigned long long>(), d_kbase.as<unsigned long long>(), nfu, (uint32_t)nk,
-                                      d_kflag.as<uint8_t>(), nullptr, nullptr, nullptr, (uint32_t)min_lines, out, ms + 2, st);
-    CU(cudaStreamSynchronize(st));
-    return rc == TSM_OK && kept_short ? TSM_E_CAPACITY : rc;
+    return blind_classes(c, S, total, (uint32_t)min_lines, b, out, ms + 1, st);
   }, &ms[0]);
 }
 
 extern "C" int tsm_clones_blind_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_BLIND, ms4, 4); }
+
+// ------------------------------------------------------------------------------------- SPEC section 22 clone churn
+// The edit marks of the pairs, on the lines of both revisions (S[i]: line records with line_base on the host; rmark[i]: one
+// zeroed byte per line).  Each pair side is a view of its revision: its line_base from the files' line counts, its hashes and
+// flags gathered from the revision's records (k_churn_gather), so that diff_core runs over the pairs without a second upload or
+// scan.  k_churn_marks then puts every marked view line onto its revision line.  ms[2] += gather + diff, ms[3] += k_churn_marks.
+static int churn_marks(tsm_ctx* c, HostSide* S, const int32_t* const pf[2], int32_t n, DevBuf* rmark, float* ms, cudaStream_t st) {
+  HostSide V[2];
+  DevBuf d_pf[2];
+  CU(cudaEventRecord(c->diff_ev[EV_CCHURN.from], st));
+  for (int i = 0; i < 2; ++i) {
+    HostSide& v = V[i];
+    v.n = n;
+    v.base.assign((size_t)n + 1, 0);
+    for (int32_t k = 0; k < n; ++k) {
+      const int32_t f = pf[i][k];
+      v.base[(size_t)k + 1] = v.base[(size_t)k] + (f >= 0 ? S[i].base[(size_t)f + 1] - S[i].base[(size_t)f] : 0);
+    }
+    v.total = v.base[(size_t)n];
+    if (!v.line_base.alloc(8 * ((size_t)n + 1)) || !v.line_hash.alloc(8 * (size_t)v.total) || !v.line_flag.alloc((size_t)v.total) ||
+        !d_pf[i].alloc(4 * (size_t)n))
+      return TSM_E_CUDA;
+    CU(cudaMemcpyAsync(v.line_base.p, v.base.data(), 8 * ((size_t)n + 1), cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_pf[i].p, pf[i], 4 * (size_t)n, cudaMemcpyHostToDevice, st));
+    if (v.total) {
+      k_churn_gather<<<(unsigned)((v.total + 255) / 256), 256, 0, st>>>(v.line_base.as<unsigned long long>(), (uint32_t)n, d_pf[i].as<int32_t>(),
+                                                                        S[i].d.line_base, S[i].d.line_hash, S[i].d.line_flag, v.total,
+                                                                        v.line_hash.as<unsigned long long>(), v.line_flag.as<uint8_t>());
+      c->launches++;
+    }
+    v.d.line_base = v.line_base.as<unsigned long long>();
+    v.d.line_hash = v.line_hash.as<unsigned long long>();
+    v.d.line_flag = v.line_flag.as<uint8_t>();
+  }
+  CU(cudaEventRecord(c->diff_ev[EV_CCHURN.to], st));
+  CU(cudaGetLastError());
+  const int launches = c->launches;
+  std::vector<int64_t> added((size_t)n), removed((size_t)n);
+  int rc = diff_core<DIFF_MARKS>(c, V[0], V[1], n, added.data(), removed.data(), nullptr, st);   // (synchronises st)
+  c->launches += launches;
+  if (rc != TSM_OK) return rc;
+  ms[2] += span_ms(c, EV_CCHURN) + c->last_ms[MS_DIFF][1] + c->last_ms[MS_DIFF][2];
+  CU(cudaEventRecord(c->diff_ev[EV_CCHURN.from], st));
+  for (int i = 0; i < 2; ++i)
+    if (V[i].total) {
+      k_churn_marks<<<(unsigned)((V[i].total + 255) / 256), 256, 0, st>>>(V[i].d.line_base, (uint32_t)n, d_pf[i].as<int32_t>(), S[i].d.line_base,
+                                                                          V[i].line_mark.as<uint8_t>(), V[i].total, rmark[i].as<uint8_t>());
+      c->launches++;
+    }
+  CU(cudaEventRecord(c->diff_ev[EV_CCHURN.to], st));
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(st));
+  ms[3] += span_ms(c, EV_CCHURN);
+  return TSM_OK;
+}
+
+// The churn of one side's classes (CloneDev of clone_classes) under its revision's marks: per unit marked / marked assertion line
+// (k_churn_units), their prefix sums, then k_churn_frags and k_churn_classes, copied into o's churn outputs.  ms[3] += their time.
+static int churn_side(tsm_ctx* c, const CloneDev& d, const uint8_t* rmark, bool new_side, tsm_clone_churn_side* o, float* ms,
+                      cudaStream_t st) {
+  const uint32_t U = d.n_units, nc = d.nc;
+  const unsigned long long nm = d.nm;
+  DevBuf d_mk, d_mka, d_P, d_PA, d_bsum, d_ch, d_cha, d_state, d_counts, d_status;
+  if (!d_mk.alloc(4 * (size_t)U) || !d_mka.alloc(4 * (size_t)U) || !d_P.alloc(8 * ((size_t)U + 1)) || !d_PA.alloc(8 * ((size_t)U + 1)) ||
+      !d_bsum.alloc(8 * ((size_t)U / XS_TILE + 4)) || !d_ch.alloc(4 * nm) || !d_cha.alloc(4 * nm) || !d_state.alloc(nm) ||
+      !d_counts.alloc(12 * (size_t)nc) || !d_status.alloc(nc)) {
+    cudaGetLastError();
+    return TSM_E_NOMEM;
+  }
+  const unsigned long long* P = d_P.as<unsigned long long>();
+  const unsigned long long* PA = d_PA.as<unsigned long long>();
+  CU(cudaEventRecord(c->diff_ev[EV_CCHURN.from], st));
+  k_churn_units<<<(U + 255) / 256, 256, 0, st>>>(rmark, d.unit_line, d.unit_flag, U, d_mk.as<uint32_t>(), d_mka.as<uint32_t>());
+  xscan(d_mk.as<uint32_t>(), U, d_bsum.as<unsigned long long>(), d_P.as<unsigned long long>(), st);
+  xscan(d_mka.as<uint32_t>(), U, d_bsum.as<unsigned long long>(), d_PA.as<unsigned long long>(), st);
+  k_churn_frags<<<(unsigned)((nm + 255) / 256), 256, 0, st>>>(d.class_base, d.class_len, nc, d.member, nm, P, PA, d_ch.as<uint32_t>(),
+                                                               d_cha.as<uint32_t>(), d_state.as<uint8_t>());
+  k_churn_classes<<<std::min<unsigned>((unsigned)c->sms * 8, (unsigned)(((size_t)nc * 32 + 255) / 256)), 256, 0, st>>>(
+      d.class_base, nc, d_state.as<uint8_t>(), new_side, d_counts.as<uint32_t>(), d_status.as<uint8_t>());
+  CU(cudaEventRecord(c->diff_ev[EV_CCHURN.to], st));
+  CU(cudaGetLastError());
+  c->launches += 9;                                        // units, 2 x xscan (3 each), frags, classes
+  if (o->changed) CU(cudaMemcpyAsync(o->changed, d_ch.p, 4 * nm, cudaMemcpyDeviceToHost, st));
+  if (o->changed_assert) CU(cudaMemcpyAsync(o->changed_assert, d_cha.p, 4 * nm, cudaMemcpyDeviceToHost, st));
+  if (o->state) CU(cudaMemcpyAsync(o->state, d_state.p, nm, cudaMemcpyDeviceToHost, st));
+  if (o->class_counts) CU(cudaMemcpyAsync(o->class_counts, d_counts.p, 12 * (size_t)nc, cudaMemcpyDeviceToHost, st));
+  if (o->status) CU(cudaMemcpyAsync(o->status, d_status.p, nc, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  ms[3] += span_ms(c, EV_CCHURN);
+  return TSM_OK;
+}
+
+// Both revisions to the device and their line records (one k_scan pass each, one synchronisation), the marks of the pairs
+// (churn_marks), then per revision its classes - clone_classes over the line records, or blind_classes - whose continuation
+// runs churn_side on the device arrays of the classes.  Both sides run also when one is short of a cap, so that every count is set.
+extern "C" int tsm_clone_churn(tsm_ctx* c, const tsm_corpus* old_rev, const tsm_corpus* new_rev, const int32_t* pair_old,
+                               const int32_t* pair_new, int64_t n_pairs, int32_t min_lines, int32_t blind, tsm_clone_churn_side* old_side,
+                               tsm_clone_churn_side* new_side, void* stream) {
+  if (!c || !old_rev || !new_rev || !old_side || !new_side || n_pairs < 0 || n_pairs > INT32_MAX || (n_pairs && (!pair_old || !pair_new)) ||
+      min_lines < 1 || min_lines > 1024)
+    return TSM_E_ARG;
+  const tsm_corpus* rev[2] = {old_rev, new_rev};
+  tsm_clone_churn_side* side[2] = {old_side, new_side};
+  const int32_t* pf[2] = {pair_old, pair_new};
+  const int32_t n = (int32_t)n_pairs;
+  for (int i = 0; i < 2; ++i) {
+    const tsm_clone_churn_side* o = side[i];
+    if (rev[i]->n_files < 0 || o->clones.class_cap < 0 || o->clones.member_cap < 0 || (blind && o->blind.kept_cap < 0)) return TSM_E_ARG;
+    std::vector<uint8_t> used((size_t)rev[i]->n_files, 0);
+    for (int32_t k = 0; k < n; ++k) {
+      const int32_t f = pf[i][k];
+      if (f < -1 || f >= rev[i]->n_files || (f >= 0 && used[(size_t)f]++) || (pair_old[k] < 0 && pair_new[k] < 0)) return TSM_E_ARG;
+    }
+  }
+  float* const ms = clear_ms(c, MS_CCHURN);
+  c->launches = 0;
+  for (int i = 0; i < 2; ++i) {
+    tsm_clone_result& out = side[i]->clones;
+    tsm_blind_result& b = side[i]->blind;
+    const size_t nf = (size_t)rev[i]->n_files;
+    out.n_classes = out.n_members = 0;
+    if (out.line_base) memset(out.line_base, 0, sizeof(int64_t) * (nf + 1));
+    if (out.class_base) out.class_base[0] = 0;
+    if (out.file_dup) memset(out.file_dup, 0, sizeof(uint32_t) * nf);
+    if (out.file_dup_assert) memset(out.file_dup_assert, 0, sizeof(uint32_t) * nf);
+    if (blind) {
+      b.n_kept = 0;
+      if (b.kept_base) memset(b.kept_base, 0, sizeof(int64_t) * (nf + 1));
+      if (b.file_kept_assert) memset(b.file_kept_assert, 0, sizeof(uint32_t) * nf);
+    }
+  }
+  HostSide* scan[2];
+  int ns = 0;
+  for (int i = 0; i < 2; ++i)
+    if (rev[i]->n_files > 0) {
+      const int rc = check_sides({rev[i]}, true);
+      if (rc != TSM_OK) return rc;
+    }
+  cudaStream_t st = (cudaStream_t)stream;
+  CallScope call(c, st);
+  CU(call.status);
+  HostSide S[2];
+  DevBuf rmark[2];
+  SyncGuard guard(st);
+  for (int i = 0; i < 2; ++i)
+    if (rev[i]->n_files > 0) {
+      const int rc = side_upload(rev[i], S[i], st);
+      if (rc != TSM_OK) return rc;
+      scan[ns++] = &S[i];
+    }
+  if (ns) {
+    const int rc = sides_records(c, scan, ns, st, &ms[0], true);
+    if (rc != TSM_OK) return rc;
+  }
+  for (int i = 0; i < 2; ++i) {
+    c->launches += S[i].launches;
+    if (side[i]->clones.line_base)
+      for (size_t f = 0; f < S[i].base.size(); ++f) side[i]->clones.line_base[f] = (int64_t)S[i].base[f];
+    if (!rmark[i].alloc((size_t)S[i].total)) return TSM_E_CUDA;
+    CU(cudaMemsetAsync(rmark[i].p, 0, (size_t)S[i].total, st));
+  }
+  if (n) {
+    const int rc = churn_marks(c, S, pf, n, rmark, ms, st);
+    if (rc != TSM_OK) return rc;
+  }
+  int rc_all = TSM_OK;
+  for (int i = 0; i < 2; ++i) {
+    if (S[i].total == 0) continue;
+    tsm_clone_churn_side* o = side[i];
+    const bool class_out = o->class_counts || o->status, member_out = o->changed || o->changed_assert || o->state;
+    const uint8_t* mark = rmark[i].as<uint8_t>();
+    auto then = [&](const CloneDev& d, cudaStream_t s2) { return churn_side(c, d, mark, i == 1, o, ms, s2); };
+    float cms[3] = {0, 0, 0};
+    int rc;
+    if (blind)
+      rc = blind_classes(c, S[i], S[i].total, (uint32_t)min_lines, &o->blind, &o->clones, cms, st, then, class_out, member_out);
+    else
+      rc = clone_classes<true>(c, S[i].d.line_hash, S[i].d.line_base, (uint32_t)S[i].n, (uint32_t)S[i].total, S[i].d.line_flag,
+                               S[i].d.line_end, S[i].d.arena, S[i].d.off, (uint32_t)min_lines, &o->clones, cms + 1, st, then, class_out,
+                               member_out);
+    ms[1] += cms[0] + cms[1] + cms[2];
+    if (rc == TSM_E_CAPACITY) rc_all = rc;
+    else if (rc != TSM_OK) return rc;
+  }
+  return rc_all;
+}
+
+extern "C" int tsm_clone_churn_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_CCHURN, ms4, 4); }
 
 // ------------------------------------------------------------------------------------- SPEC section 18 test smells
 // The smell stage over one side whose line records (with header events) and case spans exist: the section-10 kinds

@@ -47,6 +47,7 @@
 #include <memory>
 #include <numeric>
 #include <optional>
+#include <set>
 #include <sstream>
 #include <string>
 #include <thread>
@@ -1632,6 +1633,8 @@ struct DiffOptions {
   int rename_pct = -1;
   int64_t batch_bytes = kBatch;
   std::string out, asserts, churn, cases, edits, smells, moves;
+  std::string clones;                                      // --clones F, with its --min-lines, --blind and the file selection
+  int clone_min_lines = 5; bool clone_blind = false, all_files = false;
   bool zero_rows = false;
   std::vector<std::string> lead_head;
   size_t churn_lead = 0;
@@ -1758,6 +1761,153 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
   return t;
 }
 
+// ---------------------------------------------------------------------------------- clone churn (docs/SPEC.md section 22)
+// A revision of the clone churn: its selected files in the order of `clones --git --rev` (walk_git: path components compared
+// one by one) with their bytes, and those bytes packed once into a pinned arena.
+static bool path_less(const std::string& a, const std::string& b) {
+  for (size_t i = 0, j = 0;;) {
+    size_t ei = a.find('/', i), ej = b.find('/', j);
+    if (ei == std::string::npos) ei = a.size();
+    if (ej == std::string::npos) ej = b.size();
+    const int c = a.compare(i, ei - i, b, j, ej - j);
+    if (c) return c < 0;
+    if (ei == a.size() || ej == b.size()) return ei == a.size() && ej != b.size();
+    i = ei + 1; j = ej + 1;
+  }
+}
+struct PathLess { bool operator()(const std::string& a, const std::string& b) const { return path_less(a, b); } };
+using Blob = std::shared_ptr<const std::vector<uint8_t>>;
+struct Revision {
+  std::vector<std::string> paths;
+  std::vector<Blob> blobs;
+  Batch b;
+  std::map<std::string, int32_t> index;                    // path -> file index
+};
+static Revision make_revision(const std::map<std::string, Blob, PathLess>& files) {
+  Revision r;
+  std::vector<const std::vector<uint8_t>*> bytes;
+  std::vector<int32_t> len, off(files.size() + 1);
+  for (const auto& kv : files) {
+    r.index[kv.first] = (int32_t)r.paths.size();
+    r.paths.push_back(kv.first); r.blobs.push_back(kv.second); bytes.push_back(kv.second.get());
+    len.push_back((int32_t)kv.second->size());
+  }
+  const int64_t need = tsm_layout(len.data(), (int32_t)len.size(), off.data());
+  if (need < 0 || need + 4096 >= (1ll << 31))
+    die("the selected files (" + std::to_string(need < 0 ? INT64_MAX : need + 4096) + " bytes of arena) do not fit one int32-indexed "
+        "arena; clones are found across all files at once, so select fewer files");
+  r.b = pack(bytes);
+  for (size_t i = 0; i < r.paths.size(); ++i) r.b.ext[i] = (uint8_t)ext_tag(r.paths[i]);
+  return r;
+}
+
+static const char* const kCloneStatus[] = {"untouched", "changed", "removed", "diverged", "dropped", "created", "copied", "joined"};
+static const char* const kFragState[] = {"kept", "edited", "whole"};
+
+// One step: tsm_clone_churn over the two revisions and the step's changes (after --find-renames; `old_path` names the old side of
+// a rename), then one row per fragment of every touched class, the old side first.  A change binary on a side (a NUL byte in its
+// first 8000) is a deletion plus an addition: all of its lines are marked.
+static void clone_churn_step(tsm_ctx* ctx, const Revision& ro, const Revision& rn, const Change* c0, const Change* c1,
+                             const std::function<bool(const Change&)>& is_binary, const DiffOptions& d,
+                             const std::vector<std::string>& lead, std::ostream& os) {
+  std::vector<int32_t> po, pn;
+  for (const Change* c = c0; c != c1; ++c) {
+    const int32_t a = c->o >= 0 ? ro.index.at(c->old_path.empty() ? c->path : c->old_path) : -1;
+    const int32_t b = c->n >= 0 ? rn.index.at(c->path) : -1;
+    if (a >= 0 && b >= 0 && is_binary(*c)) { po.push_back(a); pn.push_back(-1); po.push_back(-1); pn.push_back(b); }
+    else { po.push_back(a); pn.push_back(b); }
+  }
+  const Revision* rev[2] = {&ro, &rn};
+  struct Side { std::vector<int64_t> base, cbase, member, kbase, kline; std::vector<uint32_t> clen, changed, changed_a, counts; std::vector<uint8_t> state, status; };
+  Side S[2];
+  tsm_clone_churn_side cs[2] = {};
+  const tsm_corpus co = ro.b.corpus(1), cn = rn.b.corpus(1);
+  auto call = [&] {
+    ck(tsm_clone_churn(ctx, &co, &cn, po.data(), pn.data(), (int64_t)po.size(), d.clone_min_lines, d.clone_blind, &cs[0], &cs[1], nullptr),
+       "tsm_clone_churn");
+  };
+  for (int s = 0; s < 2; ++s) {
+    S[s].base.resize(rev[s]->paths.size() + 1); S[s].kbase.resize(rev[s]->paths.size() + 1);
+    cs[s].clones.line_base = S[s].base.data(); cs[s].blind.kept_base = S[s].kbase.data();
+  }
+  call();                                                  // the counts; the second call fills arrays of that size
+  for (int s = 0; s < 2; ++s) {
+    Side& x = S[s];
+    tsm_clone_churn_side& c = cs[s];
+    const size_t nc = (size_t)c.clones.n_classes, nm = (size_t)c.clones.n_members, nk = (size_t)c.blind.n_kept;
+    x.cbase.resize(nc + 1); x.clen.resize(std::max<size_t>(nc, 1)); x.counts.resize(3 * std::max<size_t>(nc, 1)); x.status.resize(std::max<size_t>(nc, 1));
+    x.member.resize(std::max<size_t>(nm, 1)); x.changed.resize(std::max<size_t>(nm, 1)); x.changed_a.resize(std::max<size_t>(nm, 1));
+    x.state.resize(std::max<size_t>(nm, 1)); x.kline.resize(std::max<size_t>(nk, 1));
+    c.clones.class_base = x.cbase.data(); c.clones.class_len = x.clen.data(); c.clones.class_cap = (int64_t)nc;
+    c.clones.member = x.member.data(); c.clones.member_cap = (int64_t)nm;
+    c.blind.kept_line = x.kline.data(); c.blind.kept_cap = (int64_t)nk;
+    c.changed = x.changed.data(); c.changed_assert = x.changed_a.data(); c.state = x.state.data();
+    c.class_counts = x.counts.data(); c.status = x.status.data();
+  }
+  call();
+  for (int s = 0; s < 2; ++s) {
+    const Side& x = S[s];
+    const std::vector<int64_t>& fbase = d.clone_blind ? x.kbase : x.base;   // the numbering of member
+    for (int64_t k = 0; k < cs[s].clones.n_classes; ++k) {
+      if (!x.status[(size_t)k]) continue;
+      const int64_t b0 = x.cbase[(size_t)k], b1 = x.cbase[(size_t)k + 1];
+      for (int64_t j = b0; j < b1; ++j) {
+        const int64_t at = x.member[(size_t)j], last = at + x.clen[(size_t)k] - 1;
+        const size_t f = (size_t)(std::upper_bound(fbase.begin(), fbase.end(), at) - fbase.begin() - 1);
+        const int64_t first = (d.clone_blind ? x.kline[(size_t)at] : at) - x.base[f] + 1;
+        const int64_t end = (d.clone_blind ? x.kline[(size_t)last] : last) - x.base[f] + 1;
+        std::vector<std::string> row = lead;
+        row.insert(row.end(), {s ? "+" : "-", std::to_string(k + 1), kCloneStatus[x.status[(size_t)k]], std::to_string(b1 - b0),
+                               rev[s]->paths[f], std::to_string(first), std::to_string(end), kFragState[x.state[(size_t)j]],
+                               std::to_string(x.changed[(size_t)j]), std::to_string(x.changed_a[(size_t)j])});
+        csv_row(os, row);
+      }
+    }
+  }
+}
+
+static std::vector<std::string> clone_churn_head(std::vector<std::string> lead) {
+  lead.insert(lead.end(), {"side", "class", "status", "fragments", "fileName", "first_line", "last_line", "state", "changed_lines",
+                           "changed_assert_lines"});
+  return lead;
+}
+
+// `diff --clones`: the selected files of each root (S0 / S1 unless --all-files) are the two revisions; a file whose bytes differ, or
+// that one root lacks, is a change (then --find-renames); one clone_churn_step.
+static void diff_clone_churn(const std::string& old_root, const std::string& new_root, const DiffOptions& o) {
+  std::vector<FileEntry> fa, fb;
+  walk(old_root, 0, o.all_files, fa);
+  walk(new_root, 0, o.all_files, fb);
+  std::vector<Blob> blobs;                                 // the loader's names: the files of fa, then those of fb
+  std::map<std::string, Blob, PathLess> ra, rb;
+  std::map<std::string, int64_t> name_a, name_b;
+  for (int s = 0; s < 2; ++s)
+    for (const FileEntry& f : s ? fb : fa) {
+      auto v = std::make_shared<std::vector<uint8_t>>((size_t)f.size);
+      if (!read_file(f.abs, v->data(), f.size)) die("short read: " + f.abs);
+      if (v->size() > 0x7fff0000u) die("blob too large: " + f.rel);
+      (s ? name_b : name_a)[f.rel] = (int64_t)blobs.size();
+      (s ? rb : ra)[f.rel] = v;
+      blobs.push_back(v);
+    }
+  std::vector<Change> changes;
+  for (const auto& kv : ra) {
+    auto it = name_b.find(kv.first);
+    if (it != name_b.end() && *blobs[(size_t)it->second] == *kv.second) continue;
+    changes.push_back({0, kv.first, name_a[kv.first], it == name_b.end() ? -1 : it->second, "", -1});
+  }
+  for (const auto& kv : rb) if (!name_a.count(kv.first)) changes.push_back({0, kv.first, -1, name_b[kv.first], "", -1});
+  const Loader load = [&](int64_t s) { return *blobs[(size_t)s]; };
+  const auto ctx = small_context();
+  ChangeTotals t(1);
+  if (o.rename_pct >= 0) pair_renames(ctx.get(), changes, load, o.rename_pct, o.batch_bytes, t);
+  const Revision ro = make_revision(ra), rn = make_revision(rb);
+  std::ofstream os(o.clones, std::ios::binary);
+  csv_row(os, clone_churn_head({}));
+  clone_churn_step(ctx.get(), ro, rn, changes.data(), changes.data() + changes.size(),
+                   [&](const Change& c) { return binary(*blobs[(size_t)c.o]) || binary(*blobs[(size_t)c.n]); }, o, {}, os);
+}
+
 static int cmd_diff(const std::string& old_root, const std::string& new_root, const DiffOptions& o) {
   std::vector<FileEntry> a, b;
   walk(old_root, 0, true, a);
@@ -1777,6 +1927,7 @@ static int cmd_diff(const std::string& old_root, const std::string& new_root, co
     return v;
   };
   const ChangeTotals t = diff_changes(changes, 1, load, o);
+  if (!o.clones.empty()) diff_clone_churn(old_root, new_root, o);
   if (t.binaries) fprintf(stderr, "tosem-scan: %lld binary file(s) skipped\n", (long long)t.binaries);
   if (o.rename_pct >= 0)
     fprintf(stderr, "tosem-scan: %lld rename(s) found (%lld exact, %lld inexact)\n", (long long)t.renames, (long long)t.renames_exact,
@@ -1858,6 +2009,71 @@ struct History {
   }
 };
 
+// `history --clones`: the selected files of the current revision kept as live paths, from the boundary commit's tree (the parent of
+// the window's first commit; none for a root commit) and each commit's changes after --find-renames.  Blobs are read once while
+// they are live (cached by object name), and a revision is packed once: the new side of one tsm_clone_churn call is the old side
+// of the next.  One clone_churn_step per commit that changes a selected file.
+static void selected_blobs(gitstore::Store& gs, const gitstore::Oid& tree, const std::string& prefix, bool all_files,
+                           std::map<std::string, gitstore::Oid, PathLess>& out) {
+  std::vector<gitstore::TreeEntry> es;
+  if (!gs.tree(tree, es)) die("unreadable tree " + tree.hex());
+  for (const gitstore::TreeEntry& e : es) {
+    const std::string rel = prefix + e.name;
+    if (e.is_tree()) { selected_blobs(gs, e.oid, rel + "/", all_files, out); continue; }
+    if (!e.is_blob()) continue;
+    if (!all_files && (lower(rel).find("test") == std::string::npos || ext_tag(rel) == TSM_EXT_OTHER)) continue;   // S0, S1
+    out[rel] = e.oid;
+  }
+}
+
+static void history_clone_churn(History& h, const DiffOptions& o) {
+  std::vector<Change> changes = h.changes;
+  const auto ctx = small_context();
+  ChangeTotals t(h.chain.size());
+  if (o.rename_pct >= 0) pair_renames(ctx.get(), changes, h.load, o.rename_pct, o.batch_bytes, t);
+  std::map<std::string, gitstore::Oid, PathLess> live;
+  if (!h.chain.empty() && !h.chain[0].c.parents.empty()) {
+    gitstore::Commit p0;
+    if (!h.gs.commit(h.chain[0].c.parents[0], p0)) die("unreadable commit " + h.chain[0].c.parents[0].hex());
+    selected_blobs(h.gs, p0.tree, "", o.all_files, live);
+  }
+  std::map<gitstore::Oid, Blob> cache;
+  auto files_of = [&](const std::map<std::string, gitstore::Oid, PathLess>& paths) {
+    std::map<std::string, Blob, PathLess> f;
+    for (const auto& kv : paths) {
+      Blob& b = cache[kv.second];
+      if (!b) {
+        gitstore::Object x;
+        if (!h.gs.read(kv.second, x) || x.type != gitstore::OBJ_BLOB) die("unreadable blob " + kv.second.hex());
+        if (x.data.size() > 0x7fff0000u) die("blob too large: " + kv.first);
+        b = std::make_shared<const std::vector<uint8_t>>(std::move(x.data));
+      }
+      f[kv.first] = b;
+    }
+    return f;
+  };
+  std::ofstream os(o.clones, std::ios::binary);
+  csv_row(os, clone_churn_head(o.lead_head));
+  std::unique_ptr<Revision> cur;
+  for (size_t c0 = 0, c1 = 0; c0 < changes.size(); c0 = c1) {
+    for (c1 = c0; c1 < changes.size() && changes[c1].step == changes[c0].step; ++c1) {}
+    if (!cur) cur = std::make_unique<Revision>(make_revision(files_of(live)));
+    std::map<std::string, gitstore::Oid, PathLess> next = live;
+    for (size_t c = c0; c < c1; ++c)
+      if (changes[c].o >= 0) next.erase(changes[c].old_path.empty() ? changes[c].path : changes[c].old_path);
+    for (size_t c = c0; c < c1; ++c)
+      if (changes[c].n >= 0) next[changes[c].path] = h.objs[(size_t)changes[c].n];
+    auto rn = std::make_unique<Revision>(make_revision(files_of(next)));
+    auto is_binary = [&](const Change& c) { return binary(*cache.at(h.objs[(size_t)c.o])) || binary(*cache.at(h.objs[(size_t)c.n])); };
+    clone_churn_step(ctx.get(), *cur, *rn, changes.data() + c0, changes.data() + c1, is_binary, o, o.lead(changes[c0].step), os);
+    cur = std::move(rn);
+    live.swap(next);
+    std::set<gitstore::Oid> keep;                          // the cache holds the live blobs only
+    for (const auto& kv : live) keep.insert(kv.second);
+    for (auto it = cache.begin(); it != cache.end();) it = keep.count(it->first) ? std::next(it) : cache.erase(it);
+  }
+}
+
 // --dry-run: no GPU - the rows carry the object names, sizes and an FNV-1a checksum of both blobs instead of the counts
 // (what the CPU tests compare with `git diff-tree` / `git cat-file`).
 static int cmd_history(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files, bool dry_run, DiffOptions o) {
@@ -1886,6 +2102,7 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
     }
   } else {
     o.zero_rows = true; o.lead_head = {"commit", "parent", "time"}; o.churn_lead = 1;
+    if (!o.clones.empty()) history_clone_churn(h, o);      // (before diff_changes, which pairs the renames of h.changes in place)
     t = diff_changes(h.changes, h.chain.size(), h.load, o);
   }
   printf("commit,files,cloc,added,removed\r\n");
@@ -2258,12 +2475,13 @@ static void usage() {
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
           "       tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]\n"
           "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--smells F]\n"
-          "                         [--moves F] [--find-renames N] [--batch-bytes N]\n"
+          "                         [--moves F] [--clones F [--min-lines N] [--blind] [--all-files]] [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan body   <project-root>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases <snapshot-root>=<tag>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases --git <repository> [<revision>...] [--batch-bytes N] [--out F]\n"
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
-          "                          [--cases F] [--assert-edits F] [--smells F] [--moves F] [--find-renames N] [--batch-bytes N]\n"
+          "                          [--cases F] [--assert-edits F] [--smells F] [--moves F] [--clones F [--min-lines N] [--blind]]\n"
+          "                          [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
           "       tosem-scan clones <project-root>... [--min-lines N] [--blind] [--all-files] [--out F]\n"
           "       tosem-scan clones --git <repository> [--rev R] [--min-lines N] [--blind] [--all-files] [--out F]\n"
@@ -2281,6 +2499,8 @@ static void usage() {
           "--moves F: one row per block of changed lines that a commit moves, within or across its files, as git diff\n"
           "           --color-moved=blocks finds them (docs/SPEC.md section 20); a commit is never split across batches, and one\n"
           "           larger than --batch-bytes is a batch of its own.\n"
+          "--clones F: per commit, one row per fragment of every clone class of the parent (-) or the commit (+) that the commit\n"
+          "            edits, with the class's status (copied, diverged, ...) and the fragment's changed lines (docs/SPEC.md section 22).\n"
           "--batch-bytes N: files go to the GPU in batches of at most N bytes (per side of a diff; a larger file alone); scan: 1 GiB, else 512 MiB.\n"
           "Scans run on the GPU through libtosemscan.so (sm_90a); there is no CPU fallback.\n");
 }
@@ -2331,6 +2551,13 @@ int main(int argc, char** argv) {
   d.rename_pct = rename_pct; d.batch_bytes = batch_bytes(kBatch, 1);
   d.out = opt["--out"]; d.asserts = opt["--asserts"]; d.churn = opt["--assert-churn"]; d.cases = opt["--cases"];
   d.edits = opt["--assert-edits"]; d.smells = opt["--smells"]; d.moves = opt["--moves"];
+  if (opt.count("--clones")) {                             // (--min-lines and --blind are read only with --clones)
+    d.clones = opt["--clones"]; d.clone_blind = blind; d.all_files = all_files;
+    const long n = opt.count("--min-lines") ? strtol(opt["--min-lines"].c_str(), nullptr, 10) : 5;
+    if (n < 1 || n > 1024) die("--min-lines needs a number of lines from 1 to 1024");
+    d.clone_min_lines = (int)n;
+    if (dry_run) die("--dry-run and --clones cannot be combined (clone churn needs the GPU)");
+  }
   const std::string rev = opt.count("--rev") ? opt["--rev"] : "HEAD";
   const int64_t max_commits = opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0;
   if (cmd == "history") { if (pos.size() != 1) die("history needs the repository");

@@ -50,7 +50,9 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_diff_pairs_marks", "tsm_blame_pairs", "tsm_blame_last_ms", "tsm_clones", "tsm_clones_last_ms",
            "tsm_diff_pairs_cases", "tsm_diff_pairs_assert_edits", "tsm_assert_edits_last_ms", "tsm_smells", "tsm_smells_last_ms",
            "tsm_diff_pairs_smells", "tsm_diff_smells_last_ms", "tsm_diff_pairs_moves", "tsm_moves_last_ms", "tsm_clones_blind",
-           "tsm_clones_blind_last_ms"]
+           "tsm_clones_blind_last_ms", "tsm_clone_churn", "tsm_clone_churn_last_ms"]
+FRAG_STATES = ["kept", "edited", "whole"]          # tsm_clone_churn state[j] (docs/SPEC.md section 22)
+CLONE_STATUSES = ["untouched", "changed", "removed", "diverged", "dropped", "created", "copied", "joined"]   # status[c]
 
 
 class TsmError(RuntimeError):
@@ -109,6 +111,11 @@ class _CloneResult(C.Structure):
 class _BlindResult(C.Structure):
     _fields_ = [("kept_base", C.c_void_p), ("kept_line", C.c_void_p), ("blind_hash", C.c_void_p), ("file_kept_assert", C.c_void_p),
                 ("kept_cap", C.c_int64), ("n_kept", C.c_int64)]
+
+
+class _CloneChurnSide(C.Structure):
+    _fields_ = [("clones", _CloneResult), ("blind", _BlindResult), ("changed", C.c_void_p), ("changed_assert", C.c_void_p),
+                ("state", C.c_void_p), ("class_counts", C.c_void_p), ("status", C.c_void_p)]
 
 
 _lib = None
@@ -233,6 +240,11 @@ def lib():
             [C.POINTER(_DiffMoves), C.c_void_p]
         L.tsm_moves_last_ms.restype = C.c_int
         L.tsm_moves_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
+        L.tsm_clone_churn.restype = C.c_int
+        L.tsm_clone_churn.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus), C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
+                                      C.c_int32, C.POINTER(_CloneChurnSide), C.POINTER(_CloneChurnSide), C.c_void_p]
+        L.tsm_clone_churn_last_ms.restype = C.c_int
+        L.tsm_clone_churn_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
         _lib = L
     return _lib
 
@@ -986,4 +998,64 @@ class Scanner:
         coverage] in ms."""
         ms = (C.c_float * 4)()
         lib().tsm_clones_blind_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
+
+    def clone_churn(self, old_rev, new_rev, pair_old, pair_new, min_lines=5, blind=False, stream=None, cap=None):
+        """Clone churn (docs/SPEC.md section 22): a dict {"old": ..., "new": ...}, per revision the dict of clones(rev, min_lines,
+        blind) for that revision alone plus per fragment changed, changed_assert and state (FRAG_STATES) and per class
+        class_counts[n_classes, 3] (kept, edited, whole fragments) and status (CLONE_STATUSES).  Pair k is file pair_old[k] of
+        old_rev and file pair_new[k] of new_rev, -1 for none.  Arrays too small for the classes, fragments or kept lines are sized
+        from the counts and the call is made again (cap: the first guess of each)."""
+        po = np.ascontiguousarray(pair_old, np.int32).ravel()
+        pn = np.ascontiguousarray(pair_new, np.int32).ravel()
+        if po.size != pn.size:
+            raise ValueError("pair_old and pair_new differ in length")
+        revs = (old_rev, new_rev)
+        cs = [r.c_struct() for r in revs]
+        g = int(cap if cap is not None else 0)
+        caps = [[g, g, g], [g, g, g]]                       # per side: classes, fragments, kept lines
+        for _ in range(2):
+            outs, sides = [], []
+            for r, (cc, cm, ck) in zip(revs, caps):
+                n = r.n_files
+                o = {"line_base": np.zeros(n + 1, np.int64), "file_dup": np.zeros(n, np.uint32), "file_dup_assert": np.zeros(n, np.uint32),
+                     "class_base": np.zeros(cc + 1, np.int64), "class_len": np.zeros(max(cc, 1), np.uint32),
+                     "member": np.zeros(max(cm, 1), np.int64), "changed": np.zeros(max(cm, 1), np.uint32),
+                     "changed_assert": np.zeros(max(cm, 1), np.uint32), "state": np.zeros(max(cm, 1), np.uint8),
+                     "class_counts": np.zeros((max(cc, 1), 3), np.uint32), "status": np.zeros(max(cc, 1), np.uint8)}
+                cr = _CloneResult(*[_p(o[k]) for k in ("line_base", "file_dup", "file_dup_assert", "class_base", "class_len")], cc, 0,
+                                  _p(o["member"]), cm, 0)
+                br = _BlindResult(None, None, None, None, 0, 0)
+                if blind:
+                    o.update(kept_base=np.zeros(n + 1, np.int64), kept_line=np.zeros(max(ck, 1), np.int64),
+                             blind_hash=np.zeros(max(ck, 1), np.uint64), file_kept_assert=np.zeros(n, np.uint32))
+                    br = _BlindResult(*[_p(o[k]) for k in ("kept_base", "kept_line", "blind_hash", "file_kept_assert")], ck, 0)
+                outs.append(o)
+                sides.append(_CloneChurnSide(cr, br, *[_p(o[k]) for k in ("changed", "changed_assert", "state", "class_counts", "status")]))
+            rc = lib().tsm_clone_churn(self._ctx, C.byref(cs[0]), C.byref(cs[1]), _p(po), _p(pn), po.size, int(min_lines), int(bool(blind)),
+                                       C.byref(sides[0]), C.byref(sides[1]), stream)
+            need = [[int(sd.clones.n_classes), int(sd.clones.n_members), int(sd.blind.n_kept) if blind else 0] for sd in sides]
+            if rc == TSM_E_CAPACITY and any(w > h for nd, cp in zip(need, caps) for w, h in zip(nd, cp)):
+                caps = need
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_clone_churn")
+            res = {}
+            for name, o, (nc, nm, nk) in zip(("old", "new"), outs, need):
+                for k in ("class_len", "class_counts", "status"):
+                    o[k] = o[k][:nc]
+                o["class_base"] = o["class_base"][:nc + 1]
+                for k in ("member", "changed", "changed_assert", "state"):
+                    o[k] = o[k][:nm]
+                if blind:
+                    o["kept_line"], o["blind_hash"] = o["kept_line"][:nk], o["blind_hash"][:nk]
+                res[name] = o
+            return res
+        raise TsmError(TSM_E_CAPACITY, "tsm_clone_churn")
+
+    def clone_churn_last_ms(self):
+        """Device time of the last clone_churn call: [k_scan over both revisions, classes of both, k_churn_gather + the marks
+        diff, k_churn_marks + the churn kernels of both sides] in ms."""
+        ms = (C.c_float * 4)()
+        lib().tsm_clone_churn_last_ms(self._ctx, C.byref(ms))
         return [float(x) for x in ms]
