@@ -390,6 +390,38 @@ int tsm_smells(tsm_ctx* ctx, const tsm_corpus* corpus, int64_t* line_base, uint1
                tsm_smell_test* tests, int64_t test_cap, int64_t* n_tests, void* stream);
 int tsm_smells_last_ms(tsm_ctx* ctx, float* ms4);
 
+/* Similar tests (docs/SPEC.md section 23, `tosem-scan similar-tests`): the pairs of tests of section 18 whose sequences of kept
+ * blind lines (section 21, header line included) are at least min_similarity % alike, and the classes they link.  A test is
+ * compared when it has at least min_lines kept lines (min_lines >= 1, else TSM_E_ARG).  Tests a < b form a pair when both are
+ * compared and 200 * lcs >= P * (k(a) + k(b)), lcs being the longest common subsequence of their sequences (two kept lines are
+ * equal when their blind hashes are), k their lengths and P = min_similarity in 1..100 (else TSM_E_ARG).
+ *   tests, test_kept   every test, exactly as tsm_smells returns them (global line order), and its kept lines k (test_cap each)
+ *   pairs              every pair {a, b, lcs, score}, score = floor(120000 * lcs / (k(a) + k(b))), ascending (a, b) (pair_cap)
+ *   class_base/member  the connected components of at least two tests of the graph of the pairs (single linkage), ordered by
+ *                      their smallest test, members ascending: class c is member[class_base[c] .. class_base[c+1])
+ *                      (class_base holds class_cap + 1 entries, member member_cap)
+ *   n_candidates       the candidate pairs whose LCS was computed (those that pass the exact prefix and size filters)
+ * Any output pointer may be NULL (it is skipped); every count is always set.  A short cap for a given output returns
+ * TSM_E_CAPACITY with every count set: size the arrays and call again.  n_files = 0 is legal.  Memory errors as for tsm_clones.
+ * Kernels: k_scan with the header events, the case spans and smell stage of tsm_smells, the lexer of tsm_clones_blind; then
+ * k_st_tests, a count table of the blind hashes (k_st_count, k_st_order), the prefix tokens and their posting lists (k_st_prefix,
+ * k_st_lists), a scan of the lists' candidate counts (k_st_csums, k_st_capply), and per chunk of that virtual candidate space
+ * k_st_enum (filters) and k_st_verify (bit-parallel LCS, one warp per candidate) (csrc/tsm_simtest_kernels.cuh).  The classes are
+ * formed on the host from the pairs.
+ * tsm_similar_tests_last_ms: device time of the last call, ms4 = { k_scan, case spans + smell stage + lexer, token table +
+ * prefixes + posting lists + enumeration, verification }. */
+typedef struct tsm_similar_pair { int32_t a, b; uint32_t lcs, score; } tsm_similar_pair;
+typedef struct tsm_similar_result {
+  tsm_smell_test* tests; uint32_t* test_kept; int64_t test_cap; int64_t n_tests;
+  tsm_similar_pair* pairs; int64_t pair_cap; int64_t n_pairs;
+  int64_t* class_base; int64_t class_cap; int64_t n_classes;
+  int32_t* member; int64_t member_cap; int64_t n_members;
+  int64_t n_candidates;
+} tsm_similar_result;
+int tsm_similar_tests(tsm_ctx* ctx, const tsm_corpus* corpus, int32_t min_lines, int32_t min_similarity, tsm_similar_result* out,
+                      void* stream);
+int tsm_similar_tests_last_ms(tsm_ctx* ctx, float* ms4);
+
 /* Test-smell churn (docs/SPEC.md section 19): the section-16 cases and the section-18 tests of both sides of every revision pair,
  * and per test how many of its smell instances the revision adds (new side) or removes (old side).  cases is filled exactly as
  * tsm_diff_pairs_cases fills it.  old_tests / new_tests are the tsm_smell_test records of tsm_smells over each side's corpus

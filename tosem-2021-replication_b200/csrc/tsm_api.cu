@@ -27,6 +27,7 @@
 #include "tsm_smell_kernels.cuh"
 #include "tsm_move_kernels.cuh"
 #include "tsm_clone_churn_kernels.cuh"
+#include "tsm_simtest_kernels.cuh"
 
 using namespace tsm;
 
@@ -90,6 +91,7 @@ enum Timed {
   MS_MOVE,    // k_scan, the diff, line flags to k_move_reach, k_move_starts to k_move_mark of the last tsm_diff_pairs_moves
   MS_BLAME,   // k_blame of the last tsm_blame_pairs
   MS_CCHURN,  // k_scan of both revisions, classes of both, the marks diff, the churn kernels of the last tsm_clone_churn
+  MS_SIMTEST, // k_scan, case spans + smell stage + lexer, tokens + lists + enumeration, verification of the last tsm_similar_tests
   N_TIMED
 };
 
@@ -173,6 +175,8 @@ struct tsm_ctx {
 //   tsm_blame_pairs, behind the diff       BLAME                                                           at the end
 //   tsm_clone_churn: gather, behind scans  CCHURN                                                          behind the diff
 //     marks, then per side behind classes  CCHURN                                                          at each end
+//   tsm_similar_tests                                      FRONT   ENUM*   VERIFY* END*    LEXED   LISTS   at the counts /
+//                                                                                                         each chunk
 //   (* recorded by smell_stage, and not read in this call)
 struct EvSpan { int from, to; };
 constexpr EvSpan EV_SCAN[2] = {{0, 1}, {6, 7}}, EV_SMALL = {2, 3}, EV_LEFT = {4, 5};
@@ -184,6 +188,7 @@ constexpr EvSpan EV_CHURN_SMELLS = {0, 1}, EV_CHURN_CASES = {0, 1};   // the old
 constexpr EvSpan EV_MOVE_FLAGS = {0, 1}, EV_MOVE_JOIN = {2, 3}, EV_MOVE_RUNS = {4, 5}, EV_MOVE_MARK = {6, 7};
 constexpr EvSpan EV_BLAME = {0, 1};
 constexpr EvSpan EV_CCHURN = {0, 1};
+constexpr int EV_ST_FRONT = 2, EV_ST_ENUM = 3, EV_ST_VERIFY = 4, EV_ST_END = 5, EV_ST_LEXED = 6, EV_ST_LISTS = 7;
 
 // The start of every call that queues device work on st: the ctx's device, the ctx's pool for the call's DevBufs, and the
 // order of the ctx's calls.  A ctx orders its own work, whatever stream each call is given: the call's stream first waits
@@ -2064,54 +2069,66 @@ extern "C" int tsm_clones(tsm_ctx* c, const tsm_corpus* k, int32_t min_lines, ts
 extern "C" int tsm_clones_last_ms(tsm_ctx* c, float* ms3) { return copy_ms(c, MS_CLONE, ms3, 3); }
 
 // ------------------------------------------------------------------------------------- SPEC section 21 blind clones
-// The section-21 front over one side whose line records exist (S, total lines > 0): the lexer of tsm_blind_kernels.cuh (line
-// states, blind hashes, compaction of the kept lines), one synchronisation that reads the kept count, then clone_classes over
+// The lexer of section 21 over one side whose line records exist (S.total > 0), in the kernels of tsm_blind_kernels.cuh: line
+// states, blind hashes and kept flags, an xscan of the kept flags (rank[l] = the kept lines before line l, rank[total] = all),
+// the compaction of the kept lines (kline, khash, kflag) and per file its kept base and kept assertion lines.
+struct BlindFront { DevBuf state, hash, kept, rank, bsum, kline, khash, kflag, kbase, kassert; };
+
+static int blind_front(tsm_ctx* c, const HostSide& S, BlindFront& f, cudaStream_t st) {
+  const unsigned long long total = S.total;
+  const uint32_t T = (uint32_t)total, nfu = (uint32_t)S.n;
+  const size_t L = (size_t)total;
+  if (!f.state.alloc(L) || !f.hash.alloc(8 * L) || !f.kept.alloc(4 * L) || !f.rank.alloc(8 * (L + 1)) || !f.bsum.alloc(8 * (L / XS_TILE + 4)) ||
+      !f.kline.alloc(8 * L) || !f.khash.alloc(8 * L) || !f.kflag.alloc(L) || !f.kbase.alloc(8 * ((size_t)nfu + 1)) ||
+      !f.kassert.alloc(4 * (size_t)nfu)) {
+    cudaGetLastError();
+    return TSM_E_NOMEM;
+  }
+  const unsigned grid = (unsigned)((L + 255) / 256), fgrid = (unsigned)(((size_t)nfu * 32 + 255) / 256);
+  unsigned long long* rank = f.rank.as<unsigned long long>();
+  k_blind_state<<<grid, 256, 0, st>>>(S.d, nfu, total, f.state.as<uint8_t>());
+  k_blind_scan<<<fgrid, 256, 0, st>>>(S.d.line_base, nfu, f.state.as<uint8_t>());
+  k_blind_lines<<<grid, 256, 0, st>>>(S.d, nfu, total, f.state.as<uint8_t>(), f.hash.as<unsigned long long>(), f.kept.as<uint32_t>());
+  xscan(f.kept.as<uint32_t>(), T, f.bsum.as<unsigned long long>(), rank, st);
+  k_blind_compact<<<grid, 256, 0, st>>>(f.kept.as<uint32_t>(), rank, f.hash.as<unsigned long long>(), S.d.line_flag, total,
+                                        f.kline.as<unsigned long long>(), f.khash.as<unsigned long long>(), f.kflag.as<uint8_t>());
+  k_blind_files<<<(unsigned)(((size_t)nfu * 32 + 32 + 255) / 256), 256, 0, st>>>(S.d.line_base, nfu, rank, f.kflag.as<uint8_t>(),
+                                                                                  f.kbase.as<unsigned long long>(), f.kassert.as<uint32_t>());
+  CU(cudaGetLastError());
+  c->launches += 8;                                      // state, scan, lines, xscan (3), compact, files
+  return TSM_OK;
+}
+
+// The section-21 classes over one side whose line records exist (S, total lines > 0): blind_front, one synchronisation that reads the kept count, then clone_classes over
 // the kept lines, with then, class_out and member_out as there (CloneDev::unit_line = the kept lines' lines).  A short kept_cap
 // still runs the grouping, so that every count is set when it returns TSM_E_CAPACITY.  ms[0]: lexing + compaction, ms[1] / ms[2]:
 // those of clone_classes.
 template <typename Then = NoThen>
 static int blind_classes(tsm_ctx* c, const HostSide& S, unsigned long long total, uint32_t min_lines, tsm_blind_result* b,
                          tsm_clone_result* out, float* ms, cudaStream_t st, Then then = {}, bool class_out = false, bool member_out = false) {
-  const uint32_t T = (uint32_t)total, nfu = (uint32_t)S.n;
+  const uint32_t nfu = (uint32_t)S.n;
   const size_t L = (size_t)total;
-  DevBuf d_state, d_hash, d_kept, d_rank, d_bsum, d_kline, d_khash, d_kflag, d_kbase, d_kassert;
-  if (!d_state.alloc(L) || !d_hash.alloc(8 * L) || !d_kept.alloc(4 * L) || !d_rank.alloc(8 * (L + 1)) || !d_bsum.alloc(8 * (L / XS_TILE + 4)) ||
-      !d_kline.alloc(8 * L) || !d_khash.alloc(8 * L) || !d_kflag.alloc(L) || !d_kbase.alloc(8 * ((size_t)nfu + 1)) ||
-      !d_kassert.alloc(4 * (size_t)nfu)) {
-    cudaGetLastError();
-    return TSM_E_NOMEM;
-  }
-  const unsigned grid = (unsigned)((L + 255) / 256), fgrid = (unsigned)(((size_t)nfu * 32 + 255) / 256);
-  unsigned long long* rank = d_rank.as<unsigned long long>();
+  BlindFront bf;
   CU(cudaEventRecord(c->diff_ev[EV_BLIND_LEX], st));
-  k_blind_state<<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>());
-  k_blind_scan<<<fgrid, 256, 0, st>>>(S.d.line_base, nfu, d_state.as<uint8_t>());
-  k_blind_lines<<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>(), d_hash.as<unsigned long long>(), d_kept.as<uint32_t>());
-  xscan(d_kept.as<uint32_t>(), T, d_bsum.as<unsigned long long>(), rank, st);
-  k_blind_compact<<<grid, 256, 0, st>>>(d_kept.as<uint32_t>(), rank, d_hash.as<unsigned long long>(), S.d.line_flag, total,
-                                        d_kline.as<unsigned long long>(), d_khash.as<unsigned long long>(), d_kflag.as<uint8_t>());
-  k_blind_files<<<(unsigned)(((size_t)nfu * 32 + 32 + 255) / 256), 256, 0, st>>>(S.d.line_base, nfu, rank, d_kflag.as<uint8_t>(),
-                                                                                  d_kbase.as<unsigned long long>(), d_kassert.as<uint32_t>());
-  CU(cudaGetLastError());
+  int rc = blind_front(c, S, bf, st);
+  if (rc != TSM_OK) return rc;
   CU(cudaEventRecord(c->diff_ev[EV_BLIND_LEX_END], st));
-  c->launches += 8;                                      // state, scan, lines, xscan (3), compact, files
   unsigned long long* pin = c->h_rb->u64;
-  CU(cudaMemcpyAsync(pin + 3, rank + L, 8, cudaMemcpyDeviceToHost, st));
-  if (b->kept_base) CU(cudaMemcpyAsync(b->kept_base, d_kbase.p, 8 * ((size_t)nfu + 1), cudaMemcpyDeviceToHost, st));
-  if (b->file_kept_assert) CU(cudaMemcpyAsync(b->file_kept_assert, d_kassert.p, 4 * (size_t)nfu, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(pin + 3, bf.rank.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
+  if (b->kept_base) CU(cudaMemcpyAsync(b->kept_base, bf.kbase.p, 8 * ((size_t)nfu + 1), cudaMemcpyDeviceToHost, st));
+  if (b->file_kept_assert) CU(cudaMemcpyAsync(b->file_kept_assert, bf.kassert.p, 4 * (size_t)nfu, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   const unsigned long long nk = pin[3];
   b->n_kept = (int64_t)nk;
   ms[0] = elapsed_ms(c->diff_ev[EV_BLIND_LEX], c->diff_ev[EV_BLIND_LEX_END]);
   const bool kept_short = b->kept_cap < (int64_t)nk && (b->kept_line || b->blind_hash);
   if (!kept_short) {
-    if (b->kept_line) CU(cudaMemcpyAsync(b->kept_line, d_kline.p, 8 * nk, cudaMemcpyDeviceToHost, st));
-    if (b->blind_hash) CU(cudaMemcpyAsync(b->blind_hash, d_khash.p, 8 * nk, cudaMemcpyDeviceToHost, st));
+    if (b->kept_line) CU(cudaMemcpyAsync(b->kept_line, bf.kline.p, 8 * nk, cudaMemcpyDeviceToHost, st));
+    if (b->blind_hash) CU(cudaMemcpyAsync(b->blind_hash, bf.khash.p, 8 * nk, cudaMemcpyDeviceToHost, st));
   }
-  int rc = TSM_OK;
-  const unsigned long long* kline = d_kline.as<unsigned long long>();
-  if (nk) rc = clone_classes<false>(c, d_khash.as<unsigned long long>(), d_kbase.as<unsigned long long>(), nfu, (uint32_t)nk,
-                                    d_kflag.as<uint8_t>(), nullptr, nullptr, nullptr, min_lines, out, ms + 1, st,
+  const unsigned long long* kline = bf.kline.as<unsigned long long>();
+  if (nk) rc = clone_classes<false>(c, bf.khash.as<unsigned long long>(), bf.kbase.as<unsigned long long>(), nfu, (uint32_t)nk,
+                                    bf.kflag.as<uint8_t>(), nullptr, nullptr, nullptr, min_lines, out, ms + 1, st,
                                     [&](CloneDev d, cudaStream_t s2) { d.unit_line = kline; return then(d, s2); }, class_out, member_out);
   CU(cudaStreamSynchronize(st));
   return rc == TSM_OK && kept_short ? TSM_E_CAPACITY : rc;
@@ -2413,6 +2430,197 @@ extern "C" int tsm_smells(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, u
 }
 
 extern "C" int tsm_smells_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_SMELL, ms4, 4); }
+
+// ------------------------------------------------------------------------------------- SPEC section 23 similar tests
+// The tests and their kept blind lines of one side whose line records (with header events) exist: the case spans and smell
+// stage of tsm_smells and blind_front, then one synchronisation for the test and kept counts; the prefix tokens, their posting
+// lists and the scan of the lists' candidate counts, then one synchronisation for the candidate total; then per chunk of
+// ST_CHUNK virtual candidates k_st_enum and k_st_verify and one synchronisation that copies the chunk's pairs out.  tests /
+// kept / pairs: host copies of the tests, their kept lines and the pairs (unordered).  ms[1..3] as tsm_similar_tests_last_ms.
+static int similar_pairs(tsm_ctx* c, const HostSide& S, uint32_t min_lines, uint32_t P, std::vector<tsm_smell_test>& tests,
+                         std::vector<uint32_t>& kept, std::vector<tsm_similar_pair>& pairs, int64_t* n_candidates, float* ms,
+                         cudaStream_t st) {
+  const size_t L = (size_t)S.total;
+  CaseSpans sp;
+  SmellBufs m;
+  BlindFront bf;
+  DevBuf d_bsum;
+  if (!d_bsum.alloc(8 * (L / XS_TILE + 4))) return TSM_E_CUDA;
+  int launches = 0;
+  CU(cudaEventRecord(c->diff_ev[EV_ST_FRONT], st));
+  int rc = case_spans(S, sp, d_bsum, launches, st);
+  if (rc == TSM_OK) rc = smell_stage(c, S, sp, d_bsum, m, launches, st);
+  if (rc == TSM_OK) rc = blind_front(c, S, bf, st);
+  if (rc != TSM_OK) return rc;
+  CU(cudaEventRecord(c->diff_ev[EV_ST_LEXED], st));
+  unsigned long long* pin = c->h_rb->u64;
+  CU(cudaMemcpyAsync(pin, m.tidx.as<unsigned long long>() + sp.n_cases, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(pin + 1, bf.rank.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  c->launches += launches;
+  const unsigned long long nt = pin[0], nk = pin[1];
+  ms[1] = elapsed_ms(c->diff_ev[EV_ST_FRONT], c->diff_ev[EV_ST_LEXED]);
+  tests.resize((size_t)nt);
+  kept.resize((size_t)nt);
+  if (nt == 0) return TSM_OK;
+  if (nk >= (1ull << 30)) return TSM_E_NOMEM;              // the token tables are indexed by u32 with a spare slot
+  const size_t NT = (size_t)nt, NK = (size_t)nk;
+  size_t slots = 1;                                        // a power of two, at least 2 x the kept lines
+  while (slots < 2 * NK) slots <<= 1;
+  const uint32_t mask = (uint32_t)(slots - 1), nl = (uint32_t)slots + 1;   // + the slot of key ST_EMPTY
+  const uint32_t nb = (nl + XS_TILE - 1) / XS_TILE;
+  DevBuf d_kbeg, d_kk, d_q, d_ktest, d_ctr, d_key, d_cnt, d_eord, d_pbase, d_tbsum, d_pkey, d_pcnt, d_tok, d_ptest, d_mbase, d_cursor,
+      d_mem, d_cbase, d_cbsum, d_surv, d_pairs, d_scratch;
+  if (!d_kbeg.alloc(4 * NT) || !d_kk.alloc(4 * NT) || !d_q.alloc(4 * NT) || !d_ktest.alloc(4 * NK) || !d_ctr.alloc(16) ||
+      !d_key.alloc(8 * (size_t)nl) || !d_cnt.alloc(4 * (size_t)nl) || !d_eord.alloc(8 * NK) || !d_pbase.alloc(8 * (NT + 1)) ||
+      !d_tbsum.alloc(8 * (NT / XS_TILE + 4)) || !d_pkey.alloc(8 * (size_t)nl) || !d_pcnt.alloc(4 * (size_t)nl) ||
+      !d_tok.alloc(sizeof(StToken) * NK) || !d_ptest.alloc(4 * NK) || !d_mbase.alloc(8 * ((size_t)nl + 1)) ||
+      !d_cursor.alloc(4 * (size_t)nl) || !d_mem.alloc(4 * NK) || !d_cbase.alloc(8 * ((size_t)nl + 1)) ||
+      !d_cbsum.alloc(8 * ((size_t)nb + 4)) || !d_surv.alloc(sizeof(uint2) * ST_CHUNK) || !d_pairs.alloc(sizeof(tsm_similar_pair) * ST_CHUNK)) {
+    cudaGetLastError();
+    return TSM_E_NOMEM;
+  }
+  uint32_t* ctr = d_ctr.as<uint32_t>();                   // kmax, survivors, pairs
+  const uint32_t* ktest = d_ktest.as<uint32_t>();
+  const unsigned long long* khash = bf.khash.as<unsigned long long>();
+  CU(cudaMemsetAsync(d_ktest.p, 0xFF, 4 * NK, st));
+  CU(cudaMemsetAsync(d_ctr.p, 0, 16, st));
+  CU(cudaMemsetAsync(d_key.p, 0xFF, 8 * (size_t)nl, st));
+  CU(cudaMemsetAsync(d_cnt.p, 0, 4 * (size_t)nl, st));
+  CU(cudaMemsetAsync(d_pkey.p, 0xFF, 8 * (size_t)nl, st));
+  CU(cudaMemsetAsync(d_pcnt.p, 0, 4 * (size_t)nl, st));
+  CU(cudaMemsetAsync(d_cursor.p, 0, 4 * (size_t)nl, st));
+  const unsigned kgrid = (unsigned)((NK + 255) / 256);
+  k_st_tests<<<(unsigned)((NT + 255) / 256), 256, 0, st>>>(m.tests.as<tsm_smell_test>(), (uint32_t)nt, S.d.line_base,
+                                                           bf.rank.as<unsigned long long>(), min_lines, P, d_kbeg.as<uint32_t>(),
+                                                           d_kk.as<uint32_t>(), d_q.as<uint32_t>(), d_ktest.as<uint32_t>(), ctr);
+  if (NK) {
+    k_st_count<<<kgrid, 256, 0, st>>>(khash, ktest, (uint32_t)nk, d_key.as<unsigned long long>(), mask, d_cnt.as<uint32_t>(), d_eord.as<uint2>());
+    k_st_order<<<kgrid, 256, 0, st>>>(ktest, (uint32_t)nk, d_cnt.as<uint32_t>(), d_eord.as<uint2>());
+  }
+  xscan(d_q.as<uint32_t>(), (uint32_t)nt, d_tbsum.as<unsigned long long>(), d_pbase.as<unsigned long long>(), st);
+  if (NK)
+    k_st_prefix<<<kgrid, 256, 0, st>>>(ktest, (uint32_t)nk, d_eord.as<uint2>(), d_kbeg.as<uint32_t>(), d_kk.as<uint32_t>(), d_q.as<uint32_t>(),
+                                       d_pbase.as<unsigned long long>(), d_pkey.as<unsigned long long>(), mask, d_pcnt.as<uint32_t>(),
+                                       d_tok.as<StToken>(), d_ptest.as<uint32_t>());
+  xscan(d_pcnt.as<uint32_t>(), nl, d_cbsum.as<unsigned long long>(), d_mbase.as<unsigned long long>(), st);
+  if (NK)
+    k_st_lists<<<kgrid, 256, 0, st>>>(d_tok.as<StToken>(), d_ptest.as<uint32_t>(), d_pbase.as<unsigned long long>() + NT,
+                                      d_mbase.as<unsigned long long>(), d_cursor.as<uint32_t>(), d_mem.as<uint32_t>());
+  k_st_csums<<<nb, 256, 0, st>>>(d_pcnt.as<uint32_t>(), nl, d_cbsum.as<unsigned long long>());
+  k_xscan_top<<<1, 256, 0, st>>>(d_cbsum.as<unsigned long long>(), nb);
+  k_st_capply<<<nb, 256, 0, st>>>(d_pcnt.as<uint32_t>(), nl, d_cbsum.as<unsigned long long>(), d_cbase.as<unsigned long long>());
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(c->diff_ev[EV_ST_LISTS], st));
+  c->launches += 10 + (NK ? 4 : 0);                       // tests, 2 x xscan (3 each), the candidate scan (3); count, order, prefix, lists
+  pin[3] = 0;
+  CU(cudaMemcpyAsync(pin + 2, d_cbase.as<unsigned long long>() + nl, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(pin + 3, ctr, 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const unsigned long long n_virtual = pin[2];
+  const uint32_t kmax = (uint32_t)pin[3];
+  ms[2] = elapsed_ms(c->diff_ev[EV_ST_LEXED], c->diff_ev[EV_ST_LISTS]);
+  // The verification's warps: V of a pattern of more than 2048 kept lines lives in a scratch slot of each warp, within 1 GiB.
+  const uint32_t W = (kmax + 63) / 64, nbk = (W + 31) / 32;
+  const uint32_t slot_words = nbk > 1 ? nbk * 32 : 0;
+  unsigned vblocks = (unsigned)c->sms * 4;
+  if (slot_words) {
+    vblocks = (unsigned)std::max<size_t>(1, std::min<size_t>(vblocks, ((size_t)1 << 27) / ((size_t)slot_words * 8)));
+    if (!d_scratch.alloc(8 * (size_t)slot_words * vblocks * 8)) { cudaGetLastError(); return TSM_E_NOMEM; }
+  }
+  const StEnum ea{d_cbase.as<unsigned long long>(), nl, d_mbase.as<unsigned long long>(), d_mem.as<uint32_t>(), d_kk.as<uint32_t>(),
+                  d_q.as<uint32_t>(), d_pbase.as<unsigned long long>(), d_tok.as<StToken>(), P, d_surv.as<uint2>(), ctr + 1};
+  int64_t ncand = 0;
+  uint32_t* cnt2 = reinterpret_cast<uint32_t*>(pin + 2);
+  for (unsigned long long c0 = 0; c0 < n_virtual; c0 += ST_CHUNK) {
+    const unsigned long long n = std::min<unsigned long long>(ST_CHUNK, n_virtual - c0);
+    CU(cudaMemsetAsync(ctr + 1, 0, 8, st));
+    CU(cudaEventRecord(c->diff_ev[EV_ST_ENUM], st));
+    k_st_enum<<<(unsigned)std::min<unsigned long long>((n + 255) / 256, (unsigned long long)c->sms * 16), 256, 0, st>>>(ea, c0, n);
+    CU(cudaEventRecord(c->diff_ev[EV_ST_VERIFY], st));
+    k_st_verify<<<vblocks, 256, 0, st>>>(d_surv.as<uint2>(), ctr + 1, d_kbeg.as<uint32_t>(), d_kk.as<uint32_t>(), khash, P,
+                                         slot_words ? d_scratch.as<unsigned long long>() : nullptr, slot_words,
+                                         d_pairs.as<tsm_similar_pair>(), ctr + 2);
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_ST_END], st));
+    CU(cudaMemcpyAsync(cnt2, ctr + 1, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    c->launches += 2;
+    ncand += cnt2[0];
+    const uint32_t np = cnt2[1];
+    ms[2] += elapsed_ms(c->diff_ev[EV_ST_ENUM], c->diff_ev[EV_ST_VERIFY]);
+    ms[3] += elapsed_ms(c->diff_ev[EV_ST_VERIFY], c->diff_ev[EV_ST_END]);
+    if (np) {
+      const size_t had = pairs.size();
+      pairs.resize(had + np);
+      CU(cudaMemcpyAsync(pairs.data() + had, d_pairs.p, sizeof(tsm_similar_pair) * np, cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+    }
+  }
+  *n_candidates = ncand;
+  CU(cudaMemcpyAsync(tests.data(), m.tests.p, sizeof(tsm_smell_test) * NT, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(kept.data(), d_kk.p, 4 * NT, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TSM_OK;
+}
+
+// The line records of the corpus with its header events (line_records), then similar_pairs; on the host the pairs are sorted
+// and the classes formed by a union-find whose roots are the smallest tests of their components.
+extern "C" int tsm_similar_tests(tsm_ctx* c, const tsm_corpus* k, int32_t min_lines, int32_t min_similarity, tsm_similar_result* out,
+                                 void* stream) {
+  if (!c || !k || !out || k->n_files < 0 || min_lines < 1 || min_similarity < 1 || min_similarity > 100 || out->test_cap < 0 ||
+      out->pair_cap < 0 || out->class_cap < 0 || out->member_cap < 0)
+    return TSM_E_ARG;
+  float* const ms = clear_ms(c, MS_SIMTEST);
+  c->launches = 0;
+  out->n_tests = out->n_pairs = out->n_classes = out->n_members = out->n_candidates = 0;
+  if (out->class_base) out->class_base[0] = 0;
+  std::vector<int64_t> line_base((size_t)k->n_files + 1);
+  std::vector<tsm_smell_test> tests;
+  std::vector<uint32_t> kept;
+  std::vector<tsm_similar_pair> pairs;
+  int64_t n_lines = 0, n_candidates = 0;
+  int rc = line_records(c, k, true, line_base.data(), INT64_MAX, &n_lines, stream, [&](const HostSide& S, unsigned long long, cudaStream_t st) -> int {
+    return similar_pairs(c, S, (uint32_t)min_lines, (uint32_t)min_similarity, tests, kept, pairs, &n_candidates, ms, st);
+  }, &ms[0], TSM_SCAN_HEADER_EVENTS);
+  if (rc != TSM_OK) return rc;
+  std::sort(pairs.begin(), pairs.end(), [](const tsm_similar_pair& x, const tsm_similar_pair& y) { return x.a != y.a ? x.a < y.a : x.b < y.b; });
+  const size_t nt = tests.size();
+  std::vector<int32_t> root(nt);
+  std::vector<uint8_t> linked(nt, 0);
+  for (size_t t = 0; t < nt; ++t) root[t] = (int32_t)t;
+  auto find = [&](int32_t x) { while (root[(size_t)x] != x) x = root[(size_t)x] = root[(size_t)root[(size_t)x]]; return x; };
+  for (const tsm_similar_pair& p : pairs) {
+    const int32_t ra = find(p.a), rb = find(p.b);
+    if (ra != rb) root[(size_t)std::max(ra, rb)] = std::min(ra, rb);
+    linked[(size_t)p.a] = linked[(size_t)p.b] = 1;
+  }
+  std::vector<int64_t> class_of(nt, -1), base(1, 0);      // classes in order of their roots, the smallest members
+  for (size_t t = 0; t < nt; ++t)
+    if (linked[t] && find((int32_t)t) == (int32_t)t) { class_of[t] = (int64_t)base.size() - 1; base.push_back(0); }
+  for (size_t t = 0; t < nt; ++t) if (linked[t]) ++base[(size_t)class_of[(size_t)find((int32_t)t)] + 1];
+  for (size_t i = 1; i < base.size(); ++i) base[i] += base[i - 1];
+  const int64_t nc = (int64_t)base.size() - 1, nm = base.back();
+  out->n_tests = (int64_t)nt;
+  out->n_pairs = (int64_t)pairs.size();
+  out->n_classes = nc;
+  out->n_members = nm;
+  out->n_candidates = n_candidates;
+  if (((out->tests || out->test_kept) && out->test_cap < (int64_t)nt) || (out->pairs && out->pair_cap < out->n_pairs) ||
+      (out->class_base && out->class_cap < nc) || (out->member && out->member_cap < nm))
+    return TSM_E_CAPACITY;
+  if (out->tests) std::copy(tests.begin(), tests.end(), out->tests);
+  if (out->test_kept) std::copy(kept.begin(), kept.end(), out->test_kept);
+  if (out->pairs) std::copy(pairs.begin(), pairs.end(), out->pairs);
+  if (out->class_base) std::copy(base.begin(), base.end(), out->class_base);
+  if (out->member) {
+    std::vector<int64_t> cur(base.begin(), base.end() - 1);
+    for (size_t t = 0; t < nt; ++t) if (linked[t]) out->member[cur[(size_t)class_of[(size_t)find((int32_t)t)]]++] = (int32_t)t;
+  }
+  return TSM_OK;
+}
+
+extern "C" int tsm_similar_tests_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_SIMTEST, ms4, 4); }
 
 // ------------------------------------------------------------------------------------- SPEC section 19 test-smell churn
 // The line records of both sides with their header events, per side the case spans and the smell stage, one synchronisation

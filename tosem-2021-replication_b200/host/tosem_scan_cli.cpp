@@ -2470,6 +2470,126 @@ static int cmd_smells(const std::vector<std::string>& roots, const std::string& 
   return 0;
 }
 
+// Similar tests (docs/SPEC.md section 23): ONE tsm_similar_tests call over every selected file (pairs cross roots).  stdout: per
+// root its files, tests, compared tests, tests in a pair, and the pairs and classes with a member in it, and an <all> row;
+// --out: one row per pair in (a, b) order; --classes: one row per class member.  Lines are 1-based header lines; a test is named
+// by its section-10 case name.
+static int cmd_similar_tests(const std::vector<std::string>& roots, const std::string& git_repo, const std::string& rev, int min_lines,
+                             int similarity, bool all_files, const std::string& out_path, const std::string& classes_path) {
+  std::vector<FileEntry> files;
+  std::vector<std::string> names;
+  if (!git_repo.empty()) {
+    gitstore::Store gs;
+    std::string err;
+    if (!gs.open(git_repo, err)) die(err);
+    gitstore::Oid id; gitstore::Commit cm;
+    if (!gs.resolve(rev, id) || !gs.commit(id, cm)) die("cannot resolve revision " + rev);
+    walk_git(gs, cm.tree, "", all_files, files);
+    names.push_back(repo_name(git_repo));
+  } else {
+    for (size_t g = 0; g < roots.size(); ++g) { walk(roots[g], (int)g, all_files, files); names.push_back(repo_name(roots[g])); }
+  }
+  fprintf(stderr, "tosem-scan: %zu files selected under %zu root(s)\n", files.size(), names.size());
+  std::vector<Batch> batches = plan_batches(files, all_of(files), (1ll << 31) - 4097, INT32_MAX);
+  int64_t need = 4096;
+  for (const Batch& b : batches) need += b.bytes;
+  if (batches.size() > 1 || need >= (1ll << 31))
+    die("the selected files (" + std::to_string(need) + " bytes of arena) do not fit one int32-indexed arena; similar tests are "
+        "found across all files at once, so select fewer files");
+  const size_t ng = names.size();
+  std::vector<std::vector<int64_t>> tot(ng + 1, std::vector<int64_t>(6, 0));   // files, tests, compared, similar, pairs, classes
+  std::ofstream os, oc;
+  if (!out_path.empty()) {
+    os.open(out_path, std::ios::binary);
+    csv_row(os, {"repository", "fileName", "test", "line", "otherRepository", "otherFileName", "otherTest", "otherLine", "keptLines",
+                 "otherKeptLines", "lcs", "similarity"});
+  }
+  if (!classes_path.empty()) {
+    oc.open(classes_path, std::ios::binary);
+    csv_row(oc, {"class", "repository", "fileName", "test", "line", "last_line", "keptLines"});
+  }
+  scan_batches(files, batches, 0, (int32_t)ng, TSM_SCAN_HEADER_EVENTS, [&](const Batch& B, const Scanned& s) {
+    const int32_t nf = (int32_t)B.count();
+    const tsm_corpus c = B.corpus((int32_t)ng);
+    // A test starts at a header event, so the tests, the members (<= tests) and the classes (<= tests / 2) fit these arrays; the
+    // pairs are a guess, and a second call (which redoes all the work) sizes them only when it is short.
+    const int64_t cap_t = (int64_t)s.hev.size();
+    std::vector<tsm_smell_test> tests((size_t)std::max<int64_t>(cap_t, 1));
+    std::vector<uint32_t> kept(tests.size());
+    std::vector<int64_t> cbase((size_t)cap_t + 1);
+    std::vector<int32_t> member(tests.size());
+    std::vector<tsm_similar_pair> pairs((size_t)std::max<int64_t>(4 * cap_t, 1 << 16));
+    tsm_similar_result r{tests.data(), kept.data(), cap_t, 0, pairs.data(), (int64_t)pairs.size(), 0, cbase.data(), cap_t, 0,
+                         member.data(), cap_t, 0, 0};
+    int rc = tsm_similar_tests(s.ctx, &c, min_lines, similarity, &r, nullptr);
+    if (rc == TSM_E_CAPACITY && r.n_pairs > r.pair_cap) {
+      pairs.resize((size_t)r.n_pairs);
+      r.pairs = pairs.data(); r.pair_cap = r.n_pairs;
+      rc = tsm_similar_tests(s.ctx, &c, min_lines, similarity, &r, nullptr);
+    }
+    ck(rc, "tsm_similar_tests");
+    const int64_t nt = r.n_tests;
+    std::vector<std::string> tname((size_t)nt);             // the case name of every test
+    int32_t at_file = -1;
+    std::vector<uint32_t> start;
+    for (int64_t t = 0; t < nt; ++t) {
+      const tsm_smell_test& x = tests[(size_t)t];
+      const uint8_t* p = B.arena.get() + B.off[(size_t)x.file];
+      const uint32_t len = (uint32_t)B.len[(size_t)x.file];
+      if (at_file != x.file) {
+        at_file = x.file; start.assign(1, 0);
+        for (uint32_t q = 0; q < len; ++q) if (p[q] == '\n') start.push_back(q + 1);
+      }
+      const uint32_t e = (size_t)x.line + 1 < start.size() ? start[(size_t)x.line + 1] - 1 : len;
+      tname[(size_t)t] = case_name(files[B.idx[(size_t)x.file]].ext, p + start[(size_t)x.line], e - start[(size_t)x.line]);
+    }
+    auto grp = [&](int64_t t) { return (size_t)files[B.idx[(size_t)tests[(size_t)t].file]].grp; };
+    for (int32_t i = 0; i < nf; ++i) { tot[(size_t)files[B.idx[(size_t)i]].grp][0]++; tot[ng][0]++; }
+    std::vector<uint8_t> linked((size_t)nt, 0);
+    for (int64_t j = 0; j < r.n_members; ++j) linked[(size_t)member[(size_t)j]] = 1;
+    for (int64_t t = 0; t < nt; ++t)
+      for (size_t g : {grp(t), ng}) {
+        tot[g][1]++;
+        tot[g][2] += kept[(size_t)t] >= (uint32_t)min_lines;
+        tot[g][3] += linked[(size_t)t];
+      }
+    for (int64_t k = 0; k < r.n_pairs; ++k) {
+      const tsm_similar_pair& q = pairs[(size_t)k];
+      const size_t ga = grp(q.a), gb = grp(q.b);
+      tot[ga][4]++;
+      if (gb != ga) tot[gb][4]++;
+      tot[ng][4]++;
+      if (!os.is_open()) continue;
+      const tsm_smell_test &ta = tests[(size_t)q.a], &tb = tests[(size_t)q.b];
+      csv_row(os, {names[ga], files[B.idx[(size_t)ta.file]].rel, tname[(size_t)q.a], std::to_string(ta.line + 1), names[gb],
+                   files[B.idx[(size_t)tb.file]].rel, tname[(size_t)q.b], std::to_string(tb.line + 1), std::to_string(kept[(size_t)q.a]),
+                   std::to_string(kept[(size_t)q.b]), std::to_string(q.lcs), std::to_string(q.score / 600)});
+    }
+    tot[ng][5] = r.n_classes;
+    for (int64_t k = 0; k < r.n_classes; ++k) {
+      std::vector<uint8_t> seen(ng, 0);
+      for (int64_t j = cbase[(size_t)k]; j < cbase[(size_t)k + 1]; ++j) {
+        const int32_t t = member[(size_t)j];
+        const size_t g = grp(t);
+        if (!seen[g]) { seen[g] = 1; tot[g][5]++; }
+        if (!oc.is_open()) continue;
+        const tsm_smell_test& x = tests[(size_t)t];
+        csv_row(oc, {std::to_string(k + 1), names[g], files[B.idx[(size_t)x.file]].rel, tname[(size_t)t], std::to_string(x.line + 1),
+                     std::to_string(x.line + x.body_lines), std::to_string(kept[(size_t)t])});
+      }
+    }
+  });
+  std::ostringstream so;
+  csv_row(so, {"repository", "files", "tests", "compared_tests", "similar_tests", "pairs", "classes"});
+  for (size_t g = 0; g <= ng; ++g) {
+    std::vector<std::string> row = {g < ng ? names[g] : "<all>"};
+    for (int64_t v : tot[g]) row.push_back(std::to_string(v));
+    csv_row(so, row);
+  }
+  fputs(so.str().c_str(), stdout);
+  return 0;
+}
+
 static void usage() {
   fprintf(stderr,
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
@@ -2487,7 +2607,12 @@ static void usage() {
           "       tosem-scan clones --git <repository> [--rev R] [--min-lines N] [--blind] [--all-files] [--out F]\n"
           "       tosem-scan smells <project-root>... [--all-files] [--batch-bytes N] [--out F]\n"
           "       tosem-scan smells --git <repository> [--rev R] [--all-files] [--batch-bytes N] [--out F]\n"
+          "       tosem-scan similar-tests <project-root>... | --git <repository> [--rev R] [--min-lines N] [--similarity P] [--all-files]\n"
+          "                                [--out F] [--classes F]\n"
           "smells: per root the tests with each of nine test smells; --out F: one row per instance line (docs/SPEC.md section 18).\n"
+          "similar-tests: pairs of tests whose kept blind lines are at least P %% alike (LCS, default 70) and their classes, over\n"
+          "               tests of at least N kept lines (default 5); --out F: one row per pair; --classes F: one row per class member\n"
+          "               (docs/SPEC.md section 23).\n"
           "--blind (clones): near-miss copies - lines compared with identifiers, literals, whitespace and comments blinded, over the\n"
           "                  lines that keep a token (docs/SPEC.md section 21).\n"
           "--find-renames N (0..100): pair deleted and added files at least N %% similar, as git -M<N>%% does (docs/SPEC.md section 13).\n"
@@ -2536,6 +2661,15 @@ int main(int argc, char** argv) {
   if (cmd == "smells") {
     if (pos.empty() == !opt.count("--git")) die("smells needs project roots or --git <repository>, not both");
     return cmd_smells(pos, opt["--git"], opt.count("--rev") ? opt["--rev"] : "HEAD", all_files, opt["--out"], batch_bytes(kBatch, 1));
+  }
+  if (cmd == "similar-tests") {
+    if (pos.empty() == !opt.count("--git")) die("similar-tests needs project roots or --git <repository>, not both");
+    const long n = opt.count("--min-lines") ? strtol(opt["--min-lines"].c_str(), nullptr, 10) : 5;
+    if (n < 1 || n > INT32_MAX) die("--min-lines needs a number of lines of at least 1");
+    const long p = opt.count("--similarity") ? strtol(opt["--similarity"].c_str(), nullptr, 10) : 70;
+    if (p < 1 || p > 100) die("--similarity needs a percentage from 1 to 100");
+    return cmd_similar_tests(pos, opt["--git"], opt.count("--rev") ? opt["--rev"] : "HEAD", (int)n, (int)p, all_files, opt["--out"],
+                             opt["--classes"]);
   }
   if (cmd == "body") { if (pos.empty()) die("body needs at least one project root"); return cmd_body(pos, opt["--out"], batch_bytes(kBatch, 1)); }
   int rename_pct = -1;                                     // --find-renames N (docs/SPEC.md section 13); -1 = off

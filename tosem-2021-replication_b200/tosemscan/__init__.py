@@ -39,6 +39,8 @@ SMELLS = ["empty", "assertion_free", "duplicate_assert", "redundant_assert", "co
 TEST_CHURN = np.dtype([("case_idx", "<i4"), ("instances", "<i4", (9,)), ("churned", "<i4", (9,))])   # tsm_test_churn (section 19)
 MOVE_BLOCK = np.dtype([("line", "<i8"), ("partner", "<i8"), ("n_lines", "<i4"),
                        ("n_assert", "<i4")])   # tsm_move_block: one moved block of one side (docs/SPEC.md section 20)
+SIMILAR_PAIR = np.dtype([("a", "<i4"), ("b", "<i4"), ("lcs", "<u4"),
+                         ("score", "<u4")])   # tsm_similar_pair: two similar tests, a < b (docs/SPEC.md section 23)
 ASSERT_EDIT = np.dtype([("rev", "<i8"), ("aev", "<i8"), ("score", "<i4"), ("_pad", "<i4")])   # tsm_assert_edit: event indices
 
 # every symbol include/tosemscan.h declares (tests check the library exports exactly these)
@@ -50,7 +52,7 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_diff_pairs_marks", "tsm_blame_pairs", "tsm_blame_last_ms", "tsm_clones", "tsm_clones_last_ms",
            "tsm_diff_pairs_cases", "tsm_diff_pairs_assert_edits", "tsm_assert_edits_last_ms", "tsm_smells", "tsm_smells_last_ms",
            "tsm_diff_pairs_smells", "tsm_diff_smells_last_ms", "tsm_diff_pairs_moves", "tsm_moves_last_ms", "tsm_clones_blind",
-           "tsm_clones_blind_last_ms", "tsm_clone_churn", "tsm_clone_churn_last_ms"]
+           "tsm_clones_blind_last_ms", "tsm_clone_churn", "tsm_clone_churn_last_ms", "tsm_similar_tests", "tsm_similar_tests_last_ms"]
 FRAG_STATES = ["kept", "edited", "whole"]          # tsm_clone_churn state[j] (docs/SPEC.md section 22)
 CLONE_STATUSES = ["untouched", "changed", "removed", "diverged", "dropped", "created", "copied", "joined"]   # status[c]
 
@@ -111,6 +113,13 @@ class _CloneResult(C.Structure):
 class _BlindResult(C.Structure):
     _fields_ = [("kept_base", C.c_void_p), ("kept_line", C.c_void_p), ("blind_hash", C.c_void_p), ("file_kept_assert", C.c_void_p),
                 ("kept_cap", C.c_int64), ("n_kept", C.c_int64)]
+
+
+class _SimilarResult(C.Structure):
+    _fields_ = [("tests", C.c_void_p), ("test_kept", C.c_void_p), ("test_cap", C.c_int64), ("n_tests", C.c_int64),
+                ("pairs", C.c_void_p), ("pair_cap", C.c_int64), ("n_pairs", C.c_int64),
+                ("class_base", C.c_void_p), ("class_cap", C.c_int64), ("n_classes", C.c_int64),
+                ("member", C.c_void_p), ("member_cap", C.c_int64), ("n_members", C.c_int64), ("n_candidates", C.c_int64)]
 
 
 class _CloneChurnSide(C.Structure):
@@ -229,6 +238,10 @@ def lib():
         L.tsm_smells.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
                                  C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p]
         L.tsm_smells_last_ms.restype = C.c_int
+        L.tsm_similar_tests.restype = C.c_int
+        L.tsm_similar_tests.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_int32, C.c_int32, C.POINTER(_SimilarResult), C.c_void_p]
+        L.tsm_similar_tests_last_ms.restype = C.c_int
+        L.tsm_similar_tests_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
         L.tsm_smells_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
         L.tsm_diff_pairs_smells.restype = C.c_int
         L.tsm_diff_pairs_smells.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 3 + \
@@ -979,6 +992,42 @@ class Scanner:
         k_move_starts + k_move_runs + k_move_mark] in ms."""
         ms = (C.c_float * 4)()
         lib().tsm_moves_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
+
+    def similar_tests(self, corpus, min_lines=5, similarity=70, stream=None, cap=None):
+        """Similar tests (docs/SPEC.md section 23): a dict of numpy arrays tests[n_tests] (SMELL_TEST, as smells() gives them),
+        test_kept[n_tests] (kept blind lines of each test), pairs[n_pairs] (SIMILAR_PAIR, ascending (a, b)), class_base[n_classes+1]
+        and member[n_members] (test indices), and n_candidates (the pairs whose LCS was computed).  Arrays too small for their
+        counts are sized from the counts and the call is made again, which repeats the whole all-pairs work.  By default the tests,
+        members and classes are sized from the corpus' line count (a test starts on a line), so only more pairs than that guess
+        (at least 2^16, at most 2^22) cause a second call; cap: the first guess of every array instead."""
+        cs = corpus.c_struct()
+        if cap is None:
+            lines = int(np.count_nonzero(np.asarray(corpus.arena[:int(corpus.off[corpus.n_files])]) == 0x0A)) + corpus.n_files
+            ct = cc = cm = lines
+            cp = min(max(4 * lines, 1 << 16), 1 << 22)
+        else:
+            ct = cp = cc = cm = int(cap)
+        for _ in range(2):
+            tests, kept = np.zeros(max(ct, 1), SMELL_TEST), np.zeros(max(ct, 1), np.uint32)
+            pairs = np.zeros(max(cp, 1), SIMILAR_PAIR)
+            cbase, member = np.zeros(cc + 1, np.int64), np.zeros(max(cm, 1), np.int32)
+            r = _SimilarResult(_p(tests), _p(kept), ct, 0, _p(pairs), cp, 0, _p(cbase), cc, 0, _p(member), cm, 0, 0)
+            rc = lib().tsm_similar_tests(self._ctx, C.byref(cs), int(min_lines), int(similarity), C.byref(r), stream)
+            if rc == TSM_E_CAPACITY and (r.n_tests > ct or r.n_pairs > cp or r.n_classes > cc or r.n_members > cm):
+                ct, cp, cc, cm = int(r.n_tests), int(r.n_pairs), int(r.n_classes), int(r.n_members)
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_similar_tests")
+            return {"tests": tests[:r.n_tests], "test_kept": kept[:r.n_tests], "pairs": pairs[:r.n_pairs],
+                    "class_base": cbase[:r.n_classes + 1], "member": member[:r.n_members], "n_candidates": int(r.n_candidates)}
+        raise TsmError(TSM_E_CAPACITY, "tsm_similar_tests")
+
+    def similar_tests_last_ms(self):
+        """Device time of the last similar_tests call: [k_scan, case spans + smell stage + lexer, tokens + posting lists +
+        enumeration, verification] in ms."""
+        ms = (C.c_float * 4)()
+        lib().tsm_similar_tests_last_ms(self._ctx, C.byref(ms))
         return [float(x) for x in ms]
 
     def smells_last_ms(self):
