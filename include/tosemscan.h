@@ -401,6 +401,9 @@ int tsm_smells_last_ms(tsm_ctx* ctx, float* ms4);
  *                      their smallest test, members ascending: class c is member[class_base[c] .. class_base[c+1])
  *                      (class_base holds class_cap + 1 entries, member member_cap)
  *   n_candidates       the candidate pairs whose LCS was computed (those that pass the exact prefix and size filters)
+ *                      (a count of work, not of the answer: lines of equal counts are ordered by their slot in a hash table
+ *                      filled by atomics, so the prefixes, and with them this count, may differ from call to call; the
+ *                      pairs do not)
  * Any output pointer may be NULL (it is skipped); every count is always set.  A short cap for a given output returns
  * TSM_E_CAPACITY with every count set: size the arrays and call again.  n_files = 0 is legal.  Memory errors as for tsm_clones.
  * Kernels: k_scan with the header events, the case spans and smell stage of tsm_smells, the lexer of tsm_clones_blind; then

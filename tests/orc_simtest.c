@@ -67,3 +67,14 @@ int64_t orc_similar_row(const uint64_t* seq, const int64_t* beg, const uint32_t*
   free(row);
   return m;
 }
+
+/* The LCS of n pairs: out[i] = lcs(seq of a[i], seq of b[i]).  Returns -1 on no memory. */
+int orc_lcs_pairs(const uint64_t* seq, const int64_t* beg, const uint32_t* k, const int32_t* a, const int32_t* b, int64_t n, uint32_t* out) {
+  uint32_t kmax = 0;
+  for (int64_t i = 0; i < n; ++i) if (k[b[i]] > kmax) kmax = k[b[i]];
+  uint32_t* row = malloc(sizeof(uint32_t) * ((size_t)kmax + 1));
+  if (!row) return -1;
+  for (int64_t i = 0; i < n; ++i) out[i] = lcs_of(seq + beg[a[i]], k[a[i]], seq + beg[b[i]], k[b[i]], row);
+  free(row);
+  return 0;
+}

@@ -34,6 +34,7 @@ import orc_cases
 import orc_clones
 import orc_marks
 import orc_similarity
+import simtest_ref
 import tosemscan as ts
 from test_gpu_blame import chain_order, chains, ref_blame, reordered, same_origins
 from test_gpu_slabs import check, expected_slabs
@@ -359,6 +360,18 @@ def a_case(name):
             orc_clones.assert_equal(r, orc_clones.clones(x, 5))
             assert len(r["class_len"]) > 100 and (np.diff(r["class_base"]) > 32).any()
         return sc, lambda x, st: sc.clones(x, 5, stream=st), c, twin, chk
+    if name == "similar_tests":
+        c, twin = line_corpora()
+        sc = ts.Scanner(0, 1 << 20, 16, 4)
+
+        def call(x, st):                                    # n_candidates is left out: it may differ from call to call
+            r = sc.similar_tests(x, 3, 60, stream=st)
+            return {k: r[k] for k in ("tests", "test_kept", "pairs", "class_base", "member")}
+
+        def chk(r, x):
+            simtest_ref.assert_equal(r, simtest_ref.reference(x, 3, 60))
+            assert len(r["pairs"]) > 1000 and len(r["class_base"]) > 40
+        return sc, call, c, twin, chk
     if name in ("line_hashes", "statements"):
         c, twin = line_corpora()
         sc = ts.Scanner(0, 1 << 20, 16, 4)
@@ -374,7 +387,7 @@ def a_case(name):
 
 A_CASES = ["scan-small-revA", "scan-small-revB", "scan-streamed-revA", "scan-streamed-revB", "resident", "diff_pairs",
            "diff_pairs_detail", "diff_pairs_asserts", "diff_resident", "diff_resident_asserts", "diff_pairs_marks",
-           "diff_assert_edits", "diff_cases", "blame_pairs", "similarity", "clones", "line_hashes", "statements", "reduce"]
+           "diff_assert_edits", "diff_cases", "blame_pairs", "similarity", "clones", "similar_tests", "line_hashes", "statements", "reduce"]
 
 
 @pytest.mark.parametrize("name", A_CASES)

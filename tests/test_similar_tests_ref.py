@@ -1,6 +1,7 @@
 """The similar tests of docs/SPEC.md section 23 on the CPU: the worked example, thresholds and edge cases with known answers, the
 plain-Python and serial C references against each other, and the model of the device's prefix filter against brute force."""
 import random
+from collections import Counter
 
 import numpy as np
 import pytest
@@ -161,3 +162,86 @@ def test_prefix_filter_model_on_planted_corpora():
         for P in (1, 30, 70, 99, 100):
             want = sr.c_similar(seqs, 2, P)
             assert {(a, b) for a, b, *_ in want} <= sr.prefix_candidates(seqs, 2, P)
+
+
+# ---------------------------------------------------------------------------------------------- builders of the GPU seams module
+def test_punct_lines_have_distinct_blind_forms():
+    import blind_ref as br
+    import spec_ref
+    data = "".join("    %s\n" % sr.punct(n) for n in range(20000)).encode()
+    forms = br.blind_lines(data, 1)
+    assert forms == [b"I " + b" I ".join(c.encode() for c in sr.punct(n)[1::2]) + b" I" for n in range(20000)]
+    hashes = {spec_ref.py_bytes_hash(b"I " + b" I ".join(c.encode() for c in sr.punct(n)[1::2]) + b" I") for n in range(1 << 19)}
+    assert len(hashes) == 1 << 19                          # every id the builders use has a line hash of its own
+    assert not set(sr.punct(8 ** 6 - 1)) & set("#'\"0123456789") and len(sr.punct(8 ** 6)) == 15
+    _, seqs = sr.py_sequences([sr.py_file([[0, 1, 2], [], [2, 1]])], [1])
+    assert [len(s) for s in seqs] == [4, 1, 3] and seqs[0][0] == seqs[1][0] == seqs[2][0]
+    assert seqs[2][1:] == [seqs[0][3], seqs[0][2]]
+
+
+def seqs_of(seqs):
+    """The sequences of py_file(seqs), through the plain-Python references."""
+    return sr.py_sequences([sr.py_file(seqs)], [1])[1]
+
+
+def test_tight_cases_keep_their_pairs_only_with_the_exact_prefix():
+    eq = 0
+    for P in range(1, 101):
+        s, cases = sr.tight_cases(P)
+        full = seqs_of(s)
+        cand, short = sr.prefix_candidates(full, 1, P), sr.prefix_candidates(full, 1, P, short=1)
+        for a, b, b2, e in cases:
+            ka, kb = len(full[a]), len(full[b])
+            assert kb == sr.alpha(P, ka) and sr.lcs(full[a], full[b]) == kb
+            assert (min(a, b), max(a, b)) in cand and (min(a, b), max(a, b)) not in short
+            assert b2 is None or 200 * len(full[b2]) < P * (ka + len(full[b2]))
+            assert e == (200 * kb == P * (ka + kb))
+            eq += e
+    assert eq >= 30
+
+
+def test_repeat_cases_end_the_prefix_inside_the_run():
+    for P in (40, 60, 80):
+        s, cases = sr.repeat_cases(P)
+        full = seqs_of(s)
+        cnt = Counter(h for x in full for h in x)
+        R = full[cases[0][1]][1]
+        assert cnt[R] < cnt[full[0][0]]                    # rarer than the header, common in the corpus
+        cand, short = sr.prefix_candidates(full, 1, P), sr.prefix_candidates(full, 1, P, short=1)
+        for a, b, c, c2 in cases:
+            ka, kb = len(full[a]), len(full[b])
+            assert kb == sr.alpha(P, ka) == c2 + 1 and sr.lcs(full[a], full[b]) == kb
+            pref = sorted(sr.tokens(full[a]), key=lambda t: (cnt[t[0]], t[0], t[1]))[:ka - kb + 1]
+            assert pref[-1] == (R, c - c2)                 # the prefix ends on R's (c - c2)-th repeat
+            assert (a, b) in cand and ((a, b) in short) == (c2 < c)
+
+
+@pytest.mark.parametrize("n", [999, 2099])
+def test_copies_closed_form(n):
+    s, sets = sr.copies(n, 120, 90, n)
+    want = sr.copies_pairs(n, sets, 90)
+    full = seqs_of(s[:10])
+    assert [len(x) for x in full] == [n + 1] * 10
+    assert sr.c_similar(full, 1, 90) == [p for p in want if p[1] < 10]
+    T = (n + 1) // 10
+    u = [len(sets[a] | sets[b]) for a in range(120) for b in range(a + 1, 120)]
+    assert u.count(T) > 50 and u.count(T + 1) > 50
+
+
+def test_generated_and_filler():
+    c, planted = sr.generated(5, 3000)
+    tests, seqs = sr.c_sequences(c)
+    assert len(seqs) == 3000 and len(planted) == 300 and all(x % 10 == 9 and y < x for x, y in planted)
+    k = [len(x) for x in seqs]
+    l = sr.c_lcs_pairs(seqs, [y for _, y in planted], [x for x, _ in planted])
+    assert l.tolist() == [sr.lcs(seqs[y], seqs[x]) for x, y in planted]
+    assert sum(sr.passes(int(v), k[x], k[y], 70) for v, (x, y) in zip(l, planted)) > 150
+    flat = sr.flatten(seqs)
+    for a in (0, 9, 2999):
+        assert sr.c_partners(flat, a, 5, 70) == sr.c_partners(seqs, a, 5, 70)
+    import tosemscan as ts
+    fill = sr.filler(300, 0, per_file=50)
+    _, fs = sr.c_sequences(ts.pack(fill, np.ones(len(fill), np.uint8)))
+    assert len(fs) == 300 and len({h for x in fs for h in x[1:]}) == sum(len(x) - 1 for x in fs)
+    assert not {h for x in fs for h in x[1:]} & {h for x in seqs for h in x}
+    assert {x[0] for x in fs} == {x[0] for x in seqs}

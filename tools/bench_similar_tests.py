@@ -33,39 +33,6 @@ import tosemscan as ts  # noqa: E402
 from bench_diff_asserts import card  # noqa: E402
 
 
-def shape(v):
-    return "x" + "".join("[x]" if (v >> b) & 1 else "(x)" for b in range(16))
-
-
-def generated(seed, n_tests):
-    rng = np.random.default_rng(seed)
-    shapes = [shape(v) for v in range(1 << 16)]
-    klen = rng.integers(4, 21, n_tests)
-    common = rng.random(int(klen.sum())) < 0.2
-    ids = np.where(common, rng.integers(0, 16, common.size), rng.integers(16, 1 << 16, common.size))
-    bodies, at = [], 0
-    prng = random.Random(seed)
-    for t in range(n_tests):
-        b = ids[at:at + klen[t]].tolist()
-        at += klen[t]
-        if t % 10 == 9:
-            b = list(bodies[prng.randrange(t)])
-            for _ in range(prng.randint(1, 2)):
-                r = prng.random()
-                if r < 0.33 and len(b) > 1:
-                    b.pop(prng.randrange(len(b)))
-                elif r < 0.66:
-                    b.insert(prng.randrange(len(b) + 1), prng.randrange(16, 1 << 16))
-                else:
-                    b[prng.randrange(len(b))] = prng.randrange(16, 1 << 16)
-        bodies.append(b)
-    files = []
-    for f in range(0, n_tests, 100):
-        files.append("".join("def test_%d():\n%s" % (t, "".join("    %s\n" % shapes[v] for v in bodies[t]))
-                             for t in range(f, min(f + 100, n_tests))).encode())
-    return ts.pack(files, np.ones(len(files), np.uint8), pinned=True)
-
-
 def prefix_lists(seqs, min_lines, P):
     """Posting-list lengths of the prefix tokens (the filter model, vectorised) and the candidates they span."""
     k = np.array([len(s) for s in seqs], np.int64)
@@ -131,7 +98,7 @@ def main():
     print(json.dumps({"metric": "tsm_similar_tests over the C1 test files", "unit": "ms", "workload": "C1", "files": c.n_files,
                       "min_lines": 5, "similarity": 70, "steps": args.steps, "warmup": args.warmup, **out,
                       "prefix_model": prefix_lists(seqs, 5, 70), "equal_to_cpu_reference": True, "gpu": gpu}), flush=True)
-    c = generated(0x53494D54, args.tests)
+    c, _ = sr.generated(0x53494D54, args.tests, pinned=True)
     r, out = run(sc, c, 5, 70, args.steps, args.warmup)
     _, seqs = sr.c_sequences(c)
     k = [len(s) for s in seqs]
