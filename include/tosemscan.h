@@ -425,6 +425,49 @@ int tsm_similar_tests(tsm_ctx* ctx, const tsm_corpus* corpus, int32_t min_lines,
                       void* stream);
 int tsm_similar_tests_last_ms(tsm_ctx* ctx, float* ms4);
 
+/* Similar-test churn along a revision history (docs/SPEC.md section 24): the pairs of similar tests (section 23, at min_lines
+ * and P = min_similarity) that a step creates, changes or breaks up.  old_rev / new_rev and the pairs are those of
+ * tsm_clone_churn (n_files = 0 is legal, the marks are those of tsm_diff_pairs_marks); the k-th file of old_rev in no pair is the
+ * k-th such file of new_rev and is unchanged.  Within a pair, tests are matched through the section-16 matching of their
+ * cases (kept header line, then a name unique among the unmatched cases of both sides); in an unchanged file test i is test i.
+ * Per side (old_side: old_rev, new_side: new_rev), test_cap entries each:
+ *   tests, test_kept  every test of that revision alone and its kept lines, exactly as tsm_similar_tests gives them
+ *   match             the other side's test, or -1
+ *   change            'A' (new, no old test), 'D' (old, no new test), '=' (matched; no marked line in either body, equal
+ *                     body_lines and equal sequences) or 'M' (any other matched test)
+ *   n_candidates      the candidate pairs of that side whose LCS was computed (a count of work, as in tsm_similar_tests)
+ * events[n_events]: one {status, old_a, old_b, a, b, old_lcs, old_score, lcs, score} per pair of either side that has a test
+ * other than '=', with the first status that holds:
+ *   TSM_SIMILAR_CHANGED    a pair of old_rev whose tests map to a pair of new_rev (one of them 'M')
+ *   TSM_SIMILAR_REMOVED / DROPPED / DIVERGED    a pair of old_rev that is no pair of new_rev: both tests 'D' / one / none
+ *   TSM_SIMILAR_CREATED / COPIED / CONVERGED    a pair of new_rev that is no image of a pair of old_rev: both 'A' / one / none
+ * old_a < old_b for old-side events (removed, dropped, diverged), a < b for the others; the other side's tests are their
+ * matches (-1 when absent).  lcs / score (section 23's score) of each side that has both tests, even below P or for tests no
+ * longer compared; UINT32_MAX for a side that lacks one.  Old-side events come first, ascending (old_a, old_b), then the
+ * others, ascending (a, b).  Any output pointer may be NULL (it is skipped); every count is always set.  A short test_cap (for
+ * a given output) or event_cap returns TSM_E_CAPACITY with every count set.  TSM_E_ARG for a file index out of range, a file in
+ * two pairs of one side, a pair (-1, -1), min_lines < 1, P outside 1..100, unpaired file counts that differ, or an unpaired
+ * file whose length (or test count) differs from its counterpart's.  n_pairs = 0 is legal.
+ * Kernels: k_scan over both revisions, the marks of tsm_clone_churn (k_churn_gather, the diff, k_churn_marks), per revision the
+ * front of tsm_similar_tests; k_sc_change (one warp per matched test); per revision the tokens of tsm_similar_tests, posting
+ * lists with their dirty tests (not '=') first (k_sc_dirty, k_sc_lists), and a candidate space of only the pairs with a dirty
+ * test (k_sc_csums, k_sc_capply, k_sc_enum), verified by k_st_verify; then k_st_verify at P = 0 for the cross scores.  Pairs
+ * of two '=' tests, the same on both sides, are never enumerated (csrc/tsm_simtest_kernels.cuh).
+ * tsm_similar_churn_last_ms: device time of the last call, ms4 = { k_scan over both revisions, fronts of both + the marks diff
+ * + k_sc_change, tokens + posting lists + enumeration of both, verification of both (cross scores included) }. */
+enum { TSM_SIMILAR_CHANGED = 0, TSM_SIMILAR_REMOVED = 1, TSM_SIMILAR_DROPPED = 2, TSM_SIMILAR_DIVERGED = 3, TSM_SIMILAR_CREATED = 4,
+       TSM_SIMILAR_COPIED = 5, TSM_SIMILAR_CONVERGED = 6 };
+typedef struct tsm_similar_churn_side {
+  tsm_smell_test* tests; uint32_t* test_kept; int32_t* match; uint8_t* change; int64_t test_cap; int64_t n_tests;
+  int64_t n_candidates;
+} tsm_similar_churn_side;
+typedef struct tsm_similar_event { int32_t status, old_a, old_b, a, b; uint32_t old_lcs, old_score, lcs, score; } tsm_similar_event;
+int tsm_similar_churn(tsm_ctx* ctx, const tsm_corpus* old_rev, const tsm_corpus* new_rev, const int32_t* pair_old,
+                      const int32_t* pair_new, int64_t n_pairs, int32_t min_lines, int32_t min_similarity,
+                      tsm_similar_churn_side* old_side, tsm_similar_churn_side* new_side, tsm_similar_event* events, int64_t event_cap,
+                      int64_t* n_events, void* stream);
+int tsm_similar_churn_last_ms(tsm_ctx* ctx, float* ms4);
+
 /* Test-smell churn (docs/SPEC.md section 19): the section-16 cases and the section-18 tests of both sides of every revision pair,
  * and per test how many of its smell instances the revision adds (new side) or removes (old side).  cases is filled exactly as
  * tsm_diff_pairs_cases fills it.  old_tests / new_tests are the tsm_smell_test records of tsm_smells over each side's corpus

@@ -6,6 +6,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <chrono>
+#include <unordered_map>
 #include <new>
 #include <utility>
 #include <vector>
@@ -27,6 +28,7 @@
 #include "tsm_smell_kernels.cuh"
 #include "tsm_move_kernels.cuh"
 #include "tsm_clone_churn_kernels.cuh"
+#include "../host/tsm_names.hpp"
 #include "tsm_simtest_kernels.cuh"
 
 using namespace tsm;
@@ -92,6 +94,8 @@ enum Timed {
   MS_BLAME,   // k_blame of the last tsm_blame_pairs
   MS_CCHURN,  // k_scan of both revisions, classes of both, the marks diff, the churn kernels of the last tsm_clone_churn
   MS_SIMTEST, // k_scan, case spans + smell stage + lexer, tokens + lists + enumeration, verification of the last tsm_similar_tests
+  MS_SCHURN,  // k_scan of both revisions, fronts + marks + k_sc_change, tokens + lists + enumeration, verification of the last
+              // tsm_similar_churn
   N_TIMED
 };
 
@@ -2432,115 +2436,136 @@ extern "C" int tsm_smells(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, u
 extern "C" int tsm_smells_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_SMELL, ms4, 4); }
 
 // ------------------------------------------------------------------------------------- SPEC section 23 similar tests
-// The tests and their kept blind lines of one side whose line records (with header events) exist: the case spans and smell
-// stage of tsm_smells and blind_front, then one synchronisation for the test and kept counts; the prefix tokens, their posting
-// lists and the scan of the lists' candidate counts, then one synchronisation for the candidate total; then per chunk of
-// ST_CHUNK virtual candidates k_st_enum and k_st_verify and one synchronisation that copies the chunk's pairs out.  tests /
-// kept / pairs: host copies of the tests, their kept lines and the pairs (unordered).  ms[1..3] as tsm_similar_tests_last_ms.
-static int similar_pairs(tsm_ctx* c, const HostSide& S, uint32_t min_lines, uint32_t P, std::vector<tsm_smell_test>& tests,
-                         std::vector<uint32_t>& kept, std::vector<tsm_similar_pair>& pairs, int64_t* n_candidates, float* ms,
-                         cudaStream_t st) {
+// One revision's section-23 state on the device, resident while the call needs it: the front (case spans, smell stage and
+// blind_front; nt tests, nk kept lines) and the tokens, prefixes and posting lists of its compared tests.
+struct StSide {
+  CaseSpans sp; SmellBufs m; BlindFront bf; DevBuf bsum;
+  DevBuf kbeg, kk, q, ktest, ctr, key, cnt, eord, pbase, tbsum, pkey, pcnt, tok, ptest, mbase, cursor, mem, cbase, cbsum, surv, pairs;
+  unsigned long long nt = 0, nk = 0;
+  uint32_t nl = 0, nb = 0;
+  StEnum enum_args(uint32_t P) const {
+    return StEnum{cbase.as<unsigned long long>(), nl, mbase.as<unsigned long long>(), mem.as<uint32_t>(), kk.as<uint32_t>(),
+                  q.as<uint32_t>(), pbase.as<unsigned long long>(), tok.as<StToken>(), P, surv.as<uint2>(), ctr.as<uint32_t>() + 1};
+  }
+};
+
+// The front of one side whose line records (with header events) exist: the case spans and smell stage of tsm_smells and
+// blind_front, then one synchronisation for the test and kept counts.  ms[1] = its device time.
+static int st_front(tsm_ctx* c, const HostSide& S, StSide& f, float* ms, cudaStream_t st) {
   const size_t L = (size_t)S.total;
-  CaseSpans sp;
-  SmellBufs m;
-  BlindFront bf;
-  DevBuf d_bsum;
-  if (!d_bsum.alloc(8 * (L / XS_TILE + 4))) return TSM_E_CUDA;
+  if (!f.bsum.alloc(8 * (L / XS_TILE + 4))) return TSM_E_CUDA;
   int launches = 0;
   CU(cudaEventRecord(c->diff_ev[EV_ST_FRONT], st));
-  int rc = case_spans(S, sp, d_bsum, launches, st);
-  if (rc == TSM_OK) rc = smell_stage(c, S, sp, d_bsum, m, launches, st);
-  if (rc == TSM_OK) rc = blind_front(c, S, bf, st);
+  int rc = case_spans(S, f.sp, f.bsum, launches, st);
+  if (rc == TSM_OK) rc = smell_stage(c, S, f.sp, f.bsum, f.m, launches, st);
+  if (rc == TSM_OK) rc = blind_front(c, S, f.bf, st);
   if (rc != TSM_OK) return rc;
   CU(cudaEventRecord(c->diff_ev[EV_ST_LEXED], st));
   unsigned long long* pin = c->h_rb->u64;
-  CU(cudaMemcpyAsync(pin, m.tidx.as<unsigned long long>() + sp.n_cases, 8, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(pin + 1, bf.rank.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(pin, f.m.tidx.as<unsigned long long>() + f.sp.n_cases, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(pin + 1, f.bf.rank.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   c->launches += launches;
-  const unsigned long long nt = pin[0], nk = pin[1];
-  ms[1] = elapsed_ms(c->diff_ev[EV_ST_FRONT], c->diff_ev[EV_ST_LEXED]);
-  tests.resize((size_t)nt);
-  kept.resize((size_t)nt);
-  if (nt == 0) return TSM_OK;
+  f.nt = pin[0];
+  f.nk = pin[1];
+  ms[1] += elapsed_ms(c->diff_ev[EV_ST_FRONT], c->diff_ev[EV_ST_LEXED]);
+  return TSM_OK;
+}
+
+// The tokens of a side with nt > 0 behind st_front: k_st_tests (kbeg, kk, q, ktest; kmax at ctr[0]), the count table, the
+// prefix tokens (k_st_prefix) and the scan of the lists' lengths into mbase.  Queued only: the posting lists come next.
+static int st_tokens(const HostSide& S, StSide& f, uint32_t min_lines, uint32_t P, cudaStream_t st) {
+  const unsigned long long nt = f.nt, nk = f.nk;
   if (nk >= (1ull << 30)) return TSM_E_NOMEM;              // the token tables are indexed by u32 with a spare slot
   const size_t NT = (size_t)nt, NK = (size_t)nk;
   size_t slots = 1;                                        // a power of two, at least 2 x the kept lines
   while (slots < 2 * NK) slots <<= 1;
   const uint32_t mask = (uint32_t)(slots - 1), nl = (uint32_t)slots + 1;   // + the slot of key ST_EMPTY
-  const uint32_t nb = (nl + XS_TILE - 1) / XS_TILE;
-  DevBuf d_kbeg, d_kk, d_q, d_ktest, d_ctr, d_key, d_cnt, d_eord, d_pbase, d_tbsum, d_pkey, d_pcnt, d_tok, d_ptest, d_mbase, d_cursor,
-      d_mem, d_cbase, d_cbsum, d_surv, d_pairs, d_scratch;
-  if (!d_kbeg.alloc(4 * NT) || !d_kk.alloc(4 * NT) || !d_q.alloc(4 * NT) || !d_ktest.alloc(4 * NK) || !d_ctr.alloc(16) ||
-      !d_key.alloc(8 * (size_t)nl) || !d_cnt.alloc(4 * (size_t)nl) || !d_eord.alloc(8 * NK) || !d_pbase.alloc(8 * (NT + 1)) ||
-      !d_tbsum.alloc(8 * (NT / XS_TILE + 4)) || !d_pkey.alloc(8 * (size_t)nl) || !d_pcnt.alloc(4 * (size_t)nl) ||
-      !d_tok.alloc(sizeof(StToken) * NK) || !d_ptest.alloc(4 * NK) || !d_mbase.alloc(8 * ((size_t)nl + 1)) ||
-      !d_cursor.alloc(4 * (size_t)nl) || !d_mem.alloc(4 * NK) || !d_cbase.alloc(8 * ((size_t)nl + 1)) ||
-      !d_cbsum.alloc(8 * ((size_t)nb + 4)) || !d_surv.alloc(sizeof(uint2) * ST_CHUNK) || !d_pairs.alloc(sizeof(tsm_similar_pair) * ST_CHUNK)) {
+  f.nl = nl;
+  f.nb = (nl + XS_TILE - 1) / XS_TILE;
+  if (!f.kbeg.alloc(4 * NT) || !f.kk.alloc(4 * NT) || !f.q.alloc(4 * NT) || !f.ktest.alloc(4 * NK) || !f.ctr.alloc(16) ||
+      !f.key.alloc(8 * (size_t)nl) || !f.cnt.alloc(4 * (size_t)nl) || !f.eord.alloc(8 * NK) || !f.pbase.alloc(8 * (NT + 1)) ||
+      !f.tbsum.alloc(8 * (NT / XS_TILE + 4)) || !f.pkey.alloc(8 * (size_t)nl) || !f.pcnt.alloc(4 * (size_t)nl) ||
+      !f.tok.alloc(sizeof(StToken) * NK) || !f.ptest.alloc(4 * NK) || !f.mbase.alloc(8 * ((size_t)nl + 1)) ||
+      !f.cursor.alloc(4 * (size_t)nl) || !f.mem.alloc(4 * NK) || !f.cbase.alloc(8 * ((size_t)nl + 1)) ||
+      !f.cbsum.alloc(8 * ((size_t)f.nb + 4)) || !f.surv.alloc(sizeof(uint2) * ST_CHUNK) || !f.pairs.alloc(sizeof(tsm_similar_pair) * ST_CHUNK)) {
     cudaGetLastError();
     return TSM_E_NOMEM;
   }
-  uint32_t* ctr = d_ctr.as<uint32_t>();                   // kmax, survivors, pairs
-  const uint32_t* ktest = d_ktest.as<uint32_t>();
-  const unsigned long long* khash = bf.khash.as<unsigned long long>();
-  CU(cudaMemsetAsync(d_ktest.p, 0xFF, 4 * NK, st));
-  CU(cudaMemsetAsync(d_ctr.p, 0, 16, st));
-  CU(cudaMemsetAsync(d_key.p, 0xFF, 8 * (size_t)nl, st));
-  CU(cudaMemsetAsync(d_cnt.p, 0, 4 * (size_t)nl, st));
-  CU(cudaMemsetAsync(d_pkey.p, 0xFF, 8 * (size_t)nl, st));
-  CU(cudaMemsetAsync(d_pcnt.p, 0, 4 * (size_t)nl, st));
-  CU(cudaMemsetAsync(d_cursor.p, 0, 4 * (size_t)nl, st));
+  uint32_t* ctr = f.ctr.as<uint32_t>();                   // kmax, survivors, pairs
+  const uint32_t* ktest = f.ktest.as<uint32_t>();
+  const unsigned long long* khash = f.bf.khash.as<unsigned long long>();
+  CU(cudaMemsetAsync(f.ktest.p, 0xFF, 4 * NK, st));
+  CU(cudaMemsetAsync(f.ctr.p, 0, 16, st));
+  CU(cudaMemsetAsync(f.key.p, 0xFF, 8 * (size_t)nl, st));
+  CU(cudaMemsetAsync(f.cnt.p, 0, 4 * (size_t)nl, st));
+  CU(cudaMemsetAsync(f.pkey.p, 0xFF, 8 * (size_t)nl, st));
+  CU(cudaMemsetAsync(f.pcnt.p, 0, 4 * (size_t)nl, st));
+  CU(cudaMemsetAsync(f.cursor.p, 0, 4 * (size_t)nl, st));
   const unsigned kgrid = (unsigned)((NK + 255) / 256);
-  k_st_tests<<<(unsigned)((NT + 255) / 256), 256, 0, st>>>(m.tests.as<tsm_smell_test>(), (uint32_t)nt, S.d.line_base,
-                                                           bf.rank.as<unsigned long long>(), min_lines, P, d_kbeg.as<uint32_t>(),
-                                                           d_kk.as<uint32_t>(), d_q.as<uint32_t>(), d_ktest.as<uint32_t>(), ctr);
+  k_st_tests<<<(unsigned)((NT + 255) / 256), 256, 0, st>>>(f.m.tests.as<tsm_smell_test>(), (uint32_t)nt, S.d.line_base,
+                                                           f.bf.rank.as<unsigned long long>(), min_lines, P, f.kbeg.as<uint32_t>(),
+                                                           f.kk.as<uint32_t>(), f.q.as<uint32_t>(), f.ktest.as<uint32_t>(), ctr);
   if (NK) {
-    k_st_count<<<kgrid, 256, 0, st>>>(khash, ktest, (uint32_t)nk, d_key.as<unsigned long long>(), mask, d_cnt.as<uint32_t>(), d_eord.as<uint2>());
-    k_st_order<<<kgrid, 256, 0, st>>>(ktest, (uint32_t)nk, d_cnt.as<uint32_t>(), d_eord.as<uint2>());
+    k_st_count<<<kgrid, 256, 0, st>>>(khash, ktest, (uint32_t)nk, f.key.as<unsigned long long>(), mask, f.cnt.as<uint32_t>(), f.eord.as<uint2>());
+    k_st_order<<<kgrid, 256, 0, st>>>(ktest, (uint32_t)nk, f.cnt.as<uint32_t>(), f.eord.as<uint2>());
   }
-  xscan(d_q.as<uint32_t>(), (uint32_t)nt, d_tbsum.as<unsigned long long>(), d_pbase.as<unsigned long long>(), st);
+  xscan(f.q.as<uint32_t>(), (uint32_t)nt, f.tbsum.as<unsigned long long>(), f.pbase.as<unsigned long long>(), st);
   if (NK)
-    k_st_prefix<<<kgrid, 256, 0, st>>>(ktest, (uint32_t)nk, d_eord.as<uint2>(), d_kbeg.as<uint32_t>(), d_kk.as<uint32_t>(), d_q.as<uint32_t>(),
-                                       d_pbase.as<unsigned long long>(), d_pkey.as<unsigned long long>(), mask, d_pcnt.as<uint32_t>(),
-                                       d_tok.as<StToken>(), d_ptest.as<uint32_t>());
-  xscan(d_pcnt.as<uint32_t>(), nl, d_cbsum.as<unsigned long long>(), d_mbase.as<unsigned long long>(), st);
-  if (NK)
-    k_st_lists<<<kgrid, 256, 0, st>>>(d_tok.as<StToken>(), d_ptest.as<uint32_t>(), d_pbase.as<unsigned long long>() + NT,
-                                      d_mbase.as<unsigned long long>(), d_cursor.as<uint32_t>(), d_mem.as<uint32_t>());
-  k_st_csums<<<nb, 256, 0, st>>>(d_pcnt.as<uint32_t>(), nl, d_cbsum.as<unsigned long long>());
-  k_xscan_top<<<1, 256, 0, st>>>(d_cbsum.as<unsigned long long>(), nb);
-  k_st_capply<<<nb, 256, 0, st>>>(d_pcnt.as<uint32_t>(), nl, d_cbsum.as<unsigned long long>(), d_cbase.as<unsigned long long>());
+    k_st_prefix<<<kgrid, 256, 0, st>>>(ktest, (uint32_t)nk, f.eord.as<uint2>(), f.kbeg.as<uint32_t>(), f.kk.as<uint32_t>(), f.q.as<uint32_t>(),
+                                       f.pbase.as<unsigned long long>(), f.pkey.as<unsigned long long>(), mask, f.pcnt.as<uint32_t>(),
+                                       f.tok.as<StToken>(), f.ptest.as<uint32_t>());
+  xscan(f.pcnt.as<uint32_t>(), nl, f.cbsum.as<unsigned long long>(), f.mbase.as<unsigned long long>(), st);
   CU(cudaGetLastError());
-  CU(cudaEventRecord(c->diff_ev[EV_ST_LISTS], st));
-  c->launches += 10 + (NK ? 4 : 0);                       // tests, 2 x xscan (3 each), the candidate scan (3); count, order, prefix, lists
+  return TSM_OK;
+}
+
+// The warps and scratch of k_st_verify for patterns of up to kmax kept lines: V of a pattern of more than 2048 kept lines
+// lives in a scratch slot of each warp, within 1 GiB.
+struct StVerifyShape { uint32_t slot_words; unsigned blocks; };
+static int st_verify_shape(const tsm_ctx* c, uint32_t kmax, DevBuf& scratch, StVerifyShape& v) {
+  const uint32_t W = (kmax + 63) / 64, nbk = (W + 31) / 32;
+  v.slot_words = nbk > 1 ? nbk * 32 : 0;
+  v.blocks = (unsigned)c->sms * 4;
+  if (v.slot_words) {
+    v.blocks = (unsigned)std::max<size_t>(1, std::min<size_t>(v.blocks, ((size_t)1 << 27) / ((size_t)v.slot_words * 8)));
+    if (!scratch.alloc(8 * (size_t)v.slot_words * v.blocks * 8)) { cudaGetLastError(); return TSM_E_NOMEM; }
+  }
+  return TSM_OK;
+}
+
+// Behind the posting lists and the scan of their candidate counts into cbase (queued by the caller): one synchronisation
+// for the candidate total and kmax, then per chunk of ST_CHUNK virtual candidates the enumeration (enumerate(c0, n, st)
+// queues it) and k_st_verify, and one synchronisation that copies the chunk's pairs out.  ms[2] += lists + enumeration,
+// ms[3] += verification.
+template <typename Enumerate>
+static int st_verify_all(tsm_ctx* c, StSide& f, uint32_t P, Enumerate enumerate, std::vector<tsm_similar_pair>& pairs,
+                         int64_t* n_candidates, float* ms, cudaStream_t st) {
+  unsigned long long* pin = c->h_rb->u64;
+  uint32_t* ctr = f.ctr.as<uint32_t>();
   pin[3] = 0;
-  CU(cudaMemcpyAsync(pin + 2, d_cbase.as<unsigned long long>() + nl, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(pin + 2, f.cbase.as<unsigned long long>() + f.nl, 8, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(pin + 3, ctr, 4, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   const unsigned long long n_virtual = pin[2];
   const uint32_t kmax = (uint32_t)pin[3];
-  ms[2] = elapsed_ms(c->diff_ev[EV_ST_LEXED], c->diff_ev[EV_ST_LISTS]);
-  // The verification's warps: V of a pattern of more than 2048 kept lines lives in a scratch slot of each warp, within 1 GiB.
-  const uint32_t W = (kmax + 63) / 64, nbk = (W + 31) / 32;
-  const uint32_t slot_words = nbk > 1 ? nbk * 32 : 0;
-  unsigned vblocks = (unsigned)c->sms * 4;
-  if (slot_words) {
-    vblocks = (unsigned)std::max<size_t>(1, std::min<size_t>(vblocks, ((size_t)1 << 27) / ((size_t)slot_words * 8)));
-    if (!d_scratch.alloc(8 * (size_t)slot_words * vblocks * 8)) { cudaGetLastError(); return TSM_E_NOMEM; }
-  }
-  const StEnum ea{d_cbase.as<unsigned long long>(), nl, d_mbase.as<unsigned long long>(), d_mem.as<uint32_t>(), d_kk.as<uint32_t>(),
-                  d_q.as<uint32_t>(), d_pbase.as<unsigned long long>(), d_tok.as<StToken>(), P, d_surv.as<uint2>(), ctr + 1};
+  ms[2] += elapsed_ms(c->diff_ev[EV_ST_LEXED], c->diff_ev[EV_ST_LISTS]);
+  DevBuf d_scratch;
+  StVerifyShape vs;
+  const int rc = st_verify_shape(c, kmax, d_scratch, vs);
+  if (rc != TSM_OK) return rc;
   int64_t ncand = 0;
   uint32_t* cnt2 = reinterpret_cast<uint32_t*>(pin + 2);
   for (unsigned long long c0 = 0; c0 < n_virtual; c0 += ST_CHUNK) {
     const unsigned long long n = std::min<unsigned long long>(ST_CHUNK, n_virtual - c0);
     CU(cudaMemsetAsync(ctr + 1, 0, 8, st));
     CU(cudaEventRecord(c->diff_ev[EV_ST_ENUM], st));
-    k_st_enum<<<(unsigned)std::min<unsigned long long>((n + 255) / 256, (unsigned long long)c->sms * 16), 256, 0, st>>>(ea, c0, n);
+    enumerate(c0, n, st);
     CU(cudaEventRecord(c->diff_ev[EV_ST_VERIFY], st));
-    k_st_verify<<<vblocks, 256, 0, st>>>(d_surv.as<uint2>(), ctr + 1, d_kbeg.as<uint32_t>(), d_kk.as<uint32_t>(), khash, P,
-                                         slot_words ? d_scratch.as<unsigned long long>() : nullptr, slot_words,
-                                         d_pairs.as<tsm_similar_pair>(), ctr + 2);
+    k_st_verify<<<vs.blocks, 256, 0, st>>>(f.surv.as<uint2>(), ctr + 1, f.kbeg.as<uint32_t>(), f.kk.as<uint32_t>(),
+                                           f.bf.khash.as<unsigned long long>(), P,
+                                           vs.slot_words ? d_scratch.as<unsigned long long>() : nullptr, vs.slot_words,
+                                           f.pairs.as<tsm_similar_pair>(), ctr + 2);
     CU(cudaGetLastError());
     CU(cudaEventRecord(c->diff_ev[EV_ST_END], st));
     CU(cudaMemcpyAsync(cnt2, ctr + 1, 8, cudaMemcpyDeviceToHost, st));
@@ -2553,13 +2578,47 @@ static int similar_pairs(tsm_ctx* c, const HostSide& S, uint32_t min_lines, uint
     if (np) {
       const size_t had = pairs.size();
       pairs.resize(had + np);
-      CU(cudaMemcpyAsync(pairs.data() + had, d_pairs.p, sizeof(tsm_similar_pair) * np, cudaMemcpyDeviceToHost, st));
+      CU(cudaMemcpyAsync(pairs.data() + had, f.pairs.p, sizeof(tsm_similar_pair) * np, cudaMemcpyDeviceToHost, st));
       CU(cudaStreamSynchronize(st));
     }
   }
   *n_candidates = ncand;
-  CU(cudaMemcpyAsync(tests.data(), m.tests.p, sizeof(tsm_smell_test) * NT, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(kept.data(), d_kk.p, 4 * NT, cudaMemcpyDeviceToHost, st));
+  return TSM_OK;
+}
+
+// The tests and their kept blind lines of one side whose line records (with header events) exist: st_front; the prefix
+// tokens, their posting lists and the scan of the lists' candidate counts; then st_verify_all over every pair of each list.
+// tests / kept / pairs: host copies of the tests, their kept lines and the pairs (unordered).  ms[1..3] as
+// tsm_similar_tests_last_ms.
+static int similar_pairs(tsm_ctx* c, const HostSide& S, uint32_t min_lines, uint32_t P, std::vector<tsm_smell_test>& tests,
+                         std::vector<uint32_t>& kept, std::vector<tsm_similar_pair>& pairs, int64_t* n_candidates, float* ms,
+                         cudaStream_t st) {
+  StSide f;
+  int rc = st_front(c, S, f, ms, st);
+  if (rc != TSM_OK) return rc;
+  const size_t NT = (size_t)f.nt, NK = (size_t)f.nk;
+  tests.resize(NT);
+  kept.resize(NT);
+  if (NT == 0) return TSM_OK;
+  rc = st_tokens(S, f, min_lines, P, st);
+  if (rc != TSM_OK) return rc;
+  const unsigned kgrid = (unsigned)((NK + 255) / 256);
+  if (NK)
+    k_st_lists<<<kgrid, 256, 0, st>>>(f.tok.as<StToken>(), f.ptest.as<uint32_t>(), f.pbase.as<unsigned long long>() + NT,
+                                      f.mbase.as<unsigned long long>(), f.cursor.as<uint32_t>(), f.mem.as<uint32_t>());
+  k_st_csums<<<f.nb, 256, 0, st>>>(f.pcnt.as<uint32_t>(), f.nl, f.cbsum.as<unsigned long long>());
+  k_xscan_top<<<1, 256, 0, st>>>(f.cbsum.as<unsigned long long>(), f.nb);
+  k_st_capply<<<f.nb, 256, 0, st>>>(f.pcnt.as<uint32_t>(), f.nl, f.cbsum.as<unsigned long long>(), f.cbase.as<unsigned long long>());
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(c->diff_ev[EV_ST_LISTS], st));
+  c->launches += 10 + (NK ? 4 : 0);                       // tests, 2 x xscan (3 each), the candidate scan (3); count, order, prefix, lists
+  const StEnum ea = f.enum_args(P);
+  rc = st_verify_all(c, f, P, [&](unsigned long long c0, unsigned long long n, cudaStream_t s2) {
+    k_st_enum<<<(unsigned)std::min<unsigned long long>((n + 255) / 256, (unsigned long long)c->sms * 16), 256, 0, s2>>>(ea, c0, n);
+  }, pairs, n_candidates, ms, st);
+  if (rc != TSM_OK) return rc;
+  CU(cudaMemcpyAsync(tests.data(), f.m.tests.p, sizeof(tsm_smell_test) * NT, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(kept.data(), f.kk.p, 4 * NT, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return TSM_OK;
 }
@@ -2621,6 +2680,362 @@ extern "C" int tsm_similar_tests(tsm_ctx* c, const tsm_corpus* k, int32_t min_li
 }
 
 extern "C" int tsm_similar_tests_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_SIMTEST, ms4, 4); }
+
+// ------------------------------------------------------------------------------------- SPEC section 24 similar-test churn
+namespace {
+// The host view of one revision behind its front: its tests, the header line of each case, its marks and its files.
+struct ScRev {
+  const tsm_corpus* k = nullptr;
+  std::vector<unsigned long long> base;                    // line_base
+  std::vector<tsm_smell_test> tests;
+  std::vector<uint32_t> head, kept;                        // the header line (global) of every case; kept lines per test
+  std::vector<uint8_t> mark;
+  std::vector<size_t> tfile, cfile;                        // first test / case of every file [n_files + 1]
+  std::vector<int32_t> match;
+  std::vector<uint8_t> change;
+  void index() {
+    const size_t nf = (size_t)k->n_files;
+    tfile.assign(nf + 1, 0);
+    cfile.assign(nf + 1, 0);
+    for (const tsm_smell_test& t : tests) ++tfile[(size_t)t.file + 1];
+    for (uint32_t h : head) ++cfile[(size_t)(std::upper_bound(base.begin(), base.end(), (unsigned long long)h) - base.begin())];
+    for (size_t f = 0; f < nf; ++f) { tfile[f + 1] += tfile[f]; cfile[f + 1] += cfile[f]; }
+  }
+  // The case names (section 10) of the cases of file f.
+  std::vector<std::string> names(int32_t f) const {
+    std::vector<std::string> out;
+    const uint8_t* p = k->arena + k->off[f];
+    const int32_t size = k->len[f];
+    int32_t line = 0, pos = 0;
+    for (size_t c = cfile[(size_t)f]; c < cfile[(size_t)f + 1]; ++c) {
+      for (const int32_t h = (int32_t)(head[c] - base[(size_t)f]); line < h; ++line)
+        pos = (int32_t)((const uint8_t*)memchr(p + pos, '\n', (size_t)(size - pos)) - p) + 1;
+      const uint8_t* lf = (const uint8_t*)memchr(p + pos, '\n', (size_t)(size - pos));
+      out.push_back(tsm_names::case_name(k->ext ? k->ext[f] : 0, p + pos, (uint32_t)((lf ? (int32_t)(lf - p) : size) - pos)));
+    }
+    return out;
+  }
+};
+
+// Section 24's test identity within the changed pair (fo, fn): the section-16 matching of their cases (step 1 through the
+// kept-line correspondence of the marks, step 2 by tsm_names::match_by_name), then matched cases that are tests on both
+// sides.  Appends (old test, new test) to `both`.
+void sc_match_pair(ScRev& O, ScRev& N, int32_t fo, int32_t fn, std::vector<uint2>& both) {
+  const size_t co = O.cfile[(size_t)fo], no = O.cfile[(size_t)fo + 1] - co, cn = N.cfile[(size_t)fn], nn = N.cfile[(size_t)fn + 1] - cn;
+  const unsigned long long bo = O.base[(size_t)fo], bn = N.base[(size_t)fn];
+  std::vector<uint32_t> okept;                             // the kept old lines, in order (local)
+  for (unsigned long long l = bo; l < O.base[(size_t)fo + 1]; ++l) if (!O.mark[l]) okept.push_back((uint32_t)(l - bo));
+  std::unordered_map<uint32_t, int64_t> old_case;          // local header line -> old case (within the file)
+  for (size_t k = 0; k < no; ++k) old_case[(uint32_t)(O.head[co + k] - bo)] = (int64_t)k;
+  std::vector<int64_t> match(nn, -1);
+  std::vector<char> used(no, 0);
+  size_t r = 0, j = 0;
+  for (unsigned long long l = bn; l < N.base[(size_t)fn + 1] && j < nn; ++l) {
+    if (N.head[cn + j] == l) {
+      if (!N.mark[l] && r < okept.size()) {
+        const auto it = old_case.find(okept[r]);
+        if (it != old_case.end()) { match[j] = it->second; used[(size_t)it->second] = 1; }
+      }
+      ++j;
+    }
+    r += !N.mark[l];
+  }
+  if (std::find(match.begin(), match.end(), -1) != match.end() && std::find(used.begin(), used.end(), 0) != used.end())
+    tsm_names::match_by_name(O.names(fo), N.names(fn), match, used);
+  std::unordered_map<uint32_t, size_t> old_test;           // local header line -> old test
+  for (size_t t = O.tfile[(size_t)fo]; t < O.tfile[(size_t)fo + 1]; ++t) old_test[(uint32_t)O.tests[t].line] = t;
+  std::unordered_map<uint32_t, size_t> new_case;
+  for (size_t k = 0; k < nn; ++k) new_case[(uint32_t)(N.head[cn + k] - bn)] = k;
+  for (size_t t = N.tfile[(size_t)fn]; t < N.tfile[(size_t)fn + 1]; ++t) {
+    const int64_t k = match[new_case.at((uint32_t)N.tests[t].line)];
+    if (k < 0) continue;
+    const auto it = old_test.find((uint32_t)(O.head[co + (size_t)k] - bo));
+    if (it == old_test.end()) continue;
+    both.push_back(make_uint2((uint32_t)it->second, (uint32_t)t));
+  }
+}
+}  // namespace
+
+// The section-23 score of explicit pairs of one side's tests: k_st_verify at P = 0 over the side's resident front, in
+// chunks of ST_CHUNK, its scratch sized from the longest test of the pairs.  out[i] = {a, b, lcs, score} of pairs[i].
+static int sc_cross(tsm_ctx* c, StSide& f, const std::vector<uint2>& pairs, const std::vector<uint32_t>& kept,
+                    std::vector<tsm_similar_pair>& out, float* ms, cudaStream_t st) {
+  out.assign(pairs.size(), tsm_similar_pair{});
+  if (pairs.empty()) return TSM_OK;
+  uint32_t kmax = 0;
+  for (const uint2& p : pairs) kmax = std::max(kmax, std::max(kept[p.x], kept[p.y]));
+  DevBuf d_scratch;
+  StVerifyShape vs;
+  int rc = st_verify_shape(c, kmax, d_scratch, vs);
+  if (rc != TSM_OK) return rc;
+  std::unordered_map<unsigned long long, size_t> at;
+  for (size_t i = 0; i < pairs.size(); ++i) at[(unsigned long long)pairs[i].x << 32 | pairs[i].y] = i;
+  uint32_t* ctr = f.ctr.as<uint32_t>();
+  std::vector<tsm_similar_pair> got;
+  for (size_t c0 = 0; c0 < pairs.size(); c0 += ST_CHUNK) {
+    const uint32_t n = (uint32_t)std::min<size_t>(ST_CHUNK, pairs.size() - c0);
+    const uint32_t cnt[2] = {n, 0};
+    CU(cudaMemcpyAsync(f.surv.p, pairs.data() + c0, sizeof(uint2) * n, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(ctr + 1, cnt, 8, cudaMemcpyHostToDevice, st));
+    CU(cudaEventRecord(c->diff_ev[EV_ST_VERIFY], st));
+    k_st_verify<<<vs.blocks, 256, 0, st>>>(f.surv.as<uint2>(), ctr + 1, f.kbeg.as<uint32_t>(), f.kk.as<uint32_t>(),
+                                           f.bf.khash.as<unsigned long long>(), 0, vs.slot_words ? d_scratch.as<unsigned long long>() : nullptr,
+                                           vs.slot_words, f.pairs.as<tsm_similar_pair>(), ctr + 2);
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_ST_END], st));
+    got.resize(n);
+    CU(cudaMemcpyAsync(got.data(), f.pairs.p, sizeof(tsm_similar_pair) * n, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    c->launches++;
+    ms[3] += elapsed_ms(c->diff_ev[EV_ST_VERIFY], c->diff_ev[EV_ST_END]);
+    for (const tsm_similar_pair& p : got) out[at.at((unsigned long long)(uint32_t)p.a << 32 | (uint32_t)p.b)] = p;
+  }
+  return TSM_OK;
+}
+
+// Both revisions to the device and their line records with header events (one k_scan pass each), the marks of the pairs
+// (churn_marks), per revision the front of tsm_similar_tests (st_front); on the host the test identity (unchanged files in
+// order, sc_match_pair for the changed pairs); k_sc_change for the matched tests of changed pairs; per revision the tokens
+// (st_tokens), posting lists with the dirty tests first and the restricted enumeration (st_verify_all over k_sc_enum); then
+// the events on the host, with the cross scores of sc_cross.  Both fronts stay resident to the end.
+extern "C" int tsm_similar_churn(tsm_ctx* c, const tsm_corpus* old_rev, const tsm_corpus* new_rev, const int32_t* pair_old,
+                                 const int32_t* pair_new, int64_t n_pairs, int32_t min_lines, int32_t min_similarity,
+                                 tsm_similar_churn_side* old_side, tsm_similar_churn_side* new_side, tsm_similar_event* events,
+                                 int64_t event_cap, int64_t* n_events, void* stream) {
+  if (!c || !old_rev || !new_rev || !old_side || !new_side || !n_events || n_pairs < 0 || n_pairs > INT32_MAX ||
+      (n_pairs && (!pair_old || !pair_new)) || min_lines < 1 || min_similarity < 1 || min_similarity > 100 || event_cap < 0)
+    return TSM_E_ARG;
+  const tsm_corpus* rev[2] = {old_rev, new_rev};
+  tsm_similar_churn_side* side[2] = {old_side, new_side};
+  const int32_t* pf[2] = {pair_old, pair_new};
+  const int32_t n = (int32_t)n_pairs;
+  std::vector<int32_t> unpaired[2];
+  for (int i = 0; i < 2; ++i) {
+    if (rev[i]->n_files < 0 || side[i]->test_cap < 0) return TSM_E_ARG;
+    std::vector<uint8_t> used((size_t)rev[i]->n_files, 0);
+    for (int32_t k = 0; k < n; ++k) {
+      const int32_t f = pf[i][k];
+      if (f < -1 || f >= rev[i]->n_files || (f >= 0 && used[(size_t)f]++) || (pair_old[k] < 0 && pair_new[k] < 0)) return TSM_E_ARG;
+    }
+    for (int32_t f = 0; f < rev[i]->n_files; ++f) if (!used[(size_t)f]) unpaired[i].push_back(f);
+  }
+  if (unpaired[0].size() != unpaired[1].size()) return TSM_E_ARG;
+  for (int i = 0; i < 2; ++i)
+    if (rev[i]->n_files > 0) {
+      const int rc = check_sides({rev[i]}, true);
+      if (rc != TSM_OK) return rc;
+    }
+  for (size_t k = 0; k < unpaired[0].size(); ++k)
+    if (old_rev->len[unpaired[0][k]] != new_rev->len[unpaired[1][k]]) return TSM_E_ARG;
+  float* const ms = clear_ms(c, MS_SCHURN);
+  c->launches = 0;
+  *n_events = 0;
+  for (int i = 0; i < 2; ++i) side[i]->n_tests = side[i]->n_candidates = 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  CallScope call(c, st);
+  CU(call.status);
+  HostSide S[2];
+  DevBuf rmark[2], d_both, d_same, d_dirty[2], d_dcnt[2], d_ccur[2];
+  StSide F[2];
+  SyncGuard guard(st);
+  HostSide* scan[2];
+  int ns = 0;
+  for (int i = 0; i < 2; ++i)
+    if (rev[i]->n_files > 0) {
+      const int rc = side_upload(rev[i], S[i], st);
+      if (rc != TSM_OK) return rc;
+      scan[ns++] = &S[i];
+    }
+  if (ns) {
+    const int rc = sides_records(c, scan, ns, st, &ms[0], true, TSM_SCAN_HEADER_EVENTS);
+    if (rc != TSM_OK) return rc;
+  }
+  for (int i = 0; i < 2; ++i) {
+    c->launches += S[i].launches;
+    if (!rmark[i].alloc((size_t)S[i].total)) return TSM_E_CUDA;
+    CU(cudaMemsetAsync(rmark[i].p, 0, (size_t)S[i].total, st));
+  }
+  float mms[4] = {0, 0, 0, 0};
+  if (n) {
+    const int rc = churn_marks(c, S, pf, n, rmark, mms, st);
+    if (rc != TSM_OK) return rc;
+  }
+  ms[1] += mms[2] + mms[3];
+  ScRev R[2];
+  for (int i = 0; i < 2; ++i) {
+    ScRev& r = R[i];
+    r.k = rev[i];
+    r.base = S[i].base;
+    if (r.base.empty()) r.base.assign((size_t)rev[i]->n_files + 1, 0);
+    if (S[i].total == 0) { r.index(); continue; }
+    const int rc = st_front(c, S[i], F[i], ms, st);
+    if (rc != TSM_OK) return rc;
+    r.tests.resize((size_t)F[i].nt);
+    r.head.resize(F[i].sp.n_cases);
+    r.mark.resize((size_t)S[i].total);
+    if (F[i].nt) CU(cudaMemcpyAsync(r.tests.data(), F[i].m.tests.p, sizeof(tsm_smell_test) * (size_t)F[i].nt, cudaMemcpyDeviceToHost, st));
+    if (F[i].sp.n_cases) CU(cudaMemcpyAsync(r.head.data(), F[i].sp.first.p, 4 * (size_t)F[i].sp.n_cases, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(r.mark.data(), rmark[i].p, (size_t)S[i].total, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    r.index();
+  }
+  ScRev &O = R[0], &N = R[1];
+  O.match.assign(O.tests.size(), -1);
+  N.match.assign(N.tests.size(), -1);
+  O.change.assign(O.tests.size(), 'D');
+  N.change.assign(N.tests.size(), 'A');
+  for (size_t k = 0; k < unpaired[0].size(); ++k) {       // an unchanged file: test i is test i
+    const int32_t fo = unpaired[0][k], fn = unpaired[1][k];
+    const size_t to = O.tfile[(size_t)fo], tn = N.tfile[(size_t)fn], m = O.tfile[(size_t)fo + 1] - to;
+    if (m != N.tfile[(size_t)fn + 1] - tn) return TSM_E_ARG;
+    for (size_t t = 0; t < m; ++t) {
+      O.match[to + t] = (int32_t)(tn + t); N.match[tn + t] = (int32_t)(to + t);
+      O.change[to + t] = N.change[tn + t] = '=';
+    }
+  }
+  std::vector<uint2> both;
+  for (int32_t k = 0; k < n; ++k)
+    if (pair_old[k] >= 0 && pair_new[k] >= 0) sc_match_pair(O, N, pair_old[k], pair_new[k], both);
+  if (!both.empty()) {
+    const uint32_t nm = (uint32_t)both.size();
+    if (!d_both.alloc(sizeof(uint2) * nm) || !d_same.alloc(nm)) return TSM_E_CUDA;
+    std::vector<uint8_t> same(nm);
+    CU(cudaEventRecord(c->diff_ev[EV_ST_FRONT], st));
+    CU(cudaMemcpyAsync(d_both.p, both.data(), sizeof(uint2) * nm, cudaMemcpyHostToDevice, st));
+    ScChangeSide cs[2];
+    for (int i = 0; i < 2; ++i)
+      cs[i] = ScChangeSide{F[i].m.tests.as<tsm_smell_test>(), S[i].d.line_base, rmark[i].as<uint8_t>(), F[i].bf.rank.as<unsigned long long>(),
+                           F[i].bf.khash.as<unsigned long long>()};
+    k_sc_change<<<std::min((nm + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(cs[0], cs[1], d_both.as<uint2>(), nm, d_same.as<uint8_t>());
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_ST_END], st));
+    CU(cudaMemcpyAsync(same.data(), d_same.p, nm, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    c->launches++;
+    ms[1] += elapsed_ms(c->diff_ev[EV_ST_FRONT], c->diff_ev[EV_ST_END]);
+    for (uint32_t k = 0; k < nm; ++k) {
+      const uint2 m = both[k];
+      O.match[m.x] = (int32_t)m.y; N.match[m.y] = (int32_t)m.x;
+      O.change[m.x] = N.change[m.y] = same[k] ? '=' : 'M';
+    }
+  }
+  // Per side: the tokens, the posting lists with their dirty tests first, and the pairs with a dirty test.
+  std::vector<tsm_similar_pair> pairs[2];
+  for (int i = 0; i < 2; ++i) {
+    StSide& f = F[i];
+    ScRev& r = R[i];
+    const size_t NT = r.tests.size(), NK = (size_t)f.nk;
+    if (NT == 0) continue;
+    CU(cudaEventRecord(c->diff_ev[EV_ST_LEXED], st));
+    int rc = st_tokens(S[i], f, (uint32_t)min_lines, (uint32_t)min_similarity, st);
+    if (rc != TSM_OK) return rc;
+    std::vector<uint8_t> dirty(NT);
+    for (size_t t = 0; t < NT; ++t) dirty[t] = r.change[t] != '=';
+    if (!d_dirty[i].alloc(NT) || !d_dcnt[i].alloc(4 * (size_t)f.nl) || !d_ccur[i].alloc(4 * (size_t)f.nl)) return TSM_E_CUDA;
+    CU(cudaMemcpyAsync(d_dirty[i].p, dirty.data(), NT, cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync(d_dcnt[i].p, 0, 4 * (size_t)f.nl, st));
+    CU(cudaMemsetAsync(d_ccur[i].p, 0, 4 * (size_t)f.nl, st));
+    const unsigned kgrid = (unsigned)((NK + 255) / 256);
+    const unsigned long long* np = f.pbase.as<unsigned long long>() + NT;
+    if (NK) {
+      k_sc_dirty<<<kgrid, 256, 0, st>>>(f.tok.as<StToken>(), f.ptest.as<uint32_t>(), np, d_dirty[i].as<uint8_t>(), d_dcnt[i].as<uint32_t>());
+      k_sc_lists<<<kgrid, 256, 0, st>>>(f.tok.as<StToken>(), f.ptest.as<uint32_t>(), np, f.mbase.as<unsigned long long>(),
+                                        d_dirty[i].as<uint8_t>(), d_dcnt[i].as<uint32_t>(), f.cursor.as<uint32_t>(),
+                                        d_ccur[i].as<uint32_t>(), f.mem.as<uint32_t>());
+    }
+    k_sc_csums<<<f.nb, 256, 0, st>>>(f.pcnt.as<uint32_t>(), d_dcnt[i].as<uint32_t>(), f.nl, f.cbsum.as<unsigned long long>());
+    k_xscan_top<<<1, 256, 0, st>>>(f.cbsum.as<unsigned long long>(), f.nb);
+    k_sc_capply<<<f.nb, 256, 0, st>>>(f.pcnt.as<uint32_t>(), d_dcnt[i].as<uint32_t>(), f.nl, f.cbsum.as<unsigned long long>(),
+                                      f.cbase.as<unsigned long long>());
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_ST_LISTS], st));
+    c->launches += 10 + (NK ? 5 : 0);                     // tests, 2 x xscan (3 each), the candidate scan (3); count, order, prefix, dirty, lists
+    const StEnum ea = f.enum_args((uint32_t)min_similarity);
+    const uint32_t* pcnt = f.pcnt.as<uint32_t>();
+    const uint32_t* dcnt = d_dcnt[i].as<uint32_t>();
+    rc = st_verify_all(c, f, (uint32_t)min_similarity, [&](unsigned long long c0, unsigned long long cn, cudaStream_t s2) {
+      k_sc_enum<<<(unsigned)std::min<unsigned long long>((cn + 255) / 256, (unsigned long long)c->sms * 16), 256, 0, s2>>>(ea, pcnt, dcnt, c0, cn);
+    }, pairs[i], &side[i]->n_candidates, ms, st);
+    if (rc != TSM_OK) return rc;
+    r.kept.resize(NT);
+    CU(cudaMemcpyAsync(r.kept.data(), f.kk.p, 4 * NT, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+  }
+  // The events: each side's pairs mapped through match, then the cross scores of the pairs seen on one side only.
+  const auto key = [](int32_t a, int32_t b) { return (unsigned long long)(uint32_t)a << 32 | (uint32_t)b; };
+  std::unordered_map<unsigned long long, size_t> new_at, old_image;
+  for (size_t k = 0; k < pairs[1].size(); ++k) new_at[key(pairs[1][k].a, pairs[1][k].b)] = k;
+  std::vector<tsm_similar_event> ev_old, ev_new;
+  std::vector<uint2> cross[2];                             // pairs of each side whose score is wanted, in event order
+  const uint32_t NONE = 0xFFFFFFFFu;
+  for (const tsm_similar_pair& p : pairs[0]) {
+    const int32_t ma = O.match[(size_t)p.a], mb = O.match[(size_t)p.b];
+    tsm_similar_event e{0, p.a, p.b, ma, mb, p.lcs, p.score, NONE, NONE};
+    if (ma >= 0 && mb >= 0) {
+      const int32_t a = std::min(ma, mb), b = std::max(ma, mb);
+      const auto it = new_at.find(key(a, b));
+      if (it != new_at.end()) { old_image[key(a, b)] = (size_t)p.a << 32 | (uint32_t)p.b; continue; }   // changed: new side
+      e.status = TSM_SIMILAR_DIVERGED;
+      cross[1].push_back(make_uint2((uint32_t)a, (uint32_t)b));
+    } else {
+      e.status = ma < 0 && mb < 0 ? TSM_SIMILAR_REMOVED : TSM_SIMILAR_DROPPED;
+    }
+    ev_old.push_back(e);
+  }
+  std::unordered_map<unsigned long long, tsm_similar_pair> old_pair;
+  for (const tsm_similar_pair& p : pairs[0]) old_pair[key(p.a, p.b)] = p;
+  for (const tsm_similar_pair& p : pairs[1]) {
+    const int32_t ma = N.match[(size_t)p.a], mb = N.match[(size_t)p.b];
+    tsm_similar_event e{0, ma, mb, p.a, p.b, NONE, NONE, p.lcs, p.score};
+    const auto img = old_image.find(key(p.a, p.b));
+    if (img != old_image.end()) {
+      const tsm_similar_pair& q = old_pair.at(key((int32_t)(img->second >> 32), (int32_t)(uint32_t)img->second));
+      e.status = TSM_SIMILAR_CHANGED;
+      e.old_lcs = q.lcs; e.old_score = q.score;
+    } else if (ma >= 0 && mb >= 0) {
+      e.status = TSM_SIMILAR_CONVERGED;
+      cross[0].push_back(make_uint2((uint32_t)std::min(ma, mb), (uint32_t)std::max(ma, mb)));
+    } else {
+      e.status = ma < 0 && mb < 0 ? TSM_SIMILAR_CREATED : TSM_SIMILAR_COPIED;
+    }
+    ev_new.push_back(e);
+  }
+  std::vector<tsm_similar_pair> scored[2];
+  for (int i = 0; i < 2; ++i) {
+    const int rc = sc_cross(c, F[i], cross[i], R[i].kept, scored[i], ms, st);
+    if (rc != TSM_OK) return rc;
+  }
+  for (size_t k = 0, x = 0; k < ev_old.size(); ++k)
+    if (ev_old[k].status == TSM_SIMILAR_DIVERGED) { ev_old[k].lcs = scored[1][x].lcs; ev_old[k].score = scored[1][x].score; ++x; }
+  for (size_t k = 0, x = 0; k < ev_new.size(); ++k)
+    if (ev_new[k].status == TSM_SIMILAR_CONVERGED) { ev_new[k].old_lcs = scored[0][x].lcs; ev_new[k].old_score = scored[0][x].score; ++x; }
+  std::sort(ev_old.begin(), ev_old.end(), [](const tsm_similar_event& x, const tsm_similar_event& y) {
+    return x.old_a != y.old_a ? x.old_a < y.old_a : x.old_b < y.old_b; });
+  std::sort(ev_new.begin(), ev_new.end(), [](const tsm_similar_event& x, const tsm_similar_event& y) { return x.a != y.a ? x.a < y.a : x.b < y.b; });
+  *n_events = (int64_t)(ev_old.size() + ev_new.size());
+  for (int i = 0; i < 2; ++i) side[i]->n_tests = (int64_t)R[i].tests.size();
+  bool is_short = events && event_cap < *n_events;
+  for (int i = 0; i < 2; ++i) {
+    const tsm_similar_churn_side* o = side[i];
+    is_short |= (o->tests || o->test_kept || o->match || o->change) && o->test_cap < o->n_tests;
+  }
+  if (is_short) return TSM_E_CAPACITY;
+  if (events) {
+    std::copy(ev_old.begin(), ev_old.end(), events);
+    std::copy(ev_new.begin(), ev_new.end(), events + ev_old.size());
+  }
+  for (int i = 0; i < 2; ++i) {
+    tsm_similar_churn_side* o = side[i];
+    const ScRev& r = R[i];
+    if (o->tests) std::copy(r.tests.begin(), r.tests.end(), o->tests);
+    if (o->test_kept) std::copy(r.kept.begin(), r.kept.end(), o->test_kept);
+    if (o->match) std::copy(r.match.begin(), r.match.end(), o->match);
+    if (o->change) std::copy(r.change.begin(), r.change.end(), o->change);
+  }
+  return TSM_OK;
+}
+
+extern "C" int tsm_similar_churn_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_SCHURN, ms4, 4); }
 
 // ------------------------------------------------------------------------------------- SPEC section 19 test-smell churn
 // The line records of both sides with their header events, per side the case spans and the smell stage, one synchronisation

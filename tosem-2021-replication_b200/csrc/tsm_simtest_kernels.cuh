@@ -98,21 +98,22 @@ __global__ void __launch_bounds__(256) k_st_lists(const StToken* tok, const uint
 
 // The candidates of a list of m tests, m (m - 1) / 2, scanned exclusively into cbase[n + 1] (tile sums, k_xscan_top, apply).
 __device__ __forceinline__ unsigned long long st_pairs_of(uint32_t m) { return (unsigned long long)m * (m ? m - 1u : 0u) / 2u; }
-__global__ void __launch_bounds__(256) k_st_csums(const uint32_t* pcnt, uint32_t n, unsigned long long* bsum) {
+// Tile sums and apply of an exclusive scan of per-list u64 counts cnt(i), as the xscan of tsm_lines_kernels.cuh.
+template <typename Cnt> __device__ __forceinline__ void st_csums(Cnt cnt, uint32_t n, unsigned long long* bsum) {
   __shared__ unsigned long long sh[8];
   const uint32_t i0 = blockIdx.x * XS_TILE + threadIdx.x * 4u;
   unsigned long long s = 0;
 #pragma unroll
-  for (uint32_t k = 0; k < 4; ++k) if (i0 + k < n) s += st_pairs_of(pcnt[i0 + k]);
+  for (uint32_t k = 0; k < 4; ++k) if (i0 + k < n) s += cnt(i0 + k);
   s = block_sum(s, sh);
   if (threadIdx.x == 0) bsum[blockIdx.x] = s;
 }
-__global__ void __launch_bounds__(256) k_st_capply(const uint32_t* pcnt, uint32_t n, const unsigned long long* bsum, unsigned long long* out) {
+template <typename Cnt> __device__ __forceinline__ void st_capply(Cnt cnt, uint32_t n, const unsigned long long* bsum, unsigned long long* out) {
   __shared__ unsigned long long wsum[8];
   const uint32_t i0 = blockIdx.x * XS_TILE + threadIdx.x * 4u;
   unsigned long long v[4], s = 0;
 #pragma unroll
-  for (uint32_t k = 0; k < 4; ++k) { v[k] = i0 + k < n ? st_pairs_of(pcnt[i0 + k]) : 0ull; s += v[k]; }
+  for (uint32_t k = 0; k < 4; ++k) { v[k] = i0 + k < n ? cnt(i0 + k) : 0ull; s += v[k]; }
   unsigned long long incl = s;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
 #pragma unroll
@@ -125,6 +126,12 @@ __global__ void __launch_bounds__(256) k_st_capply(const uint32_t* pcnt, uint32_
   for (uint32_t k = 0; k < 4; ++k) { if (i0 + k < n) out[i0 + k] = off; off += v[k]; }
   if (blockIdx.x == 0 && threadIdx.x == 0) out[n] = bsum[gridDim.x];
 }
+__global__ void __launch_bounds__(256) k_st_csums(const uint32_t* pcnt, uint32_t n, unsigned long long* bsum) {
+  st_csums([=](uint32_t i) { return st_pairs_of(pcnt[i]); }, n, bsum);
+}
+__global__ void __launch_bounds__(256) k_st_capply(const uint32_t* pcnt, uint32_t n, const unsigned long long* bsum, unsigned long long* out) {
+  st_capply([=](uint32_t i) { return st_pairs_of(pcnt[i]); }, n, bsum, out);
+}
 
 struct StEnum {
   const unsigned long long* cbase; uint32_t n_lists;      // candidates before each list [n_lists + 1]
@@ -136,6 +143,26 @@ struct StEnum {
 
 __device__ __forceinline__ bool st_less(const StToken& a, const StToken& b) {
   return a.cnt != b.cnt ? a.cnt < b.cnt : a.hslot != b.hslot ? a.hslot < b.hslot : a.j < b.j;
+}
+
+// The candidate pair of tests x and y of list s: kept (appended to the survivors) when it passes the size filter and the
+// list's token is the first token the two prefixes share.
+__device__ __forceinline__ void st_keep(const StEnum& a, uint32_t s, uint32_t x, uint32_t y) {
+  const uint32_t ta = min(x, y), tb = max(x, y);
+  const uint32_t ka = a.kk[ta], kb = a.kk[tb];
+  if (200ull * min(ka, kb) < (unsigned long long)a.P * (ka + kb)) return;
+  const StToken* pa = a.tok + a.pbase[ta];
+  const StToken* pb = a.tok + a.pbase[tb];
+  const uint32_t qa = a.q[ta], qb = a.q[tb];
+  uint32_t ia = 0, ib = 0, first = ST_NONE;
+  while (ia < qa && ib < qb) {
+    const StToken u = pa[ia], w = pb[ib];
+    if (st_less(u, w)) ++ia;
+    else if (st_less(w, u)) ++ib;
+    else { first = u.pslot; break; }
+  }
+  if (first != s) return;
+  a.surv[atomicAdd(a.n_surv, 1u)] = make_uint2(ta, tb);
 }
 
 // Grid-stride over the virtual candidates [c0, c0 + n): candidate v is the pair (i, j), i < j, of the list whose range of
@@ -154,22 +181,7 @@ __global__ void __launch_bounds__(256) k_st_enum(StEnum a, unsigned long long c0
     while (j * (j - 1) / 2 > r) --j;
     while ((j + 1) * j / 2 <= r) ++j;
     const unsigned long long i = r - j * (j - 1) / 2;
-    const uint32_t x = a.mem[a.mbase[s] + i], y = a.mem[a.mbase[s] + j];
-    const uint32_t ta = min(x, y), tb = max(x, y);
-    const uint32_t ka = a.kk[ta], kb = a.kk[tb];
-    if (200ull * min(ka, kb) < (unsigned long long)a.P * (ka + kb)) continue;
-    const StToken* pa = a.tok + a.pbase[ta];
-    const StToken* pb = a.tok + a.pbase[tb];
-    const uint32_t qa = a.q[ta], qb = a.q[tb];
-    uint32_t ia = 0, ib = 0, first = ST_NONE;
-    while (ia < qa && ib < qb) {
-      const StToken u = pa[ia], w = pb[ib];
-      if (st_less(u, w)) ++ia;
-      else if (st_less(w, u)) ++ib;
-      else { first = u.pslot; break; }
-    }
-    if (first != s) continue;
-    a.surv[atomicAdd(a.n_surv, 1u)] = make_uint2(ta, tb);
+    st_keep(a, s, a.mem[a.mbase[s] + i], a.mem[a.mbase[s] + j]);
   }
 }
 
@@ -261,6 +273,93 @@ __global__ void __launch_bounds__(256) k_st_verify(const uint2* surv, const uint
     if (lane == 0 && 200ull * lcs >= (unsigned long long)P * (ka + kb))
       pairs[atomicAdd(n_pairs, 1u)] = tsm_similar_pair{(int32_t)ab.x, (int32_t)ab.y, lcs,
                                                        (uint32_t)(120000ull * lcs / ((unsigned long long)ka + kb))};
+  }
+}
+
+// ------------------------------------------------------------------------------------- SPEC section 24 similar-test churn
+// One warp per matched test (old test o, new test n): same[k] = 1 when neither body holds a marked line (deleted in the old
+// body, inserted in the new), the bodies have equal body_lines and the two sequences of kept blind hashes are equal.  A
+// test's kept lines are [rank[l0], rank[l0 + body_lines]) of its side's blind front, l0 its header line.
+struct ScChangeSide {
+  const tsm_smell_test* tests; const unsigned long long* line_base; const uint8_t* mark; const unsigned long long* rank;
+  const unsigned long long* khash;
+};
+__global__ void __launch_bounds__(256) k_sc_change(ScChangeSide o, ScChangeSide w, const uint2* match, uint32_t n, uint8_t* same) {
+  const uint32_t FULL = 0xffffffffu;
+  const uint32_t lane = threadIdx.x & 31, warps = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; k < n; k += warps) {
+    const uint2 m = match[k];
+    const tsm_smell_test to = o.tests[m.x], tn = w.tests[m.y];
+    const unsigned long long lo = o.line_base[to.file] + (uint32_t)to.line, ln = w.line_base[tn.file] + (uint32_t)tn.line;
+    const unsigned long long bo = o.rank[lo], bn = w.rank[ln];
+    const uint32_t ko = (uint32_t)(o.rank[lo + (uint32_t)to.body_lines] - bo), kn = (uint32_t)(w.rank[ln + (uint32_t)tn.body_lines] - bn);
+    bool eq = to.body_lines == tn.body_lines && ko == kn;
+    const uint32_t nb = (uint32_t)to.body_lines;
+    for (uint32_t i0 = 0; eq && i0 < nb; i0 += 32) {     // (eq and the bounds are the same in every lane)
+      const uint32_t i = i0 + lane;
+      eq = !__any_sync(FULL, i < nb && (o.mark[lo + i] | w.mark[ln + i]));
+    }
+    const unsigned long long* ho = o.khash + bo;
+    const unsigned long long* hn = w.khash + bn;
+    for (uint32_t i0 = 0; eq && i0 < ko; i0 += 32) {
+      const uint32_t i = i0 + lane;
+      eq = __all_sync(FULL, i >= ko || ho[i] == hn[i]);
+    }
+    if (lane == 0) same[k] = eq;
+  }
+}
+
+// One thread per prefix token: the dirty tests of each posting list, dcnt[list].
+__global__ void __launch_bounds__(256) k_sc_dirty(const StToken* tok, const uint32_t* ptest, const unsigned long long* np,
+                                                  const uint8_t* dirty, uint32_t* dcnt) {
+  const unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
+  if (i >= *np || !dirty[ptest[i]]) return;
+  atomicAdd(&dcnt[tok[i].pslot], 1u);
+}
+
+// k_st_lists with the dirty tests of every list first: a dirty test takes the next of the list's first dcnt slots, a clean
+// one the next slot behind them.
+__global__ void __launch_bounds__(256) k_sc_lists(const StToken* tok, const uint32_t* ptest, const unsigned long long* np,
+                                                  const unsigned long long* mbase, const uint8_t* dirty, const uint32_t* dcnt,
+                                                  uint32_t* dcur, uint32_t* ccur, uint32_t* mem) {
+  const unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x;
+  if (i >= *np) return;
+  const uint32_t ps = tok[i].pslot, t = ptest[i];
+  mem[mbase[ps] + (dirty[t] ? atomicAdd(&dcur[ps], 1u) : dcnt[ps] + atomicAdd(&ccur[ps], 1u))] = t;
+}
+
+// The restricted candidates of a list of m tests whose first d are dirty: the pairs (i, j), i < d, i < j < m, row i
+// (m - 1 - i of them) starting at sc_row(m, i) = i m - i (i + 1) / 2; d m - d (d + 1) / 2 in all (m (m - 1) / 2 when d = m).
+__device__ __forceinline__ unsigned long long sc_row(uint32_t m, unsigned long long i) { return i * m - i * (i + 1) / 2; }
+__global__ void __launch_bounds__(256) k_sc_csums(const uint32_t* pcnt, const uint32_t* dcnt, uint32_t n, unsigned long long* bsum) {
+  st_csums([=](uint32_t i) { return sc_row(pcnt[i], dcnt[i]); }, n, bsum);
+}
+__global__ void __launch_bounds__(256) k_sc_capply(const uint32_t* pcnt, const uint32_t* dcnt, uint32_t n, const unsigned long long* bsum,
+                                                   unsigned long long* out) {
+  st_capply([=](uint32_t i) { return sc_row(pcnt[i], dcnt[i]); }, n, bsum, out);
+}
+
+// k_st_enum over the restricted space: candidate v is the pair (i, j) of the list whose range of cbase holds v, i found from
+// the row offsets (the root of i^2 - (2m - 1) i + 2r = 0, then corrected), with the same filters; so every pair of tests of
+// which at least one is dirty is kept once, and no pair of two clean tests is looked at.
+__global__ void __launch_bounds__(256) k_sc_enum(StEnum a, const uint32_t* pcnt, const uint32_t* dcnt, unsigned long long c0,
+                                                 unsigned long long n) {
+  for (unsigned long long v = c0 + blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; v < c0 + n;
+       v += (unsigned long long)gridDim.x * blockDim.x) {
+    uint32_t lo = 0, hi = a.n_lists - 1;
+    while (lo < hi) {
+      const uint32_t mid = lo + (hi - lo + 1) / 2;
+      if (a.cbase[mid] <= v) lo = mid; else hi = mid - 1;
+    }
+    const uint32_t s = lo, m = pcnt[s], d = dcnt[s];
+    const unsigned long long r = v - a.cbase[s];
+    const double b = 2.0 * m - 1.0, disc = b * b - 8.0 * (double)r;
+    unsigned long long i = (unsigned long long)fmax(0.0, (b - sqrt(fmax(disc, 0.0))) * 0.5);
+    if (i >= d) i = d - 1;
+    while (i > 0 && sc_row(m, i) > r) --i;
+    while (i + 1 < d && sc_row(m, i + 1) <= r) ++i;
+    const unsigned long long j = i + 1 + (r - sc_row(m, i));
+    st_keep(a, s, a.mem[a.mbase[s] + i], a.mem[a.mbase[s] + j]);
   }
 }
 

@@ -18,11 +18,11 @@
 //   tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N]
 //   tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]
 //   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--smells F]
-//                     [--moves F] [--find-renames N] [--batch-bytes N]
+//                     [--moves F] [--clones F] [--similar-tests F] [--min-lines N] [--similarity P] [--find-renames N] [--batch-bytes N]
 //   tosem-scan body   <project-root>... [--batch-bytes N] [--out F]
 //   tosem-scan releases <snapshot-root>=<tag>... | --git <repository> [<revision>...]   [--batch-bytes N] [--out F]
 //   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F] [--cases F]
-//                      [--assert-edits F] [--smells F] [--moves F] [--find-renames N] [--batch-bytes N]
+//                      [--assert-edits F] [--smells F] [--moves F] [--clones F] [--similar-tests F] [--find-renames N] [--batch-bytes N]
 //   tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]
 //   tosem-scan clones <project-root>... | --git <repository> [--rev R]   [--min-lines N] [--blind] [--all-files] [--out F]
 // Every command that scans files does it with scan_batches: batches of at most --batch-bytes of arena (clones: all files in one),
@@ -58,14 +58,17 @@
 
 #include "../../include/tosemscan.h"
 #include "git_store.hpp"
+#include "tsm_names.hpp"
 
 namespace fs = std::filesystem;
+using tsm_names::case_name;
+using tsm_names::is_w;
+using tsm_names::method_string;
 
 static bool die(const std::string& m) { fprintf(stderr, "tosem-scan: %s\n", m.c_str()); exit(2); return false; }
 static void ck(int rc, const char* what) { if (rc != TSM_OK) die(std::string(what) + ": " + tsm_strerror(rc)); }
 
 static std::string lower(std::string s) { for (char& c : s) if (c >= 'A' && c <= 'Z') c = (char)(c + 32); return s; }
-static bool is_w(unsigned char c) { return c == 0x20 || c == 0x09 || c == 0x0D || c == 0x0B || c == 0x0C; }
 
 // ---------------------------------------------------------------------------------- CSV (RFC 4180, CRLF)
 static std::string csv_cell(const std::string& s) {
@@ -163,43 +166,6 @@ static void walk(const std::string& root, int grp, bool all_files, std::vector<F
     }
     out.push_back({rel, p.string(), ext, grp, (int64_t)fs::file_size(p), nullptr});
   }
-}
-
-// ---------------------------------------------------------------------------------- S3: method strings
-static std::string method_string(int ext, const uint8_t* line, uint32_t len) {   // docs/SPEC.md section 5
-  uint32_t b = 0, e = len;
-  while (b < e && is_w(line[b])) ++b;
-  while (e > b && is_w(line[e - 1])) --e;
-  auto sw = [&](uint32_t i, const char* pat) { const size_t m = strlen(pat); return i + m <= e && memcmp(line + i, pat, m) == 0; };
-  std::string o;
-  if (ext == TSM_EXT_PY) {
-    uint32_t i = b;
-    if (sw(i, "class")) i += 5;
-    while (i < e) {
-      if (sw(i, "def")) { i += 3; continue; }
-      if (!is_w(line[i])) o += (char)line[i];
-      ++i;
-    }
-    if (!o.empty() && o.back() == ':') o.pop_back();
-  } else if (ext == TSM_EXT_JAVA) {
-    static const char* const words[] = {"public", "private", "protected", "static", "void", "class"};
-    uint32_t i = b;
-    while (i < e) {
-      bool hit = false;
-      for (const char* w : words) if (sw(i, w)) { i += (uint32_t)strlen(w); hit = true; break; }
-      if (hit) continue;
-      if (!is_w(line[i])) o += (char)line[i];
-      ++i;
-    }
-  } else {
-    uint32_t t = b;
-    while (t < e && line[t] != ')') ++t;
-    uint32_t s = b, u = t;
-    while (s < t && (is_w(line[s]) || line[s] == '{')) ++s;
-    while (u > s && (is_w(line[u - 1]) || line[u - 1] == '{')) --u;
-    for (uint32_t i = s; i < u; ++i) if (line[i] != '{') o += (char)line[i];
-  }
-  return o;
 }
 
 // ---------------------------------------------------------------------------------- scan
@@ -850,35 +816,6 @@ static int cmd_reduce(const std::string& path, const std::string& strategy_path,
 }
 
 // ---------------------------------------------------------------------------------- body statements (SPEC section 10)
-// Case name of a header line: PY - identifier after `def`; C family - 2nd macro argument of TEST / TEST_F /
-// TEST_P, `TEST_CASE(X)` for BOOST_AUTO_TEST_CASE(X); otherwise the SPEC section 5 method string.
-static std::string case_name(int ext, const uint8_t* line, uint32_t len) {
-  uint32_t b = 0, e = len;
-  while (b < e && is_w(line[b])) ++b;
-  while (e > b && is_w(line[e - 1])) --e;
-  const std::string s((const char*)line + b, e - b);
-  if (ext == TSM_EXT_PY) {
-    const size_t d = s.find("def");
-    if (d != std::string::npos) {
-      size_t i = d + 3;
-      while (i < s.size() && is_w((unsigned char)s[i])) ++i;
-      size_t j = i;
-      while (j < s.size() && (isalnum((unsigned char)s[j]) || s[j] == '_')) ++j;
-      if (j > i) return s.substr(i, j - i);
-    }
-  } else {
-    auto trim = [](std::string t) { size_t a = 0, z = t.size(); while (a < z && is_w((unsigned char)t[a])) ++a; while (z > a && is_w((unsigned char)t[z - 1])) --z; return t.substr(a, z - a); };
-    if (s.rfind("TEST(", 0) == 0 || s.rfind("TEST_F(", 0) == 0 || s.rfind("TEST_P(", 0) == 0) {
-      const size_t c = s.find(','), r = s.find(')');
-      if (c != std::string::npos && (r == std::string::npos || c < r)) return trim(s.substr(c + 1, (r == std::string::npos ? s.size() : r) - c - 1));
-    }
-    if (s.rfind("BOOST_AUTO_TEST_CASE(", 0) == 0) {
-      const size_t r = s.find(')');
-      return "TEST_CASE(" + trim(s.substr(21, (r == std::string::npos ? s.size() : r) - 21)) + ")";
-    }
-  }
-  return method_string(ext, line, len);
-}
 
 static int cmd_body(const std::vector<std::string>& roots, const std::string& out_path, int64_t batch_bytes) {
   std::vector<FileEntry> files;
@@ -1312,11 +1249,7 @@ struct PairCaseMatch {
       : na(case_names(o.base, o.size, o.ext, oc, no)), nb(case_names(nw.base, nw.size, nw.ext, nc, nn)), match(nn, -1), used(no, 0) {
     for (size_t j = 0; j < nn; ++j)
       if (nc[j].match >= 0) { match[j] = nc[j].match - (int64_t)o_first; used[(size_t)match[j]] = 1; }
-    std::map<std::string, int64_t> cnt_new, cnt_old, old_of;
-    for (size_t j = 0; j < nn; ++j) if (match[j] < 0) ++cnt_new[nb[j]];
-    for (size_t k = 0; k < no; ++k) if (!used[k]) { ++cnt_old[na[k]]; old_of[na[k]] = (int64_t)k; }
-    for (size_t j = 0; j < nn; ++j)
-      if (match[j] < 0 && cnt_new[nb[j]] == 1 && cnt_old[nb[j]] == 1) { match[j] = old_of[nb[j]]; used[(size_t)match[j]] = 1; }
+    tsm_names::match_by_name(na, nb, match, used);
   }
 };
 
@@ -1635,6 +1568,8 @@ struct DiffOptions {
   std::string out, asserts, churn, cases, edits, smells, moves;
   std::string clones;                                      // --clones F, with its --min-lines, --blind and the file selection
   int clone_min_lines = 5; bool clone_blind = false, all_files = false;
+  std::string similar;                                     // --similar-tests F, with --min-lines (shared with --clones) and --similarity
+  int similar_min_lines = 5, similar_pct = 70;
   bool zero_rows = false;
   std::vector<std::string> lead_head;
   size_t churn_lead = 0;
@@ -1804,19 +1739,29 @@ static Revision make_revision(const std::map<std::string, Blob, PathLess>& files
 static const char* const kCloneStatus[] = {"untouched", "changed", "removed", "diverged", "dropped", "created", "copied", "joined"};
 static const char* const kFragState[] = {"kept", "edited", "whole"};
 
-// One step: tsm_clone_churn over the two revisions and the step's changes (after --find-renames; `old_path` names the old side of
-// a rename), then one row per fragment of every touched class, the old side first.  A change binary on a side (a NUL byte in its
-// first 8000) is a deletion plus an addition: all of its lines are marked.
-static void clone_churn_step(tsm_ctx* ctx, const Revision& ro, const Revision& rn, const Change* c0, const Change* c1,
-                             const std::function<bool(const Change&)>& is_binary, const DiffOptions& d,
-                             const std::vector<std::string>& lead, std::ostream& os) {
-  std::vector<int32_t> po, pn;
+// The file pairs of one step: the step's changes (after --find-renames; `old_path` names the old side of a rename) as file
+// indices of the two revisions.  A change binary on a side (a NUL byte in its first 8000) is a deletion plus an addition.
+struct StepPairs { std::vector<int32_t> po, pn; };
+static StepPairs step_pairs(const Revision& ro, const Revision& rn, const Change* c0, const Change* c1,
+                            const std::function<bool(const Change&)>& is_binary) {
+  StepPairs sp;
   for (const Change* c = c0; c != c1; ++c) {
     const int32_t a = c->o >= 0 ? ro.index.at(c->old_path.empty() ? c->path : c->old_path) : -1;
     const int32_t b = c->n >= 0 ? rn.index.at(c->path) : -1;
-    if (a >= 0 && b >= 0 && is_binary(*c)) { po.push_back(a); pn.push_back(-1); po.push_back(-1); pn.push_back(b); }
-    else { po.push_back(a); pn.push_back(b); }
+    if (a >= 0 && b >= 0 && is_binary(*c)) { sp.po.push_back(a); sp.pn.push_back(-1); sp.po.push_back(-1); sp.pn.push_back(b); }
+    else { sp.po.push_back(a); sp.pn.push_back(b); }
   }
+  return sp;
+}
+
+// What the step driver hands each step to: the two revisions, the step's pairs and the lead cells of its rows.
+using StepSink = std::function<void(tsm_ctx*, const Revision&, const Revision&, const StepPairs&, const std::vector<std::string>&)>;
+
+// One step of --clones: tsm_clone_churn over the two revisions and the step's pairs, then one row per fragment of every touched
+// class, the old side first.
+static void clone_churn_step(tsm_ctx* ctx, const Revision& ro, const Revision& rn, const StepPairs& sp, const DiffOptions& d,
+                             const std::vector<std::string>& lead, std::ostream& os) {
+  const std::vector<int32_t>&po = sp.po, &pn = sp.pn;
   const Revision* rev[2] = {&ro, &rn};
   struct Side { std::vector<int64_t> base, cbase, member, kbase, kline; std::vector<uint32_t> clen, changed, changed_a, counts; std::vector<uint8_t> state, status; };
   Side S[2];
@@ -1872,9 +1817,9 @@ static std::vector<std::string> clone_churn_head(std::vector<std::string> lead) 
   return lead;
 }
 
-// `diff --clones`: the selected files of each root (S0 / S1 unless --all-files) are the two revisions; a file whose bytes differ, or
-// that one root lacks, is a change (then --find-renames); one clone_churn_step.
-static void diff_clone_churn(const std::string& old_root, const std::string& new_root, const DiffOptions& o) {
+// `diff --clones` / `--similar-tests`: the selected files of each root (S0 / S1 unless --all-files) are the two revisions; a file
+// whose bytes differ, or that one root lacks, is a change (then --find-renames); one step, handed to every sink.
+static void diff_steps(const std::string& old_root, const std::string& new_root, const DiffOptions& o, const std::vector<StepSink>& sinks) {
   std::vector<FileEntry> fa, fb;
   walk(old_root, 0, o.all_files, fa);
   walk(new_root, 0, o.all_files, fb);
@@ -1902,10 +1847,109 @@ static void diff_clone_churn(const std::string& old_root, const std::string& new
   ChangeTotals t(1);
   if (o.rename_pct >= 0) pair_renames(ctx.get(), changes, load, o.rename_pct, o.batch_bytes, t);
   const Revision ro = make_revision(ra), rn = make_revision(rb);
-  std::ofstream os(o.clones, std::ios::binary);
-  csv_row(os, clone_churn_head({}));
-  clone_churn_step(ctx.get(), ro, rn, changes.data(), changes.data() + changes.size(),
-                   [&](const Change& c) { return binary(*blobs[(size_t)c.o]) || binary(*blobs[(size_t)c.n]); }, o, {}, os);
+  const StepPairs sp = step_pairs(ro, rn, changes.data(), changes.data() + changes.size(),
+                                  [&](const Change& c) { return binary(*blobs[(size_t)c.o]) || binary(*blobs[(size_t)c.n]); });
+  for (const StepSink& sink : sinks) sink(ctx.get(), ro, rn, sp, {});
+}
+
+// ---------------------------------------------------------------------------------- similar-test churn (docs/SPEC.md section 24)
+static const char* const kSimilarStatus[] = {"changed", "removed", "dropped", "diverged", "created", "copied", "converged"};
+
+// The 1-based header line and the case name (section 10) of every test of a revision, from the files' bytes.
+struct TestNames { std::vector<std::string> name; };
+static TestNames test_names(const Revision& r, const std::vector<tsm_smell_test>& tests) {
+  TestNames out;
+  int32_t f = -1, line = 0;
+  size_t pos = 0;
+  for (const tsm_smell_test& t : tests) {                  // tests in global line order: one walk per file
+    const std::vector<uint8_t>& b = *r.blobs[(size_t)t.file];
+    if (t.file != f) { f = t.file; line = 0; pos = 0; }
+    for (; line < t.line; ++line) pos = (size_t)((const uint8_t*)memchr(b.data() + pos, '\n', b.size() - pos) - b.data()) + 1;
+    const uint8_t* lf = (const uint8_t*)memchr(b.data() + pos, '\n', b.size() - pos);
+    out.name.push_back(case_name(ext_tag(r.paths[(size_t)f]), b.data() + pos, (uint32_t)((lf ? (size_t)(lf - b.data()) : b.size()) - pos)));
+  }
+  return out;
+}
+
+// One step of --similar-tests: tsm_similar_churn over the two revisions and the step's pairs (counts first, then the arrays), then
+// one row per event.  A row names its test and the other test of the pair, each on both sides (empty cells for a side without it).
+static void similar_churn_step(tsm_ctx* ctx, const Revision& ro, const Revision& rn, const StepPairs& sp, const DiffOptions& d,
+                               const std::vector<std::string>& lead, std::ostream& os) {
+  const tsm_corpus co = ro.b.corpus(1), cn = rn.b.corpus(1);
+  tsm_similar_churn_side cs[2] = {};
+  int64_t n_ev = 0;
+  auto call = [&](tsm_similar_event* ev) {
+    ck(tsm_similar_churn(ctx, &co, &cn, sp.po.data(), sp.pn.data(), (int64_t)sp.po.size(), d.similar_min_lines, d.similar_pct, &cs[0],
+                         &cs[1], ev, n_ev, &n_ev, nullptr), "tsm_similar_churn");
+  };
+  call(nullptr);
+  std::vector<tsm_smell_test> tests[2];
+  std::vector<int32_t> match[2];
+  std::vector<uint8_t> change[2];
+  for (int s = 0; s < 2; ++s) {
+    const size_t nt = (size_t)cs[s].n_tests;
+    tests[s].resize(std::max<size_t>(nt, 1)); match[s].resize(std::max<size_t>(nt, 1)); change[s].resize(std::max<size_t>(nt, 1));
+    cs[s].tests = tests[s].data(); cs[s].match = match[s].data(); cs[s].change = change[s].data(); cs[s].test_cap = (int64_t)nt;
+    tests[s].resize(nt);
+  }
+  std::vector<tsm_similar_event> ev(std::max<int64_t>(n_ev, 1));
+  call(ev.data());
+  const Revision* rev[2] = {&ro, &rn};
+  const TestNames names[2] = {test_names(ro, tests[0]), test_names(rn, tests[1])};
+  auto num = [](int64_t v) { return std::to_string(v); };
+  // The cells of one test given by its index on each side (-1: absent): fileName, test, oldLine, line, change, and its old path.
+  auto cells = [&](int32_t o, int32_t n, std::vector<std::string>& row, std::string& old_path) {
+    const int s = n >= 0 ? 1 : 0;
+    const int32_t t = s ? n : o;
+    const tsm_smell_test& x = tests[s][(size_t)t];
+    row.insert(row.end(), {rev[s]->paths[(size_t)x.file], names[s].name[(size_t)t], o >= 0 ? num(tests[0][(size_t)o].line + 1) : "",
+                           n >= 0 ? num(tests[1][(size_t)n].line + 1) : "", std::string(1, (char)change[s][(size_t)t])});
+    old_path = o >= 0 ? ro.paths[(size_t)tests[0][(size_t)o].file] : "";
+  };
+  const uint32_t NONE = 0xFFFFFFFFu;
+  auto pct = [&](uint32_t v) { return v == NONE ? std::string() : num(v / 600); };
+  auto lcs = [&](uint32_t v) { return v == NONE ? std::string() : num(v); };
+  for (int64_t k = 0; k < n_ev; ++k) {
+    const tsm_similar_event& e = ev[(size_t)k];
+    std::vector<std::string> row = lead;
+    row.push_back(kSimilarStatus[e.status]);
+    std::string op_a, op_b;
+    cells(e.old_a, e.a, row, op_a);
+    cells(e.old_b, e.b, row, op_b);
+    row.insert(row.end(), {lcs(e.old_lcs), pct(e.old_score), lcs(e.lcs), pct(e.score)});
+    if (d.rename_pct >= 0) row.insert(row.end(), {op_a, op_b});
+    csv_row(os, row);
+  }
+}
+
+static std::vector<std::string> similar_churn_head(std::vector<std::string> lead, bool renames) {
+  lead.insert(lead.end(), {"status", "fileName", "test", "oldLine", "line", "change", "otherFileName", "otherTest", "otherOldLine",
+                           "otherLine", "otherChange", "oldLcs", "oldSimilarity", "lcs", "similarity"});
+  if (renames) lead.insert(lead.end(), {"oldFileName", "otherOldFileName"});
+  return lead;
+}
+
+// The outputs of --clones and --similar-tests: their files with their header rows, and one sink each; `walk` runs the step driver
+// once over all of them (nothing when neither is asked for).
+static void step_outputs(const DiffOptions& o, const std::vector<std::string>& lead_head,
+                         const std::function<void(const std::vector<StepSink>&)>& walk) {
+  std::ofstream clones, similar;
+  std::vector<StepSink> sinks;
+  if (!o.clones.empty()) {
+    clones.open(o.clones, std::ios::binary);
+    csv_row(clones, clone_churn_head(lead_head));
+    sinks.push_back([&](tsm_ctx* ctx, const Revision& ro, const Revision& rn, const StepPairs& sp, const std::vector<std::string>& lead) {
+      clone_churn_step(ctx, ro, rn, sp, o, lead, clones);
+    });
+  }
+  if (!o.similar.empty()) {
+    similar.open(o.similar, std::ios::binary);
+    csv_row(similar, similar_churn_head(lead_head, o.rename_pct >= 0));
+    sinks.push_back([&](tsm_ctx* ctx, const Revision& ro, const Revision& rn, const StepPairs& sp, const std::vector<std::string>& lead) {
+      similar_churn_step(ctx, ro, rn, sp, o, lead, similar);
+    });
+  }
+  if (!sinks.empty()) walk(sinks);
 }
 
 static int cmd_diff(const std::string& old_root, const std::string& new_root, const DiffOptions& o) {
@@ -1927,7 +1971,7 @@ static int cmd_diff(const std::string& old_root, const std::string& new_root, co
     return v;
   };
   const ChangeTotals t = diff_changes(changes, 1, load, o);
-  if (!o.clones.empty()) diff_clone_churn(old_root, new_root, o);
+  step_outputs(o, {}, [&](const std::vector<StepSink>& sinks) { diff_steps(old_root, new_root, o, sinks); });
   if (t.binaries) fprintf(stderr, "tosem-scan: %lld binary file(s) skipped\n", (long long)t.binaries);
   if (o.rename_pct >= 0)
     fprintf(stderr, "tosem-scan: %lld rename(s) found (%lld exact, %lld inexact)\n", (long long)t.renames, (long long)t.renames_exact,
@@ -2009,10 +2053,10 @@ struct History {
   }
 };
 
-// `history --clones`: the selected files of the current revision kept as live paths, from the boundary commit's tree (the parent of
-// the window's first commit; none for a root commit) and each commit's changes after --find-renames.  Blobs are read once while
-// they are live (cached by object name), and a revision is packed once: the new side of one tsm_clone_churn call is the old side
-// of the next.  One clone_churn_step per commit that changes a selected file.
+// `history --clones` / `--similar-tests`: the selected files of the current revision kept as live paths, from the boundary commit's
+// tree (the parent of the window's first commit; none for a root commit) and each commit's changes after --find-renames.  Blobs
+// are read once while they are live (cached by object name), and a revision is packed once: the new side of one step is the old
+// side of the next.  Every sink gets each commit that changes a selected file, from one walk.
 static void selected_blobs(gitstore::Store& gs, const gitstore::Oid& tree, const std::string& prefix, bool all_files,
                            std::map<std::string, gitstore::Oid, PathLess>& out) {
   std::vector<gitstore::TreeEntry> es;
@@ -2026,7 +2070,7 @@ static void selected_blobs(gitstore::Store& gs, const gitstore::Oid& tree, const
   }
 }
 
-static void history_clone_churn(History& h, const DiffOptions& o) {
+static void history_steps(History& h, const DiffOptions& o, const std::vector<StepSink>& sinks) {
   std::vector<Change> changes = h.changes;
   const auto ctx = small_context();
   ChangeTotals t(h.chain.size());
@@ -2052,8 +2096,6 @@ static void history_clone_churn(History& h, const DiffOptions& o) {
     }
     return f;
   };
-  std::ofstream os(o.clones, std::ios::binary);
-  csv_row(os, clone_churn_head(o.lead_head));
   std::unique_ptr<Revision> cur;
   for (size_t c0 = 0, c1 = 0; c0 < changes.size(); c0 = c1) {
     for (c1 = c0; c1 < changes.size() && changes[c1].step == changes[c0].step; ++c1) {}
@@ -2065,7 +2107,9 @@ static void history_clone_churn(History& h, const DiffOptions& o) {
       if (changes[c].n >= 0) next[changes[c].path] = h.objs[(size_t)changes[c].n];
     auto rn = std::make_unique<Revision>(make_revision(files_of(next)));
     auto is_binary = [&](const Change& c) { return binary(*cache.at(h.objs[(size_t)c.o])) || binary(*cache.at(h.objs[(size_t)c.n])); };
-    clone_churn_step(ctx.get(), *cur, *rn, changes.data() + c0, changes.data() + c1, is_binary, o, o.lead(changes[c0].step), os);
+    const StepPairs sp = step_pairs(*cur, *rn, changes.data() + c0, changes.data() + c1, is_binary);
+    const std::vector<std::string> lead = o.lead(changes[c0].step);
+    for (const StepSink& sink : sinks) sink(ctx.get(), *cur, *rn, sp, lead);
     cur = std::move(rn);
     live.swap(next);
     std::set<gitstore::Oid> keep;                          // the cache holds the live blobs only
@@ -2102,7 +2146,8 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
     }
   } else {
     o.zero_rows = true; o.lead_head = {"commit", "parent", "time"}; o.churn_lead = 1;
-    if (!o.clones.empty()) history_clone_churn(h, o);      // (before diff_changes, which pairs the renames of h.changes in place)
+    step_outputs(o, o.lead_head, [&](const std::vector<StepSink>& sinks) { history_steps(h, o, sinks); });   // (before diff_changes,
+                                                           // which pairs the renames of h.changes in place)
     t = diff_changes(h.changes, h.chain.size(), h.load, o);
   }
   printf("commit,files,cloc,added,removed\r\n");
@@ -2595,12 +2640,12 @@ static void usage() {
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
           "       tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]\n"
           "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--smells F]\n"
-          "                         [--moves F] [--clones F [--min-lines N] [--blind] [--all-files]] [--find-renames N] [--batch-bytes N]\n"
+          "                         [--moves F] [--clones F [--min-lines N] [--blind] [--all-files]] [--similar-tests F [--min-lines N] [--similarity P]] [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan body   <project-root>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases <snapshot-root>=<tag>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases --git <repository> [<revision>...] [--batch-bytes N] [--out F]\n"
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
-          "                          [--cases F] [--assert-edits F] [--smells F] [--moves F] [--clones F [--min-lines N] [--blind]]\n"
+          "                          [--cases F] [--assert-edits F] [--smells F] [--moves F] [--clones F [--min-lines N] [--blind]] [--similar-tests F [--similarity P]]\n"
           "                          [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
           "       tosem-scan clones <project-root>... [--min-lines N] [--blind] [--all-files] [--out F]\n"
@@ -2626,6 +2671,9 @@ static void usage() {
           "           larger than --batch-bytes is a batch of its own.\n"
           "--clones F: per commit, one row per fragment of every clone class of the parent (-) or the commit (+) that the commit\n"
           "            edits, with the class's status (copied, diverged, ...) and the fragment's changed lines (docs/SPEC.md section 22).\n"
+          "--similar-tests F: per commit, one row per pair of similar tests (docs/SPEC.md section 23) that the commit creates, changes or\n"
+          "            breaks up (copied, changed, diverged, ...), with both tests on both sides and their similarity before and after\n"
+          "            (docs/SPEC.md section 24); --min-lines N (shared with --clones) and --similarity P as for similar-tests.\n"
           "--batch-bytes N: files go to the GPU in batches of at most N bytes (per side of a diff; a larger file alone); scan: 1 GiB, else 512 MiB.\n"
           "Scans run on the GPU through libtosemscan.so (sm_90a); there is no CPU fallback.\n");
 }
@@ -2691,6 +2739,15 @@ int main(int argc, char** argv) {
     if (n < 1 || n > 1024) die("--min-lines needs a number of lines from 1 to 1024");
     d.clone_min_lines = (int)n;
     if (dry_run) die("--dry-run and --clones cannot be combined (clone churn needs the GPU)");
+  }
+  if (opt.count("--similar-tests")) {                      // (--similarity is read only with --similar-tests)
+    d.similar = opt["--similar-tests"]; d.all_files = all_files;
+    const long n = opt.count("--min-lines") ? strtol(opt["--min-lines"].c_str(), nullptr, 10) : 5;
+    if (n < 1 || n > INT32_MAX) die("--min-lines needs a number of lines of at least 1");
+    const long p = opt.count("--similarity") ? strtol(opt["--similarity"].c_str(), nullptr, 10) : 70;
+    if (p < 1 || p > 100) die("--similarity needs a percentage from 1 to 100");
+    d.similar_min_lines = (int)n; d.similar_pct = (int)p;
+    if (dry_run) die("--dry-run and --similar-tests cannot be combined (similar-test churn needs the GPU)");
   }
   const std::string rev = opt.count("--rev") ? opt["--rev"] : "HEAD";
   const int64_t max_commits = opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0;

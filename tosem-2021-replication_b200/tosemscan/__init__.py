@@ -41,6 +41,9 @@ MOVE_BLOCK = np.dtype([("line", "<i8"), ("partner", "<i8"), ("n_lines", "<i4"),
                        ("n_assert", "<i4")])   # tsm_move_block: one moved block of one side (docs/SPEC.md section 20)
 SIMILAR_PAIR = np.dtype([("a", "<i4"), ("b", "<i4"), ("lcs", "<u4"),
                          ("score", "<u4")])   # tsm_similar_pair: two similar tests, a < b (docs/SPEC.md section 23)
+SIMILAR_EVENT = np.dtype([("status", "<i4"), ("old_a", "<i4"), ("old_b", "<i4"), ("a", "<i4"), ("b", "<i4"), ("old_lcs", "<u4"),
+                          ("old_score", "<u4"), ("lcs", "<u4"), ("score", "<u4")])   # tsm_similar_event (docs/SPEC.md section 24)
+SIMILAR_STATUSES = ["changed", "removed", "dropped", "diverged", "created", "copied", "converged"]   # SIMILAR_EVENT status
 ASSERT_EDIT = np.dtype([("rev", "<i8"), ("aev", "<i8"), ("score", "<i4"), ("_pad", "<i4")])   # tsm_assert_edit: event indices
 
 # every symbol include/tosemscan.h declares (tests check the library exports exactly these)
@@ -52,7 +55,8 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_diff_pairs_marks", "tsm_blame_pairs", "tsm_blame_last_ms", "tsm_clones", "tsm_clones_last_ms",
            "tsm_diff_pairs_cases", "tsm_diff_pairs_assert_edits", "tsm_assert_edits_last_ms", "tsm_smells", "tsm_smells_last_ms",
            "tsm_diff_pairs_smells", "tsm_diff_smells_last_ms", "tsm_diff_pairs_moves", "tsm_moves_last_ms", "tsm_clones_blind",
-           "tsm_clones_blind_last_ms", "tsm_clone_churn", "tsm_clone_churn_last_ms", "tsm_similar_tests", "tsm_similar_tests_last_ms"]
+           "tsm_clones_blind_last_ms", "tsm_clone_churn", "tsm_clone_churn_last_ms", "tsm_similar_tests", "tsm_similar_tests_last_ms",
+           "tsm_similar_churn", "tsm_similar_churn_last_ms"]
 FRAG_STATES = ["kept", "edited", "whole"]          # tsm_clone_churn state[j] (docs/SPEC.md section 22)
 CLONE_STATUSES = ["untouched", "changed", "removed", "diverged", "dropped", "created", "copied", "joined"]   # status[c]
 
@@ -120,6 +124,11 @@ class _SimilarResult(C.Structure):
                 ("pairs", C.c_void_p), ("pair_cap", C.c_int64), ("n_pairs", C.c_int64),
                 ("class_base", C.c_void_p), ("class_cap", C.c_int64), ("n_classes", C.c_int64),
                 ("member", C.c_void_p), ("member_cap", C.c_int64), ("n_members", C.c_int64), ("n_candidates", C.c_int64)]
+
+
+class _SimilarChurnSide(C.Structure):
+    _fields_ = [("tests", C.c_void_p), ("test_kept", C.c_void_p), ("match", C.c_void_p), ("change", C.c_void_p), ("test_cap", C.c_int64),
+                ("n_tests", C.c_int64), ("n_candidates", C.c_int64)]
 
 
 class _CloneChurnSide(C.Structure):
@@ -242,6 +251,12 @@ def lib():
         L.tsm_similar_tests.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_int32, C.c_int32, C.POINTER(_SimilarResult), C.c_void_p]
         L.tsm_similar_tests_last_ms.restype = C.c_int
         L.tsm_similar_tests_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
+        L.tsm_similar_churn.restype = C.c_int
+        L.tsm_similar_churn.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus), C.c_void_p, C.c_void_p, C.c_int64, C.c_int32,
+                                        C.c_int32, C.POINTER(_SimilarChurnSide), C.POINTER(_SimilarChurnSide), C.c_void_p, C.c_int64,
+                                        C.POINTER(C.c_int64), C.c_void_p]
+        L.tsm_similar_churn_last_ms.restype = C.c_int
+        L.tsm_similar_churn_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
         L.tsm_smells_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
         L.tsm_diff_pairs_smells.restype = C.c_int
         L.tsm_diff_pairs_smells.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 3 + \
@@ -1028,6 +1043,56 @@ class Scanner:
         enumeration, verification] in ms."""
         ms = (C.c_float * 4)()
         lib().tsm_similar_tests_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
+
+    def similar_churn(self, old_rev, new_rev, pair_old, pair_new, min_lines=5, similarity=70, stream=None, cap=None):
+        """Similar-test churn (docs/SPEC.md section 24): a dict {"old": ..., "new": ..., "events": ...}.  Per revision tests
+        (SMELL_TEST, as similar_tests gives them), test_kept, match (the other side's test, -1 for none), change (b"A", b"D",
+        b"=" or b"M" per test, as uint8) and n_candidates; events (SIMILAR_EVENT, status indexing SIMILAR_STATUSES).  Pair k
+        is file pair_old[k] of old_rev and file pair_new[k] of new_rev, -1 for none; a file in no pair is unchanged and
+        matches the same-numbered unpaired file of the other revision.  Arrays too small for their counts are sized from
+        the counts and the call is made again, which repeats the whole call (cap: the first guess of each; by default the tests
+        of each revision are sized from its line count and the events from both, at least 2^16 and at most 2^22)."""
+        po = np.ascontiguousarray(pair_old, np.int32).ravel()
+        pn = np.ascontiguousarray(pair_new, np.int32).ravel()
+        if po.size != pn.size:
+            raise ValueError("pair_old and pair_new differ in length")
+        revs = (old_rev, new_rev)
+        cs = [r.c_struct() for r in revs]
+        if cap is None:
+            caps = [int(np.count_nonzero(np.asarray(r.arena[:int(r.off[r.n_files])]) == 0x0A)) + r.n_files for r in revs]
+            ce = min(max(sum(caps), 1 << 16), 1 << 22)
+        else:
+            caps, ce = [int(cap)] * 2, int(cap)
+        for _ in range(2):
+            outs, sides = [], []
+            for ct in caps:
+                o = {"tests": np.zeros(max(ct, 1), SMELL_TEST), "test_kept": np.zeros(max(ct, 1), np.uint32),
+                     "match": np.zeros(max(ct, 1), np.int32), "change": np.zeros(max(ct, 1), np.uint8)}
+                outs.append(o)
+                sides.append(_SimilarChurnSide(*[_p(o[k]) for k in ("tests", "test_kept", "match", "change")], ct, 0, 0))
+            ev = np.zeros(max(ce, 1), SIMILAR_EVENT)
+            ne = C.c_int64()
+            rc = lib().tsm_similar_churn(self._ctx, C.byref(cs[0]), C.byref(cs[1]), _p(po), _p(pn), po.size, int(min_lines), int(similarity),
+                                         C.byref(sides[0]), C.byref(sides[1]), _p(ev), ce, C.byref(ne), stream)
+            need = [int(sd.n_tests) for sd in sides]
+            if rc == TSM_E_CAPACITY and (ne.value > ce or any(w > h for w, h in zip(need, caps))):
+                caps, ce = need, int(ne.value)
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_similar_churn")
+            res = {"events": ev[:ne.value]}
+            for name, o, sd in zip(("old", "new"), outs, sides):
+                res[name] = {k: v[:sd.n_tests] for k, v in o.items()}
+                res[name]["n_candidates"] = int(sd.n_candidates)
+            return res
+        raise TsmError(TSM_E_CAPACITY, "tsm_similar_churn")
+
+    def similar_churn_last_ms(self):
+        """Device time of the last similar_churn call: [k_scan over both revisions, fronts of both + the marks diff +
+        k_sc_change, tokens + posting lists + restricted enumeration, verification (cross scores included)] in ms."""
+        ms = (C.c_float * 4)()
+        lib().tsm_similar_churn_last_ms(self._ctx, C.byref(ms))
         return [float(x) for x in ms]
 
     def smells_last_ms(self):
