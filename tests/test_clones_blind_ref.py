@@ -2,7 +2,8 @@
 restatement (tests/blind_ref.py) agree line by line (kept flag and blind hash) and class by class, on the lexer's hazards (comment
 and string openers inside literals, escapes, unterminated literals, string prefixes, docstrings and block comments that span lines,
 pp-numbers, keywords against identifiers, literal names, non-ASCII identifier bytes, tag-0 files, CRLF, empty and all-comment
-files), on the section's worked examples, and on the C1 counts pinned in the section."""
+files), on the section's worked examples, on the C1 counts pinned in the section, and on the crafted seam corpora of
+tests/front_seams.py, which reach the seams they name (the keyword table the kernel builds, its chains and its wrap included)."""
 import os
 import types
 
@@ -11,6 +12,7 @@ import pytest
 
 import blind_ref as br
 import corpus_util as cu
+import front_seams as fs
 import orc
 import orc_blind as ob
 import spec_ref
@@ -170,3 +172,63 @@ def test_c1_pinned_counts(n):
 
 def test_blind_hash_is_section3_bytes_hash():
     assert br.blind_hash(b"I = N") == spec_ref.py_bytes_hash(b"I = N")
+
+
+# The crafted corpora of tests/front_seams.py, on which tests/test_gpu_clones_blind_seams.py runs the kernels: the two references
+# agree on each, and each reaches the seams it names.
+def test_kernel_keyword_lists_are_the_reference_sets():
+    py, cj, py_lit, cj_lit = fs.kernel_keyword_lists()
+    assert (set(py), set(cj), set(py_lit), set(cj_lit)) == (br.PY_KEYWORDS, br.CJ_KEYWORDS, br.PY_LITERALS, br.CJ_LITERALS)
+    assert len(py + cj + py_lit + cj_lit) == len(set(py + cj + py_lit + cj_lit)) + len(br.PY_KEYWORDS & br.CJ_KEYWORDS)
+
+
+def test_keyword_table_chains_and_wrap():
+    slots = fs.keyword_table()
+    names = br.PY_KEYWORDS | br.CJ_KEYWORDS | br.PY_LITERALS | br.CJ_LITERALS
+    assert sorted(w for w in slots if w) == sorted(names) and len(names) == 143
+    shift = {w: (i - fs.kw_home(w)) % fs.SLOTS for i, w in enumerate(slots) if w}
+    assert sum(1 for v in shift.values() if v) == 12 and max(shift.values()) == 3
+    assert slots[511] == b"bitor" and slots[0] == b"decltype"         # a chain that wraps from the last slot to slot 0
+    for i, w in enumerate(slots):                                      # every name is found where the kernel put it
+        if w:
+            assert fs.probe(slots, w)[0][-1] == i
+
+
+def test_keyword_corpus_walks_chains_and_wraps():
+    files, exts, reach = fs.keyword_corpus()
+    assert reach["searched_walk"] and reach["wraps"] and len(reach["displaced_found"]) == 12
+    words = files[0].split()
+    assert {b"reinterpret_cast", b"reinterpret_castX", b"abcdefghijklmnop", b"abcdefghijklmnopq"} <= set(words)
+    assert br.lex_line(b"reinterpret_cast reinterpret_castX", br.CJ, 0)[0] == [b"reinterpret_cast", b"I"]
+    both(files, exts, 1)
+
+
+def test_blind_grid_corpus():
+    files, exts, reach = fs.blind_grid_corpus()
+    assert all(fs.on_the_grid(reach).values()) and len(reach) == len(fs.PY_CONSTRUCTS) + len(fs.CJ_CONSTRUCTS)
+    both(files, exts, 2)
+
+
+def test_filter_corpus():
+    files, exts, reach = fs.filter_corpus()
+    for fam in ("py", "cj"):
+        assert all(reach[(fam, k)] == set(range(8)) for k in ("byte0", "byte7", "byte8", "last"))
+        assert reach[(fam, "neighbour_before")] and reach[(fam, "neighbour_after")]
+    both(files, exts, 2)
+
+
+def test_scan_corpus():
+    files, exts, reach = fs.scan_corpus()
+    for ext, n, lanes in reach["lanes"][:10]:
+        assert {(l, r) for l in (0, 1, 30, 31) for r in range(n // 32 + 1) if 32 * r + l < n} <= set(lanes), (ext, n)
+    assert reach["permutation"] and reach["noncommuting_neighbours"] >= 20
+    got = both(files, exts, 1)
+    kb = got["kept_base"]
+    assert kb[11] - kb[10] == 1 and kb[12] == kb[11] and kb[14] - kb[13] == 1    # the open comment does not leak into int b;
+
+
+def test_files_corpus():
+    files, exts, reach = fs.files_corpus()
+    got = both(files, exts, 1)
+    assert got["file_kept_assert"].tolist() == reach["asserts"]
+    assert got["kept_base"][-4:].tolist() == [got["kept_base"][-1]] * 4      # no kept line in the last three files

@@ -5,7 +5,8 @@ sleep, sprintf( and fingerprint(, stacked decorators, DISABLED_, duplicates diff
 assertEqual(f(a, b), f(a, b)), a C-family one-liner, brace counts that never open or go negative, CRLF, an unterminated last
 line, headerless and empty files; the C1 counts that SPEC section 18 pins; and the planted corpus generator.  The serial C reference
 (orc_smells.c, on the oracle's header and assertion rules and line hash) agrees with it, every output array, on the hand-written
-files, C1, planted corpora and fuzz corpora with long lines and binary bytes."""
+files, C1, planted corpora and fuzz corpora with long lines and binary bytes, and on the crafted seam corpora of
+tests/front_seams.py, which give their crafted lines the smell bits the builders expect and reach the seams they name."""
 import os
 
 import numpy as np
@@ -13,6 +14,7 @@ import numpy as np
 import pytest
 
 import corpus_util as cu
+import front_seams as fs
 import orc_smells as ocs
 import smell_ref as sr
 import tosemscan as ts
@@ -137,3 +139,68 @@ def test_c_reference_fuzz(long_lines, binary):
         files[i] = b"\n".join(lines)
     got = both_agree(files, exts)
     assert len(got["tests"]) > 50
+
+
+# The crafted corpora of tests/front_seams.py, on which tests/test_gpu_smells_seams.py runs the kernels: the two references agree
+# on each, give the crafted lines the smell bits their builders expect, and each corpus reaches the seams it names.
+def bits_as_built(got, want):
+    """The crafted lines whose smell bits (under their mask) differ from what the builder expects."""
+    base, smell = got["line_base"], got["line_smell"]
+    return [(f, ln, w, int(smell[base[f] + ln])) for f, ln, m, w in want if int(smell[base[f] + ln]) & m != w]
+
+
+@pytest.mark.parametrize("build", [fs.pattern_corpus, fs.token_corpus, fs.redundant_corpus])
+def test_grid_corpora(build):
+    files, exts, reach, want = build()
+    assert reach and all(fs.on_the_grid(reach).values())
+    got = both_agree(files, exts)
+    assert bits_as_built(got, want) == []
+    assert got["tests"]["body_lines"].tolist() == [len(sr.py_lines(f)) for f in files]      # every line is in the test
+
+
+def test_pattern_prefix_checks_meet_equality():
+    files, exts, reach, want = fs.pattern_corpus()
+    # gtest body from column 0: `sleep_for(` / `_until(` / `System.` start at the line's first byte
+    assert (0, 0) in reach[(3, "sleep_for")] and (0, 0) in reach[(3, "sleep_until")] and (0, 0) in reach[(3, "system_out")]
+    lines = sr.py_lines(files[0])
+    assert lines[[ln for f, ln, _, w in want if f == 0][0]].startswith(b"print(")
+
+
+def test_facts_corpus():
+    files, exts = fs.facts_corpus()
+    got = both_agree(files, exts)
+    t = got["tests"]
+    n = len(fs.EMPTY_BODIES)
+    want = [int(e) for _, e in fs.EMPTY_BODIES]
+    assert (t["smells"][:n] & 1).tolist() == want and (t["smells"][n:2 * n] & 1).tolist() == want
+    quotes = got["line_smell"][got["line_base"][2]:got["line_base"][3]]
+    assert 0 < int((quotes & fs.COND).astype(bool).sum()) < 2 * len(fs.QUOTE_LINES)   # some `if` lines are in a docstring
+
+
+def test_scan_smell_corpus_lanes():
+    files, exts = fs.scan_smell_corpus()
+    both_agree(files, exts)
+    py, java, cc = (fs.scan_facts(d, e) for d, e in zip(files, exts))
+    assert [fs.lane_round(hs, b + 1) for b, hs, _, _ in py[:4]] == [(31, 0), (0, 1), (1, 1), (8, 1)]
+    assert [fs.lane_round(bend, hs) for _, hs, bend, _ in py[4:12]] == [(31, 0)] * 2 + [(0, 1)] * 2 + [(31, 1)] * 2 + [(0, 2)] * 2
+    b, _, bend, _ = py[12]
+    lines = sr.py_lines(files[0])
+    doc = [ln for ln in range(b, bend) if lines[ln].strip() == b'"""']
+    assert [fs.lane_round(ln, b) for ln in doc] == [(31, 0), (31, 2)]
+    assert [fs.lane_round(br, b) for b, _, _, br in java[::2]] == [(31, 0), (0, 1)]              # Allman `{`
+    jl = sr.py_lines(files[1])
+    assert [fs.lane_round(next(ln for ln in range(b, bend) if b"}" in jl[ln]), b) for b, _, bend, _ in java[1::2]] == \
+        [(31, 0), (0, 1)]                                                                            # `}` ahead of the `{`
+    assert [bend - b for b, _, bend, _ in cc] == [1, 1]
+
+
+def test_header_corpus():
+    files, exts = fs.header_corpus()
+    got = both_agree(files, exts)
+    t = got["tests"]
+    ignored = [(int(f), int(ln)) for f, ln, s in zip(t["file"], t["line"], t["smells"]) if s >> 8 & 1]
+    assert ignored == [(1, 2), (4, 2), (4, 4), (4, 8), (4, 19), (5, 97)]
+    names = [sr.py_lines(files[int(f)])[int(ln)] for f, ln in zip(t["file"], t["line"])]
+    assert b"asyncdef test_c():" not in names and {b"async  def\ttest_b():", b"def  test_d():", b"async\tdef test_e():"} <= set(names)
+    assert sum(1 for n in names if n.startswith((b"TEST", b"TYPED", b"BOOST"))) == 8 + 3 + 2
+    assert [int(f) for f in t["file"][-4:]] == [6, 7, 8, 9]             # a header on the last line, with and without the LF
