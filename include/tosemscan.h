@@ -390,6 +390,31 @@ int tsm_smells(tsm_ctx* ctx, const tsm_corpus* corpus, int64_t* line_base, uint1
                tsm_smell_test* tests, int64_t test_cap, int64_t* n_tests, void* stream);
 int tsm_smells_last_ms(tsm_ctx* ctx, float* ms4);
 
+/* Lexical test smells (docs/SPEC.md section 25, `tosem-scan smells --lexical`): the tests of tsm_smells with five more smells,
+ * found on the section-21 tokens of their bodies: the assertion call of every counted assertion line and its argument list
+ * (over at most 64 lines of the body), the calls and local names of every code line.  line_base, line_smell and tests are
+ * filled exactly as tsm_smells fills them; lex holds one tsm_lex_test per test, in the same order:
+ *   n_stmts        assertion statements (counted assertion lines with an assertion call)
+ *   n_unexplained  those counted by Assertion Roulette that have no message
+ *   n_magic        those with a magic-number operand
+ *   n_locals       distinct local names the code lines assign
+ *   smells         bit k = smell k of the TSM_LSMELL_* list
+ *   n_instances    body lines with each bit, summed over the bits of line_lsmell
+ * line_lsmell[l] holds the TSM_LSMELL_* bits of every line (0 outside test bodies; obscure_setup on the header line).  Any output
+ * pointer may be NULL (it is skipped); *n_lines and *n_tests are always set.  If line_smell or line_lsmell is given with
+ * line_cap < *n_lines, or tests or lex with test_cap < *n_tests, the call returns TSM_E_CAPACITY: size the arrays and call again.
+ * n_files = 0 is legal.  Kernels: those of tsm_smells, the lexer states of tsm_clones_blind (k_blind_state, k_blind_scan), then
+ * k_lex_body, k_lex_lines (count and write passes around an xscan) and k_lex_tests (csrc/tsm_lexsmell_kernels.cuh).
+ * tsm_smells_lexical_last_ms: device time of the last call, ms4 = { k_scan, the front (kinds, case spans, smell stage, lexer
+ * states), k_lex_body + k_lex_lines, k_lex_tests }. */
+enum { TSM_LSMELL_ASSERTION_ROULETTE = 0, TSM_LSMELL_MAGIC_NUMBER = 1, TSM_LSMELL_SUBOPTIMAL_ASSERT = 2,
+       TSM_LSMELL_MYSTERY_GUEST = 3, TSM_LSMELL_OBSCURE_SETUP = 4, TSM_N_LSMELLS = 5 };
+typedef struct tsm_lex_test { int32_t n_stmts, n_unexplained, n_magic, n_locals; uint32_t smells; int32_t n_instances; } tsm_lex_test;
+int tsm_smells_lexical(tsm_ctx* ctx, const tsm_corpus* corpus, int64_t* line_base, uint16_t* line_smell, uint8_t* line_lsmell,
+                       int64_t line_cap, int64_t* n_lines, tsm_smell_test* tests, tsm_lex_test* lex, int64_t test_cap,
+                       int64_t* n_tests, void* stream);
+int tsm_smells_lexical_last_ms(tsm_ctx* ctx, float* ms4);
+
 /* Similar tests (docs/SPEC.md section 23, `tosem-scan similar-tests`): the pairs of tests of section 18 whose sequences of kept
  * blind lines (section 21, header line included) are at least min_similarity % alike, and the classes they link.  A test is
  * compared when it has at least min_lines kept lines (min_lines >= 1, else TSM_E_ARG).  Tests a < b form a pair when both are

@@ -26,6 +26,7 @@
 #include "tsm_case_kernels.cuh"
 #include "tsm_edit_kernels.cuh"
 #include "tsm_smell_kernels.cuh"
+#include "tsm_lexsmell_kernels.cuh"
 #include "tsm_move_kernels.cuh"
 #include "tsm_clone_churn_kernels.cuh"
 #include "../host/tsm_names.hpp"
@@ -96,6 +97,7 @@ enum Timed {
   MS_SIMTEST, // k_scan, case spans + smell stage + lexer, tokens + lists + enumeration, verification of the last tsm_similar_tests
   MS_SCHURN,  // k_scan of both revisions, fronts + marks + k_sc_change, tokens + lists + enumeration, verification of the last
               // tsm_similar_churn
+  MS_LEXSMELL,// k_scan, front (smell stage + lexer states), k_lex_body + k_lex_lines, k_lex_tests of the last tsm_smells_lexical
   N_TIMED
 };
 
@@ -181,6 +183,8 @@ struct tsm_ctx {
 //     marks, then per side behind classes  CCHURN                                                          at each end
 //   tsm_similar_tests                                      FRONT   ENUM*   VERIFY* END*    LEXED   LISTS   at the counts /
 //                                                                                                         each chunk
+//   tsm_smells_lexical                                     FRONT                   END     LINES   TESTS   at the test count /
+//                                                                                                         the end
 //   (* recorded by smell_stage, and not read in this call)
 struct EvSpan { int from, to; };
 constexpr EvSpan EV_SCAN[2] = {{0, 1}, {6, 7}}, EV_SMALL = {2, 3}, EV_LEFT = {4, 5};
@@ -192,6 +196,7 @@ constexpr EvSpan EV_CHURN_SMELLS = {0, 1}, EV_CHURN_CASES = {0, 1};   // the old
 constexpr EvSpan EV_MOVE_FLAGS = {0, 1}, EV_MOVE_JOIN = {2, 3}, EV_MOVE_RUNS = {4, 5}, EV_MOVE_MARK = {6, 7};
 constexpr EvSpan EV_BLAME = {0, 1};
 constexpr EvSpan EV_CCHURN = {0, 1};
+constexpr int EV_LX_FRONT = 2, EV_LX_LINES = 6, EV_LX_TESTS = 7, EV_LX_END = 5;
 constexpr int EV_ST_FRONT = 2, EV_ST_ENUM = 3, EV_ST_VERIFY = 4, EV_ST_END = 5, EV_ST_LEXED = 6, EV_ST_LISTS = 7;
 
 // The start of every call that queues device work on st: the ctx's device, the ctx's pool for the call's DevBufs, and the
@@ -2434,6 +2439,91 @@ extern "C" int tsm_smells(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, u
 }
 
 extern "C" int tsm_smells_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_SMELL, ms4, 4); }
+
+// ------------------------------------------------------------------------------------- SPEC section 25 lexical test smells
+// The line records with header events (line_records), the case spans and smell stage of tsm_smells and the line start states
+// of the section-21 lexer (k_blind_state, k_blind_scan), one synchronisation for the test count, then k_lex_body, k_lex_lines
+// (count pass, xscan of the name counts, one synchronisation for their total, write pass) and k_lex_tests.  The outputs are
+// copied when they fit.
+extern "C" int tsm_smells_lexical(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, uint16_t* line_smell, uint8_t* line_lsmell,
+                                  int64_t line_cap, int64_t* n_lines, tsm_smell_test* tests, tsm_lex_test* lex, int64_t test_cap,
+                                  int64_t* n_tests, void* stream) {
+  if (!c || !k || !n_lines || !n_tests || line_cap < 0 || test_cap < 0 || k->n_files < 0) return TSM_E_ARG;
+  const int32_t nf = k->n_files;
+  float* const ms = clear_ms(c, MS_LEXSMELL);
+  c->launches = 0;
+  *n_tests = 0;
+  std::vector<int64_t> own_base;
+  if (!line_base) { own_base.resize((size_t)nf + 1); line_base = own_base.data(); }
+  return line_records(c, k, true, line_base, INT64_MAX, n_lines, stream, [&](const HostSide& S, unsigned long long total, cudaStream_t st) -> int {
+    const size_t L = (size_t)total;
+    const uint32_t nfu = (uint32_t)S.n;
+    CaseSpans sp;
+    SmellBufs m;
+    DevBuf d_bsum, d_state, d_lxflag, d_lxend, d_lflag, d_ncnt, d_nbase, d_names, d_gset, d_lsmell, d_lex;
+    if (!d_bsum.alloc(8 * (L / XS_TILE + 4)) || !d_lxflag.alloc(L) || !d_lxend.alloc(4 * L) || !d_lflag.alloc(L) ||
+        !d_ncnt.alloc(4 * L) || !d_nbase.alloc(8 * (L + 1)) || !d_lsmell.alloc(L))
+      return TSM_E_CUDA;
+    int launches = 0;
+    CU(cudaEventRecord(c->diff_ev[EV_LX_FRONT], st));
+    int rc = case_spans(S, sp, d_bsum, launches, st);
+    if (rc == TSM_OK) rc = smell_stage(c, S, sp, d_bsum, m, launches, st);
+    if (rc != TSM_OK) return rc;
+    const unsigned grid = (unsigned)((L + 255) / 256);
+    if (!d_state.alloc(L)) return TSM_E_CUDA;
+    k_blind_state<<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>());
+    k_blind_scan<<<(unsigned)(((size_t)nfu * 32 + 255) / 256), 256, 0, st>>>(S.d.line_base, nfu, d_state.as<uint8_t>());
+    launches += 2;
+    CU(cudaMemsetAsync(d_lxflag.p, 0, L, st));
+    CU(cudaMemsetAsync(d_lsmell.p, 0, L, st));
+    CU(cudaEventRecord(c->diff_ev[EV_LX_LINES], st));
+    unsigned long long* pin = c->h_rb->u64;
+    CU(cudaMemcpyAsync(pin, m.tidx.as<unsigned long long>() + sp.n_cases, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const unsigned long long nt = *pin;
+    *n_tests = (int64_t)nt;
+    ms[1] = elapsed_ms(c->diff_ev[EV_LX_FRONT], c->diff_ev[EV_LX_LINES]);
+    if (!d_lex.alloc(sizeof(tsm_lex_test) * ((size_t)nt + 1))) return TSM_E_CUDA;
+    if (nt) {
+      const unsigned tgrid = std::min((unsigned)((nt + 7) / 8), (unsigned)c->sms * 8);
+      const tsm_smell_test* dt = m.tests.as<tsm_smell_test>();
+      k_lex_body<<<tgrid, 256, 0, st>>>(LexBody{dt, (uint32_t)nt, S.d.line_base, S.d.ext, m.kind.as<uint8_t>(), m.lines.as<SmellLine>(),
+                                                d_lxflag.as<uint8_t>(), d_lxend.as<uint32_t>()});
+      k_lex_lines<false><<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>(), d_lxflag.as<uint8_t>(), d_lxend.as<uint32_t>(),
+                                               d_lflag.as<uint8_t>(), d_ncnt.as<uint32_t>(), nullptr, nullptr);
+      xscan(d_ncnt.as<uint32_t>(), (uint32_t)total, d_bsum.as<unsigned long long>(), d_nbase.as<unsigned long long>(), st);
+      CU(cudaMemcpyAsync(pin + 1, d_nbase.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      if (!d_names.alloc(8 * (size_t)pin[1]) || !d_gset.alloc(16 * (size_t)pin[1])) return TSM_E_CUDA;
+      CU(cudaMemsetAsync(d_gset.p, 0xFF, 16 * (size_t)pin[1], st));
+      k_lex_lines<true><<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>(), d_lxflag.as<uint8_t>(), d_lxend.as<uint32_t>(),
+                                              d_lflag.as<uint8_t>(), d_ncnt.as<uint32_t>(), d_nbase.as<unsigned long long>(),
+                                              d_names.as<unsigned long long>());
+      CU(cudaEventRecord(c->diff_ev[EV_LX_TESTS], st));
+      k_lex_tests<<<tgrid, 256, 0, st>>>(LexTests{dt, (uint32_t)nt, S.d.line_base, d_lflag.as<uint8_t>(), d_nbase.as<unsigned long long>(),
+                                                 d_names.as<unsigned long long>(), d_gset.as<unsigned long long>(), d_lsmell.as<uint8_t>(),
+                                                 d_lex.as<tsm_lex_test>()});
+      launches += 7;                                       // body, lines, xscan (3), lines (write), tests
+    } else {
+      CU(cudaEventRecord(c->diff_ev[EV_LX_TESTS], st));
+    }
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_LX_END], st));
+    CU(cudaStreamSynchronize(st));
+    c->launches += launches;
+    ms[2] = elapsed_ms(c->diff_ev[EV_LX_LINES], c->diff_ev[EV_LX_TESTS]);
+    ms[3] = elapsed_ms(c->diff_ev[EV_LX_TESTS], c->diff_ev[EV_LX_END]);
+    if (((line_smell || line_lsmell) && line_cap < (int64_t)total) || ((tests || lex) && test_cap < (int64_t)nt)) return TSM_E_CAPACITY;
+    if (line_smell) CU(cudaMemcpyAsync(line_smell, m.smell.p, 2 * L, cudaMemcpyDeviceToHost, st));
+    if (line_lsmell) CU(cudaMemcpyAsync(line_lsmell, d_lsmell.p, L, cudaMemcpyDeviceToHost, st));
+    if (tests && nt) CU(cudaMemcpyAsync(tests, m.tests.p, sizeof(tsm_smell_test) * nt, cudaMemcpyDeviceToHost, st));
+    if (lex && nt) CU(cudaMemcpyAsync(lex, d_lex.p, sizeof(tsm_lex_test) * nt, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    return TSM_OK;
+  }, &ms[0], TSM_SCAN_HEADER_EVENTS);
+}
+
+extern "C" int tsm_smells_lexical_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_LEXSMELL, ms4, 4); }
 
 // ------------------------------------------------------------------------------------- SPEC section 23 similar tests
 // One revision's section-23 state on the device, resident while the call needs it: the front (case spans, smell stage and

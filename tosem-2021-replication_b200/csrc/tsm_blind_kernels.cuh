@@ -133,11 +133,45 @@ __device__ __forceinline__ uint32_t blind_string(LineBytes& B, uint32_t i, uint3
   return e;
 }
 
-// Lexes line [s, e) of family fam (1 PY, 2 CJ) from state st and returns the state at its end.  EMIT: feeds the blind form into
-// h, looking keywords up in (kw, kind).
-template <bool EMIT>
-__device__ uint32_t blind_lex(LineBytes& B, uint32_t s, uint32_t e, uint32_t fam, uint32_t st, BlindHash& h, const BlindKw* kw,
-                              const uint8_t* kind) {
+// The keyword kind (KW_*) of an identifier of k bytes whose first 16 are (lo, hi): 0 when it is no name of the table.
+__device__ __forceinline__ uint32_t blind_kw_kind(const BlindKw* kw, const uint8_t* kind, unsigned long long lo, unsigned long long hi,
+                                                  uint32_t k) {
+  uint32_t kk = 0;
+  if (k <= 16)
+    for (uint32_t sl = blind_kw_home(lo, hi); kw[sl].lo; sl = (sl + 1) & (BLIND_KW_SLOTS - 1))
+      if (kw[sl].lo == lo && kw[sl].hi == hi) { kk = kind[sl]; break; }
+  return kk;
+}
+
+// Token sinks of blind_lex, one call per token: number(), string(), ident(B, fam, i0, k, lo, hi) for the identifier of k bytes
+// at i0 whose first 16 bytes are (lo, hi), punct(c) for any other byte.  NoSink only follows the state; BlindSink feeds the
+// blind form into h, looking keywords up in (kw, kind).
+struct NoSink {
+  __device__ __forceinline__ void number() {}
+  __device__ __forceinline__ void string() {}
+  __device__ __forceinline__ void ident(LineBytes&, uint32_t, uint32_t, uint32_t, unsigned long long, unsigned long long) {}
+  __device__ __forceinline__ void punct(uint32_t) {}
+};
+struct BlindSink {
+  BlindHash h; const BlindKw* kw; const uint8_t* kind;
+  __device__ __forceinline__ void number() { h.token('N'); }
+  __device__ __forceinline__ void string() { h.token('S'); }
+  __device__ __forceinline__ void ident(LineBytes&, uint32_t fam, uint32_t, uint32_t k, unsigned long long lo, unsigned long long hi) {
+    const uint32_t kk = blind_kw_kind(kw, kind, lo, hi, k);
+    if (kk & (fam == 1 ? KW_PY : KW_CJ)) {
+      if (h.len) h.byte(' ');
+      for (uint32_t j = 0; j < k; ++j) h.byte((uint32_t)((j < 8 ? lo >> (8 * j) : hi >> (8 * (j - 8))) & 0xFFu));
+    } else {
+      h.token((kk & (fam == 1 ? KW_PY_LIT : KW_CJ_LIT)) ? 'N' : 'I');
+    }
+  }
+  __device__ __forceinline__ void punct(uint32_t c) { h.token(c); }
+};
+
+// Lexes line [s, e) of family fam (1 PY, 2 CJ) from state st, hands every token that begins on it to sink, and returns the
+// state at its end.  The one copy of the lexing rules of docs/SPEC.md section 21.
+template <typename Sink>
+__device__ uint32_t blind_lex(LineBytes& B, uint32_t s, uint32_t e, uint32_t fam, uint32_t st, Sink& sink) {
   uint32_t i = s;
   if (st) {
     i = blind_close(B, s, e, fam, st);
@@ -161,7 +195,7 @@ __device__ uint32_t blind_lex(LineBytes& B, uint32_t s, uint32_t e, uint32_t fam
           break;
         prev = d;
       }
-      if (EMIT) h.token('N');
+      sink.number();
       continue;
     }
     if (blind_ident(c)) {
@@ -183,33 +217,22 @@ __device__ uint32_t blind_lex(LineBytes& B, uint32_t s, uint32_t e, uint32_t fam
         if (prefix) {
           uint32_t st2;
           i = blind_string(B, i, e, fam, st2);
-          if (EMIT) h.token('S');
+          sink.string();
           if (st2) return st2;
           continue;
         }
       }
-      if (EMIT) {
-        uint32_t kk = 0;
-        if (k <= 16)
-          for (uint32_t sl = blind_kw_home(lo, hi); kw[sl].lo; sl = (sl + 1) & (BLIND_KW_SLOTS - 1))
-            if (kw[sl].lo == lo && kw[sl].hi == hi) { kk = kind[sl]; break; }
-        if (kk & (fam == 1 ? KW_PY : KW_CJ)) {
-          if (h.len) h.byte(' ');
-          for (uint32_t j = 0; j < k; ++j) h.byte((uint32_t)((j < 8 ? lo >> (8 * j) : hi >> (8 * (j - 8))) & 0xFFu));
-        } else {
-          h.token((kk & (fam == 1 ? KW_PY_LIT : KW_CJ_LIT)) ? 'N' : 'I');
-        }
-      }
+      sink.ident(B, fam, i0, k, lo, hi);
       continue;
     }
     if (c == '"' || c == '\'') {
       uint32_t st2;
       i = blind_string(B, i, e, fam, st2);
-      if (EMIT) h.token('S');
+      sink.string();
       if (st2) return st2;
       continue;
     }
-    if (EMIT) h.token(c);
+    sink.punct(c);
     ++i;
   }
   return 0;
@@ -247,9 +270,8 @@ __global__ void __launch_bounds__(256) k_blind_state(DiffSide d, uint32_t n, uns
     }
     if (any) {
       LineBytes B{g, 1u, 0};
-      BlindHash h{0, 0, 0};
-      out = (uint8_t)(blind_lex<false>(B, s, e, fam, 0, h, nullptr, nullptr) | (blind_lex<false>(B, s, e, fam, 1, h, nullptr, nullptr) << 2) |
-                      ((fam == 1 ? blind_lex<false>(B, s, e, fam, 2, h, nullptr, nullptr) : 2u) << 4));
+      NoSink ns;
+      out = (uint8_t)(blind_lex(B, s, e, fam, 0, ns) | (blind_lex(B, s, e, fam, 1, ns) << 2) | ((fam == 1 ? blind_lex(B, s, e, fam, 2, ns) : 2u) << 4));
     }
   }
   fn[i] = out;
@@ -291,10 +313,11 @@ __global__ void __launch_bounds__(256) k_blind_lines(DiffSide d, uint32_t n, uns
   const uint32_t f = blind_file(d.line_base, n, i), fam = blind_family(d.ext[f]);
   const uint8_t* g = d.arena + (uint32_t)d.off[f];
   const uint32_t e = d.line_end[i], s = i == d.line_base[f] ? 0u : d.line_end[i - 1] + 1u;
-  BlindHash h{0, 0, 0};
+  BlindSink sk{BlindHash{0, 0, 0}, kw, kind};
+  BlindHash& h = sk.h;
   if (fam) {
     LineBytes B{g, 1u, 0};
-    blind_lex<true>(B, s, e, fam, state[i], h, kw, kind);
+    blind_lex(B, s, e, fam, state[i], sk);
   } else {                                                      // tag 0: the content without its W bytes
     for (uint32_t wb = s & ~7u; wb < e; wb += 8) {
       unsigned long long w = __ldg(reinterpret_cast<const unsigned long long*>(g + wb));

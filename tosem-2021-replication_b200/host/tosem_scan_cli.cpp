@@ -1226,6 +1226,8 @@ static void diff_smells(tsm_ctx* ctx, const tsm_corpus& ca, const tsm_corpus& cn
 
 static const char* const kSmellNames[TSM_N_SMELLS] = {"empty", "assertion_free", "duplicate_assert", "redundant_assert",
                                                       "conditional_logic", "exception_handling", "sleepy", "print", "ignored"};
+static const char* const kLexSmellNames[TSM_N_LSMELLS] = {"assertion_roulette", "magic_number", "suboptimal_assert", "mystery_guest",
+                                                         "obscure_setup"};
 
 // The case name (docs/SPEC.md section 10) of every case of one side of a pair, from the header lines of the side's bytes.
 static std::vector<std::string> case_names(const uint8_t* base, int32_t size, int ext, const tsm_case* cs, size_t n) {
@@ -2435,8 +2437,10 @@ static int cmd_clones(const std::vector<std::string>& roots, const std::string& 
 // Test smells (docs/SPEC.md section 18): tsm_smells per batch (tests never cross files, so batches are independent).  stdout: per
 // root the files and the tests with each smell, and an <all> row; --out: one row per instance line, in file, header line, instance
 // line and smell order, lines 1-based; the statement is the stripped instance line (empty for the test-level smells).
+// --lexical: one tsm_smells_lexical call per batch instead, which adds the five smells of docs/SPEC.md section 25 after the nine,
+// in the stdout columns and the --out rows.
 static int cmd_smells(const std::vector<std::string>& roots, const std::string& git_repo, const std::string& rev, bool all_files,
-                      const std::string& out_path, int64_t batch_bytes) {
+                      const std::string& out_path, int64_t batch_bytes, bool lexical) {
   std::vector<FileEntry> files;
   std::vector<std::string> names;
   if (!git_repo.empty()) {
@@ -2452,7 +2456,8 @@ static int cmd_smells(const std::vector<std::string>& roots, const std::string& 
   }
   fprintf(stderr, "tosem-scan: %zu files selected under %zu root(s)\n", files.size(), names.size());
   const size_t ng = names.size();
-  std::vector<std::vector<int64_t>> tot(ng + 1, std::vector<int64_t>(2 + TSM_N_SMELLS, 0));   // files, tests, tests per smell
+  const int nk = TSM_N_SMELLS + (lexical ? TSM_N_LSMELLS : 0);
+  std::vector<std::vector<int64_t>> tot(ng + 1, std::vector<int64_t>(2 + (size_t)nk, 0));   // files, tests, tests per smell
   std::ofstream os;
   if (!out_path.empty()) { os.open(out_path, std::ios::binary); csv_row(os, {"repository", "fileName", "test", "line", "smell", "smellLine", "statement"}); }
   std::vector<Batch> batches = plan_batches(files, all_of(files), batch_bytes, kBatchFiles);
@@ -2464,18 +2469,26 @@ static int cmd_smells(const std::vector<std::string>& roots, const std::string& 
     for (int32_t i = 0; i < nf; ++i) lines += s.stats[(size_t)i].n_lines;   // lines (each test starts at one), so one call fills them
     std::vector<uint16_t> smell((size_t)std::max<int64_t>(lines, 1));
     std::vector<tsm_smell_test> tests(std::max<size_t>(s.hev.size(), 1));
-    ck(tsm_smells(s.ctx, &c, base.data(), smell.data(), lines, &nl, tests.data(), (int64_t)s.hev.size(), &nt, nullptr), "tsm_smells");
+    std::vector<uint8_t> lsmell(lexical ? smell.size() : 0);
+    std::vector<tsm_lex_test> lex(lexical ? tests.size() : 0);
+    if (lexical)
+      ck(tsm_smells_lexical(s.ctx, &c, base.data(), smell.data(), lsmell.data(), lines, &nl, tests.data(), lex.data(),
+                            (int64_t)s.hev.size(), &nt, nullptr), "tsm_smells_lexical");
+    else
+      ck(tsm_smells(s.ctx, &c, base.data(), smell.data(), lines, &nl, tests.data(), (int64_t)s.hev.size(), &nt, nullptr), "tsm_smells");
     for (int32_t i = 0; i < nf; ++i) { tot[(size_t)files[B.idx[(size_t)i]].grp][0]++; tot[ng][0]++; }
     int32_t at_file = -1;
     std::vector<uint32_t> start;                           // byte offset of every line of file at_file
     for (int64_t t = 0; t < nt; ++t) {
       const tsm_smell_test& r = tests[(size_t)t];
+      const uint32_t lsm = lexical ? lex[(size_t)t].smells : 0u;
       const FileEntry& fe = files[B.idx[(size_t)r.file]];
       for (size_t g : {(size_t)fe.grp, ng}) {
         tot[g][1]++;
         for (int k = 0; k < TSM_N_SMELLS; ++k) tot[g][2 + (size_t)k] += (r.smells >> k) & 1;
+        for (int k = 0; k < nk - TSM_N_SMELLS; ++k) tot[g][2 + TSM_N_SMELLS + (size_t)k] += (lsm >> k) & 1;
       }
-      if (!os.is_open() || !r.smells) continue;
+      if (!os.is_open() || !(r.smells || lsm)) continue;
       const uint8_t* p = B.arena.get() + B.off[(size_t)r.file];
       const uint32_t len = (uint32_t)B.len[(size_t)r.file];
       if (at_file != r.file) {
@@ -2499,12 +2512,19 @@ static int cmd_smells(const std::vector<std::string>& roots, const std::string& 
             csv_row(os, {names[(size_t)fe.grp], fe.rel, name, std::to_string(r.line + 1), kSmellNames[k], std::to_string(l + 1),
                          test_level ? std::string() : stripped(l)});
           }
+        const uint8_t lbits = lexical ? lsmell[(size_t)(g0 + l - r.line)] : 0;
+        for (int k = 0; k < TSM_N_LSMELLS; ++k)
+          if ((lbits >> k) & 1)
+            csv_row(os, {names[(size_t)fe.grp], fe.rel, name, std::to_string(r.line + 1), kLexSmellNames[k], std::to_string(l + 1),
+                         k == TSM_LSMELL_OBSCURE_SETUP ? std::string() : stripped(l)});
       }
     }
   });
   std::ostringstream so;
   std::vector<std::string> head = {"repository", "files", "tests"};
   for (const char* n : kSmellNames) head.push_back(n);
+  if (lexical)
+    for (const char* n : kLexSmellNames) head.push_back(n);
   csv_row(so, head);
   for (size_t g = 0; g <= ng; ++g) {
     std::vector<std::string> row = {g < ng ? names[g] : "<all>"};
@@ -2650,11 +2670,13 @@ static void usage() {
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
           "       tosem-scan clones <project-root>... [--min-lines N] [--blind] [--all-files] [--out F]\n"
           "       tosem-scan clones --git <repository> [--rev R] [--min-lines N] [--blind] [--all-files] [--out F]\n"
-          "       tosem-scan smells <project-root>... [--all-files] [--batch-bytes N] [--out F]\n"
-          "       tosem-scan smells --git <repository> [--rev R] [--all-files] [--batch-bytes N] [--out F]\n"
+          "       tosem-scan smells <project-root>... [--lexical] [--all-files] [--batch-bytes N] [--out F]\n"
+          "       tosem-scan smells --git <repository> [--rev R] [--lexical] [--all-files] [--batch-bytes N] [--out F]\n"
           "       tosem-scan similar-tests <project-root>... | --git <repository> [--rev R] [--min-lines N] [--similarity P] [--all-files]\n"
           "                                [--out F] [--classes F]\n"
           "smells: per root the tests with each of nine test smells; --out F: one row per instance line (docs/SPEC.md section 18).\n"
+          "--lexical (smells): five more smells from the assertion calls' arguments, lexed with string awareness: assertion_roulette,\n"
+          "  magic_number, suboptimal_assert, mystery_guest, obscure_setup (docs/SPEC.md section 25).\n"
           "similar-tests: pairs of tests whose kept blind lines are at least P %% alike (LCS, default 70) and their classes, over\n"
           "               tests of at least N kept lines (default 5); --out F: one row per pair; --classes F: one row per class member\n"
           "               (docs/SPEC.md section 23).\n"
@@ -2683,13 +2705,14 @@ int main(int argc, char** argv) {
   const std::string cmd = argv[1];
   std::vector<std::string> pos;
   std::map<std::string, std::string> opt;
-  bool all_files = false, rev_b = false, dry_run = false, blind = false;
+  bool all_files = false, rev_b = false, dry_run = false, blind = false, lexical = false;
   for (int i = 2; i < argc; ++i) {
     const std::string a = argv[i];
     if (a == "--all-files") all_files = true;
     else if (a == "--rev-b") rev_b = true;
     else if (a == "--dry-run") dry_run = true;
     else if (a == "--blind") blind = true;
+    else if (a == "--lexical") lexical = true;
     else if (a.rfind("--", 0) == 0) { if (i + 1 >= argc) die("missing value for " + a); opt[a] = argv[++i]; }
     else pos.push_back(a);
   }
@@ -2708,7 +2731,7 @@ int main(int argc, char** argv) {
   }
   if (cmd == "smells") {
     if (pos.empty() == !opt.count("--git")) die("smells needs project roots or --git <repository>, not both");
-    return cmd_smells(pos, opt["--git"], opt.count("--rev") ? opt["--rev"] : "HEAD", all_files, opt["--out"], batch_bytes(kBatch, 1));
+    return cmd_smells(pos, opt["--git"], opt.count("--rev") ? opt["--rev"] : "HEAD", all_files, opt["--out"], batch_bytes(kBatch, 1), lexical);
   }
   if (cmd == "similar-tests") {
     if (pos.empty() == !opt.count("--git")) die("similar-tests needs project roots or --git <repository>, not both");

@@ -36,6 +36,10 @@ SMELL_TEST = np.dtype([("file", "<i4"), ("line", "<i4"), ("body_lines", "<i4"), 
                        ("n_instances", "<i4")])   # tsm_smell_test: one test of the corpus (docs/SPEC.md section 18)
 SMELLS = ["empty", "assertion_free", "duplicate_assert", "redundant_assert", "conditional_logic", "exception_handling", "sleepy",
           "print", "ignored"]                   # bit k of tsm_smell_test.smells and of line_smell is SMELLS[k]
+LEX_TEST = np.dtype([("n_stmts", "<i4"), ("n_unexplained", "<i4"), ("n_magic", "<i4"), ("n_locals", "<i4"), ("smells", "<u4"),
+                     ("n_instances", "<i4")])   # tsm_lex_test: the lexical smells of one test (docs/SPEC.md section 25)
+LSMELLS = ["assertion_roulette", "magic_number", "suboptimal_assert", "mystery_guest",
+           "obscure_setup"]                     # bit k of tsm_lex_test.smells and of line_lsmell is LSMELLS[k]
 TEST_CHURN = np.dtype([("case_idx", "<i4"), ("instances", "<i4", (9,)), ("churned", "<i4", (9,))])   # tsm_test_churn (section 19)
 MOVE_BLOCK = np.dtype([("line", "<i8"), ("partner", "<i8"), ("n_lines", "<i4"),
                        ("n_assert", "<i4")])   # tsm_move_block: one moved block of one side (docs/SPEC.md section 20)
@@ -56,7 +60,7 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_diff_pairs_cases", "tsm_diff_pairs_assert_edits", "tsm_assert_edits_last_ms", "tsm_smells", "tsm_smells_last_ms",
            "tsm_diff_pairs_smells", "tsm_diff_smells_last_ms", "tsm_diff_pairs_moves", "tsm_moves_last_ms", "tsm_clones_blind",
            "tsm_clones_blind_last_ms", "tsm_clone_churn", "tsm_clone_churn_last_ms", "tsm_similar_tests", "tsm_similar_tests_last_ms",
-           "tsm_similar_churn", "tsm_similar_churn_last_ms"]
+           "tsm_similar_churn", "tsm_similar_churn_last_ms", "tsm_smells_lexical", "tsm_smells_lexical_last_ms"]
 FRAG_STATES = ["kept", "edited", "whole"]          # tsm_clone_churn state[j] (docs/SPEC.md section 22)
 CLONE_STATUSES = ["untouched", "changed", "removed", "diverged", "dropped", "created", "copied", "joined"]   # status[c]
 
@@ -247,6 +251,11 @@ def lib():
         L.tsm_smells.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64),
                                  C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p]
         L.tsm_smells_last_ms.restype = C.c_int
+        L.tsm_smells_lexical.restype = C.c_int
+        L.tsm_smells_lexical.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                         C.POINTER(C.c_int64), C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p]
+        L.tsm_smells_lexical_last_ms.restype = C.c_int
+        L.tsm_smells_lexical_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
         L.tsm_similar_tests.restype = C.c_int
         L.tsm_similar_tests.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_int32, C.c_int32, C.POINTER(_SimilarResult), C.c_void_p]
         L.tsm_similar_tests_last_ms.restype = C.c_int
@@ -942,6 +951,29 @@ class Scanner:
             return {"line_base": base, "line_smell": smell[:nl.value], "tests": tests[:nt.value]}
         raise TsmError(TSM_E_CAPACITY, "tsm_smells")
 
+    def smells_lexical(self, corpus, stream=None, cap=None):
+        """Test smells with the lexical smells (docs/SPEC.md section 25): the dict of smells() - line_base, line_smell and tests,
+        exactly as smells() returns them - plus line_lsmell[n_lines] (bit k is LSMELLS[k]) and lex[n_tests] (LEX_TEST records,
+        in the order of tests).  Arrays too small are sized from the counts and the call is made again (cap: the first guess)."""
+        n = corpus.n_files
+        cs = corpus.c_struct()
+        cl = ct = int(cap if cap is not None else 0)
+        for _ in range(2):
+            base = np.zeros(n + 1, np.int64)
+            smell, lsmell = np.zeros(max(cl, 1), np.uint16), np.zeros(max(cl, 1), np.uint8)
+            tests, lex = np.zeros(max(ct, 1), SMELL_TEST), np.zeros(max(ct, 1), LEX_TEST)
+            nl, nt = C.c_int64(), C.c_int64()
+            rc = lib().tsm_smells_lexical(self._ctx, C.byref(cs), _p(base), _p(smell), _p(lsmell), cl, C.byref(nl), _p(tests), _p(lex),
+                                          ct, C.byref(nt), stream)
+            if rc == TSM_E_CAPACITY and (nl.value > cl or nt.value > ct):
+                cl, ct = int(nl.value), int(nt.value)
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_smells_lexical")
+            return {"line_base": base, "line_smell": smell[:nl.value], "tests": tests[:nt.value], "line_lsmell": lsmell[:nl.value],
+                    "lex": lex[:nt.value]}
+        raise TsmError(TSM_E_CAPACITY, "tsm_smells_lexical")
+
     def diff_smells(self, olds, news, stream=None, cap=None):
         """Test-smell churn (docs/SPEC.md section 19): a dict of added, removed, detail (tsm_diff_pairs_detail's), old_cases and
         new_cases (diff_cases' CASE arrays), old_tests and new_tests (SMELL_TEST records of each side, file = the pair) and
@@ -1099,6 +1131,13 @@ class Scanner:
         """Device time of the last smells call: [k_scan, kinds + case spans, k_smell_lines, k_smell_tests] in ms."""
         ms = (C.c_float * 4)()
         lib().tsm_smells_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
+
+    def smells_lexical_last_ms(self):
+        """Device time of the last smells_lexical call: [k_scan, the front (kinds, case spans, smell stage, lexer states),
+        k_lex_body + k_lex_lines, k_lex_tests] in ms."""
+        ms = (C.c_float * 4)()
+        lib().tsm_smells_lexical_last_ms(self._ctx, C.byref(ms))
         return [float(x) for x in ms]
 
     def clones_last_ms(self):
