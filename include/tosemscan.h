@@ -405,8 +405,8 @@ int tsm_smells_last_ms(tsm_ctx* ctx, float* ms4);
  * line_cap < *n_lines, or tests or lex with test_cap < *n_tests, the call returns TSM_E_CAPACITY: size the arrays and call again.
  * n_files = 0 is legal.  Kernels: those of tsm_smells, the lexer states of tsm_clones_blind (k_blind_state, k_blind_scan), then
  * k_lex_body, k_lex_lines (count and write passes around an xscan) and k_lex_tests (csrc/tsm_lexsmell_kernels.cuh).
- * tsm_smells_lexical_last_ms: device time of the last call, ms4 = { k_scan, the front (kinds, case spans, smell stage, lexer
- * states), k_lex_body + k_lex_lines, k_lex_tests }. */
+ * tsm_smells_lexical_last_ms: device time of the last call, ms4 = { k_scan, the front (kinds, case spans, smell stage), lexer
+ * states + k_lex_body + k_lex_lines, k_lex_tests }. */
 enum { TSM_LSMELL_ASSERTION_ROULETTE = 0, TSM_LSMELL_MAGIC_NUMBER = 1, TSM_LSMELL_SUBOPTIMAL_ASSERT = 2,
        TSM_LSMELL_MYSTERY_GUEST = 3, TSM_LSMELL_OBSCURE_SETUP = 4, TSM_N_LSMELLS = 5 };
 typedef struct tsm_lex_test { int32_t n_stmts, n_unexplained, n_magic, n_locals; uint32_t smells; int32_t n_instances; } tsm_lex_test;
@@ -517,6 +517,28 @@ typedef struct tsm_diff_smells {
 int tsm_diff_pairs_smells(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
                           tsm_diff_detail* detail, tsm_diff_smells* out, void* stream);
 int tsm_diff_smells_last_ms(tsm_ctx* ctx, float* ms4);
+
+/* Lexical test-smell churn (docs/SPEC.md section 26): tsm_diff_pairs_smells with the five smells of section 25.  out is filled
+ * exactly as tsm_diff_pairs_smells fills it; lex (not NULL) holds per side one record per test of out, in the same order, sized
+ * by out's test caps (old_test_cap, new_test_cap):
+ *   old_lex / new_lex      the tsm_lex_test records of tsm_smells_lexical over that side's corpus alone
+ *   old_churn / new_churn  per lexical smell k (TSM_LSMELL_*): instances[k], the test's body lines with line_lsmell bit k, and
+ *                          churned[k], those that are removed (old side) or added (new side) instances: the line is deleted
+ *                          (inserted), or it is kept and the corresponding line of the other side (section 14) lacks bit k.
+ * Any output pointer may be NULL (it is skipped); the counts of out are always set, and a short test cap for a given lex output
+ * returns TSM_E_CAPACITY as for out (before the diff).  added / removed / detail as for tsm_diff_pairs_smells; n_files = 0 is legal.
+ * Kernels: those of tsm_diff_pairs_smells; per side, behind its smell stage, the lexical stage of tsm_smells_lexical (k_blind_state,
+ * k_blind_scan, k_lex_body, k_lex_lines twice around an xscan, k_lex_tests); k_smell_churn<true> in place of k_smell_churn, which
+ * counts the nine and the five smells in one walk (csrc/tsm_smell_kernels.cuh).
+ * tsm_diff_smells_lexical_last_ms: device time of the last call, ms4 = { k_scan over both sides, the smell and lexical stages of
+ * both sides (case spans included), k_diff_small + k_myers + k_myers_trace, case records + k_smell_churn }. */
+typedef struct tsm_lex_churn { int32_t instances[TSM_N_LSMELLS]; int32_t churned[TSM_N_LSMELLS]; } tsm_lex_churn;
+typedef struct tsm_diff_lex_smells {
+  tsm_lex_test* old_lex; tsm_lex_churn* old_churn; tsm_lex_test* new_lex; tsm_lex_churn* new_churn;
+} tsm_diff_lex_smells;
+int tsm_diff_pairs_smells_lexical(tsm_ctx* ctx, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                                  tsm_diff_detail* detail, tsm_diff_smells* out, tsm_diff_lex_smells* lex, void* stream);
+int tsm_diff_smells_lexical_last_ms(tsm_ctx* ctx, float* ms4);
 
 /* Moved code (docs/SPEC.md section 20, git's `--color-moved=blocks`): the blocks of changed lines that a step moves.  A pair's
  * step is its grp; it must be the same on both sides and below olds->n_groups (grp NULL: every pair in step 0), else TSM_E_ARG.

@@ -97,7 +97,10 @@ enum Timed {
   MS_SIMTEST, // k_scan, case spans + smell stage + lexer, tokens + lists + enumeration, verification of the last tsm_similar_tests
   MS_SCHURN,  // k_scan of both revisions, fronts + marks + k_sc_change, tokens + lists + enumeration, verification of the last
               // tsm_similar_churn
-  MS_LEXSMELL,// k_scan, front (smell stage + lexer states), k_lex_body + k_lex_lines, k_lex_tests of the last tsm_smells_lexical
+  MS_LEXSMELL,// k_scan, front (case spans + smell stage), lexer states + k_lex_body + k_lex_lines, k_lex_tests of the last
+              // tsm_smells_lexical
+  MS_LEXCHURN,// k_scan, smell and lexical stages, the diff, case records + k_smell_churn<true> of the last
+              // tsm_diff_pairs_smells_lexical
   N_TIMED
 };
 
@@ -176,6 +179,7 @@ struct tsm_ctx {
 //                                                                                                         the members / end
 //   tsm_smells (smell_stage: LINES - END)                  KINDS   LINES   TESTS   END                     at the end
 //   tsm_diff_pairs_smells: smell stages    CHURN_SMELLS            LINES*  TESTS*  END*                    before the diff
+//     (_lexical) lexical stages, then                                                      CHURN_LEX       at the end
 //     case records + churn, behind diff    CHURN_CASES                                                     at the end
 //   tsm_diff_pairs_moves, behind the diff  MOVE_FLAGS      MOVE_JOIN       MOVE_RUNS       MOVE_MARK       at the end
 //   tsm_blame_pairs, behind the diff       BLAME                                                           at the end
@@ -193,6 +197,7 @@ constexpr int EV_CLONE_GROUP = 2, EV_CLONE_MEMBERS = 3, EV_CLONE_END = 4;
 constexpr int EV_BLIND_LEX = 5, EV_BLIND_LEX_END = 6;
 constexpr int EV_SMELL_KINDS = 2, EV_SMELL_LINES = 3, EV_SMELL_TESTS = 4, EV_SMELL_END = 5;
 constexpr EvSpan EV_CHURN_SMELLS = {0, 1}, EV_CHURN_CASES = {0, 1};   // the old side's scan slots, then the same again
+constexpr EvSpan EV_CHURN_LEX = {6, 7};                                 // the new side's scan slots (diff_core leaves them)
 constexpr EvSpan EV_MOVE_FLAGS = {0, 1}, EV_MOVE_JOIN = {2, 3}, EV_MOVE_RUNS = {4, 5}, EV_MOVE_MARK = {6, 7};
 constexpr EvSpan EV_BLAME = {0, 1};
 constexpr EvSpan EV_CCHURN = {0, 1};
@@ -2441,10 +2446,72 @@ extern "C" int tsm_smells(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, u
 extern "C" int tsm_smells_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_SMELL, ms4, 4); }
 
 // ------------------------------------------------------------------------------------- SPEC section 25 lexical test smells
-// The line records with header events (line_records), the case spans and smell stage of tsm_smells and the line start states
-// of the section-21 lexer (k_blind_state, k_blind_scan), one synchronisation for the test count, then k_lex_body, k_lex_lines
-// (count pass, xscan of the name counts, one synchronisation for their total, write pass) and k_lex_tests.  The outputs are
-// copied when they fit.
+// The lexical stage of ns sides whose smell stage has run (nt[s] tests each): per side the line start states of the section-21
+// lexer (k_blind_state, k_blind_scan), then for a side with tests k_lex_body, the count pass of k_lex_lines and an xscan of its
+// name counts; one synchronisation reads the name totals of every side; then per side the write pass and k_lex_tests.  at_tests,
+// when not NULL, is recorded before the k_lex_tests launches.  bsum holds total / XS_TILE + 4 u64 of the longest side; lsmell
+// (every line) and lex (nt + 1 records) are the outputs.
+struct LexBufs { DevBuf state, lxflag, lxend, lflag, ncnt, nbase, names, gset, lsmell, lex; };
+
+static int lex_stage(tsm_ctx* c, const HostSide* const* S, const SmellBufs* m, const uint32_t* nt, int ns, DevBuf& bsum, LexBufs* x,
+                     cudaEvent_t at_tests, int& launches, cudaStream_t st) {
+  unsigned long long* const pin = c->h_rb->u64 + 2;        // the name total of each side (u64[0, 2) hold the callers' test counts)
+  for (int s = 0; s < ns; ++s) {
+    const HostSide& h = *S[s];
+    LexBufs& b = x[s];
+    const unsigned long long total = h.total;
+    const size_t L = (size_t)total;
+    const uint32_t nfu = (uint32_t)h.n;
+    if (!b.state.alloc(L) || !b.lxflag.alloc(L) || !b.lxend.alloc(4 * L) || !b.lflag.alloc(L) || !b.ncnt.alloc(4 * L) ||
+        !b.nbase.alloc(8 * (L + 1)) || !b.lsmell.alloc(L) || !b.lex.alloc(sizeof(tsm_lex_test) * ((size_t)nt[s] + 1)))
+      return TSM_E_CUDA;
+    const unsigned grid = (unsigned)((L + 255) / 256);
+    if (L) {                                               // (a side of a revision pair may have no line)
+      k_blind_state<<<grid, 256, 0, st>>>(h.d, nfu, total, b.state.as<uint8_t>());
+      k_blind_scan<<<(unsigned)(((size_t)nfu * 32 + 255) / 256), 256, 0, st>>>(h.d.line_base, nfu, b.state.as<uint8_t>());
+      launches += 2;
+    }
+    CU(cudaMemsetAsync(b.lxflag.p, 0, L, st));
+    CU(cudaMemsetAsync(b.lsmell.p, 0, L, st));
+    if (!nt[s]) continue;
+    const unsigned tgrid = std::min((unsigned)((nt[s] + 7) / 8), (unsigned)c->sms * 8);
+    k_lex_body<<<tgrid, 256, 0, st>>>(LexBody{m[s].tests.as<tsm_smell_test>(), nt[s], h.d.line_base, h.d.ext, m[s].kind.as<uint8_t>(),
+                                              m[s].lines.as<SmellLine>(), b.lxflag.as<uint8_t>(), b.lxend.as<uint32_t>()});
+    k_lex_lines<false><<<grid, 256, 0, st>>>(h.d, nfu, total, b.state.as<uint8_t>(), b.lxflag.as<uint8_t>(), b.lxend.as<uint32_t>(),
+                                             b.lflag.as<uint8_t>(), b.ncnt.as<uint32_t>(), nullptr, nullptr);
+    xscan(b.ncnt.as<uint32_t>(), (uint32_t)total, bsum.as<unsigned long long>(), b.nbase.as<unsigned long long>(), st);
+    CU(cudaMemcpyAsync(pin + s, b.nbase.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
+    launches += 5;                                         // body, lines, xscan (3)
+  }
+  CU(cudaStreamSynchronize(st));
+  for (int s = 0; s < ns; ++s) {
+    if (!nt[s]) continue;
+    const HostSide& h = *S[s];
+    LexBufs& b = x[s];
+    const unsigned long long total = h.total;
+    if (!b.names.alloc(8 * (size_t)pin[s]) || !b.gset.alloc(16 * (size_t)pin[s])) return TSM_E_CUDA;
+    CU(cudaMemsetAsync(b.gset.p, 0xFF, 16 * (size_t)pin[s], st));
+    k_lex_lines<true><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(h.d, (uint32_t)h.n, total, b.state.as<uint8_t>(), b.lxflag.as<uint8_t>(),
+                                                                       b.lxend.as<uint32_t>(), b.lflag.as<uint8_t>(), b.ncnt.as<uint32_t>(),
+                                                                       b.nbase.as<unsigned long long>(), b.names.as<unsigned long long>());
+    ++launches;
+  }
+  if (at_tests) CU(cudaEventRecord(at_tests, st));
+  for (int s = 0; s < ns; ++s) {
+    if (!nt[s]) continue;
+    const HostSide& h = *S[s];
+    LexBufs& b = x[s];
+    k_lex_tests<<<std::min((unsigned)((nt[s] + 7) / 8), (unsigned)c->sms * 8), 256, 0, st>>>(
+        LexTests{m[s].tests.as<tsm_smell_test>(), nt[s], h.d.line_base, b.lflag.as<uint8_t>(), b.nbase.as<unsigned long long>(),
+                 b.names.as<unsigned long long>(), b.gset.as<unsigned long long>(), b.lsmell.as<uint8_t>(), b.lex.as<tsm_lex_test>()});
+    ++launches;
+  }
+  CU(cudaGetLastError());
+  return TSM_OK;
+}
+
+// The line records with header events (line_records), the case spans and smell stage of tsm_smells, one synchronisation for the
+// test count, then the lexical stage (lex_stage).  The outputs are copied when they fit.
 extern "C" int tsm_smells_lexical(tsm_ctx* c, const tsm_corpus* k, int64_t* line_base, uint16_t* line_smell, uint8_t* line_lsmell,
                                   int64_t line_cap, int64_t* n_lines, tsm_smell_test* tests, tsm_lex_test* lex, int64_t test_cap,
                                   int64_t* n_tests, void* stream) {
@@ -2457,57 +2524,26 @@ extern "C" int tsm_smells_lexical(tsm_ctx* c, const tsm_corpus* k, int64_t* line
   if (!line_base) { own_base.resize((size_t)nf + 1); line_base = own_base.data(); }
   return line_records(c, k, true, line_base, INT64_MAX, n_lines, stream, [&](const HostSide& S, unsigned long long total, cudaStream_t st) -> int {
     const size_t L = (size_t)total;
-    const uint32_t nfu = (uint32_t)S.n;
     CaseSpans sp;
     SmellBufs m;
-    DevBuf d_bsum, d_state, d_lxflag, d_lxend, d_lflag, d_ncnt, d_nbase, d_names, d_gset, d_lsmell, d_lex;
-    if (!d_bsum.alloc(8 * (L / XS_TILE + 4)) || !d_lxflag.alloc(L) || !d_lxend.alloc(4 * L) || !d_lflag.alloc(L) ||
-        !d_ncnt.alloc(4 * L) || !d_nbase.alloc(8 * (L + 1)) || !d_lsmell.alloc(L))
-      return TSM_E_CUDA;
+    LexBufs x;
+    DevBuf d_bsum;
+    if (!d_bsum.alloc(8 * (L / XS_TILE + 4))) return TSM_E_CUDA;
     int launches = 0;
     CU(cudaEventRecord(c->diff_ev[EV_LX_FRONT], st));
     int rc = case_spans(S, sp, d_bsum, launches, st);
     if (rc == TSM_OK) rc = smell_stage(c, S, sp, d_bsum, m, launches, st);
     if (rc != TSM_OK) return rc;
-    const unsigned grid = (unsigned)((L + 255) / 256);
-    if (!d_state.alloc(L)) return TSM_E_CUDA;
-    k_blind_state<<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>());
-    k_blind_scan<<<(unsigned)(((size_t)nfu * 32 + 255) / 256), 256, 0, st>>>(S.d.line_base, nfu, d_state.as<uint8_t>());
-    launches += 2;
-    CU(cudaMemsetAsync(d_lxflag.p, 0, L, st));
-    CU(cudaMemsetAsync(d_lsmell.p, 0, L, st));
     CU(cudaEventRecord(c->diff_ev[EV_LX_LINES], st));
     unsigned long long* pin = c->h_rb->u64;
     CU(cudaMemcpyAsync(pin, m.tidx.as<unsigned long long>() + sp.n_cases, 8, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    const unsigned long long nt = *pin;
+    const uint32_t nt = (uint32_t)*pin;
     *n_tests = (int64_t)nt;
     ms[1] = elapsed_ms(c->diff_ev[EV_LX_FRONT], c->diff_ev[EV_LX_LINES]);
-    if (!d_lex.alloc(sizeof(tsm_lex_test) * ((size_t)nt + 1))) return TSM_E_CUDA;
-    if (nt) {
-      const unsigned tgrid = std::min((unsigned)((nt + 7) / 8), (unsigned)c->sms * 8);
-      const tsm_smell_test* dt = m.tests.as<tsm_smell_test>();
-      k_lex_body<<<tgrid, 256, 0, st>>>(LexBody{dt, (uint32_t)nt, S.d.line_base, S.d.ext, m.kind.as<uint8_t>(), m.lines.as<SmellLine>(),
-                                                d_lxflag.as<uint8_t>(), d_lxend.as<uint32_t>()});
-      k_lex_lines<false><<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>(), d_lxflag.as<uint8_t>(), d_lxend.as<uint32_t>(),
-                                               d_lflag.as<uint8_t>(), d_ncnt.as<uint32_t>(), nullptr, nullptr);
-      xscan(d_ncnt.as<uint32_t>(), (uint32_t)total, d_bsum.as<unsigned long long>(), d_nbase.as<unsigned long long>(), st);
-      CU(cudaMemcpyAsync(pin + 1, d_nbase.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
-      CU(cudaStreamSynchronize(st));
-      if (!d_names.alloc(8 * (size_t)pin[1]) || !d_gset.alloc(16 * (size_t)pin[1])) return TSM_E_CUDA;
-      CU(cudaMemsetAsync(d_gset.p, 0xFF, 16 * (size_t)pin[1], st));
-      k_lex_lines<true><<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>(), d_lxflag.as<uint8_t>(), d_lxend.as<uint32_t>(),
-                                              d_lflag.as<uint8_t>(), d_ncnt.as<uint32_t>(), d_nbase.as<unsigned long long>(),
-                                              d_names.as<unsigned long long>());
-      CU(cudaEventRecord(c->diff_ev[EV_LX_TESTS], st));
-      k_lex_tests<<<tgrid, 256, 0, st>>>(LexTests{dt, (uint32_t)nt, S.d.line_base, d_lflag.as<uint8_t>(), d_nbase.as<unsigned long long>(),
-                                                 d_names.as<unsigned long long>(), d_gset.as<unsigned long long>(), d_lsmell.as<uint8_t>(),
-                                                 d_lex.as<tsm_lex_test>()});
-      launches += 7;                                       // body, lines, xscan (3), lines (write), tests
-    } else {
-      CU(cudaEventRecord(c->diff_ev[EV_LX_TESTS], st));
-    }
-    CU(cudaGetLastError());
+    const HostSide* side = &S;
+    rc = lex_stage(c, &side, &m, &nt, 1, d_bsum, &x, c->diff_ev[EV_LX_TESTS], launches, st);
+    if (rc != TSM_OK) return rc;
     CU(cudaEventRecord(c->diff_ev[EV_LX_END], st));
     CU(cudaStreamSynchronize(st));
     c->launches += launches;
@@ -2515,9 +2551,9 @@ extern "C" int tsm_smells_lexical(tsm_ctx* c, const tsm_corpus* k, int64_t* line
     ms[3] = elapsed_ms(c->diff_ev[EV_LX_TESTS], c->diff_ev[EV_LX_END]);
     if (((line_smell || line_lsmell) && line_cap < (int64_t)total) || ((tests || lex) && test_cap < (int64_t)nt)) return TSM_E_CAPACITY;
     if (line_smell) CU(cudaMemcpyAsync(line_smell, m.smell.p, 2 * L, cudaMemcpyDeviceToHost, st));
-    if (line_lsmell) CU(cudaMemcpyAsync(line_lsmell, d_lsmell.p, L, cudaMemcpyDeviceToHost, st));
+    if (line_lsmell) CU(cudaMemcpyAsync(line_lsmell, x.lsmell.p, L, cudaMemcpyDeviceToHost, st));
     if (tests && nt) CU(cudaMemcpyAsync(tests, m.tests.p, sizeof(tsm_smell_test) * nt, cudaMemcpyDeviceToHost, st));
-    if (lex && nt) CU(cudaMemcpyAsync(lex, d_lex.p, sizeof(tsm_lex_test) * nt, cudaMemcpyDeviceToHost, st));
+    if (lex && nt) CU(cudaMemcpyAsync(lex, x.lex.p, sizeof(tsm_lex_test) * nt, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     return TSM_OK;
   }, &ms[0], TSM_SCAN_HEADER_EVENTS);
@@ -3129,16 +3165,17 @@ extern "C" int tsm_similar_churn_last_ms(tsm_ctx* c, float* ms4) { return copy_m
 
 // ------------------------------------------------------------------------------------- SPEC section 19 test-smell churn
 // The line records of both sides with their header events, per side the case spans and the smell stage, one synchronisation
-// for the case and test counts (the capacity check comes before the diff), the marks diff, the case records (with the new
-// side's by_rank) and k_smell_churn per side.  EV_CHURN_SMELLS times the smell stages, and EV_CHURN_CASES, the same slots
-// again once read, the case records and churn behind the diff.
-extern "C" int tsm_diff_pairs_smells(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
-                                     tsm_diff_detail* detail, tsm_diff_smells* out, void* stream) {
+// for the case and test counts (the capacity check comes before the diff), with lex (section 26) the lexical stage of both sides
+// (lex_stage), the marks diff, the case records (with the new side's by_rank) and k_smell_churn per side (<true> with lex).
+// EV_CHURN_SMELLS times the smell stages, EV_CHURN_LEX the lexical stages, and EV_CHURN_CASES, the first slots again once
+// read, the case records and churn behind the diff.
+static int diff_smells(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                       tsm_diff_detail* detail, tsm_diff_smells* out, tsm_diff_lex_smells* lex, void* stream) {
   if (!c || !olds || !news || !added || !removed || !out || olds->n_files != news->n_files || out->cases.old_cap < 0 ||
       out->cases.new_cap < 0 || out->old_test_cap < 0 || out->new_test_cap < 0)
     return TSM_E_ARG;
   const int32_t n = olds->n_files;
-  float* const ms = clear_ms(c, MS_CHURN);
+  float* const ms = clear_ms(c, lex ? MS_LEXCHURN : MS_CHURN);
   out->cases.n_old = out->cases.n_new = out->n_old_tests = out->n_new_tests = 0;
   if (n == 0) return TSM_OK;
   float* const dm = c->last_ms[MS_DIFF];
@@ -3147,7 +3184,8 @@ extern "C" int tsm_diff_pairs_smells(tsm_ctx* c, const tsm_corpus* olds, const t
     const HostSide* side[2] = {&P.A, &P.B};
     PairCases pc;
     SmellBufs sb[2];
-    DevBuf d_churn[2];
+    LexBufs lb[2];
+    DevBuf d_churn[2], d_lchurn[2];
     int launches = 0;
     CU(cudaEventRecord(c->diff_ev[EV_CHURN_SMELLS.from], st));
     int rc = pair_case_spans(P, pc, launches, st);
@@ -3164,8 +3202,16 @@ extern "C" int tsm_diff_pairs_smells(tsm_ctx* c, const tsm_corpus* olds, const t
     out->n_old_tests = nt[0]; out->n_new_tests = nt[1];
     if ((out->cases.old_cases && out->cases.old_cap < out->cases.n_old) || (out->cases.new_cases && out->cases.new_cap < out->cases.n_new) ||
         ((out->old_tests || out->old_churn) && out->old_test_cap < (int64_t)nt[0]) ||
-        ((out->new_tests || out->new_churn) && out->new_test_cap < (int64_t)nt[1]))
+        ((out->new_tests || out->new_churn) && out->new_test_cap < (int64_t)nt[1]) ||
+        (lex && (lex->old_lex || lex->old_churn) && out->old_test_cap < (int64_t)nt[0]) ||
+        (lex && (lex->new_lex || lex->new_churn) && out->new_test_cap < (int64_t)nt[1]))
       return TSM_E_CAPACITY;
+    if (lex) {
+      CU(cudaEventRecord(c->diff_ev[EV_CHURN_LEX.from], st));
+      rc = lex_stage(c, side, sb, nt, 2, pc.bsum, lb, nullptr, launches, st);
+      if (rc != TSM_OK) return rc;
+      CU(cudaEventRecord(c->diff_ev[EV_CHURN_LEX.to], st));
+    }
     rc = diff_core<DIFF_MARKS>(c, P.A, P.B, n, added, removed, detail, st);
     if (rc != TSM_OK) return rc;
     ms[2] = dm[1] + dm[2];
@@ -3174,12 +3220,18 @@ extern "C" int tsm_diff_pairs_smells(tsm_ctx* c, const tsm_corpus* olds, const t
     if (rc != TSM_OK) return rc;
     for (int s = 0; s < 2; ++s) {
       if (!d_churn[s].alloc(sizeof(tsm_test_churn) * (size_t)nt[s])) return TSM_E_CUDA;
+      if (lex && !d_lchurn[s].alloc(sizeof(tsm_lex_churn) * (size_t)nt[s])) return TSM_E_CUDA;
       if (!nt[s]) continue;
       const int o = 1 - s;
       const ChurnSide cs{side[s]->d.line_base, sb[s].tests.as<tsm_smell_test>(), nt[s], sb[s].smell.as<uint16_t>(),
                          side[s]->line_mark.as<uint8_t>(), pc.rank[s].as<unsigned long long>(), pc.sp[s].case_of.as<unsigned long long>(),
                          sb[o].smell.as<uint16_t>(), pc.by_rank[o].as<uint32_t>(), d_churn[s].as<tsm_test_churn>()};
-      k_smell_churn<<<std::min((nt[s] + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(cs);
+      const unsigned grid = std::min((nt[s] + 7) / 8, (uint32_t)c->sms * 8);
+      if (lex)
+        k_smell_churn<true><<<grid, 256, 0, st>>>(cs, LexChurnSide{lb[s].lsmell.as<uint8_t>(), lb[o].lsmell.as<uint8_t>(),
+                                                                   d_lchurn[s].as<tsm_lex_churn>()});
+      else
+        k_smell_churn<false><<<grid, 256, 0, st>>>(cs, LexChurnSide{});
       ++launches;
     }
     CU(cudaGetLastError());
@@ -3193,14 +3245,38 @@ extern "C" int tsm_diff_pairs_smells(tsm_ctx* c, const tsm_corpus* olds, const t
       if (h_tests[s] && nt[s]) CU(cudaMemcpyAsync(h_tests[s], sb[s].tests.p, sizeof(tsm_smell_test) * nt[s], cudaMemcpyDeviceToHost, st));
       if (h_churn[s] && nt[s]) CU(cudaMemcpyAsync(h_churn[s], d_churn[s].p, sizeof(tsm_test_churn) * nt[s], cudaMemcpyDeviceToHost, st));
     }
+    if (lex) {
+      tsm_lex_test* const h_lex[2] = {lex->old_lex, lex->new_lex};
+      tsm_lex_churn* const h_lchurn[2] = {lex->old_churn, lex->new_churn};
+      for (int s = 0; s < 2; ++s) {
+        if (h_lex[s] && nt[s]) CU(cudaMemcpyAsync(h_lex[s], lb[s].lex.p, sizeof(tsm_lex_test) * nt[s], cudaMemcpyDeviceToHost, st));
+        if (h_lchurn[s] && nt[s])
+          CU(cudaMemcpyAsync(h_lchurn[s], d_lchurn[s].p, sizeof(tsm_lex_churn) * nt[s], cudaMemcpyDeviceToHost, st));
+      }
+    }
     CU(cudaStreamSynchronize(st));
+    if (lex) ms[1] += span_ms(c, EV_CHURN_LEX);
     ms[3] = span_ms(c, EV_CHURN_CASES);
     c->launches += launches;
     return TSM_OK;
   });
 }
 
+extern "C" int tsm_diff_pairs_smells(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                                     tsm_diff_detail* detail, tsm_diff_smells* out, void* stream) {
+  return diff_smells(c, olds, news, added, removed, detail, out, nullptr, stream);
+}
+
 extern "C" int tsm_diff_smells_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_CHURN, ms4, 4); }
+
+// ------------------------------------------------------------------------------------- SPEC section 26 lexical test-smell churn
+extern "C" int tsm_diff_pairs_smells_lexical(tsm_ctx* c, const tsm_corpus* olds, const tsm_corpus* news, int64_t* added, int64_t* removed,
+                                             tsm_diff_detail* detail, tsm_diff_smells* out, tsm_diff_lex_smells* lex, void* stream) {
+  if (!lex) return TSM_E_ARG;
+  return diff_smells(c, olds, news, added, removed, detail, out, lex, stream);
+}
+
+extern "C" int tsm_diff_smells_lexical_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_LEXCHURN, ms4, 4); }
 
 // ------------------------------------------------------------------------------------- SPEC section 20 moved code
 // The line records of both sides, the marks diff, then per side k_move_lines and three exclusive scans (alnum prefix, entry and

@@ -11,7 +11,8 @@
 //                   duplicate assertions by comparing every assertion hash with every earlier one of the test through
 //                   shuffles, 32 x 32 per tile pair (O(A^2 / 32) per test); lane 0 walks the '@' lines above the header.
 //   k_smell_churn   persistent warps, one test of one side of revision pairs at a time, 32 body lines per round: per smell the
-//                   instance lines and those the revision adds or removes (docs/SPEC.md section 19), by ballots.
+//                   instance lines and those the revision adds or removes (docs/SPEC.md section 19), by ballots; <true> also
+//                   those of the five lexical smells (section 26) in the same walk.
 #pragma once
 #include "tsm_device.cuh"
 #include "tsm_diff_kernels.cuh"
@@ -371,10 +372,16 @@ struct ChurnSide {
   const uint16_t* other_smell; const uint32_t* other_by_rank; tsm_test_churn* out;
 };
 
+// The lexical smells of one side (docs/SPEC.md section 26): its line_lsmell, the other side's, and one record per test.
+struct LexChurnSide { const uint8_t* line_lsmell; const uint8_t* other_lsmell; tsm_lex_churn* out; };
+
 // Persistent warps, one test at a time, 32 body lines per round: the instances of a line are its smell bits, its churned
 // instances the bits the corresponding line of the other side lacks (all of them on a deleted or inserted line).  Lane k < 9
-// counts smell k from one ballot per smell and kind.
-__global__ void __launch_bounds__(256) k_smell_churn(ChurnSide s) {
+// counts smell k from one ballot per smell and kind.  kLex: the line's TSM_LSMELL_* bits join above the nine (bit 9 + k),
+// looked up through the same kept rank, and lanes 9..13 count them into x.out (x is unused otherwise).
+template <bool kLex>
+__global__ void __launch_bounds__(256) k_smell_churn(ChurnSide s, LexChurnSide x) {
+  constexpr uint32_t K = kLex ? TSM_N_SMELLS + TSM_N_LSMELLS : TSM_N_SMELLS;
   const uint32_t lane = threadIdx.x & 31, warps = gridDim.x * (blockDim.x >> 5);
   for (uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; t < s.n_tests; t += warps) {
     const tsm_smell_test r = s.tests[t];
@@ -383,10 +390,19 @@ __global__ void __launch_bounds__(256) k_smell_churn(ChurnSide s) {
     for (uint32_t base = b; base < e; base += 32) {
       const uint32_t l = base + lane;
       uint32_t bits = 0, churn = 0;
-      if (l < e && (bits = s.line_smell[l]) != 0)
-        churn = s.mark[l] ? bits : bits & ~(uint32_t)s.other_smell[s.other_by_rank[s.rank[l]]];
+      if constexpr (!kLex) {
+        if (l < e && (bits = s.line_smell[l]) != 0)
+          churn = s.mark[l] ? bits : bits & ~(uint32_t)s.other_smell[s.other_by_rank[s.rank[l]]];
+      } else if (l < e && (bits = s.line_smell[l] | (uint32_t)x.line_lsmell[l] << TSM_N_SMELLS) != 0) {
+        if (s.mark[l]) {
+          churn = bits;
+        } else {
+          const uint32_t m = s.other_by_rank[s.rank[l]];
+          churn = bits & ~(s.other_smell[m] | (uint32_t)x.other_lsmell[m] << TSM_N_SMELLS);
+        }
+      }
 #pragma unroll
-      for (uint32_t k = 0; k < TSM_N_SMELLS; ++k) {
+      for (uint32_t k = 0; k < K; ++k) {
         const uint32_t mi = __ballot_sync(0xffffffffu, (bits >> k) & 1u), mc = __ballot_sync(0xffffffffu, (churn >> k) & 1u);
         if (lane == k) { ni += __popc(mi); nc += __popc(mc); }
       }
@@ -394,6 +410,11 @@ __global__ void __launch_bounds__(256) k_smell_churn(ChurnSide s) {
     tsm_test_churn* o = s.out + t;
     if (lane == 0) o->case_idx = (int32_t)s.case_of[b];
     if (lane < TSM_N_SMELLS) { o->instances[lane] = (int32_t)ni; o->churned[lane] = (int32_t)nc; }
+    if constexpr (kLex)
+      if (lane >= TSM_N_SMELLS && lane < K) {
+        x.out[t].instances[lane - TSM_N_SMELLS] = (int32_t)ni;
+        x.out[t].churned[lane - TSM_N_SMELLS] = (int32_t)nc;
+      }
   }
 }
 

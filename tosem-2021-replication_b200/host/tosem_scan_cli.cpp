@@ -18,11 +18,11 @@
 //   tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N]
 //   tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]
 //   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--smells F]
-//                     [--moves F] [--clones F] [--similar-tests F] [--min-lines N] [--similarity P] [--find-renames N] [--batch-bytes N]
+//                     [--lexical] [--moves F] [--clones F] [--similar-tests F] [--min-lines N] [--similarity P] [--find-renames N] [--batch-bytes N]
 //   tosem-scan body   <project-root>... [--batch-bytes N] [--out F]
 //   tosem-scan releases <snapshot-root>=<tag>... | --git <repository> [<revision>...]   [--batch-bytes N] [--out F]
 //   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F] [--cases F]
-//                      [--assert-edits F] [--smells F] [--moves F] [--clones F] [--similar-tests F] [--find-renames N] [--batch-bytes N]
+//                      [--assert-edits F] [--smells F] [--lexical] [--moves F] [--clones F] [--similar-tests F] [--find-renames N] [--batch-bytes N]
 //   tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]
 //   tosem-scan clones <project-root>... | --git <repository> [--rev R]   [--min-lines N] [--blind] [--all-files] [--out F]
 // Every command that scans files does it with scan_batches: batches of at most --batch-bytes of arena (clones: all files in one),
@@ -1201,25 +1201,40 @@ static void diff_cases(tsm_ctx* ctx, const tsm_corpus& ca, const tsm_corpus& cn,
 }
 
 // Test-smell churn (docs/SPEC.md section 19) of one diff call: the case records (as diff_cases), the tests of both sides and their
-// churn records (tsm_diff_pairs_smells), arrays grown to the counts the library reports when they are too small.
-struct SmellLists { std::vector<tsm_smell_test> olds, news; std::vector<tsm_test_churn> old_churn, new_churn; };
+// churn records (tsm_diff_pairs_smells), arrays grown to the counts the library reports when they are too small.  lexical: one
+// tsm_diff_pairs_smells_lexical call instead, which adds the lexical records of every test (section 26); without it they stay empty.
+struct SmellLists {
+  std::vector<tsm_smell_test> olds, news; std::vector<tsm_test_churn> old_churn, new_churn;
+  std::vector<tsm_lex_test> old_lex, new_lex; std::vector<tsm_lex_churn> old_lchurn, new_lchurn;
+};
 static void diff_smells(tsm_ctx* ctx, const tsm_corpus& ca, const tsm_corpus& cn, int64_t* added, int64_t* removed,
-                        tsm_diff_detail* det, CaseLists& c, SmellLists& r) {
+                        tsm_diff_detail* det, CaseLists& c, SmellLists& r, bool lexical) {
   int64_t co = (int64_t)ca.off[ca.n_files] / 512 + 64, cc = (int64_t)cn.off[cn.n_files] / 512 + 64, to = co, tn = cc;
   for (;;) {
     c.olds.resize((size_t)co); c.news.resize((size_t)cc);
     r.olds.resize((size_t)to); r.old_churn.resize((size_t)to); r.news.resize((size_t)tn); r.new_churn.resize((size_t)tn);
     tsm_diff_smells o{{c.olds.data(), co, 0, c.news.data(), cc, 0}, r.olds.data(), r.old_churn.data(), to, 0,
                       r.news.data(), r.new_churn.data(), tn, 0};
-    const int rc = tsm_diff_pairs_smells(ctx, &ca, &cn, added, removed, det, &o, nullptr);
+    int rc;
+    if (lexical) {
+      r.old_lex.resize((size_t)to); r.old_lchurn.resize((size_t)to); r.new_lex.resize((size_t)tn); r.new_lchurn.resize((size_t)tn);
+      tsm_diff_lex_smells x{r.old_lex.data(), r.old_lchurn.data(), r.new_lex.data(), r.new_lchurn.data()};
+      rc = tsm_diff_pairs_smells_lexical(ctx, &ca, &cn, added, removed, det, &o, &x, nullptr);
+    } else {
+      rc = tsm_diff_pairs_smells(ctx, &ca, &cn, added, removed, det, &o, nullptr);
+    }
     if (rc == TSM_E_CAPACITY && (o.cases.n_old > co || o.cases.n_new > cc || o.n_old_tests > to || o.n_new_tests > tn)) {
       co = std::max(co, o.cases.n_old); cc = std::max(cc, o.cases.n_new); to = std::max(to, o.n_old_tests); tn = std::max(tn, o.n_new_tests);
       continue;
     }
-    ck(rc, "tsm_diff_pairs_smells");
+    ck(rc, lexical ? "tsm_diff_pairs_smells_lexical" : "tsm_diff_pairs_smells");
     c.olds.resize((size_t)o.cases.n_old); c.news.resize((size_t)o.cases.n_new);
     r.olds.resize((size_t)o.n_old_tests); r.old_churn.resize((size_t)o.n_old_tests);
     r.news.resize((size_t)o.n_new_tests); r.new_churn.resize((size_t)o.n_new_tests);
+    if (lexical) {
+      r.old_lex.resize((size_t)o.n_old_tests); r.old_lchurn.resize((size_t)o.n_old_tests);
+      r.new_lex.resize((size_t)o.n_new_tests); r.new_lchurn.resize((size_t)o.n_new_tests);
+    }
     return;
   }
 }
@@ -1288,13 +1303,28 @@ static void case_rows(std::ostream& os, std::vector<std::string> lead, const Cas
   }
 }
 
+// The lexical records of one side's tests (docs/SPEC.md section 26), or none (lex NULL).
+struct LexSide { const tsm_lex_test* lex; const tsm_lex_churn* churn; };
+
 // The --smells rows of one pair (docs/SPEC.md section 19) from its cases (as case_rows, new case index n_first being nc[0]) and
 // its tests ot / nt with their churn records och / nch: two tests match when their cases do.  D tests in old line order, then A
-// and M tests in new line order, each test's rows in smell order.
+// and M tests in new line order, each test's rows in smell order: the nine, then with lexical records (ol / nl) the five of
+// section 26, whose smells, instances and churn those records give.
 static void smell_rows(std::ostream& os, const std::vector<std::string>& lead, const CaseSide& o, const CaseSide& nw, const std::string* old_path,
                        const tsm_case* oc, size_t no, const tsm_case* nc, size_t nn, size_t o_first, size_t n_first,
                        const tsm_smell_test* ot, const tsm_test_churn* och, size_t nto, const tsm_smell_test* nt, const tsm_test_churn* nch,
-                       size_t ntn) {
+                       size_t ntn, LexSide ol, LexSide nl) {
+  const int nk = TSM_N_SMELLS + (ol.lex || nl.lex ? TSM_N_LSMELLS : 0);   // (a side without tests has no records)
+  auto name_of = [](int k) { return k < TSM_N_SMELLS ? kSmellNames[k] : kLexSmellNames[k - TSM_N_SMELLS]; };
+  auto smells = [](const tsm_smell_test& x, LexSide l, size_t t) {   // the nine bits, then the five
+    return (uint32_t)x.smells | (l.lex ? l.lex[t].smells << TSM_N_SMELLS : 0u);
+  };
+  auto inst = [](const tsm_test_churn& c, LexSide l, size_t t, int k) {
+    return (int64_t)(k < TSM_N_SMELLS ? c.instances[k] : l.churn[t].instances[k - TSM_N_SMELLS]);
+  };
+  auto churned = [](const tsm_test_churn& c, LexSide l, size_t t, int k) {
+    return (int64_t)(k < TSM_N_SMELLS ? c.churned[k] : l.churn[t].churned[k - TSM_N_SMELLS]);
+  };
   const PairCaseMatch pm(o, nw, oc, no, nc, nn, o_first);
   std::vector<int64_t> test_of_case(no, -1), pair_of(ntn, -1);   // old test of each old case; matched old test of each new test
   std::vector<char> old_matched(nto, 0);
@@ -1314,28 +1344,34 @@ static void smell_rows(std::ostream& os, const std::vector<std::string>& lead, c
   for (size_t t = 0; t < nto; ++t) {
     if (old_matched[t]) continue;
     const std::string& name = pm.na[(size_t)och[t].case_idx - o_first];
-    for (int k = 0; k < TSM_N_SMELLS; ++k)
-      if (ot[t].smells >> k & 1u)
-        row(*o.path, name, {"D", "", num(ot[t].line + 1), kSmellNames[k], "removed", "", num(och[t].instances[k]), "", num(och[t].churned[k])});
+    const uint32_t sm = smells(ot[t], ol, t);
+    for (int k = 0; k < nk; ++k)
+      if (sm >> k & 1u)
+        row(*o.path, name, {"D", "", num(ot[t].line + 1), name_of(k), "removed", "", num(inst(och[t], ol, t, k)), "",
+                            num(churned(och[t], ol, t, k))});
   }
   for (size_t t = 0; t < ntn; ++t) {
     const std::string& name = pm.nb[(size_t)nch[t].case_idx - n_first];
     const tsm_smell_test& x = nt[t];
     const tsm_test_churn& c = nch[t];
+    const uint32_t sn = smells(x, nl, t);
     if (pair_of[t] < 0) {
-      for (int k = 0; k < TSM_N_SMELLS; ++k)
-        if (x.smells >> k & 1u)
-          row(*nw.path, name, {"A", num(x.line + 1), "", kSmellNames[k], "introduced", num(c.instances[k]), "", num(c.churned[k]), ""});
+      for (int k = 0; k < nk; ++k)
+        if (sn >> k & 1u)
+          row(*nw.path, name, {"A", num(x.line + 1), "", name_of(k), "introduced", num(inst(c, nl, t, k)), "", num(churned(c, nl, t, k)), ""});
       continue;
     }
-    const tsm_smell_test& y = ot[(size_t)pair_of[t]];
-    const tsm_test_churn& d = och[(size_t)pair_of[t]];
-    for (int k = 0; k < TSM_N_SMELLS; ++k) {
-      const bool hn = x.smells >> k & 1u, ho = y.smells >> k & 1u;
-      const char* ev = hn && !ho ? "introduced" : ho && !hn ? "removed" : hn && ho && (c.churned[k] || d.churned[k]) ? "changed" : nullptr;
+    const size_t u = (size_t)pair_of[t];
+    const tsm_smell_test& y = ot[u];
+    const tsm_test_churn& d = och[u];
+    const uint32_t so = smells(y, ol, u);
+    for (int k = 0; k < nk; ++k) {
+      const bool hn = sn >> k & 1u, ho = so >> k & 1u;
+      const int64_t cn = churned(c, nl, t, k), co = churned(d, ol, u, k);
+      const char* ev = hn && !ho ? "introduced" : ho && !hn ? "removed" : hn && ho && (cn || co) ? "changed" : nullptr;
       if (ev)
-        row(*nw.path, name, {"M", num(x.line + 1), num(y.line + 1), kSmellNames[k], ev, num(c.instances[k]), num(d.instances[k]),
-                             num(c.churned[k]), num(d.churned[k])});
+        row(*nw.path, name, {"M", num(x.line + 1), num(y.line + 1), name_of(k), ev, num(inst(c, nl, t, k)), num(inst(d, ol, u, k)),
+                             num(cn), num(co)});
     }
   }
 }
@@ -1568,6 +1604,7 @@ struct DiffOptions {
   int rename_pct = -1;
   int64_t batch_bytes = kBatch;
   std::string out, asserts, churn, cases, edits, smells, moves;
+  bool smell_lexical = false;                              // --lexical, read only with --smells
   std::string clones;                                      // --clones F, with its --min-lines, --blind and the file selection
   int clone_min_lines = 5; bool clone_blind = false, all_files = false;
   std::string similar;                                     // --similar-tests F, with --min-lines (shared with --clones) and --similarity
@@ -1580,24 +1617,24 @@ struct DiffOptions {
 
 // The diff of one batch: per pair the lines added and removed and the detail; with `asserts` the changed assertion lines and
 // the [group][K] tables, with `edits` also the assertion edits (the same call), with `cases` the case records, with `smells`
-// the case records, the tests and their smell churn (one call, which also serves `cases`), with `moves` the moved blocks (a call
-// of its own).
+// the case records, the tests and their smell churn (one call, which also serves `cases`; with `lexical` also the lexical smells),
+// with `moves` the moved blocks (a call of its own).
 struct PairDiff {
   std::vector<int64_t> added, removed; std::vector<tsm_diff_detail> det; ChangedAsserts chg; CaseLists cases; std::vector<tsm_assert_edit> edits;
   SmellLists smells; MoveLists moves;
 };
-static PairDiff diff_batch(const PairBatch& b, bool asserts, bool cases, bool edits, bool smells, bool moves) {
+static PairDiff diff_batch(const PairBatch& b, bool asserts, bool cases, bool edits, bool smells, bool lexical, bool moves) {
   const size_t n = b.idx.size();
   PairDiff d{std::vector<int64_t>(n), std::vector<int64_t>(n), std::vector<tsm_diff_detail>(n), {}, {}, {}, {}, {}};
   const tsm_corpus ca = b.olds.corpus(b.n_groups()), cn = b.news.corpus(b.n_groups());
   if (edits) diff_assert_edits(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.chg, d.edits);
   else if (asserts) diff_asserts(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.chg);
-  else if (smells) diff_smells(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.cases, d.smells);
+  else if (smells) diff_smells(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.cases, d.smells, lexical);
   else if (cases) diff_cases(b.ctx, ca, cn, d.added.data(), d.removed.data(), d.det.data(), d.cases);
   else ck(tsm_diff_pairs_detail(b.ctx, &ca, &cn, d.added.data(), d.removed.data(), d.det.data(), nullptr), "tsm_diff_pairs_detail");
   if (asserts && (cases || smells)) {                      // a second call: the assertion tables and the cases are separate diffs
     std::vector<int64_t> a2(n), r2(n);
-    if (smells) diff_smells(b.ctx, ca, cn, a2.data(), r2.data(), nullptr, d.cases, d.smells);
+    if (smells) diff_smells(b.ctx, ca, cn, a2.data(), r2.data(), nullptr, d.cases, d.smells, lexical);
     else diff_cases(b.ctx, ca, cn, a2.data(), r2.data(), nullptr, d.cases);
   }
   if (moves) diff_moves(b.ctx, ca, cn, d.moves);
@@ -1640,7 +1677,7 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
   pair_batches(ctx.get(), changes, load, o.batch_bytes, want_asserts || ms.is_open(), ms.is_open(), t, [&](const PairBatch& b) {
     const size_t n = b.idx.size();
     if (!n) return;
-    const PairDiff d = diff_batch(b, want_asserts, cs.is_open(), es.is_open(), ss.is_open(), ms.is_open());
+    const PairDiff d = diff_batch(b, want_asserts, cs.is_open(), es.is_open(), ss.is_open(), o.smell_lexical, ms.is_open());
     auto path = [&](int s, size_t j) -> const std::string& {  // the path of pair j on side s (0 old, 1 new)
       const Change& c = changes[b.idx[j]];
       return s == 0 && !c.old_path.empty() ? c.old_path : c.path;
@@ -1674,12 +1711,16 @@ static ChangeTotals diff_changes(std::vector<Change>& changes, size_t n_steps, c
         case_rows(cs, o.lead(c.step), olds, news, renames ? &c.old_path : nullptr, d.cases.olds.data() + o0, ko - o0, d.cases.news.data() + n0,
                   kn - n0, o0);
       const size_t to0 = to, tn0 = tn;
+      auto lex_side = [](const std::vector<tsm_lex_test>& l, const std::vector<tsm_lex_churn>& c, size_t t0) {
+        return l.empty() ? LexSide{nullptr, nullptr} : LexSide{l.data() + t0, c.data() + t0};
+      };
       while (to < d.smells.olds.size() && d.smells.olds[to].file == (int32_t)i) ++to;
       while (tn < d.smells.news.size() && d.smells.news[tn].file == (int32_t)i) ++tn;
       if (to > to0 || tn > tn0)
         smell_rows(ss, o.lead(c.step), olds, news, renames ? &c.old_path : nullptr, d.cases.olds.data() + o0, ko - o0, d.cases.news.data() + n0,
                    kn - n0, o0, n0, d.smells.olds.data() + to0, d.smells.old_churn.data() + to0, to - to0, d.smells.news.data() + tn0,
-                   d.smells.new_churn.data() + tn0, tn - tn0);
+                   d.smells.new_churn.data() + tn0, tn - tn0, lex_side(d.smells.old_lex, d.smells.old_lchurn, to0),
+                   lex_side(d.smells.new_lex, d.smells.new_lchurn, tn0));
       if (ms.is_open()) move_rows(ms, o.lead(c.step), d.moves, i, km, path);
       t.added[c.step] += d.added[i]; t.removed[c.step] += d.removed[i]; t.files[c.step]++;
       if (!os.is_open() || !(o.zero_rows || d.added[i] || d.removed[i] || c.similarity >= 0)) continue;
@@ -2659,13 +2700,13 @@ static void usage() {
   fprintf(stderr,
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
           "       tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]\n"
-          "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--smells F]\n"
+          "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--smells F [--lexical]]\n"
           "                         [--moves F] [--clones F [--min-lines N] [--blind] [--all-files]] [--similar-tests F [--min-lines N] [--similarity P]] [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan body   <project-root>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases <snapshot-root>=<tag>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases --git <repository> [<revision>...] [--batch-bytes N] [--out F]\n"
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
-          "                          [--cases F] [--assert-edits F] [--smells F] [--moves F] [--clones F [--min-lines N] [--blind]] [--similar-tests F [--similarity P]]\n"
+          "                          [--cases F] [--assert-edits F] [--smells F [--lexical]] [--moves F] [--clones F [--min-lines N] [--blind]] [--similar-tests F [--similarity P]]\n"
           "                          [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
           "       tosem-scan clones <project-root>... [--min-lines N] [--blind] [--all-files] [--out F]\n"
@@ -2687,7 +2728,8 @@ static void usage() {
           "--assert-edits F: one row per deleted assertion line that an inserted one of the same hunk replaces, with their similarity\n"
           "                  (docs/SPEC.md section 17).\n"
           "--smells F: one row per (test, smell) that a revision introduces, removes or changes, with the smell's instances and the\n"
-          "            instance lines it adds and removes (docs/SPEC.md section 19).\n"
+          "            instance lines it adds and removes (docs/SPEC.md section 19); with --lexical also the five lexical smells\n"
+          "            (docs/SPEC.md section 26).\n"
           "--moves F: one row per block of changed lines that a commit moves, within or across its files, as git diff\n"
           "           --color-moved=blocks finds them (docs/SPEC.md section 20); a commit is never split across batches, and one\n"
           "           larger than --batch-bytes is a batch of its own.\n"
@@ -2756,6 +2798,7 @@ int main(int argc, char** argv) {
   d.rename_pct = rename_pct; d.batch_bytes = batch_bytes(kBatch, 1);
   d.out = opt["--out"]; d.asserts = opt["--asserts"]; d.churn = opt["--assert-churn"]; d.cases = opt["--cases"];
   d.edits = opt["--assert-edits"]; d.smells = opt["--smells"]; d.moves = opt["--moves"];
+  d.smell_lexical = lexical && opt.count("--smells");      // (--lexical is read only with --smells)
   if (opt.count("--clones")) {                             // (--min-lines and --blind are read only with --clones)
     d.clones = opt["--clones"]; d.clone_blind = blind; d.all_files = all_files;
     const long n = opt.count("--min-lines") ? strtol(opt["--min-lines"].c_str(), nullptr, 10) : 5;

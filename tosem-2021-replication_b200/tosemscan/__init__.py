@@ -41,6 +41,7 @@ LEX_TEST = np.dtype([("n_stmts", "<i4"), ("n_unexplained", "<i4"), ("n_magic", "
 LSMELLS = ["assertion_roulette", "magic_number", "suboptimal_assert", "mystery_guest",
            "obscure_setup"]                     # bit k of tsm_lex_test.smells and of line_lsmell is LSMELLS[k]
 TEST_CHURN = np.dtype([("case_idx", "<i4"), ("instances", "<i4", (9,)), ("churned", "<i4", (9,))])   # tsm_test_churn (section 19)
+LEX_CHURN = np.dtype([("instances", "<i4", (5,)), ("churned", "<i4", (5,))])   # tsm_lex_churn (section 26), smell k = LSMELLS[k]
 MOVE_BLOCK = np.dtype([("line", "<i8"), ("partner", "<i8"), ("n_lines", "<i4"),
                        ("n_assert", "<i4")])   # tsm_move_block: one moved block of one side (docs/SPEC.md section 20)
 SIMILAR_PAIR = np.dtype([("a", "<i4"), ("b", "<i4"), ("lcs", "<u4"),
@@ -60,7 +61,8 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_diff_pairs_cases", "tsm_diff_pairs_assert_edits", "tsm_assert_edits_last_ms", "tsm_smells", "tsm_smells_last_ms",
            "tsm_diff_pairs_smells", "tsm_diff_smells_last_ms", "tsm_diff_pairs_moves", "tsm_moves_last_ms", "tsm_clones_blind",
            "tsm_clones_blind_last_ms", "tsm_clone_churn", "tsm_clone_churn_last_ms", "tsm_similar_tests", "tsm_similar_tests_last_ms",
-           "tsm_similar_churn", "tsm_similar_churn_last_ms", "tsm_smells_lexical", "tsm_smells_lexical_last_ms"]
+           "tsm_similar_churn", "tsm_similar_churn_last_ms", "tsm_smells_lexical", "tsm_smells_lexical_last_ms",
+           "tsm_diff_pairs_smells_lexical", "tsm_diff_smells_lexical_last_ms"]
 FRAG_STATES = ["kept", "edited", "whole"]          # tsm_clone_churn state[j] (docs/SPEC.md section 22)
 CLONE_STATUSES = ["untouched", "changed", "removed", "diverged", "dropped", "created", "copied", "joined"]   # status[c]
 
@@ -104,6 +106,10 @@ class _DiffSmells(C.Structure):
     _fields_ = [("cases", _DiffCases),
                 ("old_tests", C.c_void_p), ("old_churn", C.c_void_p), ("old_test_cap", C.c_int64), ("n_old_tests", C.c_int64),
                 ("new_tests", C.c_void_p), ("new_churn", C.c_void_p), ("new_test_cap", C.c_int64), ("n_new_tests", C.c_int64)]
+
+
+class _DiffLexSmells(C.Structure):
+    _fields_ = [("old_lex", C.c_void_p), ("old_churn", C.c_void_p), ("new_lex", C.c_void_p), ("new_churn", C.c_void_p)]
 
 
 class _DiffMoves(C.Structure):
@@ -272,6 +278,11 @@ def lib():
             [C.POINTER(_DiffSmells), C.c_void_p]
         L.tsm_diff_smells_last_ms.restype = C.c_int
         L.tsm_diff_smells_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
+        L.tsm_diff_pairs_smells_lexical.restype = C.c_int
+        L.tsm_diff_pairs_smells_lexical.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 3 + \
+            [C.POINTER(_DiffSmells), C.POINTER(_DiffLexSmells), C.c_void_p]
+        L.tsm_diff_smells_lexical_last_ms.restype = C.c_int
+        L.tsm_diff_smells_lexical_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
         L.tsm_diff_pairs_moves.restype = C.c_int
         L.tsm_diff_pairs_moves.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus)] + [C.c_void_p] * 3 + \
             [C.POINTER(_DiffMoves), C.c_void_p]
@@ -1001,6 +1012,44 @@ class Scanner:
                     "new_churn": nch[:r.n_new_tests]}
         raise TsmError(TSM_E_CAPACITY, "tsm_diff_pairs_smells")
 
+    def diff_smells_lexical(self, olds, news, stream=None, cap=None):
+        """Lexical test-smell churn (docs/SPEC.md section 26): the dict of diff_smells(), exactly as it returns it, plus old_lex and
+        new_lex (LEX_TEST records of each side, in the order of its tests) and old_lex_churn and new_lex_churn (one LEX_CHURN
+        record per test: per lexical smell its instances and those that the revision removes (old side) or adds (new side)).
+        Arrays too small are sized from the counts and the call is made again (cap: the first guess of each)."""
+        n = olds.n_files
+        added, removed, det = np.zeros(n, np.int64), np.zeros(n, np.int64), np.zeros(max(n, 1), DIFF_DETAIL)
+        a, b = olds.c_struct(), news.c_struct()
+        co = cn = to = tn = int(cap if cap is not None else 0)
+        for _ in range(2):
+            oc, nc = np.zeros(max(co, 1), CASE), np.zeros(max(cn, 1), CASE)
+            ot, nt = np.zeros(max(to, 1), SMELL_TEST), np.zeros(max(tn, 1), SMELL_TEST)
+            och, nch = np.zeros(max(to, 1), TEST_CHURN), np.zeros(max(tn, 1), TEST_CHURN)
+            ol, nl = np.zeros(max(to, 1), LEX_TEST), np.zeros(max(tn, 1), LEX_TEST)
+            olc, nlc = np.zeros(max(to, 1), LEX_CHURN), np.zeros(max(tn, 1), LEX_CHURN)
+            r = _DiffSmells(_DiffCases(_p(oc), co, 0, _p(nc), cn, 0), _p(ot), _p(och), to, 0, _p(nt), _p(nch), tn, 0)
+            x = _DiffLexSmells(_p(ol), _p(olc), _p(nl), _p(nlc))
+            rc = lib().tsm_diff_pairs_smells_lexical(self._ctx, C.byref(a), C.byref(b), _p(added), _p(removed), _p(det), C.byref(r),
+                                                     C.byref(x), stream)
+            k = r.cases
+            if rc == TSM_E_CAPACITY and (k.n_old > co or k.n_new > cn or r.n_old_tests > to or r.n_new_tests > tn):
+                co, cn, to, tn = int(k.n_old), int(k.n_new), int(r.n_old_tests), int(r.n_new_tests)
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_diff_pairs_smells_lexical")
+            return {"added": added, "removed": removed, "detail": det[:n], "old_cases": oc[:k.n_old], "new_cases": nc[:k.n_new],
+                    "old_tests": ot[:r.n_old_tests], "new_tests": nt[:r.n_new_tests], "old_churn": och[:r.n_old_tests],
+                    "new_churn": nch[:r.n_new_tests], "old_lex": ol[:r.n_old_tests], "new_lex": nl[:r.n_new_tests],
+                    "old_lex_churn": olc[:r.n_old_tests], "new_lex_churn": nlc[:r.n_new_tests]}
+        raise TsmError(TSM_E_CAPACITY, "tsm_diff_pairs_smells_lexical")
+
+    def diff_smells_lexical_last_ms(self):
+        """Device time of the last diff_smells_lexical call: [k_scan over both sides, smell and lexical stages, the diff, case
+        records + k_smell_churn] in ms."""
+        ms = (C.c_float * 4)()
+        lib().tsm_diff_smells_lexical_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
+
     def diff_smells_last_ms(self):
         """Device time of the last diff_smells call: [k_scan over both sides, smell stages, the diff, case records +
         k_smell_churn] in ms."""
@@ -1134,8 +1183,8 @@ class Scanner:
         return [float(x) for x in ms]
 
     def smells_lexical_last_ms(self):
-        """Device time of the last smells_lexical call: [k_scan, the front (kinds, case spans, smell stage, lexer states),
-        k_lex_body + k_lex_lines, k_lex_tests] in ms."""
+        """Device time of the last smells_lexical call: [k_scan, the front (kinds, case spans, smell stage), lexer
+        states + k_lex_body + k_lex_lines, k_lex_tests] in ms."""
         ms = (C.c_float * 4)()
         lib().tsm_smells_lexical_last_ms(self._ctx, C.byref(ms))
         return [float(x) for x in ms]
