@@ -9,9 +9,12 @@ import pytest
 
 import blind_ref as br
 import corpus_util as cu
+import front_seams as fs
+import lex_seams as lx
 import lexsmell_ref as lr
 import orc_lexsmells as ol
 import smell_ref as sr
+import spec_ref
 import tosemscan as ts
 from spec_ref import py_lines
 
@@ -169,3 +172,61 @@ def test_c_reference_equals_python(name):
     for n, files, exts in corpora():
         if n == name:
             ol.assert_equal(ol.lexsmells(ts.pack(files, exts)), lr.py_lexsmells(files, exts))
+
+
+# ------------------------------------------------------------------------------------------------------ the seams corpora
+def test_kernel_names_equal_reference_tables():
+    """Every name the kernels compare an identifier with is one of the reference's, and the other way round."""
+    assert lx.kernel_names() == lx.reference_names()
+    assert b"assert_not_called" in lx.kernel_names() and b"assert_not_callee" in lx.long_name_misses()
+
+
+def test_sentinel_name_hashes_to_the_empty_slot():
+    assert spec_ref.py_bytes_hash(lx.SENTINEL) == (1 << 64) - 1
+    assert lr.lex_tokens(b"    " + lx.SENTINEL + b" = 1", br.PY, br.CODE)[0][0] == (lr.IDENT, lx.SENTINEL)
+
+
+SEAMS = {"names": lx.name_corpus, "cap": lx.cap_corpus, "automata": lambda: lx.automaton_corpus((1, 2, 3)),
+         "name_sets": lx.nameset_corpus, "body": lx.body_corpus}
+
+
+def test_seams_corpora_reach_their_seams():
+    c = {k: b() for k, b in SEAMS.items()}
+    _, _, reach = c["names"]
+    assert all(fs.on_the_grid(reach["grid"]).values()) and len(reach["grid"]) > 800
+    assert {w for _, _, _, w in reach["marks"]} >= lx.kernel_names() | lx.long_name_misses()
+    _, _, reach = c["cap"]
+    assert {(d, end, seen) for _, _, d, end, seen, _ in reach["cases"]} == \
+        {(62, None, True), (63, None, True), (64, None, False), (65, None, False), (62, 63, True), (63, 64, True),
+         (64, 65, False), (63, 63, False), (64, 64, False), (65, 65, False)}
+    _, _, reach = c["automata"]
+    assert reach[("stmt", 1, b"assert ")] == 19 + 19 ** 2 + 19 ** 3 and reach[("code", 3)] == 15 + 15 ** 2 + 15 ** 3
+    _, _, reach = c["name_sets"]
+    assert reach["wraps"][4] > 0 and reach["wraps"][5] > 0 and reach["alternating_warps"] > 0
+    assert len(reach["names"]) > 2 * reach["warps"] and reach["sentinel_tests"] == [0, 1, 2, 3, 13]
+    assert [len(set(h)) for h in reach["names"][:14]] == [1, 1, 5, 300, 5, 300, 2, 1, 300, 10, 11, 0, 0, 2]
+    assert len(reach["names"][6]) == 33 and len(reach["names"][3]) > 256
+    assert {len(set(h)) for h in reach["names"][14:]} >= set(range(21)) | {257, 300}
+    _, _, reach = c["body"]
+    assert [x[1] for x in reach["head_end"]] == [(30, 0), (31, 0), (0, 1), (1, 1), (2, 1)]
+    assert sorted({(o, c) for o, c in reach["doc"]}) == [((31, 0), (16, r)) for r in (1, 2, 3)]
+    assert reach["end_lanes"] == {1: set(range(32)), 3: set(range(32))}
+
+
+@pytest.mark.parametrize("name", ["names", "cap", "automata", "name_sets", "body"])
+def test_seams_references_agree(name):
+    files, exts, reach = SEAMS[name]()
+    want = lr.py_lexsmells(files, exts)
+    ol.assert_equal(ol.lexsmells(ts.pack(files, np.asarray(exts, np.uint8))), want)
+    if name == "cap":
+        for (form, _, d, end, seen, _), r in zip(reach["cases"], want["lex"]):
+            if reach["forms"][form] == "msg":
+                assert r["n_unexplained"] == (0 if seen else 1), (form, d, end)
+            else:
+                assert r["n_magic"] == int(seen), (form, d, end)
+    if name == "names":
+        lsm = want["line_lsmell"]
+        hits = [want["line_base"][f] + ln for f, ln, _, w in reach["marks"] if w == b"assert_not_callee" and exts[f] == 1]
+        assert len(hits) == 128 and (lsm[hits] & AR).all()
+    if name == "name_sets":
+        assert want["lex"]["n_locals"].tolist() == [len(set(h)) for h in reach["names"]]

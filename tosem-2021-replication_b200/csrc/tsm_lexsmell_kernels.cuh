@@ -250,7 +250,7 @@ struct StmtSink {
     if (py) {
       if (lx_pre(n, lx_name("assert_")) && n.k > 7) {
         ck = (lx_pre(n, lx_name("assert_called")) || lx_pre(n, lx_name("assert_awaited")) || lx_is(n, lx_name("assert_any_call")) ||
-              lx_is(n, lx_name("assert_has_calls")) || lx_is(n, lx_name("assert_not_called"))) ? CK_NONE : CK_NUMPY;
+              lx_is(n, lx_name("assert_has_calls")) || lx_is_long(B, i0, n, "assert_not_called")) ? CK_NONE : CK_NUMPY;
       } else if (prev == '.' && lx_pre(n, lx_name("assert"))) {
         if (!(lx_pre(n, lx_name("assertRaises")) || lx_pre(n, lx_name("assertWarns")) || lx_is(n, lx_name("assertLogs")) ||
               lx_is(n, lx_name("assertNoLogs")))) {
