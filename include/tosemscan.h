@@ -415,6 +415,45 @@ int tsm_smells_lexical(tsm_ctx* ctx, const tsm_corpus* corpus, int64_t* line_bas
                        int64_t* n_tests, void* stream);
 int tsm_smells_lexical_last_ms(tsm_ctx* ctx, float* ms4);
 
+/* Test-to-code links (docs/SPEC.md section 27, `tosem-scan links`): the production functions and classes each test calls,
+ * resolved by name within its repository (grp).  role[f] != 0 marks a test file, whose section-18 tests are the tests here;
+ * every other file is a production file, whose lines are searched for definitions.  stem[f] (NULL: all -1) is the id of a
+ * production file's own focal stem, and of a test file's focal stem or -1, as tsm_focal_stems gives them.
+ *   tests  one tsm_link_test per test of a test file, in global line order (file, header line, its call tokens, those of them
+ *          that link, its links, the links of names with a function definition, those with a definition in a focal file, and
+ *          TSM_LINK_EAGER / TSM_LINK_LAZY)
+ *   links  one tsm_link per (test, name) link, ascending (test, first call): the name's first definition in line order
+ *          (name_def, for printing), the target definition or -1 (ambiguous), the name's definitions, the test's calls of it
+ *          and the 0-based line and file byte of the first of them
+ *   defs   one tsm_link_def per definition in global line order (file, 0-based line, the name's file byte and length, kind
+ *          TSM_LINK_FUNCTION / TSM_LINK_CLASS, the links that target it, the links of its name, the calls of the links that
+ *          target it)
+ * Any output pointer may be NULL (it is skipped); the three counts are always set.  A short cap for a given output returns
+ * TSM_E_CAPACITY with every count set: size the arrays and call again.  role NULL, or a stem below -1, is TSM_E_ARG; a grp at or
+ * above n_groups TSM_E_LAYOUT.  n_files = 0 is legal.  A failed device allocation is TSM_E_CUDA (as for tsm_smells); more than
+ * 2^28 definitions or calls is TSM_E_NOMEM.
+ * Kernels: k_scan with the header events, the case spans and smell stage of tsm_smells and the lexer states of
+ * tsm_clones_blind; k_link_pick + xscan + k_link_gather (the tests of the test files), k_lex_body over them, k_link_mark,
+ * k_link_lines (count and write passes around two xscans), k_link_defs and k_link_calls (two open-addressing tables),
+ * k_link_first + xscan, k_link_emit, xscan of the links per test, k_link_tests and k_link_out (csrc/tsm_link_kernels.cuh).
+ * tsm_test_links_last_ms: device time of the last call, ms4 = { k_scan, the front (kinds, case spans, smell stage, lexer states,
+ * the tests of the test files and their code lines), k_link_lines, the join to the records }. */
+enum { TSM_LINK_FUNCTION = 1, TSM_LINK_CLASS = 2 };
+enum { TSM_LINK_EAGER = 1, TSM_LINK_LAZY = 2 };
+typedef struct tsm_link_test {
+  int32_t file, line, calls, linked_calls, links, function_links, focal_links; uint32_t flags;
+} tsm_link_test;
+typedef struct tsm_link { int32_t test, name_def, target, n_defs, calls, line, byte; } tsm_link;
+typedef struct tsm_link_def { int32_t file, line, name_off, name_len, kind, tests, tests_by_name, calls; } tsm_link_def;
+typedef struct tsm_links_result {
+  tsm_link_test* tests; int64_t test_cap; int64_t n_tests;
+  tsm_link* links; int64_t link_cap; int64_t n_links;
+  tsm_link_def* defs; int64_t def_cap; int64_t n_defs;
+} tsm_links_result;
+int tsm_test_links(tsm_ctx* ctx, const tsm_corpus* corpus, const uint8_t* role, const int32_t* stem, tsm_links_result* out,
+                   void* stream);
+int tsm_test_links_last_ms(tsm_ctx* ctx, float* ms4);
+
 /* Similar tests (docs/SPEC.md section 23, `tosem-scan similar-tests`): the pairs of tests of section 18 whose sequences of kept
  * blind lines (section 21, header line included) are at least min_similarity % alike, and the classes they link.  A test is
  * compared when it has at least min_lines kept lines (min_lines >= 1, else TSM_E_ARG).  Tests a < b form a pair when both are
@@ -589,6 +628,11 @@ void* tsm_host_alloc(int64_t bytes);
 void tsm_host_free(void* p);
 /* Arena size (multiple of TSM_ALIGN) for files of the given sizes; fills off[n+1]. <0 on overflow. */
 int64_t tsm_layout(const int32_t* len, int32_t n_files, int32_t* off);
+/* The naming convention of docs/SPEC.md section 27.  role[i] != 0 marks a test file.  stem[i] = the id of path i's base name
+ * without its extension for a production file; for a test file, the id of its focal stem (the base name without extension with
+ * the first applying suffix `_test`, `_tests`, `_unittest`, `Test`, `Tests` stripped, else the first applying prefix `test_`,
+ * `test`), or -1 when that is empty.  Equal strings get equal ids, numbered from 0 in order of first appearance. */
+int tsm_focal_stems(const char* const* paths, const uint8_t* role, int32_t n, int32_t* stem);
 /* Deterministic synthetic corpus (SURVEY.md section 8d; std::mt19937_64, one engine per file).
  * size_law 0: every file exactly fixed_size bytes; 1: truncated power law pdf ~ x^-1.5 on
  * [128 B, 1 MiB] rounded up to whole lines.  Slot i holds logical file first_index + i*index_stride,

@@ -6,6 +6,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <chrono>
+#include <string>
 #include <unordered_map>
 #include <new>
 #include <utility>
@@ -27,6 +28,7 @@
 #include "tsm_edit_kernels.cuh"
 #include "tsm_smell_kernels.cuh"
 #include "tsm_lexsmell_kernels.cuh"
+#include "tsm_link_kernels.cuh"
 #include "tsm_move_kernels.cuh"
 #include "tsm_clone_churn_kernels.cuh"
 #include "../host/tsm_names.hpp"
@@ -101,6 +103,8 @@ enum Timed {
               // tsm_smells_lexical
   MS_LEXCHURN,// k_scan, smell and lexical stages, the diff, case records + k_smell_churn<true> of the last
               // tsm_diff_pairs_smells_lexical
+  MS_LINKS,   // k_scan, front (smell stage, lexer states, test code lines), k_link_lines, the join to the records of the last
+              // tsm_test_links
   N_TIMED
 };
 
@@ -201,6 +205,7 @@ constexpr EvSpan EV_CHURN_LEX = {6, 7};                                 // the n
 constexpr EvSpan EV_MOVE_FLAGS = {0, 1}, EV_MOVE_JOIN = {2, 3}, EV_MOVE_RUNS = {4, 5}, EV_MOVE_MARK = {6, 7};
 constexpr EvSpan EV_BLAME = {0, 1};
 constexpr EvSpan EV_CCHURN = {0, 1};
+constexpr int EV_LK_FRONT = 2, EV_LK_LINES = 6, EV_LK_JOIN = 7, EV_LK_END = 5;
 constexpr int EV_LX_FRONT = 2, EV_LX_LINES = 6, EV_LX_TESTS = 7, EV_LX_END = 5;
 constexpr int EV_ST_FRONT = 2, EV_ST_ENUM = 3, EV_ST_VERIFY = 4, EV_ST_END = 5, EV_ST_LEXED = 6, EV_ST_LISTS = 7;
 
@@ -2560,6 +2565,195 @@ extern "C" int tsm_smells_lexical(tsm_ctx* c, const tsm_corpus* k, int64_t* line
 }
 
 extern "C" int tsm_smells_lexical_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_LEXSMELL, ms4, 4); }
+
+// ------------------------------------------------------------------------------------- SPEC section 27 test-to-code links
+// The line records with header events (line_records), the case spans and smell stage of tsm_smells and the line start states of
+// the section-21 lexer; the tests of the test files (k_link_pick, xscan, k_link_gather), their code lines (k_lex_body,
+// k_link_mark); one synchronisation for the test count, one for the definition and call totals, one for the link count; the
+// outputs are copied when they fit.
+constexpr unsigned long long kLinkMaxEntries = 1ull << 28;   // definitions or calls: 2^30 slots of the link table at most
+static uint32_t link_slots(unsigned long long keys) {     // a power of two at least twice keys (and 1 024); keys <= 2^29
+  unsigned long long s = 1024;
+  while (s < 2 * keys) s <<= 1;
+  return (uint32_t)s;
+}
+
+extern "C" int tsm_test_links(tsm_ctx* c, const tsm_corpus* k, const uint8_t* role, const int32_t* stem, tsm_links_result* out,
+                              void* stream) {
+  if (!c || !k || !role || !out || k->n_files < 0 || out->test_cap < 0 || out->link_cap < 0 || out->def_cap < 0) return TSM_E_ARG;
+  const int32_t nf = k->n_files;
+  for (int32_t f = 0; stem && f < nf; ++f)
+    if (stem[f] < -1) return TSM_E_ARG;
+  if (check_groups(k, 0, nf) != TSM_OK) return TSM_E_LAYOUT;
+  float* const ms = clear_ms(c, MS_LINKS);
+  c->launches = 0;
+  out->n_tests = out->n_links = out->n_defs = 0;
+  std::vector<int64_t> base((size_t)nf + 1);
+  int64_t n_lines = 0;
+  return line_records(c, k, true, base.data(), INT64_MAX, &n_lines, stream, [&](const HostSide& S, unsigned long long total, cudaStream_t st) -> int {
+    const size_t L = (size_t)total;
+    const uint32_t nfu = (uint32_t)S.n;
+    CaseSpans sp;
+    SmellBufs m;
+    DevBuf d_bsum, d_state, d_role, d_stem, d_grp, d_tflag, d_tpos, d_tests, d_lxflag, d_lxend, d_ltest, d_dcnt, d_ccnt, d_dbase, d_cbase;
+    if (!d_bsum.alloc(8 * (L / XS_TILE + 4)) || !d_state.alloc(L) || !d_role.alloc((size_t)nf) || !d_stem.alloc(4 * (size_t)nf) ||
+        !d_grp.alloc(2 * (size_t)nf) || !d_lxflag.alloc(L) || !d_lxend.alloc(4 * L) || !d_ltest.alloc(4 * L) || !d_dcnt.alloc(4 * L) ||
+        !d_ccnt.alloc(4 * L) || !d_dbase.alloc(8 * (L + 1)) || !d_cbase.alloc(8 * (L + 1)))
+      return TSM_E_CUDA;
+    CU(cudaMemcpyAsync(d_role.p, role, (size_t)nf, cudaMemcpyHostToDevice, st));
+    if (stem) CU(cudaMemcpyAsync(d_stem.p, stem, 4 * (size_t)nf, cudaMemcpyHostToDevice, st));
+    else CU(cudaMemsetAsync(d_stem.p, 0xFF, 4 * (size_t)nf, st));
+    if (k->grp) CU(cudaMemcpyAsync(d_grp.p, k->grp, 2 * (size_t)nf, cudaMemcpyHostToDevice, st));
+    else CU(cudaMemsetAsync(d_grp.p, 0, 2 * (size_t)nf, st));
+    int launches = 0;
+    CU(cudaEventRecord(c->diff_ev[EV_LK_FRONT], st));
+    int rc = case_spans(S, sp, d_bsum, launches, st);
+    if (rc == TSM_OK) rc = smell_stage(c, S, sp, d_bsum, m, launches, st);
+    if (rc != TSM_OK) return rc;
+    const unsigned grid = (unsigned)((L + 255) / 256);
+    k_blind_state<<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>());
+    k_blind_scan<<<(unsigned)(((size_t)nfu * 32 + 255) / 256), 256, 0, st>>>(S.d.line_base, nfu, d_state.as<uint8_t>());
+    launches += 2;
+    unsigned long long* pin = c->h_rb->u64;
+    CU(cudaMemcpyAsync(pin, m.tidx.as<unsigned long long>() + sp.n_cases, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const uint32_t na = (uint32_t)*pin;                    // the tests of every file
+    if (!d_tflag.alloc(4 * ((size_t)na + 1)) || !d_tpos.alloc(8 * ((size_t)na + 1)) || !d_tests.alloc(sizeof(tsm_smell_test) * ((size_t)na + 1)))
+      return TSM_E_CUDA;
+    const unsigned agrid = (unsigned)((na + 255) / 256);
+    if (na) k_link_pick<<<agrid, 256, 0, st>>>(m.tests.as<tsm_smell_test>(), na, d_role.as<uint8_t>(), d_tflag.as<uint32_t>());
+    xscan(d_tflag.as<uint32_t>(), na, d_bsum.as<unsigned long long>(), d_tpos.as<unsigned long long>(), st);
+    if (na) k_link_gather<<<agrid, 256, 0, st>>>(m.tests.as<tsm_smell_test>(), na, d_tflag.as<uint32_t>(), d_tpos.as<unsigned long long>(),
+                                                 d_tests.as<tsm_smell_test>());
+    CU(cudaMemcpyAsync(pin, d_tpos.as<unsigned long long>() + na, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemsetAsync(d_lxflag.p, 0, L, st));
+    CU(cudaMemsetAsync(d_ltest.p, 0xFF, 4 * L, st));
+    CU(cudaStreamSynchronize(st));
+    const uint32_t nt = (uint32_t)*pin;                    // the tests of the test files
+    launches += na ? 5 : 3;
+    const tsm_smell_test* dt = d_tests.as<tsm_smell_test>();
+    const unsigned tgrid = std::min((unsigned)((nt + 7) / 8), (unsigned)c->sms * 8);
+    if (nt) {
+      k_lex_body<<<tgrid, 256, 0, st>>>(LexBody{dt, nt, S.d.line_base, S.d.ext, m.kind.as<uint8_t>(), m.lines.as<SmellLine>(),
+                                                d_lxflag.as<uint8_t>(), d_lxend.as<uint32_t>()});
+      k_link_mark<<<tgrid, 256, 0, st>>>(dt, nt, S.d.line_base, d_lxflag.as<uint8_t>(), d_ltest.as<uint32_t>());
+      launches += 2;
+    }
+    CU(cudaEventRecord(c->diff_ev[EV_LK_LINES], st));
+    k_link_lines<false><<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>(), d_role.as<uint8_t>(), d_ltest.as<uint32_t>(),
+                                              d_dcnt.as<uint32_t>(), d_ccnt.as<uint32_t>(), nullptr, nullptr, nullptr, nullptr);
+    xscan(d_dcnt.as<uint32_t>(), (uint32_t)total, d_bsum.as<unsigned long long>(), d_dbase.as<unsigned long long>(), st);
+    xscan(d_ccnt.as<uint32_t>(), (uint32_t)total, d_bsum.as<unsigned long long>(), d_cbase.as<unsigned long long>(), st);
+    CU(cudaMemcpyAsync(pin, d_dbase.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(pin + 1, d_cbase.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const unsigned long long nd64 = pin[0], nc64 = pin[1];
+    if (nd64 > kLinkMaxEntries || nc64 > kLinkMaxEntries) return TSM_E_NOMEM;   // (tables of more than 16 GiB)
+    const uint32_t nd = (uint32_t)nd64, nc = (uint32_t)nc64;
+    const uint32_t ns = link_slots(2ull * nd), nl = link_slots(2ull * nc);
+    DevBuf d_defs, d_calls, d_name, d_ndefs, d_kmask, d_first, d_ntests, d_link, d_lcalls, d_lfirst, d_dslot, d_cslot, d_cflag, d_cpos,
+        d_tlinks, d_lbase, d_dtests, d_dcalls, d_jbsum;
+    if (!d_jbsum.alloc(8 * ((size_t)std::max(nc, nt) / XS_TILE + 4)) || !d_defs.alloc(sizeof(LinkDef) * ((size_t)nd + 1)) || !d_calls.alloc(sizeof(LinkCall) * ((size_t)nc + 1)) ||
+        !d_name.alloc(16 * (size_t)ns) || !d_ndefs.alloc(4 * (size_t)ns) || !d_kmask.alloc(4 * (size_t)ns) || !d_first.alloc(4 * (size_t)ns) ||
+        !d_ntests.alloc(4 * (size_t)ns) || !d_link.alloc(16 * (size_t)nl) || !d_lcalls.alloc(4 * (size_t)nl) ||
+        !d_lfirst.alloc(4 * (size_t)nl) || !d_dslot.alloc(4 * ((size_t)nd + 1)) || !d_cslot.alloc(4 * ((size_t)nc + 1)) ||
+        !d_cflag.alloc(4 * ((size_t)nc + 1)) || !d_cpos.alloc(8 * ((size_t)nc + 1)) || !d_tlinks.alloc(4 * ((size_t)nt + 1)) ||
+        !d_lbase.alloc(8 * ((size_t)nt + 1)) || !d_dtests.alloc(4 * ((size_t)nd + 1)) || !d_dcalls.alloc(4 * ((size_t)nd + 1)))
+      return TSM_E_CUDA;
+    k_link_lines<true><<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>(), d_role.as<uint8_t>(), d_ltest.as<uint32_t>(),
+                                             d_dcnt.as<uint32_t>(), d_ccnt.as<uint32_t>(), d_dbase.as<unsigned long long>(),
+                                             d_cbase.as<unsigned long long>(), d_defs.as<LinkDef>(), d_calls.as<LinkCall>());
+    launches += 8;                                         // lines (count), two xscans (3 each), lines (write)
+    CU(cudaEventRecord(c->diff_ev[EV_LK_JOIN], st));
+    CU(cudaMemsetAsync(d_name.p, 0, 16 * (size_t)ns, st));
+    CU(cudaMemsetAsync(d_ndefs.p, 0, 4 * (size_t)ns, st));
+    CU(cudaMemsetAsync(d_kmask.p, 0, 4 * (size_t)ns, st));
+    CU(cudaMemsetAsync(d_first.p, 0xFF, 4 * (size_t)ns, st));
+    CU(cudaMemsetAsync(d_ntests.p, 0, 4 * (size_t)ns, st));
+    CU(cudaMemsetAsync(d_link.p, 0, 16 * (size_t)nl, st));
+    CU(cudaMemsetAsync(d_lcalls.p, 0, 4 * (size_t)nl, st));
+    CU(cudaMemsetAsync(d_lfirst.p, 0xFF, 4 * (size_t)nl, st));
+    CU(cudaMemsetAsync(d_tlinks.p, 0, 4 * ((size_t)nt + 1), st));
+    CU(cudaMemsetAsync(d_dtests.p, 0, 4 * ((size_t)nd + 1), st));
+    CU(cudaMemsetAsync(d_dcalls.p, 0, 4 * ((size_t)nd + 1), st));
+    const LinkTables T{d_name.as<LinkKey>(), ns - 1, d_ndefs.as<uint32_t>(), d_kmask.as<uint32_t>(), d_first.as<uint32_t>(),
+                       d_ntests.as<uint32_t>(), d_link.as<LinkKey>(), nl - 1, d_lcalls.as<uint32_t>(), d_lfirst.as<uint32_t>()};
+    const unsigned dgrid = (unsigned)((nd + 255) / 256), cgrid = (unsigned)((nc + 255) / 256);
+    if (nd) k_link_defs<<<dgrid, 256, 0, st>>>(d_defs.as<LinkDef>(), nd, d_grp.as<uint16_t>(), d_stem.as<int32_t>(), T, d_dslot.as<uint32_t>());
+    if (nc) {
+      k_link_calls<<<cgrid, 256, 0, st>>>(d_calls.as<LinkCall>(), nc, d_ltest.as<uint32_t>(), dt, d_grp.as<uint16_t>(), T,
+                                          d_cslot.as<uint32_t>(), d_tlinks.as<uint32_t>());
+      k_link_first<<<cgrid, 256, 0, st>>>(d_cslot.as<uint32_t>(), nc, T, d_cflag.as<uint32_t>());
+    }
+    xscan(d_cflag.as<uint32_t>(), nc, d_jbsum.as<unsigned long long>(), d_cpos.as<unsigned long long>(), st);   // (nc may exceed the
+    xscan(d_tlinks.as<uint32_t>(), nt, d_jbsum.as<unsigned long long>(), d_lbase.as<unsigned long long>(), st); //  lines: own sums)
+    CU(cudaMemcpyAsync(pin, d_cpos.as<unsigned long long>() + nc, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const unsigned long long nk = *pin;                    // the links
+    DevBuf d_links, d_lbits, d_out_tests, d_out_defs;
+    if (!d_links.alloc(sizeof(tsm_link) * ((size_t)nk + 1)) || !d_lbits.alloc((size_t)nk + 1) ||
+        !d_out_tests.alloc(sizeof(tsm_link_test) * ((size_t)nt + 1)) || !d_out_defs.alloc(sizeof(tsm_link_def) * ((size_t)nd + 1)))
+      return TSM_E_CUDA;
+    if (nc)
+      k_link_emit<<<cgrid, 256, 0, st>>>(LinkEmit{d_calls.as<LinkCall>(), nc, d_cslot.as<uint32_t>(), d_cflag.as<uint32_t>(),
+                                                  d_cpos.as<unsigned long long>(), d_ltest.as<uint32_t>(), dt, d_grp.as<uint16_t>(),
+                                                  d_stem.as<int32_t>(), S.d.line_base, d_defs.as<LinkDef>(), T, d_links.as<tsm_link>(),
+                                                  d_lbits.as<uint8_t>(), d_dtests.as<uint32_t>(), d_dcalls.as<uint32_t>()});
+    if (nt)
+      k_link_tests<<<tgrid, 256, 0, st>>>(LinkTests{dt, nt, S.d.line_base, d_cbase.as<unsigned long long>(), d_lbase.as<unsigned long long>(),
+                                                    d_links.as<tsm_link>(), d_lbits.as<uint8_t>(), d_out_tests.as<tsm_link_test>()});
+    if (nd) k_link_out<<<dgrid, 256, 0, st>>>(d_defs.as<LinkDef>(), nd, d_dslot.as<uint32_t>(), S.d.line_base, T, d_dtests.as<uint32_t>(),
+                                              d_dcalls.as<uint32_t>(), d_out_defs.as<tsm_link_def>());
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_LK_END], st));
+    CU(cudaStreamSynchronize(st));
+    launches += (nd ? 2 : 0) + (nc ? 3 : 0) + 6 + (nt ? 1 : 0);   // defs + out, calls + first + emit, two xscans, tests
+    c->launches += launches;
+    out->n_tests = nt; out->n_links = (int64_t)nk; out->n_defs = nd;
+    ms[1] = elapsed_ms(c->diff_ev[EV_LK_FRONT], c->diff_ev[EV_LK_LINES]);
+    ms[2] = elapsed_ms(c->diff_ev[EV_LK_LINES], c->diff_ev[EV_LK_JOIN]);
+    ms[3] = elapsed_ms(c->diff_ev[EV_LK_JOIN], c->diff_ev[EV_LK_END]);
+    if ((out->tests && out->test_cap < (int64_t)nt) || (out->links && out->link_cap < (int64_t)nk) || (out->defs && out->def_cap < (int64_t)nd))
+      return TSM_E_CAPACITY;
+    if (out->tests && nt) CU(cudaMemcpyAsync(out->tests, d_out_tests.p, sizeof(tsm_link_test) * nt, cudaMemcpyDeviceToHost, st));
+    if (out->links && nk) CU(cudaMemcpyAsync(out->links, d_links.p, sizeof(tsm_link) * nk, cudaMemcpyDeviceToHost, st));
+    if (out->defs && nd) CU(cudaMemcpyAsync(out->defs, d_out_defs.p, sizeof(tsm_link_def) * nd, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    return TSM_OK;
+  }, &ms[0], TSM_SCAN_HEADER_EVENTS);
+}
+
+extern "C" int tsm_test_links_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_LINKS, ms4, 4); }
+
+// The naming convention of section 27: the one place it lives (the CLI and the Python package call it).
+extern "C" int tsm_focal_stems(const char* const* paths, const uint8_t* role, int32_t n, int32_t* stem) {
+  if (n < 0 || (n && (!paths || !role || !stem))) return TSM_E_ARG;
+  std::unordered_map<std::string, int32_t> ids;
+  for (int32_t i = 0; i < n; ++i) {
+    if (!paths[i]) return TSM_E_ARG;
+    std::string b = paths[i];
+    const size_t sl = b.find_last_of('/');
+    if (sl != std::string::npos) b = b.substr(sl + 1);
+    const size_t dot = b.find_last_of('.');
+    if (dot != std::string::npos && dot > 0) b.resize(dot);
+    if (role[i]) {
+      static const char* const suffixes[] = {"_test", "_tests", "_unittest", "Test", "Tests"};
+      static const char* const prefixes[] = {"test_", "test"};
+      bool cut = false;
+      for (const char* x : suffixes) {
+        const size_t m = strlen(x);
+        if (b.size() >= m && b.compare(b.size() - m, m, x) == 0) { b.resize(b.size() - m); cut = true; break; }
+      }
+      for (size_t p = 0; !cut && p < 2; ++p) {
+        const size_t m = strlen(prefixes[p]);
+        if (b.compare(0, m, prefixes[p]) == 0) { b = b.substr(m); cut = true; }
+      }
+      if (b.empty()) { stem[i] = -1; continue; }
+    }
+    stem[i] = ids.emplace(b, (int32_t)ids.size()).first->second;
+  }
+  return TSM_OK;
+}
 
 // ------------------------------------------------------------------------------------- SPEC section 23 similar tests
 // One revision's section-23 state on the device, resident while the call needs it: the front (case spans, smell stage and

@@ -2696,6 +2696,125 @@ static int cmd_similar_tests(const std::vector<std::string>& roots, const std::s
   return 0;
 }
 
+// Test-to-code links (docs/SPEC.md section 27): ONE tsm_test_links call over every file with a lexer family under the roots (names
+// resolve across files).  A file is a test file when its path contains `test` (S0); the stems of the naming convention come from
+// tsm_focal_stems.  stdout: per root its test and production files, tests, tests with a link, definitions, definitions whose name
+// some test links, links, ambiguous links, Eager and Lazy tests, and an <all> row; --out: one row per link in (test, first call)
+// order; --defs: one row per definition in line order.  Lines are 1-based; a test is named by its section-10 case name.
+static int cmd_links(const std::vector<std::string>& roots, const std::string& git_repo, const std::string& rev,
+                     const std::string& out_path, const std::string& defs_path) {
+  std::vector<FileEntry> all, files;
+  std::vector<std::string> names;
+  if (!git_repo.empty()) {
+    gitstore::Store gs;
+    std::string err;
+    if (!gs.open(git_repo, err)) die(err);
+    gitstore::Oid id; gitstore::Commit cm;
+    if (!gs.resolve(rev, id) || !gs.commit(id, cm)) die("cannot resolve revision " + rev);
+    walk_git(gs, cm.tree, "", true, all);
+    names.push_back(repo_name(git_repo));
+  } else {
+    for (size_t g = 0; g < roots.size(); ++g) { walk(roots[g], (int)g, true, all); names.push_back(repo_name(roots[g])); }
+  }
+  for (FileEntry& f : all)
+    if (f.ext != TSM_EXT_OTHER) files.push_back(std::move(f));
+  fprintf(stderr, "tosem-scan: %zu files selected under %zu root(s)\n", files.size(), names.size());
+  std::vector<Batch> batches = plan_batches(files, all_of(files), (1ll << 31) - 4097, INT32_MAX);
+  int64_t need = 4096;
+  for (const Batch& b : batches) need += b.bytes;
+  if (batches.size() > 1 || need >= (1ll << 31))
+    die("the selected files (" + std::to_string(need) + " bytes of arena) do not fit one int32-indexed arena; links are resolved "
+        "across all files at once, so select fewer files");
+  const size_t ng = names.size();
+  std::vector<std::vector<int64_t>> tot(ng + 1, std::vector<int64_t>(10, 0));
+  std::ofstream os, ds;
+  if (!out_path.empty()) {
+    os.open(out_path, std::ios::binary);
+    csv_row(os, {"repository", "fileName", "test", "line", "callee", "kind", "calls", "definitions", "defFile", "defLine", "focal"});
+  }
+  if (!defs_path.empty()) {
+    ds.open(defs_path, std::ios::binary);
+    csv_row(ds, {"repository", "fileName", "line", "name", "kind", "tests", "tests_by_name", "calls"});
+  }
+  static const char* const kinds[] = {"", "function", "class"};
+  scan_batches(files, batches, 0, (int32_t)ng, 0, [&](const Batch& B, const Scanned& s) {
+    const int32_t nf = (int32_t)B.count();
+    const tsm_corpus c = B.corpus((int32_t)ng);
+    std::vector<const char*> paths((size_t)nf);
+    std::vector<uint8_t> role((size_t)nf);
+    std::vector<int32_t> stem((size_t)std::max(nf, 1));
+    for (int32_t i = 0; i < nf; ++i) {
+      const FileEntry& fe = files[B.idx[(size_t)i]];
+      paths[(size_t)i] = fe.rel.c_str();
+      role[(size_t)i] = lower(fe.rel).find("test") != std::string::npos;   // S0
+    }
+    ck(tsm_focal_stems(paths.data(), role.data(), nf, stem.data()), "tsm_focal_stems");
+    tsm_links_result r{};
+    ck(tsm_test_links(s.ctx, &c, role.data(), stem.data(), &r, nullptr), "tsm_test_links");   // the counts
+    std::vector<tsm_link_test> tests((size_t)std::max<int64_t>(r.n_tests, 1));
+    std::vector<tsm_link> links((size_t)std::max<int64_t>(r.n_links, 1));
+    std::vector<tsm_link_def> defs((size_t)std::max<int64_t>(r.n_defs, 1));
+    r.tests = tests.data(); r.test_cap = r.n_tests; r.links = links.data(); r.link_cap = r.n_links; r.defs = defs.data(); r.def_cap = r.n_defs;
+    ck(tsm_test_links(s.ctx, &c, role.data(), stem.data(), &r, nullptr), "tsm_test_links");
+    auto grp_of = [&](int32_t f) { return (size_t)files[B.idx[(size_t)f]].grp; };
+    auto add = [&](size_t g, int k, int64_t v) { tot[g][(size_t)k] += v; tot[ng][(size_t)k] += v; };
+    for (int32_t i = 0; i < nf; ++i) add(grp_of(i), role[(size_t)i] ? 0 : 1, 1);
+    for (int64_t t = 0; t < r.n_tests; ++t) {
+      const tsm_link_test& x = tests[(size_t)t];
+      const size_t g = grp_of(x.file);
+      add(g, 2, 1); add(g, 3, x.links > 0); add(g, 8, (x.flags & TSM_LINK_EAGER) != 0); add(g, 9, (x.flags & TSM_LINK_LAZY) != 0);
+    }
+    for (int64_t d = 0; d < r.n_defs; ++d) { add(grp_of(defs[(size_t)d].file), 4, 1); add(grp_of(defs[(size_t)d].file), 5, defs[(size_t)d].tests_by_name > 0); }
+    for (int64_t k = 0; k < r.n_links; ++k) {
+      const size_t g = grp_of(tests[(size_t)links[(size_t)k].test].file);
+      add(g, 6, 1); add(g, 7, links[(size_t)k].target < 0);
+    }
+    auto name_of = [&](const tsm_link_def& d) { return std::string((const char*)B.arena.get() + B.off[(size_t)d.file] + d.name_off, (size_t)d.name_len); };
+    if (os.is_open()) {
+      int32_t at_test = -1;
+      std::string tname;
+      for (int64_t k = 0; k < r.n_links; ++k) {
+        const tsm_link& l = links[(size_t)k];
+        const tsm_link_test& x = tests[(size_t)l.test];
+        const FileEntry& fe = files[B.idx[(size_t)x.file]];
+        if (at_test != l.test) {                           // the test's case name, from its header line
+          at_test = l.test;
+          const uint8_t* p = B.arena.get() + B.off[(size_t)x.file];
+          const uint32_t len = (uint32_t)B.len[(size_t)x.file];
+          uint32_t b = 0;
+          for (int32_t n = 0; n < x.line; ++b) if (p[b] == '\n') ++n;
+          uint32_t e = b;
+          while (e < len && p[e] != '\n') ++e;
+          tname = case_name(fe.ext, p + b, e - b);
+        }
+        const tsm_link_def& nd = defs[(size_t)l.name_def];
+        const tsm_link_def* td = l.target >= 0 ? &defs[(size_t)l.target] : nullptr;
+        const bool focal = td && stem[(size_t)x.file] >= 0 && stem[(size_t)td->file] == stem[(size_t)x.file];
+        csv_row(os, {names[(size_t)fe.grp], fe.rel, tname, std::to_string(l.line + 1), name_of(nd), kinds[(td ? td : &nd)->kind],
+                     std::to_string(l.calls), std::to_string(l.n_defs), td ? files[B.idx[(size_t)td->file]].rel : std::string(),
+                     td ? std::to_string(td->line + 1) : std::string(), focal ? "1" : "0"});
+      }
+    }
+    if (ds.is_open())
+      for (int64_t k = 0; k < r.n_defs; ++k) {
+        const tsm_link_def& d = defs[(size_t)k];
+        const FileEntry& fe = files[B.idx[(size_t)d.file]];
+        csv_row(ds, {names[(size_t)fe.grp], fe.rel, std::to_string(d.line + 1), name_of(d), kinds[d.kind], std::to_string(d.tests),
+                     std::to_string(d.tests_by_name), std::to_string(d.calls)});
+      }
+  });
+  std::ostringstream so;
+  csv_row(so, {"repository", "test_files", "production_files", "tests", "linked_tests", "definitions", "linked_definitions", "links",
+               "ambiguous_links", "eager", "lazy"});
+  for (size_t g = 0; g <= ng; ++g) {
+    std::vector<std::string> row = {g < ng ? names[g] : "<all>"};
+    for (int64_t v : tot[g]) row.push_back(std::to_string(v));
+    csv_row(so, row);
+  }
+  fputs(so.str().c_str(), stdout);
+  return 0;
+}
+
 static void usage() {
   fprintf(stderr,
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
@@ -2715,12 +2834,16 @@ static void usage() {
           "       tosem-scan smells --git <repository> [--rev R] [--lexical] [--all-files] [--batch-bytes N] [--out F]\n"
           "       tosem-scan similar-tests <project-root>... | --git <repository> [--rev R] [--min-lines N] [--similarity P] [--all-files]\n"
           "                                [--out F] [--classes F]\n"
+          "       tosem-scan links <project-root>... | --git <repository> [--rev R] [--out F] [--defs F]\n"
           "smells: per root the tests with each of nine test smells; --out F: one row per instance line (docs/SPEC.md section 18).\n"
           "--lexical (smells): five more smells from the assertion calls' arguments, lexed with string awareness: assertion_roulette,\n"
           "  magic_number, suboptimal_assert, mystery_guest, obscure_setup (docs/SPEC.md section 25).\n"
           "similar-tests: pairs of tests whose kept blind lines are at least P %% alike (LCS, default 70) and their classes, over\n"
           "               tests of at least N kept lines (default 5); --out F: one row per pair; --classes F: one row per class member\n"
           "               (docs/SPEC.md section 23).\n"
+          "links: per root the tests, the production definitions and the links between them, by called name and the naming\n"
+          "       convention's focal files, with Eager and Lazy tests; --out F: one row per link; --defs F: one row per definition\n"
+          "       (docs/SPEC.md section 27).\n"
           "--blind (clones): near-miss copies - lines compared with identifiers, literals, whitespace and comments blinded, over the\n"
           "                  lines that keep a token (docs/SPEC.md section 21).\n"
           "--find-renames N (0..100): pair deleted and added files at least N %% similar, as git -M<N>%% does (docs/SPEC.md section 13).\n"
@@ -2783,6 +2906,10 @@ int main(int argc, char** argv) {
     if (p < 1 || p > 100) die("--similarity needs a percentage from 1 to 100");
     return cmd_similar_tests(pos, opt["--git"], opt.count("--rev") ? opt["--rev"] : "HEAD", (int)n, (int)p, all_files, opt["--out"],
                              opt["--classes"]);
+  }
+  if (cmd == "links") {
+    if (pos.empty() == !opt.count("--git")) die("links needs project roots or --git <repository>, not both");
+    return cmd_links(pos, opt["--git"], opt.count("--rev") ? opt["--rev"] : "HEAD", opt["--out"], opt["--defs"]);
   }
   if (cmd == "body") { if (pos.empty()) die("body needs at least one project root"); return cmd_body(pos, opt["--out"], batch_bytes(kBatch, 1)); }
   int rename_pct = -1;                                     // --find-renames N (docs/SPEC.md section 13); -1 = off

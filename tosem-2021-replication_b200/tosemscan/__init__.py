@@ -49,6 +49,15 @@ SIMILAR_PAIR = np.dtype([("a", "<i4"), ("b", "<i4"), ("lcs", "<u4"),
 SIMILAR_EVENT = np.dtype([("status", "<i4"), ("old_a", "<i4"), ("old_b", "<i4"), ("a", "<i4"), ("b", "<i4"), ("old_lcs", "<u4"),
                           ("old_score", "<u4"), ("lcs", "<u4"), ("score", "<u4")])   # tsm_similar_event (docs/SPEC.md section 24)
 SIMILAR_STATUSES = ["changed", "removed", "dropped", "diverged", "created", "copied", "converged"]   # SIMILAR_EVENT status
+LINK_TEST = np.dtype([("file", "<i4"), ("line", "<i4"), ("calls", "<i4"), ("linked_calls", "<i4"), ("links", "<i4"),
+                      ("function_links", "<i4"), ("focal_links", "<i4"),
+                      ("flags", "<u4")])   # tsm_link_test: one test of a test file and its links (docs/SPEC.md section 27)
+LINK = np.dtype([("test", "<i4"), ("name_def", "<i4"), ("target", "<i4"), ("n_defs", "<i4"), ("calls", "<i4"), ("line", "<i4"),
+                 ("byte", "<i4")])   # tsm_link: one (test, name) link, its target definition or -1 and its first call
+LINK_DEF = np.dtype([("file", "<i4"), ("line", "<i4"), ("name_off", "<i4"), ("name_len", "<i4"), ("kind", "<i4"), ("tests", "<i4"),
+                     ("tests_by_name", "<i4"), ("calls", "<i4")])   # tsm_link_def: one definition of a production file
+LINK_EAGER, LINK_LAZY = 1, 2                     # bits of LINK_TEST flags
+LINK_KINDS = {1: "function", 2: "class"}         # LINK_DEF kind
 ASSERT_EDIT = np.dtype([("rev", "<i8"), ("aev", "<i8"), ("score", "<i4"), ("_pad", "<i4")])   # tsm_assert_edit: event indices
 
 # every symbol include/tosemscan.h declares (tests check the library exports exactly these)
@@ -62,7 +71,8 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_diff_pairs_smells", "tsm_diff_smells_last_ms", "tsm_diff_pairs_moves", "tsm_moves_last_ms", "tsm_clones_blind",
            "tsm_clones_blind_last_ms", "tsm_clone_churn", "tsm_clone_churn_last_ms", "tsm_similar_tests", "tsm_similar_tests_last_ms",
            "tsm_similar_churn", "tsm_similar_churn_last_ms", "tsm_smells_lexical", "tsm_smells_lexical_last_ms",
-           "tsm_diff_pairs_smells_lexical", "tsm_diff_smells_lexical_last_ms"]
+           "tsm_diff_pairs_smells_lexical", "tsm_diff_smells_lexical_last_ms", "tsm_test_links", "tsm_test_links_last_ms",
+           "tsm_focal_stems"]
 FRAG_STATES = ["kept", "edited", "whole"]          # tsm_clone_churn state[j] (docs/SPEC.md section 22)
 CLONE_STATUSES = ["untouched", "changed", "removed", "diverged", "dropped", "created", "copied", "joined"]   # status[c]
 
@@ -134,6 +144,11 @@ class _SimilarResult(C.Structure):
                 ("pairs", C.c_void_p), ("pair_cap", C.c_int64), ("n_pairs", C.c_int64),
                 ("class_base", C.c_void_p), ("class_cap", C.c_int64), ("n_classes", C.c_int64),
                 ("member", C.c_void_p), ("member_cap", C.c_int64), ("n_members", C.c_int64), ("n_candidates", C.c_int64)]
+
+
+class _LinksResult(C.Structure):
+    _fields_ = [("tests", C.c_void_p), ("test_cap", C.c_int64), ("n_tests", C.c_int64), ("links", C.c_void_p), ("link_cap", C.c_int64),
+                ("n_links", C.c_int64), ("defs", C.c_void_p), ("def_cap", C.c_int64), ("n_defs", C.c_int64)]
 
 
 class _SimilarChurnSide(C.Structure):
@@ -262,6 +277,12 @@ def lib():
                                          C.POINTER(C.c_int64), C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p]
         L.tsm_smells_lexical_last_ms.restype = C.c_int
         L.tsm_smells_lexical_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
+        L.tsm_test_links.restype = C.c_int
+        L.tsm_test_links.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_void_p, C.c_void_p, C.POINTER(_LinksResult), C.c_void_p]
+        L.tsm_test_links_last_ms.restype = C.c_int
+        L.tsm_test_links_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
+        L.tsm_focal_stems.restype = C.c_int
+        L.tsm_focal_stems.argtypes = [C.POINTER(C.c_char_p), C.c_void_p, C.c_int32, C.c_void_p]
         L.tsm_similar_tests.restype = C.c_int
         L.tsm_similar_tests.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_int32, C.c_int32, C.POINTER(_SimilarResult), C.c_void_p]
         L.tsm_similar_tests_last_ms.restype = C.c_int
@@ -299,6 +320,19 @@ def lib():
 
 def _p(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def focal_stems(paths, role):
+    """The naming convention of docs/SPEC.md section 27 (tsm_focal_stems): per path, the id of a production file's base name
+    without its extension, or of a test file's focal stem (-1 when it is empty).  paths: str or bytes; role: nonzero = test file."""
+    n = len(paths)
+    arr = (C.c_char_p * max(n, 1))(*[p.encode() if isinstance(p, str) else bytes(p) for p in paths])
+    role = np.ascontiguousarray(role, np.uint8)
+    stem = np.zeros(max(n, 1), np.int32)
+    rc = lib().tsm_focal_stems(arr, _p(role), n, _p(stem))
+    if rc:
+        raise TsmError(rc, "tsm_focal_stems")
+    return stem[:n]
 
 
 def category_name(i):
@@ -985,6 +1019,27 @@ class Scanner:
                     "lex": lex[:nt.value]}
         raise TsmError(TSM_E_CAPACITY, "tsm_smells_lexical")
 
+    def test_links(self, corpus, role, stem=None, stream=None, cap=None):
+        """Test-to-code links (docs/SPEC.md section 27): a dict of tests (LINK_TEST, one per test of a test file), links (LINK, in
+        (test, first call) order) and defs (LINK_DEF, one per definition of a production file).  role[f] != 0 marks a test file;
+        stem[f] is focal_stems' id (None: no focal files).  Arrays too small are sized from the counts and the call is made again
+        (cap: the first guess for every array)."""
+        cs = corpus.c_struct()
+        role = np.ascontiguousarray(role, np.uint8)
+        stem = None if stem is None else np.ascontiguousarray(stem, np.int32)
+        ct = ck = cd = int(cap if cap is not None else 0)
+        for _ in range(2):
+            tests, links, defs = np.zeros(max(ct, 1), LINK_TEST), np.zeros(max(ck, 1), LINK), np.zeros(max(cd, 1), LINK_DEF)
+            r = _LinksResult(tests=_p(tests), test_cap=ct, links=_p(links), link_cap=ck, defs=_p(defs), def_cap=cd)
+            rc = lib().tsm_test_links(self._ctx, C.byref(cs), _p(role), _p(stem), C.byref(r), stream)
+            if rc == TSM_E_CAPACITY and (r.n_tests > ct or r.n_links > ck or r.n_defs > cd):
+                ct, ck, cd = int(r.n_tests), int(r.n_links), int(r.n_defs)
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_test_links")
+            return {"tests": tests[:r.n_tests], "links": links[:r.n_links], "defs": defs[:r.n_defs]}
+        raise TsmError(TSM_E_CAPACITY, "tsm_test_links")
+
     def diff_smells(self, olds, news, stream=None, cap=None):
         """Test-smell churn (docs/SPEC.md section 19): a dict of added, removed, detail (tsm_diff_pairs_detail's), old_cases and
         new_cases (diff_cases' CASE arrays), old_tests and new_tests (SMELL_TEST records of each side, file = the pair) and
@@ -1187,6 +1242,13 @@ class Scanner:
         states + k_lex_body + k_lex_lines, k_lex_tests] in ms."""
         ms = (C.c_float * 4)()
         lib().tsm_smells_lexical_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
+
+    def test_links_last_ms(self):
+        """Device time of the last test_links call: [k_scan, the front (kinds, case spans, smell stage, lexer states, the tests
+        of the test files and their code lines), k_link_lines, the join to the records] in ms."""
+        ms = (C.c_float * 4)()
+        lib().tsm_test_links_last_ms(self._ctx, C.byref(ms))
         return [float(x) for x in ms]
 
     def clones_last_ms(self):
