@@ -454,6 +454,51 @@ int tsm_test_links(tsm_ctx* ctx, const tsm_corpus* corpus, const uint8_t* role, 
                    void* stream);
 int tsm_test_links_last_ms(tsm_ctx* ctx, float* ms4);
 
+/* Test-to-code link churn along a revision history (docs/SPEC.md section 28): the links each step adds, removes, retargets and
+ * redefines, test by test, and the Eager Test / Lazy Test flags it introduces and removes.  old_rev / new_rev and the pairs are
+ * those of tsm_similar_churn (the k-th file of old_rev in no pair is the k-th such file of new_rev and is unchanged); each
+ * revision is one repository (its grp is not read).  old_role / old_stem and new_role / new_stem are the role and stem arrays
+ * of tsm_test_links for each revision (a stem array may be NULL: all -1).  Per side (old_side: old_rev, new_side: new_rev):
+ *   links    filled exactly as tsm_test_links fills it for that revision alone (its caps and counts are those of tsm_links_result)
+ *   match    per link test (links.test_cap entries): the other side's link test, or -1.  In an unchanged file test i is test i;
+ *            within a pair tests match through the section-16 matching of their cases, and a match whose other side is not a
+ *            link test does not count
+ *   change   per link test: 'A' (new only), 'D' (old only), '=' (matched; no marked line in either body, equal body_lines) or 'M'
+ * events[n_events]: one tsm_link_event per row of section 28.  event is a TSM_LINKEV_* code; cause a TSM_LINKCAUSE_* code for
+ * TSM_LINKEV_ADDED / REMOVED, else -1; old_test / test the link tests of each side (-1 where absent); old_link / link the links of
+ * the (test, name) on each side (-1 where absent); old_calls / calls the test's call tokens of the name on each side, linked or
+ * not (-1 for a side without the test); old_defs / defs the name's definitions in each revision.  Flag rows (TSM_LINKEV_EAGER_* /
+ * LAZY_*) have -1 from old_link on.  Rows come per output test, the 'D' tests in old order and then the new tests in new order;
+ * within a test its flag rows (eager before lazy), its removed links in old first-call order, then its other link events in new
+ * first-call order.
+ * Any output pointer may be NULL (it is skipped); every count is always set.  A short cap for a given output (a side's links
+ * caps, links.test_cap for match and change, event_cap) returns TSM_E_CAPACITY with every count set.  TSM_E_ARG for a NULL
+ * role, a stem below -1, a file index out of range, a file in two pairs of one side, a pair (-1, -1), unpaired file counts that
+ * differ, or an unpaired file whose length, line count, role or test count differs from its counterpart's.  n_pairs = 0
+ * and n_files = 0 are legal.  More than 2^28 definitions or calls on a side is TSM_E_NOMEM.
+ * Kernels: k_scan over both revisions with header events; the marks of tsm_clone_churn (k_churn_gather, the diff,
+ * k_churn_marks); per revision the link stage of tsm_test_links; k_lc_change (one warp per matched test of a changed pair);
+ * k_lc_calls and k_lc_links (one table of (identity, name) keys over the calls of both sides), k_case_kept + xscan per side,
+ * k_lc_by_rank and k_lc_defmap (the corresponding new line of every old definition); k_lc_events (count), xscan, k_lc_events
+ * (write) (csrc/tsm_link_churn_kernels.cuh).
+ * tsm_link_churn_last_ms: device time of the last call, ms4 = { k_scan over both revisions, both link fronts + the marks diff +
+ * k_lc_change, both link joins, the churn join and emit }. */
+enum { TSM_LINKEV_ADDED = 0, TSM_LINKEV_REMOVED = 1, TSM_LINKEV_RETARGETED = 2, TSM_LINKEV_REDEFINED = 3,
+       TSM_LINKEV_EAGER_INTRODUCED = 4, TSM_LINKEV_EAGER_REMOVED = 5, TSM_LINKEV_LAZY_INTRODUCED = 6, TSM_LINKEV_LAZY_REMOVED = 7 };
+enum { TSM_LINKCAUSE_TEST = 0, TSM_LINKCAUSE_CALL = 1, TSM_LINKCAUSE_DEFINITION = 2 };
+typedef struct tsm_link_churn_side {
+  tsm_links_result links;              /* what tsm_test_links gives for that revision alone */
+  int32_t* match; uint8_t* change;     /* [links.test_cap] per link test: other side's link test or -1; 'A' 'D' '=' 'M' */
+} tsm_link_churn_side;
+typedef struct tsm_link_event {        /* one row; -1 where a side lacks it */
+  int32_t event, cause, old_test, test, old_link, link, old_calls, calls, old_defs, defs;
+} tsm_link_event;
+int tsm_link_churn(tsm_ctx* ctx, const tsm_corpus* old_rev, const tsm_corpus* new_rev, const uint8_t* old_role, const int32_t* old_stem,
+                   const uint8_t* new_role, const int32_t* new_stem, const int32_t* pair_old, const int32_t* pair_new, int64_t n_pairs,
+                   tsm_link_churn_side* old_side, tsm_link_churn_side* new_side, tsm_link_event* events, int64_t event_cap,
+                   int64_t* n_events, void* stream);
+int tsm_link_churn_last_ms(tsm_ctx* ctx, float* ms4);
+
 /* Similar tests (docs/SPEC.md section 23, `tosem-scan similar-tests`): the pairs of tests of section 18 whose sequences of kept
  * blind lines (section 21, header line included) are at least min_similarity % alike, and the classes they link.  A test is
  * compared when it has at least min_lines kept lines (min_lines >= 1, else TSM_E_ARG).  Tests a < b form a pair when both are

@@ -29,6 +29,7 @@
 #include "tsm_smell_kernels.cuh"
 #include "tsm_lexsmell_kernels.cuh"
 #include "tsm_link_kernels.cuh"
+#include "tsm_link_churn_kernels.cuh"
 #include "tsm_move_kernels.cuh"
 #include "tsm_clone_churn_kernels.cuh"
 #include "../host/tsm_names.hpp"
@@ -105,6 +106,8 @@ enum Timed {
               // tsm_diff_pairs_smells_lexical
   MS_LINKS,   // k_scan, front (smell stage, lexer states, test code lines), k_link_lines, the join to the records of the last
               // tsm_test_links
+  MS_LCHURN,  // k_scan of both revisions, both link fronts + marks + k_lc_change, both link joins, the churn join and emit of
+              // the last tsm_link_churn
   N_TIMED
 };
 
@@ -207,6 +210,7 @@ constexpr EvSpan EV_BLAME = {0, 1};
 constexpr EvSpan EV_CCHURN = {0, 1};
 constexpr int EV_LK_FRONT = 2, EV_LK_LINES = 6, EV_LK_JOIN = 7, EV_LK_END = 5;
 constexpr int EV_LX_FRONT = 2, EV_LX_LINES = 6, EV_LX_TESTS = 7, EV_LX_END = 5;
+constexpr int EV_LC_FROM = 2, EV_LC_TO = 5;
 constexpr int EV_ST_FRONT = 2, EV_ST_ENUM = 3, EV_ST_VERIFY = 4, EV_ST_END = 5, EV_ST_LEXED = 6, EV_ST_LISTS = 7;
 
 // The start of every call that queues device work on st: the ctx's device, the ctx's pool for the call's DevBufs, and the
@@ -2578,6 +2582,160 @@ static uint32_t link_slots(unsigned long long keys) {     // a power of two at l
   return (uint32_t)s;
 }
 
+// One revision's link state, resident while the caller needs it: the tests of its test files (tests), the LinkDef and LinkCall
+// arrays, both tables, the links with their first-call slots, and the records of tsm_test_links (out_tests, links, out_defs).
+struct LinkStage {
+  CaseSpans sp; SmellBufs m;
+  DevBuf bsum, state, role, stem, grp, tflag, tpos, tests, lxflag, lxend, ltest, dcnt, ccnt, dbase, cbase;
+  DevBuf defs, calls, name, ndefs, kmask, first, ntests, link, lcalls, lfirst, dslot, cslot, cflag, cpos, tlinks, lbase, dtests, dcalls, jbsum;
+  DevBuf links, lbits, out_tests, out_defs;
+  uint32_t na = 0, nt = 0, nd = 0, nc = 0, ns = 0;         // tests, link tests, definitions, calls, slots of the name table
+  unsigned long long nk = 0;                               // links
+};
+
+// The link stage over one side whose line records (with header events) exist: the front (case spans, smell stage, lexer
+// states, the tests of the test files and their code lines), k_link_lines, then the join to the records.  grp NULL: all 0.
+// ms3 = { front, k_link_lines, join }.
+static int link_stage(tsm_ctx* c, const HostSide& S, const uint8_t* role, const int32_t* stem, const uint16_t* grp, LinkStage& K,
+                      float* ms3, int& launches, cudaStream_t st) {
+  const unsigned long long total = S.total;
+  const size_t L = (size_t)total;
+  const uint32_t nfu = (uint32_t)S.n;
+  const size_t nf = (size_t)S.n;
+  CaseSpans& sp = K.sp;
+  SmellBufs& m = K.m;
+  if (!K.bsum.alloc(8 * (L / XS_TILE + 4)) || !K.state.alloc(L) || !K.role.alloc(nf) || !K.stem.alloc(4 * nf) ||
+      !K.grp.alloc(2 * nf) || !K.lxflag.alloc(L) || !K.lxend.alloc(4 * L) || !K.ltest.alloc(4 * L) || !K.dcnt.alloc(4 * L) ||
+      !K.ccnt.alloc(4 * L) || !K.dbase.alloc(8 * (L + 1)) || !K.cbase.alloc(8 * (L + 1)))
+    return TSM_E_CUDA;
+  CU(cudaMemcpyAsync(K.role.p, role, nf, cudaMemcpyHostToDevice, st));
+  if (stem) CU(cudaMemcpyAsync(K.stem.p, stem, 4 * nf, cudaMemcpyHostToDevice, st));
+  else CU(cudaMemsetAsync(K.stem.p, 0xFF, 4 * nf, st));
+  if (grp) CU(cudaMemcpyAsync(K.grp.p, grp, 2 * nf, cudaMemcpyHostToDevice, st));
+  else CU(cudaMemsetAsync(K.grp.p, 0, 2 * nf, st));
+  CU(cudaEventRecord(c->diff_ev[EV_LK_FRONT], st));
+  int rc = case_spans(S, sp, K.bsum, launches, st);
+  if (rc == TSM_OK) rc = smell_stage(c, S, sp, K.bsum, m, launches, st);
+  if (rc != TSM_OK) return rc;
+  const unsigned grid = (unsigned)((L + 255) / 256);
+  k_blind_state<<<grid, 256, 0, st>>>(S.d, nfu, total, K.state.as<uint8_t>());
+  k_blind_scan<<<(unsigned)(((size_t)nfu * 32 + 255) / 256), 256, 0, st>>>(S.d.line_base, nfu, K.state.as<uint8_t>());
+  launches += 2;
+  unsigned long long* pin = c->h_rb->u64;
+  CU(cudaMemcpyAsync(pin, m.tidx.as<unsigned long long>() + sp.n_cases, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const uint32_t na = (uint32_t)*pin;                      // the tests of every file
+  K.na = na;
+  if (!K.tflag.alloc(4 * ((size_t)na + 1)) || !K.tpos.alloc(8 * ((size_t)na + 1)) || !K.tests.alloc(sizeof(tsm_smell_test) * ((size_t)na + 1)))
+    return TSM_E_CUDA;
+  const unsigned agrid = (unsigned)((na + 255) / 256);
+  if (na) k_link_pick<<<agrid, 256, 0, st>>>(m.tests.as<tsm_smell_test>(), na, K.role.as<uint8_t>(), K.tflag.as<uint32_t>());
+  xscan(K.tflag.as<uint32_t>(), na, K.bsum.as<unsigned long long>(), K.tpos.as<unsigned long long>(), st);
+  if (na) k_link_gather<<<agrid, 256, 0, st>>>(m.tests.as<tsm_smell_test>(), na, K.tflag.as<uint32_t>(), K.tpos.as<unsigned long long>(),
+                                               K.tests.as<tsm_smell_test>());
+  CU(cudaMemcpyAsync(pin, K.tpos.as<unsigned long long>() + na, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemsetAsync(K.lxflag.p, 0, L, st));
+  CU(cudaMemsetAsync(K.ltest.p, 0xFF, 4 * L, st));
+  CU(cudaStreamSynchronize(st));
+  const uint32_t nt = (uint32_t)*pin;                      // the tests of the test files
+  K.nt = nt;
+  launches += na ? 5 : 3;
+  const tsm_smell_test* dt = K.tests.as<tsm_smell_test>();
+  const unsigned tgrid = std::min((unsigned)((nt + 7) / 8), (unsigned)c->sms * 8);
+  if (nt) {
+    k_lex_body<<<tgrid, 256, 0, st>>>(LexBody{dt, nt, S.d.line_base, S.d.ext, m.kind.as<uint8_t>(), m.lines.as<SmellLine>(),
+                                              K.lxflag.as<uint8_t>(), K.lxend.as<uint32_t>()});
+    k_link_mark<<<tgrid, 256, 0, st>>>(dt, nt, S.d.line_base, K.lxflag.as<uint8_t>(), K.ltest.as<uint32_t>());
+    launches += 2;
+  }
+  CU(cudaEventRecord(c->diff_ev[EV_LK_LINES], st));
+  k_link_lines<false><<<grid, 256, 0, st>>>(S.d, nfu, total, K.state.as<uint8_t>(), K.role.as<uint8_t>(), K.ltest.as<uint32_t>(),
+                                            K.dcnt.as<uint32_t>(), K.ccnt.as<uint32_t>(), nullptr, nullptr, nullptr, nullptr);
+  xscan(K.dcnt.as<uint32_t>(), (uint32_t)total, K.bsum.as<unsigned long long>(), K.dbase.as<unsigned long long>(), st);
+  xscan(K.ccnt.as<uint32_t>(), (uint32_t)total, K.bsum.as<unsigned long long>(), K.cbase.as<unsigned long long>(), st);
+  CU(cudaMemcpyAsync(pin, K.dbase.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(pin + 1, K.cbase.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const unsigned long long nd64 = pin[0], nc64 = pin[1];
+  if (nd64 > kLinkMaxEntries || nc64 > kLinkMaxEntries) return TSM_E_NOMEM;   // (tables of more than 16 GiB)
+  const uint32_t nd = (uint32_t)nd64, nc = (uint32_t)nc64;
+  const uint32_t ns = link_slots(2ull * nd), nl = link_slots(2ull * nc);
+  K.nd = nd; K.nc = nc; K.ns = ns;
+  if (!K.jbsum.alloc(8 * ((size_t)std::max(nc, nt) / XS_TILE + 4)) || !K.defs.alloc(sizeof(LinkDef) * ((size_t)nd + 1)) || !K.calls.alloc(sizeof(LinkCall) * ((size_t)nc + 1)) ||
+      !K.name.alloc(16 * (size_t)ns) || !K.ndefs.alloc(4 * (size_t)ns) || !K.kmask.alloc(4 * (size_t)ns) || !K.first.alloc(4 * (size_t)ns) ||
+      !K.ntests.alloc(4 * (size_t)ns) || !K.link.alloc(16 * (size_t)nl) || !K.lcalls.alloc(4 * (size_t)nl) ||
+      !K.lfirst.alloc(4 * (size_t)nl) || !K.dslot.alloc(4 * ((size_t)nd + 1)) || !K.cslot.alloc(4 * ((size_t)nc + 1)) ||
+      !K.cflag.alloc(4 * ((size_t)nc + 1)) || !K.cpos.alloc(8 * ((size_t)nc + 1)) || !K.tlinks.alloc(4 * ((size_t)nt + 1)) ||
+      !K.lbase.alloc(8 * ((size_t)nt + 1)) || !K.dtests.alloc(4 * ((size_t)nd + 1)) || !K.dcalls.alloc(4 * ((size_t)nd + 1)))
+    return TSM_E_CUDA;
+  k_link_lines<true><<<grid, 256, 0, st>>>(S.d, nfu, total, K.state.as<uint8_t>(), K.role.as<uint8_t>(), K.ltest.as<uint32_t>(),
+                                           K.dcnt.as<uint32_t>(), K.ccnt.as<uint32_t>(), K.dbase.as<unsigned long long>(),
+                                           K.cbase.as<unsigned long long>(), K.defs.as<LinkDef>(), K.calls.as<LinkCall>());
+  launches += 8;                                           // lines (count), two xscans (3 each), lines (write)
+  CU(cudaEventRecord(c->diff_ev[EV_LK_JOIN], st));
+  CU(cudaMemsetAsync(K.name.p, 0, 16 * (size_t)ns, st));
+  CU(cudaMemsetAsync(K.ndefs.p, 0, 4 * (size_t)ns, st));
+  CU(cudaMemsetAsync(K.kmask.p, 0, 4 * (size_t)ns, st));
+  CU(cudaMemsetAsync(K.first.p, 0xFF, 4 * (size_t)ns, st));
+  CU(cudaMemsetAsync(K.ntests.p, 0, 4 * (size_t)ns, st));
+  CU(cudaMemsetAsync(K.link.p, 0, 16 * (size_t)nl, st));
+  CU(cudaMemsetAsync(K.lcalls.p, 0, 4 * (size_t)nl, st));
+  CU(cudaMemsetAsync(K.lfirst.p, 0xFF, 4 * (size_t)nl, st));
+  CU(cudaMemsetAsync(K.tlinks.p, 0, 4 * ((size_t)nt + 1), st));
+  CU(cudaMemsetAsync(K.dtests.p, 0, 4 * ((size_t)nd + 1), st));
+  CU(cudaMemsetAsync(K.dcalls.p, 0, 4 * ((size_t)nd + 1), st));
+  const LinkTables T{K.name.as<LinkKey>(), ns - 1, K.ndefs.as<uint32_t>(), K.kmask.as<uint32_t>(), K.first.as<uint32_t>(),
+                     K.ntests.as<uint32_t>(), K.link.as<LinkKey>(), nl - 1, K.lcalls.as<uint32_t>(), K.lfirst.as<uint32_t>()};
+  const unsigned dgrid = (unsigned)((nd + 255) / 256), cgrid = (unsigned)((nc + 255) / 256);
+  if (nd) k_link_defs<<<dgrid, 256, 0, st>>>(K.defs.as<LinkDef>(), nd, K.grp.as<uint16_t>(), K.stem.as<int32_t>(), T, K.dslot.as<uint32_t>());
+  if (nc) {
+    k_link_calls<<<cgrid, 256, 0, st>>>(K.calls.as<LinkCall>(), nc, K.ltest.as<uint32_t>(), dt, K.grp.as<uint16_t>(), T,
+                                        K.cslot.as<uint32_t>(), K.tlinks.as<uint32_t>());
+    k_link_first<<<cgrid, 256, 0, st>>>(K.cslot.as<uint32_t>(), nc, T, K.cflag.as<uint32_t>());
+  }
+  xscan(K.cflag.as<uint32_t>(), nc, K.jbsum.as<unsigned long long>(), K.cpos.as<unsigned long long>(), st);   // (nc may exceed the
+  xscan(K.tlinks.as<uint32_t>(), nt, K.jbsum.as<unsigned long long>(), K.lbase.as<unsigned long long>(), st); //  lines: own sums)
+  CU(cudaMemcpyAsync(pin, K.cpos.as<unsigned long long>() + nc, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const unsigned long long nk = *pin;                      // the links
+  K.nk = nk;
+  if (!K.links.alloc(sizeof(tsm_link) * ((size_t)nk + 1)) || !K.lbits.alloc((size_t)nk + 1) ||
+      !K.out_tests.alloc(sizeof(tsm_link_test) * ((size_t)nt + 1)) || !K.out_defs.alloc(sizeof(tsm_link_def) * ((size_t)nd + 1)))
+    return TSM_E_CUDA;
+  if (nc)
+    k_link_emit<<<cgrid, 256, 0, st>>>(LinkEmit{K.calls.as<LinkCall>(), nc, K.cslot.as<uint32_t>(), K.cflag.as<uint32_t>(),
+                                                K.cpos.as<unsigned long long>(), K.ltest.as<uint32_t>(), dt, K.grp.as<uint16_t>(),
+                                                K.stem.as<int32_t>(), S.d.line_base, K.defs.as<LinkDef>(), T, K.links.as<tsm_link>(),
+                                                K.lbits.as<uint8_t>(), K.dtests.as<uint32_t>(), K.dcalls.as<uint32_t>()});
+  if (nt)
+    k_link_tests<<<tgrid, 256, 0, st>>>(LinkTests{dt, nt, S.d.line_base, K.cbase.as<unsigned long long>(), K.lbase.as<unsigned long long>(),
+                                                  K.links.as<tsm_link>(), K.lbits.as<uint8_t>(), K.out_tests.as<tsm_link_test>()});
+  if (nd) k_link_out<<<dgrid, 256, 0, st>>>(K.defs.as<LinkDef>(), nd, K.dslot.as<uint32_t>(), S.d.line_base, T, K.dtests.as<uint32_t>(),
+                                            K.dcalls.as<uint32_t>(), K.out_defs.as<tsm_link_def>());
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(c->diff_ev[EV_LK_END], st));
+  CU(cudaStreamSynchronize(st));
+  launches += (nd ? 2 : 0) + (nc ? 3 : 0) + 6 + (nt ? 1 : 0);   // defs + out, calls + first + emit, two xscans, tests
+  ms3[0] = elapsed_ms(c->diff_ev[EV_LK_FRONT], c->diff_ev[EV_LK_LINES]);
+  ms3[1] = elapsed_ms(c->diff_ev[EV_LK_LINES], c->diff_ev[EV_LK_JOIN]);
+  ms3[2] = elapsed_ms(c->diff_ev[EV_LK_JOIN], c->diff_ev[EV_LK_END]);
+  return TSM_OK;
+}
+
+// The records of a link stage into out, when they fit (TSM_E_CAPACITY otherwise); the counts are always set.
+static int link_copy(const LinkStage& K, tsm_links_result* out, cudaStream_t st) {
+  const uint32_t nt = K.nt, nd = K.nd;
+  const unsigned long long nk = K.nk;
+  out->n_tests = nt; out->n_links = (int64_t)nk; out->n_defs = nd;
+  if ((out->tests && out->test_cap < (int64_t)nt) || (out->links && out->link_cap < (int64_t)nk) || (out->defs && out->def_cap < (int64_t)nd))
+    return TSM_E_CAPACITY;
+  if (out->tests && nt) CU(cudaMemcpyAsync(out->tests, K.out_tests.p, sizeof(tsm_link_test) * nt, cudaMemcpyDeviceToHost, st));
+  if (out->links && nk) CU(cudaMemcpyAsync(out->links, K.links.p, sizeof(tsm_link) * nk, cudaMemcpyDeviceToHost, st));
+  if (out->defs && nd) CU(cudaMemcpyAsync(out->defs, K.out_defs.p, sizeof(tsm_link_def) * nd, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TSM_OK;
+}
+
 extern "C" int tsm_test_links(tsm_ctx* c, const tsm_corpus* k, const uint8_t* role, const int32_t* stem, tsm_links_result* out,
                               void* stream) {
   if (!c || !k || !role || !out || k->n_files < 0 || out->test_cap < 0 || out->link_cap < 0 || out->def_cap < 0) return TSM_E_ARG;
@@ -2590,136 +2748,13 @@ extern "C" int tsm_test_links(tsm_ctx* c, const tsm_corpus* k, const uint8_t* ro
   out->n_tests = out->n_links = out->n_defs = 0;
   std::vector<int64_t> base((size_t)nf + 1);
   int64_t n_lines = 0;
-  return line_records(c, k, true, base.data(), INT64_MAX, &n_lines, stream, [&](const HostSide& S, unsigned long long total, cudaStream_t st) -> int {
-    const size_t L = (size_t)total;
-    const uint32_t nfu = (uint32_t)S.n;
-    CaseSpans sp;
-    SmellBufs m;
-    DevBuf d_bsum, d_state, d_role, d_stem, d_grp, d_tflag, d_tpos, d_tests, d_lxflag, d_lxend, d_ltest, d_dcnt, d_ccnt, d_dbase, d_cbase;
-    if (!d_bsum.alloc(8 * (L / XS_TILE + 4)) || !d_state.alloc(L) || !d_role.alloc((size_t)nf) || !d_stem.alloc(4 * (size_t)nf) ||
-        !d_grp.alloc(2 * (size_t)nf) || !d_lxflag.alloc(L) || !d_lxend.alloc(4 * L) || !d_ltest.alloc(4 * L) || !d_dcnt.alloc(4 * L) ||
-        !d_ccnt.alloc(4 * L) || !d_dbase.alloc(8 * (L + 1)) || !d_cbase.alloc(8 * (L + 1)))
-      return TSM_E_CUDA;
-    CU(cudaMemcpyAsync(d_role.p, role, (size_t)nf, cudaMemcpyHostToDevice, st));
-    if (stem) CU(cudaMemcpyAsync(d_stem.p, stem, 4 * (size_t)nf, cudaMemcpyHostToDevice, st));
-    else CU(cudaMemsetAsync(d_stem.p, 0xFF, 4 * (size_t)nf, st));
-    if (k->grp) CU(cudaMemcpyAsync(d_grp.p, k->grp, 2 * (size_t)nf, cudaMemcpyHostToDevice, st));
-    else CU(cudaMemsetAsync(d_grp.p, 0, 2 * (size_t)nf, st));
+  return line_records(c, k, true, base.data(), INT64_MAX, &n_lines, stream, [&](const HostSide& S, unsigned long long, cudaStream_t st) -> int {
+    LinkStage K;
     int launches = 0;
-    CU(cudaEventRecord(c->diff_ev[EV_LK_FRONT], st));
-    int rc = case_spans(S, sp, d_bsum, launches, st);
-    if (rc == TSM_OK) rc = smell_stage(c, S, sp, d_bsum, m, launches, st);
+    const int rc = link_stage(c, S, role, stem, k->grp, K, &ms[1], launches, st);
     if (rc != TSM_OK) return rc;
-    const unsigned grid = (unsigned)((L + 255) / 256);
-    k_blind_state<<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>());
-    k_blind_scan<<<(unsigned)(((size_t)nfu * 32 + 255) / 256), 256, 0, st>>>(S.d.line_base, nfu, d_state.as<uint8_t>());
-    launches += 2;
-    unsigned long long* pin = c->h_rb->u64;
-    CU(cudaMemcpyAsync(pin, m.tidx.as<unsigned long long>() + sp.n_cases, 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    const uint32_t na = (uint32_t)*pin;                    // the tests of every file
-    if (!d_tflag.alloc(4 * ((size_t)na + 1)) || !d_tpos.alloc(8 * ((size_t)na + 1)) || !d_tests.alloc(sizeof(tsm_smell_test) * ((size_t)na + 1)))
-      return TSM_E_CUDA;
-    const unsigned agrid = (unsigned)((na + 255) / 256);
-    if (na) k_link_pick<<<agrid, 256, 0, st>>>(m.tests.as<tsm_smell_test>(), na, d_role.as<uint8_t>(), d_tflag.as<uint32_t>());
-    xscan(d_tflag.as<uint32_t>(), na, d_bsum.as<unsigned long long>(), d_tpos.as<unsigned long long>(), st);
-    if (na) k_link_gather<<<agrid, 256, 0, st>>>(m.tests.as<tsm_smell_test>(), na, d_tflag.as<uint32_t>(), d_tpos.as<unsigned long long>(),
-                                                 d_tests.as<tsm_smell_test>());
-    CU(cudaMemcpyAsync(pin, d_tpos.as<unsigned long long>() + na, 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemsetAsync(d_lxflag.p, 0, L, st));
-    CU(cudaMemsetAsync(d_ltest.p, 0xFF, 4 * L, st));
-    CU(cudaStreamSynchronize(st));
-    const uint32_t nt = (uint32_t)*pin;                    // the tests of the test files
-    launches += na ? 5 : 3;
-    const tsm_smell_test* dt = d_tests.as<tsm_smell_test>();
-    const unsigned tgrid = std::min((unsigned)((nt + 7) / 8), (unsigned)c->sms * 8);
-    if (nt) {
-      k_lex_body<<<tgrid, 256, 0, st>>>(LexBody{dt, nt, S.d.line_base, S.d.ext, m.kind.as<uint8_t>(), m.lines.as<SmellLine>(),
-                                                d_lxflag.as<uint8_t>(), d_lxend.as<uint32_t>()});
-      k_link_mark<<<tgrid, 256, 0, st>>>(dt, nt, S.d.line_base, d_lxflag.as<uint8_t>(), d_ltest.as<uint32_t>());
-      launches += 2;
-    }
-    CU(cudaEventRecord(c->diff_ev[EV_LK_LINES], st));
-    k_link_lines<false><<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>(), d_role.as<uint8_t>(), d_ltest.as<uint32_t>(),
-                                              d_dcnt.as<uint32_t>(), d_ccnt.as<uint32_t>(), nullptr, nullptr, nullptr, nullptr);
-    xscan(d_dcnt.as<uint32_t>(), (uint32_t)total, d_bsum.as<unsigned long long>(), d_dbase.as<unsigned long long>(), st);
-    xscan(d_ccnt.as<uint32_t>(), (uint32_t)total, d_bsum.as<unsigned long long>(), d_cbase.as<unsigned long long>(), st);
-    CU(cudaMemcpyAsync(pin, d_dbase.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(pin + 1, d_cbase.as<unsigned long long>() + L, 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    const unsigned long long nd64 = pin[0], nc64 = pin[1];
-    if (nd64 > kLinkMaxEntries || nc64 > kLinkMaxEntries) return TSM_E_NOMEM;   // (tables of more than 16 GiB)
-    const uint32_t nd = (uint32_t)nd64, nc = (uint32_t)nc64;
-    const uint32_t ns = link_slots(2ull * nd), nl = link_slots(2ull * nc);
-    DevBuf d_defs, d_calls, d_name, d_ndefs, d_kmask, d_first, d_ntests, d_link, d_lcalls, d_lfirst, d_dslot, d_cslot, d_cflag, d_cpos,
-        d_tlinks, d_lbase, d_dtests, d_dcalls, d_jbsum;
-    if (!d_jbsum.alloc(8 * ((size_t)std::max(nc, nt) / XS_TILE + 4)) || !d_defs.alloc(sizeof(LinkDef) * ((size_t)nd + 1)) || !d_calls.alloc(sizeof(LinkCall) * ((size_t)nc + 1)) ||
-        !d_name.alloc(16 * (size_t)ns) || !d_ndefs.alloc(4 * (size_t)ns) || !d_kmask.alloc(4 * (size_t)ns) || !d_first.alloc(4 * (size_t)ns) ||
-        !d_ntests.alloc(4 * (size_t)ns) || !d_link.alloc(16 * (size_t)nl) || !d_lcalls.alloc(4 * (size_t)nl) ||
-        !d_lfirst.alloc(4 * (size_t)nl) || !d_dslot.alloc(4 * ((size_t)nd + 1)) || !d_cslot.alloc(4 * ((size_t)nc + 1)) ||
-        !d_cflag.alloc(4 * ((size_t)nc + 1)) || !d_cpos.alloc(8 * ((size_t)nc + 1)) || !d_tlinks.alloc(4 * ((size_t)nt + 1)) ||
-        !d_lbase.alloc(8 * ((size_t)nt + 1)) || !d_dtests.alloc(4 * ((size_t)nd + 1)) || !d_dcalls.alloc(4 * ((size_t)nd + 1)))
-      return TSM_E_CUDA;
-    k_link_lines<true><<<grid, 256, 0, st>>>(S.d, nfu, total, d_state.as<uint8_t>(), d_role.as<uint8_t>(), d_ltest.as<uint32_t>(),
-                                             d_dcnt.as<uint32_t>(), d_ccnt.as<uint32_t>(), d_dbase.as<unsigned long long>(),
-                                             d_cbase.as<unsigned long long>(), d_defs.as<LinkDef>(), d_calls.as<LinkCall>());
-    launches += 8;                                         // lines (count), two xscans (3 each), lines (write)
-    CU(cudaEventRecord(c->diff_ev[EV_LK_JOIN], st));
-    CU(cudaMemsetAsync(d_name.p, 0, 16 * (size_t)ns, st));
-    CU(cudaMemsetAsync(d_ndefs.p, 0, 4 * (size_t)ns, st));
-    CU(cudaMemsetAsync(d_kmask.p, 0, 4 * (size_t)ns, st));
-    CU(cudaMemsetAsync(d_first.p, 0xFF, 4 * (size_t)ns, st));
-    CU(cudaMemsetAsync(d_ntests.p, 0, 4 * (size_t)ns, st));
-    CU(cudaMemsetAsync(d_link.p, 0, 16 * (size_t)nl, st));
-    CU(cudaMemsetAsync(d_lcalls.p, 0, 4 * (size_t)nl, st));
-    CU(cudaMemsetAsync(d_lfirst.p, 0xFF, 4 * (size_t)nl, st));
-    CU(cudaMemsetAsync(d_tlinks.p, 0, 4 * ((size_t)nt + 1), st));
-    CU(cudaMemsetAsync(d_dtests.p, 0, 4 * ((size_t)nd + 1), st));
-    CU(cudaMemsetAsync(d_dcalls.p, 0, 4 * ((size_t)nd + 1), st));
-    const LinkTables T{d_name.as<LinkKey>(), ns - 1, d_ndefs.as<uint32_t>(), d_kmask.as<uint32_t>(), d_first.as<uint32_t>(),
-                       d_ntests.as<uint32_t>(), d_link.as<LinkKey>(), nl - 1, d_lcalls.as<uint32_t>(), d_lfirst.as<uint32_t>()};
-    const unsigned dgrid = (unsigned)((nd + 255) / 256), cgrid = (unsigned)((nc + 255) / 256);
-    if (nd) k_link_defs<<<dgrid, 256, 0, st>>>(d_defs.as<LinkDef>(), nd, d_grp.as<uint16_t>(), d_stem.as<int32_t>(), T, d_dslot.as<uint32_t>());
-    if (nc) {
-      k_link_calls<<<cgrid, 256, 0, st>>>(d_calls.as<LinkCall>(), nc, d_ltest.as<uint32_t>(), dt, d_grp.as<uint16_t>(), T,
-                                          d_cslot.as<uint32_t>(), d_tlinks.as<uint32_t>());
-      k_link_first<<<cgrid, 256, 0, st>>>(d_cslot.as<uint32_t>(), nc, T, d_cflag.as<uint32_t>());
-    }
-    xscan(d_cflag.as<uint32_t>(), nc, d_jbsum.as<unsigned long long>(), d_cpos.as<unsigned long long>(), st);   // (nc may exceed the
-    xscan(d_tlinks.as<uint32_t>(), nt, d_jbsum.as<unsigned long long>(), d_lbase.as<unsigned long long>(), st); //  lines: own sums)
-    CU(cudaMemcpyAsync(pin, d_cpos.as<unsigned long long>() + nc, 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    const unsigned long long nk = *pin;                    // the links
-    DevBuf d_links, d_lbits, d_out_tests, d_out_defs;
-    if (!d_links.alloc(sizeof(tsm_link) * ((size_t)nk + 1)) || !d_lbits.alloc((size_t)nk + 1) ||
-        !d_out_tests.alloc(sizeof(tsm_link_test) * ((size_t)nt + 1)) || !d_out_defs.alloc(sizeof(tsm_link_def) * ((size_t)nd + 1)))
-      return TSM_E_CUDA;
-    if (nc)
-      k_link_emit<<<cgrid, 256, 0, st>>>(LinkEmit{d_calls.as<LinkCall>(), nc, d_cslot.as<uint32_t>(), d_cflag.as<uint32_t>(),
-                                                  d_cpos.as<unsigned long long>(), d_ltest.as<uint32_t>(), dt, d_grp.as<uint16_t>(),
-                                                  d_stem.as<int32_t>(), S.d.line_base, d_defs.as<LinkDef>(), T, d_links.as<tsm_link>(),
-                                                  d_lbits.as<uint8_t>(), d_dtests.as<uint32_t>(), d_dcalls.as<uint32_t>()});
-    if (nt)
-      k_link_tests<<<tgrid, 256, 0, st>>>(LinkTests{dt, nt, S.d.line_base, d_cbase.as<unsigned long long>(), d_lbase.as<unsigned long long>(),
-                                                    d_links.as<tsm_link>(), d_lbits.as<uint8_t>(), d_out_tests.as<tsm_link_test>()});
-    if (nd) k_link_out<<<dgrid, 256, 0, st>>>(d_defs.as<LinkDef>(), nd, d_dslot.as<uint32_t>(), S.d.line_base, T, d_dtests.as<uint32_t>(),
-                                              d_dcalls.as<uint32_t>(), d_out_defs.as<tsm_link_def>());
-    CU(cudaGetLastError());
-    CU(cudaEventRecord(c->diff_ev[EV_LK_END], st));
-    CU(cudaStreamSynchronize(st));
-    launches += (nd ? 2 : 0) + (nc ? 3 : 0) + 6 + (nt ? 1 : 0);   // defs + out, calls + first + emit, two xscans, tests
     c->launches += launches;
-    out->n_tests = nt; out->n_links = (int64_t)nk; out->n_defs = nd;
-    ms[1] = elapsed_ms(c->diff_ev[EV_LK_FRONT], c->diff_ev[EV_LK_LINES]);
-    ms[2] = elapsed_ms(c->diff_ev[EV_LK_LINES], c->diff_ev[EV_LK_JOIN]);
-    ms[3] = elapsed_ms(c->diff_ev[EV_LK_JOIN], c->diff_ev[EV_LK_END]);
-    if ((out->tests && out->test_cap < (int64_t)nt) || (out->links && out->link_cap < (int64_t)nk) || (out->defs && out->def_cap < (int64_t)nd))
-      return TSM_E_CAPACITY;
-    if (out->tests && nt) CU(cudaMemcpyAsync(out->tests, d_out_tests.p, sizeof(tsm_link_test) * nt, cudaMemcpyDeviceToHost, st));
-    if (out->links && nk) CU(cudaMemcpyAsync(out->links, d_links.p, sizeof(tsm_link) * nk, cudaMemcpyDeviceToHost, st));
-    if (out->defs && nd) CU(cudaMemcpyAsync(out->defs, d_out_defs.p, sizeof(tsm_link_def) * nd, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    return TSM_OK;
+    return link_copy(K, out, st);
   }, &ms[0], TSM_SCAN_HEADER_EVENTS);
 }
 
@@ -3356,6 +3391,255 @@ extern "C" int tsm_similar_churn(tsm_ctx* c, const tsm_corpus* old_rev, const ts
 }
 
 extern "C" int tsm_similar_churn_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_SCHURN, ms4, 4); }
+
+// ------------------------------------------------------------------------------------- SPEC section 28 link churn
+// Both revisions to the device and their line records with header events (one k_scan pass each), the marks of the pairs
+// (churn_marks), per revision the link stage of tsm_test_links (link_stage, resident to the end); on the host the test identity
+// (unchanged files in order, sc_match_pair for the changed pairs, restricted to the link tests); k_lc_change for the matched
+// tests of changed pairs; then the join: k_lc_calls and k_lc_links over both sides into one table of (identity, name) keys, the
+// kept ranks of both sides, k_lc_by_rank and k_lc_defmap, and k_lc_events counting, an xscan placing and k_lc_events writing the
+// rows.  One synchronisation reads the row count.
+extern "C" int tsm_link_churn(tsm_ctx* c, const tsm_corpus* old_rev, const tsm_corpus* new_rev, const uint8_t* old_role,
+                              const int32_t* old_stem, const uint8_t* new_role, const int32_t* new_stem, const int32_t* pair_old,
+                              const int32_t* pair_new, int64_t n_pairs, tsm_link_churn_side* old_side, tsm_link_churn_side* new_side,
+                              tsm_link_event* events, int64_t event_cap, int64_t* n_events, void* stream) {
+  if (!c || !old_rev || !new_rev || !old_role || !new_role || !old_side || !new_side || !n_events || n_pairs < 0 ||
+      n_pairs > INT32_MAX || (n_pairs && (!pair_old || !pair_new)) || event_cap < 0)
+    return TSM_E_ARG;
+  const tsm_corpus* rev[2] = {old_rev, new_rev};
+  const uint8_t* role[2] = {old_role, new_role};
+  const int32_t* stem[2] = {old_stem, new_stem};
+  tsm_link_churn_side* side[2] = {old_side, new_side};
+  const int32_t* pf[2] = {pair_old, pair_new};
+  const int32_t n = (int32_t)n_pairs;
+  std::vector<int32_t> unpaired[2];
+  for (int i = 0; i < 2; ++i) {
+    const tsm_links_result& o = side[i]->links;
+    if (rev[i]->n_files < 0 || o.test_cap < 0 || o.link_cap < 0 || o.def_cap < 0) return TSM_E_ARG;
+    for (int32_t f = 0; stem[i] && f < rev[i]->n_files; ++f)
+      if (stem[i][f] < -1) return TSM_E_ARG;
+    std::vector<uint8_t> used((size_t)rev[i]->n_files, 0);
+    for (int32_t k = 0; k < n; ++k) {
+      const int32_t f = pf[i][k];
+      if (f < -1 || f >= rev[i]->n_files || (f >= 0 && used[(size_t)f]++) || (pair_old[k] < 0 && pair_new[k] < 0)) return TSM_E_ARG;
+    }
+    for (int32_t f = 0; f < rev[i]->n_files; ++f) if (!used[(size_t)f]) unpaired[i].push_back(f);
+  }
+  if (unpaired[0].size() != unpaired[1].size()) return TSM_E_ARG;
+  for (int i = 0; i < 2; ++i)
+    if (rev[i]->n_files > 0) {
+      const int rc = check_sides({rev[i]}, true);
+      if (rc != TSM_OK) return rc;
+    }
+  for (size_t k = 0; k < unpaired[0].size(); ++k) {
+    const int32_t fo = unpaired[0][k], fn = unpaired[1][k];
+    if (old_rev->len[fo] != new_rev->len[fn] || (old_role[fo] != 0) != (new_role[fn] != 0)) return TSM_E_ARG;
+  }
+  float* const ms = clear_ms(c, MS_LCHURN);
+  c->launches = 0;
+  *n_events = 0;
+  for (int i = 0; i < 2; ++i) side[i]->links.n_tests = side[i]->links.n_links = side[i]->links.n_defs = 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  CallScope call(c, st);
+  CU(call.status);
+  HostSide S[2];
+  LinkStage K[2];
+  DevBuf rmark[2], kept[2], rank[2], d_bsum, d_both, d_same, d_omatch, d_tab, d_slot, d_byrank, d_cfile, d_dline, d_otest, d_cnt, d_pos, d_ev;
+  SyncGuard guard(st);
+  HostSide* scan[2];
+  int ns = 0;
+  for (int i = 0; i < 2; ++i)
+    if (rev[i]->n_files > 0) {
+      const int rc = side_upload(rev[i], S[i], st);
+      if (rc != TSM_OK) return rc;
+      scan[ns++] = &S[i];
+    }
+  if (ns) {
+    const int rc = sides_records(c, scan, ns, st, &ms[0], true, TSM_SCAN_HEADER_EVENTS);
+    if (rc != TSM_OK) return rc;
+  }
+  for (size_t k = 0; k < unpaired[0].size(); ++k) {       // (the definitions' kept ranks assume equal line counts)
+    const size_t fo = (size_t)unpaired[0][k], fn = (size_t)unpaired[1][k];
+    if (S[0].base[fo + 1] - S[0].base[fo] != S[1].base[fn + 1] - S[1].base[fn]) return TSM_E_ARG;
+  }
+  for (int i = 0; i < 2; ++i) {
+    c->launches += S[i].launches;
+    if (!rmark[i].alloc((size_t)S[i].total)) return TSM_E_CUDA;
+    CU(cudaMemsetAsync(rmark[i].p, 0, (size_t)S[i].total, st));
+  }
+  float mms[4] = {0, 0, 0, 0};
+  if (n) {
+    const int rc = churn_marks(c, S, pf, n, rmark, mms, st);
+    if (rc != TSM_OK) return rc;
+  }
+  ms[1] += mms[2] + mms[3];
+  ScRev R[2];
+  std::vector<int32_t> lidx[2];                            // per test of the revision: its link test, or -1
+  for (int i = 0; i < 2; ++i) {
+    ScRev& r = R[i];
+    r.k = rev[i];
+    r.base = S[i].base;
+    if (r.base.empty()) r.base.assign((size_t)rev[i]->n_files + 1, 0);
+    if (S[i].total == 0) { r.index(); continue; }
+    float lms[3];
+    int launches = 0;
+    const int rc = link_stage(c, S[i], role[i], stem[i], nullptr, K[i], lms, launches, st);
+    if (rc != TSM_OK) return rc;
+    c->launches += launches;
+    ms[1] += lms[0] + lms[1];
+    ms[2] += lms[2];
+    r.tests.resize(K[i].na);
+    r.head.resize(K[i].sp.n_cases);
+    r.mark.resize((size_t)S[i].total);
+    if (K[i].na) CU(cudaMemcpyAsync(r.tests.data(), K[i].m.tests.p, sizeof(tsm_smell_test) * K[i].na, cudaMemcpyDeviceToHost, st));
+    if (K[i].sp.n_cases) CU(cudaMemcpyAsync(r.head.data(), K[i].sp.first.p, 4 * (size_t)K[i].sp.n_cases, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(r.mark.data(), rmark[i].p, (size_t)S[i].total, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    r.index();
+  }
+  for (int i = 0; i < 2; ++i) {
+    int32_t next = 0;
+    lidx[i].resize(R[i].tests.size());
+    for (size_t t = 0; t < R[i].tests.size(); ++t) lidx[i][t] = role[i][R[i].tests[t].file] ? next++ : -1;
+  }
+  const uint32_t n_old = K[0].nt, n_new = K[1].nt;
+  std::vector<int32_t> match[2] = {std::vector<int32_t>(n_old, -1), std::vector<int32_t>(n_new, -1)};
+  std::vector<uint8_t> change[2] = {std::vector<uint8_t>(n_old, 'D'), std::vector<uint8_t>(n_new, 'A')};
+  for (size_t k = 0; k < unpaired[0].size(); ++k) {       // an unchanged file: test i is test i
+    const int32_t fo = unpaired[0][k], fn = unpaired[1][k];
+    const size_t to = R[0].tfile[(size_t)fo], tn = R[1].tfile[(size_t)fn], m = R[0].tfile[(size_t)fo + 1] - to;
+    if (m != R[1].tfile[(size_t)fn + 1] - tn) return TSM_E_ARG;
+    for (size_t t = 0; t < m; ++t) {
+      const int32_t a = lidx[0][to + t], b = lidx[1][tn + t];
+      if (a < 0) continue;                                 // (the roles are equal: b is a link test too)
+      match[0][(size_t)a] = b; match[1][(size_t)b] = a;
+      change[0][(size_t)a] = change[1][(size_t)b] = '=';
+    }
+  }
+  std::vector<uint2> all, both;
+  for (int32_t k = 0; k < n; ++k)
+    if (pair_old[k] >= 0 && pair_new[k] >= 0) sc_match_pair(R[0], R[1], pair_old[k], pair_new[k], all);
+  for (const uint2& m : all)
+    if (lidx[0][m.x] >= 0 && lidx[1][m.y] >= 0) both.push_back(make_uint2((uint32_t)lidx[0][m.x], (uint32_t)lidx[1][m.y]));
+  if (!both.empty()) {
+    const uint32_t nm = (uint32_t)both.size();
+    if (!d_both.alloc(sizeof(uint2) * nm) || !d_same.alloc(nm)) return TSM_E_CUDA;
+    std::vector<uint8_t> same(nm);
+    CU(cudaEventRecord(c->diff_ev[EV_LC_FROM], st));
+    CU(cudaMemcpyAsync(d_both.p, both.data(), sizeof(uint2) * nm, cudaMemcpyHostToDevice, st));
+    k_lc_change<<<std::min((nm + 7) / 8, (uint32_t)c->sms * 8), 256, 0, st>>>(K[0].tests.as<tsm_smell_test>(), K[1].tests.as<tsm_smell_test>(),
+                                                                              S[0].d.line_base, S[1].d.line_base, rmark[0].as<uint8_t>(),
+                                                                              rmark[1].as<uint8_t>(), d_both.as<uint2>(), nm, d_same.as<uint8_t>());
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->diff_ev[EV_LC_TO], st));
+    CU(cudaMemcpyAsync(same.data(), d_same.p, nm, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    c->launches++;
+    ms[1] += elapsed_ms(c->diff_ev[EV_LC_FROM], c->diff_ev[EV_LC_TO]);
+    for (uint32_t k = 0; k < nm; ++k) {
+      const uint2 m = both[k];
+      match[0][m.x] = (int32_t)m.y; match[1][m.y] = (int32_t)m.x;
+      change[0][m.x] = change[1][m.y] = same[k] ? '=' : 'M';
+    }
+  }
+  // The join: one table of (identity, name) keys over the calls of both sides, the old definitions' corresponding lines, the rows.
+  std::vector<uint2> otest;                                // per output test (old test, new test)
+  for (uint32_t a = 0; a < n_old; ++a) if (match[0][a] < 0) otest.push_back(make_uint2(a, LK_NONE));
+  for (uint32_t b = 0; b < n_new; ++b) otest.push_back(make_uint2(match[1][b] >= 0 ? (uint32_t)match[1][b] : LK_NONE, b));
+  const uint32_t n_out = (uint32_t)otest.size(), nd_old = K[0].nd;
+  const uint32_t slots = link_slots((unsigned long long)K[0].nc + K[1].nc);
+  std::vector<int32_t> cfile((size_t)rev[0]->n_files + 1, -1);
+  for (size_t k = 0; k < unpaired[0].size(); ++k) cfile[(size_t)unpaired[0][k]] = unpaired[1][k];
+  for (int32_t k = 0; k < n; ++k) if (pair_old[k] >= 0) cfile[(size_t)pair_old[k]] = pair_new[k];
+  const size_t maxL = (size_t)std::max(S[0].total, S[1].total);
+  if (!d_bsum.alloc(8 * (std::max(maxL, (size_t)n_out) / XS_TILE + 4)) || !d_omatch.alloc(4 * ((size_t)n_old + 1)) ||
+      !d_tab.alloc(16 * (size_t)slots) || !d_slot.alloc(sizeof(LcSlot) * slots) || !d_byrank.alloc(4 * ((size_t)S[1].total + 1)) ||
+      !d_cfile.alloc(4 * cfile.size()) || !d_dline.alloc(4 * ((size_t)nd_old + 1)) || !d_otest.alloc(sizeof(uint2) * ((size_t)n_out + 1)) ||
+      !d_cnt.alloc(4 * ((size_t)n_out + 1)) || !d_pos.alloc(8 * ((size_t)n_out + 1)))
+    return TSM_E_CUDA;
+  for (int i = 0; i < 2; ++i)
+    if (!kept[i].alloc(4 * ((size_t)S[i].total + 1)) || !rank[i].alloc(8 * ((size_t)S[i].total + 1))) return TSM_E_CUDA;
+  CU(cudaEventRecord(c->diff_ev[EV_LC_FROM], st));
+  CU(cudaMemcpyAsync(d_omatch.p, match[0].data(), 4 * (size_t)n_old, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d_cfile.p, cfile.data(), 4 * cfile.size(), cudaMemcpyHostToDevice, st));
+  if (n_out) CU(cudaMemcpyAsync(d_otest.p, otest.data(), sizeof(uint2) * n_out, cudaMemcpyHostToDevice, st));
+  CU(cudaMemsetAsync(d_tab.p, 0, 16 * (size_t)slots, st));
+  CU(cudaMemset2DAsync(d_slot.p, sizeof(LcSlot), 0, 8, slots, st));                             // the calls
+  CU(cudaMemset2DAsync(d_slot.as<uint8_t>() + 8, sizeof(LcSlot), 0xFF, 8, slots, st));          // the links: none
+  const int32_t* om = d_omatch.as<int32_t>();
+  for (int i = 0; i < 2; ++i) {
+    const LinkStage& k = K[i];
+    if (k.nc) {
+      k_lc_calls<<<(k.nc + 255) / 256, 256, 0, st>>>(k.calls.as<LinkCall>(), k.nc, k.ltest.as<uint32_t>(), (uint32_t)i, om, n_new,
+                                                     d_tab.as<LinkKey>(), slots - 1, d_slot.as<LcSlot>());
+      c->launches++;
+    }
+  }
+  for (int i = 0; i < 2; ++i) {
+    const LinkStage& k = K[i];
+    if (k.nk) {
+      k_lc_links<<<(unsigned)((k.nk + 255) / 256), 256, 0, st>>>(k.links.as<tsm_link>(), (uint32_t)k.nk, k.defs.as<LinkDef>(), (uint32_t)i, om,
+                                                                 n_new, d_tab.as<LinkKey>(), slots - 1, d_slot.as<LcSlot>());
+      c->launches++;
+    }
+  }
+  for (int i = 0; i < 2; ++i) {
+    const uint32_t total = (uint32_t)S[i].total;
+    if (total) k_case_kept<<<(total + 255) / 256, 256, 0, st>>>(rmark[i].as<uint8_t>(), total, kept[i].as<uint32_t>());
+    xscan(kept[i].as<uint32_t>(), total, d_bsum.as<unsigned long long>(), rank[i].as<unsigned long long>(), st);
+    c->launches += total ? 4 : 0;
+  }
+  if (S[1].total)
+    k_lc_by_rank<<<(unsigned)((S[1].total + 255) / 256), 256, 0, st>>>(kept[1].as<uint32_t>(), rank[1].as<unsigned long long>(),
+                                                                       (uint32_t)S[1].total, d_byrank.as<uint32_t>());
+  if (nd_old)
+    k_lc_defmap<<<(nd_old + 255) / 256, 256, 0, st>>>(K[0].defs.as<LinkDef>(), nd_old, d_cfile.as<int32_t>(), S[0].d.line_base,
+                                                      S[1].d.line_base, rmark[0].as<uint8_t>(), rank[0].as<unsigned long long>(),
+                                                      rank[1].as<unsigned long long>(), d_byrank.as<uint32_t>(), d_dline.as<uint32_t>());
+  c->launches += (S[1].total ? 1 : 0) + (nd_old ? 1 : 0);
+  LcRev lr[2];
+  for (int i = 0; i < 2; ++i) {
+    const LinkStage& k = K[i];
+    lr[i] = LcRev{k.links.as<tsm_link>(), k.lbase.as<unsigned long long>(), k.out_tests.as<tsm_link_test>(), k.defs.as<LinkDef>(),
+                  k.name.as<LinkKey>(), k.ns ? k.ns - 1 : 0, k.ndefs.as<uint32_t>()};
+  }
+  LcEvents ea{lr[0], lr[1], d_otest.as<uint2>(), n_out, n_new, om, d_tab.as<LinkKey>(), slots - 1, d_slot.as<LcSlot>(),
+              d_cfile.as<int32_t>(), d_dline.as<uint32_t>(), d_cnt.as<uint32_t>(), d_pos.as<unsigned long long>(), nullptr};
+  const unsigned egrid = std::min((n_out + 7) / 8, (uint32_t)c->sms * 8);
+  if (n_out) k_lc_events<false><<<egrid, 256, 0, st>>>(ea);
+  xscan(d_cnt.as<uint32_t>(), n_out, d_bsum.as<unsigned long long>(), d_pos.as<unsigned long long>(), st);
+  unsigned long long* pin = c->h_rb->u64;
+  CU(cudaMemcpyAsync(pin, d_pos.as<unsigned long long>() + n_out, 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  const unsigned long long ne = *pin;
+  if (!d_ev.alloc(sizeof(tsm_link_event) * ((size_t)ne + 1))) return TSM_E_CUDA;
+  ea.out = d_ev.as<tsm_link_event>();
+  if (n_out) k_lc_events<true><<<egrid, 256, 0, st>>>(ea);
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(c->diff_ev[EV_LC_TO], st));
+  CU(cudaStreamSynchronize(st));
+  c->launches += (n_out ? 5 : 3);                          // count, xscan (3), write
+  ms[3] = elapsed_ms(c->diff_ev[EV_LC_FROM], c->diff_ev[EV_LC_TO]);
+  *n_events = (int64_t)ne;
+  bool is_short = events && event_cap < (int64_t)ne;
+  for (int i = 0; i < 2; ++i) {
+    tsm_links_result& o = side[i]->links;
+    o.n_tests = K[i].nt; o.n_links = (int64_t)K[i].nk; o.n_defs = K[i].nd;
+    is_short |= (o.tests && o.test_cap < o.n_tests) || (o.links && o.link_cap < o.n_links) || (o.defs && o.def_cap < o.n_defs) ||
+                ((side[i]->match || side[i]->change) && o.test_cap < o.n_tests);
+  }
+  if (is_short) return TSM_E_CAPACITY;
+  if (events && ne) CU(cudaMemcpyAsync(events, d_ev.p, sizeof(tsm_link_event) * ne, cudaMemcpyDeviceToHost, st));
+  for (int i = 0; i < 2; ++i) {
+    const int rc = link_copy(K[i], &side[i]->links, st);    // (synchronises st)
+    if (rc != TSM_OK) return rc;
+    if (side[i]->match) std::copy(match[i].begin(), match[i].end(), side[i]->match);
+    if (side[i]->change) std::copy(change[i].begin(), change[i].end(), side[i]->change);
+  }
+  return TSM_OK;
+}
+
+extern "C" int tsm_link_churn_last_ms(tsm_ctx* c, float* ms4) { return copy_ms(c, MS_LCHURN, ms4, 4); }
 
 // ------------------------------------------------------------------------------------- SPEC section 19 test-smell churn
 // The line records of both sides with their header events, per side the case spans and the smell stage, one synchronisation

@@ -18,11 +18,11 @@
 //   tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N]
 //   tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]
 //   tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--smells F]
-//                     [--lexical] [--moves F] [--clones F] [--similar-tests F] [--min-lines N] [--similarity P] [--find-renames N] [--batch-bytes N]
+//                     [--lexical] [--moves F] [--clones F] [--similar-tests F] [--min-lines N] [--similarity P] [--links F] [--find-renames N] [--batch-bytes N]
 //   tosem-scan body   <project-root>... [--batch-bytes N] [--out F]
 //   tosem-scan releases <snapshot-root>=<tag>... | --git <repository> [<revision>...]   [--batch-bytes N] [--out F]
 //   tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F] [--cases F]
-//                      [--assert-edits F] [--smells F] [--lexical] [--moves F] [--clones F] [--similar-tests F] [--find-renames N] [--batch-bytes N]
+//                      [--assert-edits F] [--smells F] [--lexical] [--moves F] [--clones F] [--similar-tests F] [--links F] [--find-renames N] [--batch-bytes N]
 //   tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]
 //   tosem-scan clones <project-root>... | --git <repository> [--rev R]   [--min-lines N] [--blind] [--all-files] [--out F]
 // Every command that scans files does it with scan_batches: batches of at most --batch-bytes of arena (clones: all files in one),
@@ -150,6 +150,13 @@ static std::string test_name_tag(const std::string& rel, bool fixture) {   // S2
   if (fixture) t += ", Fixture";
   return t;
 }
+
+// Which files of a revision a step walk keeps: the study's selection (S0 / S1, or every file with --all-files) or that of the
+// links (section 27: every file with a lexer family, under any path).
+using Select = std::function<bool(const std::string&)>;
+static bool study_file(const std::string& rel) { return lower(rel).find("test") != std::string::npos && ext_tag(rel) != TSM_EXT_OTHER; }
+static bool link_file(const std::string& rel) { return ext_tag(rel) != TSM_EXT_OTHER; }
+static Select selection(bool all_files) { return all_files ? Select([](const std::string&) { return true; }) : Select(study_file); }
 
 static void walk(const std::string& root, int grp, bool all_files, std::vector<FileEntry>& out) {
   std::vector<fs::path> paths;
@@ -1607,6 +1614,7 @@ struct DiffOptions {
   bool smell_lexical = false;                              // --lexical, read only with --smells
   std::string clones;                                      // --clones F, with its --min-lines, --blind and the file selection
   int clone_min_lines = 5; bool clone_blind = false, all_files = false;
+  std::string links;                                       // --links F (docs/SPEC.md section 28)
   std::string similar;                                     // --similar-tests F, with --min-lines (shared with --clones) and --similarity
   int similar_min_lines = 5, similar_pct = 70;
   bool zero_rows = false;
@@ -1860,12 +1868,16 @@ static std::vector<std::string> clone_churn_head(std::vector<std::string> lead) 
   return lead;
 }
 
-// `diff --clones` / `--similar-tests`: the selected files of each root (S0 / S1 unless --all-files) are the two revisions; a file
+// `diff --clones` / `--similar-tests` / `--links`: the files of each root that `sel` keeps are the two revisions; a file
 // whose bytes differ, or that one root lacks, is a change (then --find-renames); one step, handed to every sink.
-static void diff_steps(const std::string& old_root, const std::string& new_root, const DiffOptions& o, const std::vector<StepSink>& sinks) {
+static void diff_steps(const std::string& old_root, const std::string& new_root, const DiffOptions& o, const std::vector<StepSink>& sinks,
+                       const Select& sel) {
   std::vector<FileEntry> fa, fb;
-  walk(old_root, 0, o.all_files, fa);
-  walk(new_root, 0, o.all_files, fb);
+  for (int s = 0; s < 2; ++s) {
+    std::vector<FileEntry> all;
+    walk(s ? new_root : old_root, 0, true, all);
+    for (FileEntry& f : all) if (sel(f.rel)) (s ? fb : fa).push_back(std::move(f));
+  }
   std::vector<Blob> blobs;                                 // the loader's names: the files of fa, then those of fb
   std::map<std::string, Blob, PathLess> ra, rb;
   std::map<std::string, int64_t> name_a, name_b;
@@ -1972,11 +1984,101 @@ static std::vector<std::string> similar_churn_head(std::vector<std::string> lead
   return lead;
 }
 
-// The outputs of --clones and --similar-tests: their files with their header rows, and one sink each; `walk` runs the step driver
-// once over all of them (nothing when neither is asked for).
+// ---------------------------------------------------------------------------------- link churn (docs/SPEC.md section 28)
+static const char* const kLinkEvents[] = {"added", "removed", "retargeted", "redefined", "eager_introduced", "eager_removed",
+                                          "lazy_introduced", "lazy_removed"};
+static const char* const kLinkCauses[] = {"test", "call", "definition"};
+
+// One step of --links: per revision the roles (S0) and stems (tsm_focal_stems), tsm_link_churn over the two revisions and the step's
+// pairs (counts first, then the arrays), then one row per event in its order.
+static void link_churn_step(tsm_ctx* ctx, const Revision& ro, const Revision& rn, const StepPairs& sp, const DiffOptions& d,
+                            const std::vector<std::string>& lead, std::ostream& os) {
+  const Revision* rev[2] = {&ro, &rn};
+  const tsm_corpus co = ro.b.corpus(1), cn = rn.b.corpus(1);
+  struct Side {
+    std::vector<uint8_t> role; std::vector<int32_t> stem;
+    std::vector<tsm_link_test> tests; std::vector<tsm_link> links; std::vector<tsm_link_def> defs;
+    std::vector<int32_t> match; std::vector<uint8_t> change;
+  } S[2];
+  tsm_link_churn_side cs[2] = {};
+  for (int s = 0; s < 2; ++s) {
+    const size_t nf = rev[s]->paths.size();
+    std::vector<const char*> paths(nf);
+    S[s].role.resize(std::max<size_t>(nf, 1)); S[s].stem.resize(std::max<size_t>(nf, 1));
+    for (size_t i = 0; i < nf; ++i) {
+      paths[i] = rev[s]->paths[i].c_str();
+      S[s].role[i] = lower(rev[s]->paths[i]).find("test") != std::string::npos;   // S0
+    }
+    ck(tsm_focal_stems(paths.data(), S[s].role.data(), (int32_t)nf, S[s].stem.data()), "tsm_focal_stems");
+  }
+  int64_t n_ev = 0;
+  auto call = [&](tsm_link_event* ev) {
+    ck(tsm_link_churn(ctx, &co, &cn, S[0].role.data(), S[0].stem.data(), S[1].role.data(), S[1].stem.data(), sp.po.data(), sp.pn.data(),
+                      (int64_t)sp.po.size(), &cs[0], &cs[1], ev, n_ev, &n_ev, nullptr), "tsm_link_churn");
+  };
+  call(nullptr);                                           // the counts; the second call fills arrays of that size
+  for (int s = 0; s < 2; ++s) {
+    tsm_links_result& r = cs[s].links;
+    const size_t nt = (size_t)r.n_tests, nk = (size_t)r.n_links, nd = (size_t)r.n_defs;
+    S[s].tests.resize(std::max<size_t>(nt, 1)); S[s].links.resize(std::max<size_t>(nk, 1)); S[s].defs.resize(std::max<size_t>(nd, 1));
+    S[s].match.resize(std::max<size_t>(nt, 1)); S[s].change.resize(std::max<size_t>(nt, 1));
+    r.tests = S[s].tests.data(); r.test_cap = (int64_t)nt; r.links = S[s].links.data(); r.link_cap = (int64_t)nk;
+    r.defs = S[s].defs.data(); r.def_cap = (int64_t)nd;
+    cs[s].match = S[s].match.data(); cs[s].change = S[s].change.data();
+  }
+  std::vector<tsm_link_event> ev((size_t)std::max<int64_t>(n_ev, 1));
+  call(ev.data());
+  TestNames names[2];
+  for (int s = 0; s < 2; ++s) {
+    std::vector<tsm_smell_test> at((size_t)cs[s].links.n_tests, tsm_smell_test{});
+    for (size_t t = 0; t < at.size(); ++t) { at[t].file = S[s].tests[t].file; at[t].line = S[s].tests[t].line; }
+    names[s] = test_names(*rev[s], at);
+  }
+  auto num = [](int64_t v) { return std::to_string(v); };
+  auto opt = [&](int32_t v) { return v >= 0 ? num(v) : std::string(); };
+  auto callee = [&](int s, int32_t j) {
+    const tsm_link_def& df = S[s].defs[(size_t)S[s].links[(size_t)j].name_def];
+    return std::string((const char*)rev[s]->blobs[(size_t)df.file]->data() + df.name_off, (size_t)df.name_len);
+  };
+  auto target = [&](int s, int32_t j, std::vector<std::string>& row) {   // defFile, defLine of side s's link j
+    const int32_t t = j >= 0 ? S[s].links[(size_t)j].target : -1;
+    if (t < 0) { row.insert(row.end(), {"", ""}); return; }
+    const tsm_link_def& df = S[s].defs[(size_t)t];
+    row.insert(row.end(), {rev[s]->paths[(size_t)df.file], num(df.line + 1)});
+  };
+  for (int64_t k = 0; k < n_ev; ++k) {
+    const tsm_link_event& e = ev[(size_t)k];
+    const int s = e.test >= 0 ? 1 : 0;
+    const int32_t t = s ? e.test : e.old_test;
+    std::vector<std::string> row = lead;
+    row.insert(row.end(), {rev[s]->paths[(size_t)S[s].tests[(size_t)t].file], names[s].name[(size_t)t], std::string(1, (char)S[s].change[(size_t)t]),
+                           e.test >= 0 ? num(S[1].tests[(size_t)e.test].line + 1) : "",
+                           e.old_test >= 0 ? num(S[0].tests[(size_t)e.old_test].line + 1) : ""});
+    if (e.event >= TSM_LINKEV_EAGER_INTRODUCED) {
+      row.insert(row.end(), {"", kLinkEvents[e.event], "", "", "", "", "", "", "", "", ""});
+    } else {
+      row.insert(row.end(), {e.link >= 0 ? callee(1, e.link) : callee(0, e.old_link), kLinkEvents[e.event],
+                             e.cause >= 0 ? kLinkCauses[e.cause] : "", opt(e.calls), opt(e.old_calls), num(e.defs), num(e.old_defs)});
+      target(1, e.link, row);
+      target(0, e.old_link, row);
+    }
+    if (d.rename_pct >= 0) row.push_back(e.old_test >= 0 ? ro.paths[(size_t)S[0].tests[(size_t)e.old_test].file] : "");
+    csv_row(os, row);
+  }
+}
+
+static std::vector<std::string> link_churn_head(std::vector<std::string> lead, bool renames) {
+  lead.insert(lead.end(), {"fileName", "test", "change", "line", "oldLine", "callee", "event", "cause", "calls", "oldCalls", "definitions",
+                           "oldDefinitions", "defFile", "defLine", "oldDefFile", "oldDefLine"});
+  if (renames) lead.push_back("oldFileName");
+  return lead;
+}
+
+// The outputs of --clones, --similar-tests and --links: their files with their header rows, and one sink each; `walk` runs the step
+// driver once over the first two (nothing when neither is asked for) and once, with the links' selection, for --links.
 static void step_outputs(const DiffOptions& o, const std::vector<std::string>& lead_head,
-                         const std::function<void(const std::vector<StepSink>&)>& walk) {
-  std::ofstream clones, similar;
+                         const std::function<void(const std::vector<StepSink>&, const Select&, bool)>& walk) {
+  std::ofstream clones, similar, links;
   std::vector<StepSink> sinks;
   if (!o.clones.empty()) {
     clones.open(o.clones, std::ios::binary);
@@ -1992,7 +2094,14 @@ static void step_outputs(const DiffOptions& o, const std::vector<std::string>& l
       similar_churn_step(ctx, ro, rn, sp, o, lead, similar);
     });
   }
-  if (!sinks.empty()) walk(sinks);
+  if (!sinks.empty()) walk(sinks, selection(o.all_files), false);
+  if (!o.links.empty()) {                                  // (its own walk: the links need the production files)
+    links.open(o.links, std::ios::binary);
+    csv_row(links, link_churn_head(lead_head, o.rename_pct >= 0));
+    walk({[&](tsm_ctx* ctx, const Revision& ro, const Revision& rn, const StepPairs& sp, const std::vector<std::string>& lead) {
+      link_churn_step(ctx, ro, rn, sp, o, lead, links);
+    }}, link_file, true);
+  }
 }
 
 static int cmd_diff(const std::string& old_root, const std::string& new_root, const DiffOptions& o) {
@@ -2014,7 +2123,7 @@ static int cmd_diff(const std::string& old_root, const std::string& new_root, co
     return v;
   };
   const ChangeTotals t = diff_changes(changes, 1, load, o);
-  step_outputs(o, {}, [&](const std::vector<StepSink>& sinks) { diff_steps(old_root, new_root, o, sinks); });
+  step_outputs(o, {}, [&](const std::vector<StepSink>& sinks, const Select& sel, bool) { diff_steps(old_root, new_root, o, sinks, sel); });
   if (t.binaries) fprintf(stderr, "tosem-scan: %lld binary file(s) skipped\n", (long long)t.binaries);
   if (o.rename_pct >= 0)
     fprintf(stderr, "tosem-scan: %lld rename(s) found (%lld exact, %lld inexact)\n", (long long)t.renames, (long long)t.renames_exact,
@@ -2030,7 +2139,7 @@ static int cmd_diff(const std::string& old_root, const std::string& new_root, co
 // two pinned arenas.  GPU: diff_changes.  Rows: one per (commit, changed file).
 
 // The changed blobs under two trees, as changes of `step`; their object names are appended to `objs` (the loader's names).
-static void tree_diff(gitstore::Store& gs, const gitstore::Oid* a, const gitstore::Oid* b, const std::string& prefix, bool all_files,
+static void tree_diff(gitstore::Store& gs, const gitstore::Oid* a, const gitstore::Oid* b, const std::string& prefix, const Select& sel,
                       size_t step, std::vector<gitstore::Oid>& objs, std::vector<Change>& out) {
   std::vector<gitstore::TreeEntry> ea, eb;
   if (a && !gs.tree(*a, ea)) die("unreadable tree " + a->hex());
@@ -2048,10 +2157,10 @@ static void tree_diff(gitstore::Store& gs, const gitstore::Oid* a, const gitstor
     if (x && y && x->oid == y->oid && x->is_tree() == y->is_tree()) continue;     // same object: nothing below it changed
     const std::string path = prefix + nm;
     const bool xt = x && x->is_tree(), yt = y && y->is_tree();
-    if (xt || yt) tree_diff(gs, xt ? &x->oid : nullptr, yt ? &y->oid : nullptr, path + "/", all_files, step, objs, out);
+    if (xt || yt) tree_diff(gs, xt ? &x->oid : nullptr, yt ? &y->oid : nullptr, path + "/", sel, step, objs, out);
     const bool xb = x && x->is_blob(), yb = y && y->is_blob();                     // (symlinks and submodules are not files of the study)
     if (!xb && !yb) continue;
-    if (!all_files && (lower(path).find("test") == std::string::npos || ext_tag(path) == TSM_EXT_OTHER)) continue;   // S0, S1
+    if (!sel(path)) continue;
     Change c{step, path, -1, -1, "", -1};
     if (xb) { c.o = (int64_t)objs.size(); objs.push_back(x->oid); }
     if (yb) { c.n = (int64_t)objs.size(); objs.push_back(y->oid); }
@@ -2073,7 +2182,7 @@ struct History {
     if (!gs.read(objs[(size_t)s], x) || x.type != gitstore::OBJ_BLOB) die("unreadable blob " + objs[(size_t)s].hex());
     return std::move(x.data);
   };
-  History(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files) {
+  History(const std::string& repo, const std::string& rev, int64_t max_commits, const Select& sel) {
     std::string err;
     if (!gs.open(repo, err)) die(err);
     gitstore::Oid head;
@@ -2091,29 +2200,28 @@ struct History {
       const bool has_parent = !chain[i].c.parents.empty();
       if (has_parent && !gs.commit(chain[i].c.parents[0], parent)) die("unreadable commit " + chain[i].c.parents[0].hex());
       if (has_parent && parent.tree == chain[i].c.tree) continue;
-      tree_diff(gs, has_parent ? &parent.tree : nullptr, &chain[i].c.tree, "", all_files, i, objs, changes);
+      tree_diff(gs, has_parent ? &parent.tree : nullptr, &chain[i].c.tree, "", sel, i, objs, changes);
     }
   }
 };
 
-// `history --clones` / `--similar-tests`: the selected files of the current revision kept as live paths, from the boundary commit's
+// `history --clones` / `--similar-tests` / `--links`: the files `sel` keeps (h's selection) of the current revision kept as live paths, from the boundary commit's
 // tree (the parent of the window's first commit; none for a root commit) and each commit's changes after --find-renames.  Blobs
 // are read once while they are live (cached by object name), and a revision is packed once: the new side of one step is the old
 // side of the next.  Every sink gets each commit that changes a selected file, from one walk.
-static void selected_blobs(gitstore::Store& gs, const gitstore::Oid& tree, const std::string& prefix, bool all_files,
+static void selected_blobs(gitstore::Store& gs, const gitstore::Oid& tree, const std::string& prefix, const Select& sel,
                            std::map<std::string, gitstore::Oid, PathLess>& out) {
   std::vector<gitstore::TreeEntry> es;
   if (!gs.tree(tree, es)) die("unreadable tree " + tree.hex());
   for (const gitstore::TreeEntry& e : es) {
     const std::string rel = prefix + e.name;
-    if (e.is_tree()) { selected_blobs(gs, e.oid, rel + "/", all_files, out); continue; }
-    if (!e.is_blob()) continue;
-    if (!all_files && (lower(rel).find("test") == std::string::npos || ext_tag(rel) == TSM_EXT_OTHER)) continue;   // S0, S1
+    if (e.is_tree()) { selected_blobs(gs, e.oid, rel + "/", sel, out); continue; }
+    if (!e.is_blob() || !sel(rel)) continue;
     out[rel] = e.oid;
   }
 }
 
-static void history_steps(History& h, const DiffOptions& o, const std::vector<StepSink>& sinks) {
+static void history_steps(History& h, const DiffOptions& o, const std::vector<StepSink>& sinks, const Select& sel) {
   std::vector<Change> changes = h.changes;
   const auto ctx = small_context();
   ChangeTotals t(h.chain.size());
@@ -2122,7 +2230,7 @@ static void history_steps(History& h, const DiffOptions& o, const std::vector<St
   if (!h.chain.empty() && !h.chain[0].c.parents.empty()) {
     gitstore::Commit p0;
     if (!h.gs.commit(h.chain[0].c.parents[0], p0)) die("unreadable commit " + h.chain[0].c.parents[0].hex());
-    selected_blobs(h.gs, p0.tree, "", o.all_files, live);
+    selected_blobs(h.gs, p0.tree, "", sel, live);
   }
   std::map<gitstore::Oid, Blob> cache;
   auto files_of = [&](const std::map<std::string, gitstore::Oid, PathLess>& paths) {
@@ -2164,7 +2272,7 @@ static void history_steps(History& h, const DiffOptions& o, const std::vector<St
 // --dry-run: no GPU - the rows carry the object names, sizes and an FNV-1a checksum of both blobs instead of the counts
 // (what the CPU tests compare with `git diff-tree` / `git cat-file`).
 static int cmd_history(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files, bool dry_run, DiffOptions o) {
-  History h(repo, rev, max_commits, all_files);
+  History h(repo, rev, max_commits, selection(all_files));
   o.lead = [&](size_t step) {
     const Step& st = h.chain[step];
     return std::vector<std::string>{st.id.hex(), st.c.parents.empty() ? "" : st.c.parents[0].hex(), std::to_string(st.c.time)};
@@ -2189,8 +2297,11 @@ static int cmd_history(const std::string& repo, const std::string& rev, int64_t 
     }
   } else {
     o.zero_rows = true; o.lead_head = {"commit", "parent", "time"}; o.churn_lead = 1;
-    step_outputs(o, o.lead_head, [&](const std::vector<StepSink>& sinks) { history_steps(h, o, sinks); });   // (before diff_changes,
-                                                           // which pairs the renames of h.changes in place)
+    step_outputs(o, o.lead_head, [&](const std::vector<StepSink>& sinks, const Select& sel, bool links) {   // (before diff_changes,
+      if (!links) { history_steps(h, o, sinks, sel); return; }                                       //  which pairs the renames
+      History hl(repo, rev, max_commits, sel);                                                       //  of h.changes in place)
+      history_steps(hl, o, sinks, sel);
+    });
     t = diff_changes(h.changes, h.chain.size(), h.load, o);
   }
   printf("commit,files,cloc,added,removed\r\n");
@@ -2225,7 +2336,7 @@ struct PathState { std::vector<tsm_origin> org; int32_t owner = -1; int64_t obj 
 
 static int cmd_blame(const std::string& repo, const std::string& rev, int64_t max_commits, bool all_files, int rename_pct,
                      int64_t batch_bytes, const std::string& out_path, const std::string& asserts_path) {
-  History h(repo, rev, max_commits, all_files);
+  History h(repo, rev, max_commits, selection(all_files));
   const std::vector<Step>& chain = h.chain;
   const bool cut = !chain.empty() && !chain[0].c.parents.empty();          // the window does not reach the root
   Step p0{};
@@ -2820,12 +2931,12 @@ static void usage() {
           "usage: tosem-scan scan   <project-root>... [--rows F] [--summary F] [--gpus N] [--all-files] [--batch-bytes N] [--rev-b]\n"
           "       tosem-scan reduce <taxonomy.csv> [--strategy F] [--methods F] [--properties F] [--correlate F] [--correlate-tex F] [--correlate-counts F] [--correlate-merged F]\n"
           "       tosem-scan diff   <old-root> <new-root> [--out F] [--asserts F] [--assert-churn F] [--cases F] [--assert-edits F] [--smells F [--lexical]]\n"
-          "                         [--moves F] [--clones F [--min-lines N] [--blind] [--all-files]] [--similar-tests F [--min-lines N] [--similarity P]] [--find-renames N] [--batch-bytes N]\n"
+          "                         [--moves F] [--clones F [--min-lines N] [--blind] [--all-files]] [--similar-tests F [--min-lines N] [--similarity P]] [--links F] [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan body   <project-root>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases <snapshot-root>=<tag>... [--batch-bytes N] [--out F]\n"
           "       tosem-scan releases --git <repository> [<revision>...] [--batch-bytes N] [--out F]\n"
           "       tosem-scan history <git-repository> [--rev R] [--max-commits N] [--all-files] [--dry-run] [--out F] [--asserts F] [--assert-churn F]\n"
-          "                          [--cases F] [--assert-edits F] [--smells F [--lexical]] [--moves F] [--clones F [--min-lines N] [--blind]] [--similar-tests F [--similarity P]]\n"
+          "                          [--cases F] [--assert-edits F] [--smells F [--lexical]] [--moves F] [--clones F [--min-lines N] [--blind]] [--similar-tests F [--similarity P]] [--links F]\n"
           "                          [--find-renames N] [--batch-bytes N]\n"
           "       tosem-scan blame <git-repository> [--rev R] [--max-commits N] [--all-files] [--find-renames N] [--batch-bytes N] [--out F] [--asserts F]\n"
           "       tosem-scan clones <project-root>... [--min-lines N] [--blind] [--all-files] [--out F]\n"
@@ -2861,6 +2972,9 @@ static void usage() {
           "--similar-tests F: per commit, one row per pair of similar tests (docs/SPEC.md section 23) that the commit creates, changes or\n"
           "            breaks up (copied, changed, diverged, ...), with both tests on both sides and their similarity before and after\n"
           "            (docs/SPEC.md section 24); --min-lines N (shared with --clones) and --similarity P as for similar-tests.\n"
+          "--links F: per commit that changes a file with a lexer family (any path: production files too), one row per test-to-code\n"
+          "            link that the commit adds, removes, retargets or redefines, and per Eager / Lazy Test flag it introduces or\n"
+          "            removes, test by test (docs/SPEC.md section 28); not with --dry-run.\n"
           "--batch-bytes N: files go to the GPU in batches of at most N bytes (per side of a diff; a larger file alone); scan: 1 GiB, else 512 MiB.\n"
           "Scans run on the GPU through libtosemscan.so (sm_90a); there is no CPU fallback.\n");
 }
@@ -2941,6 +3055,10 @@ int main(int argc, char** argv) {
     if (p < 1 || p > 100) die("--similarity needs a percentage from 1 to 100");
     d.similar_min_lines = (int)n; d.similar_pct = (int)p;
     if (dry_run) die("--dry-run and --similar-tests cannot be combined (similar-test churn needs the GPU)");
+  }
+  if (opt.count("--links")) {
+    d.links = opt["--links"];
+    if (dry_run) die("--dry-run and --links cannot be combined (link churn needs the GPU)");
   }
   const std::string rev = opt.count("--rev") ? opt["--rev"] : "HEAD";
   const int64_t max_commits = opt.count("--max-commits") ? atoll(opt["--max-commits"].c_str()) : 0;

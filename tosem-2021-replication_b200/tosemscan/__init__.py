@@ -58,6 +58,12 @@ LINK_DEF = np.dtype([("file", "<i4"), ("line", "<i4"), ("name_off", "<i4"), ("na
                      ("tests_by_name", "<i4"), ("calls", "<i4")])   # tsm_link_def: one definition of a production file
 LINK_EAGER, LINK_LAZY = 1, 2                     # bits of LINK_TEST flags
 LINK_KINDS = {1: "function", 2: "class"}         # LINK_DEF kind
+LINK_EVENT = np.dtype([("event", "<i4"), ("cause", "<i4"), ("old_test", "<i4"), ("test", "<i4"), ("old_link", "<i4"), ("link", "<i4"),
+                       ("old_calls", "<i4"), ("calls", "<i4"), ("old_defs", "<i4"),
+                       ("defs", "<i4")])   # tsm_link_event: one row of the link churn (docs/SPEC.md section 28), -1 where absent
+LINK_EVENTS = ["added", "removed", "retargeted", "redefined", "eager_introduced", "eager_removed", "lazy_introduced",
+               "lazy_removed"]                   # LINK_EVENT event
+LINK_CAUSES = ["test", "call", "definition"]     # LINK_EVENT cause of added / removed (-1 for the others)
 ASSERT_EDIT = np.dtype([("rev", "<i8"), ("aev", "<i8"), ("score", "<i4"), ("_pad", "<i4")])   # tsm_assert_edit: event indices
 
 # every symbol include/tosemscan.h declares (tests check the library exports exactly these)
@@ -72,7 +78,7 @@ SYMBOLS = ["tsm_abi_version", "tsm_strerror", "tsm_category_name", "tsm_create",
            "tsm_clones_blind_last_ms", "tsm_clone_churn", "tsm_clone_churn_last_ms", "tsm_similar_tests", "tsm_similar_tests_last_ms",
            "tsm_similar_churn", "tsm_similar_churn_last_ms", "tsm_smells_lexical", "tsm_smells_lexical_last_ms",
            "tsm_diff_pairs_smells_lexical", "tsm_diff_smells_lexical_last_ms", "tsm_test_links", "tsm_test_links_last_ms",
-           "tsm_focal_stems"]
+           "tsm_focal_stems", "tsm_link_churn", "tsm_link_churn_last_ms"]
 FRAG_STATES = ["kept", "edited", "whole"]          # tsm_clone_churn state[j] (docs/SPEC.md section 22)
 CLONE_STATUSES = ["untouched", "changed", "removed", "diverged", "dropped", "created", "copied", "joined"]   # status[c]
 
@@ -149,6 +155,10 @@ class _SimilarResult(C.Structure):
 class _LinksResult(C.Structure):
     _fields_ = [("tests", C.c_void_p), ("test_cap", C.c_int64), ("n_tests", C.c_int64), ("links", C.c_void_p), ("link_cap", C.c_int64),
                 ("n_links", C.c_int64), ("defs", C.c_void_p), ("def_cap", C.c_int64), ("n_defs", C.c_int64)]
+
+
+class _LinkChurnSide(C.Structure):
+    _fields_ = [("links", _LinksResult), ("match", C.c_void_p), ("change", C.c_void_p)]
 
 
 class _SimilarChurnSide(C.Structure):
@@ -281,6 +291,12 @@ def lib():
         L.tsm_test_links.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.c_void_p, C.c_void_p, C.POINTER(_LinksResult), C.c_void_p]
         L.tsm_test_links_last_ms.restype = C.c_int
         L.tsm_test_links_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
+        L.tsm_link_churn.restype = C.c_int
+        L.tsm_link_churn.argtypes = [C.c_void_p, C.POINTER(_Corpus), C.POINTER(_Corpus), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(_LinkChurnSide), C.POINTER(_LinkChurnSide), C.c_void_p,
+                                     C.c_int64, C.POINTER(C.c_int64), C.c_void_p]
+        L.tsm_link_churn_last_ms.restype = C.c_int
+        L.tsm_link_churn_last_ms.argtypes = [C.c_void_p, C.POINTER(C.c_float * 4)]
         L.tsm_focal_stems.restype = C.c_int
         L.tsm_focal_stems.argtypes = [C.POINTER(C.c_char_p), C.c_void_p, C.c_int32, C.c_void_p]
         L.tsm_similar_tests.restype = C.c_int
@@ -1242,6 +1258,57 @@ class Scanner:
         states + k_lex_body + k_lex_lines, k_lex_tests] in ms."""
         ms = (C.c_float * 4)()
         lib().tsm_smells_lexical_last_ms(self._ctx, C.byref(ms))
+        return [float(x) for x in ms]
+
+    def link_churn(self, old_rev, new_rev, old_role, new_role, pair_old, pair_new, old_stem=None, new_stem=None, stream=None,
+                   cap=None):
+        """Test-to-code link churn (docs/SPEC.md section 28): a dict {"old": ..., "new": ..., "events": ...}.  Per revision tests,
+        links and defs (as test_links gives them for that revision alone, as one repository), match (the other side's link test,
+        -1 for none) and change (b"A", b"D", b"=" or b"M" per link test, as uint8); events (LINK_EVENT, event indexing LINK_EVENTS
+        and cause LINK_CAUSES).  role and stem per revision are those of test_links.  Pair k is file pair_old[k] of old_rev and
+        file pair_new[k] of new_rev, -1 for none; a file in no pair is unchanged and matches the same-numbered unpaired file of
+        the other revision.  Arrays too small for their counts are sized from the counts and the call is made again, which
+        repeats the whole call (cap: the first guess of every array)."""
+        po = np.ascontiguousarray(pair_old, np.int32).ravel()
+        pn = np.ascontiguousarray(pair_new, np.int32).ravel()
+        if po.size != pn.size:
+            raise ValueError("pair_old and pair_new differ in length")
+        cs = [old_rev.c_struct(), new_rev.c_struct()]
+        roles = [np.ascontiguousarray(old_role, np.uint8), np.ascontiguousarray(new_role, np.uint8)]
+        stems = [None if s is None else np.ascontiguousarray(s, np.int32) for s in (old_stem, new_stem)]
+        caps = [[int(cap if cap is not None else 0)] * 3 for _ in range(2)]
+        ce = int(cap if cap is not None else 0)
+        for _ in range(2):
+            outs, sides = [], []
+            for ct, ck, cd in caps:
+                o = {"tests": np.zeros(max(ct, 1), LINK_TEST), "links": np.zeros(max(ck, 1), LINK), "defs": np.zeros(max(cd, 1), LINK_DEF),
+                     "match": np.zeros(max(ct, 1), np.int32), "change": np.zeros(max(ct, 1), np.uint8)}
+                outs.append(o)
+                r = _LinksResult(tests=_p(o["tests"]), test_cap=ct, links=_p(o["links"]), link_cap=ck, defs=_p(o["defs"]), def_cap=cd)
+                sides.append(_LinkChurnSide(r, _p(o["match"]), _p(o["change"])))
+            ev = np.zeros(max(ce, 1), LINK_EVENT)
+            ne = C.c_int64()
+            rc = lib().tsm_link_churn(self._ctx, C.byref(cs[0]), C.byref(cs[1]), _p(roles[0]), _p(stems[0]), _p(roles[1]), _p(stems[1]),
+                                      _p(po), _p(pn), po.size, C.byref(sides[0]), C.byref(sides[1]), _p(ev), ce, C.byref(ne), stream)
+            need = [[int(sd.links.n_tests), int(sd.links.n_links), int(sd.links.n_defs)] for sd in sides]
+            if rc == TSM_E_CAPACITY and (ne.value > ce or any(w > h for nw, nh in zip(need, caps) for w, h in zip(nw, nh))):
+                caps, ce = need, int(ne.value)
+                continue
+            if rc:
+                raise TsmError(rc, "tsm_link_churn")
+            res = {"events": ev[:ne.value]}
+            for name, o, sd in zip(("old", "new"), outs, sides):
+                nt = int(sd.links.n_tests)
+                res[name] = {"tests": o["tests"][:nt], "links": o["links"][:sd.links.n_links], "defs": o["defs"][:sd.links.n_defs],
+                             "match": o["match"][:nt], "change": o["change"][:nt]}
+            return res
+        raise TsmError(TSM_E_CAPACITY, "tsm_link_churn")
+
+    def link_churn_last_ms(self):
+        """Device time of the last link_churn call: [k_scan over both revisions, both link fronts + the marks diff +
+        k_lc_change, both link joins, the churn join and emit] in ms."""
+        ms = (C.c_float * 4)()
+        lib().tsm_link_churn_last_ms(self._ctx, C.byref(ms))
         return [float(x) for x in ms]
 
     def test_links_last_ms(self):
